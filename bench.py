@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — single-stream decode throughput of the B200 RWKV-v4 uint8 engine.
+"""bench.py — single-stream decode throughput of the H100 RWKV-v4 uint8 engine.
 
-Contract (driver): `python bench.py --gpus N --steps K --warmup W [--impl reference]`
+`python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]`
 prints ONE JSON line on rank 0.
 
   step      one decoded token = ONE launch of the persistent token kernel (embedding .. head, + arg-max)
@@ -15,13 +15,17 @@ prints ONE JSON line on rank 0.
             HOST logits buffer: 32 B H2D + 201,108 B D2H + host argmax every step).
   roofline  dominant kernel class: algorithmic bytes per launch / mean CUDA-event duration of
             that class, measured in this process by the engine's launch-by-launch profile run.
-            Weights (7.2 GB) are >> L2 (126 MB), so every launch streams from HBM.
+            Weights (7.2 GB) are >> L2 (50 MB), so every launch streams from HBM.
   cpu_baseline  the CPU oracle (port of the reference CUDA forward) on the host cores, a few
             tokens of the same model.
-  --impl reference   the UNMODIFIED reference CUDA build (oracle/_ref/ref_harness, compiled from
-            /root/reference by oracle/Makefile) on GPU 0, same .bin, greedy decode through its
+  --impl reference   the UNMODIFIED reference CUDA build (oracle/_ref/ref_harness, compiled from the
+            reference sources by oracle/Makefile) on GPU 0, same .bin, greedy decode through its
             own RWKV::forward, wall clock — the reference has no CPU forward (SURVEY.md 8c);
             its line also carries the oracle's cpu_baseline.
+  --dump-outputs DIR  after the timed steps, write what the last timed step computed: its logits
+            (DIR/logits.npy, f32 [50277]) and the recurrent state it left (DIR/state_<xy|aa|bb|pp|dd>.npy,
+            f64 [L*E]; rank 0). The model and the token stream are seeded, so two builds run with the same
+            arguments can be compared output for output.
 """
 import argparse
 import importlib
@@ -49,16 +53,12 @@ def algorithmic_bytes_per_token(L, E):
 
 
 def metric_name(workload):
-    """BASELINE.json's metric; both arms print the identical string so that the driver can divide them."""
+    """BASELINE.json's metric; both arms print the identical string so that their values can be divided."""
     return "tokens/sec single-stream decode RWKV-4 %s uint8; achieved HBM GB/s vs peak" % {"7b": "7B", "14b": "14B", "1b5": "1.5B", "169m": "169M"}[workload]
 
 
-def measured_peak():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+def hbm_peak():
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not a measured figure"
 
 
 class ClockSampler(threading.Thread):
@@ -142,7 +142,7 @@ def run_reference(args, pkg, workload):
             "config": {"workload": "RWKV-4 %s shape L=%d E=%d uint8, random-init, greedy single-stream decode" % (workload, L, E),
                        "l2": "weights >> L2, every token streams from HBM"}}
     if not os.path.exists(REF_HARNESS):
-        base["unavailable"] = "oracle/_ref/ref_harness not built (needs /root/reference at build time)"
+        base["unavailable"] = "oracle/_ref/ref_harness not built (needs the reference sources at build time)"
         emit(base)
         return
     path = model_path(workload, pkg)
@@ -173,27 +173,13 @@ def run_reference(args, pkg, workload):
                  "e2e": {"value": v, "unit": "tokens/s", "h2d_bytes_per_step": 4 * E + 5 * L * E * 8,
                          "d2h_bytes_per_step": 4 * VOCAB + 5 * L * E * 8},
                  "cpu_baseline": cb, "gpu_launches": (9 + 20 * L) * args.steps,
-                 "reference_arm": "unmodified /root/reference rwkv.cu + rwkv.h on 1 GPU (its own RWKV::forward incl. its host<->device state copies)"})
+                 "reference_arm": "unmodified reference rwkv.cu + rwkv.h on 1 GPU (its own RWKV::forward incl. its host<->device state copies)"})
     for p in (dump, dump + ".tokens", tf):
         try:
             os.remove(p)
         except OSError:
             pass
     emit(base)
-
-
-def ncu_traffic(kernel, workload):
-    """DRAM bytes (read + write) per launch of the dominant kernel, from the committed `ncu --set full`
-    capture of the same command (profiles/r02_token_traffic.json); null if there is none for this case."""
-    p = os.path.join(ROOT, "profiles", "r02_token_traffic.json")
-    try:
-        with open(p) as f:
-            t = json.load(f)
-        if kernel == "token" and t.get("workload") == workload:
-            return int(t["dram_bytes_read"]) + int(t["dram_bytes_write"])
-    except (OSError, ValueError, KeyError):
-        pass
-    return None
 
 
 _REAL_STDOUT = None
@@ -218,6 +204,16 @@ def emit(obj):
         os.write(_REAL_STDOUT, data)
 
 
+def dump_outputs(out_dir, eng):
+    """The arrays the device-resident decode leaves behind after its last step: that step's logits and the
+    recurrent state."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "logits.npy"), eng.debug_read("logits").astype(np.float32))
+    for k, v in eng.state_download().items():
+        np.save(os.path.join(out_dir, "state_%s.npy" % k), v.astype(np.float64))
+
+
 def main():
     claim_stdout()
     ap = argparse.ArgumentParser()
@@ -227,6 +223,8 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default=None, choices=sorted(SHAPES))
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the logits and the state of the last timed step as DIR/<name>.npy")
     ap.add_argument("--parallelism", default="tp", choices=["tp", "replicas"],
                     help="N > 1: which arrangement the headline `value` reports. 'tp' (default) = ONE stream decoded by the "
                          "N GPUs together (strong scaling: column/row split of every matrix, two in-kernel NVLink exchanges "
@@ -292,6 +290,8 @@ def main():
     ms = eng.decode_timed([SEED_TOKEN] * args.steps, teacher_forced=False)
     sync_all()
     launches = eng.launch_count - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng)
     t = torch.tensor([ms], dtype=torch.float64, device="cuda:%d" % local_rank)
     if dist is not None:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -374,7 +374,7 @@ def main():
     prof_tokens, prof = prof_run()
     if tp:
         dist.barrier()
-    peak, peak_src = measured_peak()
+    peak, peak_src = hbm_peak()
     kernels = {}
     total_ms = sum(v["ms_sum"] for v in prof.values()) or 1.0
     for name, v in prof.items():
@@ -387,7 +387,7 @@ def main():
                          "share": round(v["ms_sum"] / total_ms, 4)}
     dom = max(kernels, key=lambda k: kernels[k]["share"])
     roofline = {"bound": "hbm", "kernel": dom, "achieved": kernels[dom]["gbs"], "peak": peak, "unit": "GB/s",
-                "frac": round(kernels[dom]["gbs"] / peak, 4), "traffic": ncu_traffic(dom, workload) if world == 1 else None, "peak_source": peak_src,
+                "frac": round(kernels[dom]["gbs"] / peak, 4), "peak_source": peak_src,
                 "how": "algorithmic bytes per launch / mean CUDA-event duration per launch (eager profile run, %d tokens)" % len(prof_tokens)}
     abytes = algorithmic_bytes_per_token(L, E)
     if world > 1:
@@ -410,7 +410,7 @@ def main():
         "dtype": "u8 weights x 23-bit fixed-point activations (byte limbs u8,u8,s8; exact int32 dp4a accumulate), f64 elementwise",
         "data": "synthetic",
         "config": {"workload": "RWKV-4 %s shape (L=%d, E=%d, V=50277) uint8, random-init reference-format .bin, greedy single-stream decode, batch 1" % (workload, L, E),
-                   "l2": "inputs larger than L2: %.2f GB of weights per token vs 126 MB L2" % (abytes / 1e9),
+                   "l2": "inputs larger than L2: %.2f GB of weights per token vs 50 MB L2" % (abytes / 1e9),
                    "parallelism": ("tp%d: one stream; K/V/R/ffn-K/ffn-R/head split by output channel, out-proj/ffn-V by input "
                                    "channel, weights sharded at load, residual/layernorm replicated, two in-kernel exchanges of "
                                    "partial sums per layer as self-tagged words stored into the peers over NVLink (no NCCL on the "

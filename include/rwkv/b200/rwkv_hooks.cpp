@@ -1,11 +1,11 @@
-// rwkv_hooks.cpp — the reference's six backend hooks, implemented on the B200 engine.
+// rwkv_hooks.cpp — the reference's six backend hooks, implemented on the H100 engine.
 //
 // The reference's host class (harrisonvanderbyl/rwkv-cpp-accelerated include/rwkv/rwkv/rwkv.h) talks to
 // its CUDA backend through six C++-linkage functions declared at rwkv.h:63-122 and defined in
 // include/rwkv/cuda/rwkv.cu:479-490 (setState), 467-477 (getOutput), 493-593 (cuda_rwkv_parralel),
 // 595-628 (cuda_rwkv), 638-717 (load), 719-730 (freeTensors). A program that compiles against the
 // REFERENCE's own, unmodified rwkv.h links against this translation unit + librwkv_b200 instead of
-// rwkv.cu and runs on the B200 engine: same symbols (same mangled names), same argument meaning.
+// rwkv.cu and runs on the H100 engine: same symbols (same mangled names), same argument meaning.
 //
 // How the 47-pointer calls map onto the engine: `load` fills the tensor table with the engine's device
 // pointers (rwkv_b200_tensor), so every later call identifies its model by the pointer it passes for
@@ -44,7 +44,7 @@ Bound *find_by(void *x, void *sxy) {
 }
 
 [[noreturn]] void die(const char *what) {
-    fprintf(stderr, "rwkv (B200 backend): %s: %s\n", what, rwkv_b200_last_error());
+    fprintf(stderr, "rwkv (H100 backend): %s: %s\n", what, rwkv_b200_last_error());
     exit(1);
 }
 
@@ -73,7 +73,7 @@ void setState(unsigned long long, unsigned long long, double *stateaa, double *,
     std::lock_guard<std::mutex> lk(g_mu);
     Bound *b = find_by(nullptr, stateaa);
     if (!b) {
-        fprintf(stderr, "rwkv (B200 backend): setState on a state that load() did not create\n");
+        fprintf(stderr, "rwkv (H100 backend): setState on a state that load() did not create\n");
         exit(1);
     }
     if (rwkv_b200_state_upload(b->model, instateaa, instatebb, instatecc, instatedd, instateee, tokenlength) != 0) die("setState");
@@ -86,7 +86,7 @@ void getOutput(unsigned long long, unsigned long long, float *, double *statexyi
     std::lock_guard<std::mutex> lk(g_mu);
     Bound *b = find_by(nullptr, statexyin);
     if (!b) {
-        fprintf(stderr, "rwkv (B200 backend): getOutput on a state that load() did not create\n");
+        fprintf(stderr, "rwkv (H100 backend): getOutput on a state that load() did not create\n");
         exit(1);
     }
     // the forward left the logits of its `tokenlength` tokens in the engine's pinned buffer
@@ -130,7 +130,7 @@ void cuda_rwkv_parralel(unsigned long long, unsigned long long, unsigned long lo
         b = find_by(x, statexy);
     }
     if (!b) {
-        fprintf(stderr, "rwkv (B200 backend): forward on tensors that load() did not create\n");
+        fprintf(stderr, "rwkv (H100 backend): forward on tensors that load() did not create\n");
         exit(1);
     }
     if (rwkv_b200_forward(b->model, token, tokenlength, mode == PARRALEL ? RWKV_B200_MODE_PARRALEL : RWKV_B200_MODE_GPT,

@@ -1,4 +1,4 @@
-// rwkv.h — host API of the B200 RWKV-v4 uint8 engine: `RWKV`, `RWKVState`, the tensor table.
+// rwkv.h — host API of the H100 RWKV-v4 uint8 engine: `RWKV`, `RWKVState`, the tensor table.
 //
 // Source-compatible with the reference's host header (harrisonvanderbyl/rwkv-cpp-accelerated
 // include/rwkv/rwkv/rwkv.h): same class names, public members, method signatures, error
@@ -214,7 +214,7 @@ class RWKV {
     double *statepp = nullptr;
     double *statedd = nullptr;
 
-    // B200 engine handle and options (not in the reference)
+    // H100 engine handle and options (not in the reference)
     rwkv_b200_model *engine = nullptr;
     bool strictState = false; // true: full state H2D before / D2H after every forward (R.h:353,372)
     int device = 0;

@@ -1,4 +1,4 @@
-/* rwkv_b200.h — C ABI of the B200 (sm_100a) RWKV-v4 uint8 decode engine.
+/* rwkv_b200.h — C ABI of the H100 (sm_90a) RWKV-v4 uint8 decode engine.
  *
  * This is the drop-in boundary: plain C, opaque handle, plain pointers and sizes,
  * no C++/torch types. Everything above it (include/rwkv/rwkv/rwkv.h, the pybind
@@ -12,7 +12,7 @@
  *
  * Conventions: functions returning int return 0 on success and a non-zero code on
  * failure; rwkv_b200_last_error() then holds a message (thread-local). There is no
- * CPU fallback: without a usable sm_100 device every compute entry point fails.
+ * CPU fallback: without a usable sm_90 device every compute entry point fails.
  */
 #ifndef RWKV_B200_H
 #define RWKV_B200_H

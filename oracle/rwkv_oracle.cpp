@@ -15,7 +15,7 @@
 //
 // Pinning status: the reference ships NO golden vectors for the forward (SURVEY.md 8c),
 // so this oracle is pinned against the reference itself: oracle/_ref/ref_harness (the
-// unmodified rwkv.cu + rwkv.h compiled for sm_100a by oracle/Makefile) is run on the
+// unmodified rwkv.cu + rwkv.h compiled for sm_90a by oracle/Makefile) is run on the
 // GPU box on the same synthetic .bin and compared with this file in
 // tests/test_parity_gpu.py::test_oracle_vs_reference_cuda. Where /root/reference or a
 // GPU is unavailable that test skips and parity is "pinned by construction only".

@@ -1,4 +1,4 @@
-"""rwkv-cpp-accelerated_b200 — B200 (sm_100a) RWKV-v4 uint8 decode engine.
+"""rwkv-cpp-accelerated_b200 — H100 (sm_90a) RWKV-v4 uint8 decode engine.
 
 The product is the CUDA library in ``csrc/`` behind the C ABI of ``include/rwkv_b200.h``;
 this package is the thin Python side used by tests and ``bench.py`` (ctypes over that

@@ -1,7 +1,7 @@
 """In-tree builds (no JIT cache): every artefact lands next to its sources so that it
 travels to the GPU box with the repo snapshot.
 
-  librwkv_b200.so        csrc/engine.cu + kernels.cuh      nvcc, sm_100a only
+  librwkv_b200.so        csrc/engine.cu + kernels.cuh      nvcc, sm_90a only
   tools/genmodel         tools/genmodel.cpp                g++
   bindings/pybind/rwkv*.so   bindings/pybind/c_binding.cpp g++ + pybind11, links librwkv_b200.so
   oracle/librwkv_oracle.so, oracle/_ref/*                  oracle/Makefile (checker only)
@@ -23,7 +23,7 @@ REF_HARNESS = os.path.join(ORACLE_DIR, "_ref", "ref_harness")
 PYBIND_DIR = os.path.join(PKG, "bindings", "pybind")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "-shared", "-cudart", "static",
 ]
 

@@ -1,4 +1,4 @@
-// common.cuh — parameters, shared-memory map and PTX helpers of the sm_100a RWKV-v4 uint8 decode path.
+// common.cuh — parameters, shared-memory map and PTX helpers of the sm_90a RWKV-v4 uint8 decode path.
 //
 // The arithmetic idea (why three byte limbs): the reference computes
 //   y_k = sum_j x_j * (w_jk * r_j + o_j)                     (include/rwkv/cuda/rwkv.cu:279-294)
@@ -34,7 +34,7 @@ constexpr int kMaxRowsPerCta = 1024;       // res64 capacity (rows x segments of
 constexpr int kTraceMax = 2048;            // trace stamps per CTA (debug)
 constexpr int kTileTraceMax = 4096;        // tiles per CTA recorded by the tile trace (debug)
 constexpr int kQMax = 4194303;             // 2^22 - 1: largest |q| of the activation quantiser
-constexpr int kSmemLimit = 232448;         // opt-in dynamic shared memory per CTA on sm_100
+constexpr int kSmemLimit = 232448;         // opt-in dynamic shared memory per CTA on sm_90 (227 KB)
 
 // Device-resident control block of one model (one per rank).
 struct Ctrl {

@@ -1,4 +1,4 @@
-// engine.cu — host side of the B200 RWKV-v4 uint8 decode engine + the C ABI (include/rwkv_b200.h).
+// engine.cu — host side of the H100 RWKV-v4 uint8 decode engine + the C ABI (include/rwkv_b200.h).
 //
 // Responsibilities:
 //   * load a reference-format .bin (include/rwkv/cuda/rwkv.cu:638-717 semantics): each rank reads only
@@ -10,7 +10,7 @@
 //   * measurement hooks used by bench.py.
 //
 // There is deliberately no CPU code path: every entry point that computes fails with an error when
-// no sm_100 device is present.
+// no sm_90 device is present.
 #include <algorithm>
 #include <cerrno>
 #include <cstdarg>
@@ -343,7 +343,8 @@ int do_load(M *m, const char *path, int quiet) {
     CK(cudaSetDevice(m->device));
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, m->device));
-    if (prop.major < 10) return fail(6, "device %d is sm_%d%d; this engine is built for sm_100a only", m->device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(6, "device %d is sm_%d%d; this engine is built for sm_90a only", m->device, prop.major, prop.minor);
     m->sms = prop.multiProcessorCount;
     m->grid = m->sms;
     CK(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));

@@ -6,13 +6,15 @@
 // matrix and the tokens' activation limbs - the same exact-integer formulation as the decode kernel (common.cuh):
 // each token's vector is quantised to a 23-bit integer and its three byte limbs are three columns of the B
 // operand (two unsigned planes, one signed plane), so the tensor cores compute bit for bit what the IDP.4A
-// loop computes: tcgen05.mma kind::i8, s8 x u8 / s8 x s8 -> s32 in TMEM, planes recombined in the epilogue.
+// loop computes: wgmma.mma_async m64nNk32, s8 x u8 / s8 x s8 -> s32 in registers, planes recombined in the epilogue.
 // No dequantisation, no fp error, and the weights go straight from HBM to shared memory by TMA in the
 // K-major, 128-byte-swizzled layout the MMA wants (they are stored [out][in] = K-major already).
 //
-// One GEMM launch: grid = (ceil(M / 128), ksplit); CTA = 6 warps: TMA producer, MMA issuer (+ TMEM
-// allocation), four epilogue warps (TMEM lanes 0-127). Tile 128 x (3 Tp) x 128 bytes of K per stage; D is
-// 128 lanes x 3 Tp columns of TMEM. Split-K partial sums are added with integer atomics (exact, order-free).
+// One GEMM launch: grid = (ceil(M / 64), ksplit); CTA = two consumer warpgroups + one TMA producer warp. Tile
+// 64 rows x (3 Tp) x 128 bytes of K per stage; each consumer warpgroup owns NB = Tp / 32 blocks of 16 tokens in
+// all three planes (at most 3 x 4 x 8 accumulator registers per thread). NB is a template parameter so that every
+// wgmma sits on a uniform path (a data-dependent branch around them makes the compiler serialise them). Split-K
+// partial sums are added with integer atomics (exact, order-free).
 // Everything around the GEMMs (layernorm, token shift, WKV scan over t, activations, quantisation) is plain
 // CUDA, one small kernel per step, with the reference's rounding points (rwkv.cu:40-57, 221-259, 313-465).
 #pragma once
@@ -25,12 +27,14 @@
 
 namespace rk {
 
-constexpr int kPrefillMinTokens = 8;   // shorter calls run token by token through the decode kernel (7B: break-even near 6)
-constexpr int kPfMaxTokens = 128;      // tokens per pass: the unsigned planes are N = 2 Tp <= 256 MMA columns
-constexpr int kPfBM = 128, kPfBK = 128, kPfStages = 3;
-constexpr int kPfThreads = 192;
+constexpr int kPrefillMinTokens = 8;   // shorter calls run token by token through the decode kernel
+constexpr int kPfMaxTokens = 128;      // tokens per pass
+constexpr int kPfBM = 64, kPfBK = 128, kPfStages = 3;
+constexpr int kPfConsumerWGs = 2;
+constexpr int kPfThreads = 128 * kPfConsumerWGs + 32;
+constexpr int kPfTokenAlign = 16 * kPfConsumerWGs; // padded token count: the same number of blocks per warpgroup
 
-// ---- tcgen05 / TMA helpers -------------------------------------------------------------------------------
+// ---- wgmma / TMA helpers ---------------------------------------------------------------------------------
 __device__ __forceinline__ void pf_mbar_wait(uint32_t bar, uint32_t parity) {
     uint32_t ok = 0;
     while (!ok) {
@@ -46,46 +50,52 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map
                  : "memory");
 }
 // Shared-memory matrix descriptor of a K-major operand tile in the 128-byte swizzle (the layout TMA writes):
-// rows of 128 bytes, 8-row groups 1024 bytes apart (SBO); LBO is unused for swizzled K-major layouts.
-__device__ __forceinline__ uint64_t umma_desc_k128(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
+// rows of 128 bytes, 8-row groups 1024 bytes apart (SBO); LBO is unused for swizzled K-major layouts. A step of
+// 32 bytes along K inside the swizzle atom advances the start address only.
+__device__ __forceinline__ uint64_t wgmma_desc_k128(uint32_t smem_addr) {
+    return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-// Instruction descriptor of tcgen05.mma kind::i8: D = s32, A = signed 8-bit, B = signed or unsigned 8-bit, both
-// K-major, M = 128, N = n.
-__device__ __forceinline__ uint32_t umma_idesc_i8(int n, bool b_signed) {
-    return (2u << 4) | (1u << 7) | ((b_signed ? 1u : 0u) << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(kPfBM >> 4) << 24);
-}
-__device__ __forceinline__ void umma_i8(uint32_t d_tmem, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-    const uint32_t z = 0;
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t}" ::"r"(d_tmem),
-                 "l"(da), "l"(db), "r"(idesc), "r"(accumulate), "r"(z), "r"(z), "r"(z), "r"(z)
-                 : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// d[64 x 16] += A[64 x 32] (s8) * B[16 x 32]^T (u8 or s8), both from shared memory, K-major.
+template <bool BSigned>
+__device__ __forceinline__ void wgmma_i8_n16(int (&d)[8], uint64_t da, uint64_t db) {
+    if constexpr (BSigned) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n16k32.s32.s8.s8 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p;\n\t}"
+                     : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+                     : "l"(da), "l"(db), "r"(1)
+                     : "memory");
+    } else {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n16k32.s32.s8.u8 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p;\n\t}"
+                     : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+                     : "l"(da), "l"(db), "r"(1)
+                     : "memory");
+    }
 }
 
 struct GemmArgs {
-    CUtensorMap map_a; // weights  [M][K]  int8, box 128 x 128
+    CUtensorMap map_a; // weights  [M][K]  int8, box 64 x 128
     CUtensorMap map_b; // limbs    [rows][K] u8, box Tp x 128 (three loads per stage: planes 0, 1, 2)
     int M, K;          // rows of the weight matrix (this launch), bytes per row
-    int Tp;            // padded token count (multiple of 16, <= 128)
+    int Tp;            // padded token count (multiple of kPfTokenAlign, <= 128)
     int b_row0;        // first limb row of this GEMM's vector: planes at b_row0, +Tp, +2Tp
     int ksplit;        // gridDim.y
     int *C;            // [M][3 Tp] int32, zeroed; columns [0, 2Tp) unsigned planes, [2Tp, 3Tp) signed plane
 };
 
-// C[m][n] += sum_k A[m][k] * B[n][k] over this CTA's K range.
+// C[m][n] += sum_k A[m][k] * B[n][k] over this CTA's K range; NB = Tp / kPfTokenAlign.
+template <int NB>
 __global__ void __launch_bounds__(kPfThreads, 1) k_gemm_i8(const __grid_constant__ GemmArgs g) {
     extern __shared__ __align__(1024) uint8_t pf_smem[];
     const uint32_t base = (smem_u32(pf_smem) + 1023u) & ~1023u;
     const int Tp = g.Tp;
     const uint32_t a_bytes = kPfBM * kPfBK, b_bytes = 3u * (uint32_t)Tp * kPfBK, stage_bytes = a_bytes + b_bytes;
-    const uint32_t bars = base + kPfStages * stage_bytes; // full[3], empty[3], accum, tmem slot
+    const uint32_t bars = base + kPfStages * stage_bytes; // full[stages], empty[stages]
     auto full = [&](int s) { return bars + 8u * (uint32_t)s; };
     auto empty = [&](int s) { return bars + 8u * (uint32_t)(kPfStages + s); };
-    const uint32_t accum = bars + 8u * 2 * kPfStages, tslot = accum + 8;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.x * kPfBM;
     const int kper = g.K / g.ksplit, k0 = blockIdx.y * kper, nkt = kper / kPfBK;
@@ -93,22 +103,13 @@ __global__ void __launch_bounds__(kPfThreads, 1) k_gemm_i8(const __grid_constant
     if (threadIdx.x == 0) {
         for (int s = 0; s < kPfStages; ++s) {
             mbar_init(full(s), 1);
-            mbar_init(empty(s), 1);
+            mbar_init(empty(s), 4 * kPfConsumerWGs); // one arrival per consumer warp
         }
-        mbar_init(accum, 1);
         mbar_fence_init();
     }
-    if (warp == 1) { // TMEM: 512 columns (3 Tp <= 384 are used)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tslot), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    uint32_t tmem;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem) : "r"(tslot) : "memory");
 
-    if (warp == 0) {
+    if (warp == 4 * kPfConsumerWGs) {
         if (lane == 0) { // ---- TMA producer ----
             for (int kt = 0; kt < nkt; ++kt) {
                 const int s = kt % kPfStages;
@@ -120,46 +121,61 @@ __global__ void __launch_bounds__(kPfThreads, 1) k_gemm_i8(const __grid_constant
                 for (int pl = 0; pl < 3; ++pl) tma_load_2d(sb + (uint32_t)(pl * Tp) * kPfBK, &g.map_b, kc, g.b_row0 + pl * Tp, full(s));
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) { // ---- MMA issuer ----
-            const uint32_t id_u = umma_idesc_i8(2 * Tp, false), id_s = umma_idesc_i8(Tp, true);
-            for (int kt = 0; kt < nkt; ++kt) {
-                const int s = kt % kPfStages;
-                pf_mbar_wait(full(s), (uint32_t)((kt / kPfStages) & 1));
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t sa = base + (uint32_t)s * stage_bytes, sb = sa + a_bytes;
-#pragma unroll
-                for (int k = 0; k < kPfBK / 32; ++k) { // UMMA_K = 32 bytes of int8
-                    const uint64_t da = umma_desc_k128(sa + 32u * k);
-                    umma_i8(tmem, da, umma_desc_k128(sb + 32u * k), id_u, (kt | k) != 0);                               // planes 0, 1 (unsigned)
-                    umma_i8(tmem + 2u * (uint32_t)Tp, da, umma_desc_k128(sb + 2u * (uint32_t)Tp * kPfBK + 32u * k), id_s, (kt | k) != 0); // plane 2 (signed)
-                }
-                umma_commit(empty(s)); // frees the stage when these MMAs have read it
-            }
-            umma_commit(accum);
-        }
-    } else { // ---- epilogue: warps 2..5 own TMEM lanes 32 * (warp % 4) ----
-        pf_mbar_wait(accum, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int lane_base = 32 * (warp & 3);
-        const int row = m0 + lane_base + lane;
-        int *crow = g.C + (size_t)row * 3 * Tp;
-        for (int c = 0; c < 3 * Tp; c += 8) {
-            uint32_t v[8];
-            asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                         : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                         : "r"(tmem + ((uint32_t)lane_base << 16) + (uint32_t)c)
-                         : "memory");
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            if (row < g.M) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) atomicAdd(crow + c + i, (int)v[i]);
-            }
-        }
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512) : "memory");
+
+    // ---- consumers: warpgroup wg owns token blocks wg * NB .. wg * NB + NB - 1 ----
+    const int wg = warp >> 2, wl = warp & 3;
+    int acc[3][NB][8];
+#pragma unroll
+    for (int pl = 0; pl < 3; ++pl)
+#pragma unroll
+        for (int i = 0; i < NB; ++i)
+#pragma unroll
+            for (int r = 0; r < 8; ++r) acc[pl][i][r] = 0;
+    for (int kt = 0; kt < nkt; ++kt) {
+        const int s = kt % kPfStages;
+        pf_mbar_wait(full(s), (uint32_t)((kt / kPfStages) & 1));
+        const uint32_t sa = base + (uint32_t)s * stage_bytes, sb = sa + a_bytes;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kPfBK / 32; ++k) { // K = 32 bytes of int8 per instruction
+            const uint64_t da = wgmma_desc_k128(sa + 32u * k);
+#pragma unroll
+            for (int i = 0; i < NB; ++i) {
+                const uint32_t bj = sb + (uint32_t)(16 * (wg * NB + i)) * kPfBK + 32u * k;
+                wgmma_i8_n16<false>(acc[0][i], da, wgmma_desc_k128(bj));                                // plane 0 (unsigned)
+                wgmma_i8_n16<false>(acc[1][i], da, wgmma_desc_k128(bj + (uint32_t)Tp * kPfBK));         // plane 1 (unsigned)
+                wgmma_i8_n16<true>(acc[2][i], da, wgmma_desc_k128(bj + 2u * (uint32_t)Tp * kPfBK));     // plane 2 (signed)
+            }
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty(s)); // this warp's MMAs have read the stage
+    }
+
+    // ---- epilogue: accumulator fragment of m64nNk32 - rows 16 * wl + lane / 4 (+8), columns 2 * (lane % 4) (+1, +8)
+    const int r0 = m0 + 16 * wl + (lane >> 2);
+#pragma unroll
+    for (int pl = 0; pl < 3; ++pl)
+#pragma unroll
+        for (int i = 0; i < NB; ++i) {
+            const int j = wg * NB + i;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int col = pl * Tp + 16 * j + 8 * h + 2 * (lane & 3);
+#pragma unroll
+                for (int half = 0; half < 2; ++half) {
+                    const int row = r0 + 8 * half;
+                    if (row < g.M) {
+                        int *c = g.C + (size_t)row * 3 * Tp + col;
+                        atomicAdd(c, acc[pl][i][4 * h + 2 * half]);
+                        atomicAdd(c + 1, acc[pl][i][4 * h + 2 * half + 1]);
+                    }
+                }
+            }
+        }
 }
 
 // ---- element-wise kernels ----------------------------------------------------------------------------------
@@ -491,7 +507,10 @@ inline int prefill_init(PrefillState &s, const Params &p) {
     PF_CK(cudaMalloc((void **)&s.sr, T * E * 4));
     PF_CK(cudaMalloc((void **)&s.act, T * 4 * E * 4));
     PF_CK(cudaMalloc((void **)&s.logits, T * V * 4));
-    PF_CK(cudaFuncSetAttribute(k_gemm_i8, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
+    PF_CK(cudaFuncSetAttribute(k_gemm_i8<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
+    PF_CK(cudaFuncSetAttribute(k_gemm_i8<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
+    PF_CK(cudaFuncSetAttribute(k_gemm_i8<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
+    PF_CK(cudaFuncSetAttribute(k_gemm_i8<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit));
     s.ready = true;
     return 0;
 }
@@ -522,12 +541,18 @@ inline int pf_gemm(PrefillState &s, cudaStream_t st, const int8_t *W, int M, int
     g.b_row0 = b_row0;
     const int mt = (M + kPfBM - 1) / kPfBM;
     int ks = 1;
-    while (mt * ks < 120 && ks < 8 && (K / (ks * 2)) % kPfBK == 0 && K / (ks * 2) >= 4 * kPfBK) ks *= 2;
+    while (mt * ks < 132 && ks < 8 && (K / (ks * 2)) % kPfBK == 0 && K / (ks * 2) >= 4 * kPfBK) ks *= 2;
     g.ksplit = ks;
     g.C = C;
     PF_CK(cudaMemsetAsync(C, 0, (size_t)M * 3 * Tp * 4, st));
     const size_t smem = (size_t)kPfStages * (kPfBM * kPfBK + 3 * (size_t)Tp * kPfBK) + 1024 + 128;
-    k_gemm_i8<<<dim3(mt, ks), kPfThreads, smem, st>>>(g);
+    static_assert(kPfMaxTokens == 4 * kPfTokenAlign, "one instantiation per block count");
+    switch (Tp / kPfTokenAlign) {
+    case 1: k_gemm_i8<1><<<dim3(mt, ks), kPfThreads, smem, st>>>(g); break;
+    case 2: k_gemm_i8<2><<<dim3(mt, ks), kPfThreads, smem, st>>>(g); break;
+    case 3: k_gemm_i8<3><<<dim3(mt, ks), kPfThreads, smem, st>>>(g); break;
+    default: k_gemm_i8<4><<<dim3(mt, ks), kPfThreads, smem, st>>>(g); break;
+    }
     PF_CK(cudaGetLastError());
     s.launches += 1;
     return 0;
@@ -536,7 +561,7 @@ inline int pf_gemm(PrefillState &s, cudaStream_t st, const int8_t *W, int M, int
 // One chunk of T <= 128 tokens on a single GPU. GPT: tokens in order on slot 0; PARRALEL: token t on slot t.
 // Per-token logits go to h_logits (pinned, [T][V]) if not null.
 inline int prefill_chunk_body(PrefillState &s, const Params &p, cudaStream_t st, int T, bool parallel, bool want_logits) {
-    const int E = p.E, L = p.L, Tp = (T + 15) & ~15;
+    const int E = p.E, L = p.L, Tp = (T + kPfTokenAlign - 1) / kPfTokenAlign * kPfTokenAlign;
     const size_t LE = (size_t)L * E;
     double *saa = reinterpret_cast<double *>(p.xch[p.rank] + p.off_saa), *sbb = reinterpret_cast<double *>(p.xch[p.rank] + p.off_sbb);
     const unsigned gT = (unsigned)T;

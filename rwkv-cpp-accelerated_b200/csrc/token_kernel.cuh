@@ -75,7 +75,7 @@ __host__ __device__ inline Slices make_slices(int E, int Er, int Vr, int b, int 
 // flight), `pf` runs `pf_dist` tiles further ahead and only asks L2 to fetch the bytes
 // (cp.async.bulk.prefetch.L2). The shared-memory ring holds at most 3.7 us of HBM time; a phase boundary
 // takes longer than that, so without the second cursor HBM idles in every boundary and the following phase
-// starts from an empty pipe. With it HBM streams continuously into L2 (126 MB) and the ring refills from
+// starts from an empty pipe. With it HBM streams continuously into L2 (50 MB) and the ring refills from
 // L2 at the consumers' pace.
 struct TileCursor {
     int l, s;           // layer (== L_run: head), sub inside the layer
@@ -376,8 +376,8 @@ __device__ __forceinline__ void gather(const Params &p, const Smem &sm, const fl
     const int total = nvec * ng;  // <= 256 * kGatherMax
     // The C CTAs of a thread-block cluster split the gather: CTA r of the cluster fetches and quantises the r-th
     // part of the concatenated vectors and writes the limb-plane words into the shared memory of all C CTAs
-    // (st.shared::cluster). All 148 SMs pulling the same 16..64 KB out of L2 is what bounds the exchange (L2
-    // bandwidth, tools/latbench.cu part 3) and the quantisation is ~2 us of ALU work per phase: both shrink by C.
+    // (st.shared::cluster). All 132 SMs pulling the same 16..64 KB out of L2 is what bounds the exchange (L2
+    // bandwidth, tools/latbench.cu part 3) and the quantisation is ALU work per phase: both shrink by C.
     // (Starting every CTA at a different offset of the vector was measured slower than walking it in the same order.)
     const int C = p.cluster;
     const int part = total / C;   // N is a multiple of 16: total is a multiple of 4
@@ -604,8 +604,8 @@ __device__ __noinline__ StatsOut slice_stats(const Params &p, const double *xown
     if (ctid < 32) {
         const int lane = ctid;
         const int nb = (int)gridDim.x;
-        // Every CTA reads every record: 148 x 32 lanes on the same few L2 lines serialise there (measured 1.6 us
-        // for one batch of loads). The writer stores kRep copies, reader b takes copy b % kRep.
+        // Every CTA reads every record: 132 x 32 lanes on the same few L2 lines serialise there
+        // for one batch of loads. The writer stores kRep copies, reader b takes copy b % kRep.
         TaggedDouble *const sums = recs + (size_t)(blockIdx.x % kRep) * 2 * nb, *const qs = sums + nb; // [nb] each
         const double v0 = lane < ne ? sm.xown[lane] : 0.0, v1 = lane + 32 < ne ? sm.xown[lane + 32] : 0.0;
         const double d0 = lane < ne ? v0 - c0 : 0.0, d1 = lane + 32 < ne ? v1 - c0 : 0.0;

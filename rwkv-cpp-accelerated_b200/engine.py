@@ -89,7 +89,7 @@ class Engine:
         ranks with tp.connect(engine) before the first forward (include/rwkv_b200.h, "tensor-parallel wiring")."""
         self.lib = load_library()
         if self.lib.rwkv_b200_device_count() <= 0:
-            raise EngineError("no CUDA device visible; the B200 engine has no CPU fallback")
+            raise EngineError("no CUDA device visible; the H100 engine has no CPU fallback")
         h = ctypes.c_void_p()
         L, E = ctypes.c_ulonglong(), ctypes.c_ulonglong()
         rc = self.lib.rwkv_b200_load_tp(path.encode(), max_gpt, device, 1 if quiet else 0, tp_rank, tp_size,
@@ -184,7 +184,7 @@ class Engine:
             raise EngineError("debug_read(%s) failed" % name)
         return a
 
-    def read_trace(self, grid=148, per_cta=2048):
+    def read_trace(self, grid=132, per_cta=2048):
         """Per-CTA globaltimer stamps of the last token kernel (set_option('trace', 1) first)."""
         a = np.zeros(grid * per_cta, np.uint64)
         got = self.lib.rwkv_b200_debug_read(self.h, b"trace", a.ctypes.data_as(ctypes.c_void_p), a.nbytes)
@@ -192,7 +192,7 @@ class Engine:
             raise EngineError("read_trace failed (trace option not enabled?)")
         return a.reshape(grid, per_cta)
 
-    def read_tile_trace(self, grid=148, per_cta=4096):
+    def read_tile_trace(self, grid=132, per_cta=4096):
         """[2][grid][per_cta] globaltimer: tile copy issued by the producer / tile seen ready by consumer thread 0."""
         a = np.zeros(2 * grid * per_cta, np.uint64)
         got = self.lib.rwkv_b200_debug_read(self.h, b"ptrace", a.ctypes.data_as(ctypes.c_void_p), a.nbytes)

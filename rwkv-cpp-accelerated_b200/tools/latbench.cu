@@ -1,6 +1,6 @@
 // latbench.cu — ground-truth latencies of the building blocks of the token kernel's phase boundaries on the
 // actual GPU, one warp, with the token kernel's shared-memory carve-out (227 KB -> almost no L1).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o latbench latbench.cu && ./latbench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o latbench latbench.cu && ./latbench
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -169,7 +169,7 @@ __global__ void __launch_bounds__(384, 1) k_env(const unsigned char *src, long l
                         asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(smem_addr(bar + 1)), "r"(parity) : "memory");
                     }
                     parity ^= 1;
-                    off = (off + 32768 * 148) & ((1ull << 30) - 1);
+                    off = (off + 32768 * 132) & ((1ull << 30) - 1);
                 }
             } else if (flags & 2) { // spin on a barrier nobody completes
                 uint32_t ok = 0;
@@ -216,7 +216,7 @@ struct Part2 {
         cudaMalloc(&dout, 256);
         cudaFuncSetAttribute(k_env, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448);
         for (int flags : {0, 1, 2, 3, 4, 7, 8, 9, 15}) {
-            k_env<<<148, 384, 232448>>>(src, out, dout, flags);
+            k_env<<<132, 384, 232448>>>(src, out, dout, flags);
             cudaError_t e = cudaDeviceSynchronize();
             if (e != cudaSuccess) {
                 printf("flags %d error: %s\n", flags, cudaGetErrorString(e));
@@ -249,14 +249,14 @@ __global__ void __launch_bounds__(384, 1) k_allgather(const unsigned char *src, 
                 asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(bar)), "r"(32768 * stream) : "memory");
                 for (int k = 0; k < stream; ++k)
                     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_addr(smem3 + 32768 * k)),
-                                 "l"(src + off + (size_t)k * 32768 * 148), "r"(32768), "r"(smem_addr(bar))
+                                 "l"(src + off + (size_t)k * 32768 * 132), "r"(32768), "r"(smem_addr(bar))
                                  : "memory");
                 uint32_t ok = 0;
                 while (!ok) {
                     asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(smem_addr(bar)), "r"(parity) : "memory");
                 }
                 parity ^= 1;
-                off = (off + (size_t)32768 * 148 * stream) & ((1ull << 30) - 1);
+                off = (off + (size_t)32768 * 132 * stream) & ((1ull << 30) - 1);
             }
         }
         return;
@@ -299,7 +299,7 @@ struct Part3 {
     Part3() {
         unsigned char *src;
         uint4 *vec;
-        long long *out, h[2 * 148];
+        long long *out, h[2 * 132];
         cudaMalloc(&src, (1ull << 30) + (64 << 20));
         cudaMalloc(&vec, 1 << 20);
         cudaMalloc(&out, sizeof(h));
@@ -308,7 +308,7 @@ struct Part3 {
         for (int groups : {1024, 3072, 4096}) {
             for (int stream : {0, 1, 3}) {
                 for (int rotate : {0, 1}) {
-                    k_allgather<<<148, 384, 232448>>>(src, vec, groups, out, stream, rotate);
+                    k_allgather<<<132, 384, 232448>>>(src, vec, groups, out, stream, rotate);
                     cudaError_t e = cudaDeviceSynchronize();
                     if (e != cudaSuccess) {
                         printf("allgather error: %s\n", cudaGetErrorString(e));
@@ -316,12 +316,12 @@ struct Part3 {
                     }
                     cudaMemcpy(h, out, sizeof(h), cudaMemcpyDeviceToHost);
                     long long mean = 0, mx = 0;
-                    for (int b = 0; b < 148; ++b) {
+                    for (int b = 0; b < 132; ++b) {
                         mean += h[2 * b];
                         if (h[2 * b] > mx) mx = h[2 * b];
                     }
-                    printf("all-gather of %5d x 16 B by 148 CTAs, %d tiles streaming per SM, rotate %d: mean %lld cycles, slowest CTA %lld\n", groups,
-                           stream, rotate, mean / 148, mx);
+                    printf("all-gather of %5d x 16 B by 132 CTAs, %d tiles streaming per SM, rotate %d: mean %lld cycles, slowest CTA %lld\n", groups,
+                           stream, rotate, mean / 132, mx);
                 }
             }
         }

@@ -12,7 +12,7 @@ pkg = importlib.import_module("rwkv-cpp-accelerated_b200")
 workload, steps = sys.argv[1], int(sys.argv[2])
 L, E = bench.SHAPES[workload]
 ab = bench.algorithmic_bytes_per_token(L, E)
-DEFAULTS = {"window": 2, "bwindow": 1, "pf_dist": 4, "poll_first": 2, "issue_gap": 0, "grid": 148}
+DEFAULTS = {"window": 2, "bwindow": 1, "pf_dist": 4, "poll_first": 2, "issue_gap": 0, "grid": 132}
 eng = pkg.Engine(bench.model_path(workload, pkg))
 stages0 = None
 for spec in sys.argv[3:]:

@@ -14,7 +14,7 @@ def shard(n, world, rank):
     return (n * rank) // world, (n * (rank + 1)) // world
 
 
-def cta_slices(n_embed, world, rank, grid=148, vocab=50277):
+def cta_slices(n_embed, world, rank, grid=132, vocab=50277):
     """Per-CTA row ranges inside rank `rank`'s shards - the arithmetic of make_slices() in csrc/token_kernel.cuh.
     Returns four lists of (first, count): residual elements (global, identical on every rank), att channels,
     ffn key channels and vocabulary rows (the last three relative to the rank's shard)."""

@@ -36,7 +36,7 @@ def test_static_library_exports_both_surfaces(static_lib):
     nm = _run(["nm", "-C", "--defined-only", static_lib])
     for sym in ("rwkv_b200_load", "rwkv_b200_forward", "cuda_rwkv_parralel(", "setState(", "getOutput(", "freeTensors(", "load(std::"):
         assert sym in nm, sym
-    assert "sm_100a" in subprocess.run(["cuobjdump", "-lelf", static_lib], capture_output=True, text=True).stdout
+    assert "sm_90a" in subprocess.run(["cuobjdump", "-lelf", static_lib], capture_output=True, text=True).stdout
 
 
 def test_reference_storygen_cmake_project_links(static_lib, tmp_path):
@@ -51,7 +51,7 @@ def test_reference_storygen_cmake_project_links(static_lib, tmp_path):
     os.symlink(static_lib, tree / "build" / "librwkv_cuda.a")    # ../../build/librwkv_cuda.a (CMakeLists.txt:35)
     b = tmp_path / "sg_build"
     gen = ["-G", "Ninja"] if shutil.which("ninja") else []
-    _run(["cmake", "-S", str(tree / "examples" / "storygen"), "-B", str(b), "-DCMAKE_CUDA_ARCHITECTURES=100a"] + gen)
+    _run(["cmake", "-S", str(tree / "examples" / "storygen"), "-B", str(b), "-DCMAKE_CUDA_ARCHITECTURES=90a"] + gen)
     _run(["cmake", "--build", str(b), "-j", "8"])
     exe = b / "storygen"
     assert exe.exists()

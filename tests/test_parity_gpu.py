@@ -1,13 +1,10 @@
-"""GPU parity: the CUDA engine (through the C ABI) vs the CPU oracle, and the oracle vs the
-unmodified reference CUDA build (oracle/_ref/ref_harness) where that binary exists.
+"""GPU parity: the CUDA engine (through the C ABI) vs the CPU oracle, and the oracle vs what the
+unmodified reference CUDA build computed (tests/golden/ref_oracle_3x768.npz).
 
 Tolerance (BASELINE.json north_star): logits within 1e-3 relative to the vector's
 max-abs; argmax identical wherever the reference's own top-1/top-2 margin exceeds 1e-3
 of max-abs (SURVEY.md H5: below that the reference's fp32 atomics decide the winner).
 """
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
@@ -204,12 +201,12 @@ def test_errors(pkg, make_model, tmp_path):
     e.close()
 
 
-def test_oracle_vs_reference_cuda(pkg, make_model, tmp_path):
-    """Pins the oracle: the UNMODIFIED reference (rwkv.cu + rwkv.h, built by oracle/Makefile
-    into oracle/_ref/) runs on this GPU on the same .bin and token stream."""
-    from oracle.oracle import Oracle, REF_HARNESS, read_ref_dump
-    if not os.path.exists(REF_HARNESS):
-        pytest.skip("oracle/_ref/ref_harness not built (needs /root/reference at build time)")
+def test_oracle_vs_reference_cuda(pkg, make_model):
+    """Pins the oracle: what the UNMODIFIED reference (rwkv.cu + rwkv.h) computed on the same .bin and token
+    stream, stored by tests/golden/make_reference_golden.py (case oracle_3x768)."""
+    from oracle.oracle import Oracle
+    from util import golden_logits_err, golden_state_err, reference_golden
+    g = reference_golden("oracle_3x768")
     path = make_model(3, 768)
     orc = Oracle(path)
     toks, tok, ref_logits = [], SEED_TOKEN, []
@@ -218,28 +215,22 @@ def test_oracle_vs_reference_cuda(pkg, make_model, tmp_path):
         lg = orc.forward(tok)
         ref_logits.append(lg)
         tok = int(lg.argmax())
-    tf = tmp_path / "toks.txt"
-    tf.write_text("\n".join(map(str, toks)))
-    dump = tmp_path / "ref.bin"
-    r = subprocess.run([REF_HARNESS, path, str(tf), str(dump)], capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-    d = read_ref_dump(str(dump))
-    assert d["steps"] == list(range(8))
+    assert toks == [int(t) for t in g["tokens"]], "the oracle's greedy stream differs from the one the reference ran"
+    assert [int(s) for s in g["steps"]] == list(range(8))
     worst = 0.0
-    for got, ref in zip(ref_logits, d["logits"]):
-        worst = max(worst, rel_err(got, ref))
+    for i, got in enumerate(ref_logits):
+        worst = max(worst, golden_logits_err(got, g, i))
     print("oracle vs reference CUDA: worst logits rel err %.3g" % worst)
     assert worst < 1e-4
     for k in ("xy", "aa", "bb", "dd"):
-        ref = d["state"][k]
-        assert np.abs(orc.state[k] - ref).max() / max(np.abs(ref).max(), 1e-6) < 1e-4, k
+        assert golden_state_err(orc.state[k], g, k) < 1e-4, k
     # and the engine against the reference itself, same stream
     eng = pkg.Engine(path)
-    for t, ref in zip(toks, d["logits"]):
+    for i, t in enumerate(toks):
         got = eng.forward([t])[0]
-        assert rel_err(got, ref) < REL_TOL
-        if margin(ref) > 1e-3:
-            assert int(got.argmax()) == int(ref.argmax())
+        assert golden_logits_err(got, g, i) < REL_TOL
+        if g["margin"][i] > 1e-3:
+            assert int(got.argmax()) == int(g["argmax"][i])
     eng.close()
 
 

@@ -18,7 +18,7 @@ def _gpus():
 
 
 @pytest.mark.parametrize("world,L,E,steps", [
-    (2, 2, 1024, 5),   # 512 channels per rank over 148 CTAs: 3-4 per CTA
+    (2, 2, 1024, 5),   # 512 channels per rank over 132 CTAs: 3-4 per CTA
     (2, 2, 4096, 4),   # 7B width
     (4, 1, 5120, 3),   # 14B width on four ranks
     (4, 3, 768, 6),    # 169M width: 192 channels per rank, one or two per CTA

@@ -20,7 +20,7 @@ def tp():
 def test_shards_and_slices_cover_everything_once(tp, n_embed, world):
     """Every att channel, ffn key channel and vocabulary row belongs to exactly one (rank, CTA); the residual
     slices are the same on every rank; the per-rank weight bytes add up to the whole model."""
-    grid, vocab, L = 148, 50277, 3
+    grid, vocab, L = 132, 50277, 3
     seen_c, seen_k, seen_v = [], [], []
     for rank in range(world):
         c0, c1 = tp.shard(n_embed, world, rank)
