@@ -115,7 +115,8 @@ int rwkv_b200_state_zero(rwkv_b200_model *m);
  * (set_option "prefill" = "0" forces token by token, "prefill_graph" = "0" eager launches).
  * Replaces `cuda_rwkv_parralel(...)` + the logits copy of `getOutput`
  * (R.h:104-122, R.cu:493-593, 471). mode GPT: tokens are consumed in order on state
- * slot 0; mode PARRALEL: token t uses state slot t. n_tokens <= max_gpt.
+ * slot 0; mode PARRALEL: token t uses state slot t. n_tokens <= max_gpt. Both modes are special cases of
+ * rwkv_b200_forward_streams (one stream on slot 0 / n_tokens streams of one token) with logits of every token.
  * `logits_out` may be NULL (state-only prefill: logits stay on the device). */
 int rwkv_b200_forward(rwkv_b200_model *m, const unsigned long long *tokens,
                       unsigned long long n_tokens, int mode, float *logits_out);
@@ -168,6 +169,39 @@ unsigned long long rwkv_b200_launch_count(const rwkv_b200_model *m);
  * the host's token in every case re-samples on the host when margin < 1e-9 (RWKV::sample does). */
 int rwkv_b200_sample_typical(rwkv_b200_model *m, float temp, double u, unsigned long long *token,
                              double *margin);
+
+/* --- multi-stream serving: independent conversations on their own state slots ------
+ * No reference counterpart. One loaded model serves up to max_gpt conversations, each on its own state slot;
+ * the weights are read once per pass for every live conversation. Every entry point below returns
+ * "not supported with tensor parallelism" when tp_size > 1, and validates its input before any work: a rejected
+ * call leaves the state untouched. */
+
+/* One ragged forward. `tokens` are stream-major: stream s owns lengths[s] consecutive tokens and advances state
+ * slot slots[s]; its first token continues from what the slot holds. Slots are distinct and < max_gpt, lengths
+ * >= 1 and add up to n_tokens <= max_gpt, token ids < 50277. A prompt chunk of one conversation and the next token
+ * of the others may share one call. logits_out (host, [n_streams][50277]) receives each stream's logits after its
+ * last token, next_out (host, [n_streams]) their arg-max taken on the device (first index on ties); both NULL =
+ * state only (no head). Calls of prefill_min tokens or more run on the tensor cores in passes of at most 128
+ * tokens (the same numbers, bit for bit, as each stream run alone there); shorter calls, and "prefill" = "0", run
+ * token by token through the decode kernel. Slots not named are not touched. */
+int rwkv_b200_forward_streams(rwkv_b200_model *m, const unsigned long long *tokens, unsigned long long n_tokens,
+                              const unsigned long long *slots, const unsigned long long *lengths,
+                              unsigned long long n_streams, float *logits_out, unsigned long long *next_out);
+
+/* rwkv_b200_sample_typical on each row of the last forward_streams call (which must have produced logits or
+ * arg-maxes for exactly n_streams streams): row s draws with the uniform u[s] into tokens_out[s], margins_out[s]
+ * (may be NULL). */
+int rwkv_b200_sample_typical_streams(rwkv_b200_model *m, unsigned long long n_streams, float temp,
+                                     const double *u, unsigned long long *tokens_out, double *margins_out);
+
+/* State of one slot: zero it (a new conversation), copy it onto another slot (fork a conversation), or move it
+ * between the device and host arrays of n_layers x n_embed doubles each (NULL arrays are skipped). */
+int rwkv_b200_slot_zero(rwkv_b200_model *m, unsigned long long slot);
+int rwkv_b200_slot_copy(rwkv_b200_model *m, unsigned long long src, unsigned long long dst);
+int rwkv_b200_slot_upload(rwkv_b200_model *m, unsigned long long slot, const double *xy, const double *aa,
+                          const double *bb, const double *pp, const double *dd);
+int rwkv_b200_slot_download(rwkv_b200_model *m, unsigned long long slot, double *xy, double *aa,
+                            double *bb, double *pp, double *dd);
 
 /* Engine knobs (all optional), key/value strings: "window" / "bwindow" (bulk copies in
  * flight per SM while streaming / while the CTAs exchange vectors), "pf_dist" (tiles the L2

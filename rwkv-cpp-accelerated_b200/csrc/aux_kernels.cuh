@@ -49,11 +49,11 @@ __global__ void k_centre_offsets(const float *__restrict__ r, const float *__res
 // Device-side restatement of the reference sampler (include/rwkv/sampler/typical.h = what the
 // reference's typical.h:20-58 actually computes): probs = exp(l)/sum, probs^e with e = uint8(1/temp),
 // renormalise, cumulative sums, first index whose cumulative probability reaches the uniform `u`
-// drawn on the host. One CTA, every thread owns a contiguous run of the vocabulary. Sums are block
+// drawn on the host. One CTA per row of logits, every thread owns a contiguous run of the vocabulary. Sums are block
 // reductions, so cumulative values can differ from the host's sequential ones by ~1e-13; the kernel
 // therefore also returns how far `u` is from the nearest interval boundary, and the caller falls
 // back to the host path when that margin is below 1e-9 (probability ~1e-9 per draw): identical
-// tokens by construction. out[0] = token, out[1] = margin.
+// tokens by construction. Row r: out[2r] = token, out[2r + 1] = margin.
 // ---------------------------------------------------------------------------------------
 constexpr int kSampleThreads = 1024;
 __device__ __forceinline__ double sample_prob(float logit, double total, int exponent) {
@@ -90,10 +90,14 @@ __device__ __forceinline__ double block_sum_scan(double v, double *sh, double &p
     __syncthreads();
     return total;
 }
-__global__ void __launch_bounds__(kSampleThreads) k_sample_typical(const float *logits, int len, int exponent, double u,
-                                                                  double *out) {
+// One CTA per row: row r samples logits + r * row_stride with u[r] into out[2r], out[2r + 1].
+__global__ void __launch_bounds__(kSampleThreads) k_sample_typical(const float *logits, size_t row_stride, int len, int exponent,
+                                                                  const double *us, double *out) {
     __shared__ double sh[64];
     __shared__ double starts[kSampleThreads + 1];
+    logits += (size_t)blockIdx.x * row_stride;
+    out += 2 * (size_t)blockIdx.x;
+    const double u = us[blockIdx.x];
     const int per = (len + kSampleThreads - 1) / kSampleThreads;
     const int i0 = min(len, (int)threadIdx.x * per), i1 = min(len, i0 + per);
     double dummy;
@@ -127,6 +131,45 @@ __global__ void __launch_bounds__(kSampleThreads) k_sample_typical(const float *
         }
         out[0] = (double)tok;
         out[1] = margin;
+    }
+}
+
+// One CTA per row of logits[rows][V]: arg-max, the first index wins ties (as the decode kernel's greedy arg-max).
+constexpr int kArgmaxThreads = 256;
+__global__ void __launch_bounds__(kArgmaxThreads) k_argmax_rows(const float *logits, int V, unsigned long long *out) {
+    __shared__ float bv[kArgmaxThreads / 32];
+    __shared__ int bi[kArgmaxThreads / 32];
+    const float *row = logits + (size_t)blockIdx.x * V;
+    float best = -INFINITY;
+    int bidx = 0x7fffffff;
+    for (int i = threadIdx.x; i < V; i += kArgmaxThreads) {
+        const float y = row[i];
+        if (y > best) { // i ascending per thread: first maximum kept
+            best = y;
+            bidx = i;
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bidx, o);
+        if (ov > best || (ov == best && oi < bidx)) {
+            best = ov;
+            bidx = oi;
+        }
+    }
+    if ((threadIdx.x & 31) == 0) {
+        bv[threadIdx.x >> 5] = best;
+        bi[threadIdx.x >> 5] = bidx;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < kArgmaxThreads / 32; ++w)
+            if (bv[w] > best || (bv[w] == best && bi[w] < bidx)) {
+                best = bv[w];
+                bidx = bi[w];
+            }
+        out[blockIdx.x] = (unsigned long long)bidx;
     }
 }
 

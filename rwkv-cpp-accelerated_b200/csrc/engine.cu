@@ -64,7 +64,11 @@ struct rwkv_b200_model {
     int sms = 0;
     int grid = 0;
     int cpl = 0;
-    double *d_sample = nullptr, *h_sample = nullptr; // device sampler result {token, margin}
+    double *d_sample = nullptr, *h_sample = nullptr; // device sampler results {token, margin} per row, [max_gpt][2]
+    double *d_u = nullptr;                            // the sampler's uniforms, [max_gpt]
+    float *d_slogits = nullptr;       // [max_gpt][V] compact logits rows (forward_streams: one per stream)
+    unsigned long long *d_next = nullptr; // [max_gpt] arg-max of each row of d_slogits
+    unsigned long long stream_rows = 0;   // rows of d_slogits the last forward_streams call produced (0: none)
     size_t xch_bytes = 0;   // exchange block (peer-visible with tensor parallelism)
     bool tp_wired = false;  // peers' exchange blocks imported
     std::vector<void *> ipc_opened;
@@ -501,7 +505,11 @@ int do_load(M *m, const char *path, int quiet) {
 
     CK(cudaMallocHost((void **)&m->h_ctrl, sizeof(rk::Ctrl) * m->max_gpt));
     CK(cudaMallocHost((void **)&m->h_logits, sizeof(float) * V * m->max_gpt));
-    CK(cudaMallocHost((void **)&m->h_next, sizeof(unsigned long long)));
+    CK(cudaMallocHost((void **)&m->h_next, sizeof(unsigned long long) * m->max_gpt));
+    CK(cudaMallocHost((void **)&m->h_sample, 2 * sizeof(double) * m->max_gpt));
+    if ((rc = dmalloc(m, &m->d_slogits, (size_t)V * m->max_gpt)) || (rc = dmalloc(m, &m->d_next, m->max_gpt)) ||
+        (rc = dmalloc(m, &m->d_sample, 2 * m->max_gpt)) || (rc = dmalloc(m, &m->d_u, m->max_gpt)))
+        return rc;
     CK(cudaHostAlloc((void **)&m->h_diag, sizeof(rk::Diag), cudaHostAllocMapped));
     memset(m->h_diag, 0, sizeof(rk::Diag));
     CK(cudaHostGetDevicePointer((void **)&p.diag, m->h_diag, 0));
@@ -516,6 +524,28 @@ int check_model(const M *m) {
 }
 
 float *dev_logits(M *m) { return reinterpret_cast<float *>(m->p.xch[m->tp_rank] + m->p.off_logits); }
+
+// the reference applies the temperature as probs ^ uint8(1 / temp) (include/rwkv/sampler/typical.h)
+int sample_exponent(float temp) { return temp != 1.0f ? (int)(unsigned char)(1.0 / (double)temp) : 1; }
+
+// The five state arrays of one slot: xy, aa, bb, pp, dd ([L][E] doubles each at offset slot * L * E).
+void slot_arrays(M *m, unsigned long long slot, double *(&a)[5]) {
+    const size_t o = (size_t)(slot * m->L * m->E);
+    double *base[5] = {m->p.sxy, (double *)m->tensors[STATEAA], (double *)m->tensors[STATEBB], m->spp, m->p.sdd};
+    for (int i = 0; i < 5; ++i) a[i] = base[i] + o;
+}
+
+// Common checks of the multi-stream entry points.
+int check_streams_model(M *m, const char *what) {
+    int rc = check_model(m);
+    if (rc) return rc;
+    if (m->tp_size > 1) return fail(7, "%s: not supported with tensor parallelism", what);
+    return 0;
+}
+int check_slot(M *m, const char *what, unsigned long long slot) {
+    if (slot >= m->max_gpt) return fail(1, "%s: slot %llu >= max_gpt %llu", what, slot, m->max_gpt);
+    return 0;
+}
 
 } // namespace
 
@@ -666,11 +696,19 @@ int rwkv_b200_forward(rwkv_b200_model *m, const unsigned long long *tokens, unsi
     const size_t V = binfmt::kVocab;
     for (unsigned long long t = 0; t < n_tokens; ++t)
         if (tokens[t] >= V) return fail(1, "token id %llu out of range", tokens[t]);
+    m->stream_rows = 0;
     if (n_tokens >= (unsigned long long)m->pf.min_tokens && m->tp_size == 1 && rk::prefill_enabled(m->pf)) {
-        rc = rk::prefill_forward(m->pf, m->p, m->stream, tokens, (int)n_tokens, mode == RWKV_B200_MODE_PARRALEL,
-                                 logits_out ? m->h_logits : nullptr);
+        // GPT: one stream on slot 0; PARRALEL: n streams of one token on slots 0..n-1. Logits of every token.
+        const bool par = mode == RWKV_B200_MODE_PARRALEL;
+        if (par && n_tokens > (unsigned long long)rk::kPfMaxTokens)
+            return fail(3, "batched prefill: PARRALEL chunks above 128 tokens are not supported");
+        std::vector<unsigned long long> slots(par ? n_tokens : 1), lens(par ? n_tokens : 1, par ? 1 : n_tokens);
+        for (size_t i = 0; i < slots.size(); ++i) slots[i] = i;
+        rc = rk::prefill_forward(m->pf, m->p, m->stream, tokens, (int)n_tokens, slots.data(), lens.data(), (int)slots.size(),
+                                 logits_out ? 1 : 0, m->d_slogits);
         if (rc) return fail(rc, "%s", rk::prefill_error());
         m->launches += rk::prefill_launches(m->pf);
+        if (logits_out) CK(cudaMemcpyAsync(m->h_logits, m->d_slogits, n_tokens * V * sizeof(float), cudaMemcpyDeviceToHost, m->stream));
         SYNC(m);
         if (logits_out && logits_out != m->h_logits) memcpy(logits_out, m->h_logits, n_tokens * V * sizeof(float));
         return 0;
@@ -697,6 +735,7 @@ int rwkv_b200_forward_greedy(rwkv_b200_model *m, unsigned long long token, unsig
     const size_t V = binfmt::kVocab;
     if (token >= V) return fail(1, "token id %llu out of range", token);
     CK(cudaSetDevice(m->device));
+    m->stream_rows = 0;
     rk::Ctrl &c = m->h_ctrl[0];
     c.token = token;
     c.next = 0;
@@ -719,19 +758,148 @@ int rwkv_b200_sample_typical(rwkv_b200_model *m, float temp, double u, unsigned 
     if (rc) return rc;
     if (!token) return fail(1, "null argument");
     CK(cudaSetDevice(m->device));
-    if (!m->d_sample) {
-        if ((rc = dmalloc(m, &m->d_sample, 2))) return rc;
-        CK(cudaMallocHost((void **)&m->h_sample, 2 * sizeof(double)));
-    }
-    // the reference applies the temperature as probs ^ uint8(1 / temp) (include/rwkv/sampler/typical.h)
-    const int exponent = temp != 1.0f ? (int)(unsigned char)(1.0 / (double)temp) : 1;
-    rk::k_sample_typical<<<1, rk::kSampleThreads, 0, m->stream>>>(dev_logits(m), (int)binfmt::kVocab, exponent, u, m->d_sample);
+    CK(cudaMemcpyAsync(m->d_u, &u, sizeof(double), cudaMemcpyHostToDevice, m->stream));
+    rk::k_sample_typical<<<1, rk::kSampleThreads, 0, m->stream>>>(dev_logits(m), 0, (int)binfmt::kVocab, sample_exponent(temp), m->d_u,
+                                                                  m->d_sample);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(m->h_sample, m->d_sample, 2 * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
     SYNC(m);
     *token = (unsigned long long)m->h_sample[0];
     if (margin) *margin = m->h_sample[1];
     m->launches += 1;
+    return 0;
+}
+
+int rwkv_b200_forward_streams(rwkv_b200_model *m, const unsigned long long *tokens, unsigned long long n_tokens,
+                              const unsigned long long *slots, const unsigned long long *lengths,
+                              unsigned long long n_streams, float *logits_out, unsigned long long *next_out) {
+    int rc = check_streams_model(m, "forward_streams");
+    if (rc) return rc;
+    if (!tokens || !slots || !lengths || n_tokens == 0 || n_streams == 0) return fail(1, "forward_streams: no tokens or no streams");
+    if (n_tokens > m->max_gpt) return fail(1, "forward_streams: %llu tokens > max_gpt %llu", n_tokens, m->max_gpt);
+    if (n_streams > n_tokens) return fail(1, "forward_streams: %llu streams for %llu tokens", n_streams, n_tokens);
+    const size_t V = binfmt::kVocab;
+    for (unsigned long long t = 0; t < n_tokens; ++t)
+        if (tokens[t] >= V) return fail(1, "forward_streams: token id %llu out of range", tokens[t]);
+    std::vector<char> used(m->max_gpt, 0);
+    unsigned long long total = 0;
+    for (unsigned long long i = 0; i < n_streams; ++i) {
+        if ((rc = check_slot(m, "forward_streams", slots[i]))) return rc;
+        if (used[slots[i]]) return fail(1, "forward_streams: slot %llu appears twice", slots[i]);
+        used[slots[i]] = 1;
+        if (lengths[i] == 0 || lengths[i] > n_tokens) return fail(1, "forward_streams: stream %llu has length %llu", i, lengths[i]);
+        total += lengths[i];
+    }
+    if (total != n_tokens) return fail(1, "forward_streams: the lengths add up to %llu, not n_tokens = %llu", total, n_tokens);
+    CK(cudaSetDevice(m->device));
+    const bool head = logits_out || next_out;
+    m->stream_rows = 0;
+    if (n_tokens >= (unsigned long long)m->pf.min_tokens && rk::prefill_enabled(m->pf)) {
+        rc = rk::prefill_forward(m->pf, m->p, m->stream, tokens, (int)n_tokens, slots, lengths, (int)n_streams, head ? 2 : 0, m->d_slogits);
+        if (rc) return fail(rc, "%s", rk::prefill_error());
+        m->launches += rk::prefill_launches(m->pf);
+    } else {
+        // token by token through the decode kernel on each stream's slot; the last logits of a stream are copied
+        // into the compact buffer, so the arg-max and the sampler read the same rows as after a batched pass
+        unsigned long long t = 0;
+        for (unsigned long long i = 0; i < n_streams; ++i)
+            for (unsigned long long j = 0; j < lengths[i]; ++j, ++t) {
+                rk::Ctrl &c = m->h_ctrl[t];
+                c.token = tokens[t];
+                c.next = 0;
+                c.slot = slots[i];
+                c.pos = 0;
+                CK(cudaMemcpyAsync(m->p.ctrl, &c, sizeof(rk::Ctrl), cudaMemcpyHostToDevice, m->stream));
+                if ((rc = launch_token(m, 0, false, nullptr, m->stream))) return rc;
+                if (head && j + 1 == lengths[i])
+                    CK(cudaMemcpyAsync(m->d_slogits + i * V, dev_logits(m), V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
+            }
+    }
+    if (next_out) {
+        rk::k_argmax_rows<<<(unsigned)n_streams, rk::kArgmaxThreads, 0, m->stream>>>(m->d_slogits, (int)V, m->d_next);
+        CK(cudaGetLastError());
+        m->launches += 1;
+        CK(cudaMemcpyAsync(m->h_next, m->d_next, n_streams * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+    }
+    if (logits_out) CK(cudaMemcpyAsync(m->h_logits, m->d_slogits, n_streams * V * sizeof(float), cudaMemcpyDeviceToHost, m->stream));
+    SYNC(m);
+    if (next_out) memcpy(next_out, m->h_next, n_streams * sizeof(unsigned long long));
+    if (logits_out && logits_out != m->h_logits) memcpy(logits_out, m->h_logits, n_streams * V * sizeof(float));
+    m->stream_rows = head ? n_streams : 0;
+    return 0;
+}
+
+int rwkv_b200_sample_typical_streams(rwkv_b200_model *m, unsigned long long n_streams, float temp, const double *u,
+                                     unsigned long long *tokens_out, double *margins_out) {
+    int rc = check_streams_model(m, "sample_typical_streams");
+    if (rc) return rc;
+    if (!u || !tokens_out) return fail(1, "sample_typical_streams: null argument");
+    if (m->stream_rows == 0) return fail(1, "sample_typical_streams: the last forward produced no per-stream logits (call forward_streams with logits or next)");
+    if (n_streams != m->stream_rows)
+        return fail(1, "sample_typical_streams: %llu rows asked, the last forward_streams produced %llu", n_streams, m->stream_rows);
+    CK(cudaSetDevice(m->device));
+    CK(cudaMemcpyAsync(m->d_u, u, n_streams * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+    rk::k_sample_typical<<<(unsigned)n_streams, rk::kSampleThreads, 0, m->stream>>>(m->d_slogits, binfmt::kVocab, (int)binfmt::kVocab,
+                                                                                   sample_exponent(temp), m->d_u, m->d_sample);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(m->h_sample, m->d_sample, 2 * n_streams * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+    SYNC(m);
+    for (unsigned long long i = 0; i < n_streams; ++i) {
+        tokens_out[i] = (unsigned long long)m->h_sample[2 * i];
+        if (margins_out) margins_out[i] = m->h_sample[2 * i + 1];
+    }
+    m->launches += 1;
+    return 0;
+}
+
+int rwkv_b200_slot_zero(rwkv_b200_model *m, unsigned long long slot) {
+    int rc = check_streams_model(m, "slot_zero");
+    if (rc || (rc = check_slot(m, "slot_zero", slot))) return rc;
+    CK(cudaSetDevice(m->device));
+    double *a[5];
+    slot_arrays(m, slot, a);
+    for (double *p : a) CK(cudaMemsetAsync(p, 0, (size_t)(m->L * m->E) * sizeof(double), m->stream));
+    SYNC(m);
+    return 0;
+}
+
+int rwkv_b200_slot_copy(rwkv_b200_model *m, unsigned long long src, unsigned long long dst) {
+    int rc = check_streams_model(m, "slot_copy");
+    if (rc || (rc = check_slot(m, "slot_copy", src)) || (rc = check_slot(m, "slot_copy", dst))) return rc;
+    if (src == dst) return 0;
+    CK(cudaSetDevice(m->device));
+    double *a[5], *b[5];
+    slot_arrays(m, src, a);
+    slot_arrays(m, dst, b);
+    for (int i = 0; i < 5; ++i) CK(cudaMemcpyAsync(b[i], a[i], (size_t)(m->L * m->E) * sizeof(double), cudaMemcpyDeviceToDevice, m->stream));
+    SYNC(m);
+    return 0;
+}
+
+int rwkv_b200_slot_upload(rwkv_b200_model *m, unsigned long long slot, const double *xy, const double *aa, const double *bb,
+                          const double *pp, const double *dd) {
+    int rc = check_streams_model(m, "slot_upload");
+    if (rc || (rc = check_slot(m, "slot_upload", slot))) return rc;
+    CK(cudaSetDevice(m->device));
+    double *a[5];
+    slot_arrays(m, slot, a);
+    const double *src[5] = {xy, aa, bb, pp, dd};
+    for (int i = 0; i < 5; ++i)
+        if (src[i]) CK(cudaMemcpyAsync(a[i], src[i], (size_t)(m->L * m->E) * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+    SYNC(m);
+    return 0;
+}
+
+int rwkv_b200_slot_download(rwkv_b200_model *m, unsigned long long slot, double *xy, double *aa, double *bb, double *pp, double *dd) {
+    int rc = check_streams_model(m, "slot_download");
+    if (rc || (rc = check_slot(m, "slot_download", slot))) return rc;
+    CK(cudaSetDevice(m->device));
+    double *a[5];
+    slot_arrays(m, slot, a);
+    double *dst[5] = {xy, aa, bb, pp, dd};
+    for (int i = 0; i < 5; ++i)
+        if (dst[i]) CK(cudaMemcpyAsync(dst[i], a[i], (size_t)(m->L * m->E) * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+    SYNC(m);
     return 0;
 }
 

@@ -66,6 +66,12 @@ def load_library():
         "rwkv_b200_tp_buffer_bytes": (c.c_size_t, [vp]),
         "rwkv_b200_tp_export": (i32, [vp, vp]),
         "rwkv_b200_tp_import": (i32, [vp, vp]),
+        "rwkv_b200_forward_streams": (i32, [vp, pull, ull, pull, pull, ull, pflt, pull]),
+        "rwkv_b200_sample_typical_streams": (i32, [vp, ull, c.c_float, pdbl, pull, pdbl]),
+        "rwkv_b200_slot_zero": (i32, [vp, ull]),
+        "rwkv_b200_slot_copy": (i32, [vp, ull, ull]),
+        "rwkv_b200_slot_upload": (i32, [vp, ull, pdbl, pdbl, pdbl, pdbl, pdbl]),
+        "rwkv_b200_slot_download": (i32, [vp, ull, pdbl, pdbl, pdbl, pdbl, pdbl]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)  # AttributeError if a declared symbol is missing
@@ -153,6 +159,49 @@ class Engine:
         self._ck(self.lib.rwkv_b200_forward_greedy(self.h, int(token), ctypes.byref(nxt),
                                                    _ptr(out, ctypes.c_float)), "forward_greedy")
         return (nxt.value, out) if want_logits else nxt.value
+
+    # -- multi-stream serving --------------------------------------------------------------
+    def forward_streams(self, streams, want_logits=True, want_next=False):
+        """One ragged forward: streams = [(slot, tokens), ...], each advancing its own state slot.
+        Returns (logits [S][V] after each stream's last token | None, device arg-max [S] | None)."""
+        slots = np.ascontiguousarray([int(s) for s, _ in streams], dtype=np.uint64)
+        seqs = [np.atleast_1d(np.asarray(t, dtype=np.uint64)) for _, t in streams]
+        lens = np.ascontiguousarray([len(t) for t in seqs], dtype=np.uint64)
+        toks = np.ascontiguousarray(np.concatenate(seqs) if seqs else np.zeros(0, np.uint64))
+        logits = np.empty((len(seqs), VOCAB), np.float32) if want_logits else None
+        nxt = np.empty(len(seqs), np.uint64) if want_next else None
+        self._ck(self.lib.rwkv_b200_forward_streams(self.h, _ptr(toks, ctypes.c_ulonglong), len(toks),
+                                                    _ptr(slots, ctypes.c_ulonglong), _ptr(lens, ctypes.c_ulonglong),
+                                                    len(seqs), _ptr(logits, ctypes.c_float),
+                                                    _ptr(nxt, ctypes.c_ulonglong)), "forward_streams")
+        return logits, nxt
+
+    def sample_typical_streams(self, temp, us):
+        """Device sampler on every row of the last forward_streams call: (tokens [S], margins [S])."""
+        u = np.ascontiguousarray(us, dtype=np.float64)
+        toks = np.empty(len(u), np.uint64)
+        margins = np.empty(len(u), np.float64)
+        self._ck(self.lib.rwkv_b200_sample_typical_streams(self.h, len(u), temp, _ptr(u, ctypes.c_double),
+                                                           _ptr(toks, ctypes.c_ulonglong), _ptr(margins, ctypes.c_double)),
+                 "sample_typical_streams")
+        return toks, margins
+
+    def slot_zero(self, slot):
+        self._ck(self.lib.rwkv_b200_slot_zero(self.h, slot), "slot_zero")
+
+    def slot_copy(self, src, dst):
+        self._ck(self.lib.rwkv_b200_slot_copy(self.h, src, dst), "slot_copy")
+
+    def slot_download(self, slot):
+        n = self.n_layers * self.n_embed
+        arrs = [np.empty(n, np.float64) for _ in range(5)]
+        self._ck(self.lib.rwkv_b200_slot_download(self.h, slot, *[_ptr(a, ctypes.c_double) for a in arrs]), "slot_download")
+        return dict(zip(("xy", "aa", "bb", "pp", "dd"), arrs))
+
+    def slot_upload(self, slot, st):
+        arrs = [np.ascontiguousarray(st[k], np.float64) if st.get(k) is not None else None
+                for k in ("xy", "aa", "bb", "pp", "dd")]
+        self._ck(self.lib.rwkv_b200_slot_upload(self.h, slot, *[_ptr(a, ctypes.c_double) for a in arrs]), "slot_upload")
 
     # -- state -----------------------------------------------------------------------------
     def state_zero(self):

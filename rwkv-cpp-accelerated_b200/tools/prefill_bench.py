@@ -1,4 +1,4 @@
-"""Batched path (tcgen05 integer GEMMs) against the token-by-token decode kernel for T tokens in one call:
+"""Batched path (wgmma integer GEMMs) against the token-by-token decode kernel for T tokens in one call:
 wall time of `forward` (host timed, synchronous call, logits of the last token only in GPT mode).
 usage: python prefill_bench.py [workload=7b] [T ...]"""
 import importlib
