@@ -172,7 +172,9 @@ int rwkv_b200_sample_typical(rwkv_b200_model *m, float temp, double u, unsigned 
 
 /* --- multi-stream serving: independent conversations on their own state slots ------
  * No reference counterpart. One loaded model serves up to max_gpt conversations, each on its own state slot;
- * the weights are read once per pass for every live conversation. Every entry point below returns
+ * the weights are read once per pass for every live conversation. A caller either steps the conversations itself
+ * (forward_streams, then the arg-max or sample_typical_streams) or hands the whole decode loop to the device
+ * (generate_streams: many steps, picks and stop checks per call). Every entry point below returns
  * "not supported with tensor parallelism" when tp_size > 1, and validates its input before any work: a rejected
  * call leaves the state untouched. */
 
@@ -193,6 +195,30 @@ int rwkv_b200_forward_streams(rwkv_b200_model *m, const unsigned long long *toke
  * (may be NULL). */
 int rwkv_b200_sample_typical_streams(rwkv_b200_model *m, unsigned long long n_streams, float temp,
                                      const double *u, unsigned long long *tokens_out, double *margins_out);
+
+/* Generate up to max_new tokens for each of n_streams conversations without returning to the host between steps.
+ * Stream s continues on state slot slots[s]; its first input is first_tokens[s]. Each step feeds every live stream
+ * its current token, picks the next one on the device, and emits it: arg-max when u == NULL (first index on ties),
+ * else the typical sampler of rwkv_b200_sample_typical_streams with temp and the uniform u[step * n_streams + s]
+ * (u: [max_new][n_streams], each in [0, 1)). Before each pick, logits[override_tokens[i]] = override_values[i]
+ * (e.g. -99 on token 0 keeps a story from ending).
+ * A stream stops after emitting a token in stop_tokens, or after budgets[s] tokens (NULL = max_new for every stream;
+ * otherwise each in 1..max_new). The emitted stop token / last token is NOT fed: the slot ends where the equivalent
+ * host loop (forward_streams, pick, append, check) would leave it, so a caller continues a conversation by feeding
+ * tokens_out[s][lengths_out[s] - 1]. Emitted tokens and the slot states are bit for bit those of that loop run on the
+ * same path: the tensor cores when n_streams >= prefill_min (and "prefill" is on), else the decode kernel; the path
+ * does not change inside a call.
+ * The device draw is final: unlike RWKV::sample, nothing re-samples on the host when the margin of u is below 1e-9.
+ * tokens_out: [n_streams][max_new] host (entries past lengths_out[s] are 0); lengths_out: [n_streams] host.
+ * Slots are distinct and < max_gpt, token ids < 50277, max_new >= 1; a count > 0 needs its array. After the call no
+ * per-stream logits are held: rwkv_b200_sample_typical_streams is refused until the next forward_streams. */
+int rwkv_b200_generate_streams(rwkv_b200_model *m, const unsigned long long *slots,
+                               const unsigned long long *first_tokens, unsigned long long n_streams,
+                               unsigned long long max_new, const unsigned long long *budgets,
+                               const unsigned long long *stop_tokens, unsigned long long n_stop,
+                               const unsigned long long *override_tokens, const float *override_values,
+                               unsigned long long n_override, float temp, const double *u,
+                               unsigned long long *tokens_out, unsigned long long *lengths_out);
 
 /* State of one slot: zero it (a new conversation), copy it onto another slot (fork a conversation), or move it
  * between the device and host arrays of n_layers x n_embed doubles each (NULL arrays are skipped). */

@@ -30,6 +30,7 @@
 #include "../../include/rwkv_b200.h"
 #include "aux_kernels.cuh"
 #include "binfmt.h"
+#include "generate.cuh"
 #include "prefill.cuh"
 #include "token_kernel.cuh"
 
@@ -88,6 +89,18 @@ struct rwkv_b200_model {
     unsigned int epoch = 0, tk = 0; // exchange epochs (token_kernel.cuh); identical on every rank
     int tp_rank = 0, tp_size = 1;
     rk::PrefillState pf{};
+    // generate_streams: per-stream records (device, and their pinned host mirror), the row map and the pass
+    // descriptors are sized at load; the rest grows with the largest call and is freed with the model
+    struct Gen {
+        rk::GenStream *gs = nullptr, *h_gs = nullptr; // [max_gpt]
+        int *row_stream = nullptr;                     // [max_gpt] stream of each row of the current group
+        rk::PassDesc *passes = nullptr;                // [ceil(max_gpt / 128)] next step's passes (tensor cores)
+        unsigned long long *out = nullptr;             // [n_streams][max_new] emitted tokens
+        unsigned long long *stop = nullptr, *ovr_tok = nullptr;
+        float *ovr_val = nullptr;
+        double *u = nullptr; // [group steps][rows] uniforms of the current group
+        size_t out_cap = 0, stop_cap = 0, ovr_cap = 0, ovr_val_cap = 0, u_cap = 0;
+    } gen;
 };
 
 namespace {
@@ -458,9 +471,13 @@ int do_load(M *m, const char *path, int quiet) {
     m->tensors[FFNK] = wfk; m->tensors[FFNV] = wfv; m->tensors[FFNR] = wfr; m->tensors[HEAD] = whead;
 
     // ---- state, activations, control ------------------------------------------------------------
-    const size_t sn = (size_t)(L * E * m->max_gpt);
-    if ((rc = dmalloc(m, &p.sxy, sn)) || (rc = dmalloc(m, &p.sdd, sn)) || (rc = dmalloc(m, &m->spp, sn))) return rc;
-    for (double *s : {p.sxy, p.sdd, m->spp}) CK(cudaMemsetAsync(s, 0, sn * sizeof(double), m->stream));
+    // The arrays the decode kernel reads and writes hold one slot more than max_gpt: generate_streams runs a finished
+    // stream that still occupies a row on that scratch slot (index max_gpt). No public entry point reaches it.
+    const size_t sn = (size_t)(L * E * m->max_gpt), sn1 = (size_t)(L * E * (m->max_gpt + 1));
+    if ((rc = dmalloc(m, &p.sxy, sn1)) || (rc = dmalloc(m, &p.sdd, sn1)) || (rc = dmalloc(m, &m->spp, sn))) return rc;
+    CK(cudaMemsetAsync(p.sxy, 0, sn1 * sizeof(double), m->stream));
+    CK(cudaMemsetAsync(p.sdd, 0, sn1 * sizeof(double), m->stream));
+    CK(cudaMemsetAsync(m->spp, 0, sn * sizeof(double), m->stream));
     double *b1, *fkb, *fvb;
     float *b3, *b4, *frb;
     if ((rc = dmalloc(m, &p.x, E)) || (rc = dmalloc(m, &p.ctrl, 1)) || (rc = dmalloc(m, &b1, E)) || (rc = dmalloc(m, &fkb, E)) ||
@@ -487,8 +504,8 @@ int do_load(M *m, const char *path, int quiet) {
         p.off_arg = (unsigned int)take(G * nb * sizeof(rk::TaggedDouble));
         p.off_done = (unsigned int)take(G * nb * 8);
         p.off_logits = (unsigned int)take(V * 4);
-        p.off_saa = take(sn * 8);
-        p.off_sbb = take(sn * 8);
+        p.off_saa = take(sn1 * 8);
+        p.off_sbb = take(sn1 * 8);
         m->xch_bytes = off;
         unsigned char *x = nullptr;
         if ((rc = dmalloc(m, &x, m->xch_bytes))) return rc;
@@ -510,6 +527,10 @@ int do_load(M *m, const char *path, int quiet) {
     if ((rc = dmalloc(m, &m->d_slogits, (size_t)V * m->max_gpt)) || (rc = dmalloc(m, &m->d_next, m->max_gpt)) ||
         (rc = dmalloc(m, &m->d_sample, 2 * m->max_gpt)) || (rc = dmalloc(m, &m->d_u, m->max_gpt)))
         return rc;
+    if ((rc = dmalloc(m, &m->gen.gs, m->max_gpt)) || (rc = dmalloc(m, &m->gen.row_stream, m->max_gpt)) ||
+        (rc = dmalloc(m, &m->gen.passes, (m->max_gpt + rk::kPfMaxTokens - 1) / rk::kPfMaxTokens)))
+        return rc;
+    CK(cudaMallocHost((void **)&m->gen.h_gs, sizeof(rk::GenStream) * m->max_gpt));
     CK(cudaHostAlloc((void **)&m->h_diag, sizeof(rk::Diag), cudaHostAllocMapped));
     memset(m->h_diag, 0, sizeof(rk::Diag));
     CK(cudaHostGetDevicePointer((void **)&p.diag, m->h_diag, 0));
@@ -544,6 +565,49 @@ int check_streams_model(M *m, const char *what) {
 }
 int check_slot(M *m, const char *what, unsigned long long slot) {
     if (slot >= m->max_gpt) return fail(1, "%s: slot %llu >= max_gpt %llu", what, slot, m->max_gpt);
+    return 0;
+}
+
+// A grow-only device buffer of at least `count` elements (called between calls, never with work in flight on it).
+template <class T> int grow(T **buf, size_t &cap, size_t count) {
+    if (count <= cap) return 0;
+    if (*buf) cudaFree(*buf);
+    *buf = nullptr;
+    cap = 0;
+    CK(cudaMalloc((void **)buf, count * sizeof(T)));
+    cap = count;
+    return 0;
+}
+
+// generate_streams enqueues this many steps between two looks at the streams' done flags: one synchronisation per
+// group, and at most this many - 1 steps spent on streams that have finished.
+constexpr unsigned long long kGenGroup = 16;
+
+// One step of generate_streams over `rows` rows on the decode kernel: each row on its stream's slot (or the scratch
+// slot once the stream is done), its logits into row r of d_slogits.
+int gen_step_decode(M *m, int rows) {
+    const size_t V = binfmt::kVocab;
+    for (int r = 0; r < rows; ++r) {
+        rk::k_gen_gate<<<1, 1, 0, m->stream>>>(m->gen.gs, m->gen.row_stream, r, m->max_gpt, m->p.ctrl);
+        CK(cudaGetLastError());
+        int rc = launch_token(m, 0, false, nullptr, m->stream);
+        if (rc) return rc;
+        CK(cudaMemcpyAsync(m->d_slogits + (size_t)r * V, dev_logits(m), V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
+        m->launches += 1;
+    }
+    return 0;
+}
+
+// One step of generate_streams on the tensor cores: ceil(rows / 128) passes whose descriptors the previous step's
+// feedback (or the group's upload) left in gen.passes; every row is a head row, so row r's logits land in d_slogits row r.
+int gen_step_passes(M *m, int rows) {
+    for (int p0 = 0, pi = 0; p0 < rows; p0 += rk::kPfMaxTokens, ++pi) {
+        const int T = std::min(rk::kPfMaxTokens, rows - p0);
+        CK(cudaMemcpyAsync(m->pf.pass, m->gen.passes + pi, sizeof(rk::PassDesc), cudaMemcpyDeviceToDevice, m->stream));
+        int rc = rk::prefill_run(m->pf, m->p, m->stream, T, T, m->d_slogits);
+        if (rc) return fail(rc, "%s", rk::prefill_error());
+    }
+    m->launches += rk::prefill_launches(m->pf);
     return 0;
 }
 
@@ -609,6 +673,9 @@ void rwkv_b200_free(rwkv_b200_model *m) {
     if (m->h_next) cudaFreeHost(m->h_next);
     if (m->h_sample) cudaFreeHost(m->h_sample);
     if (m->h_diag) cudaFreeHost(m->h_diag);
+    if (m->gen.h_gs) cudaFreeHost(m->gen.h_gs);
+    for (void *p : {(void *)m->gen.out, (void *)m->gen.stop, (void *)m->gen.ovr_tok, (void *)m->gen.ovr_val, (void *)m->gen.u})
+        if (p) cudaFree(p);
     if (m->stream) cudaStreamDestroy(m->stream);
     cudaGetLastError(); // a context killed by a trap makes every call above fail; do not leave that as "last error"
     delete m;
@@ -849,6 +916,118 @@ int rwkv_b200_sample_typical_streams(rwkv_b200_model *m, unsigned long long n_st
         if (margins_out) margins_out[i] = m->h_sample[2 * i + 1];
     }
     m->launches += 1;
+    return 0;
+}
+
+int rwkv_b200_generate_streams(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
+                               unsigned long long n_streams, unsigned long long max_new, const unsigned long long *budgets,
+                               const unsigned long long *stop_tokens, unsigned long long n_stop,
+                               const unsigned long long *override_tokens, const float *override_values,
+                               unsigned long long n_override, float temp, const double *u, unsigned long long *tokens_out,
+                               unsigned long long *lengths_out) {
+    int rc = check_streams_model(m, "generate_streams");
+    if (rc) return rc;
+    if (n_streams == 0) return fail(1, "generate_streams: no streams");
+    if (!slots || !first_tokens || !tokens_out || !lengths_out)
+        return fail(1, "generate_streams: null argument (slots, first_tokens, tokens_out and lengths_out are required)");
+    if (n_stop && !stop_tokens) return fail(1, "generate_streams: n_stop = %llu with NULL stop_tokens", n_stop);
+    if (n_override && (!override_tokens || !override_values))
+        return fail(1, "generate_streams: n_override = %llu with NULL override_tokens or override_values", n_override);
+    if (max_new == 0) return fail(1, "generate_streams: max_new is 0");
+    const size_t V = binfmt::kVocab;
+    std::vector<char> used(m->max_gpt, 0);
+    for (unsigned long long i = 0; i < n_streams; ++i) {
+        if ((rc = check_slot(m, "generate_streams", slots[i]))) return rc;
+        if (used[slots[i]]) return fail(1, "generate_streams: slot %llu appears twice", slots[i]);
+        used[slots[i]] = 1;
+        if (first_tokens[i] >= V) return fail(1, "generate_streams: first token %llu of stream %llu out of range", first_tokens[i], i);
+        if (budgets && (budgets[i] == 0 || budgets[i] > max_new))
+            return fail(1, "generate_streams: budget %llu of stream %llu is outside 1..max_new = %llu", budgets[i], i, max_new);
+    }
+    for (unsigned long long i = 0; i < n_stop; ++i)
+        if (stop_tokens[i] >= V) return fail(1, "generate_streams: stop token %llu out of range", stop_tokens[i]);
+    for (unsigned long long i = 0; i < n_override; ++i)
+        if (override_tokens[i] >= V) return fail(1, "generate_streams: override token %llu out of range", override_tokens[i]);
+    if (u)
+        for (unsigned long long i = 0; i < max_new * n_streams; ++i)
+            if (!(u[i] >= 0.0 && u[i] < 1.0)) return fail(1, "generate_streams: u[%llu] = %g is outside [0, 1)", i, u[i]);
+    CK(cudaSetDevice(m->device));
+    auto &g = m->gen;
+    if ((rc = grow(&g.out, g.out_cap, (size_t)(n_streams * max_new))) || (rc = grow(&g.stop, g.stop_cap, (size_t)n_stop)) ||
+        (rc = grow(&g.ovr_tok, g.ovr_cap, (size_t)n_override)) || (rc = grow(&g.ovr_val, g.ovr_val_cap, (size_t)n_override)) ||
+        (u && (rc = grow(&g.u, g.u_cap, (size_t)(kGenGroup * m->max_gpt)))))
+        return rc;
+    // the path is chosen once, by forward_streams' rule for n_streams tokens; a stream's numbers depend only on its row
+    const bool tc = n_streams >= (unsigned long long)m->pf.min_tokens && rk::prefill_enabled(m->pf);
+    if (tc && (rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
+    m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
+
+    rk::GenStream *hg = g.h_gs;
+    for (unsigned long long s = 0; s < n_streams; ++s) hg[s] = rk::GenStream{slots[s], budgets ? budgets[s] : max_new, first_tokens[s], 0, 0};
+    CK(cudaMemcpyAsync(g.gs, hg, n_streams * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemsetAsync(g.out, 0, n_streams * max_new * sizeof(unsigned long long), m->stream));
+    if (n_stop) CK(cudaMemcpyAsync(g.stop, stop_tokens, n_stop * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    if (n_override) {
+        CK(cudaMemcpyAsync(g.ovr_tok, override_tokens, n_override * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(g.ovr_val, override_values, n_override * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+    }
+    std::vector<int> live(n_streams);
+    for (unsigned long long s = 0; s < n_streams; ++s) live[s] = (int)s;
+    std::vector<rk::PassDesc> passes;
+    std::vector<double> ug;
+    const int exponent = sample_exponent(temp);
+    for (unsigned long long step = 0; !live.empty() && step < max_new;) {
+        // a group: the live streams are rows 0..rows-1; their inputs, and the uniforms of its steps, go up once
+        const int rows = (int)live.size();
+        const unsigned long long steps = std::min(kGenGroup, max_new - step);
+        CK(cudaMemcpyAsync(g.row_stream, live.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        if (tc) {
+            passes.assign((size_t)(rows + rk::kPfMaxTokens - 1) / rk::kPfMaxTokens, rk::PassDesc{});
+            for (int r = 0; r < rows; ++r) {
+                rk::PassDesc &pd = passes[r / rk::kPfMaxTokens];
+                const int t = r % rk::kPfMaxTokens;
+                pd.tokens[t] = hg[live[r]].tok;
+                pd.desc[t] = (uint32_t)hg[live[r]].slot | rk::kDescFirst | rk::kDescLast;
+                pd.rows[t] = t;
+                pd.out_row0 = (r / rk::kPfMaxTokens) * rk::kPfMaxTokens;
+            }
+            CK(cudaMemcpyAsync(g.passes, passes.data(), passes.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
+        }
+        if (u) {
+            ug.resize((size_t)steps * rows);
+            for (unsigned long long k = 0; k < steps; ++k)
+                for (int r = 0; r < rows; ++r) ug[k * rows + r] = u[(step + k) * n_streams + live[r]];
+            CK(cudaMemcpyAsync(g.u, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+        }
+        rk::GenFeedbackArgs fb{g.gs, g.row_stream, rows, u ? nullptr : m->d_next, m->d_sample, g.stop, (int)n_stop, g.out, max_new,
+                               tc ? g.passes : nullptr};
+        const unsigned rb = (unsigned)((rows + 127) / 128);
+        for (unsigned long long k = 0; k < steps; ++k) {
+            if ((rc = tc ? gen_step_passes(m, rows) : gen_step_decode(m, rows))) return rc;
+            if (n_override) {
+                rk::k_gen_override<<<rb, 128, 0, m->stream>>>(m->d_slogits, (int)V, rows, g.ovr_tok, g.ovr_val, (int)n_override);
+                CK(cudaGetLastError());
+                m->launches += 1;
+            }
+            if (u)
+                rk::k_sample_typical<<<(unsigned)rows, rk::kSampleThreads, 0, m->stream>>>(m->d_slogits, V, (int)V, exponent, g.u + k * rows,
+                                                                                          m->d_sample);
+            else
+                rk::k_argmax_rows<<<(unsigned)rows, rk::kArgmaxThreads, 0, m->stream>>>(m->d_slogits, (int)V, m->d_next);
+            CK(cudaGetLastError());
+            rk::k_gen_feedback<<<rb, 128, 0, m->stream>>>(fb);
+            CK(cudaGetLastError());
+            m->launches += 2;
+        }
+        // the end of a group: which streams are done (a few bytes, one synchronisation); drop them from the rows
+        CK(cudaMemcpyAsync(hg, g.gs, n_streams * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
+        SYNC(m);
+        step += steps;
+        live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hg[s].done != 0; }), live.end());
+    }
+    CK(cudaMemcpyAsync(tokens_out, g.out, n_streams * max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+    SYNC(m);
+    for (unsigned long long s = 0; s < n_streams; ++s) lengths_out[s] = hg[s].len;
     return 0;
 }
 

@@ -690,11 +690,16 @@ inline int prefill_chunk_body(PrefillState &s, const Params &p, cudaStream_t st,
     return 0;
 }
 
-// One pass: upload its layout, then replay (or record) the graph of its shape.
-inline int prefill_chunk(PrefillState &s, const Params &p, cudaStream_t st, const PassDesc &h_pass, int T, int H, float *logits) {
-    int rc;
+// The layout of the next pass from the host.
+inline int prefill_upload(PrefillState &s, cudaStream_t st, const PassDesc &h_pass) {
     // from pageable memory: the call returns once the source has been read, so the caller may reuse it
     PF_CK(cudaMemcpyAsync(s.pass, &h_pass, sizeof(PassDesc), cudaMemcpyHostToDevice, st));
+    return 0;
+}
+
+// One pass of the layout already in s.pass: replay (or record) the graph of its shape.
+inline int prefill_run(PrefillState &s, const Params &p, cudaStream_t st, int T, int H, float *logits) {
+    int rc;
     PrefillState::Graph *g = nullptr;
     for (auto &e : s.graphs)
         if (e.T == T && e.H == H) g = &e;
@@ -730,6 +735,12 @@ inline int prefill_chunk(PrefillState &s, const Params &p, cudaStream_t st, cons
         return rc;
     }
     return 0;
+}
+
+// One pass: upload its layout, then replay (or record) the graph of its shape.
+inline int prefill_chunk(PrefillState &s, const Params &p, cudaStream_t st, const PassDesc &h_pass, int T, int H, float *logits) {
+    const int rc = prefill_upload(s, st, h_pass);
+    return rc ? rc : prefill_run(s, p, st, T, H, logits);
 }
 
 // A ragged forward: `tokens` are stream-major, stream i owns lens[i] consecutive tokens and advances state slot

@@ -68,6 +68,8 @@ def load_library():
         "rwkv_b200_tp_import": (i32, [vp, vp]),
         "rwkv_b200_forward_streams": (i32, [vp, pull, ull, pull, pull, ull, pflt, pull]),
         "rwkv_b200_sample_typical_streams": (i32, [vp, ull, c.c_float, pdbl, pull, pdbl]),
+        "rwkv_b200_generate_streams": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull, c.c_float, pdbl,
+                                             pull, pull]),
         "rwkv_b200_slot_zero": (i32, [vp, ull]),
         "rwkv_b200_slot_copy": (i32, [vp, ull, ull]),
         "rwkv_b200_slot_upload": (i32, [vp, ull, pdbl, pdbl, pdbl, pdbl, pdbl]),
@@ -185,6 +187,33 @@ class Engine:
                                                            _ptr(toks, ctypes.c_ulonglong), _ptr(margins, ctypes.c_double)),
                  "sample_typical_streams")
         return toks, margins
+
+    def generate_streams(self, streams, max_new, budgets=None, stop=(), overrides=None, temp=1.0, u=None):
+        """Generate up to max_new tokens per stream on the device: streams = [(slot, first_token), ...].
+        Arg-max when u is None, else the typical sampler with u[step][stream]. budgets: tokens per stream (None =
+        max_new each); stop: token ids that end a stream (emitted, not fed); overrides = {token: logit value} applied
+        before every pick. Returns one numpy uint64 array of emitted tokens per stream."""
+        S = len(streams)
+        slots = np.ascontiguousarray([int(s) for s, _ in streams], dtype=np.uint64)
+        first = np.ascontiguousarray([int(t) for _, t in streams], dtype=np.uint64)
+        bud = np.ascontiguousarray(budgets, dtype=np.uint64) if budgets is not None else None
+        stops = np.ascontiguousarray(list(stop), dtype=np.uint64)
+        ovr = dict(overrides or {})
+        otok = np.ascontiguousarray(list(ovr.keys()), dtype=np.uint64)
+        oval = np.ascontiguousarray(list(ovr.values()), dtype=np.float32)
+        us = np.ascontiguousarray(u, dtype=np.float64) if u is not None else None
+        if bud is not None and bud.shape != (S,):
+            raise EngineError("generate_streams: %d budgets for %d streams" % (bud.size, S))
+        if us is not None and us.shape != (max_new, S):
+            raise EngineError("generate_streams: u has shape %s, expected (%d, %d)" % (us.shape, max_new, S))
+        out = np.zeros((S, max_new), np.uint64)
+        lens = np.zeros(S, np.uint64)
+        P = ctypes.c_ulonglong
+        self._ck(self.lib.rwkv_b200_generate_streams(self.h, _ptr(slots, P), _ptr(first, P), S, max_new, _ptr(bud, P),
+                                                     _ptr(stops, P), len(stops), _ptr(otok, P), _ptr(oval, ctypes.c_float),
+                                                     len(otok), temp, _ptr(us, ctypes.c_double), _ptr(out, P),
+                                                     _ptr(lens, P)), "generate_streams")
+        return [out[s, :int(lens[s])].copy() for s in range(S)]
 
     def slot_zero(self, slot):
         self._ck(self.lib.rwkv_b200_slot_zero(self.h, slot), "slot_zero")
