@@ -220,6 +220,53 @@ int rwkv_b200_generate_streams(rwkv_b200_model *m, const unsigned long long *slo
                                unsigned long long n_override, float temp, const double *u,
                                unsigned long long *tokens_out, unsigned long long *lengths_out);
 
+/* A stream's sampler for rwkv_b200_sample_streams and rwkv_b200_generate_streams_ex. Per row of logits l:
+ *  1. penalties (generate_streams_ex only): every token v the stream emitted earlier in the call has
+ *     l[v] -= presence_penalty + frequency_penalty * cnt[v], in f32 with each operation rounded (no FMA), where cnt[v]
+ *     is the decayed count: after each emitted token x, every count is multiplied by penalty_decay, then cnt[x] += 1.
+ *     The history starts empty in every call; prompt tokens are not counted;
+ *  2. the logit overrides, so an override value is final;
+ *  3. temperature 0: the arg-max, first index on ties (what forward_streams' next_out holds); u is not read;
+ *  4. temperature T > 0: p[v] = exp((l[v] - max l) / T) in double. Ranking tokens by l descending (ties: lower index
+ *     first), the kept set is the first min(n_p, top_k) of them, n_p the smallest count whose mass reaches
+ *     top_p * sum(p). The draw walks the kept tokens in vocabulary order and takes the first one with p > 0 whose
+ *     cumulative share of the kept mass reaches u. The cut and the draw run on the device without a sort; outputs
+ *     depend only on the row and the parameters (bit-deterministic). */
+typedef struct rwkv_b200_sampler {
+    float temperature;      /* 0 = arg-max (first index on ties); else > 0 */
+    float top_p;            /* (0, 1]; 1 = no cut */
+    unsigned int top_k;     /* 0 = no limit; <= 50277 */
+    float presence_penalty; /* generate_streams_ex only (|x| <= 1e6); 0 elsewhere */
+    float frequency_penalty;/* generate_streams_ex only (|x| <= 1e6); 0 elsewhere */
+    float penalty_decay;    /* (0, 1]; generate_streams_ex only (not read elsewhere) */
+} rwkv_b200_sampler;
+
+/* Draw one token per row with per-row samplers params[s] (penalties must be 0) and uniforms u[s] in [0, 1) (u may be
+ * NULL when every row has temperature 0). logits == NULL: the rows of the last forward_streams call, which must have
+ * produced logits or arg-maxes for exactly n_streams streams. Otherwise the caller's host rows
+ * ([n_streams][50277], n_streams <= max_gpt; no NaN or +inf, at least one finite value per row, -inf masks a token)
+ * are sampled, e.g. after constrained decoding edited them; they replace the per-stream logits of the last forward,
+ * so rwkv_b200_sample_typical_streams is refused until the next forward_streams. tokens_out[s] receives the token,
+ * margins_out[s] (may be NULL) the distance of u to the edges of the token's cumulative interval (1 for temperature
+ * 0): a caller with a host restatement of the rule can trust equal picks when the margin is >= 1e-9. */
+int rwkv_b200_sample_streams(rwkv_b200_model *m, unsigned long long n_streams, const rwkv_b200_sampler *params,
+                             const double *u, const float *logits, unsigned long long *tokens_out, double *margins_out);
+
+/* rwkv_b200_generate_streams with a sampler per stream (samplers[n_streams]; NULL = arg-max for every stream, u not
+ * read) in place of temp: greedy and sampled streams may share one call, and presence / frequency penalties apply to the
+ * tokens each stream emits in this call. u: [max_new][n_streams] as for generate_streams; it may be NULL only if every
+ * stream has temperature 0. Override values must be finite or -inf and may not set every token to -inf. Stops, budgets,
+ * continuation, the forward path, untouched slots and the refusals are those of generate_streams; each step is bit for
+ * bit forward_streams, the penalties in f32, the overrides, then rwkv_b200_sample_streams on those logits with the same
+ * u. The penalty history ([n_streams][50277] counts and flags) is allocated at the first call that uses penalties. */
+int rwkv_b200_generate_streams_ex(rwkv_b200_model *m, const unsigned long long *slots,
+                                  const unsigned long long *first_tokens, unsigned long long n_streams,
+                                  unsigned long long max_new, const unsigned long long *budgets,
+                                  const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                  const unsigned long long *override_tokens, const float *override_values,
+                                  unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
+                                  unsigned long long *tokens_out, unsigned long long *lengths_out);
+
 /* State of one slot: zero it (a new conversation), copy it onto another slot (fork a conversation), or move it
  * between the device and host arrays of n_layers x n_embed doubles each (NULL arrays are skipped). */
 int rwkv_b200_slot_zero(rwkv_b200_model *m, unsigned long long slot);

@@ -7,6 +7,6 @@ ABI) plus build helpers. The directory name contains a hyphen, so import it with
     import importlib
     pkg = importlib.import_module("rwkv-cpp-accelerated_b200")
 """
-from .engine import Engine, EngineError, lib_path, load_library  # noqa: F401
+from .engine import Engine, EngineError, Sampler, lib_path, load_library  # noqa: F401
 from . import build as build  # noqa: F401
 from . import tp as tp  # noqa: F401

@@ -13,6 +13,8 @@
 // no sm_90 device is present.
 #include <algorithm>
 #include <cerrno>
+#include <cfloat>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -32,6 +34,7 @@
 #include "binfmt.h"
 #include "generate.cuh"
 #include "prefill.cuh"
+#include "sampling.cuh"
 #include "token_kernel.cuh"
 
 namespace {
@@ -99,7 +102,10 @@ struct rwkv_b200_model {
         unsigned long long *stop = nullptr, *ovr_tok = nullptr;
         float *ovr_val = nullptr;
         double *u = nullptr; // [group steps][rows] uniforms of the current group
-        size_t out_cap = 0, stop_cap = 0, ovr_cap = 0, ovr_val_cap = 0, u_cap = 0;
+        rwkv_b200_sampler *samp = nullptr; // [n_streams] sampler of each stream (generate_streams_ex, sample_streams)
+        float *pen_cnt = nullptr;          // [n_streams][V] decayed counts of the emitted tokens (penalties only)
+        unsigned char *pen_seen = nullptr; // [n_streams][V] emitted in this call
+        size_t out_cap = 0, stop_cap = 0, ovr_cap = 0, ovr_val_cap = 0, u_cap = 0, samp_cap = 0, pen_cap = 0, seen_cap = 0;
     } gen;
 };
 
@@ -583,6 +589,9 @@ template <class T> int grow(T **buf, size_t &cap, size_t count) {
 // group, and at most this many - 1 steps spent on streams that have finished.
 constexpr unsigned long long kGenGroup = 16;
 
+// Largest |presence| or |frequency| penalty accepted: penalised logits stay far inside the f32 range.
+constexpr float kMaxPenalty = 1e6f;
+
 // One step of generate_streams over `rows` rows on the decode kernel: each row on its stream's slot (or the scratch
 // slot once the stream is done), its logits into row r of d_slogits.
 int gen_step_decode(M *m, int rows) {
@@ -608,6 +617,182 @@ int gen_step_passes(M *m, int rows) {
         if (rc) return fail(rc, "%s", rk::prefill_error());
     }
     m->launches += rk::prefill_launches(m->pf);
+    return 0;
+}
+
+// One stream's sampler. `history`: the call keeps the stream's emitted tokens (generate_streams_ex), so the penalties
+// may be set; elsewhere they must be 0 and penalty_decay is not read.
+int check_sampler(const char *what, unsigned long long s, const rwkv_b200_sampler &p, bool history) {
+    if (!(p.temperature >= 0.0f && p.temperature <= FLT_MAX))
+        return fail(1, "%s: stream %llu: temperature %g is not a finite value >= 0", what, s, p.temperature);
+    if (!(p.top_p > 0.0f && p.top_p <= 1.0f)) return fail(1, "%s: stream %llu: top_p %g is outside (0, 1]", what, s, p.top_p);
+    if (p.top_k > binfmt::kVocab) return fail(1, "%s: stream %llu: top_k %u > %llu", what, s, p.top_k, (unsigned long long)binfmt::kVocab);
+    if (!history) {
+        if (p.presence_penalty != 0.0f || p.frequency_penalty != 0.0f)
+            return fail(1, "%s: stream %llu: presence_penalty and frequency_penalty must be 0 here (no token history; see "
+                           "generate_streams_ex)", what, s);
+        return 0;
+    }
+    if (!(fabsf(p.presence_penalty) <= kMaxPenalty))
+        return fail(1, "%s: stream %llu: presence_penalty %g is not finite or exceeds %g in magnitude", what, s, p.presence_penalty, kMaxPenalty);
+    if (!(fabsf(p.frequency_penalty) <= kMaxPenalty))
+        return fail(1, "%s: stream %llu: frequency_penalty %g is not finite or exceeds %g in magnitude", what, s, p.frequency_penalty, kMaxPenalty);
+    if (!(p.penalty_decay > 0.0f && p.penalty_decay <= 1.0f))
+        return fail(1, "%s: stream %llu: penalty_decay %g is outside (0, 1]", what, s, p.penalty_decay);
+    return 0;
+}
+
+// Override values of generate_streams_ex: finite or -inf, and not every token -inf (a repeated token keeps its last value).
+int check_overrides(const char *what, const unsigned long long *tok, const float *val, unsigned long long n) {
+    std::vector<char> masked(binfmt::kVocab, 0);
+    for (unsigned long long i = 0; i < n; ++i) {
+        if (!(std::isfinite(val[i]) || val[i] == -INFINITY))
+            return fail(1, "%s: override value %g of token %llu is neither finite nor -inf", what, val[i], tok[i]);
+        masked[tok[i]] = val[i] == -INFINITY;
+    }
+    if (n >= binfmt::kVocab && std::count(masked.begin(), masked.end(), 1) == (long)binfmt::kVocab)
+        return fail(1, "%s: the overrides set every token to -inf", what);
+    return 0;
+}
+
+// The body of generate_streams (samplers == NULL, `temp` and `u` pick the typical sampler or the arg-max) and of
+// generate_streams_ex (`ex`: every stream has its own sampler, or all pick the arg-max when samplers == NULL).
+int generate(M *m, const char *what, bool ex, const unsigned long long *slots, const unsigned long long *first_tokens,
+             unsigned long long n_streams, unsigned long long max_new, const unsigned long long *budgets,
+             const unsigned long long *stop_tokens, unsigned long long n_stop, const unsigned long long *override_tokens,
+             const float *override_values, unsigned long long n_override, float temp, const rwkv_b200_sampler *samplers,
+             const double *u, unsigned long long *tokens_out, unsigned long long *lengths_out) {
+    int rc = check_streams_model(m, what);
+    if (rc) return rc;
+    if (n_streams == 0) return fail(1, "%s: no streams", what);
+    if (!slots || !first_tokens || !tokens_out || !lengths_out)
+        return fail(1, "%s: null argument (slots, first_tokens, tokens_out and lengths_out are required)", what);
+    if (n_stop && !stop_tokens) return fail(1, "%s: n_stop = %llu with NULL stop_tokens", what, n_stop);
+    if (n_override && (!override_tokens || !override_values))
+        return fail(1, "%s: n_override = %llu with NULL override_tokens or override_values", what, n_override);
+    if (max_new == 0) return fail(1, "%s: max_new is 0", what);
+    const size_t V = binfmt::kVocab;
+    std::vector<char> used(m->max_gpt, 0);
+    for (unsigned long long i = 0; i < n_streams; ++i) {
+        if ((rc = check_slot(m, what, slots[i]))) return rc;
+        if (used[slots[i]]) return fail(1, "%s: slot %llu appears twice", what, slots[i]);
+        used[slots[i]] = 1;
+        if (first_tokens[i] >= V) return fail(1, "%s: first token %llu of stream %llu out of range", what, first_tokens[i], i);
+        if (budgets && (budgets[i] == 0 || budgets[i] > max_new))
+            return fail(1, "%s: budget %llu of stream %llu is outside 1..max_new = %llu", what, budgets[i], i, max_new);
+    }
+    for (unsigned long long i = 0; i < n_stop; ++i)
+        if (stop_tokens[i] >= V) return fail(1, "%s: stop token %llu out of range", what, stop_tokens[i]);
+    for (unsigned long long i = 0; i < n_override; ++i)
+        if (override_tokens[i] >= V) return fail(1, "%s: override token %llu out of range", what, override_tokens[i]);
+    bool pen = false; // some stream has a presence or frequency penalty
+    if (ex) {
+        if ((rc = check_overrides(what, override_tokens, override_values, n_override))) return rc;
+        for (unsigned long long s = 0; samplers && s < n_streams; ++s) {
+            if ((rc = check_sampler(what, s, samplers[s], true))) return rc;
+            if (samplers[s].temperature > 0.0f && !u)
+                return fail(1, "%s: u is NULL but stream %llu samples (temperature %g)", what, s, samplers[s].temperature);
+            pen |= samplers[s].presence_penalty != 0.0f || samplers[s].frequency_penalty != 0.0f;
+        }
+    }
+    if (u)
+        for (unsigned long long i = 0; i < max_new * n_streams; ++i)
+            if (!(u[i] >= 0.0 && u[i] < 1.0)) return fail(1, "%s: u[%llu] = %g is outside [0, 1)", what, i, u[i]);
+    CK(cudaSetDevice(m->device));
+    auto &g = m->gen;
+    if (samplers && (rc = grow(&g.samp, g.samp_cap, (size_t)n_streams))) return rc;
+    if (pen && ((rc = grow(&g.pen_cnt, g.pen_cap, (size_t)(n_streams * V))) || (rc = grow(&g.pen_seen, g.seen_cap, (size_t)(n_streams * V)))))
+        return rc;
+    if ((rc = grow(&g.out, g.out_cap, (size_t)(n_streams * max_new))) || (rc = grow(&g.stop, g.stop_cap, (size_t)n_stop)) ||
+        (rc = grow(&g.ovr_tok, g.ovr_cap, (size_t)n_override)) || (rc = grow(&g.ovr_val, g.ovr_val_cap, (size_t)n_override)) ||
+        (u && (rc = grow(&g.u, g.u_cap, (size_t)(kGenGroup * m->max_gpt)))))
+        return rc;
+    // the path is chosen once, by forward_streams' rule for n_streams tokens; a stream's numbers depend only on its row
+    const bool tc = n_streams >= (unsigned long long)m->pf.min_tokens && rk::prefill_enabled(m->pf);
+    if (tc && (rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
+    m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
+
+    rk::GenStream *hg = g.h_gs;
+    for (unsigned long long s = 0; s < n_streams; ++s) hg[s] = rk::GenStream{slots[s], budgets ? budgets[s] : max_new, first_tokens[s], 0, 0};
+    CK(cudaMemcpyAsync(g.gs, hg, n_streams * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemsetAsync(g.out, 0, n_streams * max_new * sizeof(unsigned long long), m->stream));
+    if (n_stop) CK(cudaMemcpyAsync(g.stop, stop_tokens, n_stop * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    if (n_override) {
+        CK(cudaMemcpyAsync(g.ovr_tok, override_tokens, n_override * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(g.ovr_val, override_values, n_override * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+    }
+    if (samplers) CK(cudaMemcpyAsync(g.samp, samplers, n_streams * sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
+    if (pen) { // the history starts empty in every call: prompt tokens are not counted
+        CK(cudaMemsetAsync(g.pen_cnt, 0, n_streams * V * sizeof(float), m->stream));
+        CK(cudaMemsetAsync(g.pen_seen, 0, n_streams * V, m->stream));
+    }
+    std::vector<int> live(n_streams);
+    for (unsigned long long s = 0; s < n_streams; ++s) live[s] = (int)s;
+    std::vector<rk::PassDesc> passes;
+    std::vector<double> ug;
+    const int exponent = sample_exponent(temp);
+    for (unsigned long long step = 0; !live.empty() && step < max_new;) {
+        // a group: the live streams are rows 0..rows-1; their inputs, and the uniforms of its steps, go up once
+        const int rows = (int)live.size();
+        const unsigned long long steps = std::min(kGenGroup, max_new - step);
+        CK(cudaMemcpyAsync(g.row_stream, live.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        if (tc) {
+            passes.assign((size_t)(rows + rk::kPfMaxTokens - 1) / rk::kPfMaxTokens, rk::PassDesc{});
+            for (int r = 0; r < rows; ++r) {
+                rk::PassDesc &pd = passes[r / rk::kPfMaxTokens];
+                const int t = r % rk::kPfMaxTokens;
+                pd.tokens[t] = hg[live[r]].tok;
+                pd.desc[t] = (uint32_t)hg[live[r]].slot | rk::kDescFirst | rk::kDescLast;
+                pd.rows[t] = t;
+                pd.out_row0 = (r / rk::kPfMaxTokens) * rk::kPfMaxTokens;
+            }
+            CK(cudaMemcpyAsync(g.passes, passes.data(), passes.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
+        }
+        if (u) {
+            ug.resize((size_t)steps * rows);
+            for (unsigned long long k = 0; k < steps; ++k)
+                for (int r = 0; r < rows; ++r) ug[k * rows + r] = u[(step + k) * n_streams + live[r]];
+            CK(cudaMemcpyAsync(g.u, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+        }
+        rk::GenFeedbackArgs fb{g.gs, g.row_stream, rows, u || samplers ? nullptr : m->d_next, m->d_sample, g.stop, (int)n_stop, g.out, max_new,
+                               tc ? g.passes : nullptr};
+        const unsigned rb = (unsigned)((rows + 127) / 128);
+        for (unsigned long long k = 0; k < steps; ++k) {
+            if ((rc = tc ? gen_step_passes(m, rows) : gen_step_decode(m, rows))) return rc;
+            if (pen) {
+                const dim3 grid((unsigned)((V + rk::kPenaltyThreads - 1) / rk::kPenaltyThreads), (unsigned)rows);
+                rk::k_gen_penalty<<<grid, rk::kPenaltyThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs, g.row_stream, g.samp,
+                                                                              g.pen_cnt, g.pen_seen);
+                CK(cudaGetLastError());
+                m->launches += 1;
+            }
+            if (n_override) {
+                rk::k_gen_override<<<rb, 128, 0, m->stream>>>(m->d_slogits, (int)V, rows, g.ovr_tok, g.ovr_val, (int)n_override);
+                CK(cudaGetLastError());
+                m->launches += 1;
+            }
+            if (samplers)
+                rk::k_sample_nucleus<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.samp, g.row_stream,
+                                                                                       u ? g.u + k * rows : nullptr, m->d_sample);
+            else if (u)
+                rk::k_sample_typical<<<(unsigned)rows, rk::kSampleThreads, 0, m->stream>>>(m->d_slogits, V, (int)V, exponent, g.u + k * rows,
+                                                                                          m->d_sample);
+            else
+                rk::k_argmax_rows<<<(unsigned)rows, rk::kArgmaxThreads, 0, m->stream>>>(m->d_slogits, (int)V, m->d_next);
+            CK(cudaGetLastError());
+            rk::k_gen_feedback<<<rb, 128, 0, m->stream>>>(fb);
+            CK(cudaGetLastError());
+            m->launches += 2;
+        }
+        // the end of a group: which streams are done (a few bytes, one synchronisation); drop them from the rows
+        CK(cudaMemcpyAsync(hg, g.gs, n_streams * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
+        SYNC(m);
+        step += steps;
+        live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hg[s].done != 0; }), live.end());
+    }
+    CK(cudaMemcpyAsync(tokens_out, g.out, n_streams * max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+    SYNC(m);
+    for (unsigned long long s = 0; s < n_streams; ++s) lengths_out[s] = hg[s].len;
     return 0;
 }
 
@@ -674,7 +859,8 @@ void rwkv_b200_free(rwkv_b200_model *m) {
     if (m->h_sample) cudaFreeHost(m->h_sample);
     if (m->h_diag) cudaFreeHost(m->h_diag);
     if (m->gen.h_gs) cudaFreeHost(m->gen.h_gs);
-    for (void *p : {(void *)m->gen.out, (void *)m->gen.stop, (void *)m->gen.ovr_tok, (void *)m->gen.ovr_val, (void *)m->gen.u})
+    for (void *p : {(void *)m->gen.out, (void *)m->gen.stop, (void *)m->gen.ovr_tok, (void *)m->gen.ovr_val, (void *)m->gen.u,
+                    (void *)m->gen.samp, (void *)m->gen.pen_cnt, (void *)m->gen.pen_seen})
         if (p) cudaFree(p);
     if (m->stream) cudaStreamDestroy(m->stream);
     cudaGetLastError(); // a context killed by a trap makes every call above fail; do not leave that as "last error"
@@ -925,109 +1111,72 @@ int rwkv_b200_generate_streams(rwkv_b200_model *m, const unsigned long long *slo
                                const unsigned long long *override_tokens, const float *override_values,
                                unsigned long long n_override, float temp, const double *u, unsigned long long *tokens_out,
                                unsigned long long *lengths_out) {
-    int rc = check_streams_model(m, "generate_streams");
+    return generate(m, "generate_streams", false, slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop,
+                    override_tokens, override_values, n_override, temp, nullptr, u, tokens_out, lengths_out);
+}
+
+int rwkv_b200_generate_streams_ex(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
+                                  unsigned long long n_streams, unsigned long long max_new, const unsigned long long *budgets,
+                                  const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                  const unsigned long long *override_tokens, const float *override_values,
+                                  unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
+                                  unsigned long long *tokens_out, unsigned long long *lengths_out) {
+    // without samplers every stream takes the arg-max and u is not read
+    return generate(m, "generate_streams_ex", true, slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop,
+                    override_tokens, override_values, n_override, 1.0f, samplers, samplers ? u : nullptr, tokens_out, lengths_out);
+}
+
+int rwkv_b200_sample_streams(rwkv_b200_model *m, unsigned long long n_streams, const rwkv_b200_sampler *params, const double *u,
+                             const float *logits, unsigned long long *tokens_out, double *margins_out) {
+    const char *what = "sample_streams";
+    int rc = check_streams_model(m, what);
     if (rc) return rc;
-    if (n_streams == 0) return fail(1, "generate_streams: no streams");
-    if (!slots || !first_tokens || !tokens_out || !lengths_out)
-        return fail(1, "generate_streams: null argument (slots, first_tokens, tokens_out and lengths_out are required)");
-    if (n_stop && !stop_tokens) return fail(1, "generate_streams: n_stop = %llu with NULL stop_tokens", n_stop);
-    if (n_override && (!override_tokens || !override_values))
-        return fail(1, "generate_streams: n_override = %llu with NULL override_tokens or override_values", n_override);
-    if (max_new == 0) return fail(1, "generate_streams: max_new is 0");
+    if (!params || !tokens_out) return fail(1, "%s: null argument (params and tokens_out are required)", what);
+    if (n_streams == 0) return fail(1, "%s: no streams", what);
     const size_t V = binfmt::kVocab;
-    std::vector<char> used(m->max_gpt, 0);
-    for (unsigned long long i = 0; i < n_streams; ++i) {
-        if ((rc = check_slot(m, "generate_streams", slots[i]))) return rc;
-        if (used[slots[i]]) return fail(1, "generate_streams: slot %llu appears twice", slots[i]);
-        used[slots[i]] = 1;
-        if (first_tokens[i] >= V) return fail(1, "generate_streams: first token %llu of stream %llu out of range", first_tokens[i], i);
-        if (budgets && (budgets[i] == 0 || budgets[i] > max_new))
-            return fail(1, "generate_streams: budget %llu of stream %llu is outside 1..max_new = %llu", budgets[i], i, max_new);
+    if (logits) {
+        if (n_streams > m->max_gpt) return fail(1, "%s: %llu rows of logits > max_gpt %llu", what, n_streams, m->max_gpt);
+    } else {
+        if (m->stream_rows == 0)
+            return fail(1, "%s: the last forward produced no per-stream logits (call forward_streams with logits or next, or pass logits)", what);
+        if (n_streams != m->stream_rows)
+            return fail(1, "%s: %llu rows asked, the last forward_streams produced %llu", what, n_streams, m->stream_rows);
     }
-    for (unsigned long long i = 0; i < n_stop; ++i)
-        if (stop_tokens[i] >= V) return fail(1, "generate_streams: stop token %llu out of range", stop_tokens[i]);
-    for (unsigned long long i = 0; i < n_override; ++i)
-        if (override_tokens[i] >= V) return fail(1, "generate_streams: override token %llu out of range", override_tokens[i]);
-    if (u)
-        for (unsigned long long i = 0; i < max_new * n_streams; ++i)
-            if (!(u[i] >= 0.0 && u[i] < 1.0)) return fail(1, "generate_streams: u[%llu] = %g is outside [0, 1)", i, u[i]);
+    for (unsigned long long s = 0; s < n_streams; ++s) {
+        if ((rc = check_sampler(what, s, params[s], false))) return rc;
+        if (params[s].temperature > 0.0f && !u)
+            return fail(1, "%s: u is NULL but stream %llu samples (temperature %g)", what, s, params[s].temperature);
+        if (u && !(u[s] >= 0.0 && u[s] < 1.0)) return fail(1, "%s: u[%llu] = %g is outside [0, 1)", what, s, u[s]);
+    }
+    for (unsigned long long s = 0; logits && s < n_streams; ++s) {
+        const float *row = logits + s * V;
+        bool finite = false;
+        for (size_t v = 0; v < V; ++v) {
+            if (std::isnan(row[v]) || row[v] == INFINITY)
+                return fail(1, "%s: logits[%llu][%zu] = %g (NaN and +inf are not allowed)", what, s, v, row[v]);
+            finite |= std::isfinite(row[v]);
+        }
+        if (!finite) return fail(1, "%s: row %llu of the logits has no finite value", what, s);
+    }
     CK(cudaSetDevice(m->device));
     auto &g = m->gen;
-    if ((rc = grow(&g.out, g.out_cap, (size_t)(n_streams * max_new))) || (rc = grow(&g.stop, g.stop_cap, (size_t)n_stop)) ||
-        (rc = grow(&g.ovr_tok, g.ovr_cap, (size_t)n_override)) || (rc = grow(&g.ovr_val, g.ovr_val_cap, (size_t)n_override)) ||
-        (u && (rc = grow(&g.u, g.u_cap, (size_t)(kGenGroup * m->max_gpt)))))
-        return rc;
-    // the path is chosen once, by forward_streams' rule for n_streams tokens; a stream's numbers depend only on its row
-    const bool tc = n_streams >= (unsigned long long)m->pf.min_tokens && rk::prefill_enabled(m->pf);
-    if (tc && (rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
-    m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
-
-    rk::GenStream *hg = g.h_gs;
-    for (unsigned long long s = 0; s < n_streams; ++s) hg[s] = rk::GenStream{slots[s], budgets ? budgets[s] : max_new, first_tokens[s], 0, 0};
-    CK(cudaMemcpyAsync(g.gs, hg, n_streams * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
-    CK(cudaMemsetAsync(g.out, 0, n_streams * max_new * sizeof(unsigned long long), m->stream));
-    if (n_stop) CK(cudaMemcpyAsync(g.stop, stop_tokens, n_stop * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-    if (n_override) {
-        CK(cudaMemcpyAsync(g.ovr_tok, override_tokens, n_override * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(g.ovr_val, override_values, n_override * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+    if ((rc = grow(&g.samp, g.samp_cap, (size_t)n_streams))) return rc;
+    CK(cudaMemcpyAsync(g.samp, params, n_streams * sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
+    if (u) CK(cudaMemcpyAsync(m->d_u, u, n_streams * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+    if (logits) {
+        m->stream_rows = 0; // the compact rows now hold the caller's logits, not those of the last forward_streams
+        CK(cudaMemcpyAsync(m->d_slogits, logits, n_streams * V * sizeof(float), cudaMemcpyHostToDevice, m->stream));
     }
-    std::vector<int> live(n_streams);
-    for (unsigned long long s = 0; s < n_streams; ++s) live[s] = (int)s;
-    std::vector<rk::PassDesc> passes;
-    std::vector<double> ug;
-    const int exponent = sample_exponent(temp);
-    for (unsigned long long step = 0; !live.empty() && step < max_new;) {
-        // a group: the live streams are rows 0..rows-1; their inputs, and the uniforms of its steps, go up once
-        const int rows = (int)live.size();
-        const unsigned long long steps = std::min(kGenGroup, max_new - step);
-        CK(cudaMemcpyAsync(g.row_stream, live.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-        if (tc) {
-            passes.assign((size_t)(rows + rk::kPfMaxTokens - 1) / rk::kPfMaxTokens, rk::PassDesc{});
-            for (int r = 0; r < rows; ++r) {
-                rk::PassDesc &pd = passes[r / rk::kPfMaxTokens];
-                const int t = r % rk::kPfMaxTokens;
-                pd.tokens[t] = hg[live[r]].tok;
-                pd.desc[t] = (uint32_t)hg[live[r]].slot | rk::kDescFirst | rk::kDescLast;
-                pd.rows[t] = t;
-                pd.out_row0 = (r / rk::kPfMaxTokens) * rk::kPfMaxTokens;
-            }
-            CK(cudaMemcpyAsync(g.passes, passes.data(), passes.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
-        }
-        if (u) {
-            ug.resize((size_t)steps * rows);
-            for (unsigned long long k = 0; k < steps; ++k)
-                for (int r = 0; r < rows; ++r) ug[k * rows + r] = u[(step + k) * n_streams + live[r]];
-            CK(cudaMemcpyAsync(g.u, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
-        }
-        rk::GenFeedbackArgs fb{g.gs, g.row_stream, rows, u ? nullptr : m->d_next, m->d_sample, g.stop, (int)n_stop, g.out, max_new,
-                               tc ? g.passes : nullptr};
-        const unsigned rb = (unsigned)((rows + 127) / 128);
-        for (unsigned long long k = 0; k < steps; ++k) {
-            if ((rc = tc ? gen_step_passes(m, rows) : gen_step_decode(m, rows))) return rc;
-            if (n_override) {
-                rk::k_gen_override<<<rb, 128, 0, m->stream>>>(m->d_slogits, (int)V, rows, g.ovr_tok, g.ovr_val, (int)n_override);
-                CK(cudaGetLastError());
-                m->launches += 1;
-            }
-            if (u)
-                rk::k_sample_typical<<<(unsigned)rows, rk::kSampleThreads, 0, m->stream>>>(m->d_slogits, V, (int)V, exponent, g.u + k * rows,
-                                                                                          m->d_sample);
-            else
-                rk::k_argmax_rows<<<(unsigned)rows, rk::kArgmaxThreads, 0, m->stream>>>(m->d_slogits, (int)V, m->d_next);
-            CK(cudaGetLastError());
-            rk::k_gen_feedback<<<rb, 128, 0, m->stream>>>(fb);
-            CK(cudaGetLastError());
-            m->launches += 2;
-        }
-        // the end of a group: which streams are done (a few bytes, one synchronisation); drop them from the rows
-        CK(cudaMemcpyAsync(hg, g.gs, n_streams * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
-        SYNC(m);
-        step += steps;
-        live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hg[s].done != 0; }), live.end());
-    }
-    CK(cudaMemcpyAsync(tokens_out, g.out, n_streams * max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+    rk::k_sample_nucleus<<<(unsigned)n_streams, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.samp, nullptr,
+                                                                                u ? m->d_u : nullptr, m->d_sample);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(m->h_sample, m->d_sample, 2 * n_streams * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
     SYNC(m);
-    for (unsigned long long s = 0; s < n_streams; ++s) lengths_out[s] = hg[s].len;
+    for (unsigned long long i = 0; i < n_streams; ++i) {
+        tokens_out[i] = (unsigned long long)m->h_sample[2 * i];
+        if (margins_out) margins_out[i] = m->h_sample[2 * i + 1];
+    }
+    m->launches += 1;
     return 0;
 }
 

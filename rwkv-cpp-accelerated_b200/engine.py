@@ -19,6 +19,30 @@ class EngineError(RuntimeError):
     pass
 
 
+class Sampler(ctypes.Structure):
+    """rwkv_b200_sampler: temperature (0 = arg-max), top_p in (0, 1], top_k (0 = no limit), and the presence /
+    frequency penalties with their decay, which only generate_streams(sampling=...) applies."""
+    _fields_ = [("temperature", ctypes.c_float), ("top_p", ctypes.c_float), ("top_k", ctypes.c_uint),
+                ("presence_penalty", ctypes.c_float), ("frequency_penalty", ctypes.c_float),
+                ("penalty_decay", ctypes.c_float)]
+
+    def __init__(self, temperature=1.0, top_p=1.0, top_k=0, presence_penalty=0.0, frequency_penalty=0.0,
+                 penalty_decay=1.0):
+        super().__init__(temperature, top_p, top_k, presence_penalty, frequency_penalty, penalty_decay)
+
+
+def _samplers(spec, n):
+    """One Sampler (or dict of its fields) for all n streams, or a sequence of n of them, as a ctypes array."""
+    one = lambda x: x if isinstance(x, Sampler) else Sampler(**x)
+    if isinstance(spec, (Sampler, dict)):
+        items = [one(spec)] * n
+    else:
+        items = [one(x) for x in spec]
+        if len(items) != n:
+            raise EngineError("%d samplers for %d streams" % (len(items), n))
+    return (Sampler * n)(*items)
+
+
 def lib_path():
     # RWKV_B200_LIB: A/B-test another build of the same ABI (tools/sweep.py); default is the in-tree library
     return os.environ.get("RWKV_B200_LIB") or os.path.join(_PKG, "librwkv_b200.so")
@@ -70,6 +94,9 @@ def load_library():
         "rwkv_b200_sample_typical_streams": (i32, [vp, ull, c.c_float, pdbl, pull, pdbl]),
         "rwkv_b200_generate_streams": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull, c.c_float, pdbl,
                                              pull, pull]),
+        "rwkv_b200_sample_streams": (i32, [vp, ull, c.POINTER(Sampler), pdbl, pflt, pull, pdbl]),
+        "rwkv_b200_generate_streams_ex": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull, c.POINTER(Sampler),
+                                                pdbl, pull, pull]),
         "rwkv_b200_slot_zero": (i32, [vp, ull]),
         "rwkv_b200_slot_copy": (i32, [vp, ull, ull]),
         "rwkv_b200_slot_upload": (i32, [vp, ull, pdbl, pdbl, pdbl, pdbl, pdbl]),
@@ -188,11 +215,39 @@ class Engine:
                  "sample_typical_streams")
         return toks, margins
 
-    def generate_streams(self, streams, max_new, budgets=None, stop=(), overrides=None, temp=1.0, u=None):
+    def sample_streams(self, params, us, logits=None):
+        """Per-row sampler (include/rwkv_b200.h, rwkv_b200_sampler) on the rows of the last forward_streams call, or on
+        the host rows `logits` [S][V] when given: (tokens [S], margins [S]). params: one Sampler (or dict) for every
+        row, or one per row; us: S uniforms in [0, 1), or None when every row has temperature 0."""
+        u = np.ascontiguousarray(us, dtype=np.float64) if us is not None else None
+        lg = np.ascontiguousarray(logits, dtype=np.float32) if logits is not None else None
+        if lg is not None:
+            if lg.ndim != 2 or lg.shape[1] != VOCAB:
+                raise EngineError("sample_streams: logits have shape %s, expected (S, %d)" % (lg.shape, VOCAB))
+            n = lg.shape[0]
+        elif u is not None:
+            n = len(u)
+        elif not isinstance(params, (Sampler, dict)):
+            n = len(params)
+        else:
+            raise EngineError("sample_streams: the row count is unknown (give us, logits or one sampler per row)")
+        if u is not None and u.shape != (n,):
+            raise EngineError("sample_streams: %d uniforms for %d rows" % (u.size, n))
+        sp = _samplers(params, n)
+        toks = np.empty(n, np.uint64)
+        margins = np.empty(n, np.float64)
+        self._ck(self.lib.rwkv_b200_sample_streams(self.h, n, sp, _ptr(u, ctypes.c_double), _ptr(lg, ctypes.c_float),
+                                                   _ptr(toks, ctypes.c_ulonglong), _ptr(margins, ctypes.c_double)),
+                 "sample_streams")
+        return toks, margins
+
+    def generate_streams(self, streams, max_new, budgets=None, stop=(), overrides=None, temp=1.0, u=None, sampling=None):
         """Generate up to max_new tokens per stream on the device: streams = [(slot, first_token), ...].
         Arg-max when u is None, else the typical sampler with u[step][stream]. budgets: tokens per stream (None =
         max_new each); stop: token ids that end a stream (emitted, not fed); overrides = {token: logit value} applied
-        before every pick. Returns one numpy uint64 array of emitted tokens per stream."""
+        before every pick. sampling: one Sampler (or dict) for every stream, or one per stream; then the call is
+        rwkv_b200_generate_streams_ex (penalties, temperature, top-p, top-k; u as above, None only if every
+        temperature is 0) and temp is not used. Returns one numpy uint64 array of emitted tokens per stream."""
         S = len(streams)
         slots = np.ascontiguousarray([int(s) for s, _ in streams], dtype=np.uint64)
         first = np.ascontiguousarray([int(t) for _, t in streams], dtype=np.uint64)
@@ -209,6 +264,13 @@ class Engine:
         out = np.zeros((S, max_new), np.uint64)
         lens = np.zeros(S, np.uint64)
         P = ctypes.c_ulonglong
+        if sampling is not None:
+            self._ck(self.lib.rwkv_b200_generate_streams_ex(self.h, _ptr(slots, P), _ptr(first, P), S, max_new, _ptr(bud, P),
+                                                            _ptr(stops, P), len(stops), _ptr(otok, P),
+                                                            _ptr(oval, ctypes.c_float), len(otok), _samplers(sampling, S),
+                                                            _ptr(us, ctypes.c_double), _ptr(out, P), _ptr(lens, P)),
+                     "generate_streams_ex")
+            return [out[s, :int(lens[s])].copy() for s in range(S)]
         self._ck(self.lib.rwkv_b200_generate_streams(self.h, _ptr(slots, P), _ptr(first, P), S, max_new, _ptr(bud, P),
                                                      _ptr(stops, P), len(stops), _ptr(otok, P), _ptr(oval, ctypes.c_float),
                                                      len(otok), temp, _ptr(us, ctypes.c_double), _ptr(out, P),
