@@ -267,6 +267,39 @@ int rwkv_b200_generate_streams_ex(rwkv_b200_model *m, const unsigned long long *
                                   unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
                                   unsigned long long *tokens_out, unsigned long long *lengths_out);
 
+/* Scoring: how likely a text is under the model (perplexity, log-likelihood and multiple-choice evaluation, reranking,
+ * prompt log-probabilities). A position without a target holds RWKV_B200_NO_TARGET; at most RWKV_B200_MAX_TOP_N top
+ * alternatives per position. */
+#define RWKV_B200_NO_TARGET 0xFFFFFFFFFFFFFFFFULL
+#define RWKV_B200_MAX_TOP_N 20
+
+/* A ragged forward that scores target tokens on the device. tokens, slots and lengths are those of
+ * rwkv_b200_forward_streams, with the same validation and the same forward path: each slot advances by its tokens to the
+ * same bits as forward_streams. targets[t] is the token expected after tokens[t], or RWKV_B200_NO_TARGET for a position
+ * that is not scored (e.g. the context before a continuation; the last target of one chunk of a long document is the
+ * first token of the next chunk). For a scored position, with l the f32 logits after tokens[t] and y = targets[t]:
+ *   logprobs_out[t] = ((double)l[y] - m) - log(S), m = max l, S = sum exp((double)l[v] - m) in double, in a fixed order;
+ *   ranks_out[t]    = the number of tokens ranked before y, ranking by l descending, ties by lower index, -0 with +0
+ *                     (0 exactly when y is the arg-max that forward_streams' next_out reports);
+ *   top_tokens_out[t][k], top_logprobs_out[t][k] (k < top_n <= RWKV_B200_MAX_TOP_N): the first top_n tokens of that
+ *                     ranking, in order, with their logprobs by the same formula (bit for bit the logprob reported when
+ *                     that token is the target).
+ * An unscored position receives NaN, and RWKV_B200_NO_TARGET in its rank and top tokens (NaN top logprobs).
+ * logprobs_out ([n_tokens]) and targets are required; ranks_out ([n_tokens]) may be NULL; top_tokens_out and
+ * top_logprobs_out ([n_tokens][top_n]) are required when top_n > 0 and not read otherwise. The results depend only on
+ * each row's logits, so they are deterministic, and a stream scores the same bits in any ragged call on the same path.
+ * Only the results cross PCIe: 16 bytes per scored position plus the top entries. A call without any target is a
+ * state-only forward; on the tensor cores a pass without a scored position runs no head. Refused before any work
+ * (every slot untouched): the refusals of forward_streams, a target >= 50277 other than RWKV_B200_NO_TARGET,
+ * top_n > RWKV_B200_MAX_TOP_N, missing arrays, and tensor parallelism. After the call no per-stream logits are held:
+ * rwkv_b200_sample_typical_streams and rwkv_b200_sample_streams (without logits) are refused until the next
+ * forward_streams. */
+int rwkv_b200_score_streams(rwkv_b200_model *m, const unsigned long long *tokens, unsigned long long n_tokens,
+                            const unsigned long long *slots, const unsigned long long *lengths,
+                            unsigned long long n_streams, const unsigned long long *targets, unsigned int top_n,
+                            double *logprobs_out, unsigned long long *ranks_out,
+                            unsigned long long *top_tokens_out, double *top_logprobs_out);
+
 /* State of one slot: zero it (a new conversation), copy it onto another slot (fork a conversation), or move it
  * between the device and host arrays of n_layers x n_embed doubles each (NULL arrays are skipped). */
 int rwkv_b200_slot_zero(rwkv_b200_model *m, unsigned long long slot);

@@ -35,6 +35,7 @@
 #include "generate.cuh"
 #include "prefill.cuh"
 #include "sampling.cuh"
+#include "score.cuh"
 #include "token_kernel.cuh"
 
 namespace {
@@ -107,6 +108,13 @@ struct rwkv_b200_model {
         unsigned char *pen_seen = nullptr; // [n_streams][V] emitted in this call
         size_t out_cap = 0, stop_cap = 0, ovr_cap = 0, ovr_val_cap = 0, u_cap = 0, samp_cap = 0, pen_cap = 0, seen_cap = 0;
     } gen;
+    // score_streams: per scored row its d_slogits row and target in, its results out; grown with the largest call
+    struct Score {
+        int *rows = nullptr;
+        unsigned long long *tgt = nullptr, *rank = nullptr, *top_tok = nullptr;
+        double *lp = nullptr, *top_lp = nullptr;
+        size_t rows_cap = 0, tgt_cap = 0, rank_cap = 0, top_tok_cap = 0, lp_cap = 0, top_lp_cap = 0;
+    } score;
 };
 
 namespace {
@@ -574,6 +582,29 @@ int check_slot(M *m, const char *what, unsigned long long slot) {
     return 0;
 }
 
+// The model and the ragged token list of forward_streams and score_streams.
+int check_ragged(M *m, const char *what, const unsigned long long *tokens, unsigned long long n_tokens,
+                 const unsigned long long *slots, const unsigned long long *lengths, unsigned long long n_streams) {
+    int rc = check_streams_model(m, what);
+    if (rc) return rc;
+    if (!tokens || !slots || !lengths || n_tokens == 0 || n_streams == 0) return fail(1, "%s: no tokens or no streams", what);
+    if (n_tokens > m->max_gpt) return fail(1, "%s: %llu tokens > max_gpt %llu", what, n_tokens, m->max_gpt);
+    if (n_streams > n_tokens) return fail(1, "%s: %llu streams for %llu tokens", what, n_streams, n_tokens);
+    for (unsigned long long t = 0; t < n_tokens; ++t)
+        if (tokens[t] >= binfmt::kVocab) return fail(1, "%s: token id %llu out of range", what, tokens[t]);
+    std::vector<char> used(m->max_gpt, 0);
+    unsigned long long total = 0;
+    for (unsigned long long i = 0; i < n_streams; ++i) {
+        if ((rc = check_slot(m, what, slots[i]))) return rc;
+        if (used[slots[i]]) return fail(1, "%s: slot %llu appears twice", what, slots[i]);
+        used[slots[i]] = 1;
+        if (lengths[i] == 0 || lengths[i] > n_tokens) return fail(1, "%s: stream %llu has length %llu", what, i, lengths[i]);
+        total += lengths[i];
+    }
+    if (total != n_tokens) return fail(1, "%s: the lengths add up to %llu, not n_tokens = %llu", what, total, n_tokens);
+    return 0;
+}
+
 // A grow-only device buffer of at least `count` elements (called between calls, never with work in flight on it).
 template <class T> int grow(T **buf, size_t &cap, size_t count) {
     if (count <= cap) return 0;
@@ -860,7 +891,9 @@ void rwkv_b200_free(rwkv_b200_model *m) {
     if (m->h_diag) cudaFreeHost(m->h_diag);
     if (m->gen.h_gs) cudaFreeHost(m->gen.h_gs);
     for (void *p : {(void *)m->gen.out, (void *)m->gen.stop, (void *)m->gen.ovr_tok, (void *)m->gen.ovr_val, (void *)m->gen.u,
-                    (void *)m->gen.samp, (void *)m->gen.pen_cnt, (void *)m->gen.pen_seen})
+                    (void *)m->gen.samp, (void *)m->gen.pen_cnt, (void *)m->gen.pen_seen, (void *)m->score.rows,
+                    (void *)m->score.tgt, (void *)m->score.rank, (void *)m->score.top_tok, (void *)m->score.lp,
+                    (void *)m->score.top_lp})
         if (p) cudaFree(p);
     if (m->stream) cudaStreamDestroy(m->stream);
     cudaGetLastError(); // a context killed by a trap makes every call above fail; do not leave that as "last error"
@@ -1026,24 +1059,9 @@ int rwkv_b200_sample_typical(rwkv_b200_model *m, float temp, double u, unsigned 
 int rwkv_b200_forward_streams(rwkv_b200_model *m, const unsigned long long *tokens, unsigned long long n_tokens,
                               const unsigned long long *slots, const unsigned long long *lengths,
                               unsigned long long n_streams, float *logits_out, unsigned long long *next_out) {
-    int rc = check_streams_model(m, "forward_streams");
+    int rc = check_ragged(m, "forward_streams", tokens, n_tokens, slots, lengths, n_streams);
     if (rc) return rc;
-    if (!tokens || !slots || !lengths || n_tokens == 0 || n_streams == 0) return fail(1, "forward_streams: no tokens or no streams");
-    if (n_tokens > m->max_gpt) return fail(1, "forward_streams: %llu tokens > max_gpt %llu", n_tokens, m->max_gpt);
-    if (n_streams > n_tokens) return fail(1, "forward_streams: %llu streams for %llu tokens", n_streams, n_tokens);
     const size_t V = binfmt::kVocab;
-    for (unsigned long long t = 0; t < n_tokens; ++t)
-        if (tokens[t] >= V) return fail(1, "forward_streams: token id %llu out of range", tokens[t]);
-    std::vector<char> used(m->max_gpt, 0);
-    unsigned long long total = 0;
-    for (unsigned long long i = 0; i < n_streams; ++i) {
-        if ((rc = check_slot(m, "forward_streams", slots[i]))) return rc;
-        if (used[slots[i]]) return fail(1, "forward_streams: slot %llu appears twice", slots[i]);
-        used[slots[i]] = 1;
-        if (lengths[i] == 0 || lengths[i] > n_tokens) return fail(1, "forward_streams: stream %llu has length %llu", i, lengths[i]);
-        total += lengths[i];
-    }
-    if (total != n_tokens) return fail(1, "forward_streams: the lengths add up to %llu, not n_tokens = %llu", total, n_tokens);
     CK(cudaSetDevice(m->device));
     const bool head = logits_out || next_out;
     m->stream_rows = 0;
@@ -1177,6 +1195,100 @@ int rwkv_b200_sample_streams(rwkv_b200_model *m, unsigned long long n_streams, c
         if (margins_out) margins_out[i] = m->h_sample[2 * i + 1];
     }
     m->launches += 1;
+    return 0;
+}
+
+int rwkv_b200_score_streams(rwkv_b200_model *m, const unsigned long long *tokens, unsigned long long n_tokens,
+                            const unsigned long long *slots, const unsigned long long *lengths, unsigned long long n_streams,
+                            const unsigned long long *targets, unsigned int top_n, double *logprobs_out,
+                            unsigned long long *ranks_out, unsigned long long *top_tokens_out, double *top_logprobs_out) {
+    const char *what = "score_streams";
+    int rc = check_ragged(m, what, tokens, n_tokens, slots, lengths, n_streams);
+    if (rc) return rc;
+    if (!targets) return fail(1, "%s: targets is NULL (RWKV_B200_NO_TARGET marks a position that is not scored)", what);
+    if (!logprobs_out) return fail(1, "%s: logprobs_out is NULL", what);
+    if (top_n > (unsigned)rk::kMaxTopN) return fail(1, "%s: top_n %u > %d", what, top_n, rk::kMaxTopN);
+    if (top_n && (!top_tokens_out || !top_logprobs_out))
+        return fail(1, "%s: top_n = %u needs top_tokens_out and top_logprobs_out", what, top_n);
+    const size_t V = binfmt::kVocab;
+    // the scored positions: row j of the results is position pos[j], whose logits are row pos[j] of d_slogits
+    std::vector<int> pos;
+    std::vector<unsigned long long> tgt;
+    std::vector<unsigned char> need(n_tokens, 0);
+    for (unsigned long long i = 0, t = 0; i < n_streams; ++i)
+        for (unsigned long long k = 0; k < lengths[i]; ++k, ++t) {
+            if (targets[t] == RWKV_B200_NO_TARGET) continue;
+            if (targets[t] >= V)
+                return fail(1, "%s: targets[%llu] = %llu (stream %llu, position %llu) is neither a token id < %zu nor RWKV_B200_NO_TARGET",
+                            what, t, targets[t], i, k, V);
+            pos.push_back((int)t);
+            tgt.push_back(targets[t]);
+            need[t] = 1;
+        }
+    const size_t n = pos.size();
+    CK(cudaSetDevice(m->device));
+    m->stream_rows = 0; // the compact rows hold this call's scored positions, not per-stream logits
+    auto &sc = m->score;
+    if (n && ((rc = grow(&sc.rows, sc.rows_cap, n)) || (rc = grow(&sc.tgt, sc.tgt_cap, n)) || (rc = grow(&sc.lp, sc.lp_cap, n)) ||
+              (rc = grow(&sc.rank, sc.rank_cap, n)) || (rc = grow(&sc.top_tok, sc.top_tok_cap, n * top_n)) ||
+              (rc = grow(&sc.top_lp, sc.top_lp_cap, n * top_n))))
+        return rc;
+    if (n_tokens >= (unsigned long long)m->pf.min_tokens && rk::prefill_enabled(m->pf)) {
+        // logits of every token of a pass that holds a scored position, row t of d_slogits for token t
+        rc = rk::prefill_forward(m->pf, m->p, m->stream, tokens, (int)n_tokens, slots, lengths, (int)n_streams, n ? 1 : 0,
+                                 m->d_slogits, need.data());
+        if (rc) return fail(rc, "%s", rk::prefill_error());
+        m->launches += rk::prefill_launches(m->pf);
+    } else {
+        // token by token through the decode kernel; a scored position's logits are copied into row t of d_slogits
+        unsigned long long t = 0;
+        for (unsigned long long i = 0; i < n_streams; ++i)
+            for (unsigned long long k = 0; k < lengths[i]; ++k, ++t) {
+                rk::Ctrl &c = m->h_ctrl[t];
+                c.token = tokens[t];
+                c.next = 0;
+                c.slot = slots[i];
+                c.pos = 0;
+                CK(cudaMemcpyAsync(m->p.ctrl, &c, sizeof(rk::Ctrl), cudaMemcpyHostToDevice, m->stream));
+                if ((rc = launch_token(m, 0, false, nullptr, m->stream))) return rc;
+                if (need[t]) CK(cudaMemcpyAsync(m->d_slogits + t * V, dev_logits(m), V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
+            }
+    }
+    std::vector<double> lp(n), top_lp(n * top_n);
+    std::vector<unsigned long long> rank(n), top_tok(n * top_n);
+    if (n) {
+        CK(cudaMemcpyAsync(sc.rows, pos.data(), n * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(sc.tgt, tgt.data(), n * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        const rk::ScoreArgs a{m->d_slogits, (int)V, sc.rows, sc.tgt, (int)top_n, sc.lp, sc.rank, sc.top_tok, sc.top_lp};
+        rk::k_logprob_rows<<<(unsigned)n, rk::kNucThreads, 0, m->stream>>>(a);
+        CK(cudaGetLastError());
+        m->launches += 1;
+        CK(cudaMemcpyAsync(lp.data(), sc.lp, n * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+        if (ranks_out) CK(cudaMemcpyAsync(rank.data(), sc.rank, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+        if (top_n) {
+            CK(cudaMemcpyAsync(top_tok.data(), sc.top_tok, n * top_n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+            CK(cudaMemcpyAsync(top_lp.data(), sc.top_lp, n * top_n * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+        }
+    }
+    SYNC(m);
+    const double nan = std::nan("");
+    for (unsigned long long t = 0; t < n_tokens; ++t) {
+        logprobs_out[t] = nan;
+        if (ranks_out) ranks_out[t] = RWKV_B200_NO_TARGET;
+        for (unsigned k = 0; k < top_n; ++k) {
+            top_tokens_out[t * top_n + k] = RWKV_B200_NO_TARGET;
+            top_logprobs_out[t * top_n + k] = nan;
+        }
+    }
+    for (size_t j = 0; j < n; ++j) {
+        const size_t t = (size_t)pos[j];
+        logprobs_out[t] = lp[j];
+        if (ranks_out) ranks_out[t] = rank[j];
+        for (unsigned k = 0; k < top_n; ++k) {
+            top_tokens_out[t * top_n + k] = top_tok[j * top_n + k];
+            top_logprobs_out[t * top_n + k] = top_lp[j * top_n + k];
+        }
+    }
     return 0;
 }
 

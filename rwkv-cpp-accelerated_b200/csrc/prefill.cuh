@@ -748,8 +748,11 @@ inline int prefill_chunk(PrefillState &s, const Params &p, cudaStream_t st, cons
 // and "first" in the next. head = 0: state only. head = 1: logits of every token, row t of `logits`.
 // head = 2: logits of each stream's final token, row i of `logits` for stream i (only the pass holding that token
 // runs the head for it). `logits` is a device buffer of at least n (head 1) / nstreams (head 2) rows.
+// `need` (head 1 only, may be NULL): a pass none of whose tokens has need[t] set runs no head, so its logits rows are
+// not written.
 inline int prefill_forward(PrefillState &s, const Params &p, cudaStream_t st, const unsigned long long *tokens, int n,
-                           const unsigned long long *slots, const unsigned long long *lens, int nstreams, int head, float *logits) {
+                           const unsigned long long *slots, const unsigned long long *lens, int nstreams, int head, float *logits,
+                           const unsigned char *need = nullptr) {
     int rc = prefill_init(s, p);
     if (rc) return rc;
     PassDesc h{};
@@ -758,8 +761,10 @@ inline int prefill_forward(PrefillState &s, const Params &p, cudaStream_t st, co
     for (int t0 = 0; t0 < n; t0 += s.Tmax) {
         const int T = std::min(s.Tmax, n - t0);
         int H = 0;
+        bool needed = need == nullptr;
         h.out_row0 = head == 1 ? t0 : ended;
         for (int t = 0; t < T; ++t) {
+            if (need && need[t0 + t]) needed = true;
             while (pos == (int)lens[stream]) {
                 ++stream;
                 pos = 0;
@@ -771,6 +776,7 @@ inline int prefill_forward(PrefillState &s, const Params &p, cudaStream_t st, co
             if (fin) ++ended;
             ++pos;
         }
+        if (!needed) H = 0;
         if ((rc = prefill_chunk(s, p, st, h, T, H, logits))) return rc;
     }
     return 0;

@@ -10,6 +10,8 @@ import numpy as np
 
 VOCAB = 50277
 MODE_PARRALEL, MODE_GPT = 0, 1
+NO_TARGET = 0xFFFFFFFFFFFFFFFF  # RWKV_B200_NO_TARGET: a position score_streams does not score
+MAX_TOP_N = 20                  # RWKV_B200_MAX_TOP_N
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
@@ -97,6 +99,7 @@ def load_library():
         "rwkv_b200_sample_streams": (i32, [vp, ull, c.POINTER(Sampler), pdbl, pflt, pull, pdbl]),
         "rwkv_b200_generate_streams_ex": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull, c.POINTER(Sampler),
                                                 pdbl, pull, pull]),
+        "rwkv_b200_score_streams": (i32, [vp, pull, ull, pull, pull, ull, pull, c.c_uint, pdbl, pull, pull, pdbl]),
         "rwkv_b200_slot_zero": (i32, [vp, ull]),
         "rwkv_b200_slot_copy": (i32, [vp, ull, ull]),
         "rwkv_b200_slot_upload": (i32, [vp, ull, pdbl, pdbl, pdbl, pdbl, pdbl]),
@@ -276,6 +279,44 @@ class Engine:
                                                      len(otok), temp, _ptr(us, ctypes.c_double), _ptr(out, P),
                                                      _ptr(lens, P)), "generate_streams")
         return [out[s, :int(lens[s])].copy() for s in range(S)]
+
+    def score_streams(self, streams, targets=None, top_n=0):
+        """Score target tokens in one ragged forward: streams = [(slot, tokens), ...], each advancing its own state slot
+        as forward_streams does. targets: None scores each stream's own next tokens (tokens[1:]; its last position is
+        not scored); otherwise one list per stream, as long as its tokens, of the token expected after each position or
+        None for a position that is not scored. Returns per stream a dict of "logprobs" (float64, NaN where not scored)
+        and "ranks" (uint64, tokens ranked before the target; NO_TARGET where not scored), and with top_n > 0
+        "top_tokens" [len][top_n] and "top_logprobs" [len][top_n], the first top_n tokens by logit (ties: lower index)."""
+        slots = np.ascontiguousarray([int(s) for s, _ in streams], dtype=np.uint64)
+        seqs = [np.atleast_1d(np.asarray(t, dtype=np.uint64)) for _, t in streams]
+        lens = np.ascontiguousarray([len(t) for t in seqs], dtype=np.uint64)
+        toks = np.ascontiguousarray(np.concatenate(seqs) if seqs else np.zeros(0, np.uint64))
+        if targets is None:
+            tg = [list(t[1:]) + [None] for t in seqs]
+        else:
+            tg = list(targets)
+            if len(tg) != len(seqs) or any(len(a) != len(b) for a, b in zip(tg, seqs)):
+                raise EngineError("score_streams: targets need one list per stream, as long as its tokens")
+        tgt = np.ascontiguousarray([NO_TARGET if x is None else int(x) for row in tg for x in row], dtype=np.uint64)
+        n = len(toks)
+        lp = np.empty(n, np.float64)
+        ranks = np.empty(n, np.uint64)
+        top_tok = np.empty((n, top_n), np.uint64) if top_n > 0 else None
+        top_lp = np.empty((n, top_n), np.float64) if top_n > 0 else None
+        P = ctypes.c_ulonglong
+        self._ck(self.lib.rwkv_b200_score_streams(self.h, _ptr(toks, P), n, _ptr(slots, P), _ptr(lens, P), len(seqs),
+                                                  _ptr(tgt, P), int(top_n), _ptr(lp, ctypes.c_double), _ptr(ranks, P),
+                                                  _ptr(top_tok, P), _ptr(top_lp, ctypes.c_double)), "score_streams")
+        out, t0 = [], 0
+        for t in seqs:
+            sl = slice(t0, t0 + len(t))
+            d = {"logprobs": lp[sl].copy(), "ranks": ranks[sl].copy()}
+            if top_n > 0:
+                d["top_tokens"] = top_tok[sl].copy()
+                d["top_logprobs"] = top_lp[sl].copy()
+            out.append(d)
+            t0 += len(t)
+        return out
 
     def slot_zero(self, slot):
         self._ck(self.lib.rwkv_b200_slot_zero(self.h, slot), "slot_zero")
