@@ -300,6 +300,43 @@ int rwkv_b200_score_streams(rwkv_b200_model *m, const unsigned long long *tokens
                             double *logprobs_out, unsigned long long *ranks_out,
                             unsigned long long *top_tokens_out, double *top_logprobs_out);
 
+/* Which row rwkv_b200_generate_streams_logprobs scores an emitted token on. */
+#define RWKV_B200_LOGPROBS_RAW       0 /* the model's logits, before penalties and overrides (tau = 1) */
+#define RWKV_B200_LOGPROBS_PROCESSED 1 /* the row the sampler read, divided by the stream's temperature */
+
+/* rwkv_b200_generate_streams_ex that also reports how likely each emitted token was (completion logprobs and
+ * top_logprobs, confidence displays, the sampling log-probabilities of RL rollouts), scored on the device after each
+ * pick; only the results cross PCIe, once, at the end of the call. Every argument up to lengths_out, the emitted tokens,
+ * the lengths, the slot states and every refusal are exactly those of rwkv_b200_generate_streams_ex: asking for
+ * log-probabilities changes no token and no state bit.
+ * Entry [s][k] (k < lengths_out[s]) describes the k-th token y stream s emitted, by the rule of
+ * rwkv_b200_score_streams on a row l with a divisor tau:
+ *   z[v] = ((double)l[v] - m) / tau, m = max l;  logprobs_out[s][k] = z[y] - log(sum_v exp(z[v]));
+ *   ranks_out[s][k] and top_tokens_out[s][k][0..top_n) rank by l descending, ties by lower index, -0 with +0; each top
+ *   entry carries its token's logprob by the same formula (bit for bit the logprob reported when it is emitted).
+ * logprob_mode RWKV_B200_LOGPROBS_RAW: l is the model's logits row of the step, before penalties and overrides, and
+ *   tau = 1: bit for bit what rwkv_b200_score_streams reports for that token after the same prefix on the same path.
+ * logprob_mode RWKV_B200_LOGPROBS_PROCESSED: l is the row the sampler read, after penalties and overrides, and tau is
+ *   the stream's temperature (1 for temperature 0 and when samplers == NULL): the distribution before the top-p /
+ *   top-k cut, so a token outside the kept set still has a finite logprob.
+ * Positions at or beyond lengths_out[s] receive NaN, and RWKV_B200_NO_TARGET in the rank and top tokens (NaN top
+ * logprobs). logprobs_out ([n_streams][max_new]) is required; ranks_out (same shape) may be NULL; top_tokens_out and
+ * top_logprobs_out ([n_streams][max_new][top_n]) are required when top_n > 0 and not read otherwise. Refused before any
+ * work (every slot untouched): a logprob_mode other than the two above, top_n > RWKV_B200_MAX_TOP_N, missing arrays, and
+ * every refusal of generate_streams_ex, tensor parallelism included. Each step runs one more kernel than
+ * generate_streams_ex, plus, in raw mode with penalties or overrides, a device-to-device copy of the step's rows. The
+ * typical sampler of rwkv_b200_generate_streams has no counterpart here. */
+int rwkv_b200_generate_streams_logprobs(rwkv_b200_model *m, const unsigned long long *slots,
+                                        const unsigned long long *first_tokens, unsigned long long n_streams,
+                                        unsigned long long max_new, const unsigned long long *budgets,
+                                        const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                        const unsigned long long *override_tokens, const float *override_values,
+                                        unsigned long long n_override, const rwkv_b200_sampler *samplers,
+                                        const double *u, unsigned long long *tokens_out,
+                                        unsigned long long *lengths_out, int logprob_mode, unsigned int top_n,
+                                        double *logprobs_out, unsigned long long *ranks_out,
+                                        unsigned long long *top_tokens_out, double *top_logprobs_out);
+
 /* State of one slot: zero it (a new conversation), copy it onto another slot (fork a conversation), or move it
  * between the device and host arrays of n_layers x n_embed doubles each (NULL arrays are skipped). */
 int rwkv_b200_slot_zero(rwkv_b200_model *m, unsigned long long slot);

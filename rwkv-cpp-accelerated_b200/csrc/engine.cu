@@ -107,6 +107,12 @@ struct rwkv_b200_model {
         float *pen_cnt = nullptr;          // [n_streams][V] decayed counts of the emitted tokens (penalties only)
         unsigned char *pen_seen = nullptr; // [n_streams][V] emitted in this call
         size_t out_cap = 0, stop_cap = 0, ovr_cap = 0, ovr_val_cap = 0, u_cap = 0, samp_cap = 0, pen_cap = 0, seen_cap = 0;
+        // generate_streams_logprobs: the results of each emitted token, and the model's rows of the step (raw mode with
+        // penalties or overrides, which edit d_slogits in place)
+        double *lp = nullptr, *top_lp = nullptr;                    // [n_streams][max_new], [..][top_n]
+        unsigned long long *rank = nullptr, *top_tok = nullptr;     // [n_streams][max_new], [..][top_n]
+        float *raw = nullptr;                                       // [rows][V]
+        size_t lp_cap = 0, top_lp_cap = 0, rank_cap = 0, top_tok_cap = 0, raw_cap = 0;
     } gen;
     // score_streams: per scored row its d_slogits row and target in, its results out; grown with the largest call
     struct Score {
@@ -686,15 +692,35 @@ int check_overrides(const char *what, const unsigned long long *tok, const float
     return 0;
 }
 
-// The body of generate_streams (samplers == NULL, `temp` and `u` pick the typical sampler or the arg-max) and of
-// generate_streams_ex (`ex`: every stream has its own sampler, or all pick the arg-max when samplers == NULL).
+// What generate_streams_logprobs asks for: the mode, top_n and the caller's result arrays.
+struct LogprobRequest {
+    int mode;
+    unsigned top_n;
+    double *logprobs_out;
+    unsigned long long *ranks_out, *top_tokens_out;
+    double *top_logprobs_out;
+};
+
+// The body of generate_streams (samplers == NULL, `temp` and `u` pick the typical sampler or the arg-max), of
+// generate_streams_ex (`ex`: every stream has its own sampler, or all pick the arg-max when samplers == NULL) and of
+// generate_streams_logprobs (generate_streams_ex with `lpq`: each emitted token is scored after its pick).
 int generate(M *m, const char *what, bool ex, const unsigned long long *slots, const unsigned long long *first_tokens,
              unsigned long long n_streams, unsigned long long max_new, const unsigned long long *budgets,
              const unsigned long long *stop_tokens, unsigned long long n_stop, const unsigned long long *override_tokens,
              const float *override_values, unsigned long long n_override, float temp, const rwkv_b200_sampler *samplers,
-             const double *u, unsigned long long *tokens_out, unsigned long long *lengths_out) {
+             const double *u, unsigned long long *tokens_out, unsigned long long *lengths_out,
+             const LogprobRequest *lpq = nullptr) {
     int rc = check_streams_model(m, what);
     if (rc) return rc;
+    if (lpq) {
+        if (lpq->mode != RWKV_B200_LOGPROBS_RAW && lpq->mode != RWKV_B200_LOGPROBS_PROCESSED)
+            return fail(1, "%s: logprob_mode %d is neither RWKV_B200_LOGPROBS_RAW (0) nor RWKV_B200_LOGPROBS_PROCESSED (1)", what,
+                        lpq->mode);
+        if (lpq->top_n > (unsigned)rk::kMaxTopN) return fail(1, "%s: top_n %u > %d", what, lpq->top_n, rk::kMaxTopN);
+        if (!lpq->logprobs_out) return fail(1, "%s: logprobs_out is NULL", what);
+        if (lpq->top_n && (!lpq->top_tokens_out || !lpq->top_logprobs_out))
+            return fail(1, "%s: top_n = %u needs top_tokens_out and top_logprobs_out", what, lpq->top_n);
+    }
     if (n_streams == 0) return fail(1, "%s: no streams", what);
     if (!slots || !first_tokens || !tokens_out || !lengths_out)
         return fail(1, "%s: null argument (slots, first_tokens, tokens_out and lengths_out are required)", what);
@@ -738,6 +764,13 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
         (rc = grow(&g.ovr_tok, g.ovr_cap, (size_t)n_override)) || (rc = grow(&g.ovr_val, g.ovr_val_cap, (size_t)n_override)) ||
         (u && (rc = grow(&g.u, g.u_cap, (size_t)(kGenGroup * m->max_gpt)))))
         return rc;
+    // raw mode reads the model's rows: d_slogits itself, or a copy taken before the penalties and overrides edit it
+    const bool raw_copy = lpq && lpq->mode == RWKV_B200_LOGPROBS_RAW && (pen || n_override);
+    const size_t n_lp = (size_t)(n_streams * max_new), n_top = lpq ? n_lp * lpq->top_n : 0;
+    if (lpq && ((rc = grow(&g.lp, g.lp_cap, n_lp)) || (rc = grow(&g.rank, g.rank_cap, n_lp)) ||
+                (rc = grow(&g.top_tok, g.top_tok_cap, n_top)) || (rc = grow(&g.top_lp, g.top_lp_cap, n_top)) ||
+                (raw_copy && (rc = grow(&g.raw, g.raw_cap, (size_t)n_streams * V)))))
+        return rc;
     // the path is chosen once, by forward_streams' rule for n_streams tokens; a stream's numbers depend only on its row
     const bool tc = n_streams >= (unsigned long long)m->pf.min_tokens && rk::prefill_enabled(m->pf);
     if (tc && (rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
@@ -756,6 +789,14 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
     if (pen) { // the history starts empty in every call: prompt tokens are not counted
         CK(cudaMemsetAsync(g.pen_cnt, 0, n_streams * V * sizeof(float), m->stream));
         CK(cudaMemsetAsync(g.pen_seen, 0, n_streams * V, m->stream));
+    }
+    if (lpq) { // all ones: NaN logprobs and RWKV_B200_NO_TARGET ranks and tokens wherever no token is emitted
+        CK(cudaMemsetAsync(g.lp, 0xFF, n_lp * sizeof(double), m->stream));
+        CK(cudaMemsetAsync(g.rank, 0xFF, n_lp * sizeof(unsigned long long), m->stream));
+        if (n_top) {
+            CK(cudaMemsetAsync(g.top_tok, 0xFF, n_top * sizeof(unsigned long long), m->stream));
+            CK(cudaMemsetAsync(g.top_lp, 0xFF, n_top * sizeof(double), m->stream));
+        }
     }
     std::vector<int> live(n_streams);
     for (unsigned long long s = 0; s < n_streams; ++s) live[s] = (int)s;
@@ -787,9 +828,16 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
         }
         rk::GenFeedbackArgs fb{g.gs, g.row_stream, rows, u || samplers ? nullptr : m->d_next, m->d_sample, g.stop, (int)n_stop, g.out, max_new,
                                tc ? g.passes : nullptr};
+        rk::GenLogprobArgs la{};
+        if (lpq)
+            la = rk::GenLogprobArgs{raw_copy ? g.raw : m->d_slogits, (int)V, g.gs, g.row_stream, fb.next, m->d_sample,
+                                    lpq->mode == RWKV_B200_LOGPROBS_PROCESSED ? samplers ? g.samp : nullptr : nullptr,
+                                    (int)lpq->top_n, max_new, g.lp, g.rank, g.top_tok, g.top_lp};
         const unsigned rb = (unsigned)((rows + 127) / 128);
         for (unsigned long long k = 0; k < steps; ++k) {
             if ((rc = tc ? gen_step_passes(m, rows) : gen_step_decode(m, rows))) return rc;
+            if (raw_copy)
+                CK(cudaMemcpyAsync(g.raw, m->d_slogits, (size_t)rows * V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
             if (pen) {
                 const dim3 grid((unsigned)((V + rk::kPenaltyThreads - 1) / rk::kPenaltyThreads), (unsigned)rows);
                 rk::k_gen_penalty<<<grid, rk::kPenaltyThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs, g.row_stream, g.samp,
@@ -811,6 +859,11 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
             else
                 rk::k_argmax_rows<<<(unsigned)rows, rk::kArgmaxThreads, 0, m->stream>>>(m->d_slogits, (int)V, m->d_next);
             CK(cudaGetLastError());
+            if (lpq) {
+                rk::k_gen_logprob<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(la);
+                CK(cudaGetLastError());
+                m->launches += 1;
+            }
             rk::k_gen_feedback<<<rb, 128, 0, m->stream>>>(fb);
             CK(cudaGetLastError());
             m->launches += 2;
@@ -822,6 +875,14 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
         live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hg[s].done != 0; }), live.end());
     }
     CK(cudaMemcpyAsync(tokens_out, g.out, n_streams * max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+    if (lpq) {
+        CK(cudaMemcpyAsync(lpq->logprobs_out, g.lp, n_lp * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+        if (lpq->ranks_out) CK(cudaMemcpyAsync(lpq->ranks_out, g.rank, n_lp * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+        if (n_top) {
+            CK(cudaMemcpyAsync(lpq->top_tokens_out, g.top_tok, n_top * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+            CK(cudaMemcpyAsync(lpq->top_logprobs_out, g.top_lp, n_top * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+        }
+    }
     SYNC(m);
     for (unsigned long long s = 0; s < n_streams; ++s) lengths_out[s] = hg[s].len;
     return 0;
@@ -893,7 +954,8 @@ void rwkv_b200_free(rwkv_b200_model *m) {
     for (void *p : {(void *)m->gen.out, (void *)m->gen.stop, (void *)m->gen.ovr_tok, (void *)m->gen.ovr_val, (void *)m->gen.u,
                     (void *)m->gen.samp, (void *)m->gen.pen_cnt, (void *)m->gen.pen_seen, (void *)m->score.rows,
                     (void *)m->score.tgt, (void *)m->score.rank, (void *)m->score.top_tok, (void *)m->score.lp,
-                    (void *)m->score.top_lp})
+                    (void *)m->score.top_lp, (void *)m->gen.lp, (void *)m->gen.top_lp, (void *)m->gen.rank,
+                    (void *)m->gen.top_tok, (void *)m->gen.raw})
         if (p) cudaFree(p);
     if (m->stream) cudaStreamDestroy(m->stream);
     cudaGetLastError(); // a context killed by a trap makes every call above fail; do not leave that as "last error"
@@ -1142,6 +1204,20 @@ int rwkv_b200_generate_streams_ex(rwkv_b200_model *m, const unsigned long long *
     // without samplers every stream takes the arg-max and u is not read
     return generate(m, "generate_streams_ex", true, slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop,
                     override_tokens, override_values, n_override, 1.0f, samplers, samplers ? u : nullptr, tokens_out, lengths_out);
+}
+
+int rwkv_b200_generate_streams_logprobs(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
+                                        unsigned long long n_streams, unsigned long long max_new, const unsigned long long *budgets,
+                                        const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                        const unsigned long long *override_tokens, const float *override_values,
+                                        unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
+                                        unsigned long long *tokens_out, unsigned long long *lengths_out, int logprob_mode,
+                                        unsigned int top_n, double *logprobs_out, unsigned long long *ranks_out,
+                                        unsigned long long *top_tokens_out, double *top_logprobs_out) {
+    const LogprobRequest lpq{logprob_mode, top_n, logprobs_out, ranks_out, top_tokens_out, top_logprobs_out};
+    return generate(m, "generate_streams_logprobs", true, slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop,
+                    override_tokens, override_values, n_override, 1.0f, samplers, samplers ? u : nullptr, tokens_out, lengths_out,
+                    &lpq);
 }
 
 int rwkv_b200_sample_streams(rwkv_b200_model *m, unsigned long long n_streams, const rwkv_b200_sampler *params, const double *u,

@@ -6,6 +6,7 @@
 // k_gen_override on the logits rows, the existing pick (k_argmax_rows or k_sample_typical), and k_gen_feedback, which
 // appends the picked token, decides whether the stream is done and writes the next step's input. A stream that
 // finishes inside a group keeps its row until the group ends but is frozen: its slot is not written again.
+// generate_streams_logprobs adds k_gen_logprob (score.cuh) between the pick and k_gen_feedback.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>

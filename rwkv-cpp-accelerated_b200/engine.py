@@ -12,6 +12,7 @@ VOCAB = 50277
 MODE_PARRALEL, MODE_GPT = 0, 1
 NO_TARGET = 0xFFFFFFFFFFFFFFFF  # RWKV_B200_NO_TARGET: a position score_streams does not score
 MAX_TOP_N = 20                  # RWKV_B200_MAX_TOP_N
+LOGPROBS_RAW, LOGPROBS_PROCESSED = 0, 1  # RWKV_B200_LOGPROBS_*: the row generate_streams(logprobs=...) scores on
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
@@ -43,6 +44,25 @@ def _samplers(spec, n):
         if len(items) != n:
             raise EngineError("%d samplers for %d streams" % (len(items), n))
     return (Sampler * n)(*items)
+
+
+def _gen_args(streams, max_new, budgets, stop, overrides, u):
+    """The arrays of a generate_streams call: S, slots, first tokens, budgets, stops, override tokens and values,
+    uniforms, and the emitted tokens and lengths to fill."""
+    S = len(streams)
+    slots = np.ascontiguousarray([int(s) for s, _ in streams], dtype=np.uint64)
+    first = np.ascontiguousarray([int(t) for _, t in streams], dtype=np.uint64)
+    bud = np.ascontiguousarray(budgets, dtype=np.uint64) if budgets is not None else None
+    stops = np.ascontiguousarray(list(stop), dtype=np.uint64)
+    ovr = dict(overrides or {})
+    otok = np.ascontiguousarray(list(ovr.keys()), dtype=np.uint64)
+    oval = np.ascontiguousarray(list(ovr.values()), dtype=np.float32)
+    us = np.ascontiguousarray(u, dtype=np.float64) if u is not None else None
+    if bud is not None and bud.shape != (S,):
+        raise EngineError("generate_streams: %d budgets for %d streams" % (bud.size, S))
+    if us is not None and us.shape != (max_new, S):
+        raise EngineError("generate_streams: u has shape %s, expected (%d, %d)" % (us.shape, max_new, S))
+    return S, slots, first, bud, stops, otok, oval, us, np.zeros((S, max_new), np.uint64), np.zeros(S, np.uint64)
 
 
 def lib_path():
@@ -100,6 +120,9 @@ def load_library():
         "rwkv_b200_generate_streams_ex": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull, c.POINTER(Sampler),
                                                 pdbl, pull, pull]),
         "rwkv_b200_score_streams": (i32, [vp, pull, ull, pull, pull, ull, pull, c.c_uint, pdbl, pull, pull, pdbl]),
+        "rwkv_b200_generate_streams_logprobs": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull,
+                                                      c.POINTER(Sampler), pdbl, pull, pull, i32, c.c_uint, pdbl, pull, pull,
+                                                      pdbl]),
         "rwkv_b200_slot_zero": (i32, [vp, ull]),
         "rwkv_b200_slot_copy": (i32, [vp, ull, ull]),
         "rwkv_b200_slot_upload": (i32, [vp, ull, pdbl, pdbl, pdbl, pdbl, pdbl]),
@@ -244,28 +267,23 @@ class Engine:
                  "sample_streams")
         return toks, margins
 
-    def generate_streams(self, streams, max_new, budgets=None, stop=(), overrides=None, temp=1.0, u=None, sampling=None):
+    def generate_streams(self, streams, max_new, budgets=None, stop=(), overrides=None, temp=None, u=None, sampling=None,
+                         logprobs=None, top_n=0):
         """Generate up to max_new tokens per stream on the device: streams = [(slot, first_token), ...].
-        Arg-max when u is None, else the typical sampler with u[step][stream]. budgets: tokens per stream (None =
-        max_new each); stop: token ids that end a stream (emitted, not fed); overrides = {token: logit value} applied
-        before every pick. sampling: one Sampler (or dict) for every stream, or one per stream; then the call is
-        rwkv_b200_generate_streams_ex (penalties, temperature, top-p, top-k; u as above, None only if every
-        temperature is 0) and temp is not used. Returns one numpy uint64 array of emitted tokens per stream."""
-        S = len(streams)
-        slots = np.ascontiguousarray([int(s) for s, _ in streams], dtype=np.uint64)
-        first = np.ascontiguousarray([int(t) for _, t in streams], dtype=np.uint64)
-        bud = np.ascontiguousarray(budgets, dtype=np.uint64) if budgets is not None else None
-        stops = np.ascontiguousarray(list(stop), dtype=np.uint64)
-        ovr = dict(overrides or {})
-        otok = np.ascontiguousarray(list(ovr.keys()), dtype=np.uint64)
-        oval = np.ascontiguousarray(list(ovr.values()), dtype=np.float32)
-        us = np.ascontiguousarray(u, dtype=np.float64) if u is not None else None
-        if bud is not None and bud.shape != (S,):
-            raise EngineError("generate_streams: %d budgets for %d streams" % (bud.size, S))
-        if us is not None and us.shape != (max_new, S):
-            raise EngineError("generate_streams: u has shape %s, expected (%d, %d)" % (us.shape, max_new, S))
-        out = np.zeros((S, max_new), np.uint64)
-        lens = np.zeros(S, np.uint64)
+        Arg-max when u is None, else the typical sampler with u[step][stream] and temp (default 1.0). budgets: tokens
+        per stream (None = max_new each); stop: token ids that end a stream (emitted, not fed); overrides = {token:
+        logit value} applied before every pick. sampling: one Sampler (or dict) for every stream, or one per stream;
+        then the call is rwkv_b200_generate_streams_ex (penalties, temperature, top-p, top-k; u as above, None only if
+        every temperature is 0) and temp is not used. Returns one numpy uint64 array of emitted tokens per stream.
+        logprobs = "raw" or "processed": the same generation (sampling=None is the arg-max; the typical sampler is not
+        available) also scores each emitted token on the device (rwkv_b200_generate_streams_logprobs): "raw" on the
+        model's logits, "processed" on the row the sampler read divided by the stream's temperature. Then it returns
+        one dict per stream: "tokens", "logprobs" (float64), "ranks" (uint64, tokens ranked before the emitted one),
+        and with top_n > 0 "top_tokens" [len][top_n] and "top_logprobs" [len][top_n], each as long as the stream."""
+        if logprobs is not None:
+            return self._generate_logprobs(streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n)
+        temp = 1.0 if temp is None else temp
+        S, slots, first, bud, stops, otok, oval, us, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u)
         P = ctypes.c_ulonglong
         if sampling is not None:
             self._ck(self.lib.rwkv_b200_generate_streams_ex(self.h, _ptr(slots, P), _ptr(first, P), S, max_new, _ptr(bud, P),
@@ -279,6 +297,35 @@ class Engine:
                                                      len(otok), temp, _ptr(us, ctypes.c_double), _ptr(out, P),
                                                      _ptr(lens, P)), "generate_streams")
         return [out[s, :int(lens[s])].copy() for s in range(S)]
+
+    def _generate_logprobs(self, streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n):
+        modes = {"raw": LOGPROBS_RAW, "processed": LOGPROBS_PROCESSED}
+        if logprobs not in modes:
+            raise EngineError("generate_streams: logprobs must be 'raw' or 'processed', not %r" % (logprobs,))
+        if sampling is None and (u is not None or temp is not None):
+            raise EngineError("generate_streams: logprobs need sampling=... (or neither u nor temp, for the arg-max); "
+                              "the typical sampler reports no log-probabilities")
+        S, slots, first, bud, stops, otok, oval, us, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u)
+        lp = np.empty((S, max_new), np.float64)
+        ranks = np.empty((S, max_new), np.uint64)
+        top_tok = np.empty((S, max_new, top_n), np.uint64) if top_n > 0 else None
+        top_lp = np.empty((S, max_new, top_n), np.float64) if top_n > 0 else None
+        P = ctypes.c_ulonglong
+        sp = _samplers(sampling, S) if sampling is not None else None
+        self._ck(self.lib.rwkv_b200_generate_streams_logprobs(
+            self.h, _ptr(slots, P), _ptr(first, P), S, max_new, _ptr(bud, P), _ptr(stops, P), len(stops), _ptr(otok, P),
+            _ptr(oval, ctypes.c_float), len(otok), sp, _ptr(us, ctypes.c_double), _ptr(out, P), _ptr(lens, P),
+            modes[logprobs], int(top_n), _ptr(lp, ctypes.c_double), _ptr(ranks, P), _ptr(top_tok, P),
+            _ptr(top_lp, ctypes.c_double)), "generate_streams_logprobs")
+        res = []
+        for s in range(S):
+            n = int(lens[s])
+            d = {"tokens": out[s, :n].copy(), "logprobs": lp[s, :n].copy(), "ranks": ranks[s, :n].copy()}
+            if top_n > 0:
+                d["top_tokens"] = top_tok[s, :n].copy()
+                d["top_logprobs"] = top_lp[s, :n].copy()
+            res.append(d)
+        return res
 
     def score_streams(self, streams, targets=None, top_n=0):
         """Score target tokens in one ragged forward: streams = [(slot, tokens), ...], each advancing its own state slot
