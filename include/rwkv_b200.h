@@ -337,6 +337,60 @@ int rwkv_b200_generate_streams_logprobs(rwkv_b200_model *m, const unsigned long 
                                         double *logprobs_out, unsigned long long *ranks_out,
                                         unsigned long long *top_tokens_out, double *top_logprobs_out);
 
+/* Constrained generation: output that must follow a format (JSON with fixed keys, a number, a date, one of a few labels)
+ * without returning to the host per step. A token automaton has n_states states; state q has the edges
+ * (edge_tokens[e], edge_next[e]) for e in [edge_start[q], edge_start[q + 1]), sorted by token, no token twice in a state.
+ * A state without edges is complete. A constrained stream carries its current state q, and each step is:
+ *  1. the row passes through the penalties, then the logit overrides, exactly as in rwkv_b200_generate_streams_ex;
+ *  2. mask: every token v without an edge out of q gets l[v] = -inf, after the overrides, so an override cannot re-enable
+ *     a token the automaton forbids (the bits are those of numpy's row[~allowed] = -np.inf);
+ *  3. the pick (arg-max or the sampler of rwkv_b200_sampler) runs on the masked row with the same u;
+ *  4. after emitting y, q = next(q, y);
+ *  5. if the new state has no edges the stream is done, like after a stop token: the emitted token is not fed.
+ * Stop tokens and budgets still apply; whichever condition comes first ends the stream. The device keeps the CSR arrays
+ * and one allow bitmask per state: ceil(50277 / 32) u32 words, 6288 bytes per state, plus 8 bytes per state and per
+ * edge. The host keeps the CSR too (the override check below). Tools that build automata from regular expressions over
+ * the tokenizer's bytes are in the Python package (constrain.py). */
+#define RWKV_B200_NO_CONSTRAINT 0xFFFFFFFFFFFFFFFFULL /* constraint_ids entry of a stream without a constraint */
+#define RWKV_B200_MAX_CONSTRAINT_STATES 65536
+
+/* Upload a token automaton in CSR form (edge_start [n_states + 1], edge_tokens and edge_next [edge_start[n_states]]);
+ * *id receives its id for rwkv_b200_generate_streams_constrained. Refused: n_states == 0 or >
+ * RWKV_B200_MAX_CONSTRAINT_STATES, edge_start not starting at 0 or decreasing, an edge token >= 50277, tokens not strictly
+ * ascending within a state, an edge_next >= n_states, and tensor parallelism. */
+int rwkv_b200_constraint_add(rwkv_b200_model *m, unsigned long long n_states, const unsigned long long *edge_start,
+                             const unsigned long long *edge_tokens, const unsigned long long *edge_next,
+                             unsigned long long *id);
+/* Free an automaton (an unknown or removed id is refused). rwkv_b200_free frees every automaton of the model. */
+int rwkv_b200_constraint_remove(rwkv_b200_model *m, unsigned long long id);
+
+/* rwkv_b200_generate_streams_logprobs with a token automaton per stream, by the rule above. constraint_ids[n_streams]:
+ * an id of rwkv_b200_constraint_add, or RWKV_B200_NO_CONSTRAINT; NULL = no stream has a constraint. start_states
+ * [n_streams]: each constrained stream's first state (NULL = state 0). states_out [n_streams] (may be NULL): each
+ * constrained stream's final state (0 for the others), so a caller can continue a constrained generation in the next call
+ * or check that it completed. logprobs_out == NULL: nothing is scored, and logprob_mode, top_n, ranks_out,
+ * top_tokens_out and top_logprobs_out are not read. Streams without a constraint generate bit for bit as in
+ * generate_streams_ex; with constraint_ids == NULL and logprobs_out == NULL the call is generate_streams_ex. Log-probabilities
+ * in processed mode are taken on the masked row: the rank counts the tokens that rank before y (masked tokens rank last),
+ * and a top entry past the allowed tokens is a masked token in index order with logprob -inf. Raw mode scores the model's
+ * row. Refused before any work (every slot untouched): every refusal of generate_streams_logprobs (with logprobs_out
+ * != NULL) or generate_streams_ex, an unknown or removed id, a start state out of range or without edges, and an automaton
+ * with a state with edges whose every edge token this call's overrides set to -inf. Each step of a call with a constraint
+ * runs one more kernel (k_gen_mask). A token emitted without an edge (a broken pick) fails the call at the end of its
+ * 16-step group with a message naming the stream, the token and the state. */
+int rwkv_b200_generate_streams_constrained(rwkv_b200_model *m, const unsigned long long *slots,
+                                           const unsigned long long *first_tokens, unsigned long long n_streams,
+                                           unsigned long long max_new, const unsigned long long *budgets,
+                                           const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                           const unsigned long long *override_tokens, const float *override_values,
+                                           unsigned long long n_override, const rwkv_b200_sampler *samplers,
+                                           const double *u, unsigned long long *tokens_out,
+                                           unsigned long long *lengths_out, int logprob_mode, unsigned int top_n,
+                                           double *logprobs_out, unsigned long long *ranks_out,
+                                           unsigned long long *top_tokens_out, double *top_logprobs_out,
+                                           const unsigned long long *constraint_ids,
+                                           const unsigned long long *start_states, unsigned long long *states_out);
+
 /* State of one slot: zero it (a new conversation), copy it onto another slot (fork a conversation), or move it
  * between the device and host arrays of n_layers x n_embed doubles each (NULL arrays are skipped). */
 int rwkv_b200_slot_zero(rwkv_b200_model *m, unsigned long long slot);

@@ -9,4 +9,5 @@ ABI) plus build helpers. The directory name contains a hyphen, so import it with
 """
 from .engine import Engine, EngineError, Sampler, lib_path, load_library  # noqa: F401
 from . import build as build  # noqa: F401
+from . import constrain as constrain  # noqa: F401
 from . import tp as tp  # noqa: F401

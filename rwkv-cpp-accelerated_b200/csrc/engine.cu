@@ -19,6 +19,8 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
+#include <new>
 #include <string>
 #include <vector>
 
@@ -113,7 +115,21 @@ struct rwkv_b200_model {
         unsigned long long *rank = nullptr, *top_tok = nullptr;     // [n_streams][max_new], [..][top_n]
         float *raw = nullptr;                                       // [rows][V]
         size_t lp_cap = 0, top_lp_cap = 0, rank_cap = 0, top_tok_cap = 0, raw_cap = 0;
+        // generate_streams_constrained: each stream's automaton and state, and the record of a token without an edge
+        rk::GenConstraint *gc = nullptr;  // [n_streams]
+        unsigned long long *fault = nullptr; // [3]
+        size_t gc_cap = 0, fault_cap = 0;
     } gen;
+    // rwkv_b200_constraint_add: per id, the CSR on the host (the override check of a call) and one device block holding
+    // the allow masks, then edge_start, the edge tokens and their targets
+    struct Automaton {
+        std::vector<unsigned long long> start; // [n_states + 1]
+        std::vector<uint32_t> tok;             // [n_edges]
+        void *dev = nullptr;
+        rk::GenConstraint view; // device pointers into dev, state 0
+    };
+    std::map<unsigned long long, Automaton> automata;
+    unsigned long long next_automaton = 1;
     // score_streams: per scored row its d_slogits row and target in, its results out; grown with the largest call
     struct Score {
         int *rows = nullptr;
@@ -701,15 +717,59 @@ struct LogprobRequest {
     double *top_logprobs_out;
 };
 
+// What generate_streams_constrained adds: an automaton id per stream (or NULL), start states, final states.
+struct ConstraintRequest {
+    const unsigned long long *ids, *start_states;
+    unsigned long long *states_out;
+};
+
+// The automaton of each stream of a constrained call (a zero record: none), refused before any work: unknown ids, start
+// states out of range or without edges, and an automaton with a state whose every edge token the overrides set to -inf.
+int check_constraints(M *m, const char *what, const ConstraintRequest &cq, unsigned long long n_streams,
+                      const unsigned long long *override_tokens, const float *override_values, unsigned long long n_override,
+                      std::vector<rk::GenConstraint> &out) {
+    out.assign(n_streams, rk::GenConstraint{});
+    if (!cq.ids) return 0;
+    std::vector<char> masked(binfmt::kVocab, 0);
+    for (unsigned long long i = 0; i < n_override; ++i) masked[override_tokens[i]] = override_values[i] == -INFINITY;
+    std::vector<unsigned long long> seen;
+    for (unsigned long long s = 0; s < n_streams; ++s) {
+        const unsigned long long id = cq.ids[s];
+        if (id == RWKV_B200_NO_CONSTRAINT) continue;
+        const auto it = m->automata.find(id);
+        if (it == m->automata.end()) return fail(1, "%s: stream %llu: constraint id %llu is unknown or removed", what, s, id);
+        const M::Automaton &a = it->second;
+        const unsigned long long n_states = a.start.size() - 1, q = cq.start_states ? cq.start_states[s] : 0;
+        if (q >= n_states)
+            return fail(1, "%s: stream %llu: start state %llu of constraint %llu is out of range (%llu states)", what, s, q, id,
+                        n_states);
+        if (a.start[q] == a.start[q + 1])
+            return fail(1, "%s: stream %llu: start state %llu of constraint %llu has no edges (the automaton is complete there)",
+                        what, s, q, id);
+        out[s] = a.view;
+        out[s].state = q;
+        if (!n_override || std::find(seen.begin(), seen.end(), id) != seen.end()) continue;
+        seen.push_back(id);
+        for (unsigned long long p = 0; p < n_states; ++p) {
+            bool open = a.start[p] == a.start[p + 1];
+            for (unsigned long long e = a.start[p]; e < a.start[p + 1] && !open; ++e) open = !masked[a.tok[e]];
+            if (!open)
+                return fail(1, "%s: the overrides set every edge token of state %llu of constraint %llu to -inf", what, p, id);
+        }
+    }
+    return 0;
+}
+
 // The body of generate_streams (samplers == NULL, `temp` and `u` pick the typical sampler or the arg-max), of
-// generate_streams_ex (`ex`: every stream has its own sampler, or all pick the arg-max when samplers == NULL) and of
-// generate_streams_logprobs (generate_streams_ex with `lpq`: each emitted token is scored after its pick).
+// generate_streams_ex (`ex`: every stream has its own sampler, or all pick the arg-max when samplers == NULL), of
+// generate_streams_logprobs (generate_streams_ex with `lpq`: each emitted token is scored after its pick) and of
+// generate_streams_constrained (with `cq`: token automata mask the rows after the overrides; `lpq` may be NULL).
 int generate(M *m, const char *what, bool ex, const unsigned long long *slots, const unsigned long long *first_tokens,
              unsigned long long n_streams, unsigned long long max_new, const unsigned long long *budgets,
              const unsigned long long *stop_tokens, unsigned long long n_stop, const unsigned long long *override_tokens,
              const float *override_values, unsigned long long n_override, float temp, const rwkv_b200_sampler *samplers,
              const double *u, unsigned long long *tokens_out, unsigned long long *lengths_out,
-             const LogprobRequest *lpq = nullptr) {
+             const LogprobRequest *lpq = nullptr, const ConstraintRequest *cq = nullptr) {
     int rc = check_streams_model(m, what);
     if (rc) return rc;
     if (lpq) {
@@ -755,8 +815,13 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
     if (u)
         for (unsigned long long i = 0; i < max_new * n_streams; ++i)
             if (!(u[i] >= 0.0 && u[i] < 1.0)) return fail(1, "%s: u[%llu] = %g is outside [0, 1)", what, i, u[i]);
+    std::vector<rk::GenConstraint> hgc;
+    if (cq && (rc = check_constraints(m, what, *cq, n_streams, override_tokens, override_values, n_override, hgc))) return rc;
+    const bool constrained = std::any_of(hgc.begin(), hgc.end(), [](const rk::GenConstraint &c) { return c.mask != nullptr; });
     CK(cudaSetDevice(m->device));
     auto &g = m->gen;
+    if (constrained && ((rc = grow(&g.gc, g.gc_cap, (size_t)n_streams)) || (rc = grow(&g.fault, g.fault_cap, (size_t)3))))
+        return rc;
     if (samplers && (rc = grow(&g.samp, g.samp_cap, (size_t)n_streams))) return rc;
     if (pen && ((rc = grow(&g.pen_cnt, g.pen_cap, (size_t)(n_streams * V))) || (rc = grow(&g.pen_seen, g.seen_cap, (size_t)(n_streams * V)))))
         return rc;
@@ -764,8 +829,8 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
         (rc = grow(&g.ovr_tok, g.ovr_cap, (size_t)n_override)) || (rc = grow(&g.ovr_val, g.ovr_val_cap, (size_t)n_override)) ||
         (u && (rc = grow(&g.u, g.u_cap, (size_t)(kGenGroup * m->max_gpt)))))
         return rc;
-    // raw mode reads the model's rows: d_slogits itself, or a copy taken before the penalties and overrides edit it
-    const bool raw_copy = lpq && lpq->mode == RWKV_B200_LOGPROBS_RAW && (pen || n_override);
+    // raw mode reads the model's rows: d_slogits itself, or a copy taken before the penalties, overrides and mask edit it
+    const bool raw_copy = lpq && lpq->mode == RWKV_B200_LOGPROBS_RAW && (pen || n_override || constrained);
     const size_t n_lp = (size_t)(n_streams * max_new), n_top = lpq ? n_lp * lpq->top_n : 0;
     if (lpq && ((rc = grow(&g.lp, g.lp_cap, n_lp)) || (rc = grow(&g.rank, g.rank_cap, n_lp)) ||
                 (rc = grow(&g.top_tok, g.top_tok_cap, n_top)) || (rc = grow(&g.top_lp, g.top_lp_cap, n_top)) ||
@@ -786,6 +851,10 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
         CK(cudaMemcpyAsync(g.ovr_val, override_values, n_override * sizeof(float), cudaMemcpyHostToDevice, m->stream));
     }
     if (samplers) CK(cudaMemcpyAsync(g.samp, samplers, n_streams * sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
+    if (constrained) {
+        CK(cudaMemcpyAsync(g.gc, hgc.data(), n_streams * sizeof(rk::GenConstraint), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemsetAsync(g.fault, 0, 3 * sizeof(unsigned long long), m->stream));
+    }
     if (pen) { // the history starts empty in every call: prompt tokens are not counted
         CK(cudaMemsetAsync(g.pen_cnt, 0, n_streams * V * sizeof(float), m->stream));
         CK(cudaMemsetAsync(g.pen_seen, 0, n_streams * V, m->stream));
@@ -827,7 +896,7 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
             CK(cudaMemcpyAsync(g.u, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
         }
         rk::GenFeedbackArgs fb{g.gs, g.row_stream, rows, u || samplers ? nullptr : m->d_next, m->d_sample, g.stop, (int)n_stop, g.out, max_new,
-                               tc ? g.passes : nullptr};
+                               tc ? g.passes : nullptr, constrained ? g.gc : nullptr, g.fault};
         rk::GenLogprobArgs la{};
         if (lpq)
             la = rk::GenLogprobArgs{raw_copy ? g.raw : m->d_slogits, (int)V, g.gs, g.row_stream, fb.next, m->d_sample,
@@ -847,6 +916,12 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
             }
             if (n_override) {
                 rk::k_gen_override<<<rb, 128, 0, m->stream>>>(m->d_slogits, (int)V, rows, g.ovr_tok, g.ovr_val, (int)n_override);
+                CK(cudaGetLastError());
+                m->launches += 1;
+            }
+            if (constrained) {
+                const dim3 grid((unsigned)((V + rk::kMaskThreads - 1) / rk::kMaskThreads), (unsigned)rows);
+                rk::k_gen_mask<<<grid, rk::kMaskThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs, g.row_stream, g.gc);
                 CK(cudaGetLastError());
                 m->launches += 1;
             }
@@ -870,7 +945,12 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
         }
         // the end of a group: which streams are done (a few bytes, one synchronisation); drop them from the rows
         CK(cudaMemcpyAsync(hg, g.gs, n_streams * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
+        unsigned long long fault[3] = {0, 0, 0};
+        if (constrained) CK(cudaMemcpyAsync(fault, g.fault, sizeof(fault), cudaMemcpyDeviceToHost, m->stream));
         SYNC(m);
+        if (fault[0])
+            return fail(8, "%s: stream %llu emitted token %llu, which has no edge out of state %llu of its constraint", what,
+                        fault[0] - 1, fault[1], fault[2]);
         step += steps;
         live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hg[s].done != 0; }), live.end());
     }
@@ -883,8 +963,12 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
             CK(cudaMemcpyAsync(lpq->top_logprobs_out, g.top_lp, n_top * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
         }
     }
+    if (constrained && cq->states_out)
+        CK(cudaMemcpyAsync(hgc.data(), g.gc, n_streams * sizeof(rk::GenConstraint), cudaMemcpyDeviceToHost, m->stream));
     SYNC(m);
     for (unsigned long long s = 0; s < n_streams; ++s) lengths_out[s] = hg[s].len;
+    if (cq && cq->states_out)
+        for (unsigned long long s = 0; s < n_streams; ++s) cq->states_out[s] = hgc[s].mask ? hgc[s].state : 0;
     return 0;
 }
 
@@ -955,8 +1039,9 @@ void rwkv_b200_free(rwkv_b200_model *m) {
                     (void *)m->gen.samp, (void *)m->gen.pen_cnt, (void *)m->gen.pen_seen, (void *)m->score.rows,
                     (void *)m->score.tgt, (void *)m->score.rank, (void *)m->score.top_tok, (void *)m->score.lp,
                     (void *)m->score.top_lp, (void *)m->gen.lp, (void *)m->gen.top_lp, (void *)m->gen.rank,
-                    (void *)m->gen.top_tok, (void *)m->gen.raw})
+                    (void *)m->gen.top_tok, (void *)m->gen.raw, (void *)m->gen.gc, (void *)m->gen.fault})
         if (p) cudaFree(p);
+    for (auto &kv : m->automata) cudaFree(kv.second.dev);
     if (m->stream) cudaStreamDestroy(m->stream);
     cudaGetLastError(); // a context killed by a trap makes every call above fail; do not leave that as "last error"
     delete m;
@@ -1218,6 +1303,96 @@ int rwkv_b200_generate_streams_logprobs(rwkv_b200_model *m, const unsigned long 
     return generate(m, "generate_streams_logprobs", true, slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop,
                     override_tokens, override_values, n_override, 1.0f, samplers, samplers ? u : nullptr, tokens_out, lengths_out,
                     &lpq);
+}
+
+int rwkv_b200_constraint_add(rwkv_b200_model *m, unsigned long long n_states, const unsigned long long *edge_start,
+                             const unsigned long long *edge_tokens, const unsigned long long *edge_next, unsigned long long *id) {
+    const char *what = "constraint_add";
+    int rc = check_streams_model(m, what);
+    if (rc) return rc;
+    if (!edge_start || !id) return fail(1, "%s: null argument (edge_start and id are required)", what);
+    if (n_states == 0 || n_states > RWKV_B200_MAX_CONSTRAINT_STATES)
+        return fail(1, "%s: n_states = %llu is outside 1..%d", what, n_states, RWKV_B200_MAX_CONSTRAINT_STATES);
+    if (edge_start[0] != 0) return fail(1, "%s: edge_start[0] = %llu, not 0", what, edge_start[0]);
+    for (unsigned long long q = 0; q < n_states; ++q)
+        if (edge_start[q + 1] < edge_start[q])
+            return fail(1, "%s: edge_start decreases from state %llu to %llu (%llu > %llu)", what, q, q + 1, edge_start[q],
+                        edge_start[q + 1]);
+    const unsigned long long n_edges = edge_start[n_states];
+    if (n_edges && (!edge_tokens || !edge_next)) return fail(1, "%s: %llu edges with NULL edge_tokens or edge_next", what, n_edges);
+    for (unsigned long long q = 0; q < n_states; ++q)
+        for (unsigned long long e = edge_start[q]; e < edge_start[q + 1]; ++e) {
+            if (edge_tokens[e] >= binfmt::kVocab)
+                return fail(1, "%s: state %llu: edge token %llu out of range", what, q, edge_tokens[e]);
+            if (e > edge_start[q] && edge_tokens[e] <= edge_tokens[e - 1])
+                return fail(1, "%s: state %llu: edge tokens are not strictly ascending (%llu after %llu)", what, q, edge_tokens[e],
+                            edge_tokens[e - 1]);
+            if (edge_next[e] >= n_states)
+                return fail(1, "%s: state %llu: edge of token %llu leads to state %llu >= n_states %llu", what, q, edge_tokens[e],
+                            edge_next[e], n_states);
+        }
+    // one block: the allow masks [n_states][kMaskWords] u32, edge_start [n_states + 1] u64, tokens and targets [n_edges] u32
+    const size_t mask_bytes = (size_t)n_states * rk::kMaskWords * 4, start_bytes = (size_t)(n_states + 1) * 8;
+    const size_t bytes = mask_bytes + start_bytes + (size_t)n_edges * 8;
+    M::Automaton a;
+    std::vector<unsigned char> blob;
+    try {
+        blob.assign(bytes, 0);
+        a.start.assign(edge_start, edge_start + n_states + 1);
+        a.tok.resize(n_edges);
+    } catch (const std::bad_alloc &) {
+        return fail(9, "%s: out of host memory for %llu states and %llu edges", what, n_states, n_edges);
+    }
+    uint32_t *mask = (uint32_t *)blob.data(), *tok = (uint32_t *)(blob.data() + mask_bytes + start_bytes), *next = tok + n_edges;
+    memcpy(blob.data() + mask_bytes, edge_start, start_bytes);
+    for (unsigned long long q = 0; q < n_states; ++q)
+        for (unsigned long long e = edge_start[q]; e < edge_start[q + 1]; ++e) {
+            const uint32_t t = (uint32_t)edge_tokens[e];
+            mask[q * rk::kMaskWords + (t >> 5)] |= 1u << (t & 31);
+            tok[e] = a.tok[e] = t;
+            next[e] = (uint32_t)edge_next[e];
+        }
+    CK(cudaSetDevice(m->device));
+    CK(cudaMalloc(&a.dev, bytes));
+    const cudaError_t e = cudaMemcpy(a.dev, blob.data(), bytes, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        cudaFree(a.dev);
+        return fail(100 + (int)e, "%s: upload failed: %s", what, cudaGetErrorString(e));
+    }
+    unsigned char *d = (unsigned char *)a.dev;
+    a.view = rk::GenConstraint{(const unsigned long long *)(d + mask_bytes), (const uint32_t *)(d + mask_bytes + start_bytes),
+                               (const uint32_t *)(d + mask_bytes + start_bytes) + n_edges, (const uint32_t *)d, 0};
+    *id = m->next_automaton++;
+    m->automata.emplace(*id, std::move(a));
+    return 0;
+}
+
+int rwkv_b200_constraint_remove(rwkv_b200_model *m, unsigned long long id) {
+    int rc = check_model(m);
+    if (rc) return rc;
+    const auto it = m->automata.find(id);
+    if (it == m->automata.end()) return fail(1, "constraint_remove: constraint id %llu is unknown or removed", id);
+    CK(cudaSetDevice(m->device));
+    cudaFree(it->second.dev);
+    m->automata.erase(it);
+    return 0;
+}
+
+int rwkv_b200_generate_streams_constrained(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
+                                           unsigned long long n_streams, unsigned long long max_new, const unsigned long long *budgets,
+                                           const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                           const unsigned long long *override_tokens, const float *override_values,
+                                           unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
+                                           unsigned long long *tokens_out, unsigned long long *lengths_out, int logprob_mode,
+                                           unsigned int top_n, double *logprobs_out, unsigned long long *ranks_out,
+                                           unsigned long long *top_tokens_out, double *top_logprobs_out,
+                                           const unsigned long long *constraint_ids, const unsigned long long *start_states,
+                                           unsigned long long *states_out) {
+    const LogprobRequest lpq{logprob_mode, top_n, logprobs_out, ranks_out, top_tokens_out, top_logprobs_out};
+    const ConstraintRequest cq{constraint_ids, start_states, states_out};
+    return generate(m, "generate_streams_constrained", true, slots, first_tokens, n_streams, max_new, budgets, stop_tokens,
+                    n_stop, override_tokens, override_values, n_override, 1.0f, samplers, samplers ? u : nullptr, tokens_out,
+                    lengths_out, logprobs_out ? &lpq : nullptr, &cq);
 }
 
 int rwkv_b200_sample_streams(rwkv_b200_model *m, unsigned long long n_streams, const rwkv_b200_sampler *params, const double *u,

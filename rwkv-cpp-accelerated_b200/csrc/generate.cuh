@@ -7,10 +7,13 @@
 // appends the picked token, decides whether the stream is done and writes the next step's input. A stream that
 // finishes inside a group keeps its row until the group ends but is frozen: its slot is not written again.
 // generate_streams_logprobs adds k_gen_logprob (score.cuh) between the pick and k_gen_feedback.
+// generate_streams_constrained adds k_gen_mask after the overrides, and k_gen_feedback advances each constrained
+// stream's token automaton (GenConstraint) after appending its token.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "../../include/rwkv_b200.h"
 #include "common.cuh"
 #include "prefill.cuh"
 
@@ -39,6 +42,31 @@ __global__ void k_gen_override(float *logits, int V, int rows, const unsigned lo
     for (int i = 0; i < n; ++i) logits[(size_t)r * V + tok[i]] = val[i];
 }
 
+// A stream's token automaton (include/rwkv_b200.h, rwkv_b200_constraint_add) and its current state. State q's edges are
+// tok[start[q] .. start[q + 1]) (ascending) with targets next[..]; mask[q] has bit v set when token v has an edge out of
+// q. mask == nullptr: the stream has no constraint.
+constexpr int kMaskWords = (int)((RWKV_B200_VOCAB + 31) / 32); // u32 words of one state's allow mask
+struct GenConstraint {
+    const unsigned long long *start; // [n_states + 1]
+    const uint32_t *tok, *next;      // [n_edges]
+    const uint32_t *mask;            // [n_states][kMaskWords]
+    unsigned long long state;
+};
+
+// logits[r][v] = -inf for every token v without an edge out of the current state of row r's stream. Grid
+// (ceil(V / kMaskThreads), rows), one thread per token. Unconstrained and finished streams are left alone: a finished
+// stream may sit in a state without edges, and masking its row would leave the pick no finite value.
+constexpr int kMaskThreads = 256;
+__global__ void __launch_bounds__(kMaskThreads) k_gen_mask(float *logits, int V, const GenStream *gs, const int *row_stream,
+                                                           const GenConstraint *gc) {
+    const int r = blockIdx.y, s = row_stream[r];
+    const GenConstraint &c = gc[s];
+    if (!c.mask || gs[s].done) return;
+    const int v = blockIdx.x * kMaskThreads + threadIdx.x;
+    if (v >= V) return;
+    if (!((c.mask[c.state * kMaskWords + (v >> 5)] >> (v & 31)) & 1u)) logits[(size_t)r * V + v] = -INFINITY;
+}
+
 struct GenFeedbackArgs {
     GenStream *gs;
     const int *row_stream;           // [rows] stream of each row
@@ -50,6 +78,8 @@ struct GenFeedbackArgs {
     unsigned long long *out;         // [n_streams][max_new]
     unsigned long long max_new;
     PassDesc *passes;                // tensor-core path: the descriptors of the next step, else nullptr
+    GenConstraint *gc;               // [n_streams] generate_streams_constrained, else nullptr
+    unsigned long long *fault;       // {stream + 1, token, state} of the first emitted token without an edge (gc only)
 };
 
 // One thread per row: emit the picked token of a live stream, then write the next step's input. On the tensor-core
@@ -67,6 +97,29 @@ __global__ void k_gen_feedback(const GenFeedbackArgs a) {
         g.tok = tok;
         bool stop = g.len == g.budget;
         for (int i = 0; i < a.n_stop; ++i) stop |= a.stop[i] == tok;
+        if (a.gc && a.gc[s].mask) {
+            // advance the automaton; a state without edges completes it. The mask makes a missing edge impossible
+            // unless the pick broke its contract: record it for the host and end the stream
+            GenConstraint &c = a.gc[s];
+            const unsigned long long q = c.state, end = c.start[q + 1];
+            unsigned long long lo = c.start[q], hi = end;
+            while (lo < hi) {
+                const unsigned long long mid = (lo + hi) / 2;
+                if (c.tok[mid] < tok) lo = mid + 1;
+                else hi = mid;
+            }
+            if (lo < end && c.tok[lo] == tok) {
+                const unsigned long long q2 = c.next[lo];
+                c.state = q2;
+                stop |= c.start[q2] == c.start[q2 + 1];
+            } else {
+                if (atomicCAS(a.fault, 0ull, (unsigned long long)s + 1) == 0ull) {
+                    a.fault[1] = tok;
+                    a.fault[2] = q;
+                }
+                stop = true;
+            }
+        }
         g.done = stop ? 1ull : 0ull;
         a.gs[s] = g;
     }

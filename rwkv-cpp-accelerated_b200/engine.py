@@ -13,6 +13,8 @@ MODE_PARRALEL, MODE_GPT = 0, 1
 NO_TARGET = 0xFFFFFFFFFFFFFFFF  # RWKV_B200_NO_TARGET: a position score_streams does not score
 MAX_TOP_N = 20                  # RWKV_B200_MAX_TOP_N
 LOGPROBS_RAW, LOGPROBS_PROCESSED = 0, 1  # RWKV_B200_LOGPROBS_*: the row generate_streams(logprobs=...) scores on
+NO_CONSTRAINT = 0xFFFFFFFFFFFFFFFF       # RWKV_B200_NO_CONSTRAINT: a stream of a constrained call without an automaton
+MAX_CONSTRAINT_STATES = 65536            # RWKV_B200_MAX_CONSTRAINT_STATES
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
@@ -123,6 +125,11 @@ def load_library():
         "rwkv_b200_generate_streams_logprobs": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull,
                                                       c.POINTER(Sampler), pdbl, pull, pull, i32, c.c_uint, pdbl, pull, pull,
                                                       pdbl]),
+        "rwkv_b200_constraint_add": (i32, [vp, ull, pull, pull, pull, pull]),
+        "rwkv_b200_constraint_remove": (i32, [vp, ull]),
+        "rwkv_b200_generate_streams_constrained": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull,
+                                                         c.POINTER(Sampler), pdbl, pull, pull, i32, c.c_uint, pdbl, pull,
+                                                         pull, pdbl, pull, pull, pull]),
         "rwkv_b200_slot_zero": (i32, [vp, ull]),
         "rwkv_b200_slot_copy": (i32, [vp, ull, ull]),
         "rwkv_b200_slot_upload": (i32, [vp, ull, pdbl, pdbl, pdbl, pdbl, pdbl]),
@@ -268,7 +275,7 @@ class Engine:
         return toks, margins
 
     def generate_streams(self, streams, max_new, budgets=None, stop=(), overrides=None, temp=None, u=None, sampling=None,
-                         logprobs=None, top_n=0):
+                         logprobs=None, top_n=0, constraints=None):
         """Generate up to max_new tokens per stream on the device: streams = [(slot, first_token), ...].
         Arg-max when u is None, else the typical sampler with u[step][stream] and temp (default 1.0). budgets: tokens
         per stream (None = max_new each); stop: token ids that end a stream (emitted, not fed); overrides = {token:
@@ -279,7 +286,15 @@ class Engine:
         available) also scores each emitted token on the device (rwkv_b200_generate_streams_logprobs): "raw" on the
         model's logits, "processed" on the row the sampler read divided by the stream's temperature. Then it returns
         one dict per stream: "tokens", "logprobs" (float64), "ranks" (uint64, tokens ranked before the emitted one),
-        and with top_n > 0 "top_tokens" [len][top_n] and "top_logprobs" [len][top_n], each as long as the stream."""
+        and with top_n > 0 "top_tokens" [len][top_n] and "top_logprobs" [len][top_n], each as long as the stream.
+        constraints: one id of add_constraint for every stream, or one entry per stream: an id, (id, start_state) or
+        None (rwkv_b200_generate_streams_constrained: each step masks every token without an edge out of the stream's
+        automaton state, and a stream ends when its state has no edges). Then it returns one dict per stream with
+        "tokens" and "state" (the final automaton state, None without a constraint), plus the logprob fields when
+        logprobs is given. Like logprobs, constraints need sampling=... or the arg-max (not the typical sampler)."""
+        if constraints is not None:
+            return self._generate_constrained(streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs,
+                                              top_n, constraints)
         if logprobs is not None:
             return self._generate_logprobs(streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n)
         temp = 1.0 if temp is None else temp
@@ -324,6 +339,60 @@ class Engine:
             if top_n > 0:
                 d["top_tokens"] = top_tok[s, :n].copy()
                 d["top_logprobs"] = top_lp[s, :n].copy()
+            res.append(d)
+        return res
+
+    def add_constraint(self, automaton):
+        """Upload a token automaton (constrain.TokenAutomaton, or anything with its edge_start, edge_tokens and
+        edge_next arrays) for generate_streams(constraints=...); returns its id."""
+        start = np.ascontiguousarray(automaton.edge_start, np.uint64)
+        toks = np.ascontiguousarray(automaton.edge_tokens, np.uint64)
+        nxt = np.ascontiguousarray(automaton.edge_next, np.uint64)
+        cid = ctypes.c_ulonglong()
+        P = ctypes.c_ulonglong
+        self._ck(self.lib.rwkv_b200_constraint_add(self.h, len(start) - 1, _ptr(start, P), _ptr(toks, P), _ptr(nxt, P),
+                                                   ctypes.byref(cid)), "constraint_add")
+        return int(cid.value)
+
+    def remove_constraint(self, cid):
+        self._ck(self.lib.rwkv_b200_constraint_remove(self.h, int(cid)), "constraint_remove")
+
+    def _generate_constrained(self, streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n,
+                              constraints):
+        modes = {None: LOGPROBS_RAW, "raw": LOGPROBS_RAW, "processed": LOGPROBS_PROCESSED}
+        if logprobs not in modes:
+            raise EngineError("generate_streams: logprobs must be 'raw' or 'processed', not %r" % (logprobs,))
+        if sampling is None and (u is not None or temp is not None):
+            raise EngineError("generate_streams: constraints need sampling=... (or neither u nor temp, for the arg-max); "
+                              "the typical sampler does not take them")
+        S, slots, first, bud, stops, otok, oval, us, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u)
+        spec = [constraints] * S if isinstance(constraints, (int, np.integer)) else list(constraints)
+        if len(spec) != S:
+            raise EngineError("generate_streams: %d constraints for %d streams" % (len(spec), S))
+        pairs = [(NO_CONSTRAINT, 0) if c is None else (int(c[0]), int(c[1])) if isinstance(c, (tuple, list)) else (int(c), 0)
+                 for c in spec]
+        ids = np.ascontiguousarray([c for c, _ in pairs], np.uint64)
+        starts = np.ascontiguousarray([q for _, q in pairs], np.uint64)
+        states = np.zeros(S, np.uint64)
+        lp = np.empty((S, max_new), np.float64) if logprobs is not None else None
+        ranks = np.empty((S, max_new), np.uint64) if logprobs is not None else None
+        top_tok = np.empty((S, max_new, top_n), np.uint64) if logprobs is not None and top_n > 0 else None
+        top_lp = np.empty((S, max_new, top_n), np.float64) if logprobs is not None and top_n > 0 else None
+        P = ctypes.c_ulonglong
+        sp = _samplers(sampling, S) if sampling is not None else None
+        self._ck(self.lib.rwkv_b200_generate_streams_constrained(
+            self.h, _ptr(slots, P), _ptr(first, P), S, max_new, _ptr(bud, P), _ptr(stops, P), len(stops), _ptr(otok, P),
+            _ptr(oval, ctypes.c_float), len(otok), sp, _ptr(us, ctypes.c_double), _ptr(out, P), _ptr(lens, P),
+            modes[logprobs], int(top_n), _ptr(lp, ctypes.c_double), _ptr(ranks, P), _ptr(top_tok, P),
+            _ptr(top_lp, ctypes.c_double), _ptr(ids, P), _ptr(starts, P), _ptr(states, P)), "generate_streams_constrained")
+        res = []
+        for s in range(S):
+            n = int(lens[s])
+            d = {"tokens": out[s, :n].copy(), "state": int(states[s]) if ids[s] != np.uint64(NO_CONSTRAINT) else None}
+            if logprobs is not None:
+                d["logprobs"], d["ranks"] = lp[s, :n].copy(), ranks[s, :n].copy()
+                if top_n > 0:
+                    d["top_tokens"], d["top_logprobs"] = top_tok[s, :n].copy(), top_lp[s, :n].copy()
             res.append(d)
         return res
 
