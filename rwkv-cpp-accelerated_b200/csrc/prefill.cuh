@@ -14,7 +14,9 @@
 // 64 rows x (3 Tp) x 128 bytes of K per stage; each consumer warpgroup owns NB = Tp / 32 blocks of 16 tokens in
 // all three planes (at most 3 x 4 x 8 accumulator registers per thread). NB is a template parameter so that every
 // wgmma sits on a uniform path (a data-dependent branch around them makes the compiler serialise them). Split-K
-// partial sums are added with integer atomics (exact, order-free).
+// partial sums are added with integer atomics (exact, order-free). Any K that is a multiple of 16 (every n_embed the
+// loader accepts) works: K tiles round up and the out-of-bounds tail of the last one is zero-filled by TMA in both
+// operands; split-K is used only when every split is a whole number of 128-byte tiles.
 // Everything around the GEMMs (layernorm, token shift, WKV scan over t, activations, quantisation) is plain
 // CUDA, one small kernel per step, with the reference's rounding points (rwkv.cu:40-57, 221-259, 313-465).
 //
@@ -119,7 +121,9 @@ __global__ void __launch_bounds__(kPfThreads, 1) k_gemm_i8(const __grid_constant
     auto empty = [&](int s) { return bars + 8u * (uint32_t)(kPfStages + s); };
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.x * kPfBM;
-    const int kper = g.K / g.ksplit, k0 = blockIdx.y * kper, nkt = kper / kPfBK;
+    // K tiles round up: the last tile of a K that is not a multiple of 128 (ksplit = 1 only) reaches past the end of
+    // both operands, and TMA fills that part of the box with zeros (and still counts the whole box's bytes).
+    const int kper = g.K / g.ksplit, k0 = blockIdx.y * kper, nkt = (kper + kPfBK - 1) / kPfBK;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < kPfStages; ++s) {

@@ -1,7 +1,8 @@
 """Parity at the sizes and lengths BASELINE.json names, against the REFERENCE ITSELF: what the unmodified
 rwkv.cu + rwkv.h computed on the same seeded models (tests/golden/ref_*.npz, written by
 tests/golden/make_reference_golden.py from a greedy decode by the reference). The engine replays the same tokens
-teacher-forced, logits are compared at every dumped step and the recurrent state at the end. Plus stress models
+teacher-forced, token by token through the decode kernel and as one GPT chunk on the tensor cores; logits are compared
+at every dumped step and the recurrent state at the end. Plus stress models
 for the fixed-point activation quantiser and the layernorm statistics: outlier channels, a tiny residual stream
 and a residual stream with a large mean.
 
@@ -68,6 +69,39 @@ def test_decode_matches_the_reference_at_baseline_sizes(pkg, workload, n_tokens,
     worst, checked, compared, _ = compare_with_reference(pkg, bench_model(pkg, workload), workload, n_tokens)
     print("%s x %d tokens vs the reference CUDA build: worst logits rel err %.3g over %d compared steps, argmax checked on %d"
           % (workload, n_tokens, worst, compared, checked))
+
+
+@pytest.mark.parametrize("workload,n_tokens", [
+    ("169m", 256),   # two passes of 128
+    ("1b5", 1024),   # eight passes of 128
+    ("7b", 64),      # one pass of 64
+    ("14b", 64),     # one pass of 64 at 40 x 5120
+])
+def test_tensor_core_chunk_matches_the_reference_at_baseline_sizes(pkg, workload, n_tokens):
+    """The same token lists as one GPT-mode forward on the tensor cores (csrc/prefill.cuh), compared at every dumped
+    step and in the final state."""
+    g = reference_golden(workload)
+    toks = [int(t) for t in g["tokens"]][:n_tokens]
+    assert len(toks) == n_tokens
+    eng = pkg.Engine(bench_model(pkg, workload), max_gpt=n_tokens)
+    got = eng.forward(toks, mode=1)
+    worst, checked, compared = 0.0, 0, 0
+    for i, step in enumerate(int(s) for s in g["steps"]):
+        if step >= n_tokens:
+            continue
+        e = golden_logits_err(got[step], g, i)
+        worst = max(worst, e)
+        compared += 1
+        assert e < REL_TOL, "step %d: logits rel err %.3g" % (step, e)
+        if g["margin"][i] > 1e-3:
+            assert int(got[step].argmax()) == int(g["argmax"][i]), "step %d argmax" % step
+            checked += 1
+    st = eng.state_download()
+    eng.close()
+    serr = max(golden_state_err(st[k], g, k) for k in ("xy", "aa", "bb", "dd"))
+    print("%s x %d tokens in one tensor-core chunk vs the reference CUDA build: worst logits rel err %.3g over %d compared "
+          "steps, argmax checked on %d, state %.3g" % (workload, n_tokens, worst, compared, checked, serr))
+    assert serr < REL_TOL
 
 
 @pytest.mark.parametrize("kind", ["outliers", "tiny_residual", "offset_residual"])
