@@ -391,6 +391,47 @@ int rwkv_b200_generate_streams_constrained(rwkv_b200_model *m, const unsigned lo
                                            const unsigned long long *constraint_ids,
                                            const unsigned long long *start_states, unsigned long long *states_out);
 
+/* Beam search on the device: the n_best best continuations of each of n_groups prompts (translation, summarisation,
+ * extraction, n-best reranking). Group g owns the `beams` = B distinct slots slots[g * B .. g * B + B): slots[g * B]
+ * holds the prompt state, the others are overwritten. Its first input is first_tokens[g] (the (slot, first_token)
+ * convention of generate_streams). max_new = N, the stop tokens Z, length_penalty = alpha (any finite value) and
+ * n_best = K (1 <= K <= B) are shared by every group; B + n_stop <= RWKV_B200_MAX_TOP_N. The rule, per group:
+ *  1. Step 0 has one live beam: cum = 0, no tokens, input first_tokens[g] on slots[g * B]. Later steps have B live
+ *     beams, j = 0..B-1.
+ *  2. Expansion: each live beam's logits row l of the step gives the first B + n_stop tokens of the ranking (l
+ *     descending, ties by lower index: the ranking of rwkv_b200_score_streams) with their logprobs by score_streams'
+ *     formula, bit for bit what score_streams reports as top entries. A candidate's score is c = cum + logprob (double).
+ *  3. The group's candidates are ordered by (c descending, beam index ascending, rank in its row ascending).
+ *  4. Walk from position 0: a stop token at position < B is offered to the hypothesis list as a finished hypothesis (the
+ *     beam's tokens and the stop token, len = that length, score = c / P[len]); a stop token at position >= B is skipped;
+ *     every other token becomes the next new live beam until there are B of them (new beam j = the j-th such candidate).
+ *  5. P[n] = pow((double)n, alpha) for n = 1..N, computed on the host by the C library's pow.
+ *  6. The hypothesis list keeps the K best offered hypotheses by (score descending, offer order ascending); a new one
+ *     enters only when fewer than K are held or its score is strictly above the worst one held.
+ *  7. After the walk of step N - 1 the B live beams are offered in order j as unfinished hypotheses (len = N).
+ *  8. A group is done when it holds K hypotheses and no live beam can beat the worst of them: a live beam with cum c and
+ *     n tokens can score at most c / P[N] when alpha >= 0, and c / P[n + 1] when alpha < 0 (every logprob is <= 0). The
+ *     result is exactly what running every group to N steps returns. A done group runs no more steps.
+ *  9. Slots: after the walk, new beam j with parent p takes p's slot if no earlier new beam took it, else the next free
+ *     slot: the slots of the previous beams without a child, in ascending beam index (at step 0: slots[g * B + 1 ..
+ *     g * B + B), in that order), and a copy of the parent's state (rwkv_b200_slot_copy). A group that becomes done
+ *     copies nothing, so its slots hold the states its last step's beams left (no slot holds a hypothesis' final state:
+ *     a caller continues a hypothesis by feeding its text with forward_streams).
+ * The forward path is forward_streams' rule for n_groups * beams one-token streams, chosen once per call.
+ * Outputs, hypotheses best first, each group exactly n_best of them: tokens_out [n_groups][n_best][max_new] (0 past the
+ * length), lengths_out [n_groups][n_best], logprobs_out [n_groups][n_best] (cum: the left-to-right double sum of the
+ * token logprobs), scores_out [n_groups][n_best], finished_out [n_groups][n_best] (1: ended by a stop token), and, if
+ * not NULL, token_logprobs_out [n_groups][n_best][max_new] (NaN past the length). Refused before any work (every slot
+ * untouched): a missing required array, n_groups == 0, beams == 0, beams + n_stop > RWKV_B200_MAX_TOP_N, n_best == 0 or
+ * > beams, max_new == 0, a slot out of range or repeated, a first or stop token >= 50277, a non-finite length_penalty,
+ * and tensor parallelism. After the call no per-stream logits are held, as after generate_streams. */
+int rwkv_b200_beam_search(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
+                          unsigned long long n_groups, unsigned beams, unsigned long long max_new,
+                          const unsigned long long *stop_tokens, unsigned long long n_stop, double length_penalty,
+                          unsigned n_best, unsigned long long *tokens_out, unsigned long long *lengths_out,
+                          double *logprobs_out, double *scores_out, unsigned char *finished_out,
+                          double *token_logprobs_out);
+
 /* State of one slot: zero it (a new conversation), copy it onto another slot (fork a conversation), or move it
  * between the device and host arrays of n_layers x n_embed doubles each (NULL arrays are skipped). */
 int rwkv_b200_slot_zero(rwkv_b200_model *m, unsigned long long slot);

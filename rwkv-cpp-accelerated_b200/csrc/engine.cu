@@ -33,6 +33,7 @@
 #include "../../include/rwkv/enums/enum.h"
 #include "../../include/rwkv_b200.h"
 #include "aux_kernels.cuh"
+#include "beam.cuh"
 #include "binfmt.h"
 #include "generate.cuh"
 #include "prefill.cuh"
@@ -137,6 +138,19 @@ struct rwkv_b200_model {
         double *lp = nullptr, *top_lp = nullptr;
         size_t rows_cap = 0, tgt_cap = 0, rank_cap = 0, top_tok_cap = 0, lp_cap = 0, top_lp_cap = 0;
     } score;
+    // beam_search: the beams' records live in gen.gs (beam j of group g is record g * B + j); the rest grows with the
+    // largest call
+    struct Beam {
+        int *row0 = nullptr, *groups = nullptr;          // [G] step 0's row map, [G] the live groups of a host group
+        unsigned long long *cand_tok = nullptr;          // [rows][C]
+        double *cand_lp = nullptr, *cum = nullptr, *P = nullptr; // [rows][C], [G * B], [N + 1]
+        rk::BeamBack *back = nullptr;                    // [G][N][B]
+        rk::BeamHyp *hyp = nullptr;                      // [G][K]
+        int *n_hyp = nullptr;                            // [G]
+        unsigned long long *done = nullptr, *forks = nullptr; // [G], [G * B][2]
+        size_t row0_cap = 0, groups_cap = 0, cand_tok_cap = 0, cand_lp_cap = 0, cum_cap = 0, P_cap = 0, back_cap = 0,
+               hyp_cap = 0, n_hyp_cap = 0, done_cap = 0, forks_cap = 0;
+    } beam;
 };
 
 namespace {
@@ -646,11 +660,11 @@ constexpr unsigned long long kGenGroup = 16;
 constexpr float kMaxPenalty = 1e6f;
 
 // One step of generate_streams over `rows` rows on the decode kernel: each row on its stream's slot (or the scratch
-// slot once the stream is done), its logits into row r of d_slogits.
-int gen_step_decode(M *m, int rows) {
+// slot once the stream is done), its logits into row r of d_slogits. row_stream: the stream record of each row.
+int gen_step_decode(M *m, int rows, const int *row_stream) {
     const size_t V = binfmt::kVocab;
     for (int r = 0; r < rows; ++r) {
-        rk::k_gen_gate<<<1, 1, 0, m->stream>>>(m->gen.gs, m->gen.row_stream, r, m->max_gpt, m->p.ctrl);
+        rk::k_gen_gate<<<1, 1, 0, m->stream>>>(m->gen.gs, row_stream, r, m->max_gpt, m->p.ctrl);
         CK(cudaGetLastError());
         int rc = launch_token(m, 0, false, nullptr, m->stream);
         if (rc) return rc;
@@ -904,7 +918,7 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
                                     (int)lpq->top_n, max_new, g.lp, g.rank, g.top_tok, g.top_lp};
         const unsigned rb = (unsigned)((rows + 127) / 128);
         for (unsigned long long k = 0; k < steps; ++k) {
-            if ((rc = tc ? gen_step_passes(m, rows) : gen_step_decode(m, rows))) return rc;
+            if ((rc = tc ? gen_step_passes(m, rows) : gen_step_decode(m, rows, g.row_stream))) return rc;
             if (raw_copy)
                 CK(cudaMemcpyAsync(g.raw, m->d_slogits, (size_t)rows * V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
             if (pen) {
@@ -969,6 +983,173 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
     for (unsigned long long s = 0; s < n_streams; ++s) lengths_out[s] = hg[s].len;
     if (cq && cq->states_out)
         for (unsigned long long s = 0; s < n_streams; ++s) cq->states_out[s] = hgc[s].mask ? hgc[s].state : 0;
+    return 0;
+}
+
+// The body of rwkv_b200_beam_search: generate()'s group loop over beams. Step 0 has one row per group, later steps B
+// rows per live group (group by group); each step is forward -> k_beam_expand -> k_beam_select -> k_beam_fork. At each
+// host group's end the done flags come back and the done groups leave the rows; at the end the backpointers and the
+// hypothesis lists come back once and the host rebuilds each hypothesis' tokens.
+int beam(M *m, const unsigned long long *slots, const unsigned long long *first_tokens, unsigned long long n_groups,
+         unsigned beams, unsigned long long max_new, const unsigned long long *stop_tokens, unsigned long long n_stop,
+         double length_penalty, unsigned n_best, unsigned long long *tokens_out, unsigned long long *lengths_out,
+         double *logprobs_out, double *scores_out, unsigned char *finished_out, double *token_logprobs_out) {
+    const char *what = "beam_search";
+    int rc = check_streams_model(m, what);
+    if (rc) return rc;
+    if (!slots || !first_tokens || !tokens_out || !lengths_out || !logprobs_out || !scores_out || !finished_out)
+        return fail(1, "%s: null argument (slots, first_tokens, tokens_out, lengths_out, logprobs_out, scores_out and "
+                       "finished_out are required)", what);
+    if (n_stop && !stop_tokens) return fail(1, "%s: n_stop = %llu with NULL stop_tokens", what, n_stop);
+    if (n_groups == 0) return fail(1, "%s: no groups", what);
+    if (beams == 0) return fail(1, "%s: beams is 0", what);
+    if (n_stop > (unsigned long long)rk::kMaxTopN || beams + n_stop > (unsigned long long)rk::kMaxTopN)
+        return fail(1, "%s: beams + n_stop = %u + %llu > %d", what, beams, n_stop, rk::kMaxTopN);
+    if (n_best == 0 || n_best > beams) return fail(1, "%s: n_best %u is outside 1..beams = %u", what, n_best, beams);
+    if (max_new == 0) return fail(1, "%s: max_new is 0", what);
+    if (!std::isfinite(length_penalty)) return fail(1, "%s: length_penalty %g is not finite", what, length_penalty);
+    if (n_groups > m->max_gpt) return fail(1, "%s: %llu groups > max_gpt %llu", what, n_groups, m->max_gpt);
+    const size_t V = binfmt::kVocab;
+    const unsigned long long G = n_groups, B = beams, K = n_best, N = max_new, C = B + n_stop;
+    std::vector<char> used(m->max_gpt, 0);
+    for (unsigned long long i = 0; i < G * B; ++i) {
+        if ((rc = check_slot(m, what, slots[i]))) return rc;
+        if (used[slots[i]]) return fail(1, "%s: slot %llu appears twice", what, slots[i]);
+        used[slots[i]] = 1;
+    }
+    for (unsigned long long i = 0; i < G; ++i)
+        if (first_tokens[i] >= V) return fail(1, "%s: first token %llu of group %llu out of range", what, first_tokens[i], i);
+    for (unsigned long long i = 0; i < n_stop; ++i)
+        if (stop_tokens[i] >= V) return fail(1, "%s: stop token %llu out of range", what, stop_tokens[i]);
+    // the length penalties on the host, with the C library's pow: a host restatement gets the same bits
+    if (N > ((unsigned long long)SIZE_MAX / sizeof(rk::BeamBack)) / (G * B))
+        return fail(1, "%s: max_new = %llu: the backpointers of %llu beams do not fit in memory", what, N, G * B);
+    std::vector<double> P;
+    try {
+        P.assign(N + 1, 0.0);
+    } catch (const std::exception &) {
+        return fail(9, "%s: out of host memory for max_new = %llu", what, N);
+    }
+    for (unsigned long long n = 1; n <= N; ++n) P[n] = pow((double)n, length_penalty);
+    CK(cudaSetDevice(m->device));
+    auto &g = m->gen;
+    auto &bm = m->beam;
+    if ((rc = grow(&g.stop, g.stop_cap, (size_t)n_stop)) || (rc = grow(&bm.row0, bm.row0_cap, (size_t)G)) ||
+        (rc = grow(&bm.groups, bm.groups_cap, (size_t)G)) || (rc = grow(&bm.cand_tok, bm.cand_tok_cap, (size_t)(G * B * C))) ||
+        (rc = grow(&bm.cand_lp, bm.cand_lp_cap, (size_t)(G * B * C))) || (rc = grow(&bm.cum, bm.cum_cap, (size_t)(G * B))) ||
+        (rc = grow(&bm.P, bm.P_cap, (size_t)(N + 1))) || (rc = grow(&bm.back, bm.back_cap, (size_t)(G * N * B))) ||
+        (rc = grow(&bm.hyp, bm.hyp_cap, (size_t)(G * K))) || (rc = grow(&bm.n_hyp, bm.n_hyp_cap, (size_t)G)) ||
+        (rc = grow(&bm.done, bm.done_cap, (size_t)G)) || (rc = grow(&bm.forks, bm.forks_cap, (size_t)(2 * G * B))))
+        return rc;
+    // the path is chosen once, by forward_streams' rule for G x B one-token streams
+    const bool tc = G * B >= (unsigned long long)m->pf.min_tokens && rk::prefill_enabled(m->pf);
+    if (tc && (rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
+    m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
+
+    rk::GenStream *hg = g.h_gs;
+    for (unsigned long long s = 0; s < G * B; ++s) hg[s] = rk::GenStream{slots[s], N, s % B == 0 ? first_tokens[s / B] : 0, 0, 0};
+    std::vector<int> row0(G), live(G);
+    for (unsigned long long i = 0; i < G; ++i) {
+        row0[i] = (int)(i * B);
+        live[i] = (int)i;
+    }
+    CK(cudaMemcpyAsync(g.gs, hg, G * B * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemcpyAsync(bm.row0, row0.data(), G * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemcpyAsync(bm.P, P.data(), (N + 1) * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+    if (n_stop) CK(cudaMemcpyAsync(g.stop, stop_tokens, n_stop * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemsetAsync(bm.cum, 0, G * B * sizeof(double), m->stream));
+    CK(cudaMemsetAsync(bm.n_hyp, 0, G * sizeof(int), m->stream));
+    CK(cudaMemsetAsync(bm.done, 0, G * sizeof(unsigned long long), m->stream));
+    double *arr[5];
+    slot_arrays(m, 0, arr);
+    const size_t slot_len = (size_t)(m->L * m->E);
+    const unsigned chunks = (unsigned)((slot_len + rk::kForkChunk - 1) / rk::kForkChunk);
+    std::vector<unsigned long long> hdone(G, 0);
+    std::vector<int> rs;
+    std::vector<rk::PassDesc> passes;
+    for (unsigned long long step = 0; !live.empty() && step < N;) {
+        // a host group: the live groups' beams are rows gi * B + j (step 0: row gi); their inputs go up once
+        const int Gl = (int)live.size();
+        const unsigned long long steps = std::min(kGenGroup, N - step);
+        rs.resize((size_t)Gl * B);
+        for (int gi = 0; gi < Gl; ++gi)
+            for (unsigned long long j = 0; j < B; ++j) rs[gi * B + j] = (int)(live[gi] * B + j);
+        CK(cudaMemcpyAsync(g.row_stream, rs.data(), rs.size() * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(bm.groups, live.data(), Gl * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        if (tc) {
+            const int rows = step == 0 ? Gl : Gl * (int)B;
+            passes.assign((size_t)(rows + rk::kPfMaxTokens - 1) / rk::kPfMaxTokens, rk::PassDesc{});
+            for (int r = 0; r < rows; ++r) {
+                const rk::GenStream &bs = hg[step == 0 ? row0[r] : rs[r]];
+                rk::PassDesc &pd = passes[r / rk::kPfMaxTokens];
+                const int t = r % rk::kPfMaxTokens;
+                pd.tokens[t] = bs.tok;
+                pd.desc[t] = (uint32_t)bs.slot | rk::kDescFirst | rk::kDescLast;
+                pd.rows[t] = t;
+                pd.out_row0 = (r / rk::kPfMaxTokens) * rk::kPfMaxTokens;
+            }
+            CK(cudaMemcpyAsync(g.passes, passes.data(), passes.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
+        }
+        rk::BeamArgs ba{g.gs, bm.cum, bm.groups, bm.cand_tok, bm.cand_lp, (int)C, (int)B, (int)K, 0, 0, N, bm.P,
+                        length_penalty < 0.0 ? 1 : 0, g.stop, (int)n_stop, bm.back, bm.hyp, bm.n_hyp, bm.done, bm.forks,
+                        tc ? g.passes : nullptr};
+        for (unsigned long long k = 0; k < steps; ++k) {
+            const unsigned long long st = step + k;
+            const int nb = st == 0 ? 1 : (int)B, rows = Gl * nb;
+            const int *rmap = st == 0 ? bm.row0 : g.row_stream;
+            if ((rc = tc ? gen_step_passes(m, rows) : gen_step_decode(m, rows, rmap))) return rc;
+            rk::k_beam_expand<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs, rmap, (int)C,
+                                                                                bm.cand_tok, bm.cand_lp);
+            CK(cudaGetLastError());
+            ba.step = (int)st;
+            ba.nb = nb;
+            rk::k_beam_select<<<(unsigned)Gl, rk::kBeamSelectThreads, 0, m->stream>>>(ba);
+            CK(cudaGetLastError());
+            m->launches += 2;
+            if (st + 1 < N) { // after the last step every group is done and forks nothing
+                rk::k_beam_fork<<<dim3((unsigned)(Gl * B), chunks, 5), rk::kForkThreads, 0, m->stream>>>(
+                    bm.forks, arr[0], arr[1], arr[2], arr[3], arr[4], slot_len);
+                CK(cudaGetLastError());
+                m->launches += 1;
+            }
+        }
+        // the end of a host group: which groups are done and the beams' records (one synchronisation)
+        CK(cudaMemcpyAsync(hdone.data(), bm.done, G * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(hg, g.gs, G * B * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
+        SYNC(m);
+        step += steps;
+        live.erase(std::remove_if(live.begin(), live.end(), [&](int gg) { return hdone[gg] != 0; }), live.end());
+    }
+    std::vector<rk::BeamHyp> hyp(G * K);
+    std::vector<rk::BeamBack> back(G * N * B);
+    CK(cudaMemcpyAsync(hyp.data(), bm.hyp, G * K * sizeof(rk::BeamHyp), cudaMemcpyDeviceToHost, m->stream));
+    CK(cudaMemcpyAsync(back.data(), bm.back, G * N * B * sizeof(rk::BeamBack), cudaMemcpyDeviceToHost, m->stream));
+    SYNC(m);
+    // each hypothesis' tokens: its last token, then the backpointers of its beam from its step down to step 0
+    const double nan = std::nan("");
+    for (unsigned long long gg = 0; gg < G; ++gg)
+        for (unsigned long long i = 0; i < K; ++i) {
+            const rk::BeamHyp &h = hyp[gg * K + i];
+            const size_t o = (size_t)(gg * K + i);
+            unsigned long long *tok = tokens_out + o * N;
+            double *tlp = token_logprobs_out ? token_logprobs_out + o * N : nullptr;
+            for (unsigned long long t = 0; t < N; ++t) {
+                tok[t] = 0;
+                if (tlp) tlp[t] = nan;
+            }
+            tok[h.step] = h.tok;
+            if (tlp) tlp[h.step] = h.lp;
+            for (int s = h.step - 1, p = h.parent; s >= 0; --s) {
+                const rk::BeamBack &bk = back[(gg * N + (unsigned long long)s) * B + (unsigned long long)p];
+                tok[s] = bk.tok;
+                if (tlp) tlp[s] = bk.lp;
+                p = bk.parent;
+            }
+            lengths_out[o] = (unsigned long long)h.len;
+            logprobs_out[o] = h.cum;
+            scores_out[o] = h.score;
+            finished_out[o] = (unsigned char)h.finished;
+        }
     return 0;
 }
 
@@ -1039,7 +1220,10 @@ void rwkv_b200_free(rwkv_b200_model *m) {
                     (void *)m->gen.samp, (void *)m->gen.pen_cnt, (void *)m->gen.pen_seen, (void *)m->score.rows,
                     (void *)m->score.tgt, (void *)m->score.rank, (void *)m->score.top_tok, (void *)m->score.lp,
                     (void *)m->score.top_lp, (void *)m->gen.lp, (void *)m->gen.top_lp, (void *)m->gen.rank,
-                    (void *)m->gen.top_tok, (void *)m->gen.raw, (void *)m->gen.gc, (void *)m->gen.fault})
+                    (void *)m->gen.top_tok, (void *)m->gen.raw, (void *)m->gen.gc, (void *)m->gen.fault,
+                    (void *)m->beam.row0, (void *)m->beam.groups, (void *)m->beam.cand_tok, (void *)m->beam.cand_lp,
+                    (void *)m->beam.cum, (void *)m->beam.P, (void *)m->beam.back, (void *)m->beam.hyp,
+                    (void *)m->beam.n_hyp, (void *)m->beam.done, (void *)m->beam.forks})
         if (p) cudaFree(p);
     for (auto &kv : m->automata) cudaFree(kv.second.dev);
     if (m->stream) cudaStreamDestroy(m->stream);
@@ -1393,6 +1577,16 @@ int rwkv_b200_generate_streams_constrained(rwkv_b200_model *m, const unsigned lo
     return generate(m, "generate_streams_constrained", true, slots, first_tokens, n_streams, max_new, budgets, stop_tokens,
                     n_stop, override_tokens, override_values, n_override, 1.0f, samplers, samplers ? u : nullptr, tokens_out,
                     lengths_out, logprobs_out ? &lpq : nullptr, &cq);
+}
+
+int rwkv_b200_beam_search(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
+                          unsigned long long n_groups, unsigned beams, unsigned long long max_new,
+                          const unsigned long long *stop_tokens, unsigned long long n_stop, double length_penalty,
+                          unsigned n_best, unsigned long long *tokens_out, unsigned long long *lengths_out,
+                          double *logprobs_out, double *scores_out, unsigned char *finished_out,
+                          double *token_logprobs_out) {
+    return beam(m, slots, first_tokens, n_groups, beams, max_new, stop_tokens, n_stop, length_penalty, n_best, tokens_out,
+                lengths_out, logprobs_out, scores_out, finished_out, token_logprobs_out);
 }
 
 int rwkv_b200_sample_streams(rwkv_b200_model *m, unsigned long long n_streams, const rwkv_b200_sampler *params, const double *u,

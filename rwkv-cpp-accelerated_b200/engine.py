@@ -130,6 +130,8 @@ def load_library():
         "rwkv_b200_generate_streams_constrained": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull,
                                                          c.POINTER(Sampler), pdbl, pull, pull, i32, c.c_uint, pdbl, pull,
                                                          pull, pdbl, pull, pull, pull]),
+        "rwkv_b200_beam_search": (i32, [vp, pull, pull, ull, c.c_uint, ull, pull, ull, c.c_double, c.c_uint, pull, pull, pdbl,
+                                        pdbl, c.POINTER(c.c_ubyte), pdbl]),
         "rwkv_b200_slot_zero": (i32, [vp, ull]),
         "rwkv_b200_slot_copy": (i32, [vp, ull, ull]),
         "rwkv_b200_slot_upload": (i32, [vp, ull, pdbl, pdbl, pdbl, pdbl, pdbl]),
@@ -433,6 +435,45 @@ class Engine:
             out.append(d)
             t0 += len(t)
         return out
+
+    def beam_search(self, groups, max_new, beams, stop=(), length_penalty=1.0, n_best=1, token_logprobs=False):
+        """Beam search on the device (rwkv_b200_beam_search): groups = [(slots, first_token), ...], each with `beams`
+        distinct slots, the first holding the prompt state (the others are overwritten). stop: token ids that finish a
+        hypothesis; length_penalty: alpha of score = logprob / len ** alpha. Returns per group its n_best hypotheses,
+        best first, each a dict of "tokens" (uint64), "logprob" (the sum of the token logprobs), "score", "finished"
+        (ended by a stop token), and with token_logprobs=True "token_logprobs" (float64, one per token)."""
+        G = len(groups)
+        flat = [int(s) for slots, _ in groups for s in slots]
+        if any(len(slots) != beams for slots, _ in groups):
+            raise EngineError("beam_search: every group needs %d slots" % beams)
+        slots = np.ascontiguousarray(flat, dtype=np.uint64)
+        first = np.ascontiguousarray([int(t) for _, t in groups], dtype=np.uint64)
+        stops = np.ascontiguousarray(list(stop), dtype=np.uint64)
+        K = max(int(n_best), 1)
+        toks = np.zeros((G, K, max_new), np.uint64)
+        lens = np.zeros((G, K), np.uint64)
+        lp = np.zeros((G, K), np.float64)
+        scores = np.zeros((G, K), np.float64)
+        fin = np.zeros((G, K), np.uint8)
+        tlp = np.zeros((G, K, max_new), np.float64) if token_logprobs else None
+        P = ctypes.c_ulonglong
+        self._ck(self.lib.rwkv_b200_beam_search(self.h, _ptr(slots, P), _ptr(first, P), G, int(beams), int(max_new),
+                                                _ptr(stops, P), len(stops), float(length_penalty), int(n_best),
+                                                _ptr(toks, P), _ptr(lens, P), _ptr(lp, ctypes.c_double),
+                                                _ptr(scores, ctypes.c_double), _ptr(fin, ctypes.c_ubyte),
+                                                _ptr(tlp, ctypes.c_double)), "beam_search")
+        res = []
+        for g in range(G):
+            hyps = []
+            for i in range(K):
+                n = int(lens[g, i])
+                d = {"tokens": toks[g, i, :n].copy(), "logprob": float(lp[g, i]), "score": float(scores[g, i]),
+                     "finished": bool(fin[g, i])}
+                if token_logprobs:
+                    d["token_logprobs"] = tlp[g, i, :n].copy()
+                hyps.append(d)
+            res.append(hyps)
+        return res
 
     def slot_zero(self, slot):
         self._ck(self.lib.rwkv_b200_slot_zero(self.h, slot), "slot_zero")
