@@ -63,6 +63,31 @@ int fail(int code, const char *fmt, ...) {
                         __FILE__, __LINE__);                                                       \
     } while (0)
 
+// A device buffer that grows with the largest call and is freed with its owner (a failed free is ignored). grow() is
+// called between calls, never with work in flight on the buffer: it never shrinks, frees the old block before
+// allocating, and leaves cap 0 when the allocation fails.
+template <class T> struct DevBuf {
+    T *p = nullptr;
+    size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(DevBuf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr, o.cap = 0; }
+    DevBuf(const DevBuf &) = delete;
+    DevBuf &operator=(const DevBuf &) = delete;
+    ~DevBuf() { release(); }
+    void release() {
+        if (p) cudaFree(p);
+        p = nullptr;
+        cap = 0;
+    }
+    int grow(size_t n) {
+        if (n <= cap) return 0;
+        release();
+        CK(cudaMalloc((void **)&p, n * sizeof(T)));
+        cap = n;
+        return 0;
+    }
+};
+
 const char *kKernelNames[1] = {"token"};
 
 } // namespace
@@ -102,54 +127,48 @@ struct rwkv_b200_model {
         rk::GenStream *gs = nullptr, *h_gs = nullptr; // [max_gpt]
         int *row_stream = nullptr;                     // [max_gpt] stream of each row of the current group
         rk::PassDesc *passes = nullptr;                // [ceil(max_gpt / 128)] next step's passes (tensor cores)
-        unsigned long long *out = nullptr;             // [n_streams][max_new] emitted tokens
-        unsigned long long *stop = nullptr, *ovr_tok = nullptr;
-        float *ovr_val = nullptr;
-        double *u = nullptr; // [group steps][rows] uniforms of the current group
-        rwkv_b200_sampler *samp = nullptr; // [n_streams] sampler of each stream (generate_streams_ex, sample_streams)
-        float *pen_cnt = nullptr;          // [n_streams][V] decayed counts of the emitted tokens (penalties only)
-        unsigned char *pen_seen = nullptr; // [n_streams][V] emitted in this call
-        size_t out_cap = 0, stop_cap = 0, ovr_cap = 0, ovr_val_cap = 0, u_cap = 0, samp_cap = 0, pen_cap = 0, seen_cap = 0;
+        DevBuf<unsigned long long> out;                // [n_streams][max_new] emitted tokens
+        DevBuf<unsigned long long> stop, ovr_tok;
+        DevBuf<float> ovr_val;
+        DevBuf<double> u;               // [group steps][rows] uniforms of the current group
+        DevBuf<rwkv_b200_sampler> samp; // [n_streams] sampler of each stream (generate_streams_ex, sample_streams)
+        DevBuf<float> pen_cnt;          // [n_streams][V] decayed counts of the emitted tokens (penalties only)
+        DevBuf<unsigned char> pen_seen; // [n_streams][V] emitted in this call
         // generate_streams_logprobs: the results of each emitted token, and the model's rows of the step (raw mode with
         // penalties or overrides, which edit d_slogits in place)
-        double *lp = nullptr, *top_lp = nullptr;                    // [n_streams][max_new], [..][top_n]
-        unsigned long long *rank = nullptr, *top_tok = nullptr;     // [n_streams][max_new], [..][top_n]
-        float *raw = nullptr;                                       // [rows][V]
-        size_t lp_cap = 0, top_lp_cap = 0, rank_cap = 0, top_tok_cap = 0, raw_cap = 0;
+        DevBuf<double> lp, top_lp;                 // [n_streams][max_new], [..][top_n]
+        DevBuf<unsigned long long> rank, top_tok;  // [n_streams][max_new], [..][top_n]
+        DevBuf<float> raw;                         // [rows][V]
         // generate_streams_constrained: each stream's automaton and state, and the record of a token without an edge
-        rk::GenConstraint *gc = nullptr;  // [n_streams]
-        unsigned long long *fault = nullptr; // [3]
-        size_t gc_cap = 0, fault_cap = 0;
+        DevBuf<rk::GenConstraint> gc;      // [n_streams]
+        DevBuf<unsigned long long> fault;  // [3]
     } gen;
     // rwkv_b200_constraint_add: per id, the CSR on the host (the override check of a call) and one device block holding
     // the allow masks, then edge_start, the edge tokens and their targets
     struct Automaton {
         std::vector<unsigned long long> start; // [n_states + 1]
         std::vector<uint32_t> tok;             // [n_edges]
-        void *dev = nullptr;
+        DevBuf<unsigned char> dev;
         rk::GenConstraint view; // device pointers into dev, state 0
     };
     std::map<unsigned long long, Automaton> automata;
     unsigned long long next_automaton = 1;
     // score_streams: per scored row its d_slogits row and target in, its results out; grown with the largest call
     struct Score {
-        int *rows = nullptr;
-        unsigned long long *tgt = nullptr, *rank = nullptr, *top_tok = nullptr;
-        double *lp = nullptr, *top_lp = nullptr;
-        size_t rows_cap = 0, tgt_cap = 0, rank_cap = 0, top_tok_cap = 0, lp_cap = 0, top_lp_cap = 0;
+        DevBuf<int> rows;
+        DevBuf<unsigned long long> tgt, rank, top_tok;
+        DevBuf<double> lp, top_lp;
     } score;
     // beam_search: the beams' records live in gen.gs (beam j of group g is record g * B + j); the rest grows with the
     // largest call
     struct Beam {
-        int *row0 = nullptr, *groups = nullptr;          // [G] step 0's row map, [G] the live groups of a host group
-        unsigned long long *cand_tok = nullptr;          // [rows][C]
-        double *cand_lp = nullptr, *cum = nullptr, *P = nullptr; // [rows][C], [G * B], [N + 1]
-        rk::BeamBack *back = nullptr;                    // [G][N][B]
-        rk::BeamHyp *hyp = nullptr;                      // [G][K]
-        int *n_hyp = nullptr;                            // [G]
-        unsigned long long *done = nullptr, *forks = nullptr; // [G], [G * B][2]
-        size_t row0_cap = 0, groups_cap = 0, cand_tok_cap = 0, cand_lp_cap = 0, cum_cap = 0, P_cap = 0, back_cap = 0,
-               hyp_cap = 0, n_hyp_cap = 0, done_cap = 0, forks_cap = 0;
+        DevBuf<int> row0, groups;               // [G] step 0's row map, [G] the live groups of a host group
+        DevBuf<unsigned long long> cand_tok;    // [rows][C]
+        DevBuf<double> cand_lp, cum, P;         // [rows][C], [G * B], [N + 1]
+        DevBuf<rk::BeamBack> back;              // [G][N][B]
+        DevBuf<rk::BeamHyp> hyp;                // [G][K]
+        DevBuf<int> n_hyp;                      // [G]
+        DevBuf<unsigned long long> done, forks; // [G], [G * B][2]
     } beam;
 };
 
@@ -618,6 +637,28 @@ int check_slot(M *m, const char *what, unsigned long long slot) {
     return 0;
 }
 
+// n slots, each a slot of the model, none twice.
+int check_slots(M *m, const char *what, const unsigned long long *slots, unsigned long long n) {
+    std::vector<char> used(m->max_gpt, 0);
+    for (unsigned long long i = 0; i < n; ++i) {
+        if (int rc = check_slot(m, what, slots[i])) return rc;
+        if (used[slots[i]]) return fail(1, "%s: slot %llu appears twice", what, slots[i]);
+        used[slots[i]] = 1;
+    }
+    return 0;
+}
+
+// n token ids, each in the vocabulary; `of` names what index i counts ("first token 7 of stream 2").
+int check_tokens(const char *what, const char *name, const unsigned long long *tokens, unsigned long long n,
+                 const char *of = nullptr) {
+    for (unsigned long long i = 0; i < n; ++i) {
+        if (tokens[i] < binfmt::kVocab) continue;
+        if (of) return fail(1, "%s: %s %llu of %s %llu out of range", what, name, tokens[i], of, i);
+        return fail(1, "%s: %s %llu out of range", what, name, tokens[i]);
+    }
+    return 0;
+}
+
 // The model and the ragged token list of forward_streams and score_streams.
 int check_ragged(M *m, const char *what, const unsigned long long *tokens, unsigned long long n_tokens,
                  const unsigned long long *slots, const unsigned long long *lengths, unsigned long long n_streams) {
@@ -626,14 +667,9 @@ int check_ragged(M *m, const char *what, const unsigned long long *tokens, unsig
     if (!tokens || !slots || !lengths || n_tokens == 0 || n_streams == 0) return fail(1, "%s: no tokens or no streams", what);
     if (n_tokens > m->max_gpt) return fail(1, "%s: %llu tokens > max_gpt %llu", what, n_tokens, m->max_gpt);
     if (n_streams > n_tokens) return fail(1, "%s: %llu streams for %llu tokens", what, n_streams, n_tokens);
-    for (unsigned long long t = 0; t < n_tokens; ++t)
-        if (tokens[t] >= binfmt::kVocab) return fail(1, "%s: token id %llu out of range", what, tokens[t]);
-    std::vector<char> used(m->max_gpt, 0);
+    if ((rc = check_tokens(what, "token id", tokens, n_tokens)) || (rc = check_slots(m, what, slots, n_streams))) return rc;
     unsigned long long total = 0;
     for (unsigned long long i = 0; i < n_streams; ++i) {
-        if ((rc = check_slot(m, what, slots[i]))) return rc;
-        if (used[slots[i]]) return fail(1, "%s: slot %llu appears twice", what, slots[i]);
-        used[slots[i]] = 1;
         if (lengths[i] == 0 || lengths[i] > n_tokens) return fail(1, "%s: stream %llu has length %llu", what, i, lengths[i]);
         total += lengths[i];
     }
@@ -641,14 +677,41 @@ int check_ragged(M *m, const char *what, const unsigned long long *tokens, unsig
     return 0;
 }
 
-// A grow-only device buffer of at least `count` elements (called between calls, never with work in flight on it).
-template <class T> int grow(T **buf, size_t &cap, size_t count) {
-    if (count <= cap) return 0;
-    if (*buf) cudaFree(*buf);
-    *buf = nullptr;
-    cap = 0;
-    CK(cudaMalloc((void **)buf, count * sizeof(T)));
-    cap = count;
+// Tensor cores or the decode kernel for a forward of n tokens: forward_streams' rule, which every call that has a
+// choice follows (the multi-stream calls refuse tensor parallelism).
+bool tensor_cores(const M *m, unsigned long long n) {
+    return n >= (unsigned long long)m->pf.min_tokens && m->tp_size == 1 && rk::prefill_enabled(m->pf);
+}
+
+// Token by token through the decode kernel: stream i's lengths[i] tokens (stream-major) on slot slots[i]. Token t gets
+// its own pinned control record (the source of a copy still in flight when the next token is queued). Its logits are
+// copied (`kind`) to row(t, i, last) unless that is NULL; `last`: t is stream i's final token.
+template <class Row>
+int decode_tokens(M *m, const unsigned long long *tokens, const unsigned long long *slots, const unsigned long long *lengths,
+                  unsigned long long n_streams, cudaMemcpyKind kind, Row row) {
+    const size_t V = binfmt::kVocab;
+    for (unsigned long long i = 0, t = 0; i < n_streams; ++i)
+        for (unsigned long long k = 0; k < lengths[i]; ++k, ++t) {
+            rk::Ctrl &c = m->h_ctrl[t];
+            c.token = tokens[t];
+            c.next = 0;
+            c.slot = slots[i];
+            c.pos = 0;
+            CK(cudaMemcpyAsync(m->p.ctrl, &c, sizeof(rk::Ctrl), cudaMemcpyHostToDevice, m->stream));
+            if (int rc = launch_token(m, 0, false, nullptr, m->stream)) return rc;
+            if (float *dst = row(t, i, k + 1 == lengths[i])) CK(cudaMemcpyAsync(dst, dev_logits(m), V * sizeof(float), kind, m->stream));
+        }
+    return 0;
+}
+
+// The device sampler's picks {token, margin} of rows 0..n-1, read back with one synchronisation.
+int read_samples(M *m, unsigned long long n, unsigned long long *tokens_out, double *margins_out) {
+    CK(cudaMemcpyAsync(m->h_sample, m->d_sample, 2 * n * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+    SYNC(m);
+    for (unsigned long long i = 0; i < n; ++i) {
+        tokens_out[i] = (unsigned long long)m->h_sample[2 * i];
+        if (margins_out) margins_out[i] = m->h_sample[2 * i + 1];
+    }
     return 0;
 }
 
@@ -684,6 +747,21 @@ int gen_step_passes(M *m, int rows) {
         if (rc) return fail(rc, "%s", rk::prefill_error());
     }
     m->launches += rk::prefill_launches(m->pf);
+    return 0;
+}
+
+// The passes of a step of `rows` one-token streams, row r on stream record rec[r] (its input token and slot), each row a
+// head row: pass_layout's passes, uploaded to gen.passes in one copy.
+int upload_step_passes(M *m, const int *rec, int rows) {
+    std::vector<unsigned long long> tokens(rows), slots(rows), lens(rows, 1);
+    for (int r = 0; r < rows; ++r) {
+        tokens[r] = m->gen.h_gs[rec[r]].tok;
+        slots[r] = m->gen.h_gs[rec[r]].slot;
+    }
+    std::vector<rk::PassDesc> passes;
+    std::vector<int> heads;
+    rk::pass_layout(tokens.data(), rows, slots.data(), lens.data(), 2, nullptr, passes, heads);
+    CK(cudaMemcpyAsync(m->gen.passes, passes.data(), passes.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
     return 0;
 }
 
@@ -803,19 +881,14 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
         return fail(1, "%s: n_override = %llu with NULL override_tokens or override_values", what, n_override);
     if (max_new == 0) return fail(1, "%s: max_new is 0", what);
     const size_t V = binfmt::kVocab;
-    std::vector<char> used(m->max_gpt, 0);
-    for (unsigned long long i = 0; i < n_streams; ++i) {
-        if ((rc = check_slot(m, what, slots[i]))) return rc;
-        if (used[slots[i]]) return fail(1, "%s: slot %llu appears twice", what, slots[i]);
-        used[slots[i]] = 1;
-        if (first_tokens[i] >= V) return fail(1, "%s: first token %llu of stream %llu out of range", what, first_tokens[i], i);
-        if (budgets && (budgets[i] == 0 || budgets[i] > max_new))
+    if ((rc = check_slots(m, what, slots, n_streams)) || (rc = check_tokens(what, "first token", first_tokens, n_streams, "stream")))
+        return rc;
+    for (unsigned long long i = 0; budgets && i < n_streams; ++i)
+        if (budgets[i] == 0 || budgets[i] > max_new)
             return fail(1, "%s: budget %llu of stream %llu is outside 1..max_new = %llu", what, budgets[i], i, max_new);
-    }
-    for (unsigned long long i = 0; i < n_stop; ++i)
-        if (stop_tokens[i] >= V) return fail(1, "%s: stop token %llu out of range", what, stop_tokens[i]);
-    for (unsigned long long i = 0; i < n_override; ++i)
-        if (override_tokens[i] >= V) return fail(1, "%s: override token %llu out of range", what, override_tokens[i]);
+    if ((rc = check_tokens(what, "stop token", stop_tokens, n_stop)) ||
+        (rc = check_tokens(what, "override token", override_tokens, n_override)))
+        return rc;
     bool pen = false; // some stream has a presence or frequency penalty
     if (ex) {
         if ((rc = check_overrides(what, override_tokens, override_values, n_override))) return rc;
@@ -834,56 +907,51 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
     const bool constrained = std::any_of(hgc.begin(), hgc.end(), [](const rk::GenConstraint &c) { return c.mask != nullptr; });
     CK(cudaSetDevice(m->device));
     auto &g = m->gen;
-    if (constrained && ((rc = grow(&g.gc, g.gc_cap, (size_t)n_streams)) || (rc = grow(&g.fault, g.fault_cap, (size_t)3))))
-        return rc;
-    if (samplers && (rc = grow(&g.samp, g.samp_cap, (size_t)n_streams))) return rc;
-    if (pen && ((rc = grow(&g.pen_cnt, g.pen_cap, (size_t)(n_streams * V))) || (rc = grow(&g.pen_seen, g.seen_cap, (size_t)(n_streams * V)))))
-        return rc;
-    if ((rc = grow(&g.out, g.out_cap, (size_t)(n_streams * max_new))) || (rc = grow(&g.stop, g.stop_cap, (size_t)n_stop)) ||
-        (rc = grow(&g.ovr_tok, g.ovr_cap, (size_t)n_override)) || (rc = grow(&g.ovr_val, g.ovr_val_cap, (size_t)n_override)) ||
-        (u && (rc = grow(&g.u, g.u_cap, (size_t)(kGenGroup * m->max_gpt)))))
+    if (constrained && ((rc = g.gc.grow(n_streams)) || (rc = g.fault.grow(3)))) return rc;
+    if (samplers && (rc = g.samp.grow(n_streams))) return rc;
+    if (pen && ((rc = g.pen_cnt.grow(n_streams * V)) || (rc = g.pen_seen.grow(n_streams * V)))) return rc;
+    if ((rc = g.out.grow(n_streams * max_new)) || (rc = g.stop.grow(n_stop)) || (rc = g.ovr_tok.grow(n_override)) ||
+        (rc = g.ovr_val.grow(n_override)) || (u && (rc = g.u.grow(kGenGroup * m->max_gpt))))
         return rc;
     // raw mode reads the model's rows: d_slogits itself, or a copy taken before the penalties, overrides and mask edit it
     const bool raw_copy = lpq && lpq->mode == RWKV_B200_LOGPROBS_RAW && (pen || n_override || constrained);
     const size_t n_lp = (size_t)(n_streams * max_new), n_top = lpq ? n_lp * lpq->top_n : 0;
-    if (lpq && ((rc = grow(&g.lp, g.lp_cap, n_lp)) || (rc = grow(&g.rank, g.rank_cap, n_lp)) ||
-                (rc = grow(&g.top_tok, g.top_tok_cap, n_top)) || (rc = grow(&g.top_lp, g.top_lp_cap, n_top)) ||
-                (raw_copy && (rc = grow(&g.raw, g.raw_cap, (size_t)n_streams * V)))))
+    if (lpq && ((rc = g.lp.grow(n_lp)) || (rc = g.rank.grow(n_lp)) || (rc = g.top_tok.grow(n_top)) || (rc = g.top_lp.grow(n_top)) ||
+                (raw_copy && (rc = g.raw.grow(n_streams * V)))))
         return rc;
-    // the path is chosen once, by forward_streams' rule for n_streams tokens; a stream's numbers depend only on its row
-    const bool tc = n_streams >= (unsigned long long)m->pf.min_tokens && rk::prefill_enabled(m->pf);
+    // the path is chosen once, for n_streams tokens; a stream's numbers depend only on its row
+    const bool tc = tensor_cores(m, n_streams);
     if (tc && (rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
     m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
 
     rk::GenStream *hg = g.h_gs;
     for (unsigned long long s = 0; s < n_streams; ++s) hg[s] = rk::GenStream{slots[s], budgets ? budgets[s] : max_new, first_tokens[s], 0, 0};
     CK(cudaMemcpyAsync(g.gs, hg, n_streams * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
-    CK(cudaMemsetAsync(g.out, 0, n_streams * max_new * sizeof(unsigned long long), m->stream));
-    if (n_stop) CK(cudaMemcpyAsync(g.stop, stop_tokens, n_stop * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemsetAsync(g.out.p, 0, n_streams * max_new * sizeof(unsigned long long), m->stream));
+    if (n_stop) CK(cudaMemcpyAsync(g.stop.p, stop_tokens, n_stop * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
     if (n_override) {
-        CK(cudaMemcpyAsync(g.ovr_tok, override_tokens, n_override * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(g.ovr_val, override_values, n_override * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(g.ovr_tok.p, override_tokens, n_override * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(g.ovr_val.p, override_values, n_override * sizeof(float), cudaMemcpyHostToDevice, m->stream));
     }
-    if (samplers) CK(cudaMemcpyAsync(g.samp, samplers, n_streams * sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
+    if (samplers) CK(cudaMemcpyAsync(g.samp.p, samplers, n_streams * sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
     if (constrained) {
-        CK(cudaMemcpyAsync(g.gc, hgc.data(), n_streams * sizeof(rk::GenConstraint), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemsetAsync(g.fault, 0, 3 * sizeof(unsigned long long), m->stream));
+        CK(cudaMemcpyAsync(g.gc.p, hgc.data(), n_streams * sizeof(rk::GenConstraint), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemsetAsync(g.fault.p, 0, 3 * sizeof(unsigned long long), m->stream));
     }
     if (pen) { // the history starts empty in every call: prompt tokens are not counted
-        CK(cudaMemsetAsync(g.pen_cnt, 0, n_streams * V * sizeof(float), m->stream));
-        CK(cudaMemsetAsync(g.pen_seen, 0, n_streams * V, m->stream));
+        CK(cudaMemsetAsync(g.pen_cnt.p, 0, n_streams * V * sizeof(float), m->stream));
+        CK(cudaMemsetAsync(g.pen_seen.p, 0, n_streams * V, m->stream));
     }
     if (lpq) { // all ones: NaN logprobs and RWKV_B200_NO_TARGET ranks and tokens wherever no token is emitted
-        CK(cudaMemsetAsync(g.lp, 0xFF, n_lp * sizeof(double), m->stream));
-        CK(cudaMemsetAsync(g.rank, 0xFF, n_lp * sizeof(unsigned long long), m->stream));
+        CK(cudaMemsetAsync(g.lp.p, 0xFF, n_lp * sizeof(double), m->stream));
+        CK(cudaMemsetAsync(g.rank.p, 0xFF, n_lp * sizeof(unsigned long long), m->stream));
         if (n_top) {
-            CK(cudaMemsetAsync(g.top_tok, 0xFF, n_top * sizeof(unsigned long long), m->stream));
-            CK(cudaMemsetAsync(g.top_lp, 0xFF, n_top * sizeof(double), m->stream));
+            CK(cudaMemsetAsync(g.top_tok.p, 0xFF, n_top * sizeof(unsigned long long), m->stream));
+            CK(cudaMemsetAsync(g.top_lp.p, 0xFF, n_top * sizeof(double), m->stream));
         }
     }
     std::vector<int> live(n_streams);
     for (unsigned long long s = 0; s < n_streams; ++s) live[s] = (int)s;
-    std::vector<rk::PassDesc> passes;
     std::vector<double> ug;
     const int exponent = sample_exponent(temp);
     for (unsigned long long step = 0; !live.empty() && step < max_new;) {
@@ -891,60 +959,49 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
         const int rows = (int)live.size();
         const unsigned long long steps = std::min(kGenGroup, max_new - step);
         CK(cudaMemcpyAsync(g.row_stream, live.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-        if (tc) {
-            passes.assign((size_t)(rows + rk::kPfMaxTokens - 1) / rk::kPfMaxTokens, rk::PassDesc{});
-            for (int r = 0; r < rows; ++r) {
-                rk::PassDesc &pd = passes[r / rk::kPfMaxTokens];
-                const int t = r % rk::kPfMaxTokens;
-                pd.tokens[t] = hg[live[r]].tok;
-                pd.desc[t] = (uint32_t)hg[live[r]].slot | rk::kDescFirst | rk::kDescLast;
-                pd.rows[t] = t;
-                pd.out_row0 = (r / rk::kPfMaxTokens) * rk::kPfMaxTokens;
-            }
-            CK(cudaMemcpyAsync(g.passes, passes.data(), passes.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
-        }
+        if (tc && (rc = upload_step_passes(m, live.data(), rows))) return rc;
         if (u) {
             ug.resize((size_t)steps * rows);
             for (unsigned long long k = 0; k < steps; ++k)
                 for (int r = 0; r < rows; ++r) ug[k * rows + r] = u[(step + k) * n_streams + live[r]];
-            CK(cudaMemcpyAsync(g.u, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+            CK(cudaMemcpyAsync(g.u.p, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
         }
-        rk::GenFeedbackArgs fb{g.gs, g.row_stream, rows, u || samplers ? nullptr : m->d_next, m->d_sample, g.stop, (int)n_stop, g.out, max_new,
-                               tc ? g.passes : nullptr, constrained ? g.gc : nullptr, g.fault};
+        rk::GenFeedbackArgs fb{g.gs, g.row_stream, rows, u || samplers ? nullptr : m->d_next, m->d_sample, g.stop.p, (int)n_stop, g.out.p,
+                               max_new, tc ? g.passes : nullptr, constrained ? g.gc.p : nullptr, g.fault.p};
         rk::GenLogprobArgs la{};
         if (lpq)
-            la = rk::GenLogprobArgs{raw_copy ? g.raw : m->d_slogits, (int)V, g.gs, g.row_stream, fb.next, m->d_sample,
-                                    lpq->mode == RWKV_B200_LOGPROBS_PROCESSED ? samplers ? g.samp : nullptr : nullptr,
-                                    (int)lpq->top_n, max_new, g.lp, g.rank, g.top_tok, g.top_lp};
+            la = rk::GenLogprobArgs{raw_copy ? g.raw.p : m->d_slogits, (int)V, g.gs, g.row_stream, fb.next, m->d_sample,
+                                    lpq->mode == RWKV_B200_LOGPROBS_PROCESSED ? samplers ? g.samp.p : nullptr : nullptr,
+                                    (int)lpq->top_n, max_new, g.lp.p, g.rank.p, g.top_tok.p, g.top_lp.p};
         const unsigned rb = (unsigned)((rows + 127) / 128);
         for (unsigned long long k = 0; k < steps; ++k) {
             if ((rc = tc ? gen_step_passes(m, rows) : gen_step_decode(m, rows, g.row_stream))) return rc;
             if (raw_copy)
-                CK(cudaMemcpyAsync(g.raw, m->d_slogits, (size_t)rows * V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
+                CK(cudaMemcpyAsync(g.raw.p, m->d_slogits, (size_t)rows * V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
             if (pen) {
                 const dim3 grid((unsigned)((V + rk::kPenaltyThreads - 1) / rk::kPenaltyThreads), (unsigned)rows);
-                rk::k_gen_penalty<<<grid, rk::kPenaltyThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs, g.row_stream, g.samp,
-                                                                              g.pen_cnt, g.pen_seen);
+                rk::k_gen_penalty<<<grid, rk::kPenaltyThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs, g.row_stream, g.samp.p,
+                                                                              g.pen_cnt.p, g.pen_seen.p);
                 CK(cudaGetLastError());
                 m->launches += 1;
             }
             if (n_override) {
-                rk::k_gen_override<<<rb, 128, 0, m->stream>>>(m->d_slogits, (int)V, rows, g.ovr_tok, g.ovr_val, (int)n_override);
+                rk::k_gen_override<<<rb, 128, 0, m->stream>>>(m->d_slogits, (int)V, rows, g.ovr_tok.p, g.ovr_val.p, (int)n_override);
                 CK(cudaGetLastError());
                 m->launches += 1;
             }
             if (constrained) {
                 const dim3 grid((unsigned)((V + rk::kMaskThreads - 1) / rk::kMaskThreads), (unsigned)rows);
-                rk::k_gen_mask<<<grid, rk::kMaskThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs, g.row_stream, g.gc);
+                rk::k_gen_mask<<<grid, rk::kMaskThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs, g.row_stream, g.gc.p);
                 CK(cudaGetLastError());
                 m->launches += 1;
             }
             if (samplers)
-                rk::k_sample_nucleus<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.samp, g.row_stream,
-                                                                                       u ? g.u + k * rows : nullptr, m->d_sample);
+                rk::k_sample_nucleus<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.samp.p, g.row_stream,
+                                                                                       u ? g.u.p + k * rows : nullptr, m->d_sample);
             else if (u)
-                rk::k_sample_typical<<<(unsigned)rows, rk::kSampleThreads, 0, m->stream>>>(m->d_slogits, V, (int)V, exponent, g.u + k * rows,
-                                                                                          m->d_sample);
+                rk::k_sample_typical<<<(unsigned)rows, rk::kSampleThreads, 0, m->stream>>>(m->d_slogits, V, (int)V, exponent,
+                                                                                          g.u.p + k * rows, m->d_sample);
             else
                 rk::k_argmax_rows<<<(unsigned)rows, rk::kArgmaxThreads, 0, m->stream>>>(m->d_slogits, (int)V, m->d_next);
             CK(cudaGetLastError());
@@ -960,7 +1017,7 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
         // the end of a group: which streams are done (a few bytes, one synchronisation); drop them from the rows
         CK(cudaMemcpyAsync(hg, g.gs, n_streams * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
         unsigned long long fault[3] = {0, 0, 0};
-        if (constrained) CK(cudaMemcpyAsync(fault, g.fault, sizeof(fault), cudaMemcpyDeviceToHost, m->stream));
+        if (constrained) CK(cudaMemcpyAsync(fault, g.fault.p, sizeof(fault), cudaMemcpyDeviceToHost, m->stream));
         SYNC(m);
         if (fault[0])
             return fail(8, "%s: stream %llu emitted token %llu, which has no edge out of state %llu of its constraint", what,
@@ -968,17 +1025,17 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
         step += steps;
         live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hg[s].done != 0; }), live.end());
     }
-    CK(cudaMemcpyAsync(tokens_out, g.out, n_streams * max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+    CK(cudaMemcpyAsync(tokens_out, g.out.p, n_streams * max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
     if (lpq) {
-        CK(cudaMemcpyAsync(lpq->logprobs_out, g.lp, n_lp * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
-        if (lpq->ranks_out) CK(cudaMemcpyAsync(lpq->ranks_out, g.rank, n_lp * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(lpq->logprobs_out, g.lp.p, n_lp * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+        if (lpq->ranks_out) CK(cudaMemcpyAsync(lpq->ranks_out, g.rank.p, n_lp * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
         if (n_top) {
-            CK(cudaMemcpyAsync(lpq->top_tokens_out, g.top_tok, n_top * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
-            CK(cudaMemcpyAsync(lpq->top_logprobs_out, g.top_lp, n_top * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+            CK(cudaMemcpyAsync(lpq->top_tokens_out, g.top_tok.p, n_top * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+            CK(cudaMemcpyAsync(lpq->top_logprobs_out, g.top_lp.p, n_top * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
         }
     }
     if (constrained && cq->states_out)
-        CK(cudaMemcpyAsync(hgc.data(), g.gc, n_streams * sizeof(rk::GenConstraint), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(hgc.data(), g.gc.p, n_streams * sizeof(rk::GenConstraint), cudaMemcpyDeviceToHost, m->stream));
     SYNC(m);
     for (unsigned long long s = 0; s < n_streams; ++s) lengths_out[s] = hg[s].len;
     if (cq && cq->states_out)
@@ -1011,16 +1068,9 @@ int beam(M *m, const unsigned long long *slots, const unsigned long long *first_
     if (n_groups > m->max_gpt) return fail(1, "%s: %llu groups > max_gpt %llu", what, n_groups, m->max_gpt);
     const size_t V = binfmt::kVocab;
     const unsigned long long G = n_groups, B = beams, K = n_best, N = max_new, C = B + n_stop;
-    std::vector<char> used(m->max_gpt, 0);
-    for (unsigned long long i = 0; i < G * B; ++i) {
-        if ((rc = check_slot(m, what, slots[i]))) return rc;
-        if (used[slots[i]]) return fail(1, "%s: slot %llu appears twice", what, slots[i]);
-        used[slots[i]] = 1;
-    }
-    for (unsigned long long i = 0; i < G; ++i)
-        if (first_tokens[i] >= V) return fail(1, "%s: first token %llu of group %llu out of range", what, first_tokens[i], i);
-    for (unsigned long long i = 0; i < n_stop; ++i)
-        if (stop_tokens[i] >= V) return fail(1, "%s: stop token %llu out of range", what, stop_tokens[i]);
+    if ((rc = check_slots(m, what, slots, G * B)) || (rc = check_tokens(what, "first token", first_tokens, G, "group")) ||
+        (rc = check_tokens(what, "stop token", stop_tokens, n_stop)))
+        return rc;
     // the length penalties on the host, with the C library's pow: a host restatement gets the same bits
     if (N > ((unsigned long long)SIZE_MAX / sizeof(rk::BeamBack)) / (G * B))
         return fail(1, "%s: max_new = %llu: the backpointers of %llu beams do not fit in memory", what, N, G * B);
@@ -1034,15 +1084,12 @@ int beam(M *m, const unsigned long long *slots, const unsigned long long *first_
     CK(cudaSetDevice(m->device));
     auto &g = m->gen;
     auto &bm = m->beam;
-    if ((rc = grow(&g.stop, g.stop_cap, (size_t)n_stop)) || (rc = grow(&bm.row0, bm.row0_cap, (size_t)G)) ||
-        (rc = grow(&bm.groups, bm.groups_cap, (size_t)G)) || (rc = grow(&bm.cand_tok, bm.cand_tok_cap, (size_t)(G * B * C))) ||
-        (rc = grow(&bm.cand_lp, bm.cand_lp_cap, (size_t)(G * B * C))) || (rc = grow(&bm.cum, bm.cum_cap, (size_t)(G * B))) ||
-        (rc = grow(&bm.P, bm.P_cap, (size_t)(N + 1))) || (rc = grow(&bm.back, bm.back_cap, (size_t)(G * N * B))) ||
-        (rc = grow(&bm.hyp, bm.hyp_cap, (size_t)(G * K))) || (rc = grow(&bm.n_hyp, bm.n_hyp_cap, (size_t)G)) ||
-        (rc = grow(&bm.done, bm.done_cap, (size_t)G)) || (rc = grow(&bm.forks, bm.forks_cap, (size_t)(2 * G * B))))
+    if ((rc = g.stop.grow(n_stop)) || (rc = bm.row0.grow(G)) || (rc = bm.groups.grow(G)) || (rc = bm.cand_tok.grow(G * B * C)) ||
+        (rc = bm.cand_lp.grow(G * B * C)) || (rc = bm.cum.grow(G * B)) || (rc = bm.P.grow(N + 1)) || (rc = bm.back.grow(G * N * B)) ||
+        (rc = bm.hyp.grow(G * K)) || (rc = bm.n_hyp.grow(G)) || (rc = bm.done.grow(G)) || (rc = bm.forks.grow(2 * G * B)))
         return rc;
-    // the path is chosen once, by forward_streams' rule for G x B one-token streams
-    const bool tc = G * B >= (unsigned long long)m->pf.min_tokens && rk::prefill_enabled(m->pf);
+    // the path is chosen once, for G x B one-token streams
+    const bool tc = tensor_cores(m, G * B);
     if (tc && (rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
     m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
 
@@ -1054,19 +1101,18 @@ int beam(M *m, const unsigned long long *slots, const unsigned long long *first_
         live[i] = (int)i;
     }
     CK(cudaMemcpyAsync(g.gs, hg, G * B * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
-    CK(cudaMemcpyAsync(bm.row0, row0.data(), G * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-    CK(cudaMemcpyAsync(bm.P, P.data(), (N + 1) * sizeof(double), cudaMemcpyHostToDevice, m->stream));
-    if (n_stop) CK(cudaMemcpyAsync(g.stop, stop_tokens, n_stop * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-    CK(cudaMemsetAsync(bm.cum, 0, G * B * sizeof(double), m->stream));
-    CK(cudaMemsetAsync(bm.n_hyp, 0, G * sizeof(int), m->stream));
-    CK(cudaMemsetAsync(bm.done, 0, G * sizeof(unsigned long long), m->stream));
+    CK(cudaMemcpyAsync(bm.row0.p, row0.data(), G * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemcpyAsync(bm.P.p, P.data(), (N + 1) * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+    if (n_stop) CK(cudaMemcpyAsync(g.stop.p, stop_tokens, n_stop * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemsetAsync(bm.cum.p, 0, G * B * sizeof(double), m->stream));
+    CK(cudaMemsetAsync(bm.n_hyp.p, 0, G * sizeof(int), m->stream));
+    CK(cudaMemsetAsync(bm.done.p, 0, G * sizeof(unsigned long long), m->stream));
     double *arr[5];
     slot_arrays(m, 0, arr);
     const size_t slot_len = (size_t)(m->L * m->E);
     const unsigned chunks = (unsigned)((slot_len + rk::kForkChunk - 1) / rk::kForkChunk);
     std::vector<unsigned long long> hdone(G, 0);
     std::vector<int> rs;
-    std::vector<rk::PassDesc> passes;
     for (unsigned long long step = 0; !live.empty() && step < N;) {
         // a host group: the live groups' beams are rows gi * B + j (step 0: row gi); their inputs go up once
         const int Gl = (int)live.size();
@@ -1075,31 +1121,18 @@ int beam(M *m, const unsigned long long *slots, const unsigned long long *first_
         for (int gi = 0; gi < Gl; ++gi)
             for (unsigned long long j = 0; j < B; ++j) rs[gi * B + j] = (int)(live[gi] * B + j);
         CK(cudaMemcpyAsync(g.row_stream, rs.data(), rs.size() * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(bm.groups, live.data(), Gl * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-        if (tc) {
-            const int rows = step == 0 ? Gl : Gl * (int)B;
-            passes.assign((size_t)(rows + rk::kPfMaxTokens - 1) / rk::kPfMaxTokens, rk::PassDesc{});
-            for (int r = 0; r < rows; ++r) {
-                const rk::GenStream &bs = hg[step == 0 ? row0[r] : rs[r]];
-                rk::PassDesc &pd = passes[r / rk::kPfMaxTokens];
-                const int t = r % rk::kPfMaxTokens;
-                pd.tokens[t] = bs.tok;
-                pd.desc[t] = (uint32_t)bs.slot | rk::kDescFirst | rk::kDescLast;
-                pd.rows[t] = t;
-                pd.out_row0 = (r / rk::kPfMaxTokens) * rk::kPfMaxTokens;
-            }
-            CK(cudaMemcpyAsync(g.passes, passes.data(), passes.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
-        }
-        rk::BeamArgs ba{g.gs, bm.cum, bm.groups, bm.cand_tok, bm.cand_lp, (int)C, (int)B, (int)K, 0, 0, N, bm.P,
-                        length_penalty < 0.0 ? 1 : 0, g.stop, (int)n_stop, bm.back, bm.hyp, bm.n_hyp, bm.done, bm.forks,
+        CK(cudaMemcpyAsync(bm.groups.p, live.data(), Gl * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        if (tc && (rc = upload_step_passes(m, step == 0 ? row0.data() : rs.data(), step == 0 ? Gl : Gl * (int)B))) return rc;
+        rk::BeamArgs ba{g.gs, bm.cum.p, bm.groups.p, bm.cand_tok.p, bm.cand_lp.p, (int)C, (int)B, (int)K, 0, 0, N, bm.P.p,
+                        length_penalty < 0.0 ? 1 : 0, g.stop.p, (int)n_stop, bm.back.p, bm.hyp.p, bm.n_hyp.p, bm.done.p, bm.forks.p,
                         tc ? g.passes : nullptr};
         for (unsigned long long k = 0; k < steps; ++k) {
             const unsigned long long st = step + k;
             const int nb = st == 0 ? 1 : (int)B, rows = Gl * nb;
-            const int *rmap = st == 0 ? bm.row0 : g.row_stream;
+            const int *rmap = st == 0 ? bm.row0.p : g.row_stream;
             if ((rc = tc ? gen_step_passes(m, rows) : gen_step_decode(m, rows, rmap))) return rc;
             rk::k_beam_expand<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs, rmap, (int)C,
-                                                                                bm.cand_tok, bm.cand_lp);
+                                                                                bm.cand_tok.p, bm.cand_lp.p);
             CK(cudaGetLastError());
             ba.step = (int)st;
             ba.nb = nb;
@@ -1108,13 +1141,13 @@ int beam(M *m, const unsigned long long *slots, const unsigned long long *first_
             m->launches += 2;
             if (st + 1 < N) { // after the last step every group is done and forks nothing
                 rk::k_beam_fork<<<dim3((unsigned)(Gl * B), chunks, 5), rk::kForkThreads, 0, m->stream>>>(
-                    bm.forks, arr[0], arr[1], arr[2], arr[3], arr[4], slot_len);
+                    bm.forks.p, arr[0], arr[1], arr[2], arr[3], arr[4], slot_len);
                 CK(cudaGetLastError());
                 m->launches += 1;
             }
         }
         // the end of a host group: which groups are done and the beams' records (one synchronisation)
-        CK(cudaMemcpyAsync(hdone.data(), bm.done, G * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(hdone.data(), bm.done.p, G * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
         CK(cudaMemcpyAsync(hg, g.gs, G * B * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
         SYNC(m);
         step += steps;
@@ -1122,8 +1155,8 @@ int beam(M *m, const unsigned long long *slots, const unsigned long long *first_
     }
     std::vector<rk::BeamHyp> hyp(G * K);
     std::vector<rk::BeamBack> back(G * N * B);
-    CK(cudaMemcpyAsync(hyp.data(), bm.hyp, G * K * sizeof(rk::BeamHyp), cudaMemcpyDeviceToHost, m->stream));
-    CK(cudaMemcpyAsync(back.data(), bm.back, G * N * B * sizeof(rk::BeamBack), cudaMemcpyDeviceToHost, m->stream));
+    CK(cudaMemcpyAsync(hyp.data(), bm.hyp.p, G * K * sizeof(rk::BeamHyp), cudaMemcpyDeviceToHost, m->stream));
+    CK(cudaMemcpyAsync(back.data(), bm.back.p, G * N * B * sizeof(rk::BeamBack), cudaMemcpyDeviceToHost, m->stream));
     SYNC(m);
     // each hypothesis' tokens: its last token, then the backpointers of its beam from its step down to step 0
     const double nan = std::nan("");
@@ -1216,19 +1249,9 @@ void rwkv_b200_free(rwkv_b200_model *m) {
     if (m->h_sample) cudaFreeHost(m->h_sample);
     if (m->h_diag) cudaFreeHost(m->h_diag);
     if (m->gen.h_gs) cudaFreeHost(m->gen.h_gs);
-    for (void *p : {(void *)m->gen.out, (void *)m->gen.stop, (void *)m->gen.ovr_tok, (void *)m->gen.ovr_val, (void *)m->gen.u,
-                    (void *)m->gen.samp, (void *)m->gen.pen_cnt, (void *)m->gen.pen_seen, (void *)m->score.rows,
-                    (void *)m->score.tgt, (void *)m->score.rank, (void *)m->score.top_tok, (void *)m->score.lp,
-                    (void *)m->score.top_lp, (void *)m->gen.lp, (void *)m->gen.top_lp, (void *)m->gen.rank,
-                    (void *)m->gen.top_tok, (void *)m->gen.raw, (void *)m->gen.gc, (void *)m->gen.fault,
-                    (void *)m->beam.row0, (void *)m->beam.groups, (void *)m->beam.cand_tok, (void *)m->beam.cand_lp,
-                    (void *)m->beam.cum, (void *)m->beam.P, (void *)m->beam.back, (void *)m->beam.hyp,
-                    (void *)m->beam.n_hyp, (void *)m->beam.done, (void *)m->beam.forks})
-        if (p) cudaFree(p);
-    for (auto &kv : m->automata) cudaFree(kv.second.dev);
     if (m->stream) cudaStreamDestroy(m->stream);
+    delete m; // frees the grow-only buffers and the automata
     cudaGetLastError(); // a context killed by a trap makes every call above fail; do not leave that as "last error"
-    delete m;
 }
 
 void *rwkv_b200_tensor(rwkv_b200_model *m, int index) {
@@ -1270,7 +1293,8 @@ int rwkv_b200_state_upload(rwkv_b200_model *m, const double *xy, const double *a
     CK(cudaSetDevice(m->device));
     const size_t n = (size_t)(m->L * m->E * slots) * sizeof(double);
     const double *src[5] = {xy, aa, bb, pp, dd};
-    double *dst[5] = {m->p.sxy, (double *)m->tensors[STATEAA], (double *)m->tensors[STATEBB], m->spp, m->p.sdd};
+    double *dst[5];
+    slot_arrays(m, 0, dst);
     for (int i = 0; i < 5; ++i)
         if (src[i]) CK(cudaMemcpyAsync(dst[i], src[i], n, cudaMemcpyHostToDevice, m->stream));
     SYNC(m);
@@ -1284,8 +1308,8 @@ int rwkv_b200_state_download(rwkv_b200_model *m, double *xy, double *aa, double 
     if (slots > m->max_gpt) return fail(1, "state_download: %llu slots > max_gpt %llu", slots, m->max_gpt);
     CK(cudaSetDevice(m->device));
     const size_t n = (size_t)(m->L * m->E * slots) * sizeof(double);
-    double *dst[5] = {xy, aa, bb, pp, dd};
-    const double *src[5] = {m->p.sxy, (double *)m->tensors[STATEAA], (double *)m->tensors[STATEBB], m->spp, m->p.sdd};
+    double *dst[5] = {xy, aa, bb, pp, dd}, *src[5];
+    slot_arrays(m, 0, src);
     for (int i = 0; i < 5; ++i)
         if (dst[i]) CK(cudaMemcpyAsync(dst[i], src[i], n, cudaMemcpyDeviceToHost, m->stream));
     SYNC(m);
@@ -1297,8 +1321,9 @@ int rwkv_b200_state_zero(rwkv_b200_model *m) {
     if (rc) return rc;
     CK(cudaSetDevice(m->device));
     const size_t n = (size_t)(m->L * m->E * m->max_gpt) * sizeof(double);
-    for (double *s : {m->p.sxy, (double *)m->tensors[STATEAA], (double *)m->tensors[STATEBB], m->p.sdd, m->spp})
-        CK(cudaMemsetAsync(s, 0, n, m->stream));
+    double *a[5];
+    slot_arrays(m, 0, a);
+    for (double *s : a) CK(cudaMemsetAsync(s, 0, n, m->stream));
     SYNC(m);
     return 0;
 }
@@ -1314,32 +1339,22 @@ int rwkv_b200_forward(rwkv_b200_model *m, const unsigned long long *tokens, unsi
     for (unsigned long long t = 0; t < n_tokens; ++t)
         if (tokens[t] >= V) return fail(1, "token id %llu out of range", tokens[t]);
     m->stream_rows = 0;
-    if (n_tokens >= (unsigned long long)m->pf.min_tokens && m->tp_size == 1 && rk::prefill_enabled(m->pf)) {
-        // GPT: one stream on slot 0; PARRALEL: n streams of one token on slots 0..n-1. Logits of every token.
-        const bool par = mode == RWKV_B200_MODE_PARRALEL;
+    // GPT: one stream on slot 0; PARRALEL: n streams of one token on slots 0..n-1. Logits of every token.
+    const bool par = mode == RWKV_B200_MODE_PARRALEL;
+    std::vector<unsigned long long> slots(par ? n_tokens : 1), lens(par ? n_tokens : 1, par ? 1 : n_tokens);
+    for (size_t i = 0; i < slots.size(); ++i) slots[i] = i;
+    if (tensor_cores(m, n_tokens)) {
         if (par && n_tokens > (unsigned long long)rk::kPfMaxTokens)
             return fail(3, "batched prefill: PARRALEL chunks above 128 tokens are not supported");
-        std::vector<unsigned long long> slots(par ? n_tokens : 1), lens(par ? n_tokens : 1, par ? 1 : n_tokens);
-        for (size_t i = 0; i < slots.size(); ++i) slots[i] = i;
-        rc = rk::prefill_forward(m->pf, m->p, m->stream, tokens, (int)n_tokens, slots.data(), lens.data(), (int)slots.size(),
-                                 logits_out ? 1 : 0, m->d_slogits);
+        rc = rk::prefill_forward(m->pf, m->p, m->stream, tokens, (int)n_tokens, slots.data(), lens.data(), logits_out ? 1 : 0,
+                                 m->d_slogits);
         if (rc) return fail(rc, "%s", rk::prefill_error());
         m->launches += rk::prefill_launches(m->pf);
         if (logits_out) CK(cudaMemcpyAsync(m->h_logits, m->d_slogits, n_tokens * V * sizeof(float), cudaMemcpyDeviceToHost, m->stream));
-        SYNC(m);
-        if (logits_out && logits_out != m->h_logits) memcpy(logits_out, m->h_logits, n_tokens * V * sizeof(float));
-        return 0;
-    }
-    for (unsigned long long t = 0; t < n_tokens; ++t) {
-        rk::Ctrl &c = m->h_ctrl[t];
-        c.token = tokens[t];
-        c.next = 0;
-        c.slot = (mode == RWKV_B200_MODE_PARRALEL) ? t : 0;
-        c.pos = 0;
-        CK(cudaMemcpyAsync(m->p.ctrl, &c, sizeof(rk::Ctrl), cudaMemcpyHostToDevice, m->stream));
-        if ((rc = launch_token(m, 0, false, nullptr, m->stream))) return rc;
-        if (logits_out)
-            CK(cudaMemcpyAsync(m->h_logits + t * V, dev_logits(m), V * sizeof(float), cudaMemcpyDeviceToHost, m->stream));
+    } else {
+        // the logits of token t go to pinned row t
+        const auto row = [&](unsigned long long t, unsigned long long, bool) { return logits_out ? m->h_logits + t * V : nullptr; };
+        if ((rc = decode_tokens(m, tokens, slots.data(), lens.data(), slots.size(), cudaMemcpyDeviceToHost, row))) return rc;
     }
     SYNC(m);
     if (logits_out && logits_out != m->h_logits) memcpy(logits_out, m->h_logits, n_tokens * V * sizeof(float));
@@ -1379,10 +1394,7 @@ int rwkv_b200_sample_typical(rwkv_b200_model *m, float temp, double u, unsigned 
     rk::k_sample_typical<<<1, rk::kSampleThreads, 0, m->stream>>>(dev_logits(m), 0, (int)binfmt::kVocab, sample_exponent(temp), m->d_u,
                                                                   m->d_sample);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(m->h_sample, m->d_sample, 2 * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
-    SYNC(m);
-    *token = (unsigned long long)m->h_sample[0];
-    if (margin) *margin = m->h_sample[1];
+    if ((rc = read_samples(m, 1, token, margin))) return rc;
     m->launches += 1;
     return 0;
 }
@@ -1396,26 +1408,15 @@ int rwkv_b200_forward_streams(rwkv_b200_model *m, const unsigned long long *toke
     CK(cudaSetDevice(m->device));
     const bool head = logits_out || next_out;
     m->stream_rows = 0;
-    if (n_tokens >= (unsigned long long)m->pf.min_tokens && rk::prefill_enabled(m->pf)) {
-        rc = rk::prefill_forward(m->pf, m->p, m->stream, tokens, (int)n_tokens, slots, lengths, (int)n_streams, head ? 2 : 0, m->d_slogits);
+    if (tensor_cores(m, n_tokens)) {
+        rc = rk::prefill_forward(m->pf, m->p, m->stream, tokens, (int)n_tokens, slots, lengths, head ? 2 : 0, m->d_slogits);
         if (rc) return fail(rc, "%s", rk::prefill_error());
         m->launches += rk::prefill_launches(m->pf);
     } else {
-        // token by token through the decode kernel on each stream's slot; the last logits of a stream are copied
-        // into the compact buffer, so the arg-max and the sampler read the same rows as after a batched pass
-        unsigned long long t = 0;
-        for (unsigned long long i = 0; i < n_streams; ++i)
-            for (unsigned long long j = 0; j < lengths[i]; ++j, ++t) {
-                rk::Ctrl &c = m->h_ctrl[t];
-                c.token = tokens[t];
-                c.next = 0;
-                c.slot = slots[i];
-                c.pos = 0;
-                CK(cudaMemcpyAsync(m->p.ctrl, &c, sizeof(rk::Ctrl), cudaMemcpyHostToDevice, m->stream));
-                if ((rc = launch_token(m, 0, false, nullptr, m->stream))) return rc;
-                if (head && j + 1 == lengths[i])
-                    CK(cudaMemcpyAsync(m->d_slogits + i * V, dev_logits(m), V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
-            }
+        // the last logits of a stream are copied into the compact buffer, so the arg-max and the sampler read the same
+        // rows as after a batched pass
+        const auto row = [&](unsigned long long, unsigned long long i, bool last) { return head && last ? m->d_slogits + i * V : nullptr; };
+        if ((rc = decode_tokens(m, tokens, slots, lengths, n_streams, cudaMemcpyDeviceToDevice, row))) return rc;
     }
     if (next_out) {
         rk::k_argmax_rows<<<(unsigned)n_streams, rk::kArgmaxThreads, 0, m->stream>>>(m->d_slogits, (int)V, m->d_next);
@@ -1444,12 +1445,7 @@ int rwkv_b200_sample_typical_streams(rwkv_b200_model *m, unsigned long long n_st
     rk::k_sample_typical<<<(unsigned)n_streams, rk::kSampleThreads, 0, m->stream>>>(m->d_slogits, binfmt::kVocab, (int)binfmt::kVocab,
                                                                                    sample_exponent(temp), m->d_u, m->d_sample);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(m->h_sample, m->d_sample, 2 * n_streams * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
-    SYNC(m);
-    for (unsigned long long i = 0; i < n_streams; ++i) {
-        tokens_out[i] = (unsigned long long)m->h_sample[2 * i];
-        if (margins_out) margins_out[i] = m->h_sample[2 * i + 1];
-    }
+    if ((rc = read_samples(m, n_streams, tokens_out, margins_out))) return rc;
     m->launches += 1;
     return 0;
 }
@@ -1537,13 +1533,10 @@ int rwkv_b200_constraint_add(rwkv_b200_model *m, unsigned long long n_states, co
             next[e] = (uint32_t)edge_next[e];
         }
     CK(cudaSetDevice(m->device));
-    CK(cudaMalloc(&a.dev, bytes));
-    const cudaError_t e = cudaMemcpy(a.dev, blob.data(), bytes, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-        cudaFree(a.dev);
-        return fail(100 + (int)e, "%s: upload failed: %s", what, cudaGetErrorString(e));
-    }
-    unsigned char *d = (unsigned char *)a.dev;
+    if ((rc = a.dev.grow(bytes))) return rc;
+    const cudaError_t e = cudaMemcpy(a.dev.p, blob.data(), bytes, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) return fail(100 + (int)e, "%s: upload failed: %s", what, cudaGetErrorString(e));
+    const unsigned char *d = a.dev.p;
     a.view = rk::GenConstraint{(const unsigned long long *)(d + mask_bytes), (const uint32_t *)(d + mask_bytes + start_bytes),
                                (const uint32_t *)(d + mask_bytes + start_bytes) + n_edges, (const uint32_t *)d, 0};
     *id = m->next_automaton++;
@@ -1557,7 +1550,6 @@ int rwkv_b200_constraint_remove(rwkv_b200_model *m, unsigned long long id) {
     const auto it = m->automata.find(id);
     if (it == m->automata.end()) return fail(1, "constraint_remove: constraint id %llu is unknown or removed", id);
     CK(cudaSetDevice(m->device));
-    cudaFree(it->second.dev);
     m->automata.erase(it);
     return 0;
 }
@@ -1623,22 +1615,17 @@ int rwkv_b200_sample_streams(rwkv_b200_model *m, unsigned long long n_streams, c
     }
     CK(cudaSetDevice(m->device));
     auto &g = m->gen;
-    if ((rc = grow(&g.samp, g.samp_cap, (size_t)n_streams))) return rc;
-    CK(cudaMemcpyAsync(g.samp, params, n_streams * sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
+    if ((rc = g.samp.grow(n_streams))) return rc;
+    CK(cudaMemcpyAsync(g.samp.p, params, n_streams * sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
     if (u) CK(cudaMemcpyAsync(m->d_u, u, n_streams * sizeof(double), cudaMemcpyHostToDevice, m->stream));
     if (logits) {
         m->stream_rows = 0; // the compact rows now hold the caller's logits, not those of the last forward_streams
         CK(cudaMemcpyAsync(m->d_slogits, logits, n_streams * V * sizeof(float), cudaMemcpyHostToDevice, m->stream));
     }
-    rk::k_sample_nucleus<<<(unsigned)n_streams, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.samp, nullptr,
+    rk::k_sample_nucleus<<<(unsigned)n_streams, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.samp.p, nullptr,
                                                                                 u ? m->d_u : nullptr, m->d_sample);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(m->h_sample, m->d_sample, 2 * n_streams * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
-    SYNC(m);
-    for (unsigned long long i = 0; i < n_streams; ++i) {
-        tokens_out[i] = (unsigned long long)m->h_sample[2 * i];
-        if (margins_out) margins_out[i] = m->h_sample[2 * i + 1];
-    }
+    if ((rc = read_samples(m, n_streams, tokens_out, margins_out))) return rc;
     m->launches += 1;
     return 0;
 }
@@ -1674,45 +1661,33 @@ int rwkv_b200_score_streams(rwkv_b200_model *m, const unsigned long long *tokens
     CK(cudaSetDevice(m->device));
     m->stream_rows = 0; // the compact rows hold this call's scored positions, not per-stream logits
     auto &sc = m->score;
-    if (n && ((rc = grow(&sc.rows, sc.rows_cap, n)) || (rc = grow(&sc.tgt, sc.tgt_cap, n)) || (rc = grow(&sc.lp, sc.lp_cap, n)) ||
-              (rc = grow(&sc.rank, sc.rank_cap, n)) || (rc = grow(&sc.top_tok, sc.top_tok_cap, n * top_n)) ||
-              (rc = grow(&sc.top_lp, sc.top_lp_cap, n * top_n))))
+    if (n && ((rc = sc.rows.grow(n)) || (rc = sc.tgt.grow(n)) || (rc = sc.lp.grow(n)) || (rc = sc.rank.grow(n)) ||
+              (rc = sc.top_tok.grow(n * top_n)) || (rc = sc.top_lp.grow(n * top_n))))
         return rc;
-    if (n_tokens >= (unsigned long long)m->pf.min_tokens && rk::prefill_enabled(m->pf)) {
+    if (tensor_cores(m, n_tokens)) {
         // logits of every token of a pass that holds a scored position, row t of d_slogits for token t
-        rc = rk::prefill_forward(m->pf, m->p, m->stream, tokens, (int)n_tokens, slots, lengths, (int)n_streams, n ? 1 : 0,
-                                 m->d_slogits, need.data());
+        rc = rk::prefill_forward(m->pf, m->p, m->stream, tokens, (int)n_tokens, slots, lengths, n ? 1 : 0, m->d_slogits, need.data());
         if (rc) return fail(rc, "%s", rk::prefill_error());
         m->launches += rk::prefill_launches(m->pf);
     } else {
-        // token by token through the decode kernel; a scored position's logits are copied into row t of d_slogits
-        unsigned long long t = 0;
-        for (unsigned long long i = 0; i < n_streams; ++i)
-            for (unsigned long long k = 0; k < lengths[i]; ++k, ++t) {
-                rk::Ctrl &c = m->h_ctrl[t];
-                c.token = tokens[t];
-                c.next = 0;
-                c.slot = slots[i];
-                c.pos = 0;
-                CK(cudaMemcpyAsync(m->p.ctrl, &c, sizeof(rk::Ctrl), cudaMemcpyHostToDevice, m->stream));
-                if ((rc = launch_token(m, 0, false, nullptr, m->stream))) return rc;
-                if (need[t]) CK(cudaMemcpyAsync(m->d_slogits + t * V, dev_logits(m), V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
-            }
+        // a scored position's logits are copied into row t of d_slogits
+        const auto row = [&](unsigned long long t, unsigned long long, bool) { return need[t] ? m->d_slogits + t * V : nullptr; };
+        if ((rc = decode_tokens(m, tokens, slots, lengths, n_streams, cudaMemcpyDeviceToDevice, row))) return rc;
     }
     std::vector<double> lp(n), top_lp(n * top_n);
     std::vector<unsigned long long> rank(n), top_tok(n * top_n);
     if (n) {
-        CK(cudaMemcpyAsync(sc.rows, pos.data(), n * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(sc.tgt, tgt.data(), n * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-        const rk::ScoreArgs a{m->d_slogits, (int)V, sc.rows, sc.tgt, (int)top_n, sc.lp, sc.rank, sc.top_tok, sc.top_lp};
+        CK(cudaMemcpyAsync(sc.rows.p, pos.data(), n * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(sc.tgt.p, tgt.data(), n * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        const rk::ScoreArgs a{m->d_slogits, (int)V, sc.rows.p, sc.tgt.p, (int)top_n, sc.lp.p, sc.rank.p, sc.top_tok.p, sc.top_lp.p};
         rk::k_logprob_rows<<<(unsigned)n, rk::kNucThreads, 0, m->stream>>>(a);
         CK(cudaGetLastError());
         m->launches += 1;
-        CK(cudaMemcpyAsync(lp.data(), sc.lp, n * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
-        if (ranks_out) CK(cudaMemcpyAsync(rank.data(), sc.rank, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(lp.data(), sc.lp.p, n * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+        if (ranks_out) CK(cudaMemcpyAsync(rank.data(), sc.rank.p, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
         if (top_n) {
-            CK(cudaMemcpyAsync(top_tok.data(), sc.top_tok, n * top_n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
-            CK(cudaMemcpyAsync(top_lp.data(), sc.top_lp, n * top_n * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+            CK(cudaMemcpyAsync(top_tok.data(), sc.top_tok.p, n * top_n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+            CK(cudaMemcpyAsync(top_lp.data(), sc.top_lp.p, n * top_n * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
         }
     }
     SYNC(m);

@@ -465,7 +465,6 @@ struct PrefillState {
     bool disabled = false;
     int min_tokens = kPrefillMinTokens; // shorter calls run token by token through the decode kernel
     bool ready = false;
-    int Tmax = 0;
     PfnEncodeTiled encode = nullptr;
     PassDesc *pass = nullptr;   // device copy of the current pass's tokens, descriptors and head row map
     int *iota = nullptr;        // [kPfMaxTokens] 0, 1, 2, ...: the row map of the per-layer layernorms
@@ -527,7 +526,6 @@ inline int prefill_init(PrefillState &s, const Params &p) {
     }
     s.encode = (PfnEncodeTiled)fn;
     const size_t E = (size_t)p.E, V = kVocab, T = kPfMaxTokens;
-    s.Tmax = (int)T;
     PF_CK(cudaMalloc((void **)&s.pass, sizeof(PassDesc)));
     PF_CK(cudaMalloc((void **)&s.iota, T * sizeof(int)));
     PF_CK(cudaMalloc((void **)&s.head_desc, T * sizeof(uint32_t)));
@@ -694,13 +692,6 @@ inline int prefill_chunk_body(PrefillState &s, const Params &p, cudaStream_t st,
     return 0;
 }
 
-// The layout of the next pass from the host.
-inline int prefill_upload(PrefillState &s, cudaStream_t st, const PassDesc &h_pass) {
-    // from pageable memory: the call returns once the source has been read, so the caller may reuse it
-    PF_CK(cudaMemcpyAsync(s.pass, &h_pass, sizeof(PassDesc), cudaMemcpyHostToDevice, st));
-    return 0;
-}
-
 // One pass of the layout already in s.pass: replay (or record) the graph of its shape.
 inline int prefill_run(PrefillState &s, const Params &p, cudaStream_t st, int T, int H, float *logits) {
     int rc;
@@ -741,29 +732,21 @@ inline int prefill_run(PrefillState &s, const Params &p, cudaStream_t st, int T,
     return 0;
 }
 
-// One pass: upload its layout, then replay (or record) the graph of its shape.
-inline int prefill_chunk(PrefillState &s, const Params &p, cudaStream_t st, const PassDesc &h_pass, int T, int H, float *logits) {
-    const int rc = prefill_upload(s, st, h_pass);
-    return rc ? rc : prefill_run(s, p, st, T, H, logits);
-}
-
-// A ragged forward: `tokens` are stream-major, stream i owns lens[i] consecutive tokens and advances state slot
-// slots[i]. The list is cut into passes of at most 128 tokens; a stream that crosses a cut is "last" in one pass
-// and "first" in the next. head = 0: state only. head = 1: logits of every token, row t of `logits`.
-// head = 2: logits of each stream's final token, row i of `logits` for stream i (only the pass holding that token
-// runs the head for it). `logits` is a device buffer of at least n (head 1) / nstreams (head 2) rows.
-// `need` (head 1 only, may be NULL): a pass none of whose tokens has need[t] set runs no head, so its logits rows are
-// not written.
-inline int prefill_forward(PrefillState &s, const Params &p, cudaStream_t st, const unsigned long long *tokens, int n,
-                           const unsigned long long *slots, const unsigned long long *lens, int nstreams, int head, float *logits,
-                           const unsigned char *need = nullptr) {
-    int rc = prefill_init(s, p);
-    if (rc) return rc;
-    PassDesc h{};
+// The passes of a ragged forward: `tokens` are stream-major, stream i owns lens[i] consecutive tokens and advances
+// state slot slots[i]. The list is cut into passes of at most 128 tokens (pass i starts at token 128 i); a stream that
+// crosses a cut is "last" in one pass and "first" in the next. head = 0: state only. head = 1: logits of every token,
+// row t of the logits. head = 2: logits of each stream's final token, row i for stream i (only the pass holding that
+// token runs the head for it). `need` (head 1 only, may be NULL): a pass none of whose tokens has need[t] set runs no
+// head, so its logits rows are not written. Fills each pass's descriptor (zero past its last token) and head row count.
+inline void pass_layout(const unsigned long long *tokens, int n, const unsigned long long *slots, const unsigned long long *lens,
+                        int head, const unsigned char *need, std::vector<PassDesc> &passes, std::vector<int> &heads) {
+    passes.assign((size_t)(n + kPfMaxTokens - 1) / kPfMaxTokens, PassDesc{});
+    heads.assign(passes.size(), 0);
     int stream = 0, pos = 0;  // current stream, index of the next token inside it
     int ended = 0;            // streams whose final token lies in an earlier pass
-    for (int t0 = 0; t0 < n; t0 += s.Tmax) {
-        const int T = std::min(s.Tmax, n - t0);
+    for (size_t i = 0; i < passes.size(); ++i) {
+        PassDesc &h = passes[i];
+        const int t0 = (int)i * kPfMaxTokens, T = std::min(kPfMaxTokens, n - t0);
         int H = 0;
         bool needed = need == nullptr;
         h.out_row0 = head == 1 ? t0 : ended;
@@ -780,8 +763,23 @@ inline int prefill_forward(PrefillState &s, const Params &p, cudaStream_t st, co
             if (fin) ++ended;
             ++pos;
         }
-        if (!needed) H = 0;
-        if ((rc = prefill_chunk(s, p, st, h, T, H, logits))) return rc;
+        heads[i] = needed ? H : 0;
+    }
+}
+
+// A ragged forward (the layout and `head` of pass_layout): per pass, upload its layout, then run it. `logits` is a
+// device buffer of at least n (head 1) / one per stream (head 2) rows.
+inline int prefill_forward(PrefillState &s, const Params &p, cudaStream_t st, const unsigned long long *tokens, int n,
+                           const unsigned long long *slots, const unsigned long long *lens, int head, float *logits,
+                           const unsigned char *need = nullptr) {
+    int rc = prefill_init(s, p);
+    if (rc) return rc;
+    std::vector<PassDesc> passes;
+    std::vector<int> heads;
+    pass_layout(tokens, n, slots, lens, head, need, passes, heads);
+    for (size_t i = 0; i < passes.size(); ++i) {
+        PF_CK(cudaMemcpyAsync(s.pass, &passes[i], sizeof(PassDesc), cudaMemcpyHostToDevice, st));
+        if ((rc = prefill_run(s, p, st, std::min(kPfMaxTokens, n - (int)i * kPfMaxTokens), heads[i], logits))) return rc;
     }
     return 0;
 }

@@ -294,11 +294,9 @@ class Engine:
         automaton state, and a stream ends when its state has no edges). Then it returns one dict per stream with
         "tokens" and "state" (the final automaton state, None without a constraint), plus the logprob fields when
         logprobs is given. Like logprobs, constraints need sampling=... or the arg-max (not the typical sampler)."""
-        if constraints is not None:
-            return self._generate_constrained(streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs,
-                                              top_n, constraints)
-        if logprobs is not None:
-            return self._generate_logprobs(streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n)
+        if logprobs is not None or constraints is not None:
+            return self._generate_scored(streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n,
+                                         constraints)
         temp = 1.0 if temp is None else temp
         S, slots, first, bud, stops, otok, oval, us, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u)
         P = ctypes.c_ulonglong
@@ -315,32 +313,55 @@ class Engine:
                                                      _ptr(lens, P)), "generate_streams")
         return [out[s, :int(lens[s])].copy() for s in range(S)]
 
-    def _generate_logprobs(self, streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n):
-        modes = {"raw": LOGPROBS_RAW, "processed": LOGPROBS_PROCESSED}
+    def _generate_scored(self, streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n, constraints):
+        """generate_streams with logprobs or constraints: rwkv_b200_generate_streams_constrained when constraints are
+        given, else rwkv_b200_generate_streams_logprobs. One dict per stream."""
+        modes = {None: LOGPROBS_RAW, "raw": LOGPROBS_RAW, "processed": LOGPROBS_PROCESSED}
         if logprobs not in modes:
             raise EngineError("generate_streams: logprobs must be 'raw' or 'processed', not %r" % (logprobs,))
         if sampling is None and (u is not None or temp is not None):
+            if constraints is not None:
+                raise EngineError("generate_streams: constraints need sampling=... (or neither u nor temp, for the "
+                                  "arg-max); the typical sampler does not take them")
             raise EngineError("generate_streams: logprobs need sampling=... (or neither u nor temp, for the arg-max); "
                               "the typical sampler reports no log-probabilities")
         S, slots, first, bud, stops, otok, oval, us, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u)
-        lp = np.empty((S, max_new), np.float64)
-        ranks = np.empty((S, max_new), np.uint64)
-        top_tok = np.empty((S, max_new, top_n), np.uint64) if top_n > 0 else None
-        top_lp = np.empty((S, max_new, top_n), np.float64) if top_n > 0 else None
+        lp = ranks = top_tok = top_lp = None
+        if logprobs is not None:
+            lp = np.empty((S, max_new), np.float64)
+            ranks = np.empty((S, max_new), np.uint64)
+            if top_n > 0:
+                top_tok = np.empty((S, max_new, top_n), np.uint64)
+                top_lp = np.empty((S, max_new, top_n), np.float64)
         P = ctypes.c_ulonglong
         sp = _samplers(sampling, S) if sampling is not None else None
-        self._ck(self.lib.rwkv_b200_generate_streams_logprobs(
-            self.h, _ptr(slots, P), _ptr(first, P), S, max_new, _ptr(bud, P), _ptr(stops, P), len(stops), _ptr(otok, P),
-            _ptr(oval, ctypes.c_float), len(otok), sp, _ptr(us, ctypes.c_double), _ptr(out, P), _ptr(lens, P),
-            modes[logprobs], int(top_n), _ptr(lp, ctypes.c_double), _ptr(ranks, P), _ptr(top_tok, P),
-            _ptr(top_lp, ctypes.c_double)), "generate_streams_logprobs")
+        args = (self.h, _ptr(slots, P), _ptr(first, P), S, max_new, _ptr(bud, P), _ptr(stops, P), len(stops), _ptr(otok, P),
+                _ptr(oval, ctypes.c_float), len(otok), sp, _ptr(us, ctypes.c_double), _ptr(out, P), _ptr(lens, P),
+                modes[logprobs], int(top_n), _ptr(lp, ctypes.c_double), _ptr(ranks, P), _ptr(top_tok, P),
+                _ptr(top_lp, ctypes.c_double))
+        if constraints is None:
+            self._ck(self.lib.rwkv_b200_generate_streams_logprobs(*args), "generate_streams_logprobs")
+        else:
+            spec = [constraints] * S if isinstance(constraints, (int, np.integer)) else list(constraints)
+            if len(spec) != S:
+                raise EngineError("generate_streams: %d constraints for %d streams" % (len(spec), S))
+            pairs = [(NO_CONSTRAINT, 0) if c is None else (int(c[0]), int(c[1])) if isinstance(c, (tuple, list))
+                     else (int(c), 0) for c in spec]
+            ids = np.ascontiguousarray([c for c, _ in pairs], np.uint64)
+            starts = np.ascontiguousarray([q for _, q in pairs], np.uint64)
+            states = np.zeros(S, np.uint64)
+            self._ck(self.lib.rwkv_b200_generate_streams_constrained(*args, _ptr(ids, P), _ptr(starts, P), _ptr(states, P)),
+                     "generate_streams_constrained")
         res = []
         for s in range(S):
             n = int(lens[s])
-            d = {"tokens": out[s, :n].copy(), "logprobs": lp[s, :n].copy(), "ranks": ranks[s, :n].copy()}
-            if top_n > 0:
-                d["top_tokens"] = top_tok[s, :n].copy()
-                d["top_logprobs"] = top_lp[s, :n].copy()
+            d = {"tokens": out[s, :n].copy()}
+            if constraints is not None:
+                d["state"] = int(states[s]) if ids[s] != np.uint64(NO_CONSTRAINT) else None
+            if lp is not None:
+                d["logprobs"], d["ranks"] = lp[s, :n].copy(), ranks[s, :n].copy()
+                if top_n > 0:
+                    d["top_tokens"], d["top_logprobs"] = top_tok[s, :n].copy(), top_lp[s, :n].copy()
             res.append(d)
         return res
 
@@ -358,45 +379,6 @@ class Engine:
 
     def remove_constraint(self, cid):
         self._ck(self.lib.rwkv_b200_constraint_remove(self.h, int(cid)), "constraint_remove")
-
-    def _generate_constrained(self, streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n,
-                              constraints):
-        modes = {None: LOGPROBS_RAW, "raw": LOGPROBS_RAW, "processed": LOGPROBS_PROCESSED}
-        if logprobs not in modes:
-            raise EngineError("generate_streams: logprobs must be 'raw' or 'processed', not %r" % (logprobs,))
-        if sampling is None and (u is not None or temp is not None):
-            raise EngineError("generate_streams: constraints need sampling=... (or neither u nor temp, for the arg-max); "
-                              "the typical sampler does not take them")
-        S, slots, first, bud, stops, otok, oval, us, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u)
-        spec = [constraints] * S if isinstance(constraints, (int, np.integer)) else list(constraints)
-        if len(spec) != S:
-            raise EngineError("generate_streams: %d constraints for %d streams" % (len(spec), S))
-        pairs = [(NO_CONSTRAINT, 0) if c is None else (int(c[0]), int(c[1])) if isinstance(c, (tuple, list)) else (int(c), 0)
-                 for c in spec]
-        ids = np.ascontiguousarray([c for c, _ in pairs], np.uint64)
-        starts = np.ascontiguousarray([q for _, q in pairs], np.uint64)
-        states = np.zeros(S, np.uint64)
-        lp = np.empty((S, max_new), np.float64) if logprobs is not None else None
-        ranks = np.empty((S, max_new), np.uint64) if logprobs is not None else None
-        top_tok = np.empty((S, max_new, top_n), np.uint64) if logprobs is not None and top_n > 0 else None
-        top_lp = np.empty((S, max_new, top_n), np.float64) if logprobs is not None and top_n > 0 else None
-        P = ctypes.c_ulonglong
-        sp = _samplers(sampling, S) if sampling is not None else None
-        self._ck(self.lib.rwkv_b200_generate_streams_constrained(
-            self.h, _ptr(slots, P), _ptr(first, P), S, max_new, _ptr(bud, P), _ptr(stops, P), len(stops), _ptr(otok, P),
-            _ptr(oval, ctypes.c_float), len(otok), sp, _ptr(us, ctypes.c_double), _ptr(out, P), _ptr(lens, P),
-            modes[logprobs], int(top_n), _ptr(lp, ctypes.c_double), _ptr(ranks, P), _ptr(top_tok, P),
-            _ptr(top_lp, ctypes.c_double), _ptr(ids, P), _ptr(starts, P), _ptr(states, P)), "generate_streams_constrained")
-        res = []
-        for s in range(S):
-            n = int(lens[s])
-            d = {"tokens": out[s, :n].copy(), "state": int(states[s]) if ids[s] != np.uint64(NO_CONSTRAINT) else None}
-            if logprobs is not None:
-                d["logprobs"], d["ranks"] = lp[s, :n].copy(), ranks[s, :n].copy()
-                if top_n > 0:
-                    d["top_tokens"], d["top_logprobs"] = top_tok[s, :n].copy(), top_lp[s, :n].copy()
-            res.append(d)
-        return res
 
     def score_streams(self, streams, targets=None, top_n=0):
         """Score target tokens in one ragged forward: streams = [(slot, tokens), ...], each advancing its own state slot
