@@ -443,10 +443,9 @@ int rwkv_b200_slot_download(rwkv_b200_model *m, unsigned long long slot, double 
 
 /* Engine knobs (all optional), key/value strings: "window" / "bwindow" (bulk copies in
  * flight per SM while streaming / while the CTAs exchange vectors), "pf_dist" (tiles the L2
- * prefetch runs ahead), "stages" (ring depth), "poll_first", "timeout_ms", "max_layers",
- * "trace", "prefill", "prefill_min", "prefill_graph", "grid" (CTAs, at most the SM count),
- * "cluster" (1, 2 or 4 CTAs share a gather through distributed shared memory; measured
- * without gain, default 1). Returns non-zero for an unknown key. */
+ * prefetch runs ahead), "stages" (ring depth), "timeout_ms", "trace", "prefill",
+ * "prefill_min", "prefill_graph", "grid" (CTAs, at most the SM count). Returns non-zero for
+ * an unknown key. */
 int rwkv_b200_set_option(rwkv_b200_model *m, const char *key, const char *value);
 
 /* --- tensor-parallel wiring (tp_size > 1 only) --------------------------------- */

@@ -53,7 +53,7 @@ struct Diag {
     unsigned long long aux;
 };
 constexpr unsigned int kDiagStats = 1, kDiagVec = 2, kDiagOff = 3, kDiagPeerSum = 4, kDiagSr = 5, kDiagDone = 6,
-                       kDiagArg = 7, kDiagRingFull = 8, kDiagRingEmpty = 9, kDiagPlanesFree = 10, kDiagPlanesReady = 11;
+                       kDiagArg = 7, kDiagRingFull = 8, kDiagRingEmpty = 9;
 
 // Everything the token kernel needs, passed by value (__grid_constant__).
 // G ranks (GPUs) decode ONE stream together (G = 1: a single GPU). Split (SURVEY 8e):
@@ -64,23 +64,21 @@ constexpr unsigned int kDiagStats = 1, kDiagVec = 2, kDiagOff = 3, kDiagPeerSum 
 //   head           : column split over the vocabulary
 // The residual stream, layernorm and token shift are replicated on every rank (bit-identical).
 struct Params {
-    int L, E;
+    int E;
     int G, rank;
     int Er;                 // E / G
     int Vr, vbase;          // vocabulary rows of this rank, first global row
     int tile_bytes, stages; // ring: `stages` tiles of 8*E bytes
     int plane_cap;          // bytes reserved for limb planes in shared memory
-    int L_run;              // layers to run (debug knob; normally == L)
+    // Layers. Kept between two fields the producer lane does not read: next to E the compiler fetches both with one
+    // vector parameter load, whose registers the producer's 40 cannot hold (ptxas spills 48 more bytes).
+    int L;
     int feed_mode;          // 0: ctrl->token, 1: ctrl->next (free-running), 2: stream[ctrl->pos]
     int greedy;             // 1: finish with an on-device argmax into ctrl->next
-    int issue_gap;          // minimum SM cycles between two bulk-copy issues of the producer (0 = unpaced)
     int window;             // bulk copies in flight per CTA (<= stages)
-    int cluster;            // CTAs per thread-block cluster (1, 2 or 4): they split the gather and write each other's limb planes
     int vseg;               // segments per ffn-V row (4E/G bytes): 4, 2 or 1 so that a segment is <= E bytes and a tile 8 / vseg rows
     int bwindow;            // bulk copies in flight per CTA while the consumers exchange vectors (latency of their loads)
     int pf_dist;            // tiles the L2 prefetch cursor runs ahead of the ring (0 = no L2 prefetch)
-    int dbg;                // debug experiments (bit 0: run the slice statistics twice, cold / warm code)
-    int poll_first;         // gather: 1 = poll the first 16 bytes before fetching the rest, 0 = fetch everything at once
     unsigned int ep0;       // epoch before this token: layer l tags its exchanges with ep0 + 1 + l
     unsigned int tk;        // token epoch (tags of the once-per-token exchanges)
     unsigned int timeout_ms;
@@ -151,31 +149,6 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
                  : "memory");
     return ok != 0;
 }
-// ---- thread-block cluster helpers (distributed shared memory) ---------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-// shared-window address `addr` of this CTA -> the same location in CTA `rank` of the cluster (shared::cluster window)
-__device__ __forceinline__ uint32_t mapa(uint32_t addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-    return r;
-}
-// 4-byte store into another CTA's shared memory that reports its bytes to an mbarrier of THAT CTA: whoever waits
-// for the barrier's phase sees the data - no fence on either side (a release at cluster scope costs microseconds
-// here: it drains everything the thread has in flight)
-__device__ __forceinline__ void st_async32(uint32_t remote_addr, uint32_t v, uint32_t remote_bar) {
-    asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(remote_addr), "r"(v), "r"(remote_bar) : "memory");
-}
-// arrive on an mbarrier of another CTA of the cluster, no ordering implied
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t remote_bar) {
-    asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote_bar) : "memory");
-}
-__device__ __forceinline__ void cluster_sync_all() { // every thread of every CTA of the cluster
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 // non-blocking test of an mbarrier phase
 __device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity) {
     uint32_t ok;
@@ -239,12 +212,6 @@ __device__ __forceinline__ size_t opaque(size_t v) {
     return v;
 }
 
-// clock read that the compiler keeps between the computation of `a`, `b` and everything that uses them afterwards
-__device__ __forceinline__ long long clock_after(double &a, double &b) {
-    long long t;
-    asm volatile("mov.u64 %0, %%clock64;" : "=l"(t), "+d"(a), "+d"(b));
-    return t;
-}
 __device__ __forceinline__ void tok_sync() { // named barrier 1: the eight consumer warps
     asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
 }
@@ -297,14 +264,12 @@ struct Smem {
     double *pd;          // [kMaxSlice][8] epilogue parameters of the slice owners, staged with cp.async
     float *pf;           // [kMaxSlice][8]
     float *pk;           // [kMaxKeys][2]  ffn-V scale / offset of the own key channels
-    long long *clk;      // [16] debug cycle counters (set_option dbg=4)
-    uint64_t *cbar;      // [2] cluster mbarriers: [0] every CTA of the cluster has read its limb planes, [1] the planes are written
     uint32_t *gmax;      // [4] max |xs| of the vectors of the current gather (atomicMax of the warps' parts), [3] boundary flag
     double *osum;        // [kWarps][3] the warps' parts of the offset sums
 };
 
 __host__ __device__ inline size_t smem_fixed_bytes() {
-    return kMaxRowsPerCta * 8 + 16 * 8 + kWarps * 4 * 4 + 2 * kMaxStages * 8 + kMaxSlice * (8 + 4 + 64 + 32) + kMaxKeys * 8 + 128 + 128 + 16 + 16 + kWarps * 3 * 8;
+    return kMaxRowsPerCta * 8 + 16 * 8 + kWarps * 4 * 4 + 2 * kMaxStages * 8 + kMaxSlice * (8 + 4 + 64 + 32) + kMaxKeys * 8 + 128 + 16 + kWarps * 3 * 8;
 }
 __host__ __device__ inline size_t smem_bytes(int stages, int tile_bytes, int plane_cap) {
     return (size_t)stages * tile_bytes + plane_cap + smem_fixed_bytes();
@@ -336,10 +301,6 @@ __device__ __forceinline__ Smem carve(uint8_t *base, const Params &p) {
     q += kMaxSlice * sizeof(float);
     s.wmax = reinterpret_cast<uint32_t *>(q);
     q += kWarps * 4 * sizeof(uint32_t);
-    s.clk = reinterpret_cast<long long *>(q);
-    q += 16 * sizeof(long long);
-    s.cbar = reinterpret_cast<uint64_t *>(q);
-    q += 2 * sizeof(uint64_t);
     s.gmax = reinterpret_cast<uint32_t *>(q);
     q += 4 * sizeof(uint32_t);
     s.osum = reinterpret_cast<double *>(q);

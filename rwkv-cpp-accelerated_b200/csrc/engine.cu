@@ -116,7 +116,6 @@ struct rwkv_b200_model {
     float *h_logits = nullptr;  // pinned [max_gpt][V]
     unsigned long long *h_next = nullptr;
     rk::Diag *h_diag = nullptr; // mapped pinned: the kernel's last words before a timeout trap
-    int max_layers = -1;        // debug: run only the first n layers
     unsigned long long launches = 0;
     unsigned int epoch = 0, tk = 0; // exchange epochs (token_kernel.cuh); identical on every rank
     int tp_rank = 0, tp_size = 1;
@@ -184,19 +183,16 @@ template <class T> int dmalloc(M *m, T **out, size_t count) {
     return 0;
 }
 
-int layers_to_run(const M *m) { return m->max_layers >= 0 && m->max_layers < (int)m->L ? m->max_layers : (int)m->L; }
-
 // A failed synchronisation: if the kernel left a diagnostic record, say what it was waiting for.
 int sync_failed(M *m, cudaError_t e, const char *what) {
     const rk::Diag *d = m->h_diag;
     if (d && d->code) {
         static const char *names[] = {"", "slice statistics", "activation vector", "offset sums", "peer partial sums",
-                                      "sigmoid exchange", "completion flags", "arg-max candidates", "ring (full)", "ring (empty)",
-                                      "cluster: limb planes free", "cluster: limb planes written"};
+                                      "sigmoid exchange", "completion flags", "arg-max candidates", "ring (full)", "ring (empty)"};
         return fail(100 + (int)e,
                     "%s failed: %s; token kernel timed out waiting for %s: rank %u cta %u thread %u layer %u kind %u "
                     "expected tag %u saw %u aux %llu (a peer rank that never launched, or a protocol bug)",
-                    what, cudaGetErrorString(e), d->code < 12 ? names[d->code] : "?", d->rank, d->cta, d->thread, d->layer,
+                    what, cudaGetErrorString(e), d->code < 10 ? names[d->code] : "?", d->rank, d->cta, d->thread, d->layer,
                     d->kind, d->expect, d->seen, d->aux);
     }
     return fail(100 + (int)e, "%s failed: %s", what, cudaGetErrorString(e));
@@ -237,42 +233,36 @@ void configure_ring(M *m) {
     m->smem = rk::smem_bytes(p.stages, p.tile_bytes, p.plane_cap);
 }
 
-void fill_launch(int grid, int cluster, size_t smem, cudaLaunchConfig_t &cfg, cudaLaunchAttribute (&attrs)[2], cudaStream_t s) {
+void fill_launch(int grid, size_t smem, cudaLaunchConfig_t &cfg, cudaLaunchAttribute &attr, cudaStream_t s) {
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(rk::kThreads);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = s;
-    attrs[0].id = cudaLaunchAttributeCooperative;
-    attrs[0].val.cooperative = 1;
-    attrs[1].id = cudaLaunchAttributeClusterDimension;
-    attrs[1].val.clusterDim.x = (unsigned int)cluster;
-    attrs[1].val.clusterDim.y = 1;
-    attrs[1].val.clusterDim.z = 1;
-    cfg.attrs = attrs;
-    cfg.numAttrs = cluster > 1 ? 2 : 1;
+    attr.id = cudaLaunchAttributeCooperative;
+    attr.val.cooperative = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
 }
 
 int launch_token(M *m, int feed, bool greedy, const unsigned long long *stream, cudaStream_t s) {
     if (m->tp_size > 1 && !m->tp_wired)
         return fail(7, "tensor parallelism: call rwkv_b200_tp_import with every rank's handle before the first forward");
     rk::Params prm = m->p;
-    prm.L_run = layers_to_run(m);
     prm.feed_mode = feed;
     prm.greedy = greedy ? 1 : 0;
     prm.stream = stream;
     prm.ep0 = m->epoch;
     prm.tk = ++m->tk;
     if (prm.tk == 0) prm.tk = ++m->tk; // tag 0 means "never written"
-    m->epoch += (unsigned int)prm.L_run + 1u;
+    m->epoch += (unsigned int)prm.L + 1u;
     void *args[] = {&prm};
     const bool full = m->E == (unsigned long long)m->cpl * 512ull;
     const void *fn = token_entry(m->cpl, full, m->p.trace != nullptr);
     if (!fn) return fail(3, "no kernel for %d chunks per lane", m->cpl);
-    // cooperative: all CTAs resident together (they wait for each other's words); clusters of p.cluster CTAs share
-    // the gather through distributed shared memory
+    // cooperative: all CTAs resident together (they wait for each other's words)
     cudaLaunchConfig_t cfg{};
-    cudaLaunchAttribute attrs[2];
-    fill_launch(m->grid, m->p.cluster, m->smem, cfg, attrs, s);
+    cudaLaunchAttribute attr;
+    fill_launch(m->grid, m->smem, cfg, attr, s);
     CK(cudaLaunchKernelExC(&cfg, fn, args));
     m->launches += 1;
     return 0;
@@ -382,24 +372,12 @@ bool grid_fits(unsigned long long E, unsigned long long Er, unsigned long long V
            3 * nc <= (unsigned long long)rk::kMaxRowsPerCta && nv <= (unsigned long long)rk::kMaxRowsPerCta;
 }
 
-// A grid of `grid` CTAs in clusters of `cluster`: divisibility, slice capacities, and - the CTAs wait for each
-// other's words - that the device can hold all of them at once.
-int check_grid(M *m, int grid, int cluster) {
-    if (cluster != 1 && cluster != 2 && cluster != 4) return fail(1, "cluster must be 1, 2 or 4");
-    if (grid < cluster || grid > m->sms || grid % cluster != 0)
-        return fail(1, "grid=%d must be a multiple of cluster=%d and at most %d (the SM count)", grid, cluster, m->sms);
+// A grid of `grid` CTAs: one CTA per SM at most (the CTAs wait for each other's words, so all of them must be
+// resident at once) and the slice capacities.
+int check_grid(M *m, int grid) {
+    if (grid < 1 || grid > m->sms) return fail(1, "grid=%d must be 1..%d (the SM count)", grid, m->sms);
     if (!grid_fits(m->E, (unsigned long long)m->p.Er, (unsigned long long)m->p.Vr, grid))
         return fail(5, "a grid of %d CTAs does not fit n_embed=%llu", grid, m->E);
-    if (cluster > 1) {
-        cudaLaunchConfig_t cfg{};
-        cudaLaunchAttribute attrs[2];
-        fill_launch(grid, cluster, m->smem, cfg, attrs, m->stream);
-        const bool full = m->E == (unsigned long long)m->cpl * 512ull;
-        int nclusters = 0;
-        CK(cudaOccupancyMaxActiveClusters(&nclusters, token_entry(m->cpl, full, m->p.trace != nullptr), &cfg));
-        if (nclusters * cluster < grid)
-            return fail(5, "the device holds %d clusters of %d CTAs at once; a grid of %d needs %d", nclusters, cluster, grid, grid / cluster);
-    }
     return 0;
 }
 
@@ -457,11 +435,9 @@ int do_load(M *m, const char *path, int quiet) {
     p.timeout_ms = G > 1 ? 60000u : 4000u;
     configure_ring(m);
     p.window = std::min(p.stages, 2);
-    p.poll_first = 2;
     p.pf_dist = 4;
     p.bwindow = 1;
     p.vseg = G >= 4 ? 1 : G >= 2 ? 2 : 4; // 4E/G bytes per ffn-V row in segments of at most E bytes
-    p.cluster = 1;
     if (p.stages < 2) return fail(5, "n_embed=%llu leaves no room for a two-stage ring", E);
     if (!grid_fits(E, Er, Vr, m->grid)) return fail(5, "a grid of %d CTAs does not fit n_embed=%llu", m->grid, E);
     const bool full = E == (unsigned long long)m->cpl * 512ull;
@@ -1860,29 +1836,18 @@ int rwkv_b200_set_option(rwkv_b200_model *m, const char *key, const char *value)
             m->p.trace = nullptr;
             m->p.ptrace = nullptr;
         }
-    } else if (k == "max_layers") m->max_layers = v;
-    else if (k == "issue_gap") {
-        if (v < 0 || v > 100000) return fail(1, "issue_gap is a cycle count in 0..100000");
-        m->p.issue_gap = v;
     } else if (k == "window") {
         if (v < 1 || v > rk::kMaxStages) return fail(1, "window must be 1..%d", rk::kMaxStages);
         m->p.window = v;
-    } else if (k == "cluster" || k == "grid") {
-        const int c = k == "cluster" ? v : m->p.cluster, g = k == "grid" ? v : m->grid;
-        if (int rc2 = check_grid(m, g, c)) return rc2;
-        m->p.cluster = c;
-        m->grid = g;
+    } else if (k == "grid") {
+        if (int rc2 = check_grid(m, v)) return rc2;
+        m->grid = v;
     } else if (k == "bwindow") {
         if (v < 1 || v > rk::kMaxStages) return fail(1, "bwindow must be 1..%d", rk::kMaxStages);
         m->p.bwindow = v;
     } else if (k == "pf_dist") {
         if (v < 0 || v > 64) return fail(1, "pf_dist is 0..64 tiles");
         m->p.pf_dist = v;
-    } else if (k == "poll_first") {
-        if (v < 0 || v > 2) return fail(1, "poll_first is 0, 1 or 2");
-        m->p.poll_first = v;
-    } else if (k == "dbg") {
-        m->p.dbg = v;
     } else if (k == "timeout_ms") {
         if (v < 1) return fail(1, "timeout_ms must be positive");
         m->p.timeout_ms = (unsigned int)v;

@@ -78,7 +78,7 @@ __host__ __device__ inline Slices make_slices(int E, int Er, int Vr, int b, int 
 // starts from an empty pipe. With it HBM streams continuously into L2 (50 MB) and the ring refills from
 // L2 at the consumers' pace.
 struct TileCursor {
-    int l, s;           // layer (== L_run: head), sub inside the layer
+    int l, s;           // layer (== L: head), sub inside the layer
     int r, nr, tr;      // next row inside the sub, rows of the sub, rows per tile
     int N;              // bytes per row
     const int8_t *base; // first row of the sub
@@ -92,8 +92,8 @@ struct TileRef {
 __device__ __forceinline__ void load_sub(const Params &p, const Slices &sl, TileCursor &c) {
     const int E = p.E, Er = p.Er;
     c.r = 0;
-    if (c.l >= p.L_run) {
-        c.N = E; c.tr = 8; c.nr = c.l == p.L_run ? sl.nv : 0;
+    if (c.l >= p.L) {
+        c.N = E; c.tr = 8; c.nr = c.l == p.L ? sl.nv : 0;
         c.base = p.whead + (size_t)sl.v0 * E;
         return;
     }
@@ -111,8 +111,8 @@ __device__ __forceinline__ void load_sub(const Params &p, const Slices &sl, Tile
 // The tile under the cursor, then advance. Returns false at the end of the token's schedule.
 __device__ __forceinline__ bool next_tile(const Params &p, const Slices &sl, TileCursor &c, TileRef &t) {
     while (c.r >= c.nr) { // next sub
-        if (c.l >= p.L_run) {
-            if (c.l > p.L_run) return false;
+        if (c.l >= p.L) {
+            if (c.l > p.L) return false;
             ++c.l; // past the head: the end
             c.nr = 0;
             return false;
@@ -358,55 +358,34 @@ __device__ __forceinline__ void trace_stamp(unsigned long long *trace, double *s
 
 // ---- gather: exchanged vectors -> limb planes --------------------------------------------------------
 // The `nvec` vectors of length N (contiguous f32+tag words at `vec`) were written by their slice owners.
-// Every thread polls the first 16 bytes of its share until they carry this epoch, then fetches the rest
-// in one batch (one L2 round trip when everything has arrived, which is the normal case: the owners
-// publish within a fraction of a microsecond of each other), re-reads whatever was not there yet, takes
+// The consumer warps meet at the block barrier first - the owners of THIS CTA have published by then, and
+// the CTAs run in step - then every thread fetches its share in one batch (one L2 round trip when
+// everything has arrived, which is the normal case, and no polling traffic while the owners still
+// compute), re-reads whatever was not there yet, takes
 // the per-vector max |xs| over the block and quantises from registers into the limb planes
 // (vector v -> planes + v*3*N). Warp 7 also sums the owners' partial offset sums (OffRec) in a fixed
 // order. Result: scal[v] = S_v (value of one integer step), scal[3+v] = sum_j x_j * oc_j.
-// Every CTA starts at a different offset so that the CTAs do not hit the same L2 lines together.
+// (Starting every CTA at a different offset of the vector was measured slower than walking it in the same order.)
 // Inlined ONCE (the phase loop of the kernel has a single call site): as a separate function it would be
 // compiled against the 168-register launch budget instead of the consumers' 232 and spill.
 constexpr int kGatherMax = 20; // 16-byte groups per thread: 256 x 20 x 4 >= 4 * 5120
 __device__ __forceinline__ void gather(const Params &p, const Smem &sm, const float *vec, const TaggedDouble *offrec,
                                        const unsigned long long *maxrec, int nvec,
-                                       int N, uint32_t tag, unsigned int layer, int ctid, int gk, unsigned long long *trace) {
+                                       int N, uint32_t tag, unsigned int layer, int ctid, unsigned long long *trace) {
     const uint32_t tag2 = tag & 3u;
     const int ng = N >> 2;        // groups per vector
     const int total = nvec * ng;  // <= 256 * kGatherMax
-    // The C CTAs of a thread-block cluster split the gather: CTA r of the cluster fetches and quantises the r-th
-    // part of the concatenated vectors and writes the limb-plane words into the shared memory of all C CTAs
-    // (st.shared::cluster). All 132 SMs pulling the same 16..64 KB out of L2 is what bounds the exchange (L2
-    // bandwidth, tools/latbench.cu part 3) and the quantisation is ALU work per phase: both shrink by C.
-    // (Starting every CTA at a different offset of the vector was measured slower than walking it in the same order.)
-    const int C = p.cluster;
-    const int part = total / C;   // N is a multiple of 16: total is a multiple of 4
-    const int base = (C > 1 ? (int)cluster_ctarank() * part : 0) + ctid;
-    const int cnt = (part - ctid + kConsumers - 1) / kConsumers; // groups of this thread (may be <= 0)
+    const int cnt = (total - ctid + kConsumers - 1) / kConsumers; // groups of this thread (may be <= 0)
     const uint4 *src = reinterpret_cast<const uint4 *>(vec);
-    auto index = [&](int i) { return base + kConsumers * i; };
+    auto index = [&](int i) { return ctid + kConsumers * i; };
     const uint4 absent = make_uint4(tag2, tag2, tag2, tag2); // +0.0f carrying the tag: a slot this thread does not have
     uint4 f[kGatherMax];
     Waiter wt = waiter_begin();
-    f[0] = absent;
-    // poll_first 2: meet at the block barrier first - the owners of THIS CTA have published by then, and the
-    // CTAs run in step, so one batch of loads normally finds everything (one L2 round trip, no polling
-    // traffic while the owners still compute); 1: poll the first 16 bytes, then the batch; 0: batch at once.
     if (ctid == 0) *reinterpret_cast<volatile uint32_t *>(sm.gmax + 3) = 1u; // latency-bound window: the producer goes quiet
-    if (p.poll_first == 2) tok_sync();
+    tok_sync();
     trace_stamp(trace, sm.scal, ctid); // G1: block met
-    if (cnt > 0 && p.poll_first != 1) f[0] = ld_vec4(src + index(0));
-    if (cnt > 0 && p.poll_first == 1) {
-        const uint4 *s0 = src + index(0);
-        f[0] = ld_vec4(s0);
-        while (!vec4_ok(f[0], tag2)) {
-            if (waiter_tick(p, wt)) wait_expired(p, kDiagVec, layer, (unsigned int)nvec, tag2, f[0].x & 3u, (unsigned long long)index(0));
-            f[0] = ld_vec4(s0);
-        }
-    }
-    __syncwarp();
 #pragma unroll
-    for (int i = 1; i < kGatherMax; ++i) {
+    for (int i = 0; i < kGatherMax; ++i) {
         f[i] = absent;
         if (i < cnt) f[i] = ld_vec4(src + index(i));
     }
@@ -460,18 +439,12 @@ __device__ __forceinline__ void gather(const Params &p, const Smem &sm, const fl
             }
         }
         if (!__any_sync(0xffffffffu, bad)) break; // warp-uniform exit (see slice_stats)
-        if (waiter_tick(p, wt)) wait_expired(p, kDiagVec, layer, (unsigned int)nvec, tag2, 99u, (unsigned long long)base);
+        if (waiter_tick(p, wt)) wait_expired(p, kDiagVec, layer, (unsigned int)nvec, tag2, 99u, (unsigned long long)ctid);
     }
     trace_stamp(trace, sm.scal, ctid); // all words here
     trace_stamp(trace, sm.scal, ctid); // G3
     tok_sync(); // the maxima of all warps are in shared memory
     trace_stamp(trace, sm.scal, ctid); // G4
-    const bool probe = (p.dbg & 8) != 0; // cycle counters of the steps below, thread 0, summed over the token
-    long long pc[6];
-    auto tick = [&](int k) {
-        if (probe) asm volatile("mov.u64 %0, %%clock64;" : "=l"(pc[k])::"memory");
-    };
-    tick(0);
     if (ctid == 0) *reinterpret_cast<volatile uint32_t *>(sm.gmax + 3) = 0u; // the exchange loads are back: the producer may open its window
     float inv0, inv1, inv2;
     {   // scale of vector v (the same bits in every thread and every CTA)
@@ -482,55 +455,20 @@ __device__ __forceinline__ void gather(const Params &p, const Smem &sm, const fl
         if (ctid < 3) sm.scal[ctid] = (double)(ctid == 0 ? m0 : ctid == 1 ? m1 : m2) * (1.0 / (double)kQMax);
     }
     const uint32_t pl0 = smem_u32(sm.planes);
-    tick(1);
-    if (C == 1) {
 #pragma unroll
-        for (int i = 0; i < kGatherMax; ++i) {
-            if (i < cnt) {
-                // element 4*gg of the concatenated vectors sits 4*gg + v*2N bytes into the planes (3N bytes per vector)
-                const int gg = index(i);
-                const int v = (gg >= ng) + (gg >= 2 * ng);
-                const float iv = v == 0 ? inv0 : v == 1 ? inv1 : inv2;
-                const PlaneWords w = quantize4(f[i], iv);
-                const uint32_t a = pl0 + (uint32_t)(4 * gg + 2 * v * N);
-                sts32(a, w.w0);
-                sts32(a + (uint32_t)N, w.w1);
-                sts32(a + 2u * (uint32_t)N, w.w2);
-            }
-        }
-    } else {
-        // every CTA of the cluster has finished the GEMV that read its planes (signalled after that GEMV)
-        if (gk > 0) mbar_wait(p, smem_u32(sm.cbar), (uint32_t)(gk - 1) & 1u, kDiagPlanesFree);
-        const uint32_t me = cluster_ctarank(), bar1 = smem_u32(sm.cbar + 1);
-        uint32_t plr[4], barr[4];
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            plr[r] = mapa(pl0, (uint32_t)(r < C ? r : 0));
-            barr[r] = mapa(bar1, (uint32_t)(r < C ? r : 0));
-        }
-#pragma unroll
-        for (int i = 0; i < kGatherMax; ++i) {
-            if (i < cnt) {
-                const int gg = index(i);
-                const int v = (gg >= ng) + (gg >= 2 * ng);
-                const float iv = v == 0 ? inv0 : v == 1 ? inv1 : inv2;
-                const PlaneWords w = quantize4(f[i], iv);
-                const uint32_t o = (uint32_t)(4 * gg + 2 * v * N);
-                sts32(pl0 + o, w.w0);
-                sts32(pl0 + o + (uint32_t)N, w.w1);
-                sts32(pl0 + o + 2u * (uint32_t)N, w.w2);
-#pragma unroll
-                for (int r = 0; r < 4; ++r) {
-                    if (r < C && r != (int)me) {
-                        st_async32(plr[r] + o, w.w0, barr[r]);
-                        st_async32(plr[r] + o + (uint32_t)N, w.w1, barr[r]);
-                        st_async32(plr[r] + o + 2u * (uint32_t)N, w.w2, barr[r]);
-                    }
-                }
-            }
+    for (int i = 0; i < kGatherMax; ++i) {
+        if (i < cnt) {
+            // element 4*gg of the concatenated vectors sits 4*gg + v*2N bytes into the planes (3N bytes per vector)
+            const int gg = index(i);
+            const int v = (gg >= ng) + (gg >= 2 * ng);
+            const float iv = v == 0 ? inv0 : v == 1 ? inv1 : inv2;
+            const PlaneWords w = quantize4(f[i], iv);
+            const uint32_t a = pl0 + (uint32_t)(4 * gg + 2 * v * N);
+            sts32(a, w.w0);
+            sts32(a + (uint32_t)N, w.w1);
+            sts32(a + 2u * (uint32_t)N, w.w2);
         }
     }
-    tick(2);
     {   // this warp's part of the offset sums (fixed trees), then warps 0..7 in order by thread v
         double t0 = has_rec ? pair_to_double(ra[0], rb[0]) : 0.0, t1 = has_rec ? pair_to_double(ra[1], rb[1]) : 0.0,
                t2 = has_rec ? pair_to_double(ra[2], rb[2]) : 0.0;
@@ -547,32 +485,13 @@ __device__ __forceinline__ void gather(const Params &p, const Smem &sm, const fl
             sm.osum[wq * 3 + 2] = t2;
         }
     }
-    tick(3);
-    if (C == 1) {
-        tok_sync();
-    } else {
-        // "planes written": this CTA's eight warps arrive after their own stores; the other CTAs' words arrive as
-        // transaction bytes (12 per group of four elements) of their st.async
-        __syncwarp();
-        const uint32_t bar1 = smem_u32(sm.cbar + 1);
-        if (lane == 0) {
-            if (wq == 0) mbar_expect_tx(bar1, 12u * (uint32_t)(total - part));
-            else mbar_arrive(bar1);
-        }
-        mbar_wait(p, bar1, (uint32_t)gk & 1u, kDiagPlanesReady);
-    }
-    tick(4);
+    tok_sync();
     if (ctid < 3) {
         double t = 0.0;
 #pragma unroll
         for (int w = 0; w < kWarps; ++w) t += sm.osum[w * 3 + ctid];
         sm.scal[3 + ctid] = t;  // read by the epilogue, after the GEMV and its barrier
         sm.gmax[ctid] = 0u;     // for the next gather
-    }
-    tick(5);
-    if (probe && ctid == 0) {
-        for (int k = 0; k < 5; ++k) sm.clk[8 + k] += pc[k + 1] - pc[k];
-        sm.clk[13] += 1;
     }
     trace_stamp(trace, sm.scal, ctid); // planes ready
 }
@@ -590,51 +509,33 @@ __device__ __forceinline__ void gather(const Params &p, const Smem &sm, const fl
 struct StatsOut {
     double mean, rstd;
 };
-__device__ __noinline__ StatsOut slice_stats(const Params &p, const double *xown, double *scal, long long *clkp, volatile uint32_t *quiet,
+__device__ __noinline__ StatsOut slice_stats(const Params &p, const double *xown, double *scal, volatile uint32_t *quiet,
                                              TaggedDouble *recs, int ne, uint32_t tag, unsigned int layer, int ctid, double c0,
                                              unsigned long long *trace) {
-    struct {
-        const double *xown;
-        double *scal;
-        long long *clk;
-    } sm{xown, scal, clkp};
     own_sync(); // xown complete
     if (ctid == 0) *quiet = 1u; // latency-bound window: the producer goes quiet (token_kernel.cuh: produce_token)
-    trace_stamp(trace, sm.scal, ctid); // S1: owners synchronised
+    trace_stamp(trace, scal, ctid); // S1: owners synchronised
     if (ctid < 32) {
         const int lane = ctid;
         const int nb = (int)gridDim.x;
         // Every CTA reads every record: 132 x 32 lanes on the same few L2 lines serialise there
         // for one batch of loads. The writer stores kRep copies, reader b takes copy b % kRep.
         TaggedDouble *const sums = recs + (size_t)(blockIdx.x % kRep) * 2 * nb, *const qs = sums + nb; // [nb] each
-        const double v0 = lane < ne ? sm.xown[lane] : 0.0, v1 = lane + 32 < ne ? sm.xown[lane + 32] : 0.0;
+        const double v0 = lane < ne ? xown[lane] : 0.0, v1 = lane + 32 < ne ? xown[lane + 32] : 0.0;
         const double d0 = lane < ne ? v0 - c0 : 0.0, d1 = lane + 32 < ne ? v1 - c0 : 0.0;
         double s = v0 + v1, q = d0 * d0 + d1 * d1;
         __syncwarp(); // reconverge (see warp_sum in common.cuh)
-        const bool clk = (p.dbg & 4) != 0;
-        long long tc0 = 0, tc1 = 0, tc2 = 0, tc3 = 0, tc4 = 0;
-        if (clk) tc0 = clock_after(s, q);
-        if ((p.dbg & 2) && trace != nullptr) { // debug: split the segment
-            if (__double_as_longlong(q) == 0x7ff8000000000001ll) s = 0.0; // (consume q before the stamp)
-            trace_stamp(trace, sm.scal, ctid);
-            __syncwarp();
-        }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) { // two independent trees, interleaved
             s += __shfl_xor_sync(0xffffffffu, s, o);
             q += __shfl_xor_sync(0xffffffffu, q, o);
         }
-        if ((p.dbg & 2) && trace != nullptr) {
-            if (__double_as_longlong(q) == 0x7ff8000000000001ll) s = 0.0;
-            trace_stamp(trace, sm.scal, ctid);
-        }
-        if (clk) tc1 = clock_after(s, q);
         __syncwarp();
         if (lane < kRep) {
             st_tagged_double(&recs[(size_t)lane * 2 * nb + blockIdx.x], s, tag, false);
             st_tagged_double(&recs[(size_t)lane * 2 * nb + nb + blockIdx.x], q, tag, false);
         }
-        trace_stamp(trace, sm.scal, ctid); // S2: own record published
+        trace_stamp(trace, scal, ctid); // S2: own record published
         // every CTA's record: all in flight at once (r = lane, lane+32, ...), re-read what has not arrived
         constexpr int kPer = (kMaxGrid + 31) / 32;
         const unsigned long long none = tag64(0u, tag);
@@ -648,7 +549,7 @@ __device__ __noinline__ StatsOut slice_stats(const Params &p, const double *xown
             }
         }
         Waiter w = waiter_begin();
-        trace_stamp(trace, sm.scal, ctid); // S3: loads issued
+        trace_stamp(trace, scal, ctid); // S3: loads issued
         for (;;) {
             bool bad = false;
 #pragma unroll
@@ -668,31 +569,18 @@ __device__ __noinline__ StatsOut slice_stats(const Params &p, const double *xown
             if (waiter_tick(p, w)) wait_expired(p, kDiagStats, layer, 0, tag, (unsigned int)(a[0] >> 32), (unsigned long long)lane);
         }
         if (ctid == 0) *quiet = 0u;
-        trace_stamp(trace, sm.scal, ctid); // S4: every record here
+        trace_stamp(trace, scal, ctid); // S4: every record here
         double st = 0.0, qt = 0.0;
 #pragma unroll
         for (int i = 0; i < kPer; ++i) { // ascending record index per lane, then fixed trees: deterministic
             st += pair_to_double(a[i], b[i]);
             qt += pair_to_double(c[i], d[i]);
         }
-        if (clk) tc2 = clock_after(st, qt);
         __syncwarp();
-        if (clk) tc3 = clock_after(st, qt);
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
             st += __shfl_xor_sync(0xffffffffu, st, o);
             qt += __shfl_xor_sync(0xffffffffu, qt, o);
-        }
-        if (clk) {
-            tc4 = clock_after(st, qt);
-            if (lane == 0) {
-                long long *ck = sm.clk + ((layer & 0x8000u) ? 8 : 0); // the debug "cold" call counts separately
-                ck[0] += tc1 - tc0; // first pair of trees
-                ck[1] += tc2 - tc1; // publish + records
-                ck[2] += tc3 - tc2; // __syncwarp
-                ck[3] += tc4 - tc3; // second pair of trees
-                ck[4] += 1;
-            }
         }
         if (lane == 0) {
             const double Ed = (double)p.E;
@@ -702,13 +590,13 @@ __device__ __noinline__ StatsOut slice_stats(const Params &p, const double *xown
             double m2 = qt - 2.0 * dc * (st - Ed * c0) + Ed * dc * dc;
             if (m2 < 0.0) m2 = 0.0;
             const float sd = sqrtf((float)m2 / (float)(p.E - 1));
-            sm.scal[6] = (double)mean_acc / Ed;
-            sm.scal[7] = 1.0 / (double)sd;
+            scal[6] = (double)mean_acc / Ed;
+            scal[7] = 1.0 / (double)sd;
         }
-        trace_stamp(trace, sm.scal, ctid); // S5: statistics computed
+        trace_stamp(trace, scal, ctid); // S5: statistics computed
     }
     own_sync();
-    return StatsOut{sm.scal[6], sm.scal[7]};
+    return StatsOut{scal[6], scal[7]};
 }
 
 // Partial offset sums and the largest |xs| of this CTA's slice (data in the first `nact` consumer threads, NV
@@ -821,12 +709,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_token(const __grid_constant__ P
             mbar_init(smem_u32(&sm.full[i]), 1);
             mbar_init(smem_u32(&sm.empty[i]), kWarps);
         }
-        mbar_init(smem_u32(&sm.cbar[0]), (uint32_t)p.cluster);          // one arrival per CTA of the cluster
-        mbar_init(smem_u32(&sm.cbar[1]), (uint32_t)kWarps);    // the own consumer warps (+ the peers' st.async bytes)
         mbar_fence_init();
     }
     __syncthreads();
-    if (p.cluster > 1) cluster_sync_all(); // the peers' barriers exist before anybody arrives on them
     const int E = p.E, Er = p.Er;
     const int nb = (int)gridDim.x;
     const Slices sl = make_slices(E, Er, p.Vr, (int)blockIdx.x, nb);
@@ -847,10 +732,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_token(const __grid_constant__ P
     if (ctid == 0) {
         *reinterpret_cast<int *>(sm.scal + 8) = 0;
         *reinterpret_cast<int *>(sm.scal + 9) = 0;
-        for (int i = 0; i < 16; ++i) sm.clk[i] = 0;
         for (int i = 0; i < 4; ++i) sm.gmax[i] = 0u;
     }
-    unsigned long long *const c_trace = (TRACE && !(p.dbg & 4)) ? p.trace : nullptr;
+    unsigned long long *const c_trace = TRACE ? p.trace : nullptr;
     auto stamp = [&]() {
         if (TRACE) trace_stamp(c_trace, sm.scal, ctid);
     };
@@ -922,9 +806,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_token(const __grid_constant__ P
 
     double c0 = 0.0; // reference point of the slice statistics: the previous mean (same value on every CTA)
     // Parameters of the slice computation that follows a residual update, parked in this thread's shared
-    // slots: LN1 + att token shift of layer l (l < L_run), or LN_out + head scale (l == L_run).
+    // slots: LN1 + att token shift of layer l (l < L), or LN_out + head scale (l == L).
     auto fetch_ln1 = [&](int l) {
-        if (l < p.L_run) {
+        if (l < p.L) {
             const size_t lo = (size_t)l * E + j;
             cp_async8(pd + 0, p.ln + (size_t)(4 * l + 2) * E + j);
             cp_async8(pd + 1, p.ln + (size_t)(4 * l + 3) * E + j);
@@ -949,12 +833,12 @@ __global__ void __launch_bounds__(kThreads, 1) k_token(const __grid_constant__ P
     // the last layer, LN_out -> publish the head input (rwkv.cu:585-588). Warps 0 and 1.
     auto slice_to_att = [&](int l) {
         const uint32_t ep = p.ep0 + 1u + (uint32_t)l;
-        const StatsOut so1 = slice_stats(p, sm.xown, sm.scal, sm.clk, reinterpret_cast<volatile uint32_t *>(sm.gmax + 3), stat0, ne, ep, (unsigned int)l, ctid, c0, c_trace);
+        const StatsOut so1 = slice_stats(p, sm.xown, sm.scal, reinterpret_cast<volatile uint32_t *>(sm.gmax + 3), stat0, ne, ep, (unsigned int)l, ctid, c0, c_trace);
         const double xmean = so1.mean, rstd = so1.rstd;
         c0 = xmean;
         stamp();
         cp_async_wait();
-        if (l < p.L_run) {
+        if (l < p.L) {
             float *const vec_kvr = reinterpret_cast<float *>(xl + p.off_vec[0]);
             double of[3] = {0, 0, 0};
             uint32_t mx[3] = {0u, 0u, 0u};
@@ -1006,10 +890,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_token(const __grid_constant__ P
     // Phase 3 (ffn R) gathers nothing: its input was quantised together with ffn K's in phase 2 and its result
     // (the sigmoid gate) is needed only after ffn V, so its 2.4 us of streaming run while the relu^2 keys of
     // phase 2 travel to the other CTAs - phase 4's gather finds them in place.
-    const int n_iter = 5 * p.L_run + 1;
-    int l = 0, ph = 0, gk = 0; // layer, phase, gathers so far
+    const int n_iter = 5 * p.L + 1;
+    int l = 0, ph = 0; // layer, phase
     for (int it = 0; it < n_iter; ++it) {
-        if (opaque(it) == 5 * p.L_run) ph = 5;
+        if (opaque(it) == 5 * p.L) ph = 5;
         const int xi = ph < 3 ? ph : ph - 1; // index of the phase's exchange areas (kvr, o, rk, k4, head)
         const size_t lo = (size_t)l * E;
         const uint32_t ep = p.ep0 + 1u + (uint32_t)l;
@@ -1060,10 +944,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_token(const __grid_constant__ P
             if (owner_warps) fetch_ln1(l + 1);
         }
         // -------- gather + stream ------------------------------------------------------------------
-        if (nvec > 0) {
-            gather(p, sm, vec, offrec, maxrec, nvec, N, tag, (unsigned int)l, ctid, gk, c_trace);
-            ++gk;
-        }
+        if (nvec > 0) gather(p, sm, vec, offrec, maxrec, nvec, N, tag, (unsigned int)l, ctid, c_trace);
         {
             const bool exact = FULL && N == nseg * E; // segment == CPL * 512 bytes
             // results: [sub][row]; ffn K's rows sit behind ffn R's (phase 3 fills those while phase 2's are read)
@@ -1076,12 +957,6 @@ __global__ void __launch_bounds__(kThreads, 1) k_token(const __grid_constant__ P
             }
         }
         tok_sync();
-        // this CTA's limb planes may be overwritten - unless the next phase streams against them without a gather
-        // (2 -> 3); nobody gathers after the head
-        if (p.cluster > 1 && ctid == 0 && ph != 2 && ph != 5) {
-            const uint32_t bar = smem_u32(sm.cbar);
-            for (int r = 0; r < p.cluster; ++r) mbar_arrive_remote(mapa(bar, (uint32_t)r));
-        }
         stamp();
         cp_async_wait();
         // -------- epilogue ----------------------------------------------------------------------------
@@ -1127,7 +1002,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_token(const __grid_constant__ P
                     sm.xown[ctid] = (double)xf;
                 }
                 stamp();
-                const StatsOut so2 = slice_stats(p, sm.xown, sm.scal, sm.clk, reinterpret_cast<volatile uint32_t *>(sm.gmax + 3), stat1, ne, ep, (unsigned int)l, ctid, c0, c_trace);
+                const StatsOut so2 = slice_stats(p, sm.xown, sm.scal, reinterpret_cast<volatile uint32_t *>(sm.gmax + 3), stat1, ne, ep, (unsigned int)l, ctid, c0, c_trace);
                 const double xmean = so2.mean, rstd = so2.rstd;
                 c0 = xmean;
                 stamp();
@@ -1315,14 +1190,12 @@ __global__ void __launch_bounds__(kThreads, 1) k_token(const __grid_constant__ P
                     bad = (uint32_t)(a >> 32) != p.tk;
                 }
                 if (!__any_sync(0xffffffffu, bad)) break;
-                if (waiter_tick(p, w)) wait_expired(p, kDiagDone, (unsigned int)p.L_run, (unsigned int)ctid, p.tk, (unsigned int)(a >> 32), 0ull);
+                if (waiter_tick(p, w)) wait_expired(p, kDiagDone, (unsigned int)p.L, (unsigned int)ctid, p.tk, (unsigned int)(a >> 32), 0ull);
             }
             __threadfence_system();
         }
     }
     if (blockIdx.x == 0 && ctid == 0 && p.feed_mode == 2) p.ctrl->pos = p.ctrl->pos + 1;
-    if ((p.dbg & 4) && p.trace != nullptr && ctid == 0)
-        for (int i = 0; i < 16; ++i) p.trace[(size_t)blockIdx.x * kTraceMax + i] = (unsigned long long)sm.clk[i];
     stamp();
 }
 

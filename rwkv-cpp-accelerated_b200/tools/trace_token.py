@@ -33,10 +33,8 @@ if os.path.isdir(out_dir):
 print("stamps per CTA", n, "token time us", (tr[:, -1].max()) / 1e3)
 # stamp layout (token_kernel.cuh): start | ln0+stats, publish | per layer 21 | head 4 | end
 ST = ["st.sync", "st.pub", "st.first", "st.all", "st.calc", "st.ret"]  # slice_stats
-if any(a == "dbg=1" for a in sys.argv[3:]):
-    ST = ["cold." + x for x in ST] + ST
 GA = ["g.meet", "g.words", "g.max", "g.sync", "g.quant"]                    # gather
-names = ["ln0." + x for x in ST if not x.startswith("cold.")] + ["ln0.pub"]
+names = ["ln0." + x for x in ST] + ["ln0.pub"]
 layer = ["kvr." + x for x in GA] + ["kvr.gemv", "kvr.epi"] + \
         ["out." + x for x in GA] + ["out.gemv", "out.resid"] + ["out." + x for x in ST] + ["out.ln2pub"] + \
         ["rk." + x for x in GA] + ["rk.gemv", "rk.epi"] + ["fr.gemv", "fr.epi"] + \

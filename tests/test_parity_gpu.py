@@ -198,6 +198,9 @@ def test_errors(pkg, make_model, tmp_path):
         e.forward([1, 2])  # chunk larger than max_gpt
     with pytest.raises(pkg.EngineError):
         e.forward([50277])  # token out of range
+    for k in ("cluster", "poll_first", "dbg", "issue_gap", "max_layers"):  # removed options
+        with pytest.raises(pkg.EngineError):
+            e.set_option(k, 1)
     e.close()
 
 
@@ -232,30 +235,3 @@ def test_oracle_vs_reference_cuda(pkg, make_model):
         if g["margin"][i] > 1e-3:
             assert int(got.argmax()) == int(g["argmax"][i])
     eng.close()
-
-
-@pytest.mark.parametrize("L,E", [(2, 256), (3, 768), (2, 2048), (2, 4096), (1, 5120)])
-def test_cluster_split_gather_is_bit_identical(pkg, make_model, L, E):
-    """Thread-block clusters split the gather / quantisation and write each other's limb planes through
-    distributed shared memory: the integers, hence the logits, must not change by a bit."""
-    path = make_model(L, E)
-    eng = make_engine(pkg, path)
-    toks = [SEED_TOKEN, 17, 40000, 5, 291, 1023]
-
-    def run():
-        eng.state_zero()
-        return np.stack([eng.forward([t])[0] for t in toks])
-
-    base = run()
-    tried = 0
-    for c in (2, 4):
-        try:
-            eng.set_option("cluster", c)
-        except pkg.EngineError as ex:  # the device cannot hold the grid in clusters of c
-            print("cluster=%d not available: %s" % (c, ex))
-            continue
-        tried += 1
-        got = run()
-        assert np.array_equal(got, base), "cluster=%d changed the logits" % c
-    eng.close()
-    assert tried >= 1

@@ -84,29 +84,6 @@ def test_decode_kernel_matches_oracle(pkg, make_model, E):
 
 
 @pytest.mark.parametrize("E", sorted(WIDTHS))
-def test_cluster_options_are_bit_identical(pkg, make_model, E):
-    eng = pkg.Engine(make_model(L, E))
-    toks = [SEED_TOKEN, 17, 40000, 5, 291, 1023]
-
-    def run():
-        eng.state_zero()
-        return np.stack([eng.forward([t])[0] for t in toks])
-
-    base = run()
-    tried = 0
-    for c in (2, 4):
-        try:
-            eng.set_option("cluster", c)
-        except pkg.EngineError as ex:  # the device cannot hold the grid in clusters of c
-            print("E=%d cluster=%d not available: %s" % (E, c, ex))
-            continue
-        tried += 1
-        assert np.array_equal(run(), base), "E=%d cluster=%d changed the logits" % (E, c)
-    eng.close()
-    assert tried >= 1
-
-
-@pytest.mark.parametrize("E", sorted(WIDTHS))
 def test_gpt_chunk_on_tensor_cores_matches_oracle(pkg, make_model, E):
     """One GPT chunk on the tensor cores against the oracle token by token, against the same call through the decode
     kernel, and the next single token from the chunk's state."""
