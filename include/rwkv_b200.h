@@ -432,6 +432,98 @@ int rwkv_b200_beam_search(rwkv_b200_model *m, const unsigned long long *slots, c
                           double *logprobs_out, double *scores_out, unsigned char *finished_out,
                           double *token_logprobs_out);
 
+/* Continuous batching: a batcher accepts requests at any time between runs and serves them together, so a request that
+ * arrives while others generate starts at the next 16-step group instead of after the whole batch, and the rows freed
+ * by finished requests are refilled at once. A request names a state slot, its prompt (n_prompt >= 1 tokens), max_new
+ * >= 1, a sampler (penalties allowed), u[max_new] (NULL only at temperature 0) and its own stop tokens.
+ *
+ * The rule. For every request, the emitted tokens and the slot's final state are bit for bit what this sequence gives
+ * when the request runs alone from the same slot state, both calls on the tensor cores:
+ *   1. if n_prompt > 1: rwkv_b200_forward_streams of prompt[0 .. n_prompt - 1) on the slot, state only;
+ *   2. rwkv_b200_generate_streams_ex of the one stream (slot, prompt[n_prompt - 1]) with max_new, the request's stop
+ *      tokens, its sampler and its u.
+ * This holds whatever the other requests are, when each was submitted, rows, prefill_tokens, the max_steps of each run,
+ * and any cancellation of other requests. A request's penalty history starts empty at its first emitted token, as in
+ * step 2. A cancelled request's tokens are a prefix of that sequence's tokens. Slots that no unfinished request names
+ * are never written. The rule rests on the ragged-pass invariant: a stream's bits depend only on its own rows and its
+ * own predecessors, and cutting it across passes changes no bit.
+ *
+ * Scheduling (deterministic). A run is a series of groups of 16 steps (the last one of a run may be shorter), with one
+ * synchronisation per group:
+ *   - requests queue FIFO. At a group boundary finished requests leave first; queued requests are then admitted in
+ *     submission order while fewer than `rows` are admitted;
+ *   - an admitted request first prefills prompt[0 .. n_prompt - 1). Each step hands a budget of prefill_tokens prompt
+ *     tokens to the prefilling requests in admission order, each taking as much of its remaining prompt as the budget
+ *     allows, so the pass shape stays the same from step to step while prompt work lasts;
+ *   - a request whose prefill is complete at a group boundary (at admission when n_prompt = 1) has a decode row for the
+ *     whole group; its first input is prompt[n_prompt - 1]. Rows change only at group boundaries, so a request whose
+ *     prefill completes inside a group waits up to 15 steps for its first token. A group without decode rows ends after
+ *     its last step with prompt work;
+ *   - a step is one set of tensor-core passes: the decode rows first (one token each, with logits), then the prefill
+ *     segments (no logits), cut into passes of at most 128 tokens; then penalties, the per-request sampler and the
+ *     feedback that emits each row's token and writes it into the next step's passes.
+ * At each group end the tokens emitted in the group come back, so rwkv_b200_batcher_read between runs sees a growing
+ * prefix (streaming).
+ *
+ * The batcher always runs on the tensor cores: the rule is defined on that path. With only a few generating requests
+ * the decode kernel of rwkv_b200_generate_streams is faster (at 7B: one stream 3.1 ms per step there, a tensor-core step
+ * of 8 streams 10.3 ms, on an H100 SXM 80 GB at a 400 W power limit; tensor-core steps under 8 rows have not been
+ * measured). Not available
+ * in the batcher: logit overrides, token automata, log-probabilities, the typical sampler, admission inside a group,
+ * the decode-kernel path, tensor parallelism, priorities and preemption.
+ *
+ * Other entry points may be called between runs, but must not name a slot held by an unfinished request (queued,
+ * prefilling or generating); the batcher does not police that. rwkv_b200_free closes a model's open batcher, whose handle
+ * is then invalid. */
+typedef struct rwkv_b200_batcher rwkv_b200_batcher;
+typedef struct rwkv_b200_request {
+    unsigned long long slot;
+    const unsigned long long *prompt; /* [n_prompt] */
+    unsigned long long n_prompt;      /* >= 1 */
+    unsigned long long max_new;       /* >= 1 */
+    rwkv_b200_sampler sampler;
+    const double *u;                  /* [max_new] uniforms in [0, 1), or NULL (temperature 0) */
+    const unsigned long long *stop;   /* [n_stop] this request's stop tokens (emitted, not fed) */
+    unsigned long long n_stop;
+} rwkv_b200_request;
+
+#define RWKV_B200_BATCHER_MAX_PREFILL 2048ULL /* prefill_tokens is 1..this */
+
+/* Status of a request (rwkv_b200_batcher_read). */
+#define RWKV_B200_REQ_QUEUED     0
+#define RWKV_B200_REQ_PREFILLING 1 /* admitted, its prompt not yet fed or its decode row not yet begun */
+#define RWKV_B200_REQ_GENERATING 2
+#define RWKV_B200_REQ_DONE       3 /* a stop token or max_new tokens */
+#define RWKV_B200_REQ_CANCELLED  4
+
+/* Open the model's batcher: at most `rows` (1..max_gpt) admitted requests, prefill_tokens (1..
+ * RWKV_B200_BATCHER_MAX_PREFILL) prompt tokens per step. Refused with tensor parallelism, with set_option "prefill" = 0,
+ * and while the model has an open batcher (one per model). The batcher owns its device buffers; it shares only the
+ * model's per-step scratch (logits rows and sampler results). */
+int rwkv_b200_batcher_open(rwkv_b200_model *m, unsigned long long rows, unsigned long long prefill_tokens,
+                           rwkv_b200_batcher **out);
+/* Queue a request; *id receives its id (never 0). Copies every array (the caller may free them afterwards) and does
+ * no device work. Refused: a slot out of range or named by an unfinished request of this batcher, n_prompt or max_new
+ * of 0, a missing array, a token out of range, an invalid sampler (generate_streams_ex's checks), u NULL with a
+ * temperature > 0, and a uniform outside [0, 1). */
+int rwkv_b200_batcher_submit(rwkv_b200_batcher *b, const rwkv_b200_request *r, unsigned long long *id);
+/* Run up to max_steps steps in groups of 16; stops early when nothing is queued or admitted. *steps_run (may be NULL)
+ * receives the steps run. */
+int rwkv_b200_batcher_run(rwkv_b200_batcher *b, unsigned long long max_steps, unsigned long long *steps_run);
+/* The tokens a request has emitted so far: *len receives their count, tokens_out the first min(cap, *len) of them
+ * (tokens_out may be NULL when cap is 0), *status its RWKV_B200_REQ_* status (len and status may be NULL). An unknown
+ * or released id is refused. */
+int rwkv_b200_batcher_read(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *tokens_out,
+                           unsigned long long cap, unsigned long long *len, int *status);
+/* Cancel a queued, prefilling or generating request at once (calls are made between runs). A queued request's slot is
+ * untouched; otherwise the slot holds the state after the tokens fed so far (its emitted tokens but the last one, as
+ * after a stop token). Its tokens stay readable. A done or cancelled request, or an unknown id, is refused. */
+int rwkv_b200_batcher_cancel(rwkv_b200_batcher *b, unsigned long long id);
+/* Forget a done or cancelled request; anything else is refused. */
+int rwkv_b200_batcher_release(rwkv_b200_batcher *b, unsigned long long id);
+/* Close the batcher and free its buffers; unfinished requests are dropped where they stand. NULL is ignored. */
+void rwkv_b200_batcher_close(rwkv_b200_batcher *b);
+
 /* State of one slot: zero it (a new conversation), copy it onto another slot (fork a conversation), or move it
  * between the device and host arrays of n_layers x n_embed doubles each (NULL arrays are skipped). */
 int rwkv_b200_slot_zero(rwkv_b200_model *m, unsigned long long slot);

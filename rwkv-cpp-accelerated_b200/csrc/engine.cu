@@ -19,6 +19,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <deque>
 #include <map>
 #include <new>
 #include <string>
@@ -169,6 +170,39 @@ struct rwkv_b200_model {
         DevBuf<int> n_hyp;                      // [G]
         DevBuf<unsigned long long> done, forks; // [G], [G * B][2]
     } beam;
+    rwkv_b200_batcher *batcher = nullptr; // the open batcher (at most one), closed by rwkv_b200_free
+};
+
+// rwkv_b200_batcher: the requests on the host, and per lane (0..rows-1, one per admitted request, reused) its stream
+// record, sampler, penalty rows, stop tokens and a ring of the current group's tokens on the device. Nothing is shared
+// with m->gen, so a generate_streams call between runs leaves the batcher's requests alone.
+struct rwkv_b200_batcher {
+    rwkv_b200_model *m = nullptr;
+    int rows = 0, prefill_tokens = 0, max_pass = 0; // max_pass: passes of a step at most
+    struct Req {
+        unsigned long long slot = 0, max_new = 0;
+        std::vector<unsigned long long> prompt, stop, tokens; // tokens: emitted so far
+        std::vector<double> u;                                // empty: temperature 0
+        rwkv_b200_sampler sampler{};
+        int status = RWKV_B200_REQ_QUEUED;
+        unsigned long long fed = 0; // tokens of prompt[0 .. n_prompt - 1) in the slot
+        int lane = -1;
+    };
+    std::map<unsigned long long, Req> reqs;
+    unsigned long long next_id = 1;
+    std::deque<unsigned long long> queue;     // queued ids, submission order
+    std::vector<unsigned long long> admitted; // admitted ids, admission order
+    std::vector<char> lane_used;              // [rows]
+    std::vector<rk::GenStream> h_gs;          // [rows] host mirror of the lanes' records
+    std::vector<unsigned long long> h_out;    // [rows][kGenGroup]
+    DevBuf<rk::GenStream> gs;                 // [rows]
+    DevBuf<int> row_stream;                   // [rows] lane of each decode row
+    DevBuf<rk::PassDesc> passes;              // [kGenGroup][max_pass] the layouts of a group's steps
+    DevBuf<rwkv_b200_sampler> samp;           // [rows]
+    DevBuf<float> pen_cnt;                    // [rows][V] (allocated at the first request with penalties)
+    DevBuf<unsigned char> pen_seen;           // [rows][V]
+    DevBuf<unsigned long long> stop, stop_start, out; // lanes' stop tokens (CSR), [rows + 1], [rows][kGenGroup]
+    DevBuf<double> u;                         // [kGenGroup][rows] uniforms of the current group
 };
 
 namespace {
@@ -1162,6 +1196,199 @@ int beam(M *m, const unsigned long long *slots, const unsigned long long *first_
     return 0;
 }
 
+using B = rwkv_b200_batcher;
+
+int check_batcher(const B *b) {
+    if (!b) return fail(1, "null batcher handle");
+    return check_model(b->m);
+}
+
+// A group boundary (the previous group's finished requests have left): queued requests are admitted in submission
+// order while fewer than `rows` are admitted (each takes the lowest free lane: its record, sampler and penalty rows are
+// reset), and every admitted request whose prefill is complete gets its decode row's record. Returns the decode rows'
+// lanes in admission order.
+int batcher_boundary(B *b, std::vector<int> &dec) {
+    M *m = b->m;
+    const size_t V = binfmt::kVocab;
+    auto &ad = b->admitted;
+    while (!b->queue.empty() && ad.size() < (size_t)b->rows) {
+        const unsigned long long id = b->queue.front();
+        b->queue.pop_front();
+        B::Req &q = b->reqs[id];
+        q.lane = (int)(std::find(b->lane_used.begin(), b->lane_used.end(), 0) - b->lane_used.begin());
+        b->lane_used[q.lane] = 1;
+        q.status = RWKV_B200_REQ_PREFILLING;
+        ad.push_back(id);
+        CK(cudaMemcpyAsync(b->samp.p + q.lane, &q.sampler, sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
+        if (q.sampler.presence_penalty != 0.0f || q.sampler.frequency_penalty != 0.0f) {
+            int rc;
+            if ((rc = b->pen_cnt.grow((size_t)b->rows * V)) || (rc = b->pen_seen.grow((size_t)b->rows * V))) return rc;
+            CK(cudaMemsetAsync(b->pen_cnt.p + (size_t)q.lane * V, 0, V * sizeof(float), m->stream));
+            CK(cudaMemsetAsync(b->pen_seen.p + (size_t)q.lane * V, 0, V, m->stream));
+        }
+    }
+    dec.clear();
+    for (unsigned long long id : ad) {
+        B::Req &q = b->reqs[id];
+        if (q.status == RWKV_B200_REQ_PREFILLING && q.fed + 1 == q.prompt.size()) {
+            q.status = RWKV_B200_REQ_GENERATING;
+            b->h_gs[q.lane] = rk::GenStream{q.slot, q.max_new, q.prompt.back(), 0, 0};
+        }
+        if (q.status == RWKV_B200_REQ_GENERATING) dec.push_back(q.lane);
+    }
+    // the lanes' stop tokens, in CSR over the lanes
+    std::vector<unsigned long long> start(b->rows + 1, 0), stop;
+    for (int l = 0; l < b->rows; ++l) {
+        start[l] = stop.size();
+        for (unsigned long long id : ad)
+            if (b->reqs[id].lane == l) stop.insert(stop.end(), b->reqs[id].stop.begin(), b->reqs[id].stop.end());
+    }
+    start[b->rows] = stop.size();
+    int rc;
+    if ((rc = b->stop.grow(stop.size()))) return rc;
+    if (!stop.empty())
+        CK(cudaMemcpyAsync(b->stop.p, stop.data(), stop.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemcpyAsync(b->stop_start.p, start.data(), start.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    return 0;
+}
+
+// One group of at most `max_steps` steps (<= kGenGroup); *ran receives its length. The host lays out every step's
+// passes in advance (prefill never depends on a pick) and uploads them once; the feedback of step k writes the decode
+// rows' tokens and kDescLast bits into step k + 1's layout.
+int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
+    M *m = b->m;
+    const size_t V = binfmt::kVocab;
+    std::vector<int> dec;
+    int rc = batcher_boundary(b, dec);
+    if (rc) return rc;
+    *ran = 0;
+    if (b->admitted.empty()) return 0;
+    const int R = (int)dec.size();
+    // the prefill segments of each step: the budget goes to the prefilling requests in admission order
+    struct Seg {
+        unsigned long long id, off, n;
+    };
+    std::vector<std::vector<Seg>> segs;
+    std::map<unsigned long long, unsigned long long> fed;
+    for (unsigned long long id : b->admitted)
+        if (b->reqs[id].status == RWKV_B200_REQ_PREFILLING) fed[id] = b->reqs[id].fed;
+    for (unsigned long long k = 0; k < max_steps; ++k) {
+        std::vector<Seg> s;
+        unsigned long long budget = (unsigned long long)b->prefill_tokens;
+        for (unsigned long long id : b->admitted) {
+            const B::Req &q = b->reqs[id];
+            if (q.status != RWKV_B200_REQ_PREFILLING || budget == 0) continue;
+            const unsigned long long take = std::min(budget, q.prompt.size() - 1 - fed[id]);
+            if (take == 0) continue;
+            s.push_back(Seg{id, fed[id], take});
+            fed[id] += take;
+            budget -= take;
+        }
+        if (R == 0 && s.empty()) break; // nothing left for this group's steps to do
+        segs.push_back(std::move(s));
+    }
+    const unsigned long long steps = segs.size();
+    // every step's layout: decode rows (head rows 0..R-1), then the segments without a head
+    std::vector<rk::PassDesc> all(steps * (size_t)b->max_pass);
+    std::vector<std::vector<int>> T(steps), H(steps);
+    for (unsigned long long k = 0; k < steps; ++k) {
+        std::vector<unsigned long long> tokens, slots, lens;
+        std::vector<unsigned char> head;
+        for (int r = 0; r < R; ++r) {
+            tokens.push_back(b->h_gs[dec[r]].tok); // steps > 0: the feedback writes the pick over it
+            slots.push_back(b->h_gs[dec[r]].slot);
+            lens.push_back(1);
+            head.push_back(1);
+        }
+        for (const Seg &s : segs[k]) {
+            const B::Req &q = b->reqs[s.id];
+            tokens.insert(tokens.end(), q.prompt.begin() + (long)s.off, q.prompt.begin() + (long)(s.off + s.n));
+            slots.push_back(q.slot);
+            lens.push_back(s.n);
+            head.push_back(0);
+        }
+        const int n = (int)tokens.size();
+        std::vector<rk::PassDesc> passes;
+        rk::pass_layout(tokens.data(), n, slots.data(), lens.data(), 2, nullptr, passes, H[k], head.data());
+        for (size_t i = 0; i < passes.size(); ++i) {
+            all[k * b->max_pass + i] = passes[i];
+            T[k].push_back(std::min(rk::kPfMaxTokens, n - (int)i * rk::kPfMaxTokens));
+        }
+    }
+    CK(cudaMemcpyAsync(b->passes.p, all.data(), all.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
+    bool pen = false;
+    if (R > 0) {
+        CK(cudaMemcpyAsync(b->gs.p, b->h_gs.data(), b->rows * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(b->row_stream.p, dec.data(), R * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        // uniforms [steps][R]: row r at step k draws with its request's u[len + k]
+        std::vector<const B::Req *> of_lane(b->rows, nullptr);
+        for (unsigned long long id : b->admitted) of_lane[b->reqs[id].lane] = &b->reqs[id];
+        std::vector<double> ug(steps * (size_t)R, 0.0);
+        for (int r = 0; r < R; ++r) {
+            const rk::GenStream &g = b->h_gs[dec[r]];
+            const B::Req &q = *of_lane[dec[r]];
+            for (unsigned long long k = 0; k < steps && !q.u.empty(); ++k)
+                if (g.len + k < q.max_new) ug[k * R + r] = q.u[g.len + k];
+            pen |= q.sampler.presence_penalty != 0.0f || q.sampler.frequency_penalty != 0.0f;
+        }
+        CK(cudaMemcpyAsync(b->u.p, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+    }
+    const unsigned rb = (unsigned)((R + 127) / 128);
+    for (unsigned long long k = 0; k < steps; ++k) {
+        const rk::PassDesc *step = b->passes.p + k * b->max_pass;
+        for (size_t i = 0; i < T[k].size(); ++i) {
+            CK(cudaMemcpyAsync(m->pf.pass, step + i, sizeof(rk::PassDesc), cudaMemcpyDeviceToDevice, m->stream));
+            if ((rc = rk::prefill_run(m->pf, m->p, m->stream, T[k][i], H[k][i], m->d_slogits))) return fail(rc, "%s", rk::prefill_error());
+        }
+        m->launches += rk::prefill_launches(m->pf);
+        if (R == 0) continue;
+        if (pen) {
+            const dim3 grid((unsigned)((V + rk::kPenaltyThreads - 1) / rk::kPenaltyThreads), (unsigned)R);
+            rk::k_gen_penalty<<<grid, rk::kPenaltyThreads, 0, m->stream>>>(m->d_slogits, (int)V, b->gs.p, b->row_stream.p, b->samp.p,
+                                                                          b->pen_cnt.p, b->pen_seen.p);
+            CK(cudaGetLastError());
+            m->launches += 1;
+        }
+        rk::k_sample_nucleus<<<(unsigned)R, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, b->samp.p, b->row_stream.p,
+                                                                              b->u.p + k * R, m->d_sample);
+        CK(cudaGetLastError());
+        rk::GenFeedbackArgs fb{b->gs.p, b->row_stream.p, R, nullptr, m->d_sample, b->stop.p, 0, b->out.p, kGenGroup,
+                               k + 1 < steps ? b->passes.p + (k + 1) * b->max_pass : nullptr, nullptr, nullptr,
+                               b->stop_start.p};
+        rk::k_gen_feedback<<<rb, 128, 0, m->stream>>>(fb);
+        CK(cudaGetLastError());
+        m->launches += 2;
+    }
+    // the group's end: the lanes' records and the tokens of the group come back with one synchronisation
+    if (R > 0) {
+        CK(cudaMemcpyAsync(b->h_gs.data(), b->gs.p, b->rows * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(b->h_out.data(), b->out.p, b->h_out.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+    }
+    SYNC(m);
+    for (unsigned long long id : b->admitted) {
+        B::Req &q = b->reqs[id];
+        if (q.status == RWKV_B200_REQ_PREFILLING) {
+            q.fed = fed[id];
+            continue;
+        }
+        const rk::GenStream &g = b->h_gs[q.lane];
+        for (unsigned long long j = q.tokens.size(); j < g.len; ++j) q.tokens.push_back(b->h_out[(size_t)q.lane * kGenGroup + j % kGenGroup]);
+        if (g.done) q.status = RWKV_B200_REQ_DONE;
+    }
+    // finished requests leave here, before the next boundary admits anyone (a caller may release them in between)
+    auto &ad = b->admitted;
+    ad.erase(std::remove_if(ad.begin(), ad.end(),
+                            [&](unsigned long long id) {
+                                const B::Req &q = b->reqs.at(id);
+                                if (q.status != RWKV_B200_REQ_DONE) return false;
+                                b->lane_used[q.lane] = 0;
+                                return true;
+                            }),
+             ad.end());
+    *ran = steps;
+    return 0;
+}
+
 } // namespace
 
 // =================================================================================================
@@ -1216,6 +1443,7 @@ void rwkv_b200_free(rwkv_b200_model *m) {
     if (!m) return;
     cudaSetDevice(m->device);
     if (m->stream) cudaStreamSynchronize(m->stream);
+    rwkv_b200_batcher_close(m->batcher);
     rk::prefill_free(m->pf);
     for (void *p : m->ipc_opened) cudaIpcCloseMemHandle(p);
     for (void *p : m->allocs) cudaFree(p);
@@ -1739,6 +1967,142 @@ int rwkv_b200_slot_download(rwkv_b200_model *m, unsigned long long slot, double 
     return 0;
 }
 
+int rwkv_b200_batcher_open(rwkv_b200_model *m, unsigned long long rows, unsigned long long prefill_tokens,
+                           rwkv_b200_batcher **out) {
+    const char *what = "batcher_open";
+    int rc = check_streams_model(m, what);
+    if (rc) return rc;
+    if (!out) return fail(1, "%s: out is NULL", what);
+    *out = nullptr;
+    if (rows == 0 || rows > m->max_gpt) return fail(1, "%s: rows %llu is outside 1..max_gpt = %llu", what, rows, m->max_gpt);
+    if (prefill_tokens == 0 || prefill_tokens > RWKV_B200_BATCHER_MAX_PREFILL)
+        return fail(1, "%s: prefill_tokens %llu is outside 1..%llu", what, prefill_tokens, RWKV_B200_BATCHER_MAX_PREFILL);
+    if (!rk::prefill_enabled(m->pf)) return fail(1, "%s: the batcher runs on the tensor cores, and \"prefill\" is 0", what);
+    if (m->batcher) return fail(1, "%s: the model already has an open batcher", what);
+    CK(cudaSetDevice(m->device));
+    if ((rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
+    B *b = new B;
+    b->m = m;
+    b->rows = (int)rows;
+    b->prefill_tokens = (int)prefill_tokens;
+    b->max_pass = (int)((rows + prefill_tokens + rk::kPfMaxTokens - 1) / rk::kPfMaxTokens);
+    b->lane_used.assign(rows, 0);
+    b->h_gs.assign(rows, rk::GenStream{});
+    b->h_out.assign(rows * kGenGroup, 0);
+    if ((rc = b->gs.grow(rows)) || (rc = b->row_stream.grow(rows)) || (rc = b->passes.grow(kGenGroup * (size_t)b->max_pass)) ||
+        (rc = b->samp.grow(rows)) || (rc = b->stop_start.grow(rows + 1)) || (rc = b->out.grow(rows * kGenGroup)) ||
+        (rc = b->u.grow(kGenGroup * rows))) {
+        delete b;
+        return rc;
+    }
+    m->batcher = b;
+    *out = b;
+    return 0;
+}
+
+int rwkv_b200_batcher_submit(rwkv_b200_batcher *b, const rwkv_b200_request *r, unsigned long long *id) {
+    const char *what = "batcher_submit";
+    int rc = check_batcher(b);
+    if (rc) return rc;
+    if (!r || !id) return fail(1, "%s: null argument (the request and id are required)", what);
+    if (r->n_prompt == 0 || !r->prompt) return fail(1, "%s: no prompt (n_prompt >= 1 tokens are required)", what);
+    if (r->max_new == 0) return fail(1, "%s: max_new is 0", what);
+    if (r->n_stop && !r->stop) return fail(1, "%s: n_stop = %llu with NULL stop", what, r->n_stop);
+    const unsigned long long s = b->next_id; // the id it would get names it in messages
+    if ((rc = check_slot(b->m, what, r->slot)) || (rc = check_tokens(what, "prompt token", r->prompt, r->n_prompt)) ||
+        (rc = check_tokens(what, "stop token", r->stop, r->n_stop)) || (rc = check_sampler(what, s, r->sampler, true)))
+        return rc;
+    if (r->sampler.temperature > 0.0f && !r->u)
+        return fail(1, "%s: u is NULL but stream %llu samples (temperature %g)", what, s, r->sampler.temperature);
+    for (unsigned long long i = 0; r->u && i < r->max_new; ++i)
+        if (!(r->u[i] >= 0.0 && r->u[i] < 1.0)) return fail(1, "%s: u[%llu] = %g is outside [0, 1)", what, i, r->u[i]);
+    for (const auto &e : b->reqs)
+        if (e.second.slot == r->slot && e.second.status <= RWKV_B200_REQ_GENERATING)
+            return fail(1, "%s: slot %llu is held by unfinished request %llu", what, r->slot, e.first);
+    B::Req q;
+    q.slot = r->slot;
+    q.max_new = r->max_new;
+    q.prompt.assign(r->prompt, r->prompt + r->n_prompt);
+    if (r->n_stop) q.stop.assign(r->stop, r->stop + r->n_stop);
+    if (r->u) q.u.assign(r->u, r->u + r->max_new);
+    q.sampler = r->sampler;
+    b->reqs[s] = std::move(q);
+    b->queue.push_back(s);
+    b->next_id += 1;
+    *id = s;
+    return 0;
+}
+
+int rwkv_b200_batcher_run(rwkv_b200_batcher *b, unsigned long long max_steps, unsigned long long *steps_run) {
+    int rc = check_batcher(b);
+    if (rc) return rc;
+    if (steps_run) *steps_run = 0;
+    if (!rk::prefill_enabled(b->m->pf)) return fail(1, "batcher_run: the batcher runs on the tensor cores, and \"prefill\" is 0");
+    CK(cudaSetDevice(b->m->device));
+    b->m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
+    for (unsigned long long done = 0; done < max_steps;) {
+        unsigned long long ran = 0;
+        if ((rc = batcher_group(b, std::min(kGenGroup, max_steps - done), &ran))) return rc;
+        if (ran == 0) break;
+        done += ran;
+        if (steps_run) *steps_run = done;
+    }
+    return 0;
+}
+
+int rwkv_b200_batcher_read(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *tokens_out, unsigned long long cap,
+                           unsigned long long *len, int *status) {
+    int rc = check_batcher(b);
+    if (rc) return rc;
+    const auto it = b->reqs.find(id);
+    if (it == b->reqs.end()) return fail(1, "batcher_read: request %llu is unknown or released", id);
+    const B::Req &q = it->second;
+    if (cap && !tokens_out) return fail(1, "batcher_read: cap = %llu with NULL tokens_out", cap);
+    const size_t n = std::min<size_t>(cap, q.tokens.size());
+    if (n) memcpy(tokens_out, q.tokens.data(), n * sizeof(unsigned long long));
+    if (len) *len = q.tokens.size();
+    if (status) *status = q.status;
+    return 0;
+}
+
+int rwkv_b200_batcher_cancel(rwkv_b200_batcher *b, unsigned long long id) {
+    int rc = check_batcher(b);
+    if (rc) return rc;
+    const auto it = b->reqs.find(id);
+    if (it == b->reqs.end()) return fail(1, "batcher_cancel: request %llu is unknown or released", id);
+    B::Req &q = it->second;
+    if (q.status > RWKV_B200_REQ_GENERATING) return fail(1, "batcher_cancel: request %llu has already ended", id);
+    if (q.status == RWKV_B200_REQ_QUEUED) {
+        b->queue.erase(std::find(b->queue.begin(), b->queue.end(), id));
+    } else {
+        b->admitted.erase(std::find(b->admitted.begin(), b->admitted.end(), id));
+        b->lane_used[q.lane] = 0;
+    }
+    q.status = RWKV_B200_REQ_CANCELLED;
+    return 0;
+}
+
+int rwkv_b200_batcher_release(rwkv_b200_batcher *b, unsigned long long id) {
+    int rc = check_batcher(b);
+    if (rc) return rc;
+    const auto it = b->reqs.find(id);
+    if (it == b->reqs.end()) return fail(1, "batcher_release: request %llu is unknown or released", id);
+    if (it->second.status <= RWKV_B200_REQ_GENERATING)
+        return fail(1, "batcher_release: request %llu has not ended (cancel it first)", id);
+    b->reqs.erase(it);
+    return 0;
+}
+
+void rwkv_b200_batcher_close(rwkv_b200_batcher *b) {
+    if (!b) return;
+    if (b->m) {
+        cudaSetDevice(b->m->device);
+        cudaStreamSynchronize(b->m->stream);
+        b->m->batcher = nullptr;
+    }
+    delete b;
+}
+
 int rwkv_b200_decode_timed(rwkv_b200_model *m, const unsigned long long *tokens, unsigned long long n,
                            int teacher_forced, float *ms) {
     int rc = check_model(m);
@@ -1873,6 +2237,11 @@ long long rwkv_b200_debug_read(rwkv_b200_model *m, const char *name, void *dst, 
     if (check_model(m) || !name || !dst) return -1;
     cudaSetDevice(m->device);
     const std::string k = name;
+    if (k == "graph_records") { // tensor-core pass graphs recorded since load (a host counter)
+        if (dst_bytes < sizeof(unsigned long long)) return -1;
+        memcpy(dst, &m->pf.records, sizeof(unsigned long long));
+        return 1;
+    }
     const void *src = nullptr;
     size_t bytes = 0, count = 0;
     const size_t E = m->E;

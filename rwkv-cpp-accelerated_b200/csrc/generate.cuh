@@ -73,18 +73,24 @@ struct GenFeedbackArgs {
     int rows;
     const unsigned long long *next;  // arg-max per row, or nullptr when sampling
     const double *sample;            // {token, margin} per row when sampling
-    const unsigned long long *stop;  // [n_stop]
+    const unsigned long long *stop;  // [n_stop], or the tokens stop_start indexes
     int n_stop;
-    unsigned long long *out;         // [n_streams][max_new]
+    unsigned long long *out;         // [n_streams][max_new]: token k of stream s at [s][k % max_new]
     unsigned long long max_new;
     PassDesc *passes;                // tensor-core path: the descriptors of the next step, else nullptr
     GenConstraint *gc;               // [n_streams] generate_streams_constrained, else nullptr
     unsigned long long *fault;       // {stream + 1, token, state} of the first emitted token without an edge (gc only)
+    // the batcher: stream s's own stop tokens are stop[stop_start[s] .. stop_start[s + 1]) (n_stop is not read);
+    // nullptr: stop[0 .. n_stop) for every stream
+    const unsigned long long *stop_start;
 };
 
 // One thread per row: emit the picked token of a live stream, then write the next step's input. On the tensor-core
 // path that is the row's token and descriptor in its pass; a finished stream loses kDescLast, so no pass stores its
-// slot again.
+// slot again. `passes` is the next step's layout, whose row r is token r (the rows lead every pass set); the batcher
+// passes each step the layout of the step after it, since their prefill tokens differ. A generate_streams call emits at
+// most max_new tokens per stream, so `% max_new` leaves its index alone; a batcher lane keeps one group's tokens in a
+// ring of kGenGroup entries.
 __global__ void k_gen_feedback(const GenFeedbackArgs a) {
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= a.rows) return;
@@ -92,11 +98,15 @@ __global__ void k_gen_feedback(const GenFeedbackArgs a) {
     GenStream g = a.gs[s];
     if (!g.done) {
         const unsigned long long tok = a.next ? a.next[r] : (unsigned long long)a.sample[2 * r];
-        a.out[(size_t)s * a.max_new + g.len] = tok;
+        a.out[(size_t)s * a.max_new + g.len % a.max_new] = tok;
         g.len += 1;
         g.tok = tok;
         bool stop = g.len == g.budget;
-        for (int i = 0; i < a.n_stop; ++i) stop |= a.stop[i] == tok;
+        if (a.stop_start) {
+            for (unsigned long long i = a.stop_start[s]; i < a.stop_start[s + 1]; ++i) stop |= a.stop[i] == tok;
+        } else {
+            for (int i = 0; i < a.n_stop; ++i) stop |= a.stop[i] == tok;
+        }
         if (a.gc && a.gc[s].mask) {
             // advance the automaton; a state without edges completes it. The mask makes a missing edge impossible
             // unless the pick broke its contract: record it for the host and end the stream

@@ -485,6 +485,7 @@ struct PrefillState {
     };
     std::vector<Graph> graphs;
     bool use_graph = true;
+    unsigned long long records = 0; // graphs recorded since load (a shape that left the cache is recorded again)
 };
 inline std::string &prefill_err_slot() {
     static thread_local std::string e;
@@ -721,6 +722,7 @@ inline int prefill_run(PrefillState &s, const Params &p, cudaStream_t st, int T,
             s.graphs.erase(s.graphs.begin());
         }
         s.graphs.push_back(PrefillState::Graph{T, H, exec, n});
+        s.records += 1;
         g = &s.graphs.back();
     }
     if (g) {
@@ -737,9 +739,12 @@ inline int prefill_run(PrefillState &s, const Params &p, cudaStream_t st, int T,
 // crosses a cut is "last" in one pass and "first" in the next. head = 0: state only. head = 1: logits of every token,
 // row t of the logits. head = 2: logits of each stream's final token, row i for stream i (only the pass holding that
 // token runs the head for it). `need` (head 1 only, may be NULL): a pass none of whose tokens has need[t] set runs no
-// head, so its logits rows are not written. Fills each pass's descriptor (zero past its last token) and head row count.
+// head, so its logits rows are not written. `stream_head` (head 2 only, may be NULL = every stream): only a stream with
+// stream_head[i] set gets a head row, and its logits row counts the headed streams before it (the batcher's decode rows,
+// followed by prefill segments without logits). Fills each pass's descriptor (zero past its last token) and head row count.
 inline void pass_layout(const unsigned long long *tokens, int n, const unsigned long long *slots, const unsigned long long *lens,
-                        int head, const unsigned char *need, std::vector<PassDesc> &passes, std::vector<int> &heads) {
+                        int head, const unsigned char *need, std::vector<PassDesc> &passes, std::vector<int> &heads,
+                        const unsigned char *stream_head = nullptr) {
     passes.assign((size_t)(n + kPfMaxTokens - 1) / kPfMaxTokens, PassDesc{});
     heads.assign(passes.size(), 0);
     int stream = 0, pos = 0;  // current stream, index of the next token inside it
@@ -757,10 +762,11 @@ inline void pass_layout(const unsigned long long *tokens, int n, const unsigned 
                 pos = 0;
             }
             const bool fin = pos + 1 == (int)lens[stream];
+            const bool headed = fin && (!stream_head || stream_head[stream]);
             h.tokens[t] = tokens[t0 + t];
             h.desc[t] = (uint32_t)slots[stream] | (pos == 0 || t == 0 ? kDescFirst : 0u) | (fin || t == T - 1 ? kDescLast : 0u);
-            if (head == 1 || (head == 2 && fin)) h.rows[H++] = t;
-            if (fin) ++ended;
+            if (head == 1 || (head == 2 && headed)) h.rows[H++] = t;
+            if (headed) ++ended;
             ++pos;
         }
         heads[i] = needed ? H : 0;

@@ -36,6 +36,17 @@ class Sampler(ctypes.Structure):
         super().__init__(temperature, top_p, top_k, presence_penalty, frequency_penalty, penalty_decay)
 
 
+class Request(ctypes.Structure):
+    """rwkv_b200_request: one request of a Batcher."""
+    P = ctypes.POINTER(ctypes.c_ulonglong)
+    _fields_ = [("slot", ctypes.c_ulonglong), ("prompt", P), ("n_prompt", ctypes.c_ulonglong),
+                ("max_new", ctypes.c_ulonglong), ("sampler", Sampler), ("u", ctypes.POINTER(ctypes.c_double)),
+                ("stop", P), ("n_stop", ctypes.c_ulonglong)]
+
+
+REQ_STATUS = ("queued", "prefilling", "generating", "done", "cancelled")  # RWKV_B200_REQ_* in order
+
+
 def _samplers(spec, n):
     """One Sampler (or dict of its fields) for all n streams, or a sequence of n of them, as a ctypes array."""
     one = lambda x: x if isinstance(x, Sampler) else Sampler(**x)
@@ -132,6 +143,13 @@ def load_library():
                                                          pull, pdbl, pull, pull, pull]),
         "rwkv_b200_beam_search": (i32, [vp, pull, pull, ull, c.c_uint, ull, pull, ull, c.c_double, c.c_uint, pull, pull, pdbl,
                                         pdbl, c.POINTER(c.c_ubyte), pdbl]),
+        "rwkv_b200_batcher_open": (i32, [vp, ull, ull, c.POINTER(vp)]),
+        "rwkv_b200_batcher_submit": (i32, [vp, c.POINTER(Request), pull]),
+        "rwkv_b200_batcher_run": (i32, [vp, ull, pull]),
+        "rwkv_b200_batcher_read": (i32, [vp, ull, pull, ull, pull, c.POINTER(i32)]),
+        "rwkv_b200_batcher_cancel": (i32, [vp, ull]),
+        "rwkv_b200_batcher_release": (i32, [vp, ull]),
+        "rwkv_b200_batcher_close": (None, [vp]),
         "rwkv_b200_slot_zero": (i32, [vp, ull]),
         "rwkv_b200_slot_copy": (i32, [vp, ull, ull]),
         "rwkv_b200_slot_upload": (i32, [vp, ull, pdbl, pdbl, pdbl, pdbl, pdbl]),
@@ -457,6 +475,11 @@ class Engine:
             res.append(hyps)
         return res
 
+    def batcher(self, rows, prefill_tokens):
+        """Continuous batching (include/rwkv_b200.h, rwkv_b200_batcher_open): a Batcher with at most `rows` admitted
+        requests and `prefill_tokens` prompt tokens per step."""
+        return Batcher(self, rows, prefill_tokens)
+
     def slot_zero(self, slot):
         self._ck(self.lib.rwkv_b200_slot_zero(self.h, slot), "slot_zero")
 
@@ -543,3 +566,65 @@ class Engine:
     @property
     def launch_count(self):
         return int(self.lib.rwkv_b200_launch_count(self.h))
+
+
+class Batcher:
+    """Continuous batching on one Engine (include/rwkv_b200.h, "Continuous batching"): submit requests at any time
+    between runs, run them in groups of 16 steps, read each request's tokens as they grow. A context manager; close()
+    frees it (the engine keeps at most one open batcher)."""
+
+    def __init__(self, engine, rows, prefill_tokens):
+        self.engine, self.lib = engine, engine.lib
+        h = ctypes.c_void_p()
+        engine._ck(self.lib.rwkv_b200_batcher_open(engine.h, int(rows), int(prefill_tokens), ctypes.byref(h)),
+                   "batcher_open")
+        self.h = h
+
+    def submit(self, slot, prompt, max_new, sampling=None, u=None, stop=()):
+        """Queue a request on state slot `slot`: prompt (>= 1 token ids), up to max_new new tokens, a Sampler or dict
+        (None: arg-max), u: max_new uniforms in [0, 1) (None only at temperature 0), stop: this request's stop tokens.
+        Returns its id. Every array is copied."""
+        sp = _samplers(sampling if sampling is not None else Sampler(temperature=0.0), 1)[0]
+        pr = np.ascontiguousarray(np.atleast_1d(np.asarray(prompt, dtype=np.uint64)))
+        st = np.ascontiguousarray(list(stop), dtype=np.uint64)
+        us = np.ascontiguousarray(u, dtype=np.float64) if u is not None else None
+        if us is not None and us.shape != (int(max_new),):
+            raise EngineError("batcher.submit: u has shape %s, expected (%d,)" % (us.shape, int(max_new)))
+        P = ctypes.c_ulonglong
+        req = Request(int(slot), _ptr(pr, P), len(pr), int(max_new), sp, _ptr(us, ctypes.c_double), _ptr(st, P), len(st))
+        rid = ctypes.c_ulonglong()
+        self.engine._ck(self.lib.rwkv_b200_batcher_submit(self.h, ctypes.byref(req), ctypes.byref(rid)), "batcher_submit")
+        return int(rid.value)
+
+    def run(self, max_steps):
+        """Run up to max_steps steps (groups of 16); returns the steps run (fewer when everything has finished)."""
+        n = ctypes.c_ulonglong()
+        self.engine._ck(self.lib.rwkv_b200_batcher_run(self.h, int(max_steps), ctypes.byref(n)), "batcher_run")
+        return int(n.value)
+
+    def read(self, rid):
+        """(tokens emitted so far as np.uint64, status): status is one of REQ_STATUS."""
+        n, status = ctypes.c_ulonglong(), ctypes.c_int()
+        self.engine._ck(self.lib.rwkv_b200_batcher_read(self.h, int(rid), None, 0, ctypes.byref(n), ctypes.byref(status)),
+                        "batcher_read")
+        out = np.zeros(int(n.value), np.uint64)
+        self.engine._ck(self.lib.rwkv_b200_batcher_read(self.h, int(rid), _ptr(out, ctypes.c_ulonglong), len(out), None, None),
+                        "batcher_read")
+        return out, REQ_STATUS[status.value]
+
+    def cancel(self, rid):
+        self.engine._ck(self.lib.rwkv_b200_batcher_cancel(self.h, int(rid)), "batcher_cancel")
+
+    def release(self, rid):
+        self.engine._ck(self.lib.rwkv_b200_batcher_release(self.h, int(rid)), "batcher_release")
+
+    def close(self):
+        if getattr(self, "h", None) and getattr(self.engine, "h", None):
+            self.lib.rwkv_b200_batcher_close(self.h)
+        self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()

@@ -1,0 +1,303 @@
+"""Continuous batching (rwkv_b200_batcher_*) against each request run alone through the existing API.
+
+The oracle is a second engine that starts from the same state and runs, per request, the two calls the batcher's rule
+names, both on the tensor cores (prefill_min = 2): forward_streams of prompt[:-1] (state only), then
+generate_streams_ex of (slot, prompt[-1]) with the request's max_new, stop tokens, sampler and uniforms. A call that
+would have fewer than 2 tokens gets a pad stream on a spare slot; rows are independent, so the pad changes nothing (the
+call-wide stop tokens apply to the pad too, which is harmless). Tokens and every named slot must be bit-equal to the
+oracle whatever the schedule, and slots no request names must not change at all."""
+import numpy as np
+import pytest
+
+pytestmark = pytest.mark.gpu
+
+V = 50277
+KEYS = ("xy", "aa", "bb", "pp", "dd")
+SHAPES = [(3, 768), (2, 2048)]
+MAX_GPT = 320      # the longest prompt (300 tokens) is one forward_streams call of the oracle
+PAD = MAX_GPT - 1  # never named by a request
+LENGTHS = (1, 2, 31, 32, 33, 127, 128, 129, 300)
+
+
+def slot_of(state, slot, n):
+    return {k: state[k][slot * n:(slot + 1) * n] for k in state}
+
+
+def samplers(pkg):
+    S = pkg.Sampler
+    return [S(temperature=0.0), S(temperature=0.8, top_p=0.9), S(temperature=1.0, top_k=40, presence_penalty=0.6,
+            frequency_penalty=0.3, penalty_decay=0.95), S(temperature=0.0, presence_penalty=2.0, frequency_penalty=1.0)]
+
+
+def make_requests(pkg, n, seed, slots):
+    """n requests on the given distinct slots: every prompt length of LENGTHS, a mix of samplers."""
+    rng = np.random.default_rng(seed)
+    sp = samplers(pkg)
+    reqs = []
+    for i in range(n):
+        L = LENGTHS[i % len(LENGTHS)] if i < 2 * len(LENGTHS) else int(rng.integers(1, 200))
+        s = sp[i % len(sp)]
+        max_new = int(rng.integers(3, 40))
+        u = rng.random(max_new) if s.temperature > 0 else None
+        reqs.append(dict(slot=slots[i], prompt=[int(x) for x in rng.integers(0, V, size=L)], max_new=max_new, sampling=s,
+                         u=u, stop=()))
+    return reqs
+
+
+def engines(pkg, path, seed=99):
+    """(a, b): a runs the batcher, b the oracle, both from the same non-trivial state of every slot."""
+    a = pkg.Engine(path, max_gpt=MAX_GPT)
+    b = pkg.Engine(path, max_gpt=MAX_GPT)
+    b.set_option("prefill_min", 2)
+    rng = np.random.default_rng(seed)
+    a.forward_streams([(j, [int(rng.integers(0, V))]) for j in range(MAX_GPT)], want_logits=False)
+    b.state_upload(a.state_download(MAX_GPT), MAX_GPT)
+    return a, b
+
+
+def oracle(pkg, b, r):
+    """Steps 1 and 2 of the rule for one request on engine b; returns its tokens."""
+    slot, prompt = r["slot"], r["prompt"]
+    if len(prompt) > 1:
+        call = [(slot, prompt[:-1])]
+        if len(prompt) - 1 < 2:
+            call.append((PAD, prompt[:1]))
+        b.forward_streams(call, want_logits=False)
+    us = None if r["u"] is None else np.stack([r["u"], np.full(r["max_new"], 0.5)], axis=1)
+    out = b.generate_streams([(slot, prompt[-1]), (PAD, prompt[-1])], r["max_new"], stop=r["stop"],
+                             sampling=[r["sampling"], pkg.Sampler(temperature=0.0)], u=us)
+    return [int(x) for x in out[0]]
+
+
+def add_stops(pkg, b, reqs):
+    """Give every other request a stop token taken from its own unconstrained run, so that it fires mid-way."""
+    st = b.state_download(MAX_GPT)
+    for i, r in enumerate(reqs):
+        if i % 2 == 0:
+            continue
+        toks = oracle(pkg, b, r)
+        fresh = [k for k in range(len(toks) // 2, len(toks)) if toks[k] not in toks[:k]]
+        if fresh:
+            r["stop"] = (toks[fresh[0]],)
+    b.state_upload(st, MAX_GPT)
+
+
+def submit(bat, r):
+    return bat.submit(r["slot"], r["prompt"], r["max_new"], sampling=r["sampling"], u=r["u"], stop=r["stop"])
+
+
+def finish(bat):
+    while bat.run(1000):
+        pass
+
+
+def check_slots(a, b, before, named, what):
+    n = a.n_layers * a.n_embed
+    sa, sb = a.state_download(MAX_GPT), b.state_download(MAX_GPT)
+    for slot in range(MAX_GPT - 1):
+        ref = sb if slot in named else before
+        for k in KEYS:
+            assert np.array_equal(slot_of(sa, slot, n)[k], slot_of(ref, slot, n)[k]), \
+                "%s: slot %d state %s (%s)" % (what, slot, k, "named" if slot in named else "untouched")
+
+
+@pytest.fixture(scope="module", params=SHAPES, ids=["3x768", "2x2048"])
+def setup(request, pkg, make_model):
+    """The engines, the ~40 requests with stops, and their oracle tokens (b holds every request's final state)."""
+    L, E = request.param
+    a, b = engines(pkg, make_model(L, E))
+    before = a.state_download(MAX_GPT)
+    reqs = make_requests(pkg, 40, 7, list(range(40)))
+    add_stops(pkg, b, reqs)
+    want = [oracle(pkg, b, r) for r in reqs]
+    assert any(len(w) < r["max_new"] for w, r in zip(want, reqs)), "no stop token fired"
+    yield pkg, a, b, before, reqs, want
+    a.close()
+    b.close()
+
+
+@pytest.mark.parametrize("rows,prefill", [(4, 1), (4, 17), (64, 128), (64, 300)])
+def test_waves_equal_oracle(setup, rows, prefill):
+    """Three waves submitted between runs of 5, 16 and 40 steps: tokens and slots equal the oracle, bit for bit."""
+    pkg, a, b, before, reqs, want = setup
+    a.state_upload(before, MAX_GPT)
+    with a.batcher(rows, prefill) as bat:
+        ids = []
+        for wave, steps in ((reqs[:14], 5), (reqs[14:27], 16), (reqs[27:], 40)):
+            ids += [submit(bat, r) for r in wave]
+            bat.run(steps)
+        finish(bat)
+        for i, (rid, w) in enumerate(zip(ids, want)):
+            toks, status = bat.read(rid)
+            assert status == "done", "request %d: %s" % (i, status)
+            assert [int(x) for x in toks] == w, "request %d (prompt %d tokens): tokens" % (i, len(reqs[i]["prompt"]))
+    check_slots(a, b, before, {r["slot"] for r in reqs}, "rows=%d prefill=%d" % (rows, prefill))
+
+
+def run_schedule(pkg, a, before, reqs, rows, prefill, steps):
+    a.state_upload(before, MAX_GPT)
+    with a.batcher(rows, prefill) as bat:
+        ids = [submit(bat, r) for r in reqs]
+        while bat.run(steps):
+            pass
+        toks = [[int(x) for x in bat.read(i)[0]] for i in ids]
+    return toks, a.state_download(MAX_GPT)
+
+
+def test_two_schedules_identical(setup):
+    pkg, a, b, before, reqs, want = setup
+    t1, s1 = run_schedule(pkg, a, before, reqs[:12], 8, 64, 1000)
+    t2, s2 = run_schedule(pkg, a, before, reqs[:12], 3, 5, 7)
+    assert t1 == t2
+    for k in KEYS:
+        assert np.array_equal(s1[k], s2[k]), k
+
+
+def test_streaming_prefix(setup):
+    """After each run(16), read is a prefix of the final tokens."""
+    pkg, a, b, before, reqs, want = setup
+    a.state_upload(before, MAX_GPT)
+    seen = {}
+    with a.batcher(6, 40) as bat:
+        ids = [submit(bat, r) for r in reqs[:10]]
+        while bat.run(16):
+            for i, rid in enumerate(ids):
+                toks, _ = bat.read(rid)
+                seen.setdefault(i, []).append([int(x) for x in toks])
+        for i, rid in enumerate(ids):
+            final = [int(x) for x in bat.read(rid)[0]]
+            assert final == want[i]
+            for p in seen[i]:
+                assert final[:len(p)] == p
+        assert any(0 < len(p) < len(want[i]) for i in seen for p in seen[i]), "nothing streamed"
+
+
+def test_release_between_runs(setup):
+    """Done requests released between runs, while others still run and new ones arrive, change nothing in the rest."""
+    pkg, a, b, before, reqs, want = setup
+    a.state_upload(before, MAX_GPT)
+    with a.batcher(3, 24) as bat:
+        ids = {submit(bat, r): i for i, r in enumerate(reqs[:6])}
+        got = {}
+        pending = list(range(6, 12))
+        while bat.run(16) or pending:
+            for rid, i in list(ids.items()):
+                toks, st = bat.read(rid)
+                if st == "done":
+                    got[i] = [int(x) for x in toks]
+                    bat.release(rid)
+                    del ids[rid]
+            if pending:
+                i = pending.pop(0)
+                ids[submit(bat, reqs[i])] = i
+        for rid, i in ids.items():
+            got[i] = [int(x) for x in bat.read(rid)[0]]
+    assert [got[i] for i in range(12)] == want[:12]
+
+
+def test_cancel(setup):
+    """Cancel a queued, a prefilling and a generating request: their tokens are prefixes of the oracle's, the queued
+    request's slot is untouched, and every other request equals the run without the cancels."""
+    pkg, a, b, before, reqs, want = setup
+    a.state_upload(before, MAX_GPT)
+    n = a.n_layers * a.n_embed
+    sel = reqs[:12]
+    with a.batcher(4, 3) as bat:
+        ids = [submit(bat, r) for r in sel]
+        for _ in range(20):  # group ends until one request of each kind is seen
+            bat.run(16)
+            status = {i: bat.read(rid)[1] for i, rid in enumerate(ids)}
+            gen = [i for i in status if status[i] == "generating"]
+            pre = [i for i in status if status[i] == "prefilling"]
+            que = [i for i in status if status[i] == "queued"]
+            if gen and pre and que:
+                break
+        assert gen and pre and que, status
+        cancelled = {gen[0], pre[0], que[-1]}
+        for i in cancelled:
+            bat.cancel(ids[i])
+        finish(bat)
+        for i, rid in enumerate(ids):
+            toks, st = bat.read(rid)
+            toks = [int(x) for x in toks]
+            if i in cancelled:
+                assert st == "cancelled" and toks == want[i][:len(toks)], i
+            else:
+                assert st == "done" and toks == want[i], i
+        sa = a.state_download(MAX_GPT)
+        q = sel[que[-1]]["slot"]
+        for k in KEYS:
+            assert np.array_equal(slot_of(sa, q, n)[k], slot_of(before, q, n)[k]), "queued slot touched"
+    sb = b.state_download(MAX_GPT)
+    for i, r in enumerate(sel):
+        if i not in cancelled:
+            for k in KEYS:
+                assert np.array_equal(slot_of(sa, r["slot"], n)[k], slot_of(sb, r["slot"], n)[k]), (i, k)
+
+
+def test_next_turn_and_unrelated_forward(pkg, make_model):
+    """A second request on a finished request's slot equals the oracle chained on that slot, and a forward_streams on an
+    unrelated slot between runs changes nothing in the batcher's results."""
+    a, b = engines(pkg, make_model(3, 768))
+    before = a.state_download(MAX_GPT)
+    reqs = make_requests(pkg, 6, 11, [40, 41, 42, 43, 44, 45])
+    turn2 = make_requests(pkg, 2, 12, [40, 41])
+    with a.batcher(4, 20) as bat:
+        ids = [submit(bat, r) for r in reqs]
+        bat.run(5)
+        a.forward_streams([(50, [1, 2, 3, 4, 5, 6, 7, 8, 9])], want_logits=False)
+        b.forward_streams([(50, [1, 2, 3, 4, 5, 6, 7, 8, 9])], want_logits=False)
+        finish(bat)
+        for rid in ids[:2]:
+            bat.release(rid)
+        ids2 = [submit(bat, r) for r in turn2]
+        finish(bat)
+        got = [[int(x) for x in bat.read(i)[0]] for i in ids[2:] + ids2]
+    want = [oracle(pkg, b, r) for r in reqs]
+    want2 = [oracle(pkg, b, r) for r in turn2]
+    assert got == want[2:] + want2
+    named = {r["slot"] for r in reqs} | {50}
+    check_slots(a, b, before, named, "next turn")
+    a.close()
+    b.close()
+
+
+def test_refusals(pkg, make_model):
+    """Every refusal leaves every slot untouched; unknown ids are refused."""
+    a, _ = engines(pkg, make_model(3, 768))
+    before = a.state_download(MAX_GPT)
+    E = pkg.EngineError
+    for rows, pf in ((0, 16), (MAX_GPT + 1, 16), (4, 0), (4, 2049)):
+        with pytest.raises(E):
+            a.batcher(rows, pf)
+    a.set_option("prefill", 0)
+    with pytest.raises(E, match="prefill"):
+        a.batcher(4, 16)
+    a.set_option("prefill", 1)
+    with a.batcher(4, 16) as bat:
+        with pytest.raises(E, match="already has an open batcher"):
+            a.batcher(4, 16)
+        rid = bat.submit(3, [1, 2, 3], 8)
+        S = pkg.Sampler
+        bad = [dict(slot=MAX_GPT, prompt=[1], max_new=4), dict(slot=3, prompt=[1], max_new=4),
+               dict(slot=4, prompt=[V], max_new=4), dict(slot=4, prompt=[], max_new=4), dict(slot=4, prompt=[1], max_new=0),
+               dict(slot=4, prompt=[1], max_new=4, stop=(V,)), dict(slot=4, prompt=[1], max_new=4, sampling=S(top_p=0.0)),
+               dict(slot=4, prompt=[1], max_new=4, sampling=S(temperature=1.0)),
+               dict(slot=4, prompt=[1], max_new=2, sampling=S(temperature=1.0), u=[0.5, 1.0])]
+        for kw in bad:
+            with pytest.raises(E):
+                bat.submit(**kw)
+        for call in (bat.read, bat.cancel, bat.release):
+            with pytest.raises(E, match="unknown"):
+                call(rid + 100)
+        with pytest.raises(E, match="not ended"):
+            bat.release(rid)
+        bat.cancel(rid)  # queued: its slot stays untouched
+        with pytest.raises(E, match="already ended"):
+            bat.cancel(rid)
+        bat.release(rid)
+        assert bat.run(16) == 0
+    after = a.state_download(MAX_GPT)
+    for k in KEYS:
+        assert np.array_equal(before[k], after[k]), k
+    a.close()
