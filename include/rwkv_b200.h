@@ -432,6 +432,46 @@ int rwkv_b200_beam_search(rwkv_b200_model *m, const unsigned long long *slots, c
                           double *logprobs_out, double *scores_out, unsigned char *finished_out,
                           double *token_logprobs_out);
 
+/* Speculative generation with prompt-lookup drafts: rwkv_b200_generate_streams_ex that may emit several tokens per stream
+ * per step, with the same tokens. Every argument up to lengths_out is that of generate_streams_ex, except that each
+ * stream names draft + 1 distinct slots: slots[n_streams][draft + 1]. slots[s][0] is the stream's first slot and holds
+ * its conversation; the others are scratch, and their contents after the call are unspecified. draft = k (1..15) drafts
+ * per step, ngram (1..8) the longest n-gram looked up. context_start [n_streams + 1] (CSR, context_start[0] = 0) and
+ * context give each stream extra lookup tokens context[context_start[s] .. context_start[s + 1]) (e.g. the prompt, or a
+ * document the answer quotes); context_start == NULL: none. steps_out [n_streams] receives the steps in which each
+ * stream emitted a token, so lengths_out[s] / steps_out[s] is the stream's tokens per step.
+ * The rule. h = context_s ++ [first_s] ++ the tokens stream s emitted so far in this call, L = len(h).
+ *  1. Drafts: for n = ngram down to 1 with n < L, the largest j <= L - n - 1 with h[j .. j+n) == h[L-n .. L); the first
+ *     n that has one gives the proposal h[j+n .. min(j+n+k, L)]. The k drafts d_1..d_k are the proposal padded by
+ *     repeating its last token, or k copies of h[L-1] when no n matches.
+ *  2. A step gives stream s k + 1 consecutive rows of one tensor-core pass: row 0 feeds its current input, row i feeds
+ *     d_i. After the overrides, the pick p_i of row i uses the stream's sampler and the uniform u[(len + i) * n_streams
+ *     + s], len = the tokens emitted before the step.
+ *  3. a = the number of leading i in 1..k with d_i == p_(i-1). The step emits p_0 .. p_a in order, each with the stop and
+ *     budget check of generate_streams; tokens after a stop or past the budget are dropped. The next input is the last
+ *     emitted token, and the state continues from the slot of the row that produced it (emitted, not fed).
+ * Because each row of a pass is exact and a stream's bits depend only on its own rows, the logits of row i are bit for
+ * bit those generate_streams_ex computes at position len + i. So the emitted tokens, the lengths and the first slots'
+ * xy, aa, bb and dd are bit for bit those of generate_streams_ex on the first slots with the same first tokens, budgets,
+ * stops, overrides, samplers and u, run on the tensor cores, whatever the drafts are: drafts change the speed, never the
+ * tokens. A first slot's pp is untouched (no forward writes it); slots no stream names are untouched. steps_out depends
+ * only on the emitted tokens and the contexts, so a host can restate it exactly. Each step's passes hold floor(128 /
+ * (draft + 1)) streams; streams leave the rows at 16-step group boundaries, as in generate_streams.
+ * Refused before any work (every slot untouched): the refusals of generate_streams_ex, n_streams * (draft + 1) >
+ * max_gpt, a slot repeated anywhere in slots, draft or ngram out of range, a missing steps_out, context offsets that do
+ * not start at 0 or decrease, a context token >= 50277, a presence or frequency penalty, "prefill" set to 0, and tensor
+ * parallelism. The call always runs on the tensor cores, whatever prefill_min is. After it no per-stream logits are held. */
+int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned long long *slots,
+                                           const unsigned long long *first_tokens, unsigned long long n_streams,
+                                           unsigned long long max_new, const unsigned long long *budgets,
+                                           const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                           const unsigned long long *override_tokens, const float *override_values,
+                                           unsigned long long n_override, const rwkv_b200_sampler *samplers,
+                                           const double *u, unsigned long long *tokens_out,
+                                           unsigned long long *lengths_out, unsigned int draft, unsigned int ngram,
+                                           const unsigned long long *context_start, const unsigned long long *context,
+                                           unsigned long long *steps_out);
+
 /* Continuous batching: a batcher accepts requests at any time between runs and serves them together, so a request that
  * arrives while others generate starts at the next 16-step group instead of after the whole batch, and the rows freed
  * by finished requests are refilled at once. A request names a state slot, its prompt (n_prompt >= 1 tokens), max_new

@@ -40,6 +40,7 @@
 #include "prefill.cuh"
 #include "sampling.cuh"
 #include "score.cuh"
+#include "speculate.cuh"
 #include "token_kernel.cuh"
 
 namespace {
@@ -170,6 +171,16 @@ struct rwkv_b200_model {
         DevBuf<int> n_hyp;                      // [G]
         DevBuf<unsigned long long> done, forks; // [G], [G * B][2]
     } beam;
+    // generate_streams_speculative: the streams' records, histories, live list, passes and per-row uniforms, grown with
+    // the largest call; the emitted tokens, stops, overrides and samplers use gen's buffers
+    struct Spec {
+        DevBuf<rk::SpecStream> ss;        // [n_streams]
+        DevBuf<unsigned long long> hist;  // per stream: context, first token, up to max_new emitted tokens
+        DevBuf<int> live;                 // [live streams]
+        DevBuf<rk::PassDesc> passes;      // [passes of a step]
+        DevBuf<double> u, row_u;          // [max_new][n_streams], [rows]
+        DevBuf<unsigned long long> forks; // [n_streams][2] the final copies home -> first slot
+    } spec;
     rwkv_b200_batcher *batcher = nullptr; // the open batcher (at most one), closed by rwkv_b200_free
 };
 
@@ -747,12 +758,13 @@ int gen_step_decode(M *m, int rows, const int *row_stream) {
     return 0;
 }
 
-// One step of generate_streams on the tensor cores: ceil(rows / 128) passes whose descriptors the previous step's
-// feedback (or the group's upload) left in gen.passes; every row is a head row, so row r's logits land in d_slogits row r.
-int gen_step_passes(M *m, int rows) {
-    for (int p0 = 0, pi = 0; p0 < rows; p0 += rk::kPfMaxTokens, ++pi) {
-        const int T = std::min(rk::kPfMaxTokens, rows - p0);
-        CK(cudaMemcpyAsync(m->pf.pass, m->gen.passes + pi, sizeof(rk::PassDesc), cudaMemcpyDeviceToDevice, m->stream));
+// One step of generate_streams on the tensor cores: ceil(rows / per_pass) passes of per_pass rows (the last may be
+// shorter) whose descriptors are in `passes` on the device (the previous step's feedback, the group's upload, or
+// k_spec_draft); every row is a head row, so row r's logits land in d_slogits row r.
+int gen_step_passes(M *m, const rk::PassDesc *passes, int rows, int per_pass) {
+    for (int p0 = 0, pi = 0; p0 < rows; p0 += per_pass, ++pi) {
+        const int T = std::min(per_pass, rows - p0);
+        CK(cudaMemcpyAsync(m->pf.pass, passes + pi, sizeof(rk::PassDesc), cudaMemcpyDeviceToDevice, m->stream));
         int rc = rk::prefill_run(m->pf, m->p, m->stream, T, T, m->d_slogits);
         if (rc) return fail(rc, "%s", rk::prefill_error());
     }
@@ -985,7 +997,7 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
                                     (int)lpq->top_n, max_new, g.lp.p, g.rank.p, g.top_tok.p, g.top_lp.p};
         const unsigned rb = (unsigned)((rows + 127) / 128);
         for (unsigned long long k = 0; k < steps; ++k) {
-            if ((rc = tc ? gen_step_passes(m, rows) : gen_step_decode(m, rows, g.row_stream))) return rc;
+            if ((rc = tc ? gen_step_passes(m, g.passes, rows, rk::kPfMaxTokens) : gen_step_decode(m, rows, g.row_stream))) return rc;
             if (raw_copy)
                 CK(cudaMemcpyAsync(g.raw.p, m->d_slogits, (size_t)rows * V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
             if (pen) {
@@ -1140,7 +1152,7 @@ int beam(M *m, const unsigned long long *slots, const unsigned long long *first_
             const unsigned long long st = step + k;
             const int nb = st == 0 ? 1 : (int)B, rows = Gl * nb;
             const int *rmap = st == 0 ? bm.row0.p : g.row_stream;
-            if ((rc = tc ? gen_step_passes(m, rows) : gen_step_decode(m, rows, rmap))) return rc;
+            if ((rc = tc ? gen_step_passes(m, g.passes, rows, rk::kPfMaxTokens) : gen_step_decode(m, rows, rmap))) return rc;
             rk::k_beam_expand<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs, rmap, (int)C,
                                                                                 bm.cand_tok.p, bm.cand_lp.p);
             CK(cudaGetLastError());
@@ -1193,6 +1205,169 @@ int beam(M *m, const unsigned long long *slots, const unsigned long long *first_
             scores_out[o] = h.score;
             finished_out[o] = (unsigned char)h.finished;
         }
+    return 0;
+}
+
+// The body of rwkv_b200_generate_streams_speculative: generate()'s group loop with k + 1 rows per live stream. Each
+// step is k_spec_draft -> passes -> overrides -> pick -> k_spec_accept; at each group's end the records come back and
+// the finished streams leave the rows. At the end a stream whose home is a spare has it copied to its first slot.
+int speculate(M *m, const unsigned long long *slots, const unsigned long long *first_tokens, unsigned long long n_streams,
+              unsigned long long max_new, const unsigned long long *budgets, const unsigned long long *stop_tokens,
+              unsigned long long n_stop, const unsigned long long *override_tokens, const float *override_values,
+              unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u, unsigned long long *tokens_out,
+              unsigned long long *lengths_out, unsigned draft, unsigned ngram, const unsigned long long *context_start,
+              const unsigned long long *context, unsigned long long *steps_out) {
+    const char *what = "generate_streams_speculative";
+    int rc = check_streams_model(m, what);
+    if (rc) return rc;
+    if (n_streams == 0) return fail(1, "%s: no streams", what);
+    if (!slots || !first_tokens || !tokens_out || !lengths_out || !steps_out)
+        return fail(1, "%s: null argument (slots, first_tokens, tokens_out, lengths_out and steps_out are required)", what);
+    if (n_stop && !stop_tokens) return fail(1, "%s: n_stop = %llu with NULL stop_tokens", what, n_stop);
+    if (n_override && (!override_tokens || !override_values))
+        return fail(1, "%s: n_override = %llu with NULL override_tokens or override_values", what, n_override);
+    if (max_new == 0) return fail(1, "%s: max_new is 0", what);
+    if (draft < 1 || draft > (unsigned)rk::kSpecMaxDraft) return fail(1, "%s: draft %u is outside 1..%d", what, draft, rk::kSpecMaxDraft);
+    if (ngram < 1 || ngram > (unsigned)rk::kSpecMaxNgram) return fail(1, "%s: ngram %u is outside 1..%d", what, ngram, rk::kSpecMaxNgram);
+    if (!rk::prefill_enabled(m->pf)) return fail(1, "%s: needs the tensor cores (the \"prefill\" option is 0)", what);
+    const unsigned long long K1 = draft + 1ull, S = n_streams;
+    if (S > m->max_gpt / K1)
+        return fail(1, "%s: %llu streams x %llu rows > max_gpt %llu", what, S, K1, m->max_gpt);
+    if ((rc = check_slots(m, what, slots, S * K1)) || (rc = check_tokens(what, "first token", first_tokens, S, "stream")) ||
+        (rc = check_tokens(what, "stop token", stop_tokens, n_stop)) ||
+        (rc = check_tokens(what, "override token", override_tokens, n_override)) ||
+        (rc = check_overrides(what, override_tokens, override_values, n_override)))
+        return rc;
+    for (unsigned long long i = 0; budgets && i < S; ++i)
+        if (budgets[i] == 0 || budgets[i] > max_new)
+            return fail(1, "%s: budget %llu of stream %llu is outside 1..max_new = %llu", what, budgets[i], i, max_new);
+    for (unsigned long long s = 0; samplers && s < S; ++s) {
+        if ((rc = check_sampler(what, s, samplers[s], true))) return rc;
+        if (samplers[s].presence_penalty != 0.0f || samplers[s].frequency_penalty != 0.0f)
+            return fail(1, "%s: stream %llu: presence and frequency penalties are not supported (a row's counts would have "
+                           "to include its own drafts)", what, s);
+        if (samplers[s].temperature > 0.0f && !u)
+            return fail(1, "%s: u is NULL but stream %llu samples (temperature %g)", what, s, samplers[s].temperature);
+    }
+    if (!samplers) u = nullptr; // every stream takes the arg-max
+    if (u)
+        for (unsigned long long i = 0; i < max_new * S; ++i)
+            if (!(u[i] >= 0.0 && u[i] < 1.0)) return fail(1, "%s: u[%llu] = %g is outside [0, 1)", what, i, u[i]);
+    unsigned long long n_ctx = 0;
+    if (context_start) {
+        if (context_start[0] != 0) return fail(1, "%s: context_start[0] = %llu, not 0", what, context_start[0]);
+        for (unsigned long long s = 0; s < S; ++s)
+            if (context_start[s + 1] < context_start[s])
+                return fail(1, "%s: context_start decreases from stream %llu to %llu (%llu > %llu)", what, s, s + 1,
+                            context_start[s], context_start[s + 1]);
+        n_ctx = context_start[S];
+        if (n_ctx && !context) return fail(1, "%s: %llu context tokens with NULL context", what, n_ctx);
+        if ((rc = check_tokens(what, "context token", context, n_ctx))) return rc;
+    }
+    const size_t V = binfmt::kVocab;
+    const unsigned long long n_hist = n_ctx + S * (1 + max_new);
+    CK(cudaSetDevice(m->device));
+    auto &g = m->gen;
+    auto &sp = m->spec;
+    const int per_pass = rk::kPfMaxTokens / (int)K1; // streams per pass: a stream's rows never straddle two passes
+    const size_t n_pass = (size_t)((S + per_pass - 1) / per_pass);
+    if ((rc = g.out.grow(S * max_new)) || (rc = g.stop.grow(n_stop)) || (rc = g.ovr_tok.grow(n_override)) ||
+        (rc = g.ovr_val.grow(n_override)) || (samplers && (rc = g.samp.grow(S))) || (rc = sp.ss.grow(S)) ||
+        (rc = sp.hist.grow(n_hist)) || (rc = sp.live.grow(S)) || (rc = sp.passes.grow(n_pass)) ||
+        (u && ((rc = sp.u.grow(max_new * S)) || (rc = sp.row_u.grow(S * K1)))) || (rc = sp.forks.grow(2 * S)))
+        return rc;
+    if ((rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
+    m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
+
+    // the records and the histories: stream s's history starts with its context and its first token
+    std::vector<rk::SpecStream> hs(S);
+    std::vector<unsigned long long> hist(n_hist, 0); // stream s: its context, its first token, then room for max_new
+    for (unsigned long long s = 0, h0 = 0; s < S; ++s) {
+        rk::SpecStream &r = hs[s];
+        r = rk::SpecStream{};
+        for (unsigned long long i = 0; i < K1; ++i) r.slot[i] = slots[s * K1 + i];
+        const unsigned long long c0 = context_start ? context_start[s] : 0, c1 = context_start ? context_start[s + 1] : 0;
+        r.h0 = h0;
+        r.hl = c1 - c0 + 1;
+        r.budget = budgets ? budgets[s] : max_new;
+        std::copy(context + c0, context + c1, hist.begin() + h0);
+        hist[h0 + c1 - c0] = first_tokens[s];
+        h0 += r.hl + max_new;
+    }
+    CK(cudaMemcpyAsync(sp.hist.p, hist.data(), n_hist * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemcpyAsync(sp.ss.p, hs.data(), S * sizeof(rk::SpecStream), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemsetAsync(g.out.p, 0, S * max_new * sizeof(unsigned long long), m->stream));
+    if (n_stop) CK(cudaMemcpyAsync(g.stop.p, stop_tokens, n_stop * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    if (n_override) {
+        CK(cudaMemcpyAsync(g.ovr_tok.p, override_tokens, n_override * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(g.ovr_val.p, override_values, n_override * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+    }
+    if (samplers) CK(cudaMemcpyAsync(g.samp.p, samplers, S * sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
+    if (u) CK(cudaMemcpyAsync(sp.u.p, u, max_new * S * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+
+    std::vector<int> live(S), rs;
+    for (unsigned long long s = 0; s < S; ++s) live[s] = (int)s;
+    rk::SpecArgs sa{sp.ss.p, sp.live.p, (int)draft, (int)ngram, per_pass, sp.hist.p, sp.passes.p, u ? sp.u.p : nullptr,
+                    sp.row_u.p, S, max_new, samplers ? nullptr : m->d_next, m->d_sample, g.stop.p, (int)n_stop, g.out.p};
+    // each step emits at least one token per live stream, so max_new steps finish every stream
+    for (unsigned long long step = 0; !live.empty() && step < max_new;) {
+        const int n_live = (int)live.size(), rows = n_live * (int)K1;
+        const unsigned long long steps = std::min(kGenGroup, max_new - step);
+        rs.resize(rows);
+        for (int r = 0; r < rows; ++r) rs[r] = live[r / (int)K1];
+        CK(cudaMemcpyAsync(sp.live.p, live.data(), n_live * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(g.row_stream, rs.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        for (unsigned long long k = 0; k < steps; ++k) {
+            rk::k_spec_draft<<<(unsigned)n_live, rk::kSpecDraftThreads, 0, m->stream>>>(sa);
+            CK(cudaGetLastError());
+            m->launches += 1;
+            if ((rc = gen_step_passes(m, sp.passes.p, rows, per_pass * (int)K1))) return rc;
+            if (n_override) {
+                rk::k_gen_override<<<(unsigned)((rows + 127) / 128), 128, 0, m->stream>>>(m->d_slogits, (int)V, rows, g.ovr_tok.p,
+                                                                                        g.ovr_val.p, (int)n_override);
+                CK(cudaGetLastError());
+                m->launches += 1;
+            }
+            if (samplers)
+                rk::k_sample_nucleus<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.samp.p, g.row_stream,
+                                                                                       u ? sp.row_u.p : nullptr, m->d_sample);
+            else
+                rk::k_argmax_rows<<<(unsigned)rows, rk::kArgmaxThreads, 0, m->stream>>>(m->d_slogits, (int)V, m->d_next);
+            CK(cudaGetLastError());
+            rk::k_spec_accept<<<(unsigned)n_live, 32, 0, m->stream>>>(sa);
+            CK(cudaGetLastError());
+            m->launches += 2;
+        }
+        // the end of a group: which streams are done (one synchronisation); drop them from the rows
+        CK(cudaMemcpyAsync(hs.data(), sp.ss.p, S * sizeof(rk::SpecStream), cudaMemcpyDeviceToHost, m->stream));
+        SYNC(m);
+        step += steps;
+        live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hs[s].done != 0; }), live.end());
+    }
+    // a home on a spare: its xy, aa, bb and dd go to the first slot (pp: no forward writes it)
+    std::vector<unsigned long long> forks;
+    for (unsigned long long s = 0; s < S; ++s)
+        if (hs[s].home != 0) {
+            forks.push_back(hs[s].slot[hs[s].home]);
+            forks.push_back(hs[s].slot[0]);
+        }
+    if (!forks.empty()) {
+        double *arr[5];
+        slot_arrays(m, 0, arr);
+        const size_t slot_len = (size_t)(m->L * m->E);
+        const unsigned chunks = (unsigned)((slot_len + rk::kForkChunk - 1) / rk::kForkChunk);
+        CK(cudaMemcpyAsync(sp.forks.p, forks.data(), forks.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        rk::k_beam_fork<<<dim3((unsigned)(forks.size() / 2), chunks, 4), rk::kForkThreads, 0, m->stream>>>(
+            sp.forks.p, arr[0], arr[1], arr[2], arr[4], nullptr, slot_len);
+        CK(cudaGetLastError());
+        m->launches += 1;
+    }
+    CK(cudaMemcpyAsync(tokens_out, g.out.p, S * max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+    SYNC(m);
+    for (unsigned long long s = 0; s < S; ++s) {
+        lengths_out[s] = hs[s].len;
+        steps_out[s] = hs[s].steps;
+    }
     return 0;
 }
 
@@ -1783,6 +1958,18 @@ int rwkv_b200_beam_search(rwkv_b200_model *m, const unsigned long long *slots, c
                           double *token_logprobs_out) {
     return beam(m, slots, first_tokens, n_groups, beams, max_new, stop_tokens, n_stop, length_penalty, n_best, tokens_out,
                 lengths_out, logprobs_out, scores_out, finished_out, token_logprobs_out);
+}
+
+int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
+                                           unsigned long long n_streams, unsigned long long max_new, const unsigned long long *budgets,
+                                           const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                           const unsigned long long *override_tokens, const float *override_values,
+                                           unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
+                                           unsigned long long *tokens_out, unsigned long long *lengths_out, unsigned int draft,
+                                           unsigned int ngram, const unsigned long long *context_start,
+                                           const unsigned long long *context, unsigned long long *steps_out) {
+    return speculate(m, slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values,
+                     n_override, samplers, u, tokens_out, lengths_out, draft, ngram, context_start, context, steps_out);
 }
 
 int rwkv_b200_sample_streams(rwkv_b200_model *m, unsigned long long n_streams, const rwkv_b200_sampler *params, const double *u,

@@ -42,9 +42,12 @@ constexpr int kPfConsumerWGs = 2;
 constexpr int kPfThreads = 128 * kPfConsumerWGs + 32;
 constexpr int kPfTokenAlign = 16 * kPfConsumerWGs; // padded token count: the same number of blocks per warpgroup
 
-// Stream descriptor of one token of a pass: its state slot and two flags.
+// Stream descriptor of one token of a pass: its state slot and two flags. A "last" token stores its state into its own
+// slot, which need not be the slot its segment's "first" token loaded: a speculative step (speculate.cuh) continues one
+// segment through draft rows on other slots. Every other producer of descriptors (pass_layout, k_gen_feedback,
+// k_beam_select, the batcher) names one slot per segment, for which the two are the same.
 constexpr uint32_t kDescFirst = 1u << 31; // token shift and WKV start from the slot's state, not from token t - 1
-constexpr uint32_t kDescLast = 1u << 30;  // the slot's state is stored after this token
+constexpr uint32_t kDescLast = 1u << 30;  // the token's slot receives the state after this token
 constexpr uint32_t kDescSlot = kDescLast - 1u;
 __host__ __device__ __forceinline__ size_t desc_slot(uint32_t d) { return (size_t)(d & kDescSlot); }
 
@@ -359,7 +362,7 @@ __device__ __forceinline__ float pf_combine(const int *C, int Tp, size_t m, int 
 }
 
 // WKV over the pass (rwkv.cu:221-259): thread = channel, sequential over t. The state is loaded from the slot at
-// a stream's first token and stored back after its last. Writes the unscaled rwkv (f32) and xs = rwkv * r_out
+// a stream's first token and stored into the slot of each token marked last. Writes the unscaled rwkv (f32) and xs = rwkv * r_out
 // rounded to 22 bits.
 struct WkvArgs {
     const int *Ck, *Cv, *Cr;          // [E][3 Tp]
@@ -399,9 +402,10 @@ __global__ void __launch_bounds__(256) k_pf_wkv(const __grid_constant__ WkvArgs 
         const double ek = exp((double)kf);
         aa = (aa + ek * vv) * ew;
         bb = (bb + ek) * ew;
-        if (d & kDescLast) {
-            a.aa[so] = aa;
-            a.bb[so] = bb;
+        if (d & kDescLast) { // into the token's own slot, like k_pf_store_state (speculate.cuh: a row per draft)
+            const size_t o = desc_slot(d) * a.slot_stride + c;
+            a.aa[o] = aa;
+            a.bb[o] = bb;
         }
         const float rw = (float)y;
         a.rw[(size_t)t * a.E + c] = rw;

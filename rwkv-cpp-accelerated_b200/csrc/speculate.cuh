@@ -1,0 +1,138 @@
+// speculate.cuh — device side of rwkv_b200_generate_streams_speculative: prompt-lookup drafts verified in the tensor-core
+// pass, so that a step can emit several tokens per stream with the bits of one-token-per-step generation.
+//
+// A call keeps one record per stream (SpecStream): its k + 1 slots, which of them is home (holds the conversation),
+// its history (lookup context ++ first token ++ tokens emitted so far) and its length, budget and step count. Each step
+// of a host group is enqueued with no synchronisation inside the group:
+//   k_spec_draft   one CTA per live stream: the prompt-lookup drafts of the history (a block-parallel scan for the largest
+//                  matching position per n-gram length, reduced by max, so the result does not depend on the schedule),
+//                  then the step's layout: row 0 = the current input on the home slot (first | last), row i = draft i on
+//                  the stream's i-th other slot (last), so every row stores its state in its own slot; and the uniform
+//                  of each row for k_sample_nucleus;
+//   forward        the tensor-core passes, floor(128 / (k + 1)) streams per pass, every row a head row;
+//   k_gen_override, then k_sample_nucleus or k_argmax_rows on the rows (row_stream maps every row of s to s);
+//   k_spec_accept  one CTA per live stream: the picks, the accepted prefix, stops and budget, the emitted tokens into
+//                  the output and the history, and the new home: the slot of the row that produced the last emitted token.
+// At the end of the call, a stream whose home is not its first slot has the home's xy, aa, bb and dd copied to the first
+// slot (k_beam_fork with four arrays). The rule is stated in include/rwkv_b200.h and DESIGN §4.3.
+#pragma once
+#include <cstdint>
+#include <cuda_runtime.h>
+
+#include "prefill.cuh"
+
+namespace rk {
+
+constexpr int kSpecMaxDraft = 15;   // k <= 15: a stream's k + 1 rows fit one warp and one pass
+constexpr int kSpecMaxNgram = 8;
+constexpr int kSpecDraftThreads = 256;
+
+struct SpecStream {
+    unsigned long long slot[kSpecMaxDraft + 1]; // the stream's k + 1 slots; slot[0] is the first slot
+    unsigned long long row[kSpecMaxDraft + 1];  // this step's row tokens: [0] the input, [i] draft i
+    unsigned long long h0, hl;                  // the history is hist[h0 .. h0 + hl); its last token is the next input
+    unsigned long long budget, len, steps;      // tokens it may emit, tokens emitted, steps that emitted a token
+    unsigned long long done;                    // 1 after a stop token or the budget
+    int home;                                   // index into slot[] of the slot holding the conversation
+    int pad;
+};
+
+struct SpecArgs {
+    SpecStream *ss;                  // [n_streams]
+    const int *live;                 // [live streams] the stream of CTA i; its rows are i * (k + 1) .. + k
+    int k, ngram, per_pass;          // drafts, longest n-gram, streams per pass
+    unsigned long long *hist;        // the histories
+    PassDesc *passes;                // the step's passes
+    const double *u;                 // [max_new][n_streams], or nullptr
+    double *row_u;                   // [rows] the uniform of each row (with u only)
+    unsigned long long n_streams, max_new;
+    const unsigned long long *next;  // arg-max per row, or nullptr when sampling
+    const double *sample;            // {token, margin} per row when sampling
+    const unsigned long long *stop;  // [n_stop]
+    int n_stop;
+    unsigned long long *out;         // [n_streams][max_new]
+};
+
+// Draft rule: for n = ngram down to 1 with n < L, the largest j <= L - n - 1 with h[j .. j + n) == h[L - n .. L); the
+// first n with such a j gives the proposal h[j + n .. min(j + n + k, L)], padded with its last token; no match at any n:
+// k copies of h[L - 1]. Draft i (1-based) is then h[min(j + n + i - 1, L - 1)].
+__global__ void __launch_bounds__(kSpecDraftThreads) k_spec_draft(const SpecArgs a) {
+    const int li = blockIdx.x, s = a.live[li], tid = threadIdx.x, k = a.k;
+    SpecStream &g = a.ss[s];
+    const unsigned long long *h = a.hist + g.h0;
+    const long long L = (long long)g.hl;
+    const bool live = g.done == 0;
+    __shared__ unsigned long long suf[kSpecMaxNgram]; // suf[i] = h[L - 1 - i]
+    __shared__ int wmax[kSpecDraftThreads / 32];
+    long long from = -1; // the proposal starts at h[from]
+    if (live) {
+        if (tid < a.ngram && tid < L) suf[tid] = h[L - 1 - tid];
+        __syncthreads();
+        for (int n = a.ngram; n >= 1 && from < 0; --n) {
+            if (n >= L) continue;
+            int best = -1;
+            for (long long j = tid; j <= L - n - 1; j += kSpecDraftThreads) {
+                bool eq = true;
+                for (int i = 0; i < n && eq; ++i) eq = h[j + n - 1 - i] == suf[i];
+                if (eq) best = (int)j;
+            }
+            best = __reduce_max_sync(0xffffffffu, best);
+            if ((tid & 31) == 0) wmax[tid >> 5] = best;
+            __syncthreads();
+            for (int w = 0; w < kSpecDraftThreads / 32; ++w) best = max(best, wmax[w]);
+            __syncthreads();
+            if (best >= 0) from = best + n;
+        }
+    }
+    if (tid > k) return;
+    const unsigned long long tok = tid == 0 || from < 0 ? h[L - 1] : h[min(from + tid - 1, L - 1)];
+    g.row[tid] = tok;
+    const int r = li * (k + 1) + tid, pi = li / a.per_pass, t = (li % a.per_pass) * (k + 1) + tid;
+    PassDesc &pd = a.passes[pi];
+    pd.tokens[t] = tok;
+    pd.desc[t] = (uint32_t)g.slot[(g.home + tid) % (k + 1)] | (tid == 0 ? kDescFirst : 0u) | (live ? kDescLast : 0u);
+    pd.rows[t] = t;
+    if (t == 0) pd.out_row0 = pi * a.per_pass * (k + 1);
+    if (a.u) {
+        const unsigned long long pos = g.len + (unsigned long long)tid;
+        a.row_u[r] = pos < a.max_new ? a.u[pos * a.n_streams + (unsigned long long)s] : 0.0;
+    }
+}
+
+// One warp per live stream: lane i holds the pick p_i of row i; a = the leading i in 1..k with row[i] == p_{i - 1}.
+// Lane 0 emits p_0 .. p_a with generate_streams' stop and budget check and moves home to the slot of the last row used.
+__global__ void __launch_bounds__(32) k_spec_accept(const SpecArgs a) {
+    const int li = blockIdx.x, s = a.live[li], lane = threadIdx.x, k = a.k;
+    SpecStream &g = a.ss[s];
+    if (g.done) return;
+    const int r = li * (k + 1) + lane;
+    unsigned long long p = 0;
+    if (lane <= k) p = a.next ? a.next[r] : (unsigned long long)a.sample[2 * r];
+    const unsigned long long prev = __shfl_up_sync(0xffffffffu, p, 1);
+    const unsigned miss = __ballot_sync(0xffffffffu, lane >= 1 && (lane > k || g.row[lane] != prev));
+    const int acc = __ffs((int)miss) - 2; // the first lane that misses is a + 1 (lane k + 1 always misses)
+    __shared__ unsigned long long pk[kSpecMaxDraft + 1];
+    if (lane <= k) pk[lane] = p;
+    __syncwarp();
+    if (lane != 0) return;
+    unsigned long long len = g.len, hl = g.hl;
+    int e = 0;
+    bool stop = false;
+    for (int i = 0; i <= acc && !stop; ++i) {
+        const unsigned long long tok = pk[i];
+        a.out[(size_t)s * a.max_new + len] = tok;
+        a.hist[g.h0 + hl] = tok;
+        ++len;
+        ++hl;
+        e = i;
+        stop = len == g.budget;
+        for (int z = 0; z < a.n_stop; ++z) stop |= a.stop[z] == tok;
+    }
+    g.len = len;
+    g.hl = hl;
+    g.steps += 1;
+    g.home = (g.home + e) % (k + 1);
+    g.done = stop ? 1ull : 0ull;
+}
+
+} // namespace rk

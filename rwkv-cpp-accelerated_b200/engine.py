@@ -78,6 +78,40 @@ def _gen_args(streams, max_new, budgets, stop, overrides, u):
     return S, slots, first, bud, stops, otok, oval, us, np.zeros((S, max_new), np.uint64), np.zeros(S, np.uint64)
 
 
+def lookup_drafts(history, draft, ngram):
+    """The k = draft prompt-lookup drafts of rwkv_b200_generate_streams_speculative for a history h (context, first token,
+    tokens emitted so far): for n = ngram down to 1 with n < len(h), the largest j <= len(h) - n - 1 with
+    h[j:j+n] == h[-n:]; the first such n proposes h[j+n : j+n+draft], padded with its last token; no match: h[-1]."""
+    h = [int(x) for x in history]
+    L = len(h)
+    for n in range(ngram, 0, -1):
+        if n >= L:
+            continue
+        tail = h[L - n:]
+        for j in range(L - n - 1, -1, -1):
+            if h[j:j + n] == tail:
+                prop = h[j + n:min(j + n + draft, L)]
+                return prop + [prop[-1]] * (draft - len(prop))
+    return [h[-1]] * draft
+
+
+def speculative_steps(context, first, tokens, draft, ngram):
+    """The steps_out a speculative call reports for a stream that emitted `tokens`: each step emits p_0 and then p_i
+    while draft i equals p_(i-1), so the emitted tokens and the draft rule decide where every step ends."""
+    h = [int(x) for x in context] + [int(first)]
+    t = [int(x) for x in tokens]
+    pos = steps = 0
+    while pos < len(t):
+        d = lookup_drafts(h, draft, ngram)
+        c = 1
+        while c <= draft and pos + c < len(t) and d[c - 1] == t[pos + c - 1]:
+            c += 1
+        h += t[pos:pos + c]
+        pos += c
+        steps += 1
+    return steps
+
+
 def lib_path():
     # RWKV_B200_LIB: A/B-test another build of the same ABI (tools/sweep.py); default is the in-tree library
     return os.environ.get("RWKV_B200_LIB") or os.path.join(_PKG, "librwkv_b200.so")
@@ -143,6 +177,9 @@ def load_library():
                                                          pull, pdbl, pull, pull, pull]),
         "rwkv_b200_beam_search": (i32, [vp, pull, pull, ull, c.c_uint, ull, pull, ull, c.c_double, c.c_uint, pull, pull, pdbl,
                                         pdbl, c.POINTER(c.c_ubyte), pdbl]),
+        "rwkv_b200_generate_streams_speculative": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull,
+                                                         c.POINTER(Sampler), pdbl, pull, pull, c.c_uint, c.c_uint, pull,
+                                                         pull, pull]),
         "rwkv_b200_batcher_open": (i32, [vp, ull, ull, c.POINTER(vp)]),
         "rwkv_b200_batcher_submit": (i32, [vp, c.POINTER(Request), pull]),
         "rwkv_b200_batcher_run": (i32, [vp, ull, pull]),
@@ -474,6 +511,34 @@ class Engine:
                 hyps.append(d)
             res.append(hyps)
         return res
+
+    def generate_speculative(self, streams, max_new, draft, ngram=3, context=None, budgets=None, stop=(), overrides=None,
+                             sampling=None, u=None):
+        """generate_streams(sampling=...) with prompt-lookup drafts (rwkv_b200_generate_streams_speculative): the same
+        tokens and first-slot states, several tokens per step where the drafts are right. streams = [(slots, first_token),
+        ...], each with draft + 1 distinct slots, the first holding the conversation (the others are scratch). context:
+        None, or one token list (or None) per stream of extra lookup tokens. sampling None is the arg-max. Returns one
+        dict per stream: "tokens" (uint64) and "steps" (the steps that emitted a token)."""
+        if any(len(slots) != draft + 1 for slots, _ in streams):
+            raise EngineError("generate_speculative: every stream needs draft + 1 = %d slots" % (draft + 1))
+        S, _, first, bud, stops, otok, oval, us, out, lens = _gen_args([(sl[0], t) for sl, t in streams], max_new, budgets,
+                                                                       stop, overrides, u)
+        slots = np.ascontiguousarray([int(s) for sl, _ in streams for s in sl], dtype=np.uint64)
+        steps = np.zeros(S, np.uint64)
+        cstart = ctx = None
+        if context is not None:
+            if len(context) != S:
+                raise EngineError("generate_speculative: %d contexts for %d streams" % (len(context), S))
+            seqs = [[int(x) for x in (c if c is not None else ())] for c in context]
+            cstart = np.ascontiguousarray(np.cumsum([0] + [len(c) for c in seqs]), dtype=np.uint64)
+            ctx = np.ascontiguousarray([x for c in seqs for x in c], dtype=np.uint64)
+        sp = _samplers(sampling, S) if sampling is not None else None
+        P = ctypes.c_ulonglong
+        self._ck(self.lib.rwkv_b200_generate_streams_speculative(
+            self.h, _ptr(slots, P), _ptr(first, P), S, max_new, _ptr(bud, P), _ptr(stops, P), len(stops), _ptr(otok, P),
+            _ptr(oval, ctypes.c_float), len(otok), sp, _ptr(us, ctypes.c_double), _ptr(out, P), _ptr(lens, P), int(draft),
+            int(ngram), _ptr(cstart, P), _ptr(ctx, P), _ptr(steps, P)), "generate_streams_speculative")
+        return [{"tokens": out[s, :int(lens[s])].copy(), "steps": int(steps[s])} for s in range(S)]
 
     def batcher(self, rows, prefill_tokens):
         """Continuous batching (include/rwkv_b200.h, rwkv_b200_batcher_open): a Batcher with at most `rows` admitted
