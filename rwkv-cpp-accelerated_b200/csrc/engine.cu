@@ -247,6 +247,12 @@ int sync_failed(M *m, cudaError_t e, const char *what) {
         cudaError_t e__ = cudaStreamSynchronize((m)->stream);            \
         if (e__ != cudaSuccess) return sync_failed((m), e__, "forward"); \
     } while (0)
+// Follows every <<<>>> launch that launch_count counts: its launch error, and one launch more.
+#define LAUNCHED(m)             \
+    do {                        \
+        CK(cudaGetLastError()); \
+        (m)->launches += 1;     \
+    } while (0)
 
 // ---- kernel dispatch on the model width -------------------------------------------------
 // CPL = 16-byte chunks per lane of an n_embed-byte row; FULL = n_embed == CPL * 512 (no tail predicates).
@@ -749,23 +755,23 @@ int gen_step_decode(M *m, int rows, const int *row_stream) {
     const size_t V = binfmt::kVocab;
     for (int r = 0; r < rows; ++r) {
         rk::k_gen_gate<<<1, 1, 0, m->stream>>>(m->gen.gs, row_stream, r, m->max_gpt, m->p.ctrl);
-        CK(cudaGetLastError());
+        LAUNCHED(m);
         int rc = launch_token(m, 0, false, nullptr, m->stream);
         if (rc) return rc;
         CK(cudaMemcpyAsync(m->d_slogits + (size_t)r * V, dev_logits(m), V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
-        m->launches += 1;
     }
     return 0;
 }
 
-// One step of generate_streams on the tensor cores: ceil(rows / per_pass) passes of per_pass rows (the last may be
-// shorter) whose descriptors are in `passes` on the device (the previous step's feedback, the group's upload, or
-// k_spec_draft); every row is a head row, so row r's logits land in d_slogits row r.
-int gen_step_passes(M *m, const rk::PassDesc *passes, int rows, int per_pass) {
+// One step on the tensor cores: ceil(rows / per_pass) passes of per_pass rows (the last may be shorter) whose
+// descriptors are in `passes` on the device (the previous step's feedback, the group's upload, or k_spec_draft). Pass i
+// has heads[i] head rows (pass_layout's count); with heads NULL every row is a head row, so row r's logits land in
+// d_slogits row r.
+int gen_step_passes(M *m, const rk::PassDesc *passes, int rows, int per_pass, const int *heads = nullptr) {
     for (int p0 = 0, pi = 0; p0 < rows; p0 += per_pass, ++pi) {
         const int T = std::min(per_pass, rows - p0);
         CK(cudaMemcpyAsync(m->pf.pass, passes + pi, sizeof(rk::PassDesc), cudaMemcpyDeviceToDevice, m->stream));
-        int rc = rk::prefill_run(m->pf, m->p, m->stream, T, T, m->d_slogits);
+        int rc = rk::prefill_run(m->pf, m->p, m->stream, T, heads ? heads[pi] : T, m->d_slogits);
         if (rc) return fail(rc, "%s", rk::prefill_error());
     }
     m->launches += rk::prefill_launches(m->pf);
@@ -787,9 +793,23 @@ int upload_step_passes(M *m, const int *rec, int rows) {
     return 0;
 }
 
+// k_beam_fork over n_pairs {source, destination} slot pairs in `forks` (device): it copies xy, aa, bb, pp and dd, or
+// without `with_pp` xy, aa, bb and dd.
+int fork_slots(M *m, const unsigned long long *forks, unsigned long long n_pairs, bool with_pp) {
+    double *a[5];
+    slot_arrays(m, 0, a);
+    const size_t slot_len = (size_t)(m->L * m->E);
+    const unsigned chunks = (unsigned)((slot_len + rk::kForkChunk - 1) / rk::kForkChunk);
+    rk::k_beam_fork<<<dim3((unsigned)n_pairs, chunks, with_pp ? 5 : 4), rk::kForkThreads, 0, m->stream>>>(
+        forks, a[0], a[1], a[2], with_pp ? a[3] : a[4], with_pp ? a[4] : nullptr, slot_len);
+    LAUNCHED(m);
+    return 0;
+}
+
 // One stream's sampler. `history`: the call keeps the stream's emitted tokens (generate_streams_ex), so the penalties
-// may be set; elsewhere they must be 0 and penalty_decay is not read.
-int check_sampler(const char *what, unsigned long long s, const rwkv_b200_sampler &p, bool history) {
+// may be set; elsewhere they must be 0 and penalty_decay is not read. `has_u`: the call was given uniforms, which a
+// temperature above 0 needs.
+int check_sampler(const char *what, unsigned long long s, const rwkv_b200_sampler &p, bool history, bool has_u) {
     if (!(p.temperature >= 0.0f && p.temperature <= FLT_MAX))
         return fail(1, "%s: stream %llu: temperature %g is not a finite value >= 0", what, s, p.temperature);
     if (!(p.top_p > 0.0f && p.top_p <= 1.0f)) return fail(1, "%s: stream %llu: top_p %g is outside (0, 1]", what, s, p.top_p);
@@ -798,14 +818,22 @@ int check_sampler(const char *what, unsigned long long s, const rwkv_b200_sample
         if (p.presence_penalty != 0.0f || p.frequency_penalty != 0.0f)
             return fail(1, "%s: stream %llu: presence_penalty and frequency_penalty must be 0 here (no token history; see "
                            "generate_streams_ex)", what, s);
-        return 0;
+    } else {
+        if (!(fabsf(p.presence_penalty) <= kMaxPenalty))
+            return fail(1, "%s: stream %llu: presence_penalty %g is not finite or exceeds %g in magnitude", what, s, p.presence_penalty, kMaxPenalty);
+        if (!(fabsf(p.frequency_penalty) <= kMaxPenalty))
+            return fail(1, "%s: stream %llu: frequency_penalty %g is not finite or exceeds %g in magnitude", what, s, p.frequency_penalty, kMaxPenalty);
+        if (!(p.penalty_decay > 0.0f && p.penalty_decay <= 1.0f))
+            return fail(1, "%s: stream %llu: penalty_decay %g is outside (0, 1]", what, s, p.penalty_decay);
     }
-    if (!(fabsf(p.presence_penalty) <= kMaxPenalty))
-        return fail(1, "%s: stream %llu: presence_penalty %g is not finite or exceeds %g in magnitude", what, s, p.presence_penalty, kMaxPenalty);
-    if (!(fabsf(p.frequency_penalty) <= kMaxPenalty))
-        return fail(1, "%s: stream %llu: frequency_penalty %g is not finite or exceeds %g in magnitude", what, s, p.frequency_penalty, kMaxPenalty);
-    if (!(p.penalty_decay > 0.0f && p.penalty_decay <= 1.0f))
-        return fail(1, "%s: stream %llu: penalty_decay %g is outside (0, 1]", what, s, p.penalty_decay);
+    if (p.temperature > 0.0f && !has_u) return fail(1, "%s: u is NULL but stream %llu samples (temperature %g)", what, s, p.temperature);
+    return 0;
+}
+
+// The uniforms u[0..n-1] (none when u is NULL), each in [0, 1).
+int check_uniforms(const char *what, const double *u, unsigned long long n) {
+    for (unsigned long long i = 0; u && i < n; ++i)
+        if (!(u[i] >= 0.0 && u[i] < 1.0)) return fail(1, "%s: u[%llu] = %g is outside [0, 1)", what, i, u[i]);
     return 0;
 }
 
@@ -874,16 +902,122 @@ int check_constraints(M *m, const char *what, const ConstraintRequest &cq, unsig
     return 0;
 }
 
+// The arguments the generate_streams calls and generate_streams_speculative share: the streams (their slots, first
+// tokens, max_new and budgets), the stop tokens, overrides, samplers (NULL: none) and uniforms, and the results.
+struct GenCall {
+    const unsigned long long *slots, *first_tokens;
+    unsigned long long n_streams, max_new;
+    const unsigned long long *budgets, *stop_tokens;
+    unsigned long long n_stop;
+    const unsigned long long *override_tokens;
+    const float *override_values;
+    unsigned long long n_override;
+    const rwkv_b200_sampler *samplers;
+    const double *u;
+    unsigned long long *tokens_out, *lengths_out;
+};
+
+// The checks of a GenCall whose streams name `per_stream` slots each. `values`: the override values are checked too.
+// `also`: a result array the caller requires as well, named `also_name` in the message.
+int check_gen(M *m, const char *what, const GenCall &c, unsigned long long per_stream, bool values, const void *also = nullptr,
+              const char *also_name = nullptr) {
+    if (c.n_streams == 0) return fail(1, "%s: no streams", what);
+    if (!c.slots || !c.first_tokens || !c.tokens_out || !c.lengths_out || (also_name && !also)) {
+        if (also_name)
+            return fail(1, "%s: null argument (slots, first_tokens, tokens_out, lengths_out and %s are required)", what, also_name);
+        return fail(1, "%s: null argument (slots, first_tokens, tokens_out and lengths_out are required)", what);
+    }
+    if (c.n_stop && !c.stop_tokens) return fail(1, "%s: n_stop = %llu with NULL stop_tokens", what, c.n_stop);
+    if (c.n_override && (!c.override_tokens || !c.override_values))
+        return fail(1, "%s: n_override = %llu with NULL override_tokens or override_values", what, c.n_override);
+    if (c.max_new == 0) return fail(1, "%s: max_new is 0", what);
+    int rc;
+    if ((rc = check_slots(m, what, c.slots, c.n_streams * per_stream)) ||
+        (rc = check_tokens(what, "first token", c.first_tokens, c.n_streams, "stream")))
+        return rc;
+    for (unsigned long long i = 0; c.budgets && i < c.n_streams; ++i)
+        if (c.budgets[i] == 0 || c.budgets[i] > c.max_new)
+            return fail(1, "%s: budget %llu of stream %llu is outside 1..max_new = %llu", what, c.budgets[i], i, c.max_new);
+    if ((rc = check_tokens(what, "stop token", c.stop_tokens, c.n_stop)) ||
+        (rc = check_tokens(what, "override token", c.override_tokens, c.n_override)) ||
+        (values && (rc = check_overrides(what, c.override_tokens, c.override_values, c.n_override))))
+        return rc;
+    for (unsigned long long s = 0; c.samplers && s < c.n_streams; ++s)
+        if ((rc = check_sampler(what, s, c.samplers[s], true, c.u != nullptr))) return rc;
+    return check_uniforms(what, c.u, c.max_new * c.n_streams);
+}
+
+// The buffers of a GenCall, grown and filled: gen.out zeroed, gen.stop, gen.ovr_tok, gen.ovr_val and gen.samp uploaded.
+int upload_gen(M *m, const GenCall &c) {
+    auto &g = m->gen;
+    int rc;
+    if ((rc = g.out.grow(c.n_streams * c.max_new)) || (rc = g.stop.grow(c.n_stop)) || (rc = g.ovr_tok.grow(c.n_override)) ||
+        (rc = g.ovr_val.grow(c.n_override)) || (c.samplers && (rc = g.samp.grow(c.n_streams))))
+        return rc;
+    CK(cudaMemsetAsync(g.out.p, 0, c.n_streams * c.max_new * sizeof(unsigned long long), m->stream));
+    if (c.n_stop) CK(cudaMemcpyAsync(g.stop.p, c.stop_tokens, c.n_stop * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    if (c.n_override) {
+        CK(cudaMemcpyAsync(g.ovr_tok.p, c.override_tokens, c.n_override * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(g.ovr_val.p, c.override_values, c.n_override * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+    }
+    if (c.samplers) CK(cudaMemcpyAsync(g.samp.p, c.samplers, c.n_streams * sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
+    return 0;
+}
+
+// What a step does to its logits rows up to the pick, in this order: the penalties (pen_cnt set), the overrides
+// (n_override > 0), the automaton masks (gc set), then one pick per row into d_sample: the nucleus sampler with each
+// row's stream's sampler (samp set), the typical sampler (a step with uniforms), or else the arg-max into d_next. Row r
+// of d_slogits belongs to stream record row_stream[r].
+struct PickChain {
+    const rk::GenStream *gs;
+    const int *row_stream;
+    const rwkv_b200_sampler *samp;
+    float *pen_cnt;
+    unsigned char *pen_seen;
+    const unsigned long long *ovr_tok;
+    const float *ovr_val;
+    unsigned long long n_override;
+    const rk::GenConstraint *gc;
+    int exponent; // the typical sampler's
+};
+
+// The chain on rows 0..rows-1 of d_slogits; u: the step's uniforms, one per row (NULL: none).
+int pick_rows(M *m, const PickChain &pc, int rows, const double *u) {
+    const size_t V = binfmt::kVocab;
+    if (pc.pen_cnt) {
+        const dim3 grid((unsigned)((V + rk::kPenaltyThreads - 1) / rk::kPenaltyThreads), (unsigned)rows);
+        rk::k_gen_penalty<<<grid, rk::kPenaltyThreads, 0, m->stream>>>(m->d_slogits, (int)V, pc.gs, pc.row_stream, pc.samp, pc.pen_cnt,
+                                                                      pc.pen_seen);
+        LAUNCHED(m);
+    }
+    if (pc.n_override) {
+        rk::k_gen_override<<<(unsigned)((rows + 127) / 128), 128, 0, m->stream>>>(m->d_slogits, (int)V, rows, pc.ovr_tok, pc.ovr_val,
+                                                                                (int)pc.n_override);
+        LAUNCHED(m);
+    }
+    if (pc.gc) {
+        const dim3 grid((unsigned)((V + rk::kMaskThreads - 1) / rk::kMaskThreads), (unsigned)rows);
+        rk::k_gen_mask<<<grid, rk::kMaskThreads, 0, m->stream>>>(m->d_slogits, (int)V, pc.gs, pc.row_stream, pc.gc);
+        LAUNCHED(m);
+    }
+    if (pc.samp)
+        rk::k_sample_nucleus<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, pc.samp, pc.row_stream, u,
+                                                                               m->d_sample);
+    else if (u)
+        rk::k_sample_typical<<<(unsigned)rows, rk::kSampleThreads, 0, m->stream>>>(m->d_slogits, V, (int)V, pc.exponent, u,
+                                                                                  m->d_sample);
+    else
+        rk::k_argmax_rows<<<(unsigned)rows, rk::kArgmaxThreads, 0, m->stream>>>(m->d_slogits, (int)V, m->d_next);
+    LAUNCHED(m);
+    return 0;
+}
+
 // The body of generate_streams (samplers == NULL, `temp` and `u` pick the typical sampler or the arg-max), of
 // generate_streams_ex (`ex`: every stream has its own sampler, or all pick the arg-max when samplers == NULL), of
 // generate_streams_logprobs (generate_streams_ex with `lpq`: each emitted token is scored after its pick) and of
 // generate_streams_constrained (with `cq`: token automata mask the rows after the overrides; `lpq` may be NULL).
-int generate(M *m, const char *what, bool ex, const unsigned long long *slots, const unsigned long long *first_tokens,
-             unsigned long long n_streams, unsigned long long max_new, const unsigned long long *budgets,
-             const unsigned long long *stop_tokens, unsigned long long n_stop, const unsigned long long *override_tokens,
-             const float *override_values, unsigned long long n_override, float temp, const rwkv_b200_sampler *samplers,
-             const double *u, unsigned long long *tokens_out, unsigned long long *lengths_out,
-             const LogprobRequest *lpq = nullptr, const ConstraintRequest *cq = nullptr) {
+int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, const LogprobRequest *lpq = nullptr,
+             const ConstraintRequest *cq = nullptr) {
     int rc = check_streams_model(m, what);
     if (rc) return rc;
     if (lpq) {
@@ -895,48 +1029,22 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
         if (lpq->top_n && (!lpq->top_tokens_out || !lpq->top_logprobs_out))
             return fail(1, "%s: top_n = %u needs top_tokens_out and top_logprobs_out", what, lpq->top_n);
     }
-    if (n_streams == 0) return fail(1, "%s: no streams", what);
-    if (!slots || !first_tokens || !tokens_out || !lengths_out)
-        return fail(1, "%s: null argument (slots, first_tokens, tokens_out and lengths_out are required)", what);
-    if (n_stop && !stop_tokens) return fail(1, "%s: n_stop = %llu with NULL stop_tokens", what, n_stop);
-    if (n_override && (!override_tokens || !override_values))
-        return fail(1, "%s: n_override = %llu with NULL override_tokens or override_values", what, n_override);
-    if (max_new == 0) return fail(1, "%s: max_new is 0", what);
+    if ((rc = check_gen(m, what, c, 1, ex))) return rc;
     const size_t V = binfmt::kVocab;
-    if ((rc = check_slots(m, what, slots, n_streams)) || (rc = check_tokens(what, "first token", first_tokens, n_streams, "stream")))
-        return rc;
-    for (unsigned long long i = 0; budgets && i < n_streams; ++i)
-        if (budgets[i] == 0 || budgets[i] > max_new)
-            return fail(1, "%s: budget %llu of stream %llu is outside 1..max_new = %llu", what, budgets[i], i, max_new);
-    if ((rc = check_tokens(what, "stop token", stop_tokens, n_stop)) ||
-        (rc = check_tokens(what, "override token", override_tokens, n_override)))
-        return rc;
+    const unsigned long long n_streams = c.n_streams, max_new = c.max_new;
     bool pen = false; // some stream has a presence or frequency penalty
-    if (ex) {
-        if ((rc = check_overrides(what, override_tokens, override_values, n_override))) return rc;
-        for (unsigned long long s = 0; samplers && s < n_streams; ++s) {
-            if ((rc = check_sampler(what, s, samplers[s], true))) return rc;
-            if (samplers[s].temperature > 0.0f && !u)
-                return fail(1, "%s: u is NULL but stream %llu samples (temperature %g)", what, s, samplers[s].temperature);
-            pen |= samplers[s].presence_penalty != 0.0f || samplers[s].frequency_penalty != 0.0f;
-        }
-    }
-    if (u)
-        for (unsigned long long i = 0; i < max_new * n_streams; ++i)
-            if (!(u[i] >= 0.0 && u[i] < 1.0)) return fail(1, "%s: u[%llu] = %g is outside [0, 1)", what, i, u[i]);
+    for (unsigned long long s = 0; c.samplers && s < n_streams; ++s)
+        pen |= c.samplers[s].presence_penalty != 0.0f || c.samplers[s].frequency_penalty != 0.0f;
     std::vector<rk::GenConstraint> hgc;
-    if (cq && (rc = check_constraints(m, what, *cq, n_streams, override_tokens, override_values, n_override, hgc))) return rc;
-    const bool constrained = std::any_of(hgc.begin(), hgc.end(), [](const rk::GenConstraint &c) { return c.mask != nullptr; });
+    if (cq && (rc = check_constraints(m, what, *cq, n_streams, c.override_tokens, c.override_values, c.n_override, hgc))) return rc;
+    const bool constrained = std::any_of(hgc.begin(), hgc.end(), [](const rk::GenConstraint &gc) { return gc.mask != nullptr; });
     CK(cudaSetDevice(m->device));
     auto &g = m->gen;
     if (constrained && ((rc = g.gc.grow(n_streams)) || (rc = g.fault.grow(3)))) return rc;
-    if (samplers && (rc = g.samp.grow(n_streams))) return rc;
     if (pen && ((rc = g.pen_cnt.grow(n_streams * V)) || (rc = g.pen_seen.grow(n_streams * V)))) return rc;
-    if ((rc = g.out.grow(n_streams * max_new)) || (rc = g.stop.grow(n_stop)) || (rc = g.ovr_tok.grow(n_override)) ||
-        (rc = g.ovr_val.grow(n_override)) || (u && (rc = g.u.grow(kGenGroup * m->max_gpt))))
-        return rc;
+    if (c.u && (rc = g.u.grow(kGenGroup * m->max_gpt))) return rc;
     // raw mode reads the model's rows: d_slogits itself, or a copy taken before the penalties, overrides and mask edit it
-    const bool raw_copy = lpq && lpq->mode == RWKV_B200_LOGPROBS_RAW && (pen || n_override || constrained);
+    const bool raw_copy = lpq && lpq->mode == RWKV_B200_LOGPROBS_RAW && (pen || c.n_override || constrained);
     const size_t n_lp = (size_t)(n_streams * max_new), n_top = lpq ? n_lp * lpq->top_n : 0;
     if (lpq && ((rc = g.lp.grow(n_lp)) || (rc = g.rank.grow(n_lp)) || (rc = g.top_tok.grow(n_top)) || (rc = g.top_lp.grow(n_top)) ||
                 (raw_copy && (rc = g.raw.grow(n_streams * V)))))
@@ -947,15 +1055,10 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
     m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
 
     rk::GenStream *hg = g.h_gs;
-    for (unsigned long long s = 0; s < n_streams; ++s) hg[s] = rk::GenStream{slots[s], budgets ? budgets[s] : max_new, first_tokens[s], 0, 0};
+    for (unsigned long long s = 0; s < n_streams; ++s)
+        hg[s] = rk::GenStream{c.slots[s], c.budgets ? c.budgets[s] : max_new, c.first_tokens[s], 0, 0};
     CK(cudaMemcpyAsync(g.gs, hg, n_streams * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
-    CK(cudaMemsetAsync(g.out.p, 0, n_streams * max_new * sizeof(unsigned long long), m->stream));
-    if (n_stop) CK(cudaMemcpyAsync(g.stop.p, stop_tokens, n_stop * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-    if (n_override) {
-        CK(cudaMemcpyAsync(g.ovr_tok.p, override_tokens, n_override * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(g.ovr_val.p, override_values, n_override * sizeof(float), cudaMemcpyHostToDevice, m->stream));
-    }
-    if (samplers) CK(cudaMemcpyAsync(g.samp.p, samplers, n_streams * sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
+    if ((rc = upload_gen(m, c))) return rc;
     if (constrained) {
         CK(cudaMemcpyAsync(g.gc.p, hgc.data(), n_streams * sizeof(rk::GenConstraint), cudaMemcpyHostToDevice, m->stream));
         CK(cudaMemsetAsync(g.fault.p, 0, 3 * sizeof(unsigned long long), m->stream));
@@ -975,66 +1078,38 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
     std::vector<int> live(n_streams);
     for (unsigned long long s = 0; s < n_streams; ++s) live[s] = (int)s;
     std::vector<double> ug;
-    const int exponent = sample_exponent(temp);
+    const PickChain pc{g.gs, g.row_stream, c.samplers ? g.samp.p : nullptr, pen ? g.pen_cnt.p : nullptr, g.pen_seen.p,
+                       g.ovr_tok.p, g.ovr_val.p, c.n_override, constrained ? g.gc.p : nullptr, sample_exponent(temp)};
     for (unsigned long long step = 0; !live.empty() && step < max_new;) {
         // a group: the live streams are rows 0..rows-1; their inputs, and the uniforms of its steps, go up once
         const int rows = (int)live.size();
         const unsigned long long steps = std::min(kGenGroup, max_new - step);
         CK(cudaMemcpyAsync(g.row_stream, live.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
         if (tc && (rc = upload_step_passes(m, live.data(), rows))) return rc;
-        if (u) {
+        if (c.u) {
             ug.resize((size_t)steps * rows);
             for (unsigned long long k = 0; k < steps; ++k)
-                for (int r = 0; r < rows; ++r) ug[k * rows + r] = u[(step + k) * n_streams + live[r]];
+                for (int r = 0; r < rows; ++r) ug[k * rows + r] = c.u[(step + k) * n_streams + live[r]];
             CK(cudaMemcpyAsync(g.u.p, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
         }
-        rk::GenFeedbackArgs fb{g.gs, g.row_stream, rows, u || samplers ? nullptr : m->d_next, m->d_sample, g.stop.p, (int)n_stop, g.out.p,
-                               max_new, tc ? g.passes : nullptr, constrained ? g.gc.p : nullptr, g.fault.p};
+        rk::GenFeedbackArgs fb{g.gs, g.row_stream, rows, c.u || c.samplers ? nullptr : m->d_next, m->d_sample, g.stop.p, (int)c.n_stop,
+                               g.out.p, max_new, tc ? g.passes : nullptr, constrained ? g.gc.p : nullptr, g.fault.p};
         rk::GenLogprobArgs la{};
         if (lpq)
             la = rk::GenLogprobArgs{raw_copy ? g.raw.p : m->d_slogits, (int)V, g.gs, g.row_stream, fb.next, m->d_sample,
-                                    lpq->mode == RWKV_B200_LOGPROBS_PROCESSED ? samplers ? g.samp.p : nullptr : nullptr,
-                                    (int)lpq->top_n, max_new, g.lp.p, g.rank.p, g.top_tok.p, g.top_lp.p};
-        const unsigned rb = (unsigned)((rows + 127) / 128);
+                                    lpq->mode == RWKV_B200_LOGPROBS_PROCESSED ? pc.samp : nullptr, (int)lpq->top_n, max_new,
+                                    g.lp.p, g.rank.p, g.top_tok.p, g.top_lp.p};
         for (unsigned long long k = 0; k < steps; ++k) {
             if ((rc = tc ? gen_step_passes(m, g.passes, rows, rk::kPfMaxTokens) : gen_step_decode(m, rows, g.row_stream))) return rc;
             if (raw_copy)
                 CK(cudaMemcpyAsync(g.raw.p, m->d_slogits, (size_t)rows * V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
-            if (pen) {
-                const dim3 grid((unsigned)((V + rk::kPenaltyThreads - 1) / rk::kPenaltyThreads), (unsigned)rows);
-                rk::k_gen_penalty<<<grid, rk::kPenaltyThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs, g.row_stream, g.samp.p,
-                                                                              g.pen_cnt.p, g.pen_seen.p);
-                CK(cudaGetLastError());
-                m->launches += 1;
-            }
-            if (n_override) {
-                rk::k_gen_override<<<rb, 128, 0, m->stream>>>(m->d_slogits, (int)V, rows, g.ovr_tok.p, g.ovr_val.p, (int)n_override);
-                CK(cudaGetLastError());
-                m->launches += 1;
-            }
-            if (constrained) {
-                const dim3 grid((unsigned)((V + rk::kMaskThreads - 1) / rk::kMaskThreads), (unsigned)rows);
-                rk::k_gen_mask<<<grid, rk::kMaskThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs, g.row_stream, g.gc.p);
-                CK(cudaGetLastError());
-                m->launches += 1;
-            }
-            if (samplers)
-                rk::k_sample_nucleus<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.samp.p, g.row_stream,
-                                                                                       u ? g.u.p + k * rows : nullptr, m->d_sample);
-            else if (u)
-                rk::k_sample_typical<<<(unsigned)rows, rk::kSampleThreads, 0, m->stream>>>(m->d_slogits, V, (int)V, exponent,
-                                                                                          g.u.p + k * rows, m->d_sample);
-            else
-                rk::k_argmax_rows<<<(unsigned)rows, rk::kArgmaxThreads, 0, m->stream>>>(m->d_slogits, (int)V, m->d_next);
-            CK(cudaGetLastError());
+            if ((rc = pick_rows(m, pc, rows, c.u ? g.u.p + k * rows : nullptr))) return rc;
             if (lpq) {
                 rk::k_gen_logprob<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(la);
-                CK(cudaGetLastError());
-                m->launches += 1;
+                LAUNCHED(m);
             }
-            rk::k_gen_feedback<<<rb, 128, 0, m->stream>>>(fb);
-            CK(cudaGetLastError());
-            m->launches += 2;
+            rk::k_gen_feedback<<<(unsigned)((rows + 127) / 128), 128, 0, m->stream>>>(fb);
+            LAUNCHED(m);
         }
         // the end of a group: which streams are done (a few bytes, one synchronisation); drop them from the rows
         CK(cudaMemcpyAsync(hg, g.gs, n_streams * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
@@ -1047,7 +1122,7 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
         step += steps;
         live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hg[s].done != 0; }), live.end());
     }
-    CK(cudaMemcpyAsync(tokens_out, g.out.p, n_streams * max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+    CK(cudaMemcpyAsync(c.tokens_out, g.out.p, n_streams * max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
     if (lpq) {
         CK(cudaMemcpyAsync(lpq->logprobs_out, g.lp.p, n_lp * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
         if (lpq->ranks_out) CK(cudaMemcpyAsync(lpq->ranks_out, g.rank.p, n_lp * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
@@ -1059,315 +1134,9 @@ int generate(M *m, const char *what, bool ex, const unsigned long long *slots, c
     if (constrained && cq->states_out)
         CK(cudaMemcpyAsync(hgc.data(), g.gc.p, n_streams * sizeof(rk::GenConstraint), cudaMemcpyDeviceToHost, m->stream));
     SYNC(m);
-    for (unsigned long long s = 0; s < n_streams; ++s) lengths_out[s] = hg[s].len;
+    for (unsigned long long s = 0; s < n_streams; ++s) c.lengths_out[s] = hg[s].len;
     if (cq && cq->states_out)
         for (unsigned long long s = 0; s < n_streams; ++s) cq->states_out[s] = hgc[s].mask ? hgc[s].state : 0;
-    return 0;
-}
-
-// The body of rwkv_b200_beam_search: generate()'s group loop over beams. Step 0 has one row per group, later steps B
-// rows per live group (group by group); each step is forward -> k_beam_expand -> k_beam_select -> k_beam_fork. At each
-// host group's end the done flags come back and the done groups leave the rows; at the end the backpointers and the
-// hypothesis lists come back once and the host rebuilds each hypothesis' tokens.
-int beam(M *m, const unsigned long long *slots, const unsigned long long *first_tokens, unsigned long long n_groups,
-         unsigned beams, unsigned long long max_new, const unsigned long long *stop_tokens, unsigned long long n_stop,
-         double length_penalty, unsigned n_best, unsigned long long *tokens_out, unsigned long long *lengths_out,
-         double *logprobs_out, double *scores_out, unsigned char *finished_out, double *token_logprobs_out) {
-    const char *what = "beam_search";
-    int rc = check_streams_model(m, what);
-    if (rc) return rc;
-    if (!slots || !first_tokens || !tokens_out || !lengths_out || !logprobs_out || !scores_out || !finished_out)
-        return fail(1, "%s: null argument (slots, first_tokens, tokens_out, lengths_out, logprobs_out, scores_out and "
-                       "finished_out are required)", what);
-    if (n_stop && !stop_tokens) return fail(1, "%s: n_stop = %llu with NULL stop_tokens", what, n_stop);
-    if (n_groups == 0) return fail(1, "%s: no groups", what);
-    if (beams == 0) return fail(1, "%s: beams is 0", what);
-    if (n_stop > (unsigned long long)rk::kMaxTopN || beams + n_stop > (unsigned long long)rk::kMaxTopN)
-        return fail(1, "%s: beams + n_stop = %u + %llu > %d", what, beams, n_stop, rk::kMaxTopN);
-    if (n_best == 0 || n_best > beams) return fail(1, "%s: n_best %u is outside 1..beams = %u", what, n_best, beams);
-    if (max_new == 0) return fail(1, "%s: max_new is 0", what);
-    if (!std::isfinite(length_penalty)) return fail(1, "%s: length_penalty %g is not finite", what, length_penalty);
-    if (n_groups > m->max_gpt) return fail(1, "%s: %llu groups > max_gpt %llu", what, n_groups, m->max_gpt);
-    const size_t V = binfmt::kVocab;
-    const unsigned long long G = n_groups, B = beams, K = n_best, N = max_new, C = B + n_stop;
-    if ((rc = check_slots(m, what, slots, G * B)) || (rc = check_tokens(what, "first token", first_tokens, G, "group")) ||
-        (rc = check_tokens(what, "stop token", stop_tokens, n_stop)))
-        return rc;
-    // the length penalties on the host, with the C library's pow: a host restatement gets the same bits
-    if (N > ((unsigned long long)SIZE_MAX / sizeof(rk::BeamBack)) / (G * B))
-        return fail(1, "%s: max_new = %llu: the backpointers of %llu beams do not fit in memory", what, N, G * B);
-    std::vector<double> P;
-    try {
-        P.assign(N + 1, 0.0);
-    } catch (const std::exception &) {
-        return fail(9, "%s: out of host memory for max_new = %llu", what, N);
-    }
-    for (unsigned long long n = 1; n <= N; ++n) P[n] = pow((double)n, length_penalty);
-    CK(cudaSetDevice(m->device));
-    auto &g = m->gen;
-    auto &bm = m->beam;
-    if ((rc = g.stop.grow(n_stop)) || (rc = bm.row0.grow(G)) || (rc = bm.groups.grow(G)) || (rc = bm.cand_tok.grow(G * B * C)) ||
-        (rc = bm.cand_lp.grow(G * B * C)) || (rc = bm.cum.grow(G * B)) || (rc = bm.P.grow(N + 1)) || (rc = bm.back.grow(G * N * B)) ||
-        (rc = bm.hyp.grow(G * K)) || (rc = bm.n_hyp.grow(G)) || (rc = bm.done.grow(G)) || (rc = bm.forks.grow(2 * G * B)))
-        return rc;
-    // the path is chosen once, for G x B one-token streams
-    const bool tc = tensor_cores(m, G * B);
-    if (tc && (rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
-    m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
-
-    rk::GenStream *hg = g.h_gs;
-    for (unsigned long long s = 0; s < G * B; ++s) hg[s] = rk::GenStream{slots[s], N, s % B == 0 ? first_tokens[s / B] : 0, 0, 0};
-    std::vector<int> row0(G), live(G);
-    for (unsigned long long i = 0; i < G; ++i) {
-        row0[i] = (int)(i * B);
-        live[i] = (int)i;
-    }
-    CK(cudaMemcpyAsync(g.gs, hg, G * B * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
-    CK(cudaMemcpyAsync(bm.row0.p, row0.data(), G * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-    CK(cudaMemcpyAsync(bm.P.p, P.data(), (N + 1) * sizeof(double), cudaMemcpyHostToDevice, m->stream));
-    if (n_stop) CK(cudaMemcpyAsync(g.stop.p, stop_tokens, n_stop * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-    CK(cudaMemsetAsync(bm.cum.p, 0, G * B * sizeof(double), m->stream));
-    CK(cudaMemsetAsync(bm.n_hyp.p, 0, G * sizeof(int), m->stream));
-    CK(cudaMemsetAsync(bm.done.p, 0, G * sizeof(unsigned long long), m->stream));
-    double *arr[5];
-    slot_arrays(m, 0, arr);
-    const size_t slot_len = (size_t)(m->L * m->E);
-    const unsigned chunks = (unsigned)((slot_len + rk::kForkChunk - 1) / rk::kForkChunk);
-    std::vector<unsigned long long> hdone(G, 0);
-    std::vector<int> rs;
-    for (unsigned long long step = 0; !live.empty() && step < N;) {
-        // a host group: the live groups' beams are rows gi * B + j (step 0: row gi); their inputs go up once
-        const int Gl = (int)live.size();
-        const unsigned long long steps = std::min(kGenGroup, N - step);
-        rs.resize((size_t)Gl * B);
-        for (int gi = 0; gi < Gl; ++gi)
-            for (unsigned long long j = 0; j < B; ++j) rs[gi * B + j] = (int)(live[gi] * B + j);
-        CK(cudaMemcpyAsync(g.row_stream, rs.data(), rs.size() * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(bm.groups.p, live.data(), Gl * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-        if (tc && (rc = upload_step_passes(m, step == 0 ? row0.data() : rs.data(), step == 0 ? Gl : Gl * (int)B))) return rc;
-        rk::BeamArgs ba{g.gs, bm.cum.p, bm.groups.p, bm.cand_tok.p, bm.cand_lp.p, (int)C, (int)B, (int)K, 0, 0, N, bm.P.p,
-                        length_penalty < 0.0 ? 1 : 0, g.stop.p, (int)n_stop, bm.back.p, bm.hyp.p, bm.n_hyp.p, bm.done.p, bm.forks.p,
-                        tc ? g.passes : nullptr};
-        for (unsigned long long k = 0; k < steps; ++k) {
-            const unsigned long long st = step + k;
-            const int nb = st == 0 ? 1 : (int)B, rows = Gl * nb;
-            const int *rmap = st == 0 ? bm.row0.p : g.row_stream;
-            if ((rc = tc ? gen_step_passes(m, g.passes, rows, rk::kPfMaxTokens) : gen_step_decode(m, rows, rmap))) return rc;
-            rk::k_beam_expand<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs, rmap, (int)C,
-                                                                                bm.cand_tok.p, bm.cand_lp.p);
-            CK(cudaGetLastError());
-            ba.step = (int)st;
-            ba.nb = nb;
-            rk::k_beam_select<<<(unsigned)Gl, rk::kBeamSelectThreads, 0, m->stream>>>(ba);
-            CK(cudaGetLastError());
-            m->launches += 2;
-            if (st + 1 < N) { // after the last step every group is done and forks nothing
-                rk::k_beam_fork<<<dim3((unsigned)(Gl * B), chunks, 5), rk::kForkThreads, 0, m->stream>>>(
-                    bm.forks.p, arr[0], arr[1], arr[2], arr[3], arr[4], slot_len);
-                CK(cudaGetLastError());
-                m->launches += 1;
-            }
-        }
-        // the end of a host group: which groups are done and the beams' records (one synchronisation)
-        CK(cudaMemcpyAsync(hdone.data(), bm.done.p, G * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
-        CK(cudaMemcpyAsync(hg, g.gs, G * B * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
-        SYNC(m);
-        step += steps;
-        live.erase(std::remove_if(live.begin(), live.end(), [&](int gg) { return hdone[gg] != 0; }), live.end());
-    }
-    std::vector<rk::BeamHyp> hyp(G * K);
-    std::vector<rk::BeamBack> back(G * N * B);
-    CK(cudaMemcpyAsync(hyp.data(), bm.hyp.p, G * K * sizeof(rk::BeamHyp), cudaMemcpyDeviceToHost, m->stream));
-    CK(cudaMemcpyAsync(back.data(), bm.back.p, G * N * B * sizeof(rk::BeamBack), cudaMemcpyDeviceToHost, m->stream));
-    SYNC(m);
-    // each hypothesis' tokens: its last token, then the backpointers of its beam from its step down to step 0
-    const double nan = std::nan("");
-    for (unsigned long long gg = 0; gg < G; ++gg)
-        for (unsigned long long i = 0; i < K; ++i) {
-            const rk::BeamHyp &h = hyp[gg * K + i];
-            const size_t o = (size_t)(gg * K + i);
-            unsigned long long *tok = tokens_out + o * N;
-            double *tlp = token_logprobs_out ? token_logprobs_out + o * N : nullptr;
-            for (unsigned long long t = 0; t < N; ++t) {
-                tok[t] = 0;
-                if (tlp) tlp[t] = nan;
-            }
-            tok[h.step] = h.tok;
-            if (tlp) tlp[h.step] = h.lp;
-            for (int s = h.step - 1, p = h.parent; s >= 0; --s) {
-                const rk::BeamBack &bk = back[(gg * N + (unsigned long long)s) * B + (unsigned long long)p];
-                tok[s] = bk.tok;
-                if (tlp) tlp[s] = bk.lp;
-                p = bk.parent;
-            }
-            lengths_out[o] = (unsigned long long)h.len;
-            logprobs_out[o] = h.cum;
-            scores_out[o] = h.score;
-            finished_out[o] = (unsigned char)h.finished;
-        }
-    return 0;
-}
-
-// The body of rwkv_b200_generate_streams_speculative: generate()'s group loop with k + 1 rows per live stream. Each
-// step is k_spec_draft -> passes -> overrides -> pick -> k_spec_accept; at each group's end the records come back and
-// the finished streams leave the rows. At the end a stream whose home is a spare has it copied to its first slot.
-int speculate(M *m, const unsigned long long *slots, const unsigned long long *first_tokens, unsigned long long n_streams,
-              unsigned long long max_new, const unsigned long long *budgets, const unsigned long long *stop_tokens,
-              unsigned long long n_stop, const unsigned long long *override_tokens, const float *override_values,
-              unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u, unsigned long long *tokens_out,
-              unsigned long long *lengths_out, unsigned draft, unsigned ngram, const unsigned long long *context_start,
-              const unsigned long long *context, unsigned long long *steps_out) {
-    const char *what = "generate_streams_speculative";
-    int rc = check_streams_model(m, what);
-    if (rc) return rc;
-    if (n_streams == 0) return fail(1, "%s: no streams", what);
-    if (!slots || !first_tokens || !tokens_out || !lengths_out || !steps_out)
-        return fail(1, "%s: null argument (slots, first_tokens, tokens_out, lengths_out and steps_out are required)", what);
-    if (n_stop && !stop_tokens) return fail(1, "%s: n_stop = %llu with NULL stop_tokens", what, n_stop);
-    if (n_override && (!override_tokens || !override_values))
-        return fail(1, "%s: n_override = %llu with NULL override_tokens or override_values", what, n_override);
-    if (max_new == 0) return fail(1, "%s: max_new is 0", what);
-    if (draft < 1 || draft > (unsigned)rk::kSpecMaxDraft) return fail(1, "%s: draft %u is outside 1..%d", what, draft, rk::kSpecMaxDraft);
-    if (ngram < 1 || ngram > (unsigned)rk::kSpecMaxNgram) return fail(1, "%s: ngram %u is outside 1..%d", what, ngram, rk::kSpecMaxNgram);
-    if (!rk::prefill_enabled(m->pf)) return fail(1, "%s: needs the tensor cores (the \"prefill\" option is 0)", what);
-    const unsigned long long K1 = draft + 1ull, S = n_streams;
-    if (S > m->max_gpt / K1)
-        return fail(1, "%s: %llu streams x %llu rows > max_gpt %llu", what, S, K1, m->max_gpt);
-    if ((rc = check_slots(m, what, slots, S * K1)) || (rc = check_tokens(what, "first token", first_tokens, S, "stream")) ||
-        (rc = check_tokens(what, "stop token", stop_tokens, n_stop)) ||
-        (rc = check_tokens(what, "override token", override_tokens, n_override)) ||
-        (rc = check_overrides(what, override_tokens, override_values, n_override)))
-        return rc;
-    for (unsigned long long i = 0; budgets && i < S; ++i)
-        if (budgets[i] == 0 || budgets[i] > max_new)
-            return fail(1, "%s: budget %llu of stream %llu is outside 1..max_new = %llu", what, budgets[i], i, max_new);
-    for (unsigned long long s = 0; samplers && s < S; ++s) {
-        if ((rc = check_sampler(what, s, samplers[s], true))) return rc;
-        if (samplers[s].presence_penalty != 0.0f || samplers[s].frequency_penalty != 0.0f)
-            return fail(1, "%s: stream %llu: presence and frequency penalties are not supported (a row's counts would have "
-                           "to include its own drafts)", what, s);
-        if (samplers[s].temperature > 0.0f && !u)
-            return fail(1, "%s: u is NULL but stream %llu samples (temperature %g)", what, s, samplers[s].temperature);
-    }
-    if (!samplers) u = nullptr; // every stream takes the arg-max
-    if (u)
-        for (unsigned long long i = 0; i < max_new * S; ++i)
-            if (!(u[i] >= 0.0 && u[i] < 1.0)) return fail(1, "%s: u[%llu] = %g is outside [0, 1)", what, i, u[i]);
-    unsigned long long n_ctx = 0;
-    if (context_start) {
-        if (context_start[0] != 0) return fail(1, "%s: context_start[0] = %llu, not 0", what, context_start[0]);
-        for (unsigned long long s = 0; s < S; ++s)
-            if (context_start[s + 1] < context_start[s])
-                return fail(1, "%s: context_start decreases from stream %llu to %llu (%llu > %llu)", what, s, s + 1,
-                            context_start[s], context_start[s + 1]);
-        n_ctx = context_start[S];
-        if (n_ctx && !context) return fail(1, "%s: %llu context tokens with NULL context", what, n_ctx);
-        if ((rc = check_tokens(what, "context token", context, n_ctx))) return rc;
-    }
-    const size_t V = binfmt::kVocab;
-    const unsigned long long n_hist = n_ctx + S * (1 + max_new);
-    CK(cudaSetDevice(m->device));
-    auto &g = m->gen;
-    auto &sp = m->spec;
-    const int per_pass = rk::kPfMaxTokens / (int)K1; // streams per pass: a stream's rows never straddle two passes
-    const size_t n_pass = (size_t)((S + per_pass - 1) / per_pass);
-    if ((rc = g.out.grow(S * max_new)) || (rc = g.stop.grow(n_stop)) || (rc = g.ovr_tok.grow(n_override)) ||
-        (rc = g.ovr_val.grow(n_override)) || (samplers && (rc = g.samp.grow(S))) || (rc = sp.ss.grow(S)) ||
-        (rc = sp.hist.grow(n_hist)) || (rc = sp.live.grow(S)) || (rc = sp.passes.grow(n_pass)) ||
-        (u && ((rc = sp.u.grow(max_new * S)) || (rc = sp.row_u.grow(S * K1)))) || (rc = sp.forks.grow(2 * S)))
-        return rc;
-    if ((rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
-    m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
-
-    // the records and the histories: stream s's history starts with its context and its first token
-    std::vector<rk::SpecStream> hs(S);
-    std::vector<unsigned long long> hist(n_hist, 0); // stream s: its context, its first token, then room for max_new
-    for (unsigned long long s = 0, h0 = 0; s < S; ++s) {
-        rk::SpecStream &r = hs[s];
-        r = rk::SpecStream{};
-        for (unsigned long long i = 0; i < K1; ++i) r.slot[i] = slots[s * K1 + i];
-        const unsigned long long c0 = context_start ? context_start[s] : 0, c1 = context_start ? context_start[s + 1] : 0;
-        r.h0 = h0;
-        r.hl = c1 - c0 + 1;
-        r.budget = budgets ? budgets[s] : max_new;
-        std::copy(context + c0, context + c1, hist.begin() + h0);
-        hist[h0 + c1 - c0] = first_tokens[s];
-        h0 += r.hl + max_new;
-    }
-    CK(cudaMemcpyAsync(sp.hist.p, hist.data(), n_hist * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-    CK(cudaMemcpyAsync(sp.ss.p, hs.data(), S * sizeof(rk::SpecStream), cudaMemcpyHostToDevice, m->stream));
-    CK(cudaMemsetAsync(g.out.p, 0, S * max_new * sizeof(unsigned long long), m->stream));
-    if (n_stop) CK(cudaMemcpyAsync(g.stop.p, stop_tokens, n_stop * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-    if (n_override) {
-        CK(cudaMemcpyAsync(g.ovr_tok.p, override_tokens, n_override * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(g.ovr_val.p, override_values, n_override * sizeof(float), cudaMemcpyHostToDevice, m->stream));
-    }
-    if (samplers) CK(cudaMemcpyAsync(g.samp.p, samplers, S * sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
-    if (u) CK(cudaMemcpyAsync(sp.u.p, u, max_new * S * sizeof(double), cudaMemcpyHostToDevice, m->stream));
-
-    std::vector<int> live(S), rs;
-    for (unsigned long long s = 0; s < S; ++s) live[s] = (int)s;
-    rk::SpecArgs sa{sp.ss.p, sp.live.p, (int)draft, (int)ngram, per_pass, sp.hist.p, sp.passes.p, u ? sp.u.p : nullptr,
-                    sp.row_u.p, S, max_new, samplers ? nullptr : m->d_next, m->d_sample, g.stop.p, (int)n_stop, g.out.p};
-    // each step emits at least one token per live stream, so max_new steps finish every stream
-    for (unsigned long long step = 0; !live.empty() && step < max_new;) {
-        const int n_live = (int)live.size(), rows = n_live * (int)K1;
-        const unsigned long long steps = std::min(kGenGroup, max_new - step);
-        rs.resize(rows);
-        for (int r = 0; r < rows; ++r) rs[r] = live[r / (int)K1];
-        CK(cudaMemcpyAsync(sp.live.p, live.data(), n_live * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(g.row_stream, rs.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-        for (unsigned long long k = 0; k < steps; ++k) {
-            rk::k_spec_draft<<<(unsigned)n_live, rk::kSpecDraftThreads, 0, m->stream>>>(sa);
-            CK(cudaGetLastError());
-            m->launches += 1;
-            if ((rc = gen_step_passes(m, sp.passes.p, rows, per_pass * (int)K1))) return rc;
-            if (n_override) {
-                rk::k_gen_override<<<(unsigned)((rows + 127) / 128), 128, 0, m->stream>>>(m->d_slogits, (int)V, rows, g.ovr_tok.p,
-                                                                                        g.ovr_val.p, (int)n_override);
-                CK(cudaGetLastError());
-                m->launches += 1;
-            }
-            if (samplers)
-                rk::k_sample_nucleus<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.samp.p, g.row_stream,
-                                                                                       u ? sp.row_u.p : nullptr, m->d_sample);
-            else
-                rk::k_argmax_rows<<<(unsigned)rows, rk::kArgmaxThreads, 0, m->stream>>>(m->d_slogits, (int)V, m->d_next);
-            CK(cudaGetLastError());
-            rk::k_spec_accept<<<(unsigned)n_live, 32, 0, m->stream>>>(sa);
-            CK(cudaGetLastError());
-            m->launches += 2;
-        }
-        // the end of a group: which streams are done (one synchronisation); drop them from the rows
-        CK(cudaMemcpyAsync(hs.data(), sp.ss.p, S * sizeof(rk::SpecStream), cudaMemcpyDeviceToHost, m->stream));
-        SYNC(m);
-        step += steps;
-        live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hs[s].done != 0; }), live.end());
-    }
-    // a home on a spare: its xy, aa, bb and dd go to the first slot (pp: no forward writes it)
-    std::vector<unsigned long long> forks;
-    for (unsigned long long s = 0; s < S; ++s)
-        if (hs[s].home != 0) {
-            forks.push_back(hs[s].slot[hs[s].home]);
-            forks.push_back(hs[s].slot[0]);
-        }
-    if (!forks.empty()) {
-        double *arr[5];
-        slot_arrays(m, 0, arr);
-        const size_t slot_len = (size_t)(m->L * m->E);
-        const unsigned chunks = (unsigned)((slot_len + rk::kForkChunk - 1) / rk::kForkChunk);
-        CK(cudaMemcpyAsync(sp.forks.p, forks.data(), forks.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-        rk::k_beam_fork<<<dim3((unsigned)(forks.size() / 2), chunks, 4), rk::kForkThreads, 0, m->stream>>>(
-            sp.forks.p, arr[0], arr[1], arr[2], arr[4], nullptr, slot_len);
-        CK(cudaGetLastError());
-        m->launches += 1;
-    }
-    CK(cudaMemcpyAsync(tokens_out, g.out.p, S * max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
-    SYNC(m);
-    for (unsigned long long s = 0; s < S; ++s) {
-        lengths_out[s] = hs[s].len;
-        steps_out[s] = hs[s].steps;
-    }
     return 0;
 }
 
@@ -1432,7 +1201,6 @@ int batcher_boundary(B *b, std::vector<int> &dec) {
 // rows' tokens and kDescLast bits into step k + 1's layout.
 int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
     M *m = b->m;
-    const size_t V = binfmt::kVocab;
     std::vector<int> dec;
     int rc = batcher_boundary(b, dec);
     if (rc) return rc;
@@ -1465,7 +1233,8 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
     const unsigned long long steps = segs.size();
     // every step's layout: decode rows (head rows 0..R-1), then the segments without a head
     std::vector<rk::PassDesc> all(steps * (size_t)b->max_pass);
-    std::vector<std::vector<int>> T(steps), H(steps);
+    std::vector<int> step_rows(steps);
+    std::vector<std::vector<int>> H(steps);
     for (unsigned long long k = 0; k < steps; ++k) {
         std::vector<unsigned long long> tokens, slots, lens;
         std::vector<unsigned char> head;
@@ -1482,13 +1251,10 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
             lens.push_back(s.n);
             head.push_back(0);
         }
-        const int n = (int)tokens.size();
+        step_rows[k] = (int)tokens.size();
         std::vector<rk::PassDesc> passes;
-        rk::pass_layout(tokens.data(), n, slots.data(), lens.data(), 2, nullptr, passes, H[k], head.data());
-        for (size_t i = 0; i < passes.size(); ++i) {
-            all[k * b->max_pass + i] = passes[i];
-            T[k].push_back(std::min(rk::kPfMaxTokens, n - (int)i * rk::kPfMaxTokens));
-        }
+        rk::pass_layout(tokens.data(), step_rows[k], slots.data(), lens.data(), 2, nullptr, passes, H[k], head.data());
+        std::copy(passes.begin(), passes.end(), all.begin() + k * b->max_pass);
     }
     CK(cudaMemcpyAsync(b->passes.p, all.data(), all.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
     bool pen = false;
@@ -1508,31 +1274,16 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
         }
         CK(cudaMemcpyAsync(b->u.p, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
     }
-    const unsigned rb = (unsigned)((R + 127) / 128);
+    const PickChain pc{b->gs.p, b->row_stream.p, b->samp.p, pen ? b->pen_cnt.p : nullptr, b->pen_seen.p};
     for (unsigned long long k = 0; k < steps; ++k) {
-        const rk::PassDesc *step = b->passes.p + k * b->max_pass;
-        for (size_t i = 0; i < T[k].size(); ++i) {
-            CK(cudaMemcpyAsync(m->pf.pass, step + i, sizeof(rk::PassDesc), cudaMemcpyDeviceToDevice, m->stream));
-            if ((rc = rk::prefill_run(m->pf, m->p, m->stream, T[k][i], H[k][i], m->d_slogits))) return fail(rc, "%s", rk::prefill_error());
-        }
-        m->launches += rk::prefill_launches(m->pf);
+        if ((rc = gen_step_passes(m, b->passes.p + k * b->max_pass, step_rows[k], rk::kPfMaxTokens, H[k].data()))) return rc;
         if (R == 0) continue;
-        if (pen) {
-            const dim3 grid((unsigned)((V + rk::kPenaltyThreads - 1) / rk::kPenaltyThreads), (unsigned)R);
-            rk::k_gen_penalty<<<grid, rk::kPenaltyThreads, 0, m->stream>>>(m->d_slogits, (int)V, b->gs.p, b->row_stream.p, b->samp.p,
-                                                                          b->pen_cnt.p, b->pen_seen.p);
-            CK(cudaGetLastError());
-            m->launches += 1;
-        }
-        rk::k_sample_nucleus<<<(unsigned)R, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, b->samp.p, b->row_stream.p,
-                                                                              b->u.p + k * R, m->d_sample);
-        CK(cudaGetLastError());
+        if ((rc = pick_rows(m, pc, R, b->u.p + k * R))) return rc;
         rk::GenFeedbackArgs fb{b->gs.p, b->row_stream.p, R, nullptr, m->d_sample, b->stop.p, 0, b->out.p, kGenGroup,
                                k + 1 < steps ? b->passes.p + (k + 1) * b->max_pass : nullptr, nullptr, nullptr,
                                b->stop_start.p};
-        rk::k_gen_feedback<<<rb, 128, 0, m->stream>>>(fb);
-        CK(cudaGetLastError());
-        m->launches += 2;
+        rk::k_gen_feedback<<<(unsigned)((R + 127) / 128), 128, 0, m->stream>>>(fb);
+        LAUNCHED(m);
     }
     // the group's end: the lanes' records and the tokens of the group come back with one synchronisation
     if (R > 0) {
@@ -1772,10 +1523,8 @@ int rwkv_b200_sample_typical(rwkv_b200_model *m, float temp, double u, unsigned 
     CK(cudaMemcpyAsync(m->d_u, &u, sizeof(double), cudaMemcpyHostToDevice, m->stream));
     rk::k_sample_typical<<<1, rk::kSampleThreads, 0, m->stream>>>(dev_logits(m), 0, (int)binfmt::kVocab, sample_exponent(temp), m->d_u,
                                                                   m->d_sample);
-    CK(cudaGetLastError());
-    if ((rc = read_samples(m, 1, token, margin))) return rc;
-    m->launches += 1;
-    return 0;
+    LAUNCHED(m);
+    return read_samples(m, 1, token, margin);
 }
 
 int rwkv_b200_forward_streams(rwkv_b200_model *m, const unsigned long long *tokens, unsigned long long n_tokens,
@@ -1799,8 +1548,7 @@ int rwkv_b200_forward_streams(rwkv_b200_model *m, const unsigned long long *toke
     }
     if (next_out) {
         rk::k_argmax_rows<<<(unsigned)n_streams, rk::kArgmaxThreads, 0, m->stream>>>(m->d_slogits, (int)V, m->d_next);
-        CK(cudaGetLastError());
-        m->launches += 1;
+        LAUNCHED(m);
         CK(cudaMemcpyAsync(m->h_next, m->d_next, n_streams * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
     }
     if (logits_out) CK(cudaMemcpyAsync(m->h_logits, m->d_slogits, n_streams * V * sizeof(float), cudaMemcpyDeviceToHost, m->stream));
@@ -1823,10 +1571,8 @@ int rwkv_b200_sample_typical_streams(rwkv_b200_model *m, unsigned long long n_st
     CK(cudaMemcpyAsync(m->d_u, u, n_streams * sizeof(double), cudaMemcpyHostToDevice, m->stream));
     rk::k_sample_typical<<<(unsigned)n_streams, rk::kSampleThreads, 0, m->stream>>>(m->d_slogits, binfmt::kVocab, (int)binfmt::kVocab,
                                                                                    sample_exponent(temp), m->d_u, m->d_sample);
-    CK(cudaGetLastError());
-    if ((rc = read_samples(m, n_streams, tokens_out, margins_out))) return rc;
-    m->launches += 1;
-    return 0;
+    LAUNCHED(m);
+    return read_samples(m, n_streams, tokens_out, margins_out);
 }
 
 int rwkv_b200_generate_streams(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
@@ -1835,8 +1581,9 @@ int rwkv_b200_generate_streams(rwkv_b200_model *m, const unsigned long long *slo
                                const unsigned long long *override_tokens, const float *override_values,
                                unsigned long long n_override, float temp, const double *u, unsigned long long *tokens_out,
                                unsigned long long *lengths_out) {
-    return generate(m, "generate_streams", false, slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop,
-                    override_tokens, override_values, n_override, temp, nullptr, u, tokens_out, lengths_out);
+    const GenCall c{slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values,
+                    n_override, nullptr, u, tokens_out, lengths_out};
+    return generate(m, "generate_streams", false, c, temp);
 }
 
 int rwkv_b200_generate_streams_ex(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
@@ -1846,8 +1593,9 @@ int rwkv_b200_generate_streams_ex(rwkv_b200_model *m, const unsigned long long *
                                   unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
                                   unsigned long long *tokens_out, unsigned long long *lengths_out) {
     // without samplers every stream takes the arg-max and u is not read
-    return generate(m, "generate_streams_ex", true, slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop,
-                    override_tokens, override_values, n_override, 1.0f, samplers, samplers ? u : nullptr, tokens_out, lengths_out);
+    const GenCall c{slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values,
+                    n_override, samplers, samplers ? u : nullptr, tokens_out, lengths_out};
+    return generate(m, "generate_streams_ex", true, c, 1.0f);
 }
 
 int rwkv_b200_generate_streams_logprobs(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
@@ -1858,10 +1606,10 @@ int rwkv_b200_generate_streams_logprobs(rwkv_b200_model *m, const unsigned long 
                                         unsigned long long *tokens_out, unsigned long long *lengths_out, int logprob_mode,
                                         unsigned int top_n, double *logprobs_out, unsigned long long *ranks_out,
                                         unsigned long long *top_tokens_out, double *top_logprobs_out) {
+    const GenCall c{slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values,
+                    n_override, samplers, samplers ? u : nullptr, tokens_out, lengths_out};
     const LogprobRequest lpq{logprob_mode, top_n, logprobs_out, ranks_out, top_tokens_out, top_logprobs_out};
-    return generate(m, "generate_streams_logprobs", true, slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop,
-                    override_tokens, override_values, n_override, 1.0f, samplers, samplers ? u : nullptr, tokens_out, lengths_out,
-                    &lpq);
+    return generate(m, "generate_streams_logprobs", true, c, 1.0f, &lpq);
 }
 
 int rwkv_b200_constraint_add(rwkv_b200_model *m, unsigned long long n_states, const unsigned long long *edge_start,
@@ -1943,23 +1691,152 @@ int rwkv_b200_generate_streams_constrained(rwkv_b200_model *m, const unsigned lo
                                            unsigned long long *top_tokens_out, double *top_logprobs_out,
                                            const unsigned long long *constraint_ids, const unsigned long long *start_states,
                                            unsigned long long *states_out) {
+    const GenCall c{slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values,
+                    n_override, samplers, samplers ? u : nullptr, tokens_out, lengths_out};
     const LogprobRequest lpq{logprob_mode, top_n, logprobs_out, ranks_out, top_tokens_out, top_logprobs_out};
     const ConstraintRequest cq{constraint_ids, start_states, states_out};
-    return generate(m, "generate_streams_constrained", true, slots, first_tokens, n_streams, max_new, budgets, stop_tokens,
-                    n_stop, override_tokens, override_values, n_override, 1.0f, samplers, samplers ? u : nullptr, tokens_out,
-                    lengths_out, logprobs_out ? &lpq : nullptr, &cq);
+    return generate(m, "generate_streams_constrained", true, c, 1.0f, logprobs_out ? &lpq : nullptr, &cq);
 }
 
+// Beam search: generate()'s group loop over beams. Step 0 has one row per group, later steps B rows per live group
+// (group by group); each step is forward -> k_beam_expand -> k_beam_select -> k_beam_fork. At each host group's end the
+// done flags come back and the done groups leave the rows; at the end the backpointers and the hypothesis lists come
+// back once and the host rebuilds each hypothesis' tokens.
 int rwkv_b200_beam_search(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
                           unsigned long long n_groups, unsigned beams, unsigned long long max_new,
                           const unsigned long long *stop_tokens, unsigned long long n_stop, double length_penalty,
                           unsigned n_best, unsigned long long *tokens_out, unsigned long long *lengths_out,
                           double *logprobs_out, double *scores_out, unsigned char *finished_out,
                           double *token_logprobs_out) {
-    return beam(m, slots, first_tokens, n_groups, beams, max_new, stop_tokens, n_stop, length_penalty, n_best, tokens_out,
-                lengths_out, logprobs_out, scores_out, finished_out, token_logprobs_out);
+    const char *what = "beam_search";
+    int rc = check_streams_model(m, what);
+    if (rc) return rc;
+    if (!slots || !first_tokens || !tokens_out || !lengths_out || !logprobs_out || !scores_out || !finished_out)
+        return fail(1, "%s: null argument (slots, first_tokens, tokens_out, lengths_out, logprobs_out, scores_out and "
+                       "finished_out are required)", what);
+    if (n_stop && !stop_tokens) return fail(1, "%s: n_stop = %llu with NULL stop_tokens", what, n_stop);
+    if (n_groups == 0) return fail(1, "%s: no groups", what);
+    if (beams == 0) return fail(1, "%s: beams is 0", what);
+    if (n_stop > (unsigned long long)rk::kMaxTopN || beams + n_stop > (unsigned long long)rk::kMaxTopN)
+        return fail(1, "%s: beams + n_stop = %u + %llu > %d", what, beams, n_stop, rk::kMaxTopN);
+    if (n_best == 0 || n_best > beams) return fail(1, "%s: n_best %u is outside 1..beams = %u", what, n_best, beams);
+    if (max_new == 0) return fail(1, "%s: max_new is 0", what);
+    if (!std::isfinite(length_penalty)) return fail(1, "%s: length_penalty %g is not finite", what, length_penalty);
+    if (n_groups > m->max_gpt) return fail(1, "%s: %llu groups > max_gpt %llu", what, n_groups, m->max_gpt);
+    const size_t V = binfmt::kVocab;
+    const unsigned long long G = n_groups, B = beams, K = n_best, N = max_new, C = B + n_stop;
+    if ((rc = check_slots(m, what, slots, G * B)) || (rc = check_tokens(what, "first token", first_tokens, G, "group")) ||
+        (rc = check_tokens(what, "stop token", stop_tokens, n_stop)))
+        return rc;
+    // the length penalties on the host, with the C library's pow: a host restatement gets the same bits
+    if (N > ((unsigned long long)SIZE_MAX / sizeof(rk::BeamBack)) / (G * B))
+        return fail(1, "%s: max_new = %llu: the backpointers of %llu beams do not fit in memory", what, N, G * B);
+    std::vector<double> P;
+    try {
+        P.assign(N + 1, 0.0);
+    } catch (const std::exception &) {
+        return fail(9, "%s: out of host memory for max_new = %llu", what, N);
+    }
+    for (unsigned long long n = 1; n <= N; ++n) P[n] = pow((double)n, length_penalty);
+    CK(cudaSetDevice(m->device));
+    auto &g = m->gen;
+    auto &bm = m->beam;
+    if ((rc = g.stop.grow(n_stop)) || (rc = bm.row0.grow(G)) || (rc = bm.groups.grow(G)) || (rc = bm.cand_tok.grow(G * B * C)) ||
+        (rc = bm.cand_lp.grow(G * B * C)) || (rc = bm.cum.grow(G * B)) || (rc = bm.P.grow(N + 1)) || (rc = bm.back.grow(G * N * B)) ||
+        (rc = bm.hyp.grow(G * K)) || (rc = bm.n_hyp.grow(G)) || (rc = bm.done.grow(G)) || (rc = bm.forks.grow(2 * G * B)))
+        return rc;
+    // the path is chosen once, for G x B one-token streams
+    const bool tc = tensor_cores(m, G * B);
+    if (tc && (rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
+    m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
+
+    rk::GenStream *hg = g.h_gs;
+    for (unsigned long long s = 0; s < G * B; ++s) hg[s] = rk::GenStream{slots[s], N, s % B == 0 ? first_tokens[s / B] : 0, 0, 0};
+    std::vector<int> row0(G), live(G);
+    for (unsigned long long i = 0; i < G; ++i) {
+        row0[i] = (int)(i * B);
+        live[i] = (int)i;
+    }
+    CK(cudaMemcpyAsync(g.gs, hg, G * B * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemcpyAsync(bm.row0.p, row0.data(), G * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemcpyAsync(bm.P.p, P.data(), (N + 1) * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+    if (n_stop) CK(cudaMemcpyAsync(g.stop.p, stop_tokens, n_stop * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemsetAsync(bm.cum.p, 0, G * B * sizeof(double), m->stream));
+    CK(cudaMemsetAsync(bm.n_hyp.p, 0, G * sizeof(int), m->stream));
+    CK(cudaMemsetAsync(bm.done.p, 0, G * sizeof(unsigned long long), m->stream));
+    std::vector<unsigned long long> hdone(G, 0);
+    std::vector<int> rs;
+    for (unsigned long long step = 0; !live.empty() && step < N;) {
+        // a host group: the live groups' beams are rows gi * B + j (step 0: row gi); their inputs go up once
+        const int Gl = (int)live.size();
+        const unsigned long long steps = std::min(kGenGroup, N - step);
+        rs.resize((size_t)Gl * B);
+        for (int gi = 0; gi < Gl; ++gi)
+            for (unsigned long long j = 0; j < B; ++j) rs[gi * B + j] = (int)(live[gi] * B + j);
+        CK(cudaMemcpyAsync(g.row_stream, rs.data(), rs.size() * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(bm.groups.p, live.data(), Gl * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        if (tc && (rc = upload_step_passes(m, step == 0 ? row0.data() : rs.data(), step == 0 ? Gl : Gl * (int)B))) return rc;
+        rk::BeamArgs ba{g.gs, bm.cum.p, bm.groups.p, bm.cand_tok.p, bm.cand_lp.p, (int)C, (int)B, (int)K, 0, 0, N, bm.P.p,
+                        length_penalty < 0.0 ? 1 : 0, g.stop.p, (int)n_stop, bm.back.p, bm.hyp.p, bm.n_hyp.p, bm.done.p, bm.forks.p,
+                        tc ? g.passes : nullptr};
+        for (unsigned long long k = 0; k < steps; ++k) {
+            const unsigned long long st = step + k;
+            const int nb = st == 0 ? 1 : (int)B, rows = Gl * nb;
+            const int *rmap = st == 0 ? bm.row0.p : g.row_stream;
+            if ((rc = tc ? gen_step_passes(m, g.passes, rows, rk::kPfMaxTokens) : gen_step_decode(m, rows, rmap))) return rc;
+            rk::k_beam_expand<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs, rmap, (int)C,
+                                                                                bm.cand_tok.p, bm.cand_lp.p);
+            LAUNCHED(m);
+            ba.step = (int)st;
+            ba.nb = nb;
+            rk::k_beam_select<<<(unsigned)Gl, rk::kBeamSelectThreads, 0, m->stream>>>(ba);
+            LAUNCHED(m);
+            // after the last step every group is done and forks nothing
+            if (st + 1 < N && (rc = fork_slots(m, bm.forks.p, Gl * B, true))) return rc;
+        }
+        // the end of a host group: which groups are done and the beams' records (one synchronisation)
+        CK(cudaMemcpyAsync(hdone.data(), bm.done.p, G * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(hg, g.gs, G * B * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
+        SYNC(m);
+        step += steps;
+        live.erase(std::remove_if(live.begin(), live.end(), [&](int gg) { return hdone[gg] != 0; }), live.end());
+    }
+    std::vector<rk::BeamHyp> hyp(G * K);
+    std::vector<rk::BeamBack> back(G * N * B);
+    CK(cudaMemcpyAsync(hyp.data(), bm.hyp.p, G * K * sizeof(rk::BeamHyp), cudaMemcpyDeviceToHost, m->stream));
+    CK(cudaMemcpyAsync(back.data(), bm.back.p, G * N * B * sizeof(rk::BeamBack), cudaMemcpyDeviceToHost, m->stream));
+    SYNC(m);
+    // each hypothesis' tokens: its last token, then the backpointers of its beam from its step down to step 0
+    const double nan = std::nan("");
+    for (unsigned long long gg = 0; gg < G; ++gg)
+        for (unsigned long long i = 0; i < K; ++i) {
+            const rk::BeamHyp &h = hyp[gg * K + i];
+            const size_t o = (size_t)(gg * K + i);
+            unsigned long long *tok = tokens_out + o * N;
+            double *tlp = token_logprobs_out ? token_logprobs_out + o * N : nullptr;
+            for (unsigned long long t = 0; t < N; ++t) {
+                tok[t] = 0;
+                if (tlp) tlp[t] = nan;
+            }
+            tok[h.step] = h.tok;
+            if (tlp) tlp[h.step] = h.lp;
+            for (int s = h.step - 1, p = h.parent; s >= 0; --s) {
+                const rk::BeamBack &bk = back[(gg * N + (unsigned long long)s) * B + (unsigned long long)p];
+                tok[s] = bk.tok;
+                if (tlp) tlp[s] = bk.lp;
+                p = bk.parent;
+            }
+            lengths_out[o] = (unsigned long long)h.len;
+            logprobs_out[o] = h.cum;
+            scores_out[o] = h.score;
+            finished_out[o] = (unsigned char)h.finished;
+        }
+    return 0;
 }
 
+// Speculative generation: generate()'s group loop with k + 1 rows per live stream. Each step is k_spec_draft -> passes
+// -> pick_rows (overrides, pick) -> k_spec_accept; at each group's end the records come back and the finished streams
+// leave the rows. At the end a stream whose home is a spare has it copied to its first slot.
 int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
                                            unsigned long long n_streams, unsigned long long max_new, const unsigned long long *budgets,
                                            const unsigned long long *stop_tokens, unsigned long long n_stop,
@@ -1968,8 +1845,112 @@ int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned lo
                                            unsigned long long *tokens_out, unsigned long long *lengths_out, unsigned int draft,
                                            unsigned int ngram, const unsigned long long *context_start,
                                            const unsigned long long *context, unsigned long long *steps_out) {
-    return speculate(m, slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values,
-                     n_override, samplers, u, tokens_out, lengths_out, draft, ngram, context_start, context, steps_out);
+    const char *what = "generate_streams_speculative";
+    int rc = check_streams_model(m, what);
+    if (rc) return rc;
+    if (draft < 1 || draft > (unsigned)rk::kSpecMaxDraft) return fail(1, "%s: draft %u is outside 1..%d", what, draft, rk::kSpecMaxDraft);
+    if (ngram < 1 || ngram > (unsigned)rk::kSpecMaxNgram) return fail(1, "%s: ngram %u is outside 1..%d", what, ngram, rk::kSpecMaxNgram);
+    if (!rk::prefill_enabled(m->pf)) return fail(1, "%s: needs the tensor cores (the \"prefill\" option is 0)", what);
+    const unsigned long long K1 = draft + 1ull, S = n_streams;
+    if (S > m->max_gpt / K1)
+        return fail(1, "%s: %llu streams x %llu rows > max_gpt %llu", what, S, K1, m->max_gpt);
+    if (!samplers) u = nullptr; // every stream takes the arg-max
+    const GenCall c{slots, first_tokens, S, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values, n_override,
+                    samplers, u, tokens_out, lengths_out};
+    if ((rc = check_gen(m, what, c, K1, true, steps_out, "steps_out"))) return rc;
+    for (unsigned long long s = 0; samplers && s < S; ++s)
+        if (samplers[s].presence_penalty != 0.0f || samplers[s].frequency_penalty != 0.0f)
+            return fail(1, "%s: stream %llu: presence and frequency penalties are not supported (a row's counts would have "
+                           "to include its own drafts)", what, s);
+    unsigned long long n_ctx = 0;
+    if (context_start) {
+        if (context_start[0] != 0) return fail(1, "%s: context_start[0] = %llu, not 0", what, context_start[0]);
+        for (unsigned long long s = 0; s < S; ++s)
+            if (context_start[s + 1] < context_start[s])
+                return fail(1, "%s: context_start decreases from stream %llu to %llu (%llu > %llu)", what, s, s + 1,
+                            context_start[s], context_start[s + 1]);
+        n_ctx = context_start[S];
+        if (n_ctx && !context) return fail(1, "%s: %llu context tokens with NULL context", what, n_ctx);
+        if ((rc = check_tokens(what, "context token", context, n_ctx))) return rc;
+    }
+    const unsigned long long n_hist = n_ctx + S * (1 + max_new);
+    CK(cudaSetDevice(m->device));
+    auto &g = m->gen;
+    auto &sp = m->spec;
+    const int per_pass = rk::kPfMaxTokens / (int)K1; // streams per pass: a stream's rows never straddle two passes
+    const size_t n_pass = (size_t)((S + per_pass - 1) / per_pass);
+    if ((rc = sp.ss.grow(S)) || (rc = sp.hist.grow(n_hist)) || (rc = sp.live.grow(S)) || (rc = sp.passes.grow(n_pass)) ||
+        (u && ((rc = sp.u.grow(max_new * S)) || (rc = sp.row_u.grow(S * K1)))) || (rc = sp.forks.grow(2 * S)))
+        return rc;
+    if ((rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
+    m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
+
+    // the records and the histories: stream s's history starts with its context and its first token
+    std::vector<rk::SpecStream> hs(S);
+    std::vector<unsigned long long> hist(n_hist, 0); // stream s: its context, its first token, then room for max_new
+    for (unsigned long long s = 0, h0 = 0; s < S; ++s) {
+        rk::SpecStream &r = hs[s];
+        r = rk::SpecStream{};
+        for (unsigned long long i = 0; i < K1; ++i) r.slot[i] = slots[s * K1 + i];
+        const unsigned long long c0 = context_start ? context_start[s] : 0, c1 = context_start ? context_start[s + 1] : 0;
+        r.h0 = h0;
+        r.hl = c1 - c0 + 1;
+        r.budget = budgets ? budgets[s] : max_new;
+        std::copy(context + c0, context + c1, hist.begin() + h0);
+        hist[h0 + c1 - c0] = first_tokens[s];
+        h0 += r.hl + max_new;
+    }
+    CK(cudaMemcpyAsync(sp.hist.p, hist.data(), n_hist * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemcpyAsync(sp.ss.p, hs.data(), S * sizeof(rk::SpecStream), cudaMemcpyHostToDevice, m->stream));
+    if ((rc = upload_gen(m, c))) return rc;
+    if (u) CK(cudaMemcpyAsync(sp.u.p, u, max_new * S * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+
+    std::vector<int> live(S), rs;
+    for (unsigned long long s = 0; s < S; ++s) live[s] = (int)s;
+    rk::SpecArgs sa{sp.ss.p, sp.live.p, (int)draft, (int)ngram, per_pass, sp.hist.p, sp.passes.p, u ? sp.u.p : nullptr,
+                    sp.row_u.p, S, max_new, samplers ? nullptr : m->d_next, m->d_sample, g.stop.p, (int)n_stop, g.out.p};
+    const PickChain pc{nullptr, g.row_stream, samplers ? g.samp.p : nullptr, nullptr, nullptr, g.ovr_tok.p, g.ovr_val.p, n_override};
+    // each step emits at least one token per live stream, so max_new steps finish every stream
+    for (unsigned long long step = 0; !live.empty() && step < max_new;) {
+        const int n_live = (int)live.size(), rows = n_live * (int)K1;
+        const unsigned long long steps = std::min(kGenGroup, max_new - step);
+        rs.resize(rows);
+        for (int r = 0; r < rows; ++r) rs[r] = live[r / (int)K1];
+        CK(cudaMemcpyAsync(sp.live.p, live.data(), n_live * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(g.row_stream, rs.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        for (unsigned long long k = 0; k < steps; ++k) {
+            rk::k_spec_draft<<<(unsigned)n_live, rk::kSpecDraftThreads, 0, m->stream>>>(sa);
+            LAUNCHED(m);
+            if ((rc = gen_step_passes(m, sp.passes.p, rows, per_pass * (int)K1)) ||
+                (rc = pick_rows(m, pc, rows, u ? sp.row_u.p : nullptr)))
+                return rc;
+            rk::k_spec_accept<<<(unsigned)n_live, 32, 0, m->stream>>>(sa);
+            LAUNCHED(m);
+        }
+        // the end of a group: which streams are done (one synchronisation); drop them from the rows
+        CK(cudaMemcpyAsync(hs.data(), sp.ss.p, S * sizeof(rk::SpecStream), cudaMemcpyDeviceToHost, m->stream));
+        SYNC(m);
+        step += steps;
+        live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hs[s].done != 0; }), live.end());
+    }
+    // a home on a spare: its xy, aa, bb and dd go to the first slot (pp: no forward writes it)
+    std::vector<unsigned long long> forks;
+    for (unsigned long long s = 0; s < S; ++s)
+        if (hs[s].home != 0) {
+            forks.push_back(hs[s].slot[hs[s].home]);
+            forks.push_back(hs[s].slot[0]);
+        }
+    if (!forks.empty()) {
+        CK(cudaMemcpyAsync(sp.forks.p, forks.data(), forks.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        if ((rc = fork_slots(m, sp.forks.p, forks.size() / 2, false))) return rc;
+    }
+    CK(cudaMemcpyAsync(tokens_out, g.out.p, S * max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+    SYNC(m);
+    for (unsigned long long s = 0; s < S; ++s) {
+        lengths_out[s] = hs[s].len;
+        steps_out[s] = hs[s].steps;
+    }
+    return 0;
 }
 
 int rwkv_b200_sample_streams(rwkv_b200_model *m, unsigned long long n_streams, const rwkv_b200_sampler *params, const double *u,
@@ -1988,12 +1969,9 @@ int rwkv_b200_sample_streams(rwkv_b200_model *m, unsigned long long n_streams, c
         if (n_streams != m->stream_rows)
             return fail(1, "%s: %llu rows asked, the last forward_streams produced %llu", what, n_streams, m->stream_rows);
     }
-    for (unsigned long long s = 0; s < n_streams; ++s) {
-        if ((rc = check_sampler(what, s, params[s], false))) return rc;
-        if (params[s].temperature > 0.0f && !u)
-            return fail(1, "%s: u is NULL but stream %llu samples (temperature %g)", what, s, params[s].temperature);
-        if (u && !(u[s] >= 0.0 && u[s] < 1.0)) return fail(1, "%s: u[%llu] = %g is outside [0, 1)", what, s, u[s]);
-    }
+    for (unsigned long long s = 0; s < n_streams; ++s)
+        if ((rc = check_sampler(what, s, params[s], false, u != nullptr))) return rc;
+    if ((rc = check_uniforms(what, u, n_streams))) return rc;
     for (unsigned long long s = 0; logits && s < n_streams; ++s) {
         const float *row = logits + s * V;
         bool finite = false;
@@ -2015,10 +1993,8 @@ int rwkv_b200_sample_streams(rwkv_b200_model *m, unsigned long long n_streams, c
     }
     rk::k_sample_nucleus<<<(unsigned)n_streams, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.samp.p, nullptr,
                                                                                 u ? m->d_u : nullptr, m->d_sample);
-    CK(cudaGetLastError());
-    if ((rc = read_samples(m, n_streams, tokens_out, margins_out))) return rc;
-    m->launches += 1;
-    return 0;
+    LAUNCHED(m);
+    return read_samples(m, n_streams, tokens_out, margins_out);
 }
 
 int rwkv_b200_score_streams(rwkv_b200_model *m, const unsigned long long *tokens, unsigned long long n_tokens,
@@ -2072,8 +2048,7 @@ int rwkv_b200_score_streams(rwkv_b200_model *m, const unsigned long long *tokens
         CK(cudaMemcpyAsync(sc.tgt.p, tgt.data(), n * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
         const rk::ScoreArgs a{m->d_slogits, (int)V, sc.rows.p, sc.tgt.p, (int)top_n, sc.lp.p, sc.rank.p, sc.top_tok.p, sc.top_lp.p};
         rk::k_logprob_rows<<<(unsigned)n, rk::kNucThreads, 0, m->stream>>>(a);
-        CK(cudaGetLastError());
-        m->launches += 1;
+        LAUNCHED(m);
         CK(cudaMemcpyAsync(lp.data(), sc.lp.p, n * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
         if (ranks_out) CK(cudaMemcpyAsync(rank.data(), sc.rank.p, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
         if (top_n) {
@@ -2197,12 +2172,9 @@ int rwkv_b200_batcher_submit(rwkv_b200_batcher *b, const rwkv_b200_request *r, u
     if (r->n_stop && !r->stop) return fail(1, "%s: n_stop = %llu with NULL stop", what, r->n_stop);
     const unsigned long long s = b->next_id; // the id it would get names it in messages
     if ((rc = check_slot(b->m, what, r->slot)) || (rc = check_tokens(what, "prompt token", r->prompt, r->n_prompt)) ||
-        (rc = check_tokens(what, "stop token", r->stop, r->n_stop)) || (rc = check_sampler(what, s, r->sampler, true)))
+        (rc = check_tokens(what, "stop token", r->stop, r->n_stop)) ||
+        (rc = check_sampler(what, s, r->sampler, true, r->u != nullptr)) || (rc = check_uniforms(what, r->u, r->max_new)))
         return rc;
-    if (r->sampler.temperature > 0.0f && !r->u)
-        return fail(1, "%s: u is NULL but stream %llu samples (temperature %g)", what, s, r->sampler.temperature);
-    for (unsigned long long i = 0; r->u && i < r->max_new; ++i)
-        if (!(r->u[i] >= 0.0 && r->u[i] < 1.0)) return fail(1, "%s: u[%llu] = %g is outside [0, 1)", what, i, r->u[i]);
     for (const auto &e : b->reqs)
         if (e.second.slot == r->slot && e.second.status <= RWKV_B200_REQ_GENERATING)
             return fail(1, "%s: slot %llu is held by unfinished request %llu", what, r->slot, e.first);

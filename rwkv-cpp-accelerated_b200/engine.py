@@ -59,11 +59,15 @@ def _samplers(spec, n):
     return (Sampler * n)(*items)
 
 
-def _gen_args(streams, max_new, budgets, stop, overrides, u):
-    """The arrays of a generate_streams call: S, slots, first tokens, budgets, stops, override tokens and values,
-    uniforms, and the emitted tokens and lengths to fill."""
+def _gen_args(streams, max_new, budgets, stop, overrides, u, slots=None):
+    """The arguments the generate_streams calls share: S; the ten after the model handle (slots, first tokens, S,
+    max_new, budgets, stops, n_stop, override tokens, values, n_override); the three after the sampler or temperature
+    (uniforms, emitted tokens, lengths); and the emitted tokens and lengths arrays they fill. slots: every stream's slots
+    flattened, when a stream names several (generate_speculative); None: each stream's one slot."""
     S = len(streams)
-    slots = np.ascontiguousarray([int(s) for s, _ in streams], dtype=np.uint64)
+    if slots is None:
+        slots = [int(s) for s, _ in streams]
+    slots = np.ascontiguousarray(slots, dtype=np.uint64)
     first = np.ascontiguousarray([int(t) for _, t in streams], dtype=np.uint64)
     bud = np.ascontiguousarray(budgets, dtype=np.uint64) if budgets is not None else None
     stops = np.ascontiguousarray(list(stop), dtype=np.uint64)
@@ -75,7 +79,11 @@ def _gen_args(streams, max_new, budgets, stop, overrides, u):
         raise EngineError("generate_streams: %d budgets for %d streams" % (bud.size, S))
     if us is not None and us.shape != (max_new, S):
         raise EngineError("generate_streams: u has shape %s, expected (%d, %d)" % (us.shape, max_new, S))
-    return S, slots, first, bud, stops, otok, oval, us, np.zeros((S, max_new), np.uint64), np.zeros(S, np.uint64)
+    out, lens = np.zeros((S, max_new), np.uint64), np.zeros(S, np.uint64)
+    P = ctypes.c_ulonglong
+    lead = (_ptr(slots, P), _ptr(first, P), S, max_new, _ptr(bud, P), _ptr(stops, P), len(stops), _ptr(otok, P),
+            _ptr(oval, ctypes.c_float), len(otok))
+    return S, lead, (_ptr(us, ctypes.c_double), _ptr(out, P), _ptr(lens, P)), out, lens
 
 
 def lookup_drafts(history, draft, ngram):
@@ -353,19 +361,12 @@ class Engine:
             return self._generate_scored(streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n,
                                          constraints)
         temp = 1.0 if temp is None else temp
-        S, slots, first, bud, stops, otok, oval, us, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u)
-        P = ctypes.c_ulonglong
+        S, lead, tail, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u)
         if sampling is not None:
-            self._ck(self.lib.rwkv_b200_generate_streams_ex(self.h, _ptr(slots, P), _ptr(first, P), S, max_new, _ptr(bud, P),
-                                                            _ptr(stops, P), len(stops), _ptr(otok, P),
-                                                            _ptr(oval, ctypes.c_float), len(otok), _samplers(sampling, S),
-                                                            _ptr(us, ctypes.c_double), _ptr(out, P), _ptr(lens, P)),
+            self._ck(self.lib.rwkv_b200_generate_streams_ex(self.h, *lead, _samplers(sampling, S), *tail),
                      "generate_streams_ex")
-            return [out[s, :int(lens[s])].copy() for s in range(S)]
-        self._ck(self.lib.rwkv_b200_generate_streams(self.h, _ptr(slots, P), _ptr(first, P), S, max_new, _ptr(bud, P),
-                                                     _ptr(stops, P), len(stops), _ptr(otok, P), _ptr(oval, ctypes.c_float),
-                                                     len(otok), temp, _ptr(us, ctypes.c_double), _ptr(out, P),
-                                                     _ptr(lens, P)), "generate_streams")
+        else:
+            self._ck(self.lib.rwkv_b200_generate_streams(self.h, *lead, temp, *tail), "generate_streams")
         return [out[s, :int(lens[s])].copy() for s in range(S)]
 
     def _generate_scored(self, streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n, constraints):
@@ -380,7 +381,7 @@ class Engine:
                                   "arg-max); the typical sampler does not take them")
             raise EngineError("generate_streams: logprobs need sampling=... (or neither u nor temp, for the arg-max); "
                               "the typical sampler reports no log-probabilities")
-        S, slots, first, bud, stops, otok, oval, us, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u)
+        S, lead, tail, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u)
         lp = ranks = top_tok = top_lp = None
         if logprobs is not None:
             lp = np.empty((S, max_new), np.float64)
@@ -390,10 +391,8 @@ class Engine:
                 top_lp = np.empty((S, max_new, top_n), np.float64)
         P = ctypes.c_ulonglong
         sp = _samplers(sampling, S) if sampling is not None else None
-        args = (self.h, _ptr(slots, P), _ptr(first, P), S, max_new, _ptr(bud, P), _ptr(stops, P), len(stops), _ptr(otok, P),
-                _ptr(oval, ctypes.c_float), len(otok), sp, _ptr(us, ctypes.c_double), _ptr(out, P), _ptr(lens, P),
-                modes[logprobs], int(top_n), _ptr(lp, ctypes.c_double), _ptr(ranks, P), _ptr(top_tok, P),
-                _ptr(top_lp, ctypes.c_double))
+        args = (self.h, *lead, sp, *tail, modes[logprobs], int(top_n), _ptr(lp, ctypes.c_double), _ptr(ranks, P),
+                _ptr(top_tok, P), _ptr(top_lp, ctypes.c_double))
         if constraints is None:
             self._ck(self.lib.rwkv_b200_generate_streams_logprobs(*args), "generate_streams_logprobs")
         else:
@@ -521,9 +520,8 @@ class Engine:
         dict per stream: "tokens" (uint64) and "steps" (the steps that emitted a token)."""
         if any(len(slots) != draft + 1 for slots, _ in streams):
             raise EngineError("generate_speculative: every stream needs draft + 1 = %d slots" % (draft + 1))
-        S, _, first, bud, stops, otok, oval, us, out, lens = _gen_args([(sl[0], t) for sl, t in streams], max_new, budgets,
-                                                                       stop, overrides, u)
-        slots = np.ascontiguousarray([int(s) for sl, _ in streams for s in sl], dtype=np.uint64)
+        S, lead, tail, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u,
+                                             slots=[int(s) for sl, _ in streams for s in sl])
         steps = np.zeros(S, np.uint64)
         cstart = ctx = None
         if context is not None:
@@ -534,10 +532,9 @@ class Engine:
             ctx = np.ascontiguousarray([x for c in seqs for x in c], dtype=np.uint64)
         sp = _samplers(sampling, S) if sampling is not None else None
         P = ctypes.c_ulonglong
-        self._ck(self.lib.rwkv_b200_generate_streams_speculative(
-            self.h, _ptr(slots, P), _ptr(first, P), S, max_new, _ptr(bud, P), _ptr(stops, P), len(stops), _ptr(otok, P),
-            _ptr(oval, ctypes.c_float), len(otok), sp, _ptr(us, ctypes.c_double), _ptr(out, P), _ptr(lens, P), int(draft),
-            int(ngram), _ptr(cstart, P), _ptr(ctx, P), _ptr(steps, P)), "generate_streams_speculative")
+        self._ck(self.lib.rwkv_b200_generate_streams_speculative(self.h, *lead, sp, *tail, int(draft), int(ngram),
+                                                                 _ptr(cstart, P), _ptr(ctx, P), _ptr(steps, P)),
+                 "generate_streams_speculative")
         return [{"tokens": out[s, :int(lens[s])].copy(), "steps": int(steps[s])} for s in range(S)]
 
     def batcher(self, rows, prefill_tokens):
