@@ -361,7 +361,8 @@ int rwkv_b200_generate_streams_logprobs(rwkv_b200_model *m, const unsigned long 
 int rwkv_b200_constraint_add(rwkv_b200_model *m, unsigned long long n_states, const unsigned long long *edge_start,
                              const unsigned long long *edge_tokens, const unsigned long long *edge_next,
                              unsigned long long *id);
-/* Free an automaton (an unknown or removed id is refused). rwkv_b200_free frees every automaton of the model. */
+/* Free an automaton (an unknown or removed id is refused, and so is an id that an unfinished request of the model's
+ * batcher names). rwkv_b200_free frees every automaton of the model. */
 int rwkv_b200_constraint_remove(rwkv_b200_model *m, unsigned long long id);
 
 /* rwkv_b200_generate_streams_logprobs with a token automaton per stream, by the rule above. constraint_ids[n_streams]:
@@ -485,7 +486,17 @@ int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned lo
  * This holds whatever the other requests are, when each was submitted, rows, prefill_tokens, the max_steps of each run,
  * and any cancellation of other requests. A request's penalty history starts empty at its first emitted token, as in
  * step 2. A cancelled request's tokens are a prefix of that sequence's tokens. Slots that no unfinished request names
- * are never written. The rule rests on the ragged-pass invariant: a stream's bits depend only on its own rows and its
+ * are never written.
+ * A request submitted with rwkv_b200_batcher_submit_ex may also carry logit overrides, a token automaton and
+ * log-probabilities. Then step 2 is rwkv_b200_generate_streams_constrained of the one stream with, besides the above,
+ * the request's overrides as the call's overrides, its constraint id and start state (or constraint_ids == NULL), and
+ * its logprob_mode and top_n (or logprobs_out == NULL); without any of the three that call is generate_streams_ex, as
+ * above. Its emitted tokens, the slot's final state, the log-probabilities, ranks and top entries and the final
+ * automaton state are bit for bit that call's. Each step's order is the one-shot calls': forward, the copy of the
+ * model's rows that raw mode reads (when some edit would change them), penalties, this request's overrides, its
+ * automaton's mask, the pick, the scoring, the feedback. A request whose automaton reaches a state without edges ends
+ * as RWKV_B200_REQ_DONE, like after a stop token (emitted, not fed). A cancelled request's log-probabilities are a
+ * prefix of that call's, and its automaton state is the state after its emitted tokens. The rule rests on the ragged-pass invariant: a stream's bits depend only on its own rows and its
  * own predecessors, and cutting it across passes changes no bit.
  *
  * Scheduling (deterministic). A run is a series of groups of 16 steps (the last one of a run may be shorter), with one
@@ -500,7 +511,7 @@ int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned lo
  *     prefill completes inside a group waits up to 15 steps for its first token. A group without decode rows ends after
  *     its last step with prompt work;
  *   - a step is one set of tensor-core passes: the decode rows first (one token each, with logits), then the prefill
- *     segments (no logits), cut into passes of at most 128 tokens; then penalties, the per-request sampler and the
+ *     segments (no logits), cut into passes of at most 128 tokens; then penalties, overrides, masks, the per-request sampler, scoring and the
  *     feedback that emits each row's token and writes it into the next step's passes.
  * At each group end the tokens emitted in the group come back, so rwkv_b200_batcher_read between runs sees a growing
  * prefix (streaming).
@@ -508,9 +519,8 @@ int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned lo
  * The batcher always runs on the tensor cores: the rule is defined on that path. With only a few generating requests
  * the decode kernel of rwkv_b200_generate_streams is faster (at 7B: one stream 3.1 ms per step there, a tensor-core step
  * of 8 streams 10.3 ms, on an H100 SXM 80 GB at a 400 W power limit; tensor-core steps under 8 rows have not been
- * measured). Not available
- * in the batcher: logit overrides, token automata, log-probabilities, the typical sampler, admission inside a group,
- * the decode-kernel path, tensor parallelism, priorities and preemption.
+ * measured). Not available in the batcher: the typical sampler, admission inside a group, the decode-kernel path,
+ * tensor parallelism, priorities and preemption.
  *
  * Other entry points may be called between runs, but must not name a slot held by an unfinished request (queued,
  * prefilling or generating); the batcher does not police that. rwkv_b200_free closes a model's open batcher, whose handle
@@ -526,6 +536,18 @@ typedef struct rwkv_b200_request {
     const unsigned long long *stop;   /* [n_stop] this request's stop tokens (emitted, not fed) */
     unsigned long long n_stop;
 } rwkv_b200_request;
+
+/* What rwkv_b200_batcher_submit_ex adds to a request (the rule above). */
+typedef struct rwkv_b200_request_ex {
+    const unsigned long long *override_tokens; /* [n_override] logit overrides, in order (a repeated token keeps its last) */
+    const float *override_values;              /* [n_override] finite or -inf, not every token -inf */
+    unsigned long long n_override;
+    unsigned long long constraint_id;          /* an id of rwkv_b200_constraint_add, or RWKV_B200_NO_CONSTRAINT */
+    unsigned long long start_state;            /* the automaton's first state (read with a constraint only) */
+    int logprobs;                              /* 0: none; else every emitted token is scored */
+    int logprob_mode;                          /* RWKV_B200_LOGPROBS_RAW or _PROCESSED (read when logprobs != 0) */
+    unsigned int top_n;                        /* 0..RWKV_B200_MAX_TOP_N top entries per token (idem) */
+} rwkv_b200_request_ex;
 
 #define RWKV_B200_BATCHER_MAX_PREFILL 2048ULL /* prefill_tokens is 1..this */
 
@@ -547,6 +569,15 @@ int rwkv_b200_batcher_open(rwkv_b200_model *m, unsigned long long rows, unsigned
  * of 0, a missing array, a token out of range, an invalid sampler (generate_streams_ex's checks), u NULL with a
  * temperature > 0, and a uniform outside [0, 1). */
 int rwkv_b200_batcher_submit(rwkv_b200_batcher *b, const rwkv_b200_request *r, unsigned long long *id);
+/* rwkv_b200_batcher_submit with the extension x (NULL: exactly rwkv_b200_batcher_submit). Refused as well, with nothing
+ * queued and no id used: an override token out of range, an override value that is NaN or +inf, overrides that set
+ * every token to -inf, n_override > 0 with a NULL array, an unknown or removed constraint id, a start state out of range
+ * or without edges, overrides that set every edge token of some state of the automaton to -inf, and with logprobs a
+ * logprob_mode other than the two or top_n > RWKV_B200_MAX_TOP_N. While the request is unfinished its automaton cannot
+ * be removed (rwkv_b200_constraint_remove refuses). A group whose decode rows use none of these features enqueues
+ * exactly what it would without them. */
+int rwkv_b200_batcher_submit_ex(rwkv_b200_batcher *b, const rwkv_b200_request *r, const rwkv_b200_request_ex *x,
+                                unsigned long long *id);
 /* Run up to max_steps steps in groups of 16; stops early when nothing is queued or admitted. *steps_run (may be NULL)
  * receives the steps run. */
 int rwkv_b200_batcher_run(rwkv_b200_batcher *b, unsigned long long max_steps, unsigned long long *steps_run);
@@ -555,6 +586,14 @@ int rwkv_b200_batcher_run(rwkv_b200_batcher *b, unsigned long long max_steps, un
  * or released id is refused. */
 int rwkv_b200_batcher_read(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *tokens_out,
                            unsigned long long cap, unsigned long long *len, int *status);
+/* rwkv_b200_batcher_read with the results of submit_ex: the first min(cap, *len) emitted tokens, their logprobs and
+ * ranks, and top_tokens_out / top_logprobs_out [cap][top_n] (the request's top_n), as generate_streams_logprobs reports
+ * them; *state_out the automaton's current state (0 without a constraint). Every array and pointer may be NULL (then it
+ * is skipped); the log-probability arrays are refused for a request that is not scored. */
+int rwkv_b200_batcher_read_ex(rwkv_b200_batcher *b, unsigned long long id, unsigned long long cap,
+                              unsigned long long *tokens_out, double *logprobs_out, unsigned long long *ranks_out,
+                              unsigned long long *top_tokens_out, double *top_logprobs_out,
+                              unsigned long long *state_out, unsigned long long *len, int *status);
 /* Cancel a queued, prefilling or generating request at once (calls are made between runs). A queued request's slot is
  * untouched; otherwise the slot holds the state after the tokens fed so far (its emitted tokens but the last one, as
  * after a stop token). Its tokens stay readable. A done or cancelled request, or an unknown id, is refused. */

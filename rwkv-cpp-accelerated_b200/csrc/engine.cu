@@ -185,8 +185,9 @@ struct rwkv_b200_model {
 };
 
 // rwkv_b200_batcher: the requests on the host, and per lane (0..rows-1, one per admitted request, reused) its stream
-// record, sampler, penalty rows, stop tokens and a ring of the current group's tokens on the device. Nothing is shared
-// with m->gen, so a generate_streams call between runs leaves the batcher's requests alone.
+// record, sampler, penalty rows, stop tokens, overrides, automaton, log-probability choice and a ring of the current
+// group's tokens (and their log-probabilities) on the device. Nothing is shared with m->gen, so a generate_streams call
+// between runs leaves the batcher's requests alone.
 struct rwkv_b200_batcher {
     rwkv_b200_model *m = nullptr;
     int rows = 0, prefill_tokens = 0, max_pass = 0; // max_pass: passes of a step at most
@@ -198,6 +199,15 @@ struct rwkv_b200_batcher {
         int status = RWKV_B200_REQ_QUEUED;
         unsigned long long fed = 0; // tokens of prompt[0 .. n_prompt - 1) in the slot
         int lane = -1;
+        // rwkv_b200_batcher_submit_ex: the overrides, the automaton (gc.mask == nullptr: none; gc.state is the current
+        // state) and its id, and the scoring (lp.mode < 0: none) with the results of the emitted tokens so far
+        std::vector<unsigned long long> ovr_tok;
+        std::vector<float> ovr_val;
+        rk::GenConstraint gc{};
+        unsigned long long constraint_id = RWKV_B200_NO_CONSTRAINT;
+        rk::LogprobLane lp{-1, 0};
+        std::vector<double> logprobs, top_logprobs;             // [tokens], [tokens][lp.top_n]
+        std::vector<unsigned long long> ranks, top_tokens;      // [tokens], [tokens][lp.top_n]
     };
     std::map<unsigned long long, Req> reqs;
     unsigned long long next_id = 1;
@@ -214,6 +224,20 @@ struct rwkv_b200_batcher {
     DevBuf<unsigned char> pen_seen;           // [rows][V]
     DevBuf<unsigned long long> stop, stop_start, out; // lanes' stop tokens (CSR), [rows + 1], [rows][kGenGroup]
     DevBuf<double> u;                         // [kGenGroup][rows] uniforms of the current group
+    // the features of submit_ex, each grown at the first group whose decode lanes use it
+    DevBuf<unsigned long long> ovr_tok, ovr_start; // decode lanes' overrides (CSR), [rows + 1]
+    DevBuf<float> ovr_val;
+    unsigned long long n_ovr = 0;             // the overrides of the current group's decode lanes
+    std::vector<rk::GenConstraint> h_gc;      // [rows] host mirror of the lanes' automata (mask nullptr: none)
+    DevBuf<rk::GenConstraint> gc;             // [rows]
+    DevBuf<unsigned long long> fault;         // [3] k_gen_feedback's record of a token without an edge
+    std::vector<rk::LogprobLane> h_lp;        // [rows] each lane's scoring (mode < 0: none)
+    DevBuf<rk::LogprobLane> lp_lane;          // [rows]
+    DevBuf<double> lp, top_lp;                // rings [rows][kGenGroup], [rows][kGenGroup][kMaxTopN]
+    DevBuf<unsigned long long> rank, top_tok; // [rows][kGenGroup], [rows][kGenGroup][kMaxTopN]
+    std::vector<double> h_lpv, h_top_lp;      // host copies of the rings
+    std::vector<unsigned long long> h_rank, h_top_tok;
+    DevBuf<float> raw;                        // [rows][V] the model's rows of a step, for raw lanes (see batcher_group)
 };
 
 namespace {
@@ -850,6 +874,15 @@ int check_overrides(const char *what, const unsigned long long *tok, const float
     return 0;
 }
 
+// A logprob_mode and top_n of generate_streams_logprobs or batcher_submit_ex.
+int check_logprob_mode(const char *what, int mode, unsigned top_n) {
+    if (mode != RWKV_B200_LOGPROBS_RAW && mode != RWKV_B200_LOGPROBS_PROCESSED)
+        return fail(1, "%s: logprob_mode %d is neither RWKV_B200_LOGPROBS_RAW (0) nor RWKV_B200_LOGPROBS_PROCESSED (1)", what,
+                    mode);
+    if (top_n > (unsigned)rk::kMaxTopN) return fail(1, "%s: top_n %u > %d", what, top_n, rk::kMaxTopN);
+    return 0;
+}
+
 // What generate_streams_logprobs asks for: the mode, top_n and the caller's result arrays.
 struct LogprobRequest {
     int mode;
@@ -979,6 +1012,9 @@ struct PickChain {
     unsigned long long n_override;
     const rk::GenConstraint *gc;
     int exponent; // the typical sampler's
+    // the batcher: each row's own overrides, ovr_*[ovr_start[s] .. ovr_start[s + 1]) of its stream s (n_override > 0
+    // only says that some row has one); nullptr: all n_override for every row
+    const unsigned long long *ovr_start;
 };
 
 // The chain on rows 0..rows-1 of d_slogits; u: the step's uniforms, one per row (NULL: none).
@@ -992,7 +1028,7 @@ int pick_rows(M *m, const PickChain &pc, int rows, const double *u) {
     }
     if (pc.n_override) {
         rk::k_gen_override<<<(unsigned)((rows + 127) / 128), 128, 0, m->stream>>>(m->d_slogits, (int)V, rows, pc.ovr_tok, pc.ovr_val,
-                                                                                (int)pc.n_override);
+                                                                                (int)pc.n_override, pc.row_stream, pc.ovr_start);
         LAUNCHED(m);
     }
     if (pc.gc) {
@@ -1021,10 +1057,7 @@ int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, cons
     int rc = check_streams_model(m, what);
     if (rc) return rc;
     if (lpq) {
-        if (lpq->mode != RWKV_B200_LOGPROBS_RAW && lpq->mode != RWKV_B200_LOGPROBS_PROCESSED)
-            return fail(1, "%s: logprob_mode %d is neither RWKV_B200_LOGPROBS_RAW (0) nor RWKV_B200_LOGPROBS_PROCESSED (1)", what,
-                        lpq->mode);
-        if (lpq->top_n > (unsigned)rk::kMaxTopN) return fail(1, "%s: top_n %u > %d", what, lpq->top_n, rk::kMaxTopN);
+        if ((rc = check_logprob_mode(what, lpq->mode, lpq->top_n))) return rc;
         if (!lpq->logprobs_out) return fail(1, "%s: logprobs_out is NULL", what);
         if (lpq->top_n && (!lpq->top_tokens_out || !lpq->top_logprobs_out))
             return fail(1, "%s: top_n = %u needs top_tokens_out and top_logprobs_out", what, lpq->top_n);
@@ -1148,9 +1181,9 @@ int check_batcher(const B *b) {
 }
 
 // A group boundary (the previous group's finished requests have left): queued requests are admitted in submission
-// order while fewer than `rows` are admitted (each takes the lowest free lane: its record, sampler and penalty rows are
-// reset), and every admitted request whose prefill is complete gets its decode row's record. Returns the decode rows'
-// lanes in admission order.
+// order while fewer than `rows` are admitted (each takes the lowest free lane: its record, sampler, penalty rows,
+// automaton and scoring are reset), and every admitted request whose prefill is complete gets its decode row's records
+// (stream, automaton, scoring). Returns the decode rows' lanes in admission order.
 int batcher_boundary(B *b, std::vector<int> &dec) {
     M *m = b->m;
     const size_t V = binfmt::kVocab;
@@ -1163,6 +1196,8 @@ int batcher_boundary(B *b, std::vector<int> &dec) {
         b->lane_used[q.lane] = 1;
         q.status = RWKV_B200_REQ_PREFILLING;
         ad.push_back(id);
+        b->h_gc[q.lane] = rk::GenConstraint{};
+        b->h_lp[q.lane] = rk::LogprobLane{-1, 0};
         CK(cudaMemcpyAsync(b->samp.p + q.lane, &q.sampler, sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
         if (q.sampler.presence_penalty != 0.0f || q.sampler.frequency_penalty != 0.0f) {
             int rc;
@@ -1177,8 +1212,34 @@ int batcher_boundary(B *b, std::vector<int> &dec) {
         if (q.status == RWKV_B200_REQ_PREFILLING && q.fed + 1 == q.prompt.size()) {
             q.status = RWKV_B200_REQ_GENERATING;
             b->h_gs[q.lane] = rk::GenStream{q.slot, q.max_new, q.prompt.back(), 0, 0};
+            b->h_gc[q.lane] = q.gc;
+            b->h_lp[q.lane] = q.lp;
         }
         if (q.status == RWKV_B200_REQ_GENERATING) dec.push_back(q.lane);
+    }
+    // the decode lanes' overrides, in CSR over the lanes, when one of them has some
+    b->n_ovr = 0;
+    for (unsigned long long id : ad)
+        if (b->reqs[id].status == RWKV_B200_REQ_GENERATING) b->n_ovr += b->reqs[id].ovr_tok.size();
+    if (b->n_ovr) {
+        std::vector<unsigned long long> start(b->rows + 1, 0), tok;
+        std::vector<float> val;
+        for (int l = 0; l < b->rows; ++l) {
+            start[l] = tok.size();
+            for (unsigned long long id : ad) {
+                const B::Req &q = b->reqs[id];
+                if (q.lane != l || q.status != RWKV_B200_REQ_GENERATING) continue;
+                tok.insert(tok.end(), q.ovr_tok.begin(), q.ovr_tok.end());
+                val.insert(val.end(), q.ovr_val.begin(), q.ovr_val.end());
+            }
+        }
+        start[b->rows] = tok.size();
+        int rc;
+        if ((rc = b->ovr_tok.grow(tok.size())) || (rc = b->ovr_val.grow(val.size())) || (rc = b->ovr_start.grow(b->rows + 1)))
+            return rc;
+        CK(cudaMemcpyAsync(b->ovr_tok.p, tok.data(), tok.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(b->ovr_val.p, val.data(), val.size() * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(b->ovr_start.p, start.data(), start.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
     }
     // the lanes' stop tokens, in CSR over the lanes
     std::vector<unsigned long long> start(b->rows + 1, 0), stop;
@@ -1257,13 +1318,15 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
         std::copy(passes.begin(), passes.end(), all.begin() + k * b->max_pass);
     }
     CK(cudaMemcpyAsync(b->passes.p, all.data(), all.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
-    bool pen = false;
+    // what the decode lanes use: each feature's work is enqueued only when one of them needs it
+    bool pen = false, constrained = false, scored = false, raw = false;
+    int top = 0; // the largest top_n of a scored lane
+    std::vector<const B::Req *> of_lane(b->rows, nullptr);
+    for (unsigned long long id : b->admitted) of_lane[b->reqs[id].lane] = &b->reqs[id];
     if (R > 0) {
         CK(cudaMemcpyAsync(b->gs.p, b->h_gs.data(), b->rows * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
         CK(cudaMemcpyAsync(b->row_stream.p, dec.data(), R * sizeof(int), cudaMemcpyHostToDevice, m->stream));
         // uniforms [steps][R]: row r at step k draws with its request's u[len + k]
-        std::vector<const B::Req *> of_lane(b->rows, nullptr);
-        for (unsigned long long id : b->admitted) of_lane[b->reqs[id].lane] = &b->reqs[id];
         std::vector<double> ug(steps * (size_t)R, 0.0);
         for (int r = 0; r < R; ++r) {
             const rk::GenStream &g = b->h_gs[dec[r]];
@@ -1271,26 +1334,80 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
             for (unsigned long long k = 0; k < steps && !q.u.empty(); ++k)
                 if (g.len + k < q.max_new) ug[k * R + r] = q.u[g.len + k];
             pen |= q.sampler.presence_penalty != 0.0f || q.sampler.frequency_penalty != 0.0f;
+            constrained |= q.gc.mask != nullptr;
+            if (q.lp.mode >= 0) {
+                scored = true;
+                raw |= q.lp.mode == RWKV_B200_LOGPROBS_RAW;
+                top = std::max(top, q.lp.top_n);
+            }
         }
         CK(cudaMemcpyAsync(b->u.p, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
     }
-    const PickChain pc{b->gs.p, b->row_stream.p, b->samp.p, pen ? b->pen_cnt.p : nullptr, b->pen_seen.p};
+    const size_t V = binfmt::kVocab, ring = (size_t)b->rows * kGenGroup, top_ring = top ? ring * rk::kMaxTopN : 0;
+    if (constrained) {
+        if ((rc = b->gc.grow(b->rows)) || (rc = b->fault.grow(3))) return rc;
+        CK(cudaMemcpyAsync(b->gc.p, b->h_gc.data(), b->rows * sizeof(rk::GenConstraint), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemsetAsync(b->fault.p, 0, 3 * sizeof(unsigned long long), m->stream));
+    }
+    // raw lanes read the model's rows: d_slogits itself, or a copy taken before the penalties, overrides and masks edit it
+    const bool raw_copy = raw && (pen || b->n_ovr || constrained);
+    if (scored) {
+        if ((rc = b->lp_lane.grow(b->rows)) || (rc = b->lp.grow(ring)) || (rc = b->rank.grow(ring)) ||
+            (rc = b->top_lp.grow(top_ring)) || (rc = b->top_tok.grow(top_ring)) || (raw_copy && (rc = b->raw.grow((size_t)b->rows * V))))
+            return rc;
+        CK(cudaMemcpyAsync(b->lp_lane.p, b->h_lp.data(), b->rows * sizeof(rk::LogprobLane), cudaMemcpyHostToDevice, m->stream));
+    }
+    const PickChain pc{b->gs.p, b->row_stream.p, b->samp.p, pen ? b->pen_cnt.p : nullptr, b->pen_seen.p, b->ovr_tok.p,
+                       b->ovr_val.p, b->n_ovr, constrained ? b->gc.p : nullptr, 0, b->ovr_start.p};
+    const rk::GenLogprobArgs la{m->d_slogits, (int)V, b->gs.p, b->row_stream.p, nullptr, m->d_sample, b->samp.p,
+                                top ? rk::kMaxTopN : 0, kGenGroup, b->lp.p, b->rank.p, b->top_tok.p, b->top_lp.p,
+                                b->lp_lane.p, raw_copy ? b->raw.p : nullptr};
     for (unsigned long long k = 0; k < steps; ++k) {
         if ((rc = gen_step_passes(m, b->passes.p + k * b->max_pass, step_rows[k], rk::kPfMaxTokens, H[k].data()))) return rc;
         if (R == 0) continue;
+        if (raw_copy) CK(cudaMemcpyAsync(b->raw.p, m->d_slogits, (size_t)R * V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
         if ((rc = pick_rows(m, pc, R, b->u.p + k * R))) return rc;
+        if (scored) {
+            rk::k_gen_logprob<<<(unsigned)R, rk::kNucThreads, 0, m->stream>>>(la);
+            LAUNCHED(m);
+        }
         rk::GenFeedbackArgs fb{b->gs.p, b->row_stream.p, R, nullptr, m->d_sample, b->stop.p, 0, b->out.p, kGenGroup,
-                               k + 1 < steps ? b->passes.p + (k + 1) * b->max_pass : nullptr, nullptr, nullptr,
-                               b->stop_start.p};
+                               k + 1 < steps ? b->passes.p + (k + 1) * b->max_pass : nullptr, constrained ? b->gc.p : nullptr,
+                               b->fault.p, b->stop_start.p};
         rk::k_gen_feedback<<<(unsigned)((R + 127) / 128), 128, 0, m->stream>>>(fb);
         LAUNCHED(m);
     }
-    // the group's end: the lanes' records and the tokens of the group come back with one synchronisation
+    // the group's end: the lanes' records and the tokens of the group (with their results and the automata's states
+    // when a lane uses them) come back with one synchronisation
+    unsigned long long fault[3] = {0, 0, 0};
     if (R > 0) {
         CK(cudaMemcpyAsync(b->h_gs.data(), b->gs.p, b->rows * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
         CK(cudaMemcpyAsync(b->h_out.data(), b->out.p, b->h_out.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
     }
+    if (constrained) {
+        CK(cudaMemcpyAsync(b->h_gc.data(), b->gc.p, b->rows * sizeof(rk::GenConstraint), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(fault, b->fault.p, sizeof(fault), cudaMemcpyDeviceToHost, m->stream));
+    }
+    if (scored) {
+        b->h_lpv.resize(ring);
+        b->h_rank.resize(ring);
+        b->h_top_lp.resize(top_ring);
+        b->h_top_tok.resize(top_ring);
+        CK(cudaMemcpyAsync(b->h_lpv.data(), b->lp.p, ring * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(b->h_rank.data(), b->rank.p, ring * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+        if (top) {
+            CK(cudaMemcpyAsync(b->h_top_lp.data(), b->top_lp.p, top_ring * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+            CK(cudaMemcpyAsync(b->h_top_tok.data(), b->top_tok.p, top_ring * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+        }
+    }
     SYNC(m);
+    if (fault[0]) {
+        unsigned long long rid = 0;
+        for (unsigned long long id : b->admitted)
+            if (b->reqs[id].lane == (int)(fault[0] - 1)) rid = id;
+        return fail(8, "batcher_run: request %llu emitted token %llu, which has no edge out of state %llu of its constraint", rid,
+                    fault[1], fault[2]);
+    }
     for (unsigned long long id : b->admitted) {
         B::Req &q = b->reqs[id];
         if (q.status == RWKV_B200_REQ_PREFILLING) {
@@ -1298,7 +1415,18 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
             continue;
         }
         const rk::GenStream &g = b->h_gs[q.lane];
-        for (unsigned long long j = q.tokens.size(); j < g.len; ++j) q.tokens.push_back(b->h_out[(size_t)q.lane * kGenGroup + j % kGenGroup]);
+        for (unsigned long long j = q.tokens.size(); j < g.len; ++j) {
+            const size_t e = (size_t)q.lane * kGenGroup + j % kGenGroup;
+            q.tokens.push_back(b->h_out[e]);
+            if (q.lp.mode < 0) continue;
+            q.logprobs.push_back(b->h_lpv[e]);
+            q.ranks.push_back(b->h_rank[e]);
+            for (int t = 0; t < q.lp.top_n; ++t) {
+                q.top_tokens.push_back(b->h_top_tok[e * rk::kMaxTopN + t]);
+                q.top_logprobs.push_back(b->h_top_lp[e * rk::kMaxTopN + t]);
+            }
+        }
+        if (q.gc.mask) q.gc.state = b->h_gc[q.lane].state;
         if (g.done) q.status = RWKV_B200_REQ_DONE;
     }
     // finished requests leave here, before the next boundary admits anyone (a caller may release them in between)
@@ -1676,6 +1804,12 @@ int rwkv_b200_constraint_remove(rwkv_b200_model *m, unsigned long long id) {
     if (rc) return rc;
     const auto it = m->automata.find(id);
     if (it == m->automata.end()) return fail(1, "constraint_remove: constraint id %llu is unknown or removed", id);
+    // the lane records of the model's batcher point into the automaton's device block
+    if (const rwkv_b200_batcher *b = m->batcher)
+        for (const auto &e : b->reqs)
+            if (e.second.constraint_id == id && e.second.status <= RWKV_B200_REQ_GENERATING)
+                return fail(1, "constraint_remove: constraint id %llu is named by unfinished request %llu of the model's batcher",
+                            id, e.first);
     CK(cudaSetDevice(m->device));
     m->automata.erase(it);
     return 0;
@@ -2151,6 +2285,8 @@ int rwkv_b200_batcher_open(rwkv_b200_model *m, unsigned long long rows, unsigned
     b->lane_used.assign(rows, 0);
     b->h_gs.assign(rows, rk::GenStream{});
     b->h_out.assign(rows * kGenGroup, 0);
+    b->h_gc.assign(rows, rk::GenConstraint{});
+    b->h_lp.assign(rows, rk::LogprobLane{-1, 0});
     if ((rc = b->gs.grow(rows)) || (rc = b->row_stream.grow(rows)) || (rc = b->passes.grow(kGenGroup * (size_t)b->max_pass)) ||
         (rc = b->samp.grow(rows)) || (rc = b->stop_start.grow(rows + 1)) || (rc = b->out.grow(rows * kGenGroup)) ||
         (rc = b->u.grow(kGenGroup * rows))) {
@@ -2162,7 +2298,8 @@ int rwkv_b200_batcher_open(rwkv_b200_model *m, unsigned long long rows, unsigned
     return 0;
 }
 
-int rwkv_b200_batcher_submit(rwkv_b200_batcher *b, const rwkv_b200_request *r, unsigned long long *id) {
+int rwkv_b200_batcher_submit_ex(rwkv_b200_batcher *b, const rwkv_b200_request *r, const rwkv_b200_request_ex *x,
+                                unsigned long long *id) {
     const char *what = "batcher_submit";
     int rc = check_batcher(b);
     if (rc) return rc;
@@ -2175,6 +2312,17 @@ int rwkv_b200_batcher_submit(rwkv_b200_batcher *b, const rwkv_b200_request *r, u
         (rc = check_tokens(what, "stop token", r->stop, r->n_stop)) ||
         (rc = check_sampler(what, s, r->sampler, true, r->u != nullptr)) || (rc = check_uniforms(what, r->u, r->max_new)))
         return rc;
+    std::vector<rk::GenConstraint> gc(1);
+    if (x) {
+        if (x->n_override && (!x->override_tokens || !x->override_values))
+            return fail(1, "%s: n_override = %llu with NULL override_tokens or override_values", what, x->n_override);
+        const ConstraintRequest cq{&x->constraint_id, &x->start_state, nullptr};
+        if ((rc = check_tokens(what, "override token", x->override_tokens, x->n_override)) ||
+            (rc = check_overrides(what, x->override_tokens, x->override_values, x->n_override)) ||
+            (rc = check_constraints(b->m, what, cq, 1, x->override_tokens, x->override_values, x->n_override, gc)) ||
+            (x->logprobs && (rc = check_logprob_mode(what, x->logprob_mode, x->top_n))))
+            return rc;
+    }
     for (const auto &e : b->reqs)
         if (e.second.slot == r->slot && e.second.status <= RWKV_B200_REQ_GENERATING)
             return fail(1, "%s: slot %llu is held by unfinished request %llu", what, r->slot, e.first);
@@ -2185,11 +2333,22 @@ int rwkv_b200_batcher_submit(rwkv_b200_batcher *b, const rwkv_b200_request *r, u
     if (r->n_stop) q.stop.assign(r->stop, r->stop + r->n_stop);
     if (r->u) q.u.assign(r->u, r->u + r->max_new);
     q.sampler = r->sampler;
+    if (x) {
+        q.ovr_tok.assign(x->override_tokens, x->override_tokens + x->n_override);
+        q.ovr_val.assign(x->override_values, x->override_values + x->n_override);
+        q.gc = gc[0];
+        if (q.gc.mask) q.constraint_id = x->constraint_id;
+        if (x->logprobs) q.lp = rk::LogprobLane{x->logprob_mode, (int)x->top_n};
+    }
     b->reqs[s] = std::move(q);
     b->queue.push_back(s);
     b->next_id += 1;
     *id = s;
     return 0;
+}
+
+int rwkv_b200_batcher_submit(rwkv_b200_batcher *b, const rwkv_b200_request *r, unsigned long long *id) {
+    return rwkv_b200_batcher_submit_ex(b, r, nullptr, id);
 }
 
 int rwkv_b200_batcher_run(rwkv_b200_batcher *b, unsigned long long max_steps, unsigned long long *steps_run) {
@@ -2219,6 +2378,31 @@ int rwkv_b200_batcher_read(rwkv_b200_batcher *b, unsigned long long id, unsigned
     if (cap && !tokens_out) return fail(1, "batcher_read: cap = %llu with NULL tokens_out", cap);
     const size_t n = std::min<size_t>(cap, q.tokens.size());
     if (n) memcpy(tokens_out, q.tokens.data(), n * sizeof(unsigned long long));
+    if (len) *len = q.tokens.size();
+    if (status) *status = q.status;
+    return 0;
+}
+
+int rwkv_b200_batcher_read_ex(rwkv_b200_batcher *b, unsigned long long id, unsigned long long cap,
+                              unsigned long long *tokens_out, double *logprobs_out, unsigned long long *ranks_out,
+                              unsigned long long *top_tokens_out, double *top_logprobs_out, unsigned long long *state_out,
+                              unsigned long long *len, int *status) {
+    const char *what = "batcher_read_ex";
+    int rc = check_batcher(b);
+    if (rc) return rc;
+    const auto it = b->reqs.find(id);
+    if (it == b->reqs.end()) return fail(1, "%s: request %llu is unknown or released", what, id);
+    const B::Req &q = it->second;
+    if (q.lp.mode < 0 && (logprobs_out || ranks_out || top_tokens_out || top_logprobs_out))
+        return fail(1, "%s: request %llu has no log-probabilities (submit_ex with logprobs = 0 or without an extension)", what,
+                    id);
+    const size_t n = std::min<size_t>(cap, q.tokens.size()), nt = n * (size_t)std::max(q.lp.top_n, 0);
+    if (tokens_out && n) memcpy(tokens_out, q.tokens.data(), n * sizeof(unsigned long long));
+    if (logprobs_out && n) memcpy(logprobs_out, q.logprobs.data(), n * sizeof(double));
+    if (ranks_out && n) memcpy(ranks_out, q.ranks.data(), n * sizeof(unsigned long long));
+    if (top_tokens_out && nt) memcpy(top_tokens_out, q.top_tokens.data(), nt * sizeof(unsigned long long));
+    if (top_logprobs_out && nt) memcpy(top_logprobs_out, q.top_logprobs.data(), nt * sizeof(double));
+    if (state_out) *state_out = q.gc.mask ? q.gc.state : 0;
     if (len) *len = q.tokens.size();
     if (status) *status = q.status;
     return 0;

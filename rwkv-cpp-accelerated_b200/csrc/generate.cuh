@@ -35,11 +35,20 @@ __global__ void k_gen_gate(const GenStream *gs, const int *row_stream, int r, un
     ctrl->slot = g.done ? scratch : g.slot;
 }
 
-// logits[r][tok[i]] = val[i] for every row, in the order given (a repeated token keeps its last value).
-__global__ void k_gen_override(float *logits, int V, int rows, const unsigned long long *tok, const float *val, int n) {
+// logits[r][tok[i]] = val[i] for every row, in the order given (a repeated token keeps its last value). The batcher
+// gives each row its own list: with `start` set, row r applies i in [start[s], start[s + 1]) of its stream s =
+// row_stream[r] (n is not read); start == nullptr: i in [0, n) for every row.
+__global__ void k_gen_override(float *logits, int V, int rows, const unsigned long long *tok, const float *val, int n,
+                               const int *row_stream = nullptr, const unsigned long long *start = nullptr) {
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= rows) return;
-    for (int i = 0; i < n; ++i) logits[(size_t)r * V + tok[i]] = val[i];
+    unsigned long long i0 = 0, i1 = (unsigned long long)n;
+    if (start) {
+        const int s = row_stream[r];
+        i0 = start[s];
+        i1 = start[s + 1];
+    }
+    for (unsigned long long i = i0; i < i1; ++i) logits[(size_t)r * V + tok[i]] = val[i];
 }
 
 // A stream's token automaton (include/rwkv_b200.h, rwkv_b200_constraint_add) and its current state. State q's edges are

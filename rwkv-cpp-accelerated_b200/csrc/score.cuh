@@ -134,6 +134,12 @@ __global__ void __launch_bounds__(kNucThreads) k_logprob_rows(ScoreArgs a) {
                 a.top_tokens + (size_t)j * a.top_n, a.top_logprobs + (size_t)j * a.top_n);
 }
 
+// What the batcher asks of one lane: mode < 0: no scoring, else RWKV_B200_LOGPROBS_*; top_n <= the call's top_n.
+struct LogprobLane {
+    int mode;
+    int top_n;
+};
+
 struct GenLogprobArgs {
     const float *logits;                 // [rows][V] the rows of the current step
     int V;
@@ -142,26 +148,44 @@ struct GenLogprobArgs {
     const unsigned long long *next;      // arg-max per row, or nullptr when sampling
     const double *sample;                // {token, margin} per row when sampling
     const rwkv_b200_sampler *samp;       // processed mode with samplers: tau = temperature (> 0), else nullptr: tau = 1
-    int top_n;
+    int top_n;                           // top entries per token, and the stride of the top arrays
     unsigned long long max_new;
-    double *logprob;                     // [n_streams][max_new]
+    double *logprob;                     // [n_streams][max_new]: token k of stream s at [s][k % max_new]
     unsigned long long *rank;            // [n_streams][max_new]
     unsigned long long *top_tokens;      // [n_streams][max_new][top_n]
     double *top_logprobs;                // [n_streams][max_new][top_n]
+    // the batcher: each stream's own mode and top_n (samp then holds every stream's sampler); raw-mode streams read
+    // `raw` ([rows][V], nullptr: `logits`). lane == nullptr: every stream has the call's mode (samp) and top_n
+    const LogprobLane *lane;
+    const float *raw;
 };
 
 // generate_streams_logprobs: one CTA of kNucThreads per row of the step, between the pick and k_gen_feedback. It scores
-// the picked token of a live stream at entry [s][len]. A stream that finished earlier in the group still has a row, and
-// its len may equal max_new, so writing for it would land on stream s + 1: it returns at once (the whole CTA, before
-// any barrier).
+// the picked token of a live stream at entry [s][len]; with `lane` (the batcher) at [s][len % max_new], a ring of
+// kGenGroup entries per lane, as k_gen_feedback keeps its tokens. A stream that finished earlier in the group still has a row, and its len may equal max_new, so writing
+// for it would land on stream s + 1; it and a batcher lane without scoring return at once (the whole CTA, before any
+// barrier).
 __global__ void __launch_bounds__(kNucThreads) k_gen_logprob(const GenLogprobArgs a) {
     const int r = blockIdx.x, s = a.row_stream[r];
     const GenStream &g = a.gs[s];
     if (g.done) return;
+    const float *logits = a.logits;
+    const rwkv_b200_sampler *samp = a.samp;
+    int top_n = a.top_n;
+    if (a.lane) {
+        const LogprobLane ln = a.lane[s];
+        if (ln.mode < 0) return;
+        top_n = ln.top_n;
+        if (ln.mode == RWKV_B200_LOGPROBS_RAW) {
+            samp = nullptr;
+            if (a.raw) logits = a.raw;
+        }
+    }
     const int y = a.next ? (int)a.next[r] : (int)a.sample[2 * r];
-    const float T = a.samp ? a.samp[s].temperature : 0.0f;
-    const size_t o = (size_t)s * a.max_new + g.len;
-    logprob_row(a.logits + (size_t)r * a.V, a.V, y, T > 0.0f ? (double)T : 1.0, a.top_n, a.logprob + o, a.rank + o,
+    const float T = samp ? samp[s].temperature : 0.0f;
+    // the division only where it can matter: a 64-bit `%` on every path costs k_gen_logprob spills at 64 registers
+    const size_t o = (size_t)s * a.max_new + (a.lane ? g.len % a.max_new : g.len);
+    logprob_row(logits + (size_t)r * a.V, a.V, y, T > 0.0f ? (double)T : 1.0, top_n, a.logprob + o, a.rank + o,
                 a.top_tokens + o * a.top_n, a.top_logprobs + o * a.top_n);
 }
 

@@ -44,6 +44,14 @@ class Request(ctypes.Structure):
                 ("stop", P), ("n_stop", ctypes.c_ulonglong)]
 
 
+class RequestEx(ctypes.Structure):
+    """rwkv_b200_request_ex: what Batcher.submit adds to a request (overrides, an automaton, log-probabilities)."""
+    _fields_ = [("override_tokens", ctypes.POINTER(ctypes.c_ulonglong)), ("override_values", ctypes.POINTER(ctypes.c_float)),
+                ("n_override", ctypes.c_ulonglong), ("constraint_id", ctypes.c_ulonglong),
+                ("start_state", ctypes.c_ulonglong), ("logprobs", ctypes.c_int), ("logprob_mode", ctypes.c_int),
+                ("top_n", ctypes.c_uint)]
+
+
 REQ_STATUS = ("queued", "prefilling", "generating", "done", "cancelled")  # RWKV_B200_REQ_* in order
 
 
@@ -190,8 +198,10 @@ def load_library():
                                                          pull, pull]),
         "rwkv_b200_batcher_open": (i32, [vp, ull, ull, c.POINTER(vp)]),
         "rwkv_b200_batcher_submit": (i32, [vp, c.POINTER(Request), pull]),
+        "rwkv_b200_batcher_submit_ex": (i32, [vp, c.POINTER(Request), c.POINTER(RequestEx), pull]),
         "rwkv_b200_batcher_run": (i32, [vp, ull, pull]),
         "rwkv_b200_batcher_read": (i32, [vp, ull, pull, ull, pull, c.POINTER(i32)]),
+        "rwkv_b200_batcher_read_ex": (i32, [vp, ull, ull, pull, pdbl, pull, pull, pdbl, pull, pull, c.POINTER(i32)]),
         "rwkv_b200_batcher_cancel": (i32, [vp, ull]),
         "rwkv_b200_batcher_release": (i32, [vp, ull]),
         "rwkv_b200_batcher_close": (None, [vp]),
@@ -641,11 +651,15 @@ class Batcher:
         engine._ck(self.lib.rwkv_b200_batcher_open(engine.h, int(rows), int(prefill_tokens), ctypes.byref(h)),
                    "batcher_open")
         self.h = h
+        self._ext = {}  # id -> (top_n or None without log-probabilities, constrained) of requests sent through submit_ex
 
-    def submit(self, slot, prompt, max_new, sampling=None, u=None, stop=()):
+    def submit(self, slot, prompt, max_new, sampling=None, u=None, stop=(), overrides=None, constraint=None, logprobs=None,
+               top_n=0):
         """Queue a request on state slot `slot`: prompt (>= 1 token ids), up to max_new new tokens, a Sampler or dict
         (None: arg-max), u: max_new uniforms in [0, 1) (None only at temperature 0), stop: this request's stop tokens.
-        Returns its id. Every array is copied."""
+        overrides = {token: logit value} as in generate_streams; constraint: an id of Engine.add_constraint, or (id,
+        start_state); logprobs = "raw" or "processed" scores every emitted token, with top_n top entries (read them with
+        result). Returns its id. Every array is copied."""
         sp = _samplers(sampling if sampling is not None else Sampler(temperature=0.0), 1)[0]
         pr = np.ascontiguousarray(np.atleast_1d(np.asarray(prompt, dtype=np.uint64)))
         st = np.ascontiguousarray(list(stop), dtype=np.uint64)
@@ -655,7 +669,23 @@ class Batcher:
         P = ctypes.c_ulonglong
         req = Request(int(slot), _ptr(pr, P), len(pr), int(max_new), sp, _ptr(us, ctypes.c_double), _ptr(st, P), len(st))
         rid = ctypes.c_ulonglong()
-        self.engine._ck(self.lib.rwkv_b200_batcher_submit(self.h, ctypes.byref(req), ctypes.byref(rid)), "batcher_submit")
+        if overrides is None and constraint is None and logprobs is None:
+            self.engine._ck(self.lib.rwkv_b200_batcher_submit(self.h, ctypes.byref(req), ctypes.byref(rid)), "batcher_submit")
+            return int(rid.value)
+        modes = {None: LOGPROBS_RAW, "raw": LOGPROBS_RAW, "processed": LOGPROBS_PROCESSED}
+        if logprobs not in modes:
+            raise EngineError("batcher.submit: logprobs must be 'raw' or 'processed', not %r" % (logprobs,))
+        ovr = dict(overrides or {})
+        otok = np.ascontiguousarray(list(ovr.keys()), dtype=np.uint64)
+        oval = np.ascontiguousarray(list(ovr.values()), dtype=np.float32)
+        cid, q0 = NO_CONSTRAINT, 0
+        if constraint is not None:
+            cid, q0 = (int(constraint[0]), int(constraint[1])) if isinstance(constraint, (tuple, list)) else (int(constraint), 0)
+        x = RequestEx(_ptr(otok, P), _ptr(oval, ctypes.c_float), len(otok), cid, q0, 1 if logprobs is not None else 0,
+                      modes[logprobs], int(top_n))
+        self.engine._ck(self.lib.rwkv_b200_batcher_submit_ex(self.h, ctypes.byref(req), ctypes.byref(x), ctypes.byref(rid)),
+                        "batcher_submit")
+        self._ext[int(rid.value)] = (int(top_n) if logprobs is not None else None, constraint is not None)
         return int(rid.value)
 
     def run(self, max_steps):
@@ -674,11 +704,41 @@ class Batcher:
                         "batcher_read")
         return out, REQ_STATUS[status.value]
 
+    def result(self, rid):
+        """Everything a request has produced so far, as a dict: "tokens" (np.uint64) and "status" (one of REQ_STATUS);
+        with logprobs "logprobs" (float64) and "ranks" (uint64), and with top_n > 0 "top_tokens" / "top_logprobs"
+        [len][top_n], as generate_streams(logprobs=...) returns them; with a constraint "state" (the automaton's
+        current state)."""
+        top_n, constrained = self._ext.get(int(rid), (None, False))
+        n, status = ctypes.c_ulonglong(), ctypes.c_int()
+        self.engine._ck(self.lib.rwkv_b200_batcher_read(self.h, int(rid), None, 0, ctypes.byref(n), ctypes.byref(status)),
+                        "batcher_read")
+        L = int(n.value)
+        toks = np.zeros(L, np.uint64)
+        lp = np.zeros(L, np.float64) if top_n is not None else None
+        ranks = np.zeros(L, np.uint64) if top_n is not None else None
+        top_tok = np.zeros((L, top_n), np.uint64) if top_n else None
+        top_lp = np.zeros((L, top_n), np.float64) if top_n else None
+        state = ctypes.c_ulonglong()
+        P, D = ctypes.c_ulonglong, ctypes.c_double
+        self.engine._ck(self.lib.rwkv_b200_batcher_read_ex(self.h, int(rid), L, _ptr(toks, P), _ptr(lp, D), _ptr(ranks, P),
+                                                           _ptr(top_tok, P), _ptr(top_lp, D), ctypes.byref(state), None,
+                                                           None), "batcher_read_ex")
+        d = {"tokens": toks, "status": REQ_STATUS[status.value]}
+        if top_n is not None:
+            d["logprobs"], d["ranks"] = lp, ranks
+            if top_n:
+                d["top_tokens"], d["top_logprobs"] = top_tok, top_lp
+        if constrained:
+            d["state"] = int(state.value)
+        return d
+
     def cancel(self, rid):
         self.engine._ck(self.lib.rwkv_b200_batcher_cancel(self.h, int(rid)), "batcher_cancel")
 
     def release(self, rid):
         self.engine._ck(self.lib.rwkv_b200_batcher_release(self.h, int(rid)), "batcher_release")
+        self._ext.pop(int(rid), None)
 
     def close(self):
         if getattr(self, "h", None) and getattr(self.engine, "h", None):
