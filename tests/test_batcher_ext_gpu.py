@@ -1,26 +1,25 @@
 """Batcher requests with logit overrides, token automata and log-probabilities (rwkv_b200_batcher_submit_ex) against
 each request run alone through the existing API.
 
-The oracle is that of tests/test_batcher_gpu.py: a second engine from the same state, prefill_min = 2, forward_streams of
-prompt[:-1] (state only) and then one generate_streams call of (slot, prompt[-1]) plus a pad stream on a spare slot. Here
-that call also carries the request's overrides, its automaton (the pad has none) and its log-probability mode and top_n,
-so it is generate_streams_constrained, generate_streams_logprobs or generate_streams_ex. The pad gets the call-wide
-overrides, mode and stops, which is harmless: rows are independent. Tokens, log-probabilities, ranks, top entries (NaN
-and -inf compared as bits), final automaton states and every named slot must equal the oracle; unnamed slots must not
-change."""
+The oracle is the plain batcher tests' (decoding.batcher_oracle): a second engine from the same state, prefill_min = 2,
+forward_streams of prompt[:-1] (state only) and then one generate_streams call of (slot, prompt[-1]) plus a pad stream on
+a spare slot. Here that call also carries the request's overrides, its automaton (the pad has none) and its
+log-probability mode and top_n, so it is generate_streams_constrained, generate_streams_logprobs or generate_streams_ex.
+The pad gets the call-wide overrides, mode and stops, which is harmless: rows are independent. Tokens, log-probabilities,
+ranks, top entries (NaN and -inf compared as bits), final automaton states and every named slot must equal the oracle;
+unnamed slots must not change."""
 import ctypes
 
 import numpy as np
 import pytest
 
-from test_batcher_gpu import KEYS, LENGTHS, MAX_GPT, PAD, check_slots, engines, finish, samplers
-from test_constrain_gpu import OVERRIDES, REGEXES, prefix_state
+from decoding import (FIELDS, KEYS5, LENGTHS, MAX_GPT, OVERRIDES, PAD, SHAPES, V, add_stops, batcher_oracle,
+                      batcher_samplers, bits, check_slots, engine_pair, ext, finish, regex_automata, run_schedule,
+                      submit)
 
 pytestmark = pytest.mark.gpu
 
-V = 50277
-SHAPES = [(3, 768), (2, 2048)]
-FIELDS = ("tokens", "logprobs", "ranks", "top_tokens", "top_logprobs")
+RESULT_FIELDS = ("tokens",) + FIELDS
 BIAS = {11: 1e3, 187: -99.0, 50: -np.inf}  # token 11 wins every unmasked pick
 EOS = {0: 50.0}                            # the automata's eos (token 0) wins wherever a state allows it
 # per request i, kind i % 10: (overrides, automaton, logprobs, top_n); automaton "date+" starts after "2024-"
@@ -40,10 +39,7 @@ KINDS = [
 
 @pytest.fixture(scope="module")
 def autos(pkg):
-    C = pkg.constrain
-    tb = C.token_bytes()
-    au = {k: C.token_automaton(C.compile_regex(REGEXES[k]), tb, eos=0) for k in ("date", "labels", "json")}
-    return au, {"date+": prefix_state(au["date"], tb, "2024-")}
+    return regex_automata(pkg.constrain, ("date", "labels", "json"))
 
 
 def register(engs, autos):
@@ -57,9 +53,9 @@ def register(engs, autos):
     return ids
 
 
-def make_requests(pkg, n, seed, slots, ids, autos, kinds=None):
+def make_mixed_requests(pkg, n, seed, slots, ids, autos, kinds=None):
     rng = np.random.default_rng(seed)
-    sp = samplers(pkg)
+    sp = batcher_samplers(pkg)
     reqs = []
     for i in range(n):
         ovr, auto, lp, top = KINDS[(kinds[i] if kinds else i) % len(KINDS)]
@@ -75,63 +71,14 @@ def make_requests(pkg, n, seed, slots, ids, autos, kinds=None):
     return reqs
 
 
-def ext(r):
-    return r["overrides"] is not None or r["constraint"] is not None or r["logprobs"] is not None
-
-
-def oracle(pkg, b, r):
-    """The rule's two calls for one request on engine b: its result dict as Batcher.result gives it (no status)."""
-    slot, prompt = r["slot"], r["prompt"]
-    if len(prompt) > 1:
-        call = [(slot, prompt[:-1])]
-        if len(prompt) - 1 < 2:
-            call.append((PAD, prompt[:1]))
-        b.forward_streams(call, want_logits=False)
-    us = None if r["u"] is None else np.stack([r["u"], np.full(r["max_new"], 0.5)], axis=1)
-    kw = dict(stop=r["stop"], sampling=[r["sampling"], pkg.Sampler(temperature=0.0)], u=us, overrides=r["overrides"])
-    if r["logprobs"] is not None or r["constraint"] is not None:
-        kw.update(logprobs=r["logprobs"], top_n=r["top_n"],
-                  constraints=[r["constraint"], None] if r["constraint"] is not None else None)
-    out = b.generate_streams([(slot, prompt[-1]), (PAD, prompt[-1])], r["max_new"], **kw)[0]
-    d = dict(out) if isinstance(out, dict) else {"tokens": out}
-    if d.get("state", 0) is None:
-        del d["state"]
-    return d
-
-
-def add_stops(pkg, b, reqs):
-    """Every other unconstrained request gets a stop token from its own run, so that it fires mid-way."""
-    st = b.state_download(MAX_GPT)
-    for i, r in enumerate(reqs):
-        if i % 2 == 0 or r["constraint"] is not None:
-            continue
-        toks = [int(x) for x in oracle(pkg, b, r)["tokens"]]
-        fresh = [k for k in range(len(toks) // 2, len(toks)) if toks[k] not in toks[:k]]
-        if fresh:
-            r["stop"] = (toks[fresh[0]],)
-    b.state_upload(st, MAX_GPT)
-
-
-def submit(bat, r):
-    if not ext(r):
-        return bat.submit(r["slot"], r["prompt"], r["max_new"], sampling=r["sampling"], u=r["u"], stop=r["stop"])
-    return bat.submit(r["slot"], r["prompt"], r["max_new"], sampling=r["sampling"], u=r["u"], stop=r["stop"],
-                      overrides=r["overrides"], constraint=r["constraint"], logprobs=r["logprobs"], top_n=r["top_n"])
-
-
-def bits(x):
-    x = np.ascontiguousarray(x)
-    return x.view(np.uint64) if x.dtype == np.float64 else x
-
-
-def check(got, want, what, prefix=False):
+def check_result(got, want, what, prefix=False):
     """got (Batcher.result) equals want (oracle) in every field, bit for bit; prefix: got is a prefix of want."""
     assert set(got) - {"status"} == set(want), (what, sorted(got), sorted(want))
     n = len(got["tokens"])
     assert n == len(want["tokens"]) or (prefix and n <= len(want["tokens"])), (what, n, len(want["tokens"]))
-    for k in FIELDS:
+    for k in RESULT_FIELDS:
         if k in want:
-            assert np.array_equal(bits(got[k]), bits(want[k][:n])), (what, k)
+            assert bits(got[k]) == bits(want[k][:n]), (what, k)
     if "state" in want and not prefix:
         assert got["state"] == want["state"], (what, "state")
 
@@ -140,12 +87,12 @@ def check(got, want, what, prefix=False):
 def setup(request, pkg, make_model, autos):
     """The engines with the automata, ~40 mixed requests with stops, and their oracle results."""
     L, E = request.param
-    a, b = engines(pkg, make_model(L, E))
+    a, b = engine_pair(pkg, make_model(L, E), MAX_GPT, tc=True, one_draw=True)
     ids = register((a, b), autos)
     before = a.state_download(MAX_GPT)
-    reqs = make_requests(pkg, 40, 7, list(range(40)), ids, autos)
+    reqs = make_mixed_requests(pkg, 40, 7, list(range(40)), ids, autos)
     add_stops(pkg, b, reqs)
-    want = [oracle(pkg, b, r) for r in reqs]
+    want = [batcher_oracle(pkg, b, r) for r in reqs]
     assert any(len(w["tokens"]) < r["max_new"] for w, r in zip(want, reqs) if r["constraint"] is None), "no stop fired"
     yield pkg, a, b, before, reqs, want, ids
     a.close()
@@ -167,35 +114,27 @@ def test_mixed_waves_equal_oracle(setup, autos, rows, prefill):
         for i, (rid, w) in enumerate(zip(rids, want)):
             got = bat.result(rid)
             assert got["status"] == "done", (i, got["status"])
-            check(got, w, "request %d" % i)
+            check_result(got, w, "request %d" % i)
             r = reqs[i]
             if r["constraint"] is not None:
                 assert len(got["tokens"]) < r["max_new"], i
                 assert autos[0][r["auto"]].complete(got["state"]), i
             tokens, status = bat.read(rid)
             assert status == "done" and np.array_equal(tokens, got["tokens"])
-    check_slots(a, b, before, {r["slot"] for r in reqs}, "rows=%d prefill=%d" % (rows, prefill))
-
-
-def run_schedule(a, before, reqs, rows, prefill, steps):
-    a.state_upload(before, MAX_GPT)
-    with a.batcher(rows, prefill) as bat:
-        rids = [submit(bat, r) for r in reqs]
-        while bat.run(steps):
-            pass
-        res = [bat.result(i) for i in rids]
-    return res, a.state_download(MAX_GPT)
+    check_slots(a, b, before, MAX_GPT, {r["slot"] for r in reqs}, keys=KEYS5, skip=(PAD,),
+                what="rows=%d prefill=%d" % (rows, prefill))
 
 
 def test_two_schedules_identical(setup):
     pkg, a, b, before, reqs, want, ids = setup
-    r1, s1 = run_schedule(a, before, reqs[:14], 8, 64, 1000)
-    r2, s2 = run_schedule(a, before, reqs[:14], 3, 5, 7)
+    result = lambda bat, rid: bat.result(rid)
+    r1, s1 = run_schedule(a, before, reqs[:14], 8, 64, 1000, result)
+    r2, s2 = run_schedule(a, before, reqs[:14], 3, 5, 7, result)
     for i, (x, y) in enumerate(zip(r1, r2)):
         assert set(x) == set(y)
         for k in x:
-            assert np.array_equal(bits(x[k]), bits(y[k])) if k in FIELDS else x[k] == y[k], (i, k)
-    for k in KEYS:
+            assert bits(x[k]) == bits(y[k]) if k in RESULT_FIELDS else x[k] == y[k], (i, k)
+    for k in KEYS5:
         assert np.array_equal(s1[k], s2[k]), k
 
 
@@ -210,9 +149,9 @@ def test_streaming_prefix(setup):
             for i, rid in enumerate(rids):
                 seen.setdefault(i, []).append(bat.result(rid))
         for i, rid in enumerate(rids):
-            check(bat.result(rid), want[i], "request %d" % i)
+            check_result(bat.result(rid), want[i], "request %d" % i)
             for p in seen[i]:
-                check(p, want[i], "request %d, streamed" % i, prefix=True)
+                check_result(p, want[i], "request %d, streamed" % i, prefix=True)
     assert any(0 < len(p["tokens"]) < len(want[i]["tokens"]) for i in seen for p in seen[i]), "nothing streamed"
 
 
@@ -239,10 +178,10 @@ def test_cancel_constrained_scored(setup, autos):
         for i in pick:
             got = bat.result(rids[i])
             assert got["status"] == "cancelled"
-            check(got, want[i], "cancelled request %d" % i, prefix=True)
+            check_result(got, want[i], "cancelled request %d" % i, prefix=True)
             assert autos[0][reqs[i]["auto"]].walk([int(x) for x in got["tokens"]]) == got["state"], i
         for i in others:
-            check(bat.result(rids[i]), want[i], "request %d" % i)
+            check_result(bat.result(rids[i]), want[i], "request %d" % i)
 
 
 def test_lane_reuse(setup, autos):
@@ -252,15 +191,15 @@ def test_lane_reuse(setup, autos):
     a.state_upload(before, MAX_GPT)
     held = b.state_download(MAX_GPT)
     b.state_upload(before, MAX_GPT)
-    trio = make_requests(pkg, 3, 21, [100, 101, 102], ids, autos, kinds=[6, 0, 3])
+    trio = make_mixed_requests(pkg, 3, 21, [100, 101, 102], ids, autos, kinds=[6, 0, 3])
     assert trio[0]["overrides"] and trio[0]["constraint"] and trio[0]["logprobs"] == "raw"
     with a.batcher(1, 32) as bat:
         rids = [submit(bat, r) for r in trio]
         finish(bat)
         got = [bat.result(i) for i in rids]
     for i, r in enumerate(trio):
-        check(got[i], oracle(pkg, b, r), "lane reuse %d" % i)
-    check_slots(a, b, before, {100, 101, 102}, "lane reuse")
+        check_result(got[i], batcher_oracle(pkg, b, r), "lane reuse %d" % i)
+    check_slots(a, b, before, MAX_GPT, {100, 101, 102}, keys=KEYS5, skip=(PAD,), what="lane reuse")
     b.state_upload(held, MAX_GPT)
 
 
@@ -302,7 +241,7 @@ def test_cost_when_unused(setup):
 def test_refusals(pkg, make_model, autos):
     """Every refusal of submit_ex leaves every slot untouched, queues nothing and uses no id; remove_constraint is refused
     while a queued or running request names the id, and succeeds once that request is done or cancelled."""
-    a, _ = engines(pkg, make_model(3, 768))
+    a, _ = engine_pair(pkg, make_model(3, 768), MAX_GPT, tc=True, one_draw=True)
     ids = register((a,), autos)
     au, starts = autos
     before = a.state_download(MAX_GPT)
@@ -340,7 +279,7 @@ def test_refusals(pkg, make_model, autos):
         bat.cancel(plain)
         assert bat.run(16) == 0, "a refused request was queued"
         after = a.state_download(MAX_GPT)
-        for k in KEYS:
+        for k in KEYS5:
             assert np.array_equal(before[k], after[k]), k
         # the automaton of an unfinished request cannot be removed
         q = bat.submit(6, [1, 2, 3], 64, constraint=ids["json"])

@@ -9,30 +9,16 @@ oracle whatever the schedule, and slots no request names must not change at all.
 import numpy as np
 import pytest
 
+from decoding import (KEYS5, LENGTHS, MAX_GPT, PAD, SHAPES, V, add_stops, batcher_oracle, batcher_samplers, check_slots,
+                      engine_pair, finish, run_schedule, slot_of, submit)
+
 pytestmark = pytest.mark.gpu
-
-V = 50277
-KEYS = ("xy", "aa", "bb", "pp", "dd")
-SHAPES = [(3, 768), (2, 2048)]
-MAX_GPT = 320      # the longest prompt (300 tokens) is one forward_streams call of the oracle
-PAD = MAX_GPT - 1  # never named by a request
-LENGTHS = (1, 2, 31, 32, 33, 127, 128, 129, 300)
-
-
-def slot_of(state, slot, n):
-    return {k: state[k][slot * n:(slot + 1) * n] for k in state}
-
-
-def samplers(pkg):
-    S = pkg.Sampler
-    return [S(temperature=0.0), S(temperature=0.8, top_p=0.9), S(temperature=1.0, top_k=40, presence_penalty=0.6,
-            frequency_penalty=0.3, penalty_decay=0.95), S(temperature=0.0, presence_penalty=2.0, frequency_penalty=1.0)]
 
 
 def make_requests(pkg, n, seed, slots):
     """n requests on the given distinct slots: every prompt length of LENGTHS, a mix of samplers."""
     rng = np.random.default_rng(seed)
-    sp = samplers(pkg)
+    sp = batcher_samplers(pkg)
     reqs = []
     for i in range(n):
         L = LENGTHS[i % len(LENGTHS)] if i < 2 * len(LENGTHS) else int(rng.integers(1, 200))
@@ -44,72 +30,20 @@ def make_requests(pkg, n, seed, slots):
     return reqs
 
 
-def engines(pkg, path, seed=99):
-    """(a, b): a runs the batcher, b the oracle, both from the same non-trivial state of every slot."""
-    a = pkg.Engine(path, max_gpt=MAX_GPT)
-    b = pkg.Engine(path, max_gpt=MAX_GPT)
-    b.set_option("prefill_min", 2)
-    rng = np.random.default_rng(seed)
-    a.forward_streams([(j, [int(rng.integers(0, V))]) for j in range(MAX_GPT)], want_logits=False)
-    b.state_upload(a.state_download(MAX_GPT), MAX_GPT)
-    return a, b
-
-
-def oracle(pkg, b, r):
-    """Steps 1 and 2 of the rule for one request on engine b; returns its tokens."""
-    slot, prompt = r["slot"], r["prompt"]
-    if len(prompt) > 1:
-        call = [(slot, prompt[:-1])]
-        if len(prompt) - 1 < 2:
-            call.append((PAD, prompt[:1]))
-        b.forward_streams(call, want_logits=False)
-    us = None if r["u"] is None else np.stack([r["u"], np.full(r["max_new"], 0.5)], axis=1)
-    out = b.generate_streams([(slot, prompt[-1]), (PAD, prompt[-1])], r["max_new"], stop=r["stop"],
-                             sampling=[r["sampling"], pkg.Sampler(temperature=0.0)], u=us)
-    return [int(x) for x in out[0]]
-
-
-def add_stops(pkg, b, reqs):
-    """Give every other request a stop token taken from its own unconstrained run, so that it fires mid-way."""
-    st = b.state_download(MAX_GPT)
-    for i, r in enumerate(reqs):
-        if i % 2 == 0:
-            continue
-        toks = oracle(pkg, b, r)
-        fresh = [k for k in range(len(toks) // 2, len(toks)) if toks[k] not in toks[:k]]
-        if fresh:
-            r["stop"] = (toks[fresh[0]],)
-    b.state_upload(st, MAX_GPT)
-
-
-def submit(bat, r):
-    return bat.submit(r["slot"], r["prompt"], r["max_new"], sampling=r["sampling"], u=r["u"], stop=r["stop"])
-
-
-def finish(bat):
-    while bat.run(1000):
-        pass
-
-
-def check_slots(a, b, before, named, what):
-    n = a.n_layers * a.n_embed
-    sa, sb = a.state_download(MAX_GPT), b.state_download(MAX_GPT)
-    for slot in range(MAX_GPT - 1):
-        ref = sb if slot in named else before
-        for k in KEYS:
-            assert np.array_equal(slot_of(sa, slot, n)[k], slot_of(ref, slot, n)[k]), \
-                "%s: slot %d state %s (%s)" % (what, slot, k, "named" if slot in named else "untouched")
+def oracle_tokens(pkg, b, r):
+    """The rule's two calls for one request on engine b (decoding.batcher_oracle); returns its tokens."""
+    return [int(x) for x in batcher_oracle(pkg, b, r)["tokens"]]
 
 
 @pytest.fixture(scope="module", params=SHAPES, ids=["3x768", "2x2048"])
 def setup(request, pkg, make_model):
     """The engines, the ~40 requests with stops, and their oracle tokens (b holds every request's final state)."""
     L, E = request.param
-    a, b = engines(pkg, make_model(L, E))
+    a, b = engine_pair(pkg, make_model(L, E), MAX_GPT, tc=True, one_draw=True)
     before = a.state_download(MAX_GPT)
     reqs = make_requests(pkg, 40, 7, list(range(40)))
     add_stops(pkg, b, reqs)
-    want = [oracle(pkg, b, r) for r in reqs]
+    want = [oracle_tokens(pkg, b, r) for r in reqs]
     assert any(len(w) < r["max_new"] for w, r in zip(want, reqs)), "no stop token fired"
     yield pkg, a, b, before, reqs, want
     a.close()
@@ -131,25 +65,17 @@ def test_waves_equal_oracle(setup, rows, prefill):
             toks, status = bat.read(rid)
             assert status == "done", "request %d: %s" % (i, status)
             assert [int(x) for x in toks] == w, "request %d (prompt %d tokens): tokens" % (i, len(reqs[i]["prompt"]))
-    check_slots(a, b, before, {r["slot"] for r in reqs}, "rows=%d prefill=%d" % (rows, prefill))
-
-
-def run_schedule(pkg, a, before, reqs, rows, prefill, steps):
-    a.state_upload(before, MAX_GPT)
-    with a.batcher(rows, prefill) as bat:
-        ids = [submit(bat, r) for r in reqs]
-        while bat.run(steps):
-            pass
-        toks = [[int(x) for x in bat.read(i)[0]] for i in ids]
-    return toks, a.state_download(MAX_GPT)
+    check_slots(a, b, before, MAX_GPT, {r["slot"] for r in reqs}, keys=KEYS5, skip=(PAD,),
+                what="rows=%d prefill=%d" % (rows, prefill))
 
 
 def test_two_schedules_identical(setup):
     pkg, a, b, before, reqs, want = setup
-    t1, s1 = run_schedule(pkg, a, before, reqs[:12], 8, 64, 1000)
-    t2, s2 = run_schedule(pkg, a, before, reqs[:12], 3, 5, 7)
+    tokens = lambda bat, rid: [int(x) for x in bat.read(rid)[0]]
+    t1, s1 = run_schedule(a, before, reqs[:12], 8, 64, 1000, tokens)
+    t2, s2 = run_schedule(a, before, reqs[:12], 3, 5, 7, tokens)
     assert t1 == t2
-    for k in KEYS:
+    for k in KEYS5:
         assert np.array_equal(s1[k], s2[k]), k
 
 
@@ -226,19 +152,19 @@ def test_cancel(setup):
                 assert st == "done" and toks == want[i], i
         sa = a.state_download(MAX_GPT)
         q = sel[que[-1]]["slot"]
-        for k in KEYS:
+        for k in KEYS5:
             assert np.array_equal(slot_of(sa, q, n)[k], slot_of(before, q, n)[k]), "queued slot touched"
     sb = b.state_download(MAX_GPT)
     for i, r in enumerate(sel):
         if i not in cancelled:
-            for k in KEYS:
+            for k in KEYS5:
                 assert np.array_equal(slot_of(sa, r["slot"], n)[k], slot_of(sb, r["slot"], n)[k]), (i, k)
 
 
 def test_next_turn_and_unrelated_forward(pkg, make_model):
     """A second request on a finished request's slot equals the oracle chained on that slot, and a forward_streams on an
     unrelated slot between runs changes nothing in the batcher's results."""
-    a, b = engines(pkg, make_model(3, 768))
+    a, b = engine_pair(pkg, make_model(3, 768), MAX_GPT, tc=True, one_draw=True)
     before = a.state_download(MAX_GPT)
     reqs = make_requests(pkg, 6, 11, [40, 41, 42, 43, 44, 45])
     turn2 = make_requests(pkg, 2, 12, [40, 41])
@@ -253,18 +179,18 @@ def test_next_turn_and_unrelated_forward(pkg, make_model):
         ids2 = [submit(bat, r) for r in turn2]
         finish(bat)
         got = [[int(x) for x in bat.read(i)[0]] for i in ids[2:] + ids2]
-    want = [oracle(pkg, b, r) for r in reqs]
-    want2 = [oracle(pkg, b, r) for r in turn2]
+    want = [oracle_tokens(pkg, b, r) for r in reqs]
+    want2 = [oracle_tokens(pkg, b, r) for r in turn2]
     assert got == want[2:] + want2
     named = {r["slot"] for r in reqs} | {50}
-    check_slots(a, b, before, named, "next turn")
+    check_slots(a, b, before, MAX_GPT, named, keys=KEYS5, skip=(PAD,), what="next turn")
     a.close()
     b.close()
 
 
 def test_refusals(pkg, make_model):
     """Every refusal leaves every slot untouched; unknown ids are refused."""
-    a, _ = engines(pkg, make_model(3, 768))
+    a, _ = engine_pair(pkg, make_model(3, 768), MAX_GPT, tc=True, one_draw=True)
     before = a.state_download(MAX_GPT)
     E = pkg.EngineError
     for rows, pf in ((0, 16), (MAX_GPT + 1, 16), (4, 0), (4, 2049)):
@@ -298,6 +224,6 @@ def test_refusals(pkg, make_model):
         bat.release(rid)
         assert bat.run(16) == 0
     after = a.state_download(MAX_GPT)
-    for k in KEYS:
+    for k in KEYS5:
         assert np.array_equal(before[k], after[k]), k
     a.close()

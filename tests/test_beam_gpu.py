@@ -10,33 +10,9 @@ import math
 import numpy as np
 import pytest
 
+from decoding import KEYS5, SHAPES, check_slots, engine_pair, rand_tokens, slot_of
+
 pytestmark = pytest.mark.gpu
-
-V = 50277
-KEYS = ("xy", "aa", "bb", "pp", "dd")
-SHAPES = [(3, 768), (2, 2048)]
-
-
-def rand_tokens(n, seed):
-    return [int(x) for x in np.random.default_rng(seed).integers(0, V, size=n)]
-
-
-def slot_of(state, slot, n):
-    return {k: state[k][slot * n:(slot + 1) * n] for k in state}
-
-
-def engines(pkg, path, max_gpt, tc, seed=99):
-    """(a, b): a runs beam_search, b the host loop on the same path, both from the same non-trivial state. tc: both take
-    the tensor cores down to 2 rows (the loop's pad keeps a lone row there), else both the decode kernel."""
-    a = pkg.Engine(path, max_gpt=max_gpt)
-    b = pkg.Engine(path, max_gpt=max_gpt)
-    for e in (a, b):
-        e.set_option("prefill_min", 2) if tc else e.set_option("prefill", 0)
-    for i in range(0, max_gpt, 128):
-        n = min(128, max_gpt - i)
-        a.forward_streams([(i + j, [t]) for j, t in enumerate(rand_tokens(n, seed + i))], want_logits=False)
-    b.state_upload(a.state_download(max_gpt), max_gpt)
-    return a, b
 
 
 def offer(hyps, K, h):
@@ -114,7 +90,7 @@ def host_beam(eng, groups, max_new, B, stop=(), alpha=1.0, K=1, pad_slot=None, l
     return [g["hyps"] for g in st]
 
 
-def check(a, b, before, groups, got, want, max_gpt, what=""):
+def check_hypotheses(a, b, before, groups, got, want, max_gpt, what=""):
     assert len(got) == len(want)
     for gi, (gh, wh) in enumerate(zip(got, want)):
         assert len(gh) == len(wh), what + ": group %d holds %d hypotheses, expected %d" % (gi, len(gh), len(wh))
@@ -124,15 +100,7 @@ def check(a, b, before, groups, got, want, max_gpt, what=""):
             assert x["logprob"] == y["cum"] and x["score"] == y["score"], tag + ": logprob / score"
             assert x["finished"] == y["finished"], tag + ": finished"
             assert [float(v) for v in x["token_logprobs"]] == y["lps"], tag + ": token logprobs"
-    n = a.n_layers * a.n_embed
-    sa, sb = a.state_download(max_gpt), b.state_download(max_gpt)
-    named = {int(s) for slots, _ in groups for s in slots}
-    for slot in range(max_gpt):
-        for k in KEYS:
-            if slot in named:
-                assert np.array_equal(slot_of(sa, slot, n)[k], slot_of(sb, slot, n)[k]), what + ": slot %d state %s" % (slot, k)
-            else:
-                assert np.array_equal(slot_of(sa, slot, n)[k], slot_of(before, slot, n)[k]), what + ": slot %d was touched" % slot
+    check_slots(a, b, before, max_gpt, {int(s) for slots, _ in groups for s in slots}, keys=KEYS5, what=what)
 
 
 def make_groups(G, B, max_gpt, seed):
@@ -184,7 +152,7 @@ def test_bit_exact_against_the_host_loop(pkg, make_model, L, E, G, B, K, alpha, 
     host groups (max_new = 40)."""
     max_new = 40
     max_gpt = max(G * B + 2, max_new + 1)  # a spare slot pads the loop's lone rows, another scores whole texts
-    a, b = engines(pkg, make_model(L, E), max_gpt, tc)
+    a, b = engine_pair(pkg, make_model(L, E), max_gpt, tc, a_prefill_min=True)
     groups, spare = make_groups(G, B, max_gpt, seed=G * 10 + B)
     stop = []
     if with_stops:
@@ -200,7 +168,7 @@ def test_bit_exact_against_the_host_loop(pkg, make_model, L, E, G, B, K, alpha, 
         assert log["offers"], "no stop token was offered as a finished hypothesis"
     print("G=%d B=%d K=%d alpha=%g: finished offers at steps %s, groups done after steps %s"
           % (G, B, K, alpha, sorted(set(log["offers"])), log["done_at"]))
-    check(a, b, before, groups, got, want, max_gpt, "G=%d B=%d K=%d alpha=%g" % (G, B, K, alpha))
+    check_hypotheses(a, b, before, groups, got, want, max_gpt, "G=%d B=%d K=%d alpha=%g" % (G, B, K, alpha))
     # every hypothesis is what score_streams reports for its text from the prompt state
     n = a.n_layers * a.n_embed
     for (slots, first), hyps in zip(groups, got):
@@ -216,7 +184,7 @@ def test_one_beam_without_penalty_is_greedy_generation(pkg, make_model, L, E, tc
     does."""
     max_new, G = 40, 4
     max_gpt = G + 1
-    a, b = engines(pkg, make_model(L, E), max_gpt, tc)
+    a, b = engine_pair(pkg, make_model(L, E), max_gpt, tc, a_prefill_min=True)
     groups = [([s], t) for s, t in zip([3, 0, 2, 1], rand_tokens(G, 5))]
     streams = [(slots[0], t) for slots, t in groups]
     st = a.state_download(max_gpt)
@@ -230,11 +198,7 @@ def test_one_beam_without_penalty_is_greedy_generation(pkg, make_model, L, E, tc
     want = b.generate_streams(streams, max_new, stop=stop)
     assert [[int(t) for t in hs[0]["tokens"]] for hs in got] == [[int(t) for t in w] for w in want]
     assert [hs[0]["finished"] for hs in got] == [int(w[-1]) in stop for w in want]
-    n = a.n_layers * a.n_embed
-    sa, sb = a.state_download(max_gpt), b.state_download(max_gpt)
-    for slots, _ in groups:
-        for k in KEYS:
-            assert np.array_equal(slot_of(sa, slots[0], n)[k], slot_of(sb, slots[0], n)[k]), "slot %d %s" % (slots[0], k)
+    check_slots(a, b, st, max_gpt, {slots[0] for slots, _ in groups}, keys=KEYS5, untouched=())
     a.close()
     b.close()
 
@@ -243,7 +207,7 @@ def test_groups_are_independent(pkg, make_model):
     """A group's hypotheses are the same alone as among 32 other groups (both on the tensor cores)."""
     G, B, max_new = 33, 4, 24
     max_gpt = G * B
-    a, _ = engines(pkg, make_model(3, 768), max_gpt, tc=True)
+    a, _ = engine_pair(pkg, make_model(3, 768), max_gpt, tc=True, a_prefill_min=True)
     groups, _ = make_groups(G, B, max_gpt, seed=5)
     st = a.state_download(max_gpt)
     seen = a.beam_search(groups, max_new, B, stop=[0, 11], length_penalty=1.0, n_best=3, token_logprobs=True)

@@ -16,16 +16,11 @@ import time
 import numpy as np
 import pytest
 
-from util import INCLUDE, ROOT
+from util import INCLUDE, ROOT, SEED_TOKEN, rel_err
 
 pytestmark = pytest.mark.gpu
 
 REF_DIR = os.path.join(ROOT, "oracle", "_ref")
-SEED_TOKEN = 4118
-
-
-def rel_err(got, ref):
-    return float(np.abs(got.astype(np.float64) - ref.astype(np.float64)).max() / max(np.abs(ref).max(), 1e-6))
 
 
 def test_reference_header_runs_on_b200_hooks(pkg, make_model, tmp_path):

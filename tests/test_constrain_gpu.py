@@ -12,19 +12,10 @@ import re
 import numpy as np
 import pytest
 
-pytestmark = pytest.mark.gpu
+from decoding import (OVERRIDES, REGEXES, SHAPES, V, check_processed_rows, check_slots, engine_pair, host_decode,
+                      mixed_samplers, prefix_state, rand_tokens, regex_automata, replay_with_score, stops_at)
 
-V = 50277
-KEYS = ("xy", "aa", "bb", "dd")
-SHAPES = [(3, 768), (2, 2048)]
-FIELDS = ("logprobs", "ranks", "top_tokens", "top_logprobs")
-REGEXES = {
-    "date": r"\d{4}-\d{2}-\d{2}",
-    "labels": r"positive|negative|neutral",
-    "json": r'\{"name": "[a-z]{1,12}", "age": \d{1,3}\}',
-    "number": r"-?\d+(\.\d+)?",
-}
-OVERRIDES = {11: 3.0, 187: -99.0, 50: -np.inf}
+pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module")
@@ -38,140 +29,8 @@ def tbytes(C):
 
 
 @pytest.fixture(scope="module")
-def autos(C, tbytes):
-    return {k: C.token_automaton(C.compile_regex(p), tbytes, eos=0) for k, p in REGEXES.items()}
-
-
-_ALLOWED = {}
-
-
-def allowed(ta, q):
-    key = (id(ta), q)
-    if key not in _ALLOWED:
-        a = np.zeros(V, bool)
-        a[ta.edges(q)[0].astype(np.int64)] = True
-        _ALLOWED[key] = a
-    return _ALLOWED[key]
-
-
-def rand_tokens(n, seed):
-    return [int(x) for x in np.random.default_rng(seed).integers(0, V, size=n)]
-
-
-def slot_of(state, slot, n):
-    return {k: state[k][slot * n:(slot + 1) * n] for k in state}
-
-
-def engines(pkg, path, max_gpt, tc, seed=99):
-    """(a, b): a generates, b runs the host loop on the same forward path, both from the same non-trivial state."""
-    a = pkg.Engine(path, max_gpt=max_gpt)
-    b = pkg.Engine(path, max_gpt=max_gpt)
-    if tc:
-        b.set_option("prefill_min", 2)  # the loop's calls shrink below 8 streams as streams finish
-    else:
-        a.set_option("prefill", 0)
-        b.set_option("prefill", 0)
-    for i in range(0, max_gpt, 128):
-        n = min(128, max_gpt - i)
-        a.forward_streams([(i + j, [t]) for j, t in enumerate(rand_tokens(n, seed + i))], want_logits=False)
-    b.state_upload(a.state_download(max_gpt), max_gpt)
-    return a, b
-
-
-def check_slots(a, b, before, streams, max_gpt):
-    n = a.n_layers * a.n_embed
-    sa, sb = a.state_download(max_gpt), b.state_download(max_gpt)
-    named = {slot for slot, _ in streams}
-    for slot in range(max_gpt):
-        if slot in named:
-            for k in KEYS:
-                assert np.array_equal(slot_of(sa, slot, n)[k], slot_of(sb, slot, n)[k]), "slot %d state %s" % (slot, k)
-        else:
-            for k in ("xy", "aa", "bb", "pp", "dd"):
-                assert np.array_equal(slot_of(sa, slot, n)[k], slot_of(before, slot, n)[k]), "slot %d was touched" % slot
-
-
-def mixed_samplers(pkg, S):
-    """Greedy and sampled streams, penalties with decay < 1 and = 1, cuts by top-p and top-k."""
-    Sm = pkg.Sampler
-    kinds = [Sm(1.0, 0.85, 0, 0.2, 0.2, 0.996), Sm(0.0), Sm(0.8, 1.0, 40, 0.5, 0.0, 1.0), Sm(1.0, 0.85),
-             Sm(0.0, 1.0, 0, 1.0, 0.3, 0.9), Sm(1.2, 0.95, 100, 0.0, 0.4, 1.0), Sm(0.0, 1.0, 0, 0.3, 0.0, 1.0)]
-    return [kinds[s % len(kinds)] for s in range(S)]
-
-
-def host_loop(pkg, eng, streams, max_new, samplers, u, budgets, stop, overrides, cons, pad_slot=None, rows_out=None):
-    """The exact host loop; cons[s] = (automaton, start state) or None. Returns (tokens, final states). rows_out, when
-    given, receives every (stream, masked row) in step order."""
-    S = len(streams)
-    budgets = list(budgets) if budgets is not None else [max_new] * S
-    cnt = [np.zeros(V, np.float32) for _ in range(S)]
-    seen = [np.zeros(V, bool) for _ in range(S)]
-    pen = [sp.presence_penalty != 0 or sp.frequency_penalty != 0 for sp in samplers]
-    cur = [int(t) for _, t in streams]
-    state = [c[1] if c else None for c in cons]
-    out = [[] for _ in range(S)]
-    live = list(range(S))
-    for step in range(max_new):
-        if not live:
-            break
-        call = [(streams[s][0], [cur[s]]) for s in live]
-        if pad_slot is not None and len(call) == 1:
-            call.append((pad_slot, [cur[live[0]]]))
-        logits, _ = eng.forward_streams(call)
-        ps, us = [], []
-        for i, s in enumerate(live):
-            sp, row = samplers[s], logits[i]
-            if pen[s]:
-                k = seen[s]
-                row[k] = row[k] - (np.float32(sp.presence_penalty) + np.float32(sp.frequency_penalty) * cnt[s][k])
-            for tok, val in (overrides or {}).items():
-                row[tok] = val
-            if cons[s]:
-                row[~allowed(cons[s][0], state[s])] = -np.inf
-            if rows_out is not None:
-                rows_out.append((s, row.copy()))
-            ps.append(pkg.Sampler(sp.temperature, sp.top_p, sp.top_k))
-            us.append(float(u[step][s]) if u is not None else 0.0)
-        if len(call) > len(live):
-            ps.append(pkg.Sampler(0.0))
-            us.append(0.0)
-        toks, _ = eng.sample_streams(ps, us, logits=logits)
-        ended = set()
-        for i, s in enumerate(live):
-            x = int(toks[i])
-            out[s].append(x)
-            cur[s] = x
-            if pen[s]:
-                cnt[s] = cnt[s] * np.float32(samplers[s].penalty_decay)
-                cnt[s][x] += np.float32(1.0)
-                seen[s][x] = True
-            if cons[s]:
-                state[s] = cons[s][0].walk([x], state[s])
-                assert state[s] is not None, "the host loop picked a masked token"
-                if cons[s][0].complete(state[s]):
-                    ended.add(s)
-        live = [s for s in live if len(out[s]) < budgets[s] and out[s][-1] not in stop and s not in ended]
-    return out, state
-
-
-def stops_at(seqs, targets):
-    stop = []
-    for j, t in targets.items():
-        seq = seqs[j]
-        fresh = [i for i in range(t, len(seq)) if seq[i] not in seq[:i]]
-        if fresh:
-            stop.append(seq[fresh[0]])
-    return stop
-
-
-def prefix_state(ta, tbytes, text):
-    """The state after the shortest token spelling of `text` (one token per byte where needed)."""
-    ids = []
-    for ch in text.encode():
-        ids.append([t for t in range(2, V) if tbytes[t] == bytes([ch])][0])
-    q = ta.walk(ids)
-    assert q is not None
-    return q
+def autos(C):
+    return regex_automata(C)[0]
 
 
 # -- 1. bit for bit against the host loop ----------------------------------------------------------------------------
@@ -207,7 +66,7 @@ def ids_of(eng, autos, cons):
 
 
 def against_host_loop(pkg, make_model, autos, tbytes, L, E, S, max_gpt, max_new, tc, greedy_only=False):
-    a, b = engines(pkg, make_model(L, E), max_gpt, tc=tc)
+    a, b = engine_pair(pkg, make_model(L, E), max_gpt, tc=tc)
     streams = [(s, t) for s, t in zip([(7 * i + 2) % (max_gpt - 1) for i in range(S)], rand_tokens(S, 21))]  # pad: max_gpt - 1
     samplers = [pkg.Sampler(0.0)] * S if greedy_only else mixed_samplers(pkg, S)
     u = np.random.default_rng(22).random((max_new, S))
@@ -220,13 +79,13 @@ def against_host_loop(pkg, make_model, autos, tbytes, L, E, S, max_gpt, max_new,
     stop = stops_at([[int(x) for x in r["tokens"]] for r in first], {1: 9})  # a stop in an unconstrained stream
     got = a.generate_streams(streams, max_new, budgets=budgets, stop=stop, overrides=OVERRIDES, u=u, sampling=samplers,
                              constraints=ids)
-    want, states = host_loop(pkg, b, streams, max_new, samplers, u, budgets, stop, OVERRIDES, cons,
-                             pad_slot=max_gpt - 1 if tc else None)
+    want, states = host_decode(pkg, b, streams, max_new, samplers, u=u, budgets=budgets, stop=stop, overrides=OVERRIDES,
+                               constraints=cons, pad_slot=max_gpt - 1 if tc else None)
     assert [len(g["tokens"]) for g in got] == [len(w) for w in want], "lengths"
     for s, (g, w) in enumerate(zip(got, want)):
         assert [int(x) for x in g["tokens"]] == w, "tokens of stream %d" % s
         assert g["state"] == states[s], "state of stream %d" % s
-    check_slots(a, b, st, streams, max_gpt)
+    check_slots(a, b, st, max_gpt, {slot for slot, _ in streams})
     completed = [s for s in range(S) if cons[s] and cons[s][0].complete(states[s])]
     assert completed and any(len(want[s]) % 16 for s in completed), "no stream completed mid-group"
     a.close()
@@ -300,7 +159,7 @@ def test_no_side_effects(pkg, make_model, C, tc):
     that allows every token, are generate_streams_ex: the same tokens and slot states."""
     max_gpt, max_new = 12, 32
     S = 10 if tc else 3
-    a, b = engines(pkg, make_model(3, 768), max_gpt, tc=tc)
+    a, b = engine_pair(pkg, make_model(3, 768), max_gpt, tc=tc)
     streams = list(zip(range(S), rand_tokens(S, 31)))
     samplers = mixed_samplers(pkg, S)
     u = np.random.default_rng(32).random((max_new, S))
@@ -314,7 +173,7 @@ def test_no_side_effects(pkg, make_model, C, tc):
         for s, w in enumerate(want):
             assert np.array_equal(out[s, :len(w)], w) and not out[s, len(w):].any()
         assert not states.any()
-        check_slots(a, b, st, streams, max_gpt)
+        check_slots(a, b, st, max_gpt, {slot for slot, _ in streams})
     a.close()
     b.close()
 
@@ -355,15 +214,11 @@ def test_two_calls_continued_equal_one(pkg, make_model, autos):
 
 # -- 4. log-probabilities --------------------------------------------------------------------------------------------
 
-def bits(x):
-    return np.ascontiguousarray(x).tobytes()
-
-
 @pytest.mark.parametrize("tc", [False, True])
 def test_raw_logprobs_equal_score_streams(pkg, make_model, autos, tbytes, tc):
     max_gpt, max_new = 12, 32
     S = 10 if tc else 3
-    a, b = engines(pkg, make_model(3, 768), max_gpt, tc=tc)
+    a, b = engine_pair(pkg, make_model(3, 768), max_gpt, tc=tc)
     streams = list(zip([(5 * i + 2) % (max_gpt - 1) for i in range(S)], rand_tokens(S, 51)))
     samplers = mixed_samplers(pkg, S)
     u = np.random.default_rng(52).random((max_new, S))
@@ -371,48 +226,17 @@ def test_raw_logprobs_equal_score_streams(pkg, make_model, autos, tbytes, tc):
     st = a.state_download(max_gpt)
     got = a.generate_streams(streams, max_new, overrides=OVERRIDES, u=u, sampling=samplers, constraints=ids_of(a, autos, cons),
                              logprobs="raw", top_n=20)
-    pad = max_gpt - 1 if tc else None
-    cur = [t for _, t in streams]
-    lens = [len(g["tokens"]) for g in got]
-    for k in range(max(lens)):
-        live = [s for s in range(S) if lens[s] > k]
-        call = [(streams[s][0], [cur[s]]) for s in live]
-        tg = [[int(got[s]["tokens"][k])] for s in live]
-        if pad is not None and len(call) == 1:
-            call.append((pad, [cur[live[0]]]))
-            tg.append([None])
-        res = b.score_streams(call, tg, top_n=20)
-        for i, s in enumerate(live):
-            for f in FIELDS:
-                assert bits(res[i][f][0]) == bits(got[s][f][k]), (s, k, f)
-            cur[s] = int(got[s]["tokens"][k])
-    check_slots(a, b, st, streams, max_gpt)
+    replay_with_score(b, streams, got, 20, max_gpt - 1 if tc else None)
+    check_slots(a, b, st, max_gpt, {slot for slot, _ in streams})
     a.close()
     b.close()
-
-
-def rule(row, y, tau, top_n):
-    l = np.asarray(row, np.float32).astype(np.float64)
-    with np.errstate(invalid="ignore"):
-        z = (l - l.max()) / tau
-    log_s = np.log(np.exp(z).sum())
-    order = np.lexsort((np.arange(V), -l))
-    rank = int(np.nonzero(order == y)[0][0])
-    top = order[:top_n]
-    return z[y] - log_s, rank, top, z[top] - log_s
-
-
-def close(a, b):
-    a, b = np.asarray(a), np.asarray(b)
-    inf = np.isinf(b)
-    return np.array_equal(a[inf], b[inf]) and (not (~inf).any() or np.max(np.abs(a[~inf] - b[~inf])) <= 1e-9)
 
 
 @pytest.mark.parametrize("tc", [False, True])
 def test_processed_logprobs_on_the_masked_rows(pkg, make_model, autos, tbytes, tc):
     max_gpt, max_new, top_n = 12, 24, 20
     S = 9 if tc else 4
-    a, b = engines(pkg, make_model(2, 2048), max_gpt, tc=tc)
+    a, b = engine_pair(pkg, make_model(2, 2048), max_gpt, tc=tc)
     streams = list(zip([(3 * i + 1) % (max_gpt - 1) for i in range(S)], rand_tokens(S, 61)))
     samplers = mixed_samplers(pkg, S)
     u = np.random.default_rng(62).random((max_new, S))
@@ -421,23 +245,10 @@ def test_processed_logprobs_on_the_masked_rows(pkg, make_model, autos, tbytes, t
     got = a.generate_streams(streams, max_new, overrides=OVERRIDES, u=u, sampling=samplers,
                              constraints=ids_of(a, autos, cons), logprobs="processed", top_n=top_n)
     rows = []
-    want, _ = host_loop(pkg, b, streams, max_new, samplers, u, None, (), OVERRIDES, cons,
-                        pad_slot=max_gpt - 1 if tc else None, rows_out=rows)
+    want, _ = host_decode(pkg, b, streams, max_new, samplers, u=u, overrides=OVERRIDES, constraints=cons,
+                          pad_slot=max_gpt - 1 if tc else None, rows_out=rows)
     assert [[int(x) for x in g["tokens"]] for g in got] == want
-    k_of = [0] * S
-    masked_tops = 0
-    for s, row in rows:
-        k = k_of[s]
-        k_of[s] += 1
-        g, sp = got[s], samplers[s]
-        y = int(g["tokens"][k])
-        tau = float(np.float32(sp.temperature)) if sp.temperature > 0 else 1.0
-        lp, rank, top, top_lp = rule(row, y, tau, top_n)
-        assert int(g["ranks"][k]) == rank, (s, k)
-        assert abs(g["logprobs"][k] - lp) <= 1e-9, (s, k)
-        assert [int(x) for x in g["top_tokens"][k]] == [int(x) for x in top], (s, k)
-        assert close(g["top_logprobs"][k], top_lp), (s, k)
-        masked_tops += int(np.sum(g["top_logprobs"][k] == -np.inf))
+    masked_tops = check_processed_rows(got, rows, samplers, top_n)
     assert masked_tops > 0  # the labels' first states allow fewer than 20 tokens
     a.close()
     b.close()

@@ -13,57 +13,11 @@ import ctypes
 import numpy as np
 import pytest
 
+from decoding import (FIELDS, MIXED, NO_TARGET, SHAPES, V, bits, check_processed_rows, check_slots, engine_pair, host_decode,
+                      mixed_samplers, rand_tokens, replay_with_score, slot_of, stops_at)
+
 pytestmark = pytest.mark.gpu
-
-V = 50277
-KEYS = ("xy", "aa", "bb", "dd")
-SHAPES = [(3, 768), (2, 2048)]
-NO_TARGET = 2 ** 64 - 1
-FIELDS = ("logprobs", "ranks", "top_tokens", "top_logprobs")
-
-
-def rand_tokens(n, seed):
-    return [int(x) for x in np.random.default_rng(seed).integers(0, V, size=n)]
-
-
-def slot_of(state, slot, n):
-    return {k: state[k][slot * n:(slot + 1) * n] for k in state}
-
-
-def engines(pkg, path, max_gpt, tc, seed=99):
-    """(a, b) from the same non-trivial state on the same forward path; b replays calls that shrink below 8 streams."""
-    a = pkg.Engine(path, max_gpt=max_gpt)
-    b = pkg.Engine(path, max_gpt=max_gpt)
-    if tc:
-        b.set_option("prefill_min", 2)
-    else:
-        a.set_option("prefill", 0)
-        b.set_option("prefill", 0)
-    for i in range(0, max_gpt, 128):
-        n = min(128, max_gpt - i)
-        a.forward_streams([(i + j, [t]) for j, t in enumerate(rand_tokens(n, seed + i))], want_logits=False)
-    b.state_upload(a.state_download(max_gpt), max_gpt)
-    return a, b
-
-
-def mixed_samplers(pkg, S):
-    """Greedy and sampled streams, penalties with decay < 1 and = 1, cuts by top-p and top-k."""
-    Sm = pkg.Sampler
-    kinds = [Sm(1.0, 0.85, 0, 0.2, 0.2, 0.996), Sm(0.0), Sm(0.8, 1.0, 40, 0.5, 0.0, 1.0), Sm(1.0, 0.85),
-             Sm(0.0, 1.0, 0, 1.0, 0.3, 0.9), Sm(1.2, 0.95, 100, 0.0, 0.4, 1.0), Sm(0.0, 1.0, 0, 0.3, 0.0, 1.0),
-             Sm(0.6, 1.0, 5, 0.0, 0.0, 1.0)]
-    return [kinds[s % len(kinds)] for s in range(S)]
-
-
-def stops_at(seqs, targets):
-    """A stop token per stream j near step targets[j]: the first token there that the stream has not emitted before."""
-    stop = []
-    for j, t in targets.items():
-        seq = seqs[j]
-        fresh = [i for i in range(t, len(seq)) if seq[i] not in seq[:i]]
-        if fresh:
-            stop.append(seq[fresh[0]])
-    return stop
+KINDS = MIXED + [(0.6, 1.0, 5, 0.0, 0.0, 1.0)]  # and a temperature below 1 with a top-k cut
 
 
 def full_call(eng, streams, max_new, samplers=None, u=None, budgets=None, stop=(), overrides=None, mode=0, top_n=0,
@@ -91,24 +45,6 @@ def full_call(eng, streams, max_new, samplers=None, u=None, budgets=None, stop=(
     return rc, eng.lib.rwkv_b200_last_error().decode(), out, lens, o_lp, o_rank, o_tt[:, :, :top_n], o_tl[:, :, :top_n]
 
 
-def bits(x):
-    return np.ascontiguousarray(x).tobytes()
-
-
-def check_state(a, b, before, streams, max_gpt):
-    """Named slots equal on a and b; slots not named are where `before` left them on a."""
-    n = a.n_layers * a.n_embed
-    sa, sb = a.state_download(max_gpt), b.state_download(max_gpt)
-    named = {slot for slot, _ in streams}
-    for slot in range(max_gpt):
-        if slot in named:
-            for k in KEYS:
-                assert np.array_equal(slot_of(sa, slot, n)[k], slot_of(sb, slot, n)[k]), "slot %d state %s" % (slot, k)
-        else:
-            for k in ("xy", "aa", "bb", "pp", "dd"):
-                assert np.array_equal(slot_of(sa, slot, n)[k], slot_of(before, slot, n)[k]), "slot %d was touched" % slot
-
-
 def check_tail(lens, lp, rank, tt, tl):
     """Entries at or beyond each length: NaN and NO_TARGET; entries inside: finite logprob, a real rank."""
     for s, n in enumerate(int(x) for x in lens):
@@ -120,10 +56,10 @@ def check_tail(lens, lp, rank, tt, tl):
 # -- 1. nothing changes when log-probabilities are asked for ---------------------------------------------------------
 
 def unchanged_case(pkg, path, max_gpt, S, max_new, tc, budgets, stop_targets, top_n):
-    a, b = engines(pkg, path, max_gpt, tc=tc)
+    a, b = engine_pair(pkg, path, max_gpt, tc=tc)
     perm = [int(x) for x in np.random.default_rng(S).permutation(max_gpt)]
     streams = list(zip(perm[:S], rand_tokens(S, 7 + S)))
-    samplers = mixed_samplers(pkg, S)
+    samplers = mixed_samplers(pkg, S, KINDS)
     u = np.random.default_rng(22 + S).random((max_new, S))
     overrides = {0: -np.inf, 11: 3.0, 187: -99.0}
     st = a.state_download(max_gpt)
@@ -139,7 +75,7 @@ def unchanged_case(pkg, path, max_gpt, S, max_new, tc, budgets, stop_targets, to
         for g, w in zip(got, want):
             assert bits(g["tokens"]) == bits(w), mode
             assert np.all(np.isfinite(g["logprobs"])) and np.all(g["ranks"] < V)
-        check_state(a, b, st, streams, max_gpt)
+        check_slots(a, b, st, max_gpt, {slot for slot, _ in streams})
     a.close()
     b.close()
 
@@ -162,24 +98,6 @@ def test_unchanged_150_streams(pkg, make_model):
 
 # -- 2. raw mode is score_streams, bit for bit -----------------------------------------------------------------------
 
-def replay_with_score(b, streams, got, top_n, pad_slot):
-    """Per step one score_streams call on b: every live stream's current token, its emitted token as target."""
-    cur = [t for _, t in streams]
-    lens = [len(g["tokens"]) for g in got]
-    for k in range(max(lens)):
-        live = [s for s in range(len(streams)) if lens[s] > k]
-        call = [(streams[s][0], [cur[s]]) for s in live]
-        tg = [[int(got[s]["tokens"][k])] for s in live]
-        if pad_slot is not None and len(call) == 1:  # one token alone would take the decode kernel
-            call.append((pad_slot, [cur[live[0]]]))
-            tg.append([None])
-        res = b.score_streams(call, tg, top_n=top_n)
-        for i, s in enumerate(live):
-            for f in FIELDS:
-                assert bits(res[i][f][0]) == bits(got[s][f][k]), (s, k, f)
-            cur[s] = int(got[s]["tokens"][k])
-
-
 @pytest.mark.parametrize("L,E", SHAPES)
 @pytest.mark.parametrize("tc", [False, True])
 def test_raw_equals_score_streams(pkg, make_model, L, E, tc):
@@ -187,9 +105,9 @@ def test_raw_equals_score_streams(pkg, make_model, L, E, tc):
     max_gpt, max_new = 12, 32
     S = 10 if tc else 3
     path = make_model(L, E)
-    a, b = engines(pkg, path, max_gpt, tc=tc)
+    a, b = engine_pair(pkg, path, max_gpt, tc=tc)
     streams = list(zip([(5 * i + 2) % (max_gpt - 1) for i in range(S)], rand_tokens(S, 21)))
-    samplers = mixed_samplers(pkg, S)
+    samplers = mixed_samplers(pkg, S, KINDS)
     u = np.random.default_rng(23).random((max_new, S))
     overrides = {0: -np.inf, 11: 3.0, 187: -99.0}
     budgets = [max_new - (5 * i) % 23 for i in range(S)]
@@ -197,7 +115,7 @@ def test_raw_equals_score_streams(pkg, make_model, L, E, tc):
     got = a.generate_streams(streams, max_new, budgets=budgets, overrides=overrides, u=u, sampling=samplers,
                              logprobs="raw", top_n=20)
     replay_with_score(b, streams, got, 20, max_gpt - 1 if tc else None)
-    check_state(a, b, st, streams, max_gpt)
+    check_slots(a, b, st, max_gpt, {slot for slot, _ in streams})
     if tc:
         # each whole emitted text in one score_streams call from the stream's starting state, on slot 0 of an engine
         # that takes max_new tokens in one call
@@ -221,65 +139,24 @@ def test_raw_equals_score_streams(pkg, make_model, L, E, tc):
 
 # -- 3. processed mode against the rule ------------------------------------------------------------------------------
 
-def rule(row, y, tau, top_n):
-    l = np.asarray(row, np.float32).astype(np.float64)
-    z = (l - l.max()) / tau
-    log_s = np.log(np.exp(z).sum())
-    order = np.lexsort((np.arange(V), -l))
-    rank = int(np.nonzero(order == y)[0][0])
-    top = order[:top_n]
-    return z[y] - log_s, rank, top, z[top] - log_s
-
-
-def close(a, b):
-    a, b = np.asarray(a), np.asarray(b)
-    inf = np.isinf(b)
-    return np.array_equal(a[inf], b[inf]) and (not (~inf).any() or np.max(np.abs(a[~inf] - b[~inf])) <= 1e-9)
-
-
 @pytest.mark.parametrize("L,E", SHAPES)
 @pytest.mark.parametrize("tc", [False, True])
 def test_processed_against_the_rule(pkg, make_model, L, E, tc):
     max_gpt, max_new, top_n = 12, 24, 8
     S = 9 if tc else 4
-    a, b = engines(pkg, make_model(L, E), max_gpt, tc=tc)
+    a, b = engine_pair(pkg, make_model(L, E), max_gpt, tc=tc)
     streams = list(zip([(3 * i + 1) % (max_gpt - 1) for i in range(S)], rand_tokens(S, 41)))
-    samplers = mixed_samplers(pkg, S)
+    samplers = mixed_samplers(pkg, S, KINDS)
     u = np.random.default_rng(42).random((max_new, S))
     overrides = {0: -np.inf, 11: 3.0, 187: -99.0}
     budgets = [max_new - (7 * i) % 19 for i in range(S)]
     got = a.generate_streams(streams, max_new, budgets=budgets, overrides=overrides, u=u, sampling=samplers,
                              logprobs="processed", top_n=top_n)
-    # the host loop, teacher-forced with the emitted tokens: forward_streams logits, f32 penalties, overrides
-    cnt = [np.zeros(V, np.float32) for _ in range(S)]
-    seen = [np.zeros(V, bool) for _ in range(S)]
-    cur = [t for _, t in streams]
-    lens = [len(g["tokens"]) for g in got]
-    for k in range(max(lens)):
-        live = [s for s in range(S) if lens[s] > k]
-        call = [(streams[s][0], [cur[s]]) for s in live]
-        if tc and len(call) == 1:
-            call.append((max_gpt - 1, [cur[live[0]]]))
-        logits, _ = b.forward_streams(call)
-        for i, s in enumerate(live):
-            sp, row = samplers[s], logits[i]
-            if sp.presence_penalty != 0 or sp.frequency_penalty != 0:
-                m = seen[s]
-                row[m] = row[m] - (np.float32(sp.presence_penalty) + np.float32(sp.frequency_penalty) * cnt[s][m])
-            for tok, val in overrides.items():
-                row[tok] = val
-            y = int(got[s]["tokens"][k])
-            tau = float(np.float32(sp.temperature)) if sp.temperature > 0 else 1.0
-            lp, rank, top, top_lp = rule(row, y, tau, top_n)
-            assert int(got[s]["ranks"][k]) == rank, (s, k)
-            assert abs(got[s]["logprobs"][k] - lp) <= 1e-9, (s, k, got[s]["logprobs"][k], lp)
-            assert [int(x) for x in got[s]["top_tokens"][k]] == [int(x) for x in top], (s, k)
-            assert close(got[s]["top_logprobs"][k], top_lp), (s, k)
-            if sp.presence_penalty != 0 or sp.frequency_penalty != 0:
-                cnt[s] = cnt[s] * np.float32(sp.penalty_decay)
-                cnt[s][y] += np.float32(1.0)
-                seen[s][y] = True
-            cur[s] = y
+    rows = []
+    want, _ = host_decode(pkg, b, streams, max_new, samplers, u=u, budgets=budgets, overrides=overrides,
+                          pad_slot=max_gpt - 1 if tc else None, rows_out=rows)
+    assert [[int(x) for x in g["tokens"]] for g in got] == want
+    check_processed_rows(got, rows, samplers, top_n)
     a.close()
     b.close()
 
@@ -315,7 +192,7 @@ def test_consistency(pkg, make_model, L, E):
     max_gpt, max_new, S = 16, 24, 14
     a = pkg.Engine(make_model(L, E), max_gpt=max_gpt)
     streams = list(zip(range(S), rand_tokens(S, 61)))
-    samplers = mixed_samplers(pkg, S)
+    samplers = mixed_samplers(pkg, S, KINDS)
     u = np.random.default_rng(62).random((max_new, S))
     st = a.state_download(max_gpt)
     got = a.generate_streams(streams, max_new, u=u, sampling=samplers, overrides={0: -np.inf, 11: 3.0},
@@ -360,7 +237,7 @@ def test_boundaries(pkg, make_model, tc):
     nor into its neighbour's first entry."""
     max_gpt, max_new = 12, 32
     S = 9 if tc else 4
-    a, b = engines(pkg, make_model(3, 768), max_gpt, tc=tc)
+    a, b = engine_pair(pkg, make_model(3, 768), max_gpt, tc=tc)
     streams = list(zip(range(S), rand_tokens(S, 71)))
     samplers = [pkg.Sampler(0.0)] * S
     budgets = [32, 5, 21, 32, 1, 16, 30, 17, 32][:S]
@@ -381,7 +258,7 @@ def test_boundaries(pkg, make_model, tc):
     got = [{"tokens": out[s, :int(lens[s])], "logprobs": lp[s, :int(lens[s])], "ranks": rank[s, :int(lens[s])],
             "top_tokens": tt[s, :int(lens[s])], "top_logprobs": tl[s, :int(lens[s])]} for s in range(S)]
     replay_with_score(b, streams, got, 3, max_gpt - 1 if tc else None)
-    check_state(a, b, before, streams, max_gpt)
+    check_slots(a, b, before, max_gpt, {slot for slot, _ in streams})
     a.close()
     b.close()
 

@@ -13,16 +13,9 @@ import sys
 import numpy as np
 import pytest
 
-from util import ROOT, golden_logits_err, golden_state_err, reference_golden, stress_model
+from util import REL_TOL, ROOT, SEED_TOKEN, golden_logits_err, golden_state_err, reference_golden, rel_err, stress_model
 
 pytestmark = pytest.mark.gpu
-
-REL_TOL = 1e-3
-SEED_TOKEN = 4118
-
-
-def rel_err(got, ref):
-    return float(np.abs(got.astype(np.float64) - ref.astype(np.float64)).max() / max(np.abs(ref).max(), 1e-6))
 
 
 def compare_with_reference(pkg, path, name, n_tokens):

@@ -16,11 +16,9 @@ import ctypes
 import numpy as np
 import pytest
 
-pytestmark = pytest.mark.gpu
+from decoding import SHAPES, V, check_generated, engine_pair, host_decode, mixed_samplers, rand_tokens, stops_at
 
-V = 50277
-KEYS = ("xy", "aa", "bb", "dd")
-SHAPES = [(3, 768), (2, 2048)]
+pytestmark = pytest.mark.gpu
 
 
 def rule(l, sp, u):
@@ -138,114 +136,20 @@ def test_deterministic_and_same_bits_from_host_logits(pkg, make_model, L, E):
 
 # -- generation ------------------------------------------------------------------------------------------------------
 
-def rand_tokens(n, seed):
-    return [int(x) for x in np.random.default_rng(seed).integers(0, V, size=n)]
-
-
-def slot_of(state, slot, n):
-    return {k: state[k][slot * n:(slot + 1) * n] for k in state}
-
-
-def engines(pkg, path, max_gpt, tc, seed=99):
-    """(a, b): a generates, b runs the host loop on the same forward path, both from the same non-trivial state."""
-    a = pkg.Engine(path, max_gpt=max_gpt)
-    b = pkg.Engine(path, max_gpt=max_gpt)
-    if tc:
-        b.set_option("prefill_min", 2)  # the loop's calls shrink below 8 streams as streams finish
-    else:
-        a.set_option("prefill", 0)
-        b.set_option("prefill", 0)
-    for i in range(0, max_gpt, 128):
-        n = min(128, max_gpt - i)
-        a.forward_streams([(i + j, [t]) for j, t in enumerate(rand_tokens(n, seed + i))], want_logits=False)
-    b.state_upload(a.state_download(max_gpt), max_gpt)
-    return a, b
-
-
-def check(a, b, before, streams, got, want, max_gpt):
-    n = a.n_layers * a.n_embed
-    assert [len(x) for x in got] == [len(x) for x in want], "lengths"
-    for s, (g, w) in enumerate(zip(got, want)):
-        assert [int(x) for x in g] == [int(x) for x in w], "tokens of stream %d" % s
-    sa, sb = a.state_download(max_gpt), b.state_download(max_gpt)
-    named = {slot for slot, _ in streams}
-    for slot in range(max_gpt):
-        if slot in named:
-            for k in KEYS:
-                assert np.array_equal(slot_of(sa, slot, n)[k], slot_of(sb, slot, n)[k]), "slot %d state %s" % (slot, k)
-        else:
-            for k in ("xy", "aa", "bb", "pp", "dd"):
-                assert np.array_equal(slot_of(sa, slot, n)[k], slot_of(before, slot, n)[k]), "slot %d was touched" % slot
-
-
-def host_loop(pkg, eng, streams, max_new, samplers, u=None, budgets=None, stop=(), overrides=None, pad_slot=None):
-    """forward_streams logits, float32 penalties, overrides, sample_streams(logits=...) with the same u, append, stop."""
-    S = len(streams)
-    budgets = list(budgets) if budgets is not None else [max_new] * S
-    cnt = [np.zeros(V, np.float32) for _ in range(S)]
-    seen = [np.zeros(V, bool) for _ in range(S)]
-    pen = [sp.presence_penalty != 0 or sp.frequency_penalty != 0 for sp in samplers]
-    cur = [int(t) for _, t in streams]
-    out = [[] for _ in range(S)]
-    live = list(range(S))
-    for step in range(max_new):
-        if not live:
-            break
-        call = [(streams[s][0], [cur[s]]) for s in live]
-        if pad_slot is not None and len(call) == 1:
-            call.append((pad_slot, [cur[live[0]]]))
-        logits, _ = eng.forward_streams(call)
-        ps, us = [], []
-        for i, s in enumerate(live):
-            sp, row = samplers[s], logits[i]
-            if pen[s]:
-                k = seen[s]
-                row[k] = row[k] - (np.float32(sp.presence_penalty) + np.float32(sp.frequency_penalty) * cnt[s][k])
-            for tok, val in (overrides or {}).items():
-                row[tok] = val
-            ps.append(pkg.Sampler(sp.temperature, sp.top_p, sp.top_k))
-            us.append(float(u[step][s]) if u is not None else 0.0)
-        if len(call) > len(live):
-            ps.append(pkg.Sampler(0.0))
-            us.append(0.0)
-        toks, _ = eng.sample_streams(ps, us, logits=logits)
-        for i, s in enumerate(live):
-            x = int(toks[i])
-            out[s].append(x)
-            cur[s] = x
-            if pen[s]:
-                cnt[s] = cnt[s] * np.float32(samplers[s].penalty_decay)
-                cnt[s][x] += np.float32(1.0)
-                seen[s][x] = True
-        live = [s for s in live if len(out[s]) < budgets[s] and out[s][-1] not in stop]
-    return out
-
-
-def stops_at(seqs, targets):
-    """A stop token per stream j near step targets[j]: the first token there that the stream has not emitted before."""
-    stop = []
-    for j, t in targets.items():
-        seq = seqs[j]
-        fresh = [i for i in range(t, len(seq)) if seq[i] not in seq[:i]]
-        alone = [i for i in fresh if all(seq[i] not in other for k, other in enumerate(seqs) if k != j)]
-        if alone or fresh:
-            stop.append(seq[(alone or fresh)[0]])
-    return stop
-
-
 def greedy_case(pkg, make_model, L, E, max_gpt, S, max_new, tc, stop_targets=None, budgets=None):
-    a, b = engines(pkg, make_model(L, E), max_gpt, tc=tc)
+    a, b = engine_pair(pkg, make_model(L, E), max_gpt, tc=tc)
     perm = [int(x) for x in np.random.default_rng(S).permutation(max_gpt)]
     streams = [(s, t) for s, t in zip(perm[:S], rand_tokens(S, 7 + S))]
     stop = []
     if stop_targets:
         st = a.state_download(max_gpt)
-        stop = stops_at([[int(x) for x in q] for q in a.generate_streams(streams, max_new)], stop_targets)
+        stop = stops_at([[int(x) for x in q] for q in a.generate_streams(streams, max_new)], stop_targets,
+                        prefer_unique=True)
         a.state_upload(st, max_gpt)
     before = a.state_download(max_gpt)
     got = a.generate_streams(streams, max_new, budgets=budgets, stop=stop, sampling=pkg.Sampler(0.0, 0.5, 3))
     want = b.generate_streams(streams, max_new, budgets=budgets, stop=stop)
-    check(a, b, before, streams, got, want, max_gpt)
+    check_generated(a, b, before, streams, got, want, max_gpt)
     a.close()
     b.close()
 
@@ -266,21 +170,13 @@ def test_greedy_generation_150_streams(pkg, make_model):
     greedy_case(pkg, make_model, 3, 768, max_gpt=256, S=150, max_new=20, tc=True, budgets=budgets)
 
 
-def mixed_samplers(pkg, S):
-    """Greedy and sampled streams, penalties with decay < 1 and = 1, cuts by top-p and top-k."""
-    Sm = pkg.Sampler
-    kinds = [Sm(1.0, 0.85, 0, 0.2, 0.2, 0.996), Sm(0.0), Sm(0.8, 1.0, 40, 0.5, 0.0, 1.0), Sm(1.0, 0.85),
-             Sm(0.0, 1.0, 0, 1.0, 0.3, 0.9), Sm(1.2, 0.95, 100, 0.0, 0.4, 1.0), Sm(0.0, 1.0, 0, 0.3, 0.0, 1.0)]
-    return [kinds[s % len(kinds)] for s in range(S)]
-
-
 @pytest.mark.parametrize("L,E", SHAPES)
 @pytest.mark.parametrize("S", [3, 10])
 def test_sampled_generation_against_the_host_loop(pkg, make_model, L, E, S):
     """S = 3 on the decode kernel, S = 10 on the tensor cores; per-stream samplers, overrides, stops and budgets."""
     max_gpt, max_new = 12, 40
     tc = S >= 8
-    a, b = engines(pkg, make_model(L, E), max_gpt, tc=tc)
+    a, b = engine_pair(pkg, make_model(L, E), max_gpt, tc=tc)
     streams = [(s, t) for s, t in zip([(5 * i + 2) % (max_gpt - 1) for i in range(S)], rand_tokens(S, 21))]  # max_gpt - 1: pad
     samplers = mixed_samplers(pkg, S)
     u = np.random.default_rng(22).random((max_new, S))
@@ -289,14 +185,14 @@ def test_sampled_generation_against_the_host_loop(pkg, make_model, L, E, S):
     st = a.state_download(max_gpt)
     seqs = [[int(x) for x in q] for q in a.generate_streams(streams, max_new, overrides=overrides, u=u, sampling=samplers)]
     a.state_upload(st, max_gpt)
-    stop = stops_at(seqs, {0: 9, S - 1: 25})
+    stop = stops_at(seqs, {0: 9, S - 1: 25}, prefer_unique=True)
     before = a.state_download(max_gpt)
     got = a.generate_streams(streams, max_new, budgets=budgets, stop=stop, overrides=overrides, u=u, sampling=samplers)
-    want = host_loop(pkg, b, streams, max_new, samplers, u=u, budgets=budgets, stop=stop, overrides=overrides,
-                     pad_slot=max_gpt - 1 if tc else None)
+    want, _ = host_decode(pkg, b, streams, max_new, samplers, u=u, budgets=budgets, stop=stop, overrides=overrides,
+                          pad_slot=max_gpt - 1 if tc else None)
     assert len({len(w) for w in want}) >= 2
     assert all(0 not in w for w in want)
-    check(a, b, before, streams, got, want, max_gpt)
+    check_generated(a, b, before, streams, got, want, max_gpt)
     a.close()
     b.close()
 

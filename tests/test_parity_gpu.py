@@ -8,49 +8,10 @@ of max-abs (SURVEY.md H5: below that the reference's fp32 atomics decide the win
 import numpy as np
 import pytest
 
+from decoding import run_pair
+from util import REL_TOL, SEED_TOKEN
+
 pytestmark = pytest.mark.gpu
-
-REL_TOL = 1e-3
-SEED_TOKEN = 4118  # "###", first token of the storygen prompt
-
-
-def make_engine(pkg, path, **kw):
-    return pkg.Engine(path, **kw)
-
-
-def rel_err(got, ref):
-    return float(np.abs(got.astype(np.float64) - ref.astype(np.float64)).max() / max(np.abs(ref).max(), 1e-6))
-
-
-def margin(ref):
-    top = np.partition(ref, -2)[-2:]
-    return float((top.max() - top.min()) / max(np.abs(ref).max(), 1e-6))
-
-
-def run_pair(pkg, path, steps, threads=None):
-    from oracle.oracle import Oracle
-    eng = make_engine(pkg, path)
-    orc = Oracle(path, threads=threads)
-    tok, worst, checked_argmax = SEED_TOKEN, 0.0, 0
-    for step in range(steps):
-        got = eng.forward([tok])[0]
-        ref = orc.forward(tok)
-        e = rel_err(got, ref)
-        worst = max(worst, e)
-        assert e < REL_TOL, "step %d: logits rel err %.3g" % (step, e)
-        if margin(ref) > 1e-3:
-            assert int(got.argmax()) == int(ref.argmax()), "step %d argmax" % step
-            checked_argmax += 1
-        tok = int(ref.argmax())  # teacher forcing on the oracle's greedy stream
-    st = eng.state_download()
-    for k in ("xy", "aa", "bb", "dd"):
-        ref = orc.state[k]
-        scale = max(np.abs(ref).max(), 1e-6)
-        assert np.abs(st[k] - ref).max() / scale < REL_TOL, "state %s" % k
-    assert np.all(st["pp"] == 0.0)
-    eng.close()
-    orc.close()
-    return worst, checked_argmax
 
 
 @pytest.mark.parametrize("L,E,steps", [
@@ -105,7 +66,7 @@ def test_deterministic_across_runs(pkg, make_model):
 
 def test_forward_greedy_matches_host_argmax(pkg, make_model):
     path = make_model(2, 2048)
-    e = make_engine(pkg, path)
+    e = pkg.Engine(path)
     tok = SEED_TOKEN
     for _ in range(6):
         nxt, lg = e.forward_greedy(tok, want_logits=True)

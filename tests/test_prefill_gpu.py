@@ -5,24 +5,15 @@ quantise the same numbers and accumulate exactly; they differ only in the order 
 import numpy as np
 import pytest
 
+from util import rel_err, token_stream
+
 pytestmark = pytest.mark.gpu
-
-SEED_TOKEN = 4118
-
-
-def rel_err(got, ref):
-    return float(np.abs(got.astype(np.float64) - ref.astype(np.float64)).max() / max(np.abs(ref).max(), 1e-6))
-
-
-def token_stream(n, seed=3):
-    rng = np.random.default_rng(seed)
-    return [SEED_TOKEN] + [int(x) for x in rng.integers(0, 50277, size=n - 1)]
 
 
 @pytest.mark.parametrize("L,E,T", [(3, 768, 16), (2, 2048, 40), (2, 4096, 16), (2, 4096, 64), (2, 4096, 128), (1, 5120, 32)])
 def test_gpt_chunk_on_tensor_cores_matches_decode_kernel(pkg, make_model, L, E, T):
     path = make_model(L, E)
-    toks = token_stream(T)
+    toks = token_stream(T, seed=3)
     a = pkg.Engine(path, max_gpt=T)
     chunk = a.forward(toks, mode=1)          # >= 16 tokens: the batched path
     sa = a.state_download()
@@ -86,7 +77,7 @@ def test_prefill_throughput_reported(pkg, make_model):
     import time
     path = make_model(2, 4096)
     T = 128
-    toks = token_stream(T)
+    toks = token_stream(T, seed=3)
     a = pkg.Engine(path, max_gpt=T)
     a.forward(toks, mode=1, want_logits=False)
     t0 = time.perf_counter()

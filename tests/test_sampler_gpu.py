@@ -6,20 +6,10 @@ import subprocess
 import numpy as np
 import pytest
 
+from decoding import host_pick
 from util import ROOT, compile_cpp
 
 pytestmark = pytest.mark.gpu
-
-
-def host_pick(logits, temp, u):
-    """include/rwkv/sampler/typical.h restated in numpy (float64, sequential cumulative sum)."""
-    p = np.exp(logits.astype(np.float64))
-    p /= p.sum()
-    e = int(np.uint8(int(1.0 / temp))) if temp != 1.0 else 1
-    p = np.ones_like(p) if e == 0 else p ** e
-    cp = np.cumsum(p / p.sum())
-    cp[-1] = 1.0
-    return int(np.searchsorted(cp, u, side="left")), cp
 
 
 @pytest.mark.parametrize("temp", [0.9, 0.5, 1.0, 0.3, 2.0])

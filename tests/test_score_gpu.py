@@ -12,23 +12,9 @@ import shutil
 import numpy as np
 import pytest
 
+from decoding import KEYS4, SHAPES, V, logprob_rule
+
 pytestmark = pytest.mark.gpu
-
-V = 50277
-KEYS = ("xy", "aa", "bb", "dd")
-SHAPES = [(3, 768), (2, 2048)]
-
-
-def rule(row, y, top_n):
-    """(logprob, rank, top tokens, top logprobs) of target y on one f32 logits row."""
-    l = np.asarray(row, np.float32).astype(np.float64)
-    m = l.max()
-    log_s = np.log(np.exp(l - m).sum())
-    order = np.lexsort((np.arange(V), -l))
-    lp = lambda v: (l[v] - m) - log_s
-    rank = int(np.nonzero(order == y)[0][0])
-    top = order[:top_n]
-    return lp(y), rank, top, np.array([lp(v) for v in top])
 
 
 def alone_logits(ref, state, seq, tc):
@@ -48,7 +34,7 @@ def check_against_rule(res, logits, targets, top_n):
             if top_n:
                 assert np.all(res["top_tokens"][t] == np.uint64(2 ** 64 - 1)) and np.all(np.isnan(res["top_logprobs"][t]))
             continue
-        lp, rank, top, top_lp = rule(logits[t], y, top_n)
+        lp, rank, top, top_lp = logprob_rule(logits[t], y, top_n)
         assert int(res["ranks"][t]) == rank, (t, y)
         assert abs(res["logprobs"][t] - lp) <= 1e-9, (t, res["logprobs"][t], lp)
         if top_n:
@@ -70,7 +56,7 @@ def all_states(eng):
 
 
 def same_state(a, b):
-    return all(np.array_equal(a[k], b[k]) for k in KEYS)
+    return all(np.array_equal(a[k], b[k]) for k in KEYS4)
 
 
 @pytest.mark.parametrize("L,E", SHAPES)
@@ -231,7 +217,7 @@ def test_state_slots_and_chunks(pkg, make_model, L, E):
     n = eng.n_layers * eng.n_embed
     for s in range(eng.max_gpt):
         if s not in slots:
-            assert all(np.array_equal(after_score[k][s * n:(s + 1) * n], before[k][s * n:(s + 1) * n]) for k in KEYS), s
+            assert all(np.array_equal(after_score[k][s * n:(s + 1) * n], before[k][s * n:(s + 1) * n]) for k in KEYS4), s
     # the 150-token stream across the pass boundary scores as it does alone
     eng.state_upload(before, eng.max_gpt)
     alone = eng.score_streams([streams[0]], [tg[0]], top_n=5)[0]

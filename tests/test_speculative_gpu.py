@@ -2,7 +2,7 @@
 
 The oracle is a second engine with prefill_min = 2, started from the same state of every slot, which runs
 generate_streams(sampling=...) on the streams' first slots with the same first tokens, budgets, stops, overrides,
-samplers and uniforms (a lone stream gets a pad stream on a slot nobody names, as in test_batcher_gpu.py). Tokens,
+samplers and uniforms (a lone stream gets a pad stream on a slot nobody names, as the batcher's oracle does). Tokens,
 lengths and every first slot's five state arrays must be bit-equal to the oracle's (pp: untouched), every slot no stream
 names must be unchanged, and steps_out must equal the host restatement of the draft rule (engine.speculative_steps)."""
 import importlib
@@ -10,29 +10,20 @@ import importlib
 import numpy as np
 import pytest
 
+from decoding import KEYS5, SHAPES, V, check_slots, engine_pair, slot_of
+
 pytestmark = pytest.mark.gpu
 
 eng_mod = importlib.import_module("rwkv-cpp-accelerated_b200.engine")
 
-V = 50277
-KEYS = ("xy", "aa", "bb", "pp", "dd")
-SHAPES = [(3, 768), (2, 2048)]
 MAX_GPT = 160      # S = 9 streams with k = 15 name 144 slots
 PAD = MAX_GPT - 1  # the oracle's pad stream; never named by a speculative stream
-
-
-def slot_of(state, slot, n):
-    return {k: state[k][slot * n:(slot + 1) * n] for k in state}
 
 
 @pytest.fixture(scope="module", params=SHAPES, ids=["3x768", "2x2048"])
 def setup(request, pkg, make_model):
     L, E = request.param
-    a = pkg.Engine(make_model(L, E), max_gpt=MAX_GPT)
-    b = pkg.Engine(make_model(L, E), max_gpt=MAX_GPT)
-    b.set_option("prefill_min", 2)
-    rng = np.random.default_rng(5)
-    a.forward_streams([(j, [int(rng.integers(0, V))]) for j in range(MAX_GPT)], want_logits=False)
+    a, b = engine_pair(pkg, make_model(L, E), MAX_GPT, tc=True, seed=5, one_draw=True)
     before = a.state_download(MAX_GPT)
     yield pkg, a, b, before
     a.close()
@@ -110,20 +101,12 @@ def run_case(setup, S, k, max_new, seed, ctx_kind="none", ngram=3, sampling=None
         assert got[s]["steps"] == len(counts) == eng_mod.speculative_steps(ctx, firsts[s][1], toks, k, ngram), \
             "stream %d: steps" % s
         homes.append(sum(c - 1 for c in counts) % (k + 1))
+    first_slots = {sl[0] for sl in slot_lists}
+    spares = {s for sl in slot_lists for s in sl[1:]}
+    sa = check_slots(a, b, before, MAX_GPT, first_slots, keys=KEYS5, skip=spares)
     n = a.n_layers * a.n_embed
-    sa, sb = a.state_download(MAX_GPT), b.state_download(MAX_GPT)
-    named = {s for sl in slot_lists for s in sl}
-    for s in range(S):
-        first = slot_lists[s][0]
-        for key in KEYS:
-            assert np.array_equal(slot_of(sa, first, n)[key], slot_of(sb, first, n)[key]), \
-                "stream %d: first slot %d state %s" % (s, first, key)
-        assert np.array_equal(slot_of(sa, first, n)["pp"], slot_of(before, first, n)["pp"])
-    for slot in range(MAX_GPT):
-        if slot not in named:
-            for key in KEYS:
-                assert np.array_equal(slot_of(sa, slot, n)[key], slot_of(before, slot, n)[key]), \
-                    "unnamed slot %d state %s changed" % (slot, key)
+    for first in first_slots:
+        assert np.array_equal(slot_of(sa, first, n)["pp"], slot_of(before, first, n)["pp"]), "first slot %d: pp" % first
     return got, homes
 
 
@@ -212,5 +195,5 @@ def test_refusals(setup):
             a.generate_speculative(two, 8, 3)
     finally:
         a.set_option("prefill", 1)
-    assert all(np.array_equal(x, y) for x, y in ((a.state_download(MAX_GPT)[k], before[k]) for k in KEYS)), \
+    assert all(np.array_equal(x, y) for x, y in ((a.state_download(MAX_GPT)[k], before[k]) for k in KEYS5)), \
         "a refused call changed a slot"

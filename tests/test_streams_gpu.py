@@ -10,68 +10,10 @@ import time
 import numpy as np
 import pytest
 
-from test_sampler_gpu import host_pick
+from decoding import KEYS4, KEYS5, check_against_solo, host_pick, rand_tokens, run_ragged_vs_solo, slot_of, solo
+from util import rel_err
 
 pytestmark = pytest.mark.gpu
-
-V = 50277
-KEYS = ("xy", "aa", "bb", "dd")
-
-
-def rel_err(got, ref):
-    return float(np.abs(got.astype(np.float64) - ref.astype(np.float64)).max() / max(np.abs(ref).max(), 1e-6))
-
-
-def rand_tokens(n, seed):
-    return [int(x) for x in np.random.default_rng(seed).integers(0, V, size=n)]
-
-
-def slot_of(state, slot, n):
-    return {k: state[k][slot * n:(slot + 1) * n] for k in state}
-
-
-def solo(eng, toks, start=None):
-    """Logits of the last token and the state after running `toks` alone in GPT mode on slot 0 from `start`."""
-    if start is None:
-        eng.state_zero()
-    else:
-        eng.state_upload(start)
-    last = eng.forward(toks, mode=1)[-1]
-    return last, eng.state_download()
-
-
-def check_against_solo(got_logits, got_state, ref_logits, ref_state, length, what):
-    n = ref_state["xy"].size
-    if length > 1:
-        assert np.array_equal(got_logits, ref_logits), what + ": logits differ from the solo run"
-        for k in KEYS:
-            assert np.array_equal(got_state[k], ref_state[k][:n]), what + ": state " + k
-    else:
-        assert rel_err(got_logits, ref_logits) < 2e-5, what
-        for k in KEYS:
-            assert rel_err(got_state[k], ref_state[k][:n]) < 2e-5, what + ": state " + k
-
-
-def run_ragged_vs_solo(pkg, path, max_gpt, streams):
-    a = pkg.Engine(path, max_gpt=max_gpt)
-    n = a.n_layers * a.n_embed
-    a.forward(rand_tokens(min(max_gpt, 128), 99), mode=0, want_logits=False)  # every slot holds some state
-    before = a.state_download(max_gpt)
-    logits, nxt = a.forward_streams(streams, want_next=True)
-    after = a.state_download(max_gpt)
-    named = {s for s, _ in streams}
-    for slot in range(max_gpt):
-        if slot not in named:
-            for k in ("xy", "aa", "bb", "pp", "dd"):
-                assert np.array_equal(slot_of(after, slot, n)[k], slot_of(before, slot, n)[k]), "slot %d was touched" % slot
-    assert [int(x) for x in nxt] == [int(np.argmax(r)) for r in logits]
-    b = pkg.Engine(path, max_gpt=max(len(t) for _, t in streams))
-    b.set_option("prefill_min", 2)
-    for i, (slot, toks) in enumerate(streams):
-        ref, sb = solo(b, toks, slot_of(before, slot, n))
-        check_against_solo(logits[i], slot_of(after, slot, n), ref, sb, len(toks), "stream %d (slot %d, %d tokens)" % (i, slot, len(toks)))
-    a.close()
-    b.close()
 
 
 @pytest.mark.parametrize("L,E", [(3, 768), (2, 2048)])
@@ -95,7 +37,7 @@ def test_gpt_and_parralel_are_special_cases(pkg, make_model):
     ref = b.forward(toks, mode=1)
     assert np.array_equal(got[0], ref[-1])
     sa, sb = a.state_download(64), b.state_download(64)
-    for k in KEYS:
+    for k in KEYS4:
         assert np.array_equal(sa[k], sb[k]), k
     T = 16
     for seed in (2, 3):  # two steps: the second continues from the slots the first left
@@ -104,7 +46,7 @@ def test_gpt_and_parralel_are_special_cases(pkg, make_model):
         ref = b.forward(toks, mode=0)
         assert np.array_equal(got, ref)
     sa, sb = a.state_download(64), b.state_download(64)
-    for k in KEYS:
+    for k in KEYS4:
         assert np.array_equal(sa[k], sb[k]), k
     a.close()
     b.close()
@@ -130,7 +72,7 @@ def test_short_calls_run_through_the_decode_kernel(pkg, make_model):
         for i, (slot, toks) in enumerate(streams):
             ref, sb = solo(b, toks, slot_of(before, slot, n))
             assert np.array_equal(logits[i], ref), (step, i)
-            for k in KEYS:
+            for k in KEYS4:
                 assert np.array_equal(slot_of(after, slot, n)[k], sb[k][:n]), (step, i, k)
     a.close()
     b.close()
@@ -207,9 +149,9 @@ def test_slot_operations(pkg, make_model):
     a.slot_copy(2, 5)
     logits, _ = a.forward_streams([(2, [4118]), (5, [4118])])
     assert np.array_equal(logits[0], logits[1])
-    assert all(np.array_equal(a.slot_download(2)[k], a.slot_download(5)[k]) for k in KEYS)
+    assert all(np.array_equal(a.slot_download(2)[k], a.slot_download(5)[k]) for k in KEYS4)
     rng = np.random.default_rng(6)
-    st = {k: rng.standard_normal(n) for k in ("xy", "aa", "bb", "pp", "dd")}
+    st = {k: rng.standard_normal(n) for k in KEYS5}
     a.slot_upload(7, st)
     back = a.slot_download(7)
     assert all(np.array_equal(back[k], st[k]) for k in st)

@@ -13,18 +13,12 @@ the oracle's top-1 / top-2 margin exceeds 1e-3 of max|logits|; the tensor-core p
 import numpy as np
 import pytest
 
-from test_generate_gpu import check as check_generated
-from test_generate_gpu import host_loop
-from test_parity_gpu import margin, rel_err, run_pair
-from test_streams_gpu import run_ragged_vs_solo
+from decoding import KEYS4, V, check_generated, host_loop, run_pair, run_ragged_vs_solo
+from util import REL_TOL, margin, rel_err, token_stream
 
 pytestmark = pytest.mark.gpu
 
-REL_TOL = 1e-3
 PATH_TOL = 2e-5
-SEED_TOKEN = 4118
-V = 50277
-KEYS = ("xy", "aa", "bb", "dd")
 L = 2
 
 # n_embed -> tokens of the single-stream GPT chunk on the tensor cores. Every padded pass size (Tp = 32, 64, 96, 128)
@@ -43,17 +37,12 @@ WIDTHS = {
 FEATURE_WIDTHS = [784, 2560]  # one width with a K tail, one real model width
 
 
-def token_stream(n, seed):
-    rng = np.random.default_rng(seed)
-    return [SEED_TOKEN] + [int(x) for x in rng.integers(0, V, size=n - 1)]
-
-
 def oracle_run(path, toks):
     """The oracle's logits after every token of `toks` from the zero state, and its state after the last."""
     from oracle.oracle import Oracle
     orc = Oracle(path)
     logits = np.stack([orc.forward(t) for t in toks])
-    state = {k: orc.state[k].copy() for k in KEYS}
+    state = {k: orc.state[k].copy() for k in KEYS4}
     orc.close()
     return logits, state
 
@@ -73,7 +62,7 @@ def check_rows(got, ref, what):
 
 def state_err(got, ref):
     n = ref["xy"].size
-    return max(rel_err(got[k][:n], ref[k]) for k in KEYS)
+    return max(rel_err(got[k][:n], ref[k]) for k in KEYS4)
 
 
 @pytest.mark.parametrize("E", sorted(WIDTHS))
@@ -106,7 +95,7 @@ def test_gpt_chunk_on_tensor_cores_matches_oracle(pkg, make_model, E):
           "vs decode kernel %.3g" % (E, T, worst, checked, T, se, path_worst))
     assert path_worst < PATH_TOL
     n = a.n_layers * a.n_embed
-    for k in KEYS:
+    for k in KEYS4:
         assert rel_err(sa[k][:n], sb[k][:n]) < PATH_TOL, k
     nxt = int(single[-1].argmax())
     assert rel_err(a.forward([nxt])[0], b.forward([nxt])[0]) < PATH_TOL

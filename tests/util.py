@@ -18,6 +18,28 @@ def compile_cpp(src, out, link_engine=False, extra=()):
 
 VOCAB = 50277
 GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
+REL_TOL = 1e-3     # logits within 1e-3 of max|logits| of the oracle's (BASELINE.json north_star)
+SEED_TOKEN = 4118  # "###", first token of the storygen prompt
+
+
+def rel_err(got, ref):
+    """max|got - ref| relative to max|ref|, in float64."""
+    import numpy as np
+    return float(np.abs(got.astype(np.float64) - ref.astype(np.float64)).max() / max(np.abs(ref).max(), 1e-6))
+
+
+def margin(ref):
+    """The gap between the two largest entries of `ref`, relative to max|ref|."""
+    import numpy as np
+    top = np.partition(ref, -2)[-2:]
+    return float((top.max() - top.min()) / max(np.abs(ref).max(), 1e-6))
+
+
+def token_stream(n, seed):
+    """SEED_TOKEN followed by n - 1 seeded random tokens."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    return [SEED_TOKEN] + [int(x) for x in rng.integers(0, VOCAB, size=n - 1)]
 
 
 def stress_model(src, dst, kind, L=3, E=768):
