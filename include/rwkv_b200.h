@@ -603,6 +603,97 @@ int rwkv_b200_batcher_release(rwkv_b200_batcher *b, unsigned long long id);
 /* Close the batcher and free its buffers; unfinished requests are dropped where they stand. NULL is ignored. */
 void rwkv_b200_batcher_close(rwkv_b200_batcher *b);
 
+/* Stop strings: end a stream when the text it emits contains one of its stop strings ("\n\nUser:", "</answer>"), which
+ * may start or end in the middle of a token and be spelled by many token sequences. A stop set is 1..n non-empty byte
+ * strings of at most RWKV_B200_MAX_STOP_BYTES bytes in total. A stream with a set carries a match state; B is the byte
+ * string of the tokens it emits in the call, each token's bytes as GPT2Tokenizer::decode({id}) gives them (the table of
+ * rwkv_b200_token_bytes_set), prefixed by the text its start state carries over from an earlier call.
+ *  1. The stream ends after the first emitted token t_j whose bytes complete an occurrence of a string of the set in B
+ *     (the occurrence may begin in earlier tokens or in the carried text). t_j is emitted, not fed, like a stop token:
+ *     it is in tokens_out and counts in the length, and the slot holds the state after t_(j-1) was fed.
+ *  2. hit = 1 + the index of the matched string (among the strings ending at the earliest end byte, the lowest index),
+ *     or 0 when the stream ended otherwise; tail = the bytes of t_j after the end of the occurrence; state = the final
+ *     match state. So the text before the match is B[:len(B) - tail - len(string)].
+ *  3. Stop tokens, budgets and token automata keep their meaning; whichever comes first ends the stream, and when a stop
+ *     string and one of them end it on the same token, hit still reports the string.
+ * The tokens and lengths are a prefix of the same call without stop sets, and each named slot holds bit for bit the state
+ * of that call run with the stream's budget set to min(budget, j + 1). A stream without a set (RWKV_B200_NO_STOP_SET)
+ * generates exactly as without this feature, and a call in which no stream has a set enqueues exactly what the call
+ * without a stop request enqueues.
+ * Match states: state q is the q-th distinct prefix of the set's strings in order of first appearance (0 the empty
+ * prefix, then the prefixes of string 0 by length, then the new prefixes of string 1, and so on); the state after B is
+ * the longest suffix of B that is a prefix of some string, and a start state q carries prefix q over. The device holds
+ * each set as an Aho-Corasick DFA, next[states][256] and hit[states] in u32 (at most 4097 states, about 4 MB), and walks
+ * each emitted token's bytes through it in the kernel that emits the token, stopping at the first byte that ends a
+ * string. Not available: beam search, the typical sampler of rwkv_b200_generate_streams, seeding the state from prompt
+ * text, and regular-expression patterns. */
+#define RWKV_B200_NO_STOP_SET 0xFFFFFFFFFFFFFFFFULL /* set_ids entry of a stream without a stop set */
+#define RWKV_B200_MAX_STOP_BYTES 4096
+
+/* The bytes of every token: token v is bytes[start[v] .. start[v + 1]), v < 50277 (start: [50277 + 1], ascending from
+ * 0). Uploaded once per model; a later call replaces the table. Refused: start not starting at 0 or decreasing, NULL
+ * bytes with a non-empty table, tensor parallelism, and a replacement while an unfinished batcher request has a set. */
+int rwkv_b200_token_bytes_set(rwkv_b200_model *m, const unsigned long long *start, const unsigned char *bytes);
+/* Build and upload the automaton of a stop set: string i is bytes[string_start[i] .. string_start[i + 1]), i <
+ * n_strings; *id receives its id. Refused: no strings, string_start not starting at 0, an empty string (or offsets that
+ * decrease), more than RWKV_B200_MAX_STOP_BYTES bytes in total, and tensor parallelism. */
+int rwkv_b200_stop_set_add(rwkv_b200_model *m, unsigned long long n_strings, const unsigned long long *string_start,
+                           const unsigned char *bytes, unsigned long long *id);
+/* Free a stop set (an unknown or removed id is refused, and so is one that an unfinished request of the model's batcher
+ * names). rwkv_b200_free frees every set. */
+int rwkv_b200_stop_set_remove(rwkv_b200_model *m, unsigned long long id);
+
+/* What a generate call adds for stop strings, per stream. */
+typedef struct rwkv_b200_stop_request {
+    const unsigned long long *set_ids;      /* [n_streams] an id of rwkv_b200_stop_set_add or RWKV_B200_NO_STOP_SET; NULL: none */
+    const unsigned long long *start_states; /* [n_streams] each stream's first match state; NULL: 0 */
+    unsigned long long *states_out;         /* [n_streams] the final match state (0 without a set), or NULL */
+    unsigned long long *hit_out;            /* [n_streams] hit by rule 2 (0 without a set), or NULL */
+    unsigned long long *tail_out;           /* [n_streams] tail by rule 2 (0 unless hit), or NULL */
+} rwkv_b200_stop_request;
+
+/* rwkv_b200_generate_streams_constrained with stop strings by the rule above (stop == NULL: exactly that call).
+ * Refused before any work (every slot untouched): every refusal of generate_streams_constrained, an unknown or removed set
+ * id, a start state out of range, and a set used before the model has a token-bytes table. */
+int rwkv_b200_generate_streams_stop(rwkv_b200_model *m, const unsigned long long *slots,
+                                    const unsigned long long *first_tokens, unsigned long long n_streams,
+                                    unsigned long long max_new, const unsigned long long *budgets,
+                                    const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                    const unsigned long long *override_tokens, const float *override_values,
+                                    unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
+                                    unsigned long long *tokens_out, unsigned long long *lengths_out, int logprob_mode,
+                                    unsigned int top_n, double *logprobs_out, unsigned long long *ranks_out,
+                                    unsigned long long *top_tokens_out, double *top_logprobs_out,
+                                    const unsigned long long *constraint_ids, const unsigned long long *start_states,
+                                    unsigned long long *states_out, const rwkv_b200_stop_request *stop);
+
+/* rwkv_b200_generate_streams_speculative with stop strings (stop == NULL: exactly that call). Each emitted token of a
+ * step is walked in order, so a string that ends inside an accepted run of drafts ends the stream at that token. The
+ * tokens, lengths, first slots and hit, tail and state are bit for bit those of rwkv_b200_generate_streams_stop on the
+ * first slots, by the speculative rule. Refused as well: the stop refusals of rwkv_b200_generate_streams_stop. */
+int rwkv_b200_generate_streams_speculative_stop(rwkv_b200_model *m, const unsigned long long *slots,
+                                                const unsigned long long *first_tokens, unsigned long long n_streams,
+                                                unsigned long long max_new, const unsigned long long *budgets,
+                                                const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                                const unsigned long long *override_tokens, const float *override_values,
+                                                unsigned long long n_override, const rwkv_b200_sampler *samplers,
+                                                const double *u, unsigned long long *tokens_out,
+                                                unsigned long long *lengths_out, unsigned int draft, unsigned int ngram,
+                                                const unsigned long long *context_start, const unsigned long long *context,
+                                                unsigned long long *steps_out, const rwkv_b200_stop_request *stop);
+
+/* rwkv_b200_batcher_submit_ex (x may be NULL) with a stop set: set_id (RWKV_B200_NO_STOP_SET: exactly submit_ex) and its
+ * start state. The batcher rule's step 2 becomes rwkv_b200_generate_streams_stop of the one stream with the set and start
+ * state; a request whose stop string matches ends as RWKV_B200_REQ_DONE. Refused as well, with nothing queued: an unknown
+ * or removed set id, a start state out of range, and a model without a token-bytes table. While the request is
+ * unfinished its set cannot be removed. */
+int rwkv_b200_batcher_submit_stop(rwkv_b200_batcher *b, const rwkv_b200_request *r, const rwkv_b200_request_ex *x,
+                                  unsigned long long set_id, unsigned long long start_state, unsigned long long *id);
+/* A request's hit, tail and current match state by the rule above (0, 0, 0 without a set); each pointer may be NULL. A
+ * cancelled request's state is the state after its emitted tokens. An unknown or released id is refused. */
+int rwkv_b200_batcher_read_stop(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *hit,
+                                unsigned long long *tail, unsigned long long *state);
+
 /* State of one slot: zero it (a new conversation), copy it onto another slot (fork a conversation), or move it
  * between the device and host arrays of n_layers x n_embed doubles each (NULL arrays are skipped). */
 int rwkv_b200_slot_zero(rwkv_b200_model *m, unsigned long long slot);

@@ -143,7 +143,19 @@ struct rwkv_b200_model {
         // generate_streams_constrained: each stream's automaton and state, and the record of a token without an edge
         DevBuf<rk::GenConstraint> gc;      // [n_streams]
         DevBuf<unsigned long long> fault;  // [3]
+        DevBuf<rk::GenStop> gst;           // [n_streams] generate_streams_stop and the speculative call: stop sets
     } gen;
+    // stop strings: the token bytes (rwkv_b200_token_bytes_set) and per set id its automaton (rwkv_b200_stop_set_add):
+    // next [states][256] then hit [states] in one device block
+    DevBuf<unsigned long long> tb_start; // [V + 1]
+    DevBuf<unsigned char> tb_bytes;
+    bool has_tb = false;
+    struct StopSet {
+        unsigned long long states = 0;
+        DevBuf<uint32_t> dev;
+    };
+    std::map<unsigned long long, StopSet> stop_sets;
+    unsigned long long next_stop_set = 1;
     // rwkv_b200_constraint_add: per id, the CSR on the host (the override check of a call) and one device block holding
     // the allow masks, then edge_start, the edge tokens and their targets
     struct Automaton {
@@ -208,6 +220,9 @@ struct rwkv_b200_batcher {
         rk::LogprobLane lp{-1, 0};
         std::vector<double> logprobs, top_logprobs;             // [tokens], [tokens][lp.top_n]
         std::vector<unsigned long long> ranks, top_tokens;      // [tokens], [tokens][lp.top_n]
+        // rwkv_b200_batcher_submit_stop: the stop set (gst.next == nullptr: none) with its match state and result
+        rk::GenStop gst{};
+        unsigned long long stop_set = RWKV_B200_NO_STOP_SET;
     };
     std::map<unsigned long long, Req> reqs;
     unsigned long long next_id = 1;
@@ -238,6 +253,8 @@ struct rwkv_b200_batcher {
     std::vector<double> h_lpv, h_top_lp;      // host copies of the rings
     std::vector<unsigned long long> h_rank, h_top_tok;
     DevBuf<float> raw;                        // [rows][V] the model's rows of a step, for raw lanes (see batcher_group)
+    std::vector<rk::GenStop> h_gst;           // [rows] host mirror of the lanes' stop sets (next nullptr: none)
+    DevBuf<rk::GenStop> gst;                  // [rows]
 };
 
 namespace {
@@ -935,6 +952,41 @@ int check_constraints(M *m, const char *what, const ConstraintRequest &cq, unsig
     return 0;
 }
 
+// The stop set of each stream of a call with a stop request (a zero record: none), refused before any work: unknown ids,
+// a set used before the model has token bytes, and start states out of range.
+int check_stops(M *m, const char *what, const rwkv_b200_stop_request *sq, unsigned long long n_streams,
+                std::vector<rk::GenStop> &out) {
+    out.assign(n_streams, rk::GenStop{});
+    if (!sq || !sq->set_ids) return 0;
+    for (unsigned long long s = 0; s < n_streams; ++s) {
+        const unsigned long long id = sq->set_ids[s];
+        if (id == RWKV_B200_NO_STOP_SET) continue;
+        const auto it = m->stop_sets.find(id);
+        if (it == m->stop_sets.end()) return fail(1, "%s: stream %llu: stop set id %llu is unknown or removed", what, s, id);
+        if (!m->has_tb)
+            return fail(1, "%s: stream %llu: stop set %llu is used before the model has a token-bytes table "
+                           "(rwkv_b200_token_bytes_set)", what, s, id);
+        const M::StopSet &ss = it->second;
+        const unsigned long long q = sq->start_states ? sq->start_states[s] : 0;
+        if (q >= ss.states)
+            return fail(1, "%s: stream %llu: start state %llu of stop set %llu is out of range (%llu states)", what, s, q, id,
+                        ss.states);
+        out[s] = rk::GenStop{ss.dev.p, ss.dev.p + ss.states * 256, m->tb_start.p, m->tb_bytes.p, q, 0, 0};
+    }
+    return 0;
+}
+
+// A call's stop results from the streams' final records (the request's NULL arrays are skipped).
+void write_stops(const rwkv_b200_stop_request *sq, const std::vector<rk::GenStop> &st) {
+    if (!sq) return;
+    for (size_t s = 0; s < st.size(); ++s) {
+        const bool on = st[s].next != nullptr;
+        if (sq->states_out) sq->states_out[s] = on ? st[s].state : 0;
+        if (sq->hit_out) sq->hit_out[s] = on ? st[s].match : 0;
+        if (sq->tail_out) sq->tail_out[s] = on ? st[s].tail : 0;
+    }
+}
+
 // The arguments the generate_streams calls and generate_streams_speculative share: the streams (their slots, first
 // tokens, max_new and budgets), the stop tokens, overrides, samplers (NULL: none) and uniforms, and the results.
 struct GenCall {
@@ -1051,9 +1103,10 @@ int pick_rows(M *m, const PickChain &pc, int rows, const double *u) {
 // The body of generate_streams (samplers == NULL, `temp` and `u` pick the typical sampler or the arg-max), of
 // generate_streams_ex (`ex`: every stream has its own sampler, or all pick the arg-max when samplers == NULL), of
 // generate_streams_logprobs (generate_streams_ex with `lpq`: each emitted token is scored after its pick) and of
-// generate_streams_constrained (with `cq`: token automata mask the rows after the overrides; `lpq` may be NULL).
+// generate_streams_constrained (with `cq`: token automata mask the rows after the overrides; `lpq` may be NULL) and of
+// generate_streams_stop (with `sq` as well: k_gen_feedback walks each emitted token through the stream's stop set).
 int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, const LogprobRequest *lpq = nullptr,
-             const ConstraintRequest *cq = nullptr) {
+             const ConstraintRequest *cq = nullptr, const rwkv_b200_stop_request *sq = nullptr) {
     int rc = check_streams_model(m, what);
     if (rc) return rc;
     if (lpq) {
@@ -1071,9 +1124,13 @@ int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, cons
     std::vector<rk::GenConstraint> hgc;
     if (cq && (rc = check_constraints(m, what, *cq, n_streams, c.override_tokens, c.override_values, c.n_override, hgc))) return rc;
     const bool constrained = std::any_of(hgc.begin(), hgc.end(), [](const rk::GenConstraint &gc) { return gc.mask != nullptr; });
+    std::vector<rk::GenStop> hst;
+    if ((rc = check_stops(m, what, sq, n_streams, hst))) return rc;
+    const bool stopped = std::any_of(hst.begin(), hst.end(), [](const rk::GenStop &st) { return st.next != nullptr; });
     CK(cudaSetDevice(m->device));
     auto &g = m->gen;
     if (constrained && ((rc = g.gc.grow(n_streams)) || (rc = g.fault.grow(3)))) return rc;
+    if (stopped && (rc = g.gst.grow(n_streams))) return rc;
     if (pen && ((rc = g.pen_cnt.grow(n_streams * V)) || (rc = g.pen_seen.grow(n_streams * V)))) return rc;
     if (c.u && (rc = g.u.grow(kGenGroup * m->max_gpt))) return rc;
     // raw mode reads the model's rows: d_slogits itself, or a copy taken before the penalties, overrides and mask edit it
@@ -1096,6 +1153,7 @@ int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, cons
         CK(cudaMemcpyAsync(g.gc.p, hgc.data(), n_streams * sizeof(rk::GenConstraint), cudaMemcpyHostToDevice, m->stream));
         CK(cudaMemsetAsync(g.fault.p, 0, 3 * sizeof(unsigned long long), m->stream));
     }
+    if (stopped) CK(cudaMemcpyAsync(g.gst.p, hst.data(), n_streams * sizeof(rk::GenStop), cudaMemcpyHostToDevice, m->stream));
     if (pen) { // the history starts empty in every call: prompt tokens are not counted
         CK(cudaMemsetAsync(g.pen_cnt.p, 0, n_streams * V * sizeof(float), m->stream));
         CK(cudaMemsetAsync(g.pen_seen.p, 0, n_streams * V, m->stream));
@@ -1126,7 +1184,8 @@ int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, cons
             CK(cudaMemcpyAsync(g.u.p, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
         }
         rk::GenFeedbackArgs fb{g.gs, g.row_stream, rows, c.u || c.samplers ? nullptr : m->d_next, m->d_sample, g.stop.p, (int)c.n_stop,
-                               g.out.p, max_new, tc ? g.passes : nullptr, constrained ? g.gc.p : nullptr, g.fault.p};
+                               g.out.p, max_new, tc ? g.passes : nullptr, constrained ? g.gc.p : nullptr, g.fault.p, nullptr,
+                               stopped ? g.gst.p : nullptr};
         rk::GenLogprobArgs la{};
         if (lpq)
             la = rk::GenLogprobArgs{raw_copy ? g.raw.p : m->d_slogits, (int)V, g.gs, g.row_stream, fb.next, m->d_sample,
@@ -1166,10 +1225,12 @@ int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, cons
     }
     if (constrained && cq->states_out)
         CK(cudaMemcpyAsync(hgc.data(), g.gc.p, n_streams * sizeof(rk::GenConstraint), cudaMemcpyDeviceToHost, m->stream));
+    if (stopped) CK(cudaMemcpyAsync(hst.data(), g.gst.p, n_streams * sizeof(rk::GenStop), cudaMemcpyDeviceToHost, m->stream));
     SYNC(m);
     for (unsigned long long s = 0; s < n_streams; ++s) c.lengths_out[s] = hg[s].len;
     if (cq && cq->states_out)
         for (unsigned long long s = 0; s < n_streams; ++s) cq->states_out[s] = hgc[s].mask ? hgc[s].state : 0;
+    write_stops(sq, hst);
     return 0;
 }
 
@@ -1198,6 +1259,7 @@ int batcher_boundary(B *b, std::vector<int> &dec) {
         ad.push_back(id);
         b->h_gc[q.lane] = rk::GenConstraint{};
         b->h_lp[q.lane] = rk::LogprobLane{-1, 0};
+        b->h_gst[q.lane] = rk::GenStop{};
         CK(cudaMemcpyAsync(b->samp.p + q.lane, &q.sampler, sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
         if (q.sampler.presence_penalty != 0.0f || q.sampler.frequency_penalty != 0.0f) {
             int rc;
@@ -1214,6 +1276,7 @@ int batcher_boundary(B *b, std::vector<int> &dec) {
             b->h_gs[q.lane] = rk::GenStream{q.slot, q.max_new, q.prompt.back(), 0, 0};
             b->h_gc[q.lane] = q.gc;
             b->h_lp[q.lane] = q.lp;
+            b->h_gst[q.lane] = q.gst;
         }
         if (q.status == RWKV_B200_REQ_GENERATING) dec.push_back(q.lane);
     }
@@ -1319,7 +1382,7 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
     }
     CK(cudaMemcpyAsync(b->passes.p, all.data(), all.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
     // what the decode lanes use: each feature's work is enqueued only when one of them needs it
-    bool pen = false, constrained = false, scored = false, raw = false;
+    bool pen = false, constrained = false, scored = false, raw = false, stopped = false;
     int top = 0; // the largest top_n of a scored lane
     std::vector<const B::Req *> of_lane(b->rows, nullptr);
     for (unsigned long long id : b->admitted) of_lane[b->reqs[id].lane] = &b->reqs[id];
@@ -1335,6 +1398,7 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
                 if (g.len + k < q.max_new) ug[k * R + r] = q.u[g.len + k];
             pen |= q.sampler.presence_penalty != 0.0f || q.sampler.frequency_penalty != 0.0f;
             constrained |= q.gc.mask != nullptr;
+            stopped |= q.gst.next != nullptr;
             if (q.lp.mode >= 0) {
                 scored = true;
                 raw |= q.lp.mode == RWKV_B200_LOGPROBS_RAW;
@@ -1348,6 +1412,10 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
         if ((rc = b->gc.grow(b->rows)) || (rc = b->fault.grow(3))) return rc;
         CK(cudaMemcpyAsync(b->gc.p, b->h_gc.data(), b->rows * sizeof(rk::GenConstraint), cudaMemcpyHostToDevice, m->stream));
         CK(cudaMemsetAsync(b->fault.p, 0, 3 * sizeof(unsigned long long), m->stream));
+    }
+    if (stopped) {
+        if ((rc = b->gst.grow(b->rows))) return rc;
+        CK(cudaMemcpyAsync(b->gst.p, b->h_gst.data(), b->rows * sizeof(rk::GenStop), cudaMemcpyHostToDevice, m->stream));
     }
     // raw lanes read the model's rows: d_slogits itself, or a copy taken before the penalties, overrides and masks edit it
     const bool raw_copy = raw && (pen || b->n_ovr || constrained);
@@ -1373,7 +1441,7 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
         }
         rk::GenFeedbackArgs fb{b->gs.p, b->row_stream.p, R, nullptr, m->d_sample, b->stop.p, 0, b->out.p, kGenGroup,
                                k + 1 < steps ? b->passes.p + (k + 1) * b->max_pass : nullptr, constrained ? b->gc.p : nullptr,
-                               b->fault.p, b->stop_start.p};
+                               b->fault.p, b->stop_start.p, stopped ? b->gst.p : nullptr};
         rk::k_gen_feedback<<<(unsigned)((R + 127) / 128), 128, 0, m->stream>>>(fb);
         LAUNCHED(m);
     }
@@ -1388,6 +1456,7 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
         CK(cudaMemcpyAsync(b->h_gc.data(), b->gc.p, b->rows * sizeof(rk::GenConstraint), cudaMemcpyDeviceToHost, m->stream));
         CK(cudaMemcpyAsync(fault, b->fault.p, sizeof(fault), cudaMemcpyDeviceToHost, m->stream));
     }
+    if (stopped) CK(cudaMemcpyAsync(b->h_gst.data(), b->gst.p, b->rows * sizeof(rk::GenStop), cudaMemcpyDeviceToHost, m->stream));
     if (scored) {
         b->h_lpv.resize(ring);
         b->h_rank.resize(ring);
@@ -1427,6 +1496,7 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
             }
         }
         if (q.gc.mask) q.gc.state = b->h_gc[q.lane].state;
+        if (q.gst.next) q.gst = b->h_gst[q.lane];
         if (g.done) q.status = RWKV_B200_REQ_DONE;
     }
     // finished requests leave here, before the next boundary admits anyone (a caller may release them in between)
@@ -1832,6 +1902,95 @@ int rwkv_b200_generate_streams_constrained(rwkv_b200_model *m, const unsigned lo
     return generate(m, "generate_streams_constrained", true, c, 1.0f, logprobs_out ? &lpq : nullptr, &cq);
 }
 
+int rwkv_b200_token_bytes_set(rwkv_b200_model *m, const unsigned long long *start, const unsigned char *bytes) {
+    const char *what = "token_bytes_set";
+    int rc = check_streams_model(m, what);
+    if (rc) return rc;
+    const size_t V = binfmt::kVocab;
+    if (!start) return fail(1, "%s: start is NULL", what);
+    if (start[0] != 0) return fail(1, "%s: start[0] = %llu, not 0", what, start[0]);
+    for (size_t v = 0; v < V; ++v)
+        if (start[v + 1] < start[v])
+            return fail(1, "%s: start decreases from token %zu to %zu (%llu > %llu)", what, v, v + 1, start[v], start[v + 1]);
+    const unsigned long long n = start[V];
+    if (n && !bytes) return fail(1, "%s: %llu bytes with NULL bytes", what, n);
+    // the lane records of the model's batcher point into the table
+    if (const rwkv_b200_batcher *b = m->batcher)
+        for (const auto &e : b->reqs)
+            if (e.second.gst.next && e.second.status <= RWKV_B200_REQ_GENERATING)
+                return fail(1, "%s: unfinished request %llu of the model's batcher has a stop set", what, e.first);
+    CK(cudaSetDevice(m->device));
+    CK(cudaStreamSynchronize(m->stream));
+    if ((rc = m->tb_start.grow(V + 1)) || (rc = m->tb_bytes.grow(std::max<unsigned long long>(n, 1)))) {
+        m->has_tb = false;
+        return rc;
+    }
+    CK(cudaMemcpy(m->tb_start.p, start, (V + 1) * sizeof(unsigned long long), cudaMemcpyHostToDevice));
+    if (n) CK(cudaMemcpy(m->tb_bytes.p, bytes, n, cudaMemcpyHostToDevice));
+    m->has_tb = true;
+    return 0;
+}
+
+int rwkv_b200_stop_set_add(rwkv_b200_model *m, unsigned long long n_strings, const unsigned long long *string_start,
+                           const unsigned char *bytes, unsigned long long *id) {
+    const char *what = "stop_set_add";
+    int rc = check_streams_model(m, what);
+    if (rc) return rc;
+    if (!string_start || !bytes || !id) return fail(1, "%s: null argument (string_start, bytes and id are required)", what);
+    if (n_strings == 0) return fail(1, "%s: no strings", what);
+    if (string_start[0] != 0) return fail(1, "%s: string_start[0] = %llu, not 0", what, string_start[0]);
+    for (unsigned long long i = 0; i < n_strings; ++i)
+        if (string_start[i + 1] <= string_start[i]) return fail(1, "%s: string %llu is empty or its offsets decrease", what, i);
+    if (string_start[n_strings] > RWKV_B200_MAX_STOP_BYTES)
+        return fail(1, "%s: %llu bytes in total > %d", what, string_start[n_strings], RWKV_B200_MAX_STOP_BYTES);
+    std::vector<uint32_t> next, hit;
+    const uint32_t states = stopmatch::build(string_start, bytes, n_strings, next, hit);
+    next.insert(next.end(), hit.begin(), hit.end()); // one block: next [states][256], then hit [states]
+    M::StopSet ss;
+    ss.states = states;
+    CK(cudaSetDevice(m->device));
+    if ((rc = ss.dev.grow(next.size()))) return rc;
+    CK(cudaMemcpy(ss.dev.p, next.data(), next.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    *id = m->next_stop_set++;
+    m->stop_sets.emplace(*id, std::move(ss));
+    return 0;
+}
+
+int rwkv_b200_stop_set_remove(rwkv_b200_model *m, unsigned long long id) {
+    int rc = check_model(m);
+    if (rc) return rc;
+    const auto it = m->stop_sets.find(id);
+    if (it == m->stop_sets.end()) return fail(1, "stop_set_remove: stop set id %llu is unknown or removed", id);
+    // the lane records of the model's batcher point into the set's device block
+    if (const rwkv_b200_batcher *b = m->batcher)
+        for (const auto &e : b->reqs)
+            if (e.second.stop_set == id && e.second.status <= RWKV_B200_REQ_GENERATING)
+                return fail(1, "stop_set_remove: stop set id %llu is named by unfinished request %llu of the model's batcher", id,
+                            e.first);
+    CK(cudaSetDevice(m->device));
+    CK(cudaStreamSynchronize(m->stream));
+    m->stop_sets.erase(it);
+    return 0;
+}
+
+int rwkv_b200_generate_streams_stop(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
+                                    unsigned long long n_streams, unsigned long long max_new, const unsigned long long *budgets,
+                                    const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                    const unsigned long long *override_tokens, const float *override_values,
+                                    unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
+                                    unsigned long long *tokens_out, unsigned long long *lengths_out, int logprob_mode,
+                                    unsigned int top_n, double *logprobs_out, unsigned long long *ranks_out,
+                                    unsigned long long *top_tokens_out, double *top_logprobs_out,
+                                    const unsigned long long *constraint_ids, const unsigned long long *start_states,
+                                    unsigned long long *states_out, const rwkv_b200_stop_request *stop) {
+    const GenCall c{slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values,
+                    n_override, samplers, samplers ? u : nullptr, tokens_out, lengths_out};
+    const LogprobRequest lpq{logprob_mode, top_n, logprobs_out, ranks_out, top_tokens_out, top_logprobs_out};
+    const ConstraintRequest cq{constraint_ids, start_states, states_out};
+    return generate(m, stop ? "generate_streams_stop" : "generate_streams_constrained", true, c, 1.0f,
+                    logprobs_out ? &lpq : nullptr, &cq, stop);
+}
+
 // Beam search: generate()'s group loop over beams. Step 0 has one row per group, later steps B rows per live group
 // (group by group); each step is forward -> k_beam_expand -> k_beam_select -> k_beam_fork. At each host group's end the
 // done flags come back and the done groups leave the rows; at the end the backpointers and the hypothesis lists come
@@ -1970,16 +2129,19 @@ int rwkv_b200_beam_search(rwkv_b200_model *m, const unsigned long long *slots, c
 
 // Speculative generation: generate()'s group loop with k + 1 rows per live stream. Each step is k_spec_draft -> passes
 // -> pick_rows (overrides, pick) -> k_spec_accept; at each group's end the records come back and the finished streams
-// leave the rows. At the end a stream whose home is a spare has it copied to its first slot.
-int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
-                                           unsigned long long n_streams, unsigned long long max_new, const unsigned long long *budgets,
-                                           const unsigned long long *stop_tokens, unsigned long long n_stop,
-                                           const unsigned long long *override_tokens, const float *override_values,
-                                           unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
-                                           unsigned long long *tokens_out, unsigned long long *lengths_out, unsigned int draft,
-                                           unsigned int ngram, const unsigned long long *context_start,
-                                           const unsigned long long *context, unsigned long long *steps_out) {
-    const char *what = "generate_streams_speculative";
+// leave the rows. At the end a stream whose home is a spare has it copied to its first slot. With a stop request,
+// k_spec_accept also walks each emitted token through the stream's stop set.
+int rwkv_b200_generate_streams_speculative_stop(rwkv_b200_model *m, const unsigned long long *slots,
+                                                const unsigned long long *first_tokens, unsigned long long n_streams,
+                                                unsigned long long max_new, const unsigned long long *budgets,
+                                                const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                                const unsigned long long *override_tokens, const float *override_values,
+                                                unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
+                                                unsigned long long *tokens_out, unsigned long long *lengths_out, unsigned int draft,
+                                                unsigned int ngram, const unsigned long long *context_start,
+                                                const unsigned long long *context, unsigned long long *steps_out,
+                                                const rwkv_b200_stop_request *sq) {
+    const char *what = sq ? "generate_streams_speculative_stop" : "generate_streams_speculative";
     int rc = check_streams_model(m, what);
     if (rc) return rc;
     if (draft < 1 || draft > (unsigned)rk::kSpecMaxDraft) return fail(1, "%s: draft %u is outside 1..%d", what, draft, rk::kSpecMaxDraft);
@@ -2007,10 +2169,14 @@ int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned lo
         if (n_ctx && !context) return fail(1, "%s: %llu context tokens with NULL context", what, n_ctx);
         if ((rc = check_tokens(what, "context token", context, n_ctx))) return rc;
     }
+    std::vector<rk::GenStop> hst;
+    if ((rc = check_stops(m, what, sq, S, hst))) return rc;
+    const bool stopped = std::any_of(hst.begin(), hst.end(), [](const rk::GenStop &st) { return st.next != nullptr; });
     const unsigned long long n_hist = n_ctx + S * (1 + max_new);
     CK(cudaSetDevice(m->device));
     auto &g = m->gen;
     auto &sp = m->spec;
+    if (stopped && (rc = g.gst.grow(S))) return rc;
     const int per_pass = rk::kPfMaxTokens / (int)K1; // streams per pass: a stream's rows never straddle two passes
     const size_t n_pass = (size_t)((S + per_pass - 1) / per_pass);
     if ((rc = sp.ss.grow(S)) || (rc = sp.hist.grow(n_hist)) || (rc = sp.live.grow(S)) || (rc = sp.passes.grow(n_pass)) ||
@@ -2038,11 +2204,13 @@ int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned lo
     CK(cudaMemcpyAsync(sp.ss.p, hs.data(), S * sizeof(rk::SpecStream), cudaMemcpyHostToDevice, m->stream));
     if ((rc = upload_gen(m, c))) return rc;
     if (u) CK(cudaMemcpyAsync(sp.u.p, u, max_new * S * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+    if (stopped) CK(cudaMemcpyAsync(g.gst.p, hst.data(), S * sizeof(rk::GenStop), cudaMemcpyHostToDevice, m->stream));
 
     std::vector<int> live(S), rs;
     for (unsigned long long s = 0; s < S; ++s) live[s] = (int)s;
     rk::SpecArgs sa{sp.ss.p, sp.live.p, (int)draft, (int)ngram, per_pass, sp.hist.p, sp.passes.p, u ? sp.u.p : nullptr,
-                    sp.row_u.p, S, max_new, samplers ? nullptr : m->d_next, m->d_sample, g.stop.p, (int)n_stop, g.out.p};
+                    sp.row_u.p, S, max_new, samplers ? nullptr : m->d_next, m->d_sample, g.stop.p, (int)n_stop, g.out.p,
+                    stopped ? g.gst.p : nullptr};
     const PickChain pc{nullptr, g.row_stream, samplers ? g.samp.p : nullptr, nullptr, nullptr, g.ovr_tok.p, g.ovr_val.p, n_override};
     // each step emits at least one token per live stream, so max_new steps finish every stream
     for (unsigned long long step = 0; !live.empty() && step < max_new;) {
@@ -2079,12 +2247,27 @@ int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned lo
         if ((rc = fork_slots(m, sp.forks.p, forks.size() / 2, false))) return rc;
     }
     CK(cudaMemcpyAsync(tokens_out, g.out.p, S * max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+    if (stopped) CK(cudaMemcpyAsync(hst.data(), g.gst.p, S * sizeof(rk::GenStop), cudaMemcpyDeviceToHost, m->stream));
     SYNC(m);
     for (unsigned long long s = 0; s < S; ++s) {
         lengths_out[s] = hs[s].len;
         steps_out[s] = hs[s].steps;
     }
+    write_stops(sq, hst);
     return 0;
+}
+
+int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
+                                           unsigned long long n_streams, unsigned long long max_new, const unsigned long long *budgets,
+                                           const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                           const unsigned long long *override_tokens, const float *override_values,
+                                           unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
+                                           unsigned long long *tokens_out, unsigned long long *lengths_out, unsigned int draft,
+                                           unsigned int ngram, const unsigned long long *context_start,
+                                           const unsigned long long *context, unsigned long long *steps_out) {
+    return rwkv_b200_generate_streams_speculative_stop(m, slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop,
+                                                       override_tokens, override_values, n_override, samplers, u, tokens_out,
+                                                       lengths_out, draft, ngram, context_start, context, steps_out, nullptr);
 }
 
 int rwkv_b200_sample_streams(rwkv_b200_model *m, unsigned long long n_streams, const rwkv_b200_sampler *params, const double *u,
@@ -2287,6 +2470,7 @@ int rwkv_b200_batcher_open(rwkv_b200_model *m, unsigned long long rows, unsigned
     b->h_out.assign(rows * kGenGroup, 0);
     b->h_gc.assign(rows, rk::GenConstraint{});
     b->h_lp.assign(rows, rk::LogprobLane{-1, 0});
+    b->h_gst.assign(rows, rk::GenStop{});
     if ((rc = b->gs.grow(rows)) || (rc = b->row_stream.grow(rows)) || (rc = b->passes.grow(kGenGroup * (size_t)b->max_pass)) ||
         (rc = b->samp.grow(rows)) || (rc = b->stop_start.grow(rows + 1)) || (rc = b->out.grow(rows * kGenGroup)) ||
         (rc = b->u.grow(kGenGroup * rows))) {
@@ -2405,6 +2589,34 @@ int rwkv_b200_batcher_read_ex(rwkv_b200_batcher *b, unsigned long long id, unsig
     if (state_out) *state_out = q.gc.mask ? q.gc.state : 0;
     if (len) *len = q.tokens.size();
     if (status) *status = q.status;
+    return 0;
+}
+
+int rwkv_b200_batcher_submit_stop(rwkv_b200_batcher *b, const rwkv_b200_request *r, const rwkv_b200_request_ex *x,
+                                  unsigned long long set_id, unsigned long long start_state, unsigned long long *id) {
+    int rc = check_batcher(b);
+    if (rc) return rc;
+    const rwkv_b200_stop_request sq{&set_id, &start_state, nullptr, nullptr, nullptr};
+    std::vector<rk::GenStop> gst;
+    if ((rc = check_stops(b->m, "batcher_submit", &sq, 1, gst)) || (rc = rwkv_b200_batcher_submit_ex(b, r, x, id))) return rc;
+    if (gst[0].next) {
+        B::Req &q = b->reqs.at(*id);
+        q.gst = gst[0];
+        q.stop_set = set_id;
+    }
+    return 0;
+}
+
+int rwkv_b200_batcher_read_stop(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *hit, unsigned long long *tail,
+                                unsigned long long *state) {
+    int rc = check_batcher(b);
+    if (rc) return rc;
+    const auto it = b->reqs.find(id);
+    if (it == b->reqs.end()) return fail(1, "batcher_read_stop: request %llu is unknown or released", id);
+    const rk::GenStop &g = it->second.gst;
+    if (hit) *hit = g.next ? g.match : 0;
+    if (tail) *tail = g.next ? g.tail : 0;
+    if (state) *state = g.next ? g.state : 0;
     return 0;
 }
 

@@ -8,7 +8,8 @@
 // finishes inside a group keeps its row until the group ends but is frozen: its slot is not written again.
 // generate_streams_logprobs adds k_gen_logprob (score.cuh) between the pick and k_gen_feedback.
 // generate_streams_constrained adds k_gen_mask after the overrides, and k_gen_feedback advances each constrained
-// stream's token automaton (GenConstraint) after appending its token.
+// stream's token automaton (GenConstraint) after appending its token. generate_streams_stop has k_gen_feedback walk each
+// emitted token's bytes through the stream's stop-string automaton (GenStop) as well.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -16,6 +17,7 @@
 #include "../../include/rwkv_b200.h"
 #include "common.cuh"
 #include "prefill.cuh"
+#include "stopmatch.h"
 
 namespace rk {
 
@@ -76,6 +78,29 @@ __global__ void __launch_bounds__(kMaskThreads) k_gen_mask(float *logits, int V,
     if (!((c.mask[c.state * kMaskWords + (v >> 5)] >> (v & 31)) & 1u)) logits[(size_t)r * V + v] = -INFINITY;
 }
 
+// A stream's stop set (include/rwkv_b200.h, rwkv_b200_stop_set_add): the set's byte automaton (stopmatch.h), the model's
+// token bytes (token v is bytes[tb_start[v] .. tb_start[v + 1])), the current state, and once a string matched, its hit
+// (1 + the string's index) and the bytes of the last token after the match. next == nullptr: the stream has no set.
+struct GenStop {
+    const uint32_t *next, *hit;       // [states][256], [states]
+    const unsigned long long *tb_start; // [V + 1]
+    const unsigned char *tb_bytes;
+    unsigned long long state, match, tail;
+};
+
+// Walk the bytes of emitted token tok through the stream's stop automaton; true when a stop string ends in them.
+__device__ __forceinline__ bool gen_stop_walk(GenStop &m, unsigned long long tok) {
+    const unsigned long long b0 = m.tb_start[tok];
+    uint32_t q = (uint32_t)m.state;
+    unsigned long long tail = 0;
+    const uint32_t h = stopmatch::walk(m.next, m.hit, q, m.tb_bytes + b0, m.tb_start[tok + 1] - b0, tail);
+    m.state = q;
+    if (!h) return false;
+    m.match = h;
+    m.tail = tail;
+    return true;
+}
+
 struct GenFeedbackArgs {
     GenStream *gs;
     const int *row_stream;           // [rows] stream of each row
@@ -92,6 +117,7 @@ struct GenFeedbackArgs {
     // the batcher: stream s's own stop tokens are stop[stop_start[s] .. stop_start[s + 1]) (n_stop is not read);
     // nullptr: stop[0 .. n_stop) for every stream
     const unsigned long long *stop_start;
+    GenStop *gst; // [n_streams] generate_streams_stop and batcher lanes with stop sets, else nullptr
 };
 
 // One thread per row: emit the picked token of a live stream, then write the next step's input. On the tensor-core
@@ -139,6 +165,7 @@ __global__ void k_gen_feedback(const GenFeedbackArgs a) {
                 stop = true;
             }
         }
+        if (a.gst && a.gst[s].next) stop |= gen_stop_walk(a.gst[s], tok);
         g.done = stop ? 1ull : 0ull;
         a.gs[s] = g;
     }

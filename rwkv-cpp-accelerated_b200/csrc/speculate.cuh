@@ -19,6 +19,7 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "generate.cuh"
 #include "prefill.cuh"
 
 namespace rk {
@@ -51,6 +52,7 @@ struct SpecArgs {
     const unsigned long long *stop;  // [n_stop]
     int n_stop;
     unsigned long long *out;         // [n_streams][max_new]
+    GenStop *gst;                    // [n_streams] generate_streams_speculative_stop, else nullptr
 };
 
 // Draft rule: for n = ngram down to 1 with n < L, the largest j <= L - n - 1 with h[j .. j + n) == h[L - n .. L); the
@@ -100,7 +102,8 @@ __global__ void __launch_bounds__(kSpecDraftThreads) k_spec_draft(const SpecArgs
 }
 
 // One warp per live stream: lane i holds the pick p_i of row i; a = the leading i in 1..k with row[i] == p_{i - 1}.
-// Lane 0 emits p_0 .. p_a with generate_streams' stop and budget check and moves home to the slot of the last row used.
+// Lane 0 emits p_0 .. p_a with generate_streams' stop, stop-string and budget checks and moves home to the slot of the
+// last row used.
 __global__ void __launch_bounds__(32) k_spec_accept(const SpecArgs a) {
     const int li = blockIdx.x, s = a.live[li], lane = threadIdx.x, k = a.k;
     SpecStream &g = a.ss[s];
@@ -127,6 +130,7 @@ __global__ void __launch_bounds__(32) k_spec_accept(const SpecArgs a) {
         e = i;
         stop = len == g.budget;
         for (int z = 0; z < a.n_stop; ++z) stop |= a.stop[z] == tok;
+        if (a.gst && a.gst[s].next) stop |= gen_stop_walk(a.gst[s], tok);
     }
     g.len = len;
     g.hl = hl;

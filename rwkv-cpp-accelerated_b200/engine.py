@@ -15,6 +15,8 @@ MAX_TOP_N = 20                  # RWKV_B200_MAX_TOP_N
 LOGPROBS_RAW, LOGPROBS_PROCESSED = 0, 1  # RWKV_B200_LOGPROBS_*: the row generate_streams(logprobs=...) scores on
 NO_CONSTRAINT = 0xFFFFFFFFFFFFFFFF       # RWKV_B200_NO_CONSTRAINT: a stream of a constrained call without an automaton
 MAX_CONSTRAINT_STATES = 65536            # RWKV_B200_MAX_CONSTRAINT_STATES
+NO_STOP_SET = 0xFFFFFFFFFFFFFFFF         # RWKV_B200_NO_STOP_SET: a stream of a stop-string call without a set
+MAX_STOP_BYTES = 4096                    # RWKV_B200_MAX_STOP_BYTES
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
@@ -52,7 +54,84 @@ class RequestEx(ctypes.Structure):
                 ("top_n", ctypes.c_uint)]
 
 
+class StopRequest(ctypes.Structure):
+    """rwkv_b200_stop_request: per stream its stop set id and start state, and where the results go."""
+    P = ctypes.POINTER(ctypes.c_ulonglong)
+    _fields_ = [("set_ids", P), ("start_states", P), ("states_out", P), ("hit_out", P), ("tail_out", P)]
+
+
 REQ_STATUS = ("queued", "prefilling", "generating", "done", "cancelled")  # RWKV_B200_REQ_* in order
+
+
+def _stop_strings(strings):
+    """One str (UTF-8) or bytes, or a sequence of them, as a list of bytes."""
+    items = [strings] if isinstance(strings, (str, bytes, bytearray)) else list(strings)
+    enc = []
+    for s in items:
+        if isinstance(s, str):
+            enc.append(s.encode("utf-8"))
+        elif isinstance(s, (bytes, bytearray)):
+            enc.append(bytes(s))
+        else:
+            raise EngineError("stop strings are str or bytes, not %r" % type(s).__name__)
+    return enc
+
+
+def stop_set_bytes(strings):
+    """A stop set as rwkv_b200_stop_set_add takes it: (string_start [n + 1] uint64, bytes uint8). strings: one str
+    (UTF-8) or bytes, or a sequence of them."""
+    enc = _stop_strings(strings)
+    start = np.ascontiguousarray(np.cumsum([0] + [len(s) for s in enc]), dtype=np.uint64)
+    return start, np.frombuffer(b"".join(enc) or b"\0", np.uint8).copy()
+
+
+def stop_spec(spec, S, what):
+    """stop_strings of a generate call as (set ids [S], start states [S]): one set id for every stream, or one entry per
+    stream: an id, (id, start_state) or None."""
+    items = [spec] * S if isinstance(spec, (int, np.integer)) else list(spec)
+    if len(items) != S:
+        raise EngineError("%s: %d stop_strings entries for %d streams" % (what, len(items), S))
+    pairs = [(NO_STOP_SET, 0) if c is None else (int(c[0]), int(c[1])) if isinstance(c, (tuple, list)) else (int(c), 0)
+             for c in items]
+    return (np.ascontiguousarray([c for c, _ in pairs], np.uint64), np.ascontiguousarray([q for _, q in pairs], np.uint64))
+
+
+def stop_prefixes(strings):
+    """The match states of a stop set (include/rwkv_b200.h, "Stop strings"): state q stands for prefixes[q], the q-th
+    distinct prefix of the strings in order of first appearance (the empty prefix first)."""
+    out, seen = [b""], {b""}
+    for s in _stop_strings(strings):
+        for k in range(1, len(s) + 1):
+            if s[:k] not in seen:
+                seen.add(s[:k])
+                out.append(s[:k])
+    return out
+
+
+def stop_match(strings, chunks, state=0):
+    """The stop-string rule restated on the host: walk chunks (the bytes of each emitted token, in order) from match
+    state `state`. Returns (j, hit, tail, state): j the index of the first chunk in which a string ends (None if none
+    does), hit the index of that string (the lowest among those ending at the same byte), tail the bytes of chunk j
+    after it, and the match state after the last byte walked."""
+    enc = _stop_strings(strings)
+    pre = stop_prefixes(enc)
+    index = {p: q for q, p in enumerate(pre)}
+    keep = max(len(s) for s in enc)
+    text = pre[state]
+    for j, chunk in enumerate(chunks):
+        chunk = bytes(chunk)
+        for i in range(len(chunk)):
+            text = (text + chunk[i:i + 1])[-keep:]
+            ends = [k for k, s in enumerate(enc) if text.endswith(s)]
+            if ends:
+                return j, ends[0], len(chunk) - i - 1, index[_longest_prefix(text, index)]
+    return None, None, 0, index[_longest_prefix(text, index)]
+
+
+def _longest_prefix(text, index):
+    for k in range(len(text) + 1):
+        if text[k:] in index:
+            return text[k:]
 
 
 def _samplers(spec, n):
@@ -202,6 +281,17 @@ def load_library():
         "rwkv_b200_batcher_run": (i32, [vp, ull, pull]),
         "rwkv_b200_batcher_read": (i32, [vp, ull, pull, ull, pull, c.POINTER(i32)]),
         "rwkv_b200_batcher_read_ex": (i32, [vp, ull, ull, pull, pdbl, pull, pull, pdbl, pull, pull, c.POINTER(i32)]),
+        "rwkv_b200_token_bytes_set": (i32, [vp, pull, c.POINTER(c.c_ubyte)]),
+        "rwkv_b200_stop_set_add": (i32, [vp, ull, pull, c.POINTER(c.c_ubyte), pull]),
+        "rwkv_b200_stop_set_remove": (i32, [vp, ull]),
+        "rwkv_b200_generate_streams_stop": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull,
+                                                  c.POINTER(Sampler), pdbl, pull, pull, i32, c.c_uint, pdbl, pull, pull,
+                                                  pdbl, pull, pull, pull, c.POINTER(StopRequest)]),
+        "rwkv_b200_generate_streams_speculative_stop": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull,
+                                                              c.POINTER(Sampler), pdbl, pull, pull, c.c_uint, c.c_uint,
+                                                              pull, pull, pull, c.POINTER(StopRequest)]),
+        "rwkv_b200_batcher_submit_stop": (i32, [vp, c.POINTER(Request), c.POINTER(RequestEx), ull, ull, pull]),
+        "rwkv_b200_batcher_read_stop": (i32, [vp, ull, pull, pull, pull]),
         "rwkv_b200_batcher_cancel": (i32, [vp, ull]),
         "rwkv_b200_batcher_release": (i32, [vp, ull]),
         "rwkv_b200_batcher_close": (None, [vp]),
@@ -350,7 +440,7 @@ class Engine:
         return toks, margins
 
     def generate_streams(self, streams, max_new, budgets=None, stop=(), overrides=None, temp=None, u=None, sampling=None,
-                         logprobs=None, top_n=0, constraints=None):
+                         logprobs=None, top_n=0, constraints=None, stop_strings=None):
         """Generate up to max_new tokens per stream on the device: streams = [(slot, first_token), ...].
         Arg-max when u is None, else the typical sampler with u[step][stream] and temp (default 1.0). budgets: tokens
         per stream (None = max_new each); stop: token ids that end a stream (emitted, not fed); overrides = {token:
@@ -366,10 +456,15 @@ class Engine:
         None (rwkv_b200_generate_streams_constrained: each step masks every token without an edge out of the stream's
         automaton state, and a stream ends when its state has no edges). Then it returns one dict per stream with
         "tokens" and "state" (the final automaton state, None without a constraint), plus the logprob fields when
-        logprobs is given. Like logprobs, constraints need sampling=... or the arg-max (not the typical sampler)."""
-        if logprobs is not None or constraints is not None:
+        logprobs is given. Like logprobs, constraints need sampling=... or the arg-max (not the typical sampler).
+        stop_strings: one id of add_stop_set for every stream, or one entry per stream: an id, (id, start_state) or None
+        (rwkv_b200_generate_streams_stop: a stream ends after the token whose bytes complete one of its set's strings).
+        Then it returns one dict per stream with "tokens", "stop_hit" (the index of the matched string, or None),
+        "stop_tail" (bytes of the last token after the match) and "stop_state" (the final match state, None without a
+        set), plus the logprob and constraint fields when those are given. It needs sampling=... or the arg-max too."""
+        if logprobs is not None or constraints is not None or stop_strings is not None:
             return self._generate_scored(streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n,
-                                         constraints)
+                                         constraints, stop_strings)
         temp = 1.0 if temp is None else temp
         S, lead, tail, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u)
         if sampling is not None:
@@ -379,13 +474,18 @@ class Engine:
             self._ck(self.lib.rwkv_b200_generate_streams(self.h, *lead, temp, *tail), "generate_streams")
         return [out[s, :int(lens[s])].copy() for s in range(S)]
 
-    def _generate_scored(self, streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n, constraints):
-        """generate_streams with logprobs or constraints: rwkv_b200_generate_streams_constrained when constraints are
-        given, else rwkv_b200_generate_streams_logprobs. One dict per stream."""
+    def _generate_scored(self, streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n, constraints,
+                         stop_strings=None):
+        """generate_streams with logprobs, constraints or stop strings: rwkv_b200_generate_streams_stop with stop
+        strings, rwkv_b200_generate_streams_constrained with constraints, else rwkv_b200_generate_streams_logprobs. One
+        dict per stream."""
         modes = {None: LOGPROBS_RAW, "raw": LOGPROBS_RAW, "processed": LOGPROBS_PROCESSED}
         if logprobs not in modes:
             raise EngineError("generate_streams: logprobs must be 'raw' or 'processed', not %r" % (logprobs,))
         if sampling is None and (u is not None or temp is not None):
+            if stop_strings is not None:
+                raise EngineError("generate_streams: stop_strings need sampling=... (or neither u nor temp, for the "
+                                  "arg-max); the typical sampler does not take them")
             if constraints is not None:
                 raise EngineError("generate_streams: constraints need sampling=... (or neither u nor temp, for the "
                                   "arg-max); the typical sampler does not take them")
@@ -403,9 +503,8 @@ class Engine:
         sp = _samplers(sampling, S) if sampling is not None else None
         args = (self.h, *lead, sp, *tail, modes[logprobs], int(top_n), _ptr(lp, ctypes.c_double), _ptr(ranks, P),
                 _ptr(top_tok, P), _ptr(top_lp, ctypes.c_double))
-        if constraints is None:
-            self._ck(self.lib.rwkv_b200_generate_streams_logprobs(*args), "generate_streams_logprobs")
-        else:
+        ids = starts = states = None
+        if constraints is not None:
             spec = [constraints] * S if isinstance(constraints, (int, np.integer)) else list(constraints)
             if len(spec) != S:
                 raise EngineError("generate_streams: %d constraints for %d streams" % (len(spec), S))
@@ -414,12 +513,20 @@ class Engine:
             ids = np.ascontiguousarray([c for c, _ in pairs], np.uint64)
             starts = np.ascontiguousarray([q for _, q in pairs], np.uint64)
             states = np.zeros(S, np.uint64)
-            self._ck(self.lib.rwkv_b200_generate_streams_constrained(*args, _ptr(ids, P), _ptr(starts, P), _ptr(states, P)),
-                     "generate_streams_constrained")
+        cargs = (_ptr(ids, P), _ptr(starts, P), _ptr(states, P))
+        if stop_strings is not None:
+            sreq, sres = self._stop_request(stop_strings, S, "generate_streams")
+            self._ck(self.lib.rwkv_b200_generate_streams_stop(*args, *cargs, ctypes.byref(sreq)), "generate_streams_stop")
+        elif constraints is not None:
+            self._ck(self.lib.rwkv_b200_generate_streams_constrained(*args, *cargs), "generate_streams_constrained")
+        else:
+            self._ck(self.lib.rwkv_b200_generate_streams_logprobs(*args), "generate_streams_logprobs")
         res = []
         for s in range(S):
             n = int(lens[s])
             d = {"tokens": out[s, :n].copy()}
+            if stop_strings is not None:
+                d.update(sres(s))
             if constraints is not None:
                 d["state"] = int(states[s]) if ids[s] != np.uint64(NO_CONSTRAINT) else None
             if lp is not None:
@@ -443,6 +550,43 @@ class Engine:
 
     def remove_constraint(self, cid):
         self._ck(self.lib.rwkv_b200_constraint_remove(self.h, int(cid)), "constraint_remove")
+
+    def add_stop_set(self, strings):
+        """Upload a stop set (one str (UTF-8) or bytes, or a sequence of them) for generate_streams(stop_strings=...),
+        generate_speculative and Batcher.submit; returns its id. The first set also uploads the token bytes
+        (constrain.token_bytes()) that the device walks."""
+        if not getattr(self, "_token_bytes", False):
+            from . import constrain
+            tb = constrain.token_bytes()
+            start = np.ascontiguousarray(np.cumsum([0] + [len(b) for b in tb]), dtype=np.uint64)
+            data = np.frombuffer(b"".join(tb), np.uint8).copy()
+            self._ck(self.lib.rwkv_b200_token_bytes_set(self.h, _ptr(start, ctypes.c_ulonglong), _ptr(data, ctypes.c_ubyte)),
+                     "token_bytes_set")
+            self._token_bytes = True
+        start, data = stop_set_bytes(strings)
+        sid = ctypes.c_ulonglong()
+        self._ck(self.lib.rwkv_b200_stop_set_add(self.h, len(start) - 1, _ptr(start, ctypes.c_ulonglong),
+                                                 _ptr(data, ctypes.c_ubyte), ctypes.byref(sid)), "stop_set_add")
+        return int(sid.value)
+
+    def remove_stop_set(self, sid):
+        self._ck(self.lib.rwkv_b200_stop_set_remove(self.h, int(sid)), "stop_set_remove")
+
+    @staticmethod
+    def _stop_request(stop_strings, S, what):
+        """(StopRequest, result(s) -> dict of "stop_hit", "stop_tail", "stop_state") of stop_strings for S streams."""
+        ids, starts = stop_spec(stop_strings, S, what)
+        out = [np.zeros(S, np.uint64) for _ in range(3)]
+        P = ctypes.c_ulonglong
+        req = StopRequest(_ptr(ids, P), _ptr(starts, P), *[_ptr(a, P) for a in out])
+        req._keep = (ids, starts, out)
+        state, hit, tail = out
+
+        def result(s):
+            on = ids[s] != np.uint64(NO_STOP_SET)
+            return {"stop_hit": int(hit[s]) - 1 if hit[s] else None, "stop_tail": int(tail[s]),
+                    "stop_state": int(state[s]) if on else None}
+        return req, result
 
     def score_streams(self, streams, targets=None, top_n=0):
         """Score target tokens in one ragged forward: streams = [(slot, tokens), ...], each advancing its own state slot
@@ -522,12 +666,13 @@ class Engine:
         return res
 
     def generate_speculative(self, streams, max_new, draft, ngram=3, context=None, budgets=None, stop=(), overrides=None,
-                             sampling=None, u=None):
+                             sampling=None, u=None, stop_strings=None):
         """generate_streams(sampling=...) with prompt-lookup drafts (rwkv_b200_generate_streams_speculative): the same
         tokens and first-slot states, several tokens per step where the drafts are right. streams = [(slots, first_token),
         ...], each with draft + 1 distinct slots, the first holding the conversation (the others are scratch). context:
         None, or one token list (or None) per stream of extra lookup tokens. sampling None is the arg-max. Returns one
-        dict per stream: "tokens" (uint64) and "steps" (the steps that emitted a token)."""
+        dict per stream: "tokens" (uint64) and "steps" (the steps that emitted a token). stop_strings as in
+        generate_streams (rwkv_b200_generate_streams_speculative_stop) adds "stop_hit", "stop_tail" and "stop_state"."""
         if any(len(slots) != draft + 1 for slots, _ in streams):
             raise EngineError("generate_speculative: every stream needs draft + 1 = %d slots" % (draft + 1))
         S, lead, tail, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u,
@@ -542,10 +687,14 @@ class Engine:
             ctx = np.ascontiguousarray([x for c in seqs for x in c], dtype=np.uint64)
         sp = _samplers(sampling, S) if sampling is not None else None
         P = ctypes.c_ulonglong
-        self._ck(self.lib.rwkv_b200_generate_streams_speculative(self.h, *lead, sp, *tail, int(draft), int(ngram),
-                                                                 _ptr(cstart, P), _ptr(ctx, P), _ptr(steps, P)),
-                 "generate_streams_speculative")
-        return [{"tokens": out[s, :int(lens[s])].copy(), "steps": int(steps[s])} for s in range(S)]
+        args = (self.h, *lead, sp, *tail, int(draft), int(ngram), _ptr(cstart, P), _ptr(ctx, P), _ptr(steps, P))
+        if stop_strings is None:
+            self._ck(self.lib.rwkv_b200_generate_streams_speculative(*args), "generate_streams_speculative")
+            return [{"tokens": out[s, :int(lens[s])].copy(), "steps": int(steps[s])} for s in range(S)]
+        sreq, sres = self._stop_request(stop_strings, S, "generate_speculative")
+        self._ck(self.lib.rwkv_b200_generate_streams_speculative_stop(*args, ctypes.byref(sreq)),
+                 "generate_streams_speculative_stop")
+        return [dict({"tokens": out[s, :int(lens[s])].copy(), "steps": int(steps[s])}, **sres(s)) for s in range(S)]
 
     def batcher(self, rows, prefill_tokens):
         """Continuous batching (include/rwkv_b200.h, rwkv_b200_batcher_open): a Batcher with at most `rows` admitted
@@ -652,14 +801,16 @@ class Batcher:
                    "batcher_open")
         self.h = h
         self._ext = {}  # id -> (top_n or None without log-probabilities, constrained) of requests sent through submit_ex
+        self._stop = set()  # ids of requests with a stop set
 
     def submit(self, slot, prompt, max_new, sampling=None, u=None, stop=(), overrides=None, constraint=None, logprobs=None,
-               top_n=0):
+               top_n=0, stop_strings=None):
         """Queue a request on state slot `slot`: prompt (>= 1 token ids), up to max_new new tokens, a Sampler or dict
         (None: arg-max), u: max_new uniforms in [0, 1) (None only at temperature 0), stop: this request's stop tokens.
         overrides = {token: logit value} as in generate_streams; constraint: an id of Engine.add_constraint, or (id,
         start_state); logprobs = "raw" or "processed" scores every emitted token, with top_n top entries (read them with
-        result). Returns its id. Every array is copied."""
+        result); stop_strings: an id of Engine.add_stop_set, or (id, start_state). Returns its id. Every array is
+        copied."""
         sp = _samplers(sampling if sampling is not None else Sampler(temperature=0.0), 1)[0]
         pr = np.ascontiguousarray(np.atleast_1d(np.asarray(prompt, dtype=np.uint64)))
         st = np.ascontiguousarray(list(stop), dtype=np.uint64)
@@ -669,8 +820,15 @@ class Batcher:
         P = ctypes.c_ulonglong
         req = Request(int(slot), _ptr(pr, P), len(pr), int(max_new), sp, _ptr(us, ctypes.c_double), _ptr(st, P), len(st))
         rid = ctypes.c_ulonglong()
-        if overrides is None and constraint is None and logprobs is None:
+        plain = overrides is None and constraint is None and logprobs is None
+        if plain and stop_strings is None:
             self.engine._ck(self.lib.rwkv_b200_batcher_submit(self.h, ctypes.byref(req), ctypes.byref(rid)), "batcher_submit")
+            return int(rid.value)
+        if plain:
+            ids, starts = stop_spec([stop_strings], 1, "batcher.submit")
+            self.engine._ck(self.lib.rwkv_b200_batcher_submit_stop(self.h, ctypes.byref(req), None, int(ids[0]),
+                                                                   int(starts[0]), ctypes.byref(rid)), "batcher_submit")
+            self._stop.add(int(rid.value))
             return int(rid.value)
         modes = {None: LOGPROBS_RAW, "raw": LOGPROBS_RAW, "processed": LOGPROBS_PROCESSED}
         if logprobs not in modes:
@@ -683,8 +841,14 @@ class Batcher:
             cid, q0 = (int(constraint[0]), int(constraint[1])) if isinstance(constraint, (tuple, list)) else (int(constraint), 0)
         x = RequestEx(_ptr(otok, P), _ptr(oval, ctypes.c_float), len(otok), cid, q0, 1 if logprobs is not None else 0,
                       modes[logprobs], int(top_n))
-        self.engine._ck(self.lib.rwkv_b200_batcher_submit_ex(self.h, ctypes.byref(req), ctypes.byref(x), ctypes.byref(rid)),
-                        "batcher_submit")
+        if stop_strings is None:
+            self.engine._ck(self.lib.rwkv_b200_batcher_submit_ex(self.h, ctypes.byref(req), ctypes.byref(x),
+                                                                 ctypes.byref(rid)), "batcher_submit")
+        else:
+            ids, starts = stop_spec([stop_strings], 1, "batcher.submit")
+            self.engine._ck(self.lib.rwkv_b200_batcher_submit_stop(self.h, ctypes.byref(req), ctypes.byref(x), int(ids[0]),
+                                                                   int(starts[0]), ctypes.byref(rid)), "batcher_submit")
+            self._stop.add(int(rid.value))
         self._ext[int(rid.value)] = (int(top_n) if logprobs is not None else None, constraint is not None)
         return int(rid.value)
 
@@ -708,7 +872,8 @@ class Batcher:
         """Everything a request has produced so far, as a dict: "tokens" (np.uint64) and "status" (one of REQ_STATUS);
         with logprobs "logprobs" (float64) and "ranks" (uint64), and with top_n > 0 "top_tokens" / "top_logprobs"
         [len][top_n], as generate_streams(logprobs=...) returns them; with a constraint "state" (the automaton's
-        current state)."""
+        current state); with a stop set "stop_hit", "stop_tail" and "stop_state" as generate_streams(stop_strings=...)
+        returns them."""
         top_n, constrained = self._ext.get(int(rid), (None, False))
         n, status = ctypes.c_ulonglong(), ctypes.c_int()
         self.engine._ck(self.lib.rwkv_b200_batcher_read(self.h, int(rid), None, 0, ctypes.byref(n), ctypes.byref(status)),
@@ -731,6 +896,12 @@ class Batcher:
                 d["top_tokens"], d["top_logprobs"] = top_tok, top_lp
         if constrained:
             d["state"] = int(state.value)
+        if int(rid) in self._stop:
+            hit, tail, mstate = ctypes.c_ulonglong(), ctypes.c_ulonglong(), ctypes.c_ulonglong()
+            self.engine._ck(self.lib.rwkv_b200_batcher_read_stop(self.h, int(rid), ctypes.byref(hit), ctypes.byref(tail),
+                                                                 ctypes.byref(mstate)), "batcher_read_stop")
+            d.update(stop_hit=int(hit.value) - 1 if hit.value else None, stop_tail=int(tail.value),
+                     stop_state=int(mstate.value))
         return d
 
     def cancel(self, rid):
@@ -739,6 +910,7 @@ class Batcher:
     def release(self, rid):
         self.engine._ck(self.lib.rwkv_b200_batcher_release(self.h, int(rid)), "batcher_release")
         self._ext.pop(int(rid), None)
+        self._stop.discard(int(rid))
 
     def close(self):
         if getattr(self, "h", None) and getattr(self.engine, "h", None):
