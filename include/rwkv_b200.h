@@ -682,6 +682,43 @@ int rwkv_b200_generate_streams_speculative_stop(rwkv_b200_model *m, const unsign
                                                 const unsigned long long *context_start, const unsigned long long *context,
                                                 unsigned long long *steps_out, const rwkv_b200_stop_request *stop);
 
+/* rwkv_b200_generate_streams_speculative_stop with log-probabilities and token automata: every argument up to steps_out
+ * is that call's, the rest are those of rwkv_b200_generate_streams_stop with the same meaning. The tokens, lengths, the
+ * first slots' xy, aa, bb and dd, logprobs_out, ranks_out, the top arrays, states_out and the stop hit, tail and state
+ * are bit for bit those of rwkv_b200_generate_streams_stop on the first slots with the same arguments, run on the tensor
+ * cores, whatever the drafts are; steps_out keeps the draft rule above. With logprobs_out == NULL and constraint_ids ==
+ * NULL the call is rwkv_b200_generate_streams_speculative_stop and enqueues the same launches.
+ * Rows of a constrained stream, q its automaton state at the start of a step: row 0 has state r_0 = q. For i = 1..k, row
+ * i is live when row i - 1 is live, d_i has an edge out of r_(i-1) and the target of that edge has edges; its state r_i
+ * is that target. The first row that fails this is dead, and so is every row after it. A live row is masked by its own
+ * state after the overrides, as rule 2 of constrained generation masks a row; a dead row is not masked. A dead row is
+ * never emitted: when d_i has no edge out of r_(i-1), the pick p_(i-1) on the masked row i - 1 is an allowed token, so
+ * p_(i-1) != d_i and the step stops before row i; when d_i completes the automaton, emitting it (as p_(i-1)) ends the
+ * stream. So every emitted row is masked exactly as generate_streams_constrained masks it, and no pick sees a row without
+ * a finite value (the override check below keeps the live rows open).
+ * Each emitted token runs through generate_streams_stop's checks in its order: the budget, the stop tokens, the automaton
+ * (advance; end on a state without edges; a token without an edge fails the call at the end of its 16-step group with
+ * generate_streams_constrained's message and code), then the stop strings. Emitted token p_i of a step is entry [s][len +
+ * i] of the log-probability arrays, scored on row i: raw mode on the model's row (a copy of the step's rows is taken
+ * before the overrides and masks when the call has either), processed mode on the row the pick read, divided by the
+ * stream's temperature. Rows that emit no token are not scored. Each step runs k_gen_mask with automata and one scoring
+ * kernel with logprobs_out.
+ * Refused before any work (every slot untouched): every refusal of rwkv_b200_generate_streams_speculative_stop
+ * (including presence and frequency penalties), those of rwkv_b200_generate_streams_logprobs with logprobs_out != NULL
+ * (the mode, top_n > RWKV_B200_MAX_TOP_N, missing top arrays), and those of rwkv_b200_generate_streams_constrained (an
+ * unknown or removed id, a start state out of range or without edges, overrides that set every edge token of a state to
+ * -inf). */
+int rwkv_b200_generate_streams_speculative_constrained(
+    rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens, unsigned long long n_streams,
+    unsigned long long max_new, const unsigned long long *budgets, const unsigned long long *stop_tokens,
+    unsigned long long n_stop, const unsigned long long *override_tokens, const float *override_values,
+    unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u, unsigned long long *tokens_out,
+    unsigned long long *lengths_out, unsigned int draft, unsigned int ngram, const unsigned long long *context_start,
+    const unsigned long long *context, unsigned long long *steps_out, int logprob_mode, unsigned int top_n,
+    double *logprobs_out, unsigned long long *ranks_out, unsigned long long *top_tokens_out, double *top_logprobs_out,
+    const unsigned long long *constraint_ids, const unsigned long long *start_states, unsigned long long *states_out,
+    const rwkv_b200_stop_request *stop);
+
 /* rwkv_b200_batcher_submit_ex (x may be NULL) with a stop set: set_id (RWKV_B200_NO_STOP_SET: exactly submit_ex) and its
  * start state. The batcher rule's step 2 becomes rwkv_b200_generate_streams_stop of the one stream with the set and start
  * state; a request whose stop string matches ends as RWKV_B200_REQ_DONE. Refused as well, with nothing queued: an unknown

@@ -183,8 +183,9 @@ struct rwkv_b200_model {
         DevBuf<int> n_hyp;                      // [G]
         DevBuf<unsigned long long> done, forks; // [G], [G * B][2]
     } beam;
-    // generate_streams_speculative: the streams' records, histories, live list, passes and per-row uniforms, grown with
-    // the largest call; the emitted tokens, stops, overrides and samplers use gen's buffers
+    // generate_streams_speculative: the streams' records, histories, live list, passes, per-row uniforms and automaton
+    // states, grown with the largest call; the emitted tokens, stops, overrides, samplers, automata, log-probabilities
+    // and the raw copy use gen's buffers
     struct Spec {
         DevBuf<rk::SpecStream> ss;        // [n_streams]
         DevBuf<unsigned long long> hist;  // per stream: context, first token, up to max_new emitted tokens
@@ -192,6 +193,7 @@ struct rwkv_b200_model {
         DevBuf<rk::PassDesc> passes;      // [passes of a step]
         DevBuf<double> u, row_u;          // [max_new][n_streams], [rows]
         DevBuf<unsigned long long> forks; // [n_streams][2] the final copies home -> first slot
+        DevBuf<unsigned long long> row_state; // [rows] each row's automaton state (constrained calls)
     } spec;
     rwkv_b200_batcher *batcher = nullptr; // the open batcher (at most one), closed by rwkv_b200_free
 };
@@ -1067,6 +1069,8 @@ struct PickChain {
     // the batcher: each row's own overrides, ovr_*[ovr_start[s] .. ovr_start[s + 1]) of its stream s (n_override > 0
     // only says that some row has one); nullptr: all n_override for every row
     const unsigned long long *ovr_start;
+    // speculative generation: the automaton state of each row (k_gen_mask's row_state); nullptr: each stream's state
+    const unsigned long long *row_state;
 };
 
 // The chain on rows 0..rows-1 of d_slogits; u: the step's uniforms, one per row (NULL: none).
@@ -1085,7 +1089,7 @@ int pick_rows(M *m, const PickChain &pc, int rows, const double *u) {
     }
     if (pc.gc) {
         const dim3 grid((unsigned)((V + rk::kMaskThreads - 1) / rk::kMaskThreads), (unsigned)rows);
-        rk::k_gen_mask<<<grid, rk::kMaskThreads, 0, m->stream>>>(m->d_slogits, (int)V, pc.gs, pc.row_stream, pc.gc);
+        rk::k_gen_mask<<<grid, rk::kMaskThreads, 0, m->stream>>>(m->d_slogits, (int)V, pc.gs, pc.row_stream, pc.gc, pc.row_state);
         LAUNCHED(m);
     }
     if (pc.samp)
@@ -2128,22 +2132,30 @@ int rwkv_b200_beam_search(rwkv_b200_model *m, const unsigned long long *slots, c
 }
 
 // Speculative generation: generate()'s group loop with k + 1 rows per live stream. Each step is k_spec_draft -> passes
-// -> pick_rows (overrides, pick) -> k_spec_accept; at each group's end the records come back and the finished streams
-// leave the rows. At the end a stream whose home is a spare has it copied to its first slot. With a stop request,
-// k_spec_accept also walks each emitted token through the stream's stop set.
-int rwkv_b200_generate_streams_speculative_stop(rwkv_b200_model *m, const unsigned long long *slots,
-                                                const unsigned long long *first_tokens, unsigned long long n_streams,
-                                                unsigned long long max_new, const unsigned long long *budgets,
-                                                const unsigned long long *stop_tokens, unsigned long long n_stop,
-                                                const unsigned long long *override_tokens, const float *override_values,
-                                                unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
-                                                unsigned long long *tokens_out, unsigned long long *lengths_out, unsigned int draft,
-                                                unsigned int ngram, const unsigned long long *context_start,
-                                                const unsigned long long *context, unsigned long long *steps_out,
-                                                const rwkv_b200_stop_request *sq) {
-    const char *what = sq ? "generate_streams_speculative_stop" : "generate_streams_speculative";
+// -> pick_rows (overrides, automaton masks, pick) -> k_spec_accept (-> k_spec_logprob); at each group's end the records
+// come back and the finished streams leave the rows. At the end a stream whose home is a spare has it copied to its first
+// slot. With a stop request, k_spec_accept also walks each emitted token through the stream's stop set; with token
+// automata, k_spec_draft gives each row its state and k_spec_accept advances the automaton; with logprobs_out, each
+// emitted token is scored after k_spec_accept.
+int rwkv_b200_generate_streams_speculative_constrained(
+    rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens, unsigned long long n_streams,
+    unsigned long long max_new, const unsigned long long *budgets, const unsigned long long *stop_tokens, unsigned long long n_stop,
+    const unsigned long long *override_tokens, const float *override_values, unsigned long long n_override,
+    const rwkv_b200_sampler *samplers, const double *u, unsigned long long *tokens_out, unsigned long long *lengths_out,
+    unsigned int draft, unsigned int ngram, const unsigned long long *context_start, const unsigned long long *context,
+    unsigned long long *steps_out, int logprob_mode, unsigned int top_n, double *logprobs_out, unsigned long long *ranks_out,
+    unsigned long long *top_tokens_out, double *top_logprobs_out, const unsigned long long *constraint_ids,
+    const unsigned long long *start_states, unsigned long long *states_out, const rwkv_b200_stop_request *sq) {
+    const char *what = logprobs_out || constraint_ids ? "generate_streams_speculative_constrained"
+                       : sq                           ? "generate_streams_speculative_stop"
+                                                      : "generate_streams_speculative";
     int rc = check_streams_model(m, what);
     if (rc) return rc;
+    if (logprobs_out) {
+        if ((rc = check_logprob_mode(what, logprob_mode, top_n))) return rc;
+        if (top_n && (!top_tokens_out || !top_logprobs_out))
+            return fail(1, "%s: top_n = %u needs top_tokens_out and top_logprobs_out", what, top_n);
+    }
     if (draft < 1 || draft > (unsigned)rk::kSpecMaxDraft) return fail(1, "%s: draft %u is outside 1..%d", what, draft, rk::kSpecMaxDraft);
     if (ngram < 1 || ngram > (unsigned)rk::kSpecMaxNgram) return fail(1, "%s: ngram %u is outside 1..%d", what, ngram, rk::kSpecMaxNgram);
     if (!rk::prefill_enabled(m->pf)) return fail(1, "%s: needs the tensor cores (the \"prefill\" option is 0)", what);
@@ -2169,6 +2181,10 @@ int rwkv_b200_generate_streams_speculative_stop(rwkv_b200_model *m, const unsign
         if (n_ctx && !context) return fail(1, "%s: %llu context tokens with NULL context", what, n_ctx);
         if ((rc = check_tokens(what, "context token", context, n_ctx))) return rc;
     }
+    std::vector<rk::GenConstraint> hgc;
+    const ConstraintRequest cq{constraint_ids, start_states, states_out};
+    if ((rc = check_constraints(m, what, cq, S, override_tokens, override_values, n_override, hgc))) return rc;
+    const bool constrained = std::any_of(hgc.begin(), hgc.end(), [](const rk::GenConstraint &gc) { return gc.mask != nullptr; });
     std::vector<rk::GenStop> hst;
     if ((rc = check_stops(m, what, sq, S, hst))) return rc;
     const bool stopped = std::any_of(hst.begin(), hst.end(), [](const rk::GenStop &st) { return st.next != nullptr; });
@@ -2177,6 +2193,13 @@ int rwkv_b200_generate_streams_speculative_stop(rwkv_b200_model *m, const unsign
     auto &g = m->gen;
     auto &sp = m->spec;
     if (stopped && (rc = g.gst.grow(S))) return rc;
+    if (constrained && ((rc = g.gc.grow(S)) || (rc = g.fault.grow(3)) || (rc = sp.row_state.grow(S * K1)))) return rc;
+    // raw mode reads the model's rows: d_slogits itself, or a copy taken before the overrides and masks edit it
+    const bool scored = logprobs_out != nullptr, raw_copy = scored && logprob_mode == RWKV_B200_LOGPROBS_RAW && (n_override || constrained);
+    const size_t n_lp = (size_t)(S * max_new), n_top = scored ? n_lp * top_n : 0;
+    if (scored && ((rc = g.lp.grow(n_lp)) || (rc = g.rank.grow(n_lp)) || (rc = g.top_tok.grow(n_top)) || (rc = g.top_lp.grow(n_top)) ||
+                   (raw_copy && (rc = g.raw.grow(S * K1 * binfmt::kVocab)))))
+        return rc;
     const int per_pass = rk::kPfMaxTokens / (int)K1; // streams per pass: a stream's rows never straddle two passes
     const size_t n_pass = (size_t)((S + per_pass - 1) / per_pass);
     if ((rc = sp.ss.grow(S)) || (rc = sp.hist.grow(n_hist)) || (rc = sp.live.grow(S)) || (rc = sp.passes.grow(n_pass)) ||
@@ -2205,13 +2228,41 @@ int rwkv_b200_generate_streams_speculative_stop(rwkv_b200_model *m, const unsign
     if ((rc = upload_gen(m, c))) return rc;
     if (u) CK(cudaMemcpyAsync(sp.u.p, u, max_new * S * sizeof(double), cudaMemcpyHostToDevice, m->stream));
     if (stopped) CK(cudaMemcpyAsync(g.gst.p, hst.data(), S * sizeof(rk::GenStop), cudaMemcpyHostToDevice, m->stream));
+    if (constrained) {
+        CK(cudaMemcpyAsync(g.gc.p, hgc.data(), S * sizeof(rk::GenConstraint), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemsetAsync(g.fault.p, 0, 3 * sizeof(unsigned long long), m->stream));
+    }
+    if (scored) { // all ones: NaN logprobs and RWKV_B200_NO_TARGET ranks and tokens wherever no token is emitted
+        CK(cudaMemsetAsync(g.lp.p, 0xFF, n_lp * sizeof(double), m->stream));
+        CK(cudaMemsetAsync(g.rank.p, 0xFF, n_lp * sizeof(unsigned long long), m->stream));
+        if (n_top) {
+            CK(cudaMemsetAsync(g.top_tok.p, 0xFF, n_top * sizeof(unsigned long long), m->stream));
+            CK(cudaMemsetAsync(g.top_lp.p, 0xFF, n_top * sizeof(double), m->stream));
+        }
+    }
 
     std::vector<int> live(S), rs;
     for (unsigned long long s = 0; s < S; ++s) live[s] = (int)s;
     rk::SpecArgs sa{sp.ss.p, sp.live.p, (int)draft, (int)ngram, per_pass, sp.hist.p, sp.passes.p, u ? sp.u.p : nullptr,
                     sp.row_u.p, S, max_new, samplers ? nullptr : m->d_next, m->d_sample, g.stop.p, (int)n_stop, g.out.p,
-                    stopped ? g.gst.p : nullptr};
-    const PickChain pc{nullptr, g.row_stream, samplers ? g.samp.p : nullptr, nullptr, nullptr, g.ovr_tok.p, g.ovr_val.p, n_override};
+                    stopped ? g.gst.p : nullptr, constrained ? g.gc.p : nullptr, sp.row_state.p, g.fault.p};
+    PickChain pc{nullptr, g.row_stream, samplers ? g.samp.p : nullptr, nullptr, nullptr, g.ovr_tok.p, g.ovr_val.p, n_override};
+    if (constrained) {
+        pc.gc = g.gc.p;
+        pc.row_state = sp.row_state.p;
+    }
+    rk::GenLogprobArgs la{};
+    if (scored) {
+        la.logits = raw_copy ? g.raw.p : m->d_slogits;
+        la.V = (int)binfmt::kVocab;
+        la.samp = logprob_mode == RWKV_B200_LOGPROBS_PROCESSED ? pc.samp : nullptr;
+        la.top_n = (int)top_n;
+        la.max_new = max_new;
+        la.logprob = g.lp.p;
+        la.rank = g.rank.p;
+        la.top_tokens = g.top_tok.p;
+        la.top_logprobs = g.top_lp.p;
+    }
     // each step emits at least one token per live stream, so max_new steps finish every stream
     for (unsigned long long step = 0; !live.empty() && step < max_new;) {
         const int n_live = (int)live.size(), rows = n_live * (int)K1;
@@ -2223,15 +2274,27 @@ int rwkv_b200_generate_streams_speculative_stop(rwkv_b200_model *m, const unsign
         for (unsigned long long k = 0; k < steps; ++k) {
             rk::k_spec_draft<<<(unsigned)n_live, rk::kSpecDraftThreads, 0, m->stream>>>(sa);
             LAUNCHED(m);
-            if ((rc = gen_step_passes(m, sp.passes.p, rows, per_pass * (int)K1)) ||
-                (rc = pick_rows(m, pc, rows, u ? sp.row_u.p : nullptr)))
-                return rc;
+            if ((rc = gen_step_passes(m, sp.passes.p, rows, per_pass * (int)K1))) return rc;
+            if (raw_copy)
+                CK(cudaMemcpyAsync(g.raw.p, m->d_slogits, (size_t)rows * binfmt::kVocab * sizeof(float), cudaMemcpyDeviceToDevice,
+                                   m->stream));
+            if ((rc = pick_rows(m, pc, rows, u ? sp.row_u.p : nullptr))) return rc;
             rk::k_spec_accept<<<(unsigned)n_live, 32, 0, m->stream>>>(sa);
             LAUNCHED(m);
+            if (scored) {
+                rk::k_spec_logprob<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(sa, la);
+                LAUNCHED(m);
+            }
         }
-        // the end of a group: which streams are done (one synchronisation); drop them from the rows
+        // the end of a group: which streams are done and any token without an edge (one synchronisation); drop the
+        // finished streams from the rows
         CK(cudaMemcpyAsync(hs.data(), sp.ss.p, S * sizeof(rk::SpecStream), cudaMemcpyDeviceToHost, m->stream));
+        unsigned long long fault[3] = {0, 0, 0};
+        if (constrained) CK(cudaMemcpyAsync(fault, g.fault.p, sizeof(fault), cudaMemcpyDeviceToHost, m->stream));
         SYNC(m);
+        if (fault[0])
+            return fail(8, "%s: stream %llu emitted token %llu, which has no edge out of state %llu of its constraint", what,
+                        fault[0] - 1, fault[1], fault[2]);
         step += steps;
         live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hs[s].done != 0; }), live.end());
     }
@@ -2247,14 +2310,42 @@ int rwkv_b200_generate_streams_speculative_stop(rwkv_b200_model *m, const unsign
         if ((rc = fork_slots(m, sp.forks.p, forks.size() / 2, false))) return rc;
     }
     CK(cudaMemcpyAsync(tokens_out, g.out.p, S * max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+    if (scored) {
+        CK(cudaMemcpyAsync(logprobs_out, g.lp.p, n_lp * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+        if (ranks_out) CK(cudaMemcpyAsync(ranks_out, g.rank.p, n_lp * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+        if (n_top) {
+            CK(cudaMemcpyAsync(top_tokens_out, g.top_tok.p, n_top * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+            CK(cudaMemcpyAsync(top_logprobs_out, g.top_lp.p, n_top * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+        }
+    }
+    if (constrained && states_out)
+        CK(cudaMemcpyAsync(hgc.data(), g.gc.p, S * sizeof(rk::GenConstraint), cudaMemcpyDeviceToHost, m->stream));
     if (stopped) CK(cudaMemcpyAsync(hst.data(), g.gst.p, S * sizeof(rk::GenStop), cudaMemcpyDeviceToHost, m->stream));
     SYNC(m);
     for (unsigned long long s = 0; s < S; ++s) {
         lengths_out[s] = hs[s].len;
         steps_out[s] = hs[s].steps;
     }
+    if (states_out)
+        for (unsigned long long s = 0; s < S; ++s) states_out[s] = hgc[s].mask ? hgc[s].state : 0;
     write_stops(sq, hst);
     return 0;
+}
+
+int rwkv_b200_generate_streams_speculative_stop(rwkv_b200_model *m, const unsigned long long *slots,
+                                                const unsigned long long *first_tokens, unsigned long long n_streams,
+                                                unsigned long long max_new, const unsigned long long *budgets,
+                                                const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                                const unsigned long long *override_tokens, const float *override_values,
+                                                unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
+                                                unsigned long long *tokens_out, unsigned long long *lengths_out, unsigned int draft,
+                                                unsigned int ngram, const unsigned long long *context_start,
+                                                const unsigned long long *context, unsigned long long *steps_out,
+                                                const rwkv_b200_stop_request *sq) {
+    return rwkv_b200_generate_streams_speculative_constrained(
+        m, slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values, n_override,
+        samplers, u, tokens_out, lengths_out, draft, ngram, context_start, context, steps_out, RWKV_B200_LOGPROBS_RAW, 0, nullptr,
+        nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, sq);
 }
 
 int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,

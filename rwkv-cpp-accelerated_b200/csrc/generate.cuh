@@ -64,18 +64,60 @@ struct GenConstraint {
     unsigned long long state;
 };
 
+// No state: a missing edge, and the per-row state of a row that is not masked (k_gen_mask's row_state).
+constexpr unsigned long long kNoState = ~0ull;
+
+// The target of token tok's edge out of state q, or kNoState when q has no edge for tok: a binary search over q's
+// ascending edge tokens.
+__device__ __forceinline__ unsigned long long gen_edge(const GenConstraint &c, unsigned long long q, unsigned long long tok) {
+    const unsigned long long end = c.start[q + 1];
+    unsigned long long lo = c.start[q], hi = end;
+    while (lo < hi) {
+        const unsigned long long mid = (lo + hi) / 2;
+        if (c.tok[mid] < tok) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo < end && c.tok[lo] == tok ? (unsigned long long)c.next[lo] : kNoState;
+}
+
+// Advance a constrained stream's automaton by its emitted token tok; true when that ends the stream: the new state has
+// no edges (complete), or tok has no edge. The mask makes a missing edge impossible unless the pick broke its contract:
+// the first one is recorded in fault {s + 1, token, state} for the host.
+__device__ __forceinline__ bool gen_constraint_step(GenConstraint &c, unsigned long long tok, int s, unsigned long long *fault) {
+    const unsigned long long q = c.state, q2 = gen_edge(c, q, tok);
+    if (q2 != kNoState) {
+        c.state = q2;
+        return c.start[q2] == c.start[q2 + 1];
+    }
+    if (atomicCAS(fault, 0ull, (unsigned long long)s + 1) == 0ull) {
+        fault[1] = tok;
+        fault[2] = q;
+    }
+    return true;
+}
+
 // logits[r][v] = -inf for every token v without an edge out of the current state of row r's stream. Grid
 // (ceil(V / kMaskThreads), rows), one thread per token. Unconstrained and finished streams are left alone: a finished
-// stream may sit in a state without edges, and masking its row would leave the pick no finite value.
+// stream may sit in a state without edges, and masking its row would leave the pick no finite value. With row_state
+// (speculative generation), row r is masked by state row_state[r] of its stream's automaton instead, and left alone
+// where that is kNoState; gs is not read.
 constexpr int kMaskThreads = 256;
 __global__ void __launch_bounds__(kMaskThreads) k_gen_mask(float *logits, int V, const GenStream *gs, const int *row_stream,
-                                                           const GenConstraint *gc) {
+                                                           const GenConstraint *gc,
+                                                           const unsigned long long *row_state = nullptr) {
     const int r = blockIdx.y, s = row_stream[r];
     const GenConstraint &c = gc[s];
-    if (!c.mask || gs[s].done) return;
+    unsigned long long q;
+    if (row_state) {
+        q = row_state[r];
+        if (q == kNoState) return;
+    } else {
+        if (!c.mask || gs[s].done) return;
+        q = c.state;
+    }
     const int v = blockIdx.x * kMaskThreads + threadIdx.x;
     if (v >= V) return;
-    if (!((c.mask[c.state * kMaskWords + (v >> 5)] >> (v & 31)) & 1u)) logits[(size_t)r * V + v] = -INFINITY;
+    if (!((c.mask[q * kMaskWords + (v >> 5)] >> (v & 31)) & 1u)) logits[(size_t)r * V + v] = -INFINITY;
 }
 
 // A stream's stop set (include/rwkv_b200.h, rwkv_b200_stop_set_add): the set's byte automaton (stopmatch.h), the model's
@@ -142,29 +184,7 @@ __global__ void k_gen_feedback(const GenFeedbackArgs a) {
         } else {
             for (int i = 0; i < a.n_stop; ++i) stop |= a.stop[i] == tok;
         }
-        if (a.gc && a.gc[s].mask) {
-            // advance the automaton; a state without edges completes it. The mask makes a missing edge impossible
-            // unless the pick broke its contract: record it for the host and end the stream
-            GenConstraint &c = a.gc[s];
-            const unsigned long long q = c.state, end = c.start[q + 1];
-            unsigned long long lo = c.start[q], hi = end;
-            while (lo < hi) {
-                const unsigned long long mid = (lo + hi) / 2;
-                if (c.tok[mid] < tok) lo = mid + 1;
-                else hi = mid;
-            }
-            if (lo < end && c.tok[lo] == tok) {
-                const unsigned long long q2 = c.next[lo];
-                c.state = q2;
-                stop |= c.start[q2] == c.start[q2 + 1];
-            } else {
-                if (atomicCAS(a.fault, 0ull, (unsigned long long)s + 1) == 0ull) {
-                    a.fault[1] = tok;
-                    a.fault[2] = q;
-                }
-                stop = true;
-            }
-        }
+        if (a.gc && a.gc[s].mask) stop |= gen_constraint_step(a.gc[s], tok, s, a.fault);
         if (a.gst && a.gst[s].next) stop |= gen_stop_walk(a.gst[s], tok);
         g.done = stop ? 1ull : 0ull;
         a.gs[s] = g;

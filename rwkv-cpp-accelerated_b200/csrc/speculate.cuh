@@ -12,7 +12,10 @@
 //   forward        the tensor-core passes, floor(128 / (k + 1)) streams per pass, every row a head row;
 //   k_gen_override, then k_sample_nucleus or k_argmax_rows on the rows (row_stream maps every row of s to s);
 //   k_spec_accept  one CTA per live stream: the picks, the accepted prefix, stops and budget, the emitted tokens into
-//                  the output and the history, and the new home: the slot of the row that produced the last emitted token.
+//                  the output and the history, and the new home: the slot of the row that produced the last emitted token;
+//   k_spec_logprob (with log-probabilities) one CTA per row: the emitted token of the row, if it emitted one, scored.
+// With token automata, k_spec_draft also walks the drafts through the stream's automaton into a state per row, by which
+// k_gen_mask masks the rows, and k_spec_accept advances the automaton by each emitted token (DESIGN §4.3).
 // At the end of the call, a stream whose home is not its first slot has the home's xy, aa, bb and dd copied to the first
 // slot (k_beam_fork with four arrays). The rule is stated in include/rwkv_b200.h and DESIGN §4.3.
 #pragma once
@@ -21,6 +24,7 @@
 
 #include "generate.cuh"
 #include "prefill.cuh"
+#include "score.cuh"
 
 namespace rk {
 
@@ -35,7 +39,7 @@ struct SpecStream {
     unsigned long long budget, len, steps;      // tokens it may emit, tokens emitted, steps that emitted a token
     unsigned long long done;                    // 1 after a stop token or the budget
     int home;                                   // index into slot[] of the slot holding the conversation
-    int pad;
+    int emitted;                                // tokens the last step emitted: len - emitted .. len - 1
 };
 
 struct SpecArgs {
@@ -53,6 +57,11 @@ struct SpecArgs {
     int n_stop;
     unsigned long long *out;         // [n_streams][max_new]
     GenStop *gst;                    // [n_streams] generate_streams_speculative_stop, else nullptr
+    // generate_streams_speculative_constrained with token automata, else nullptr: each stream's automaton and state, the
+    // state of each row this step (kNoState: not masked) and the record of an emitted token without an edge
+    GenConstraint *gc;               // [n_streams]
+    unsigned long long *row_state;   // [rows]
+    unsigned long long *fault;       // [3]
 };
 
 // Draft rule: for n = ngram down to 1 with n < L, the largest j <= L - n - 1 with h[j .. j + n) == h[L - n .. L); the
@@ -87,9 +96,25 @@ __global__ void __launch_bounds__(kSpecDraftThreads) k_spec_draft(const SpecArgs
         }
     }
     if (tid > k) return;
-    const unsigned long long tok = tid == 0 || from < 0 ? h[L - 1] : h[min(from + tid - 1, L - 1)];
+    auto row_tok = [&](int i) { return i == 0 || from < 0 ? h[L - 1] : h[min(from + i - 1, L - 1)]; };
+    const unsigned long long tok = row_tok(tid);
     g.row[tid] = tok;
     const int r = li * (k + 1) + tid, pi = li / a.per_pass, t = (li % a.per_pass) * (k + 1) + tid;
+    if (a.gc && tid == 0) {
+        // row 0 has the stream's state; row i is live while row i - 1 is, draft i has an edge out of its state and that
+        // edge leads to a state with edges. A dead row cannot be emitted: with no edge, the pick of the masked row
+        // i - 1 differs from draft i; at a complete state, emitting draft i ends the stream
+        const GenConstraint &c = a.gc[s];
+        unsigned long long q = live && c.mask ? c.state : kNoState;
+        a.row_state[r] = q;
+        for (int i = 1; i <= k; ++i) {
+            if (q != kNoState) {
+                q = gen_edge(c, q, row_tok(i));
+                if (q != kNoState && c.start[q] == c.start[q + 1]) q = kNoState;
+            }
+            a.row_state[r + i] = q;
+        }
+    }
     PassDesc &pd = a.passes[pi];
     pd.tokens[t] = tok;
     pd.desc[t] = (uint32_t)g.slot[(g.home + tid) % (k + 1)] | (tid == 0 ? kDescFirst : 0u) | (live ? kDescLast : 0u);
@@ -102,12 +127,15 @@ __global__ void __launch_bounds__(kSpecDraftThreads) k_spec_draft(const SpecArgs
 }
 
 // One warp per live stream: lane i holds the pick p_i of row i; a = the leading i in 1..k with row[i] == p_{i - 1}.
-// Lane 0 emits p_0 .. p_a with generate_streams' stop, stop-string and budget checks and moves home to the slot of the
-// last row used.
+// Lane 0 emits p_0 .. p_a with k_gen_feedback's checks in its order (budget, stop tokens, automaton, stop strings) and
+// moves home to the slot of the last row used.
 __global__ void __launch_bounds__(32) k_spec_accept(const SpecArgs a) {
     const int li = blockIdx.x, s = a.live[li], lane = threadIdx.x, k = a.k;
     SpecStream &g = a.ss[s];
-    if (g.done) return;
+    if (g.done) {
+        if (lane == 0) g.emitted = 0;
+        return;
+    }
     const int r = li * (k + 1) + lane;
     unsigned long long p = 0;
     if (lane <= k) p = a.next ? a.next[r] : (unsigned long long)a.sample[2 * r];
@@ -130,13 +158,30 @@ __global__ void __launch_bounds__(32) k_spec_accept(const SpecArgs a) {
         e = i;
         stop = len == g.budget;
         for (int z = 0; z < a.n_stop; ++z) stop |= a.stop[z] == tok;
+        if (a.gc && a.gc[s].mask) stop |= gen_constraint_step(a.gc[s], tok, s, a.fault);
         if (a.gst && a.gst[s].next) stop |= gen_stop_walk(a.gst[s], tok);
     }
     g.len = len;
     g.hl = hl;
     g.steps += 1;
+    g.emitted = e + 1;
     g.home = (g.home + e) % (k + 1);
     g.done = stop ? 1ull : 0ull;
+}
+
+// The log-probabilities of a step's emitted tokens, after k_spec_accept: one CTA of kNucThreads per row r = li * (k + 1)
+// + i; row i of a stream that emitted more than i tokens this step scores its pick p_i, emitted at position len -
+// emitted + i, on la.logits (the raw copy, or the rows the pick read) divided by the stream's temperature in processed
+// mode (la.samp), with generate_streams_logprobs' rule (logprob_row). Other rows return at once (the whole CTA).
+__global__ void __launch_bounds__(kNucThreads) k_spec_logprob(const SpecArgs a, const GenLogprobArgs la) {
+    const int r = blockIdx.x, li = r / (a.k + 1), i = r % (a.k + 1), s = a.live[li];
+    const SpecStream &g = a.ss[s];
+    if (i >= g.emitted) return;
+    const int y = a.next ? (int)a.next[r] : (int)a.sample[2 * r];
+    const float T = la.samp ? la.samp[s].temperature : 0.0f;
+    const size_t o = (size_t)s * a.max_new + (size_t)(g.len - (unsigned long long)g.emitted + (unsigned long long)i);
+    logprob_row(la.logits + (size_t)r * la.V, la.V, y, T > 0.0f ? (double)T : 1.0, la.top_n, la.logprob + o, la.rank + o,
+                la.top_tokens + o * la.top_n, la.top_logprobs + o * la.top_n);
 }
 
 } // namespace rk

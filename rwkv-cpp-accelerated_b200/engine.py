@@ -173,6 +173,53 @@ def _gen_args(streams, max_new, budgets, stop, overrides, u, slots=None):
     return S, lead, (_ptr(us, ctypes.c_double), _ptr(out, P), _ptr(lens, P)), out, lens
 
 
+_LOGPROB_MODES = {None: LOGPROBS_RAW, "raw": LOGPROBS_RAW, "processed": LOGPROBS_PROCESSED}
+
+
+def _logprob_mode(logprobs, what):
+    if logprobs not in _LOGPROB_MODES:
+        raise EngineError("%s: logprobs must be 'raw' or 'processed', not %r" % (what, logprobs))
+    return _LOGPROB_MODES[logprobs]
+
+
+def _scored_args(S, max_new, logprobs, top_n, constraints, what):
+    """The log-probability and automaton arguments of a call of S streams (logprobs None: no scoring; constraints None:
+    no automata): the six from logprob_mode to top_logprobs_out, the three from constraint_ids to states_out, and
+    result(s, n) -> the dict of "state" and the logprob fields of stream s with n emitted tokens."""
+    P = ctypes.c_ulonglong
+    lp = ranks = top_tok = top_lp = None
+    if logprobs is not None:
+        lp = np.empty((S, max_new), np.float64)
+        ranks = np.empty((S, max_new), np.uint64)
+        if top_n > 0:
+            top_tok = np.empty((S, max_new, top_n), np.uint64)
+            top_lp = np.empty((S, max_new, top_n), np.float64)
+    ids = starts = states = None
+    if constraints is not None:
+        spec = [constraints] * S if isinstance(constraints, (int, np.integer)) else list(constraints)
+        if len(spec) != S:
+            raise EngineError("%s: %d constraints for %d streams" % (what, len(spec), S))
+        pairs = [(NO_CONSTRAINT, 0) if c is None else (int(c[0]), int(c[1])) if isinstance(c, (tuple, list))
+                 else (int(c), 0) for c in spec]
+        ids = np.ascontiguousarray([c for c, _ in pairs], np.uint64)
+        starts = np.ascontiguousarray([q for _, q in pairs], np.uint64)
+        states = np.zeros(S, np.uint64)
+    lp_args = (_LOGPROB_MODES[logprobs], int(top_n), _ptr(lp, ctypes.c_double), _ptr(ranks, P), _ptr(top_tok, P),
+               _ptr(top_lp, ctypes.c_double))
+    c_args = (_ptr(ids, P), _ptr(starts, P), _ptr(states, P))
+
+    def result(s, n):
+        d = {}
+        if constraints is not None:
+            d["state"] = int(states[s]) if ids[s] != np.uint64(NO_CONSTRAINT) else None
+        if lp is not None:
+            d["logprobs"], d["ranks"] = lp[s, :n].copy(), ranks[s, :n].copy()
+            if top_n > 0:
+                d["top_tokens"], d["top_logprobs"] = top_tok[s, :n].copy(), top_lp[s, :n].copy()
+        return d
+    return lp_args, c_args, result
+
+
 def lookup_drafts(history, draft, ngram):
     """The k = draft prompt-lookup drafts of rwkv_b200_generate_streams_speculative for a history h (context, first token,
     tokens emitted so far): for n = ngram down to 1 with n < len(h), the largest j <= len(h) - n - 1 with
@@ -290,6 +337,10 @@ def load_library():
         "rwkv_b200_generate_streams_speculative_stop": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull,
                                                               c.POINTER(Sampler), pdbl, pull, pull, c.c_uint, c.c_uint,
                                                               pull, pull, pull, c.POINTER(StopRequest)]),
+        "rwkv_b200_generate_streams_speculative_constrained": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt,
+                                                                     ull, c.POINTER(Sampler), pdbl, pull, pull, c.c_uint,
+                                                                     c.c_uint, pull, pull, pull, i32, c.c_uint, pdbl, pull,
+                                                                     pull, pdbl, pull, pull, pull, c.POINTER(StopRequest)]),
         "rwkv_b200_batcher_submit_stop": (i32, [vp, c.POINTER(Request), c.POINTER(RequestEx), ull, ull, pull]),
         "rwkv_b200_batcher_read_stop": (i32, [vp, ull, pull, pull, pull]),
         "rwkv_b200_batcher_cancel": (i32, [vp, ull]),
@@ -479,9 +530,7 @@ class Engine:
         """generate_streams with logprobs, constraints or stop strings: rwkv_b200_generate_streams_stop with stop
         strings, rwkv_b200_generate_streams_constrained with constraints, else rwkv_b200_generate_streams_logprobs. One
         dict per stream."""
-        modes = {None: LOGPROBS_RAW, "raw": LOGPROBS_RAW, "processed": LOGPROBS_PROCESSED}
-        if logprobs not in modes:
-            raise EngineError("generate_streams: logprobs must be 'raw' or 'processed', not %r" % (logprobs,))
+        _logprob_mode(logprobs, "generate_streams")
         if sampling is None and (u is not None or temp is not None):
             if stop_strings is not None:
                 raise EngineError("generate_streams: stop_strings need sampling=... (or neither u nor temp, for the "
@@ -492,28 +541,9 @@ class Engine:
             raise EngineError("generate_streams: logprobs need sampling=... (or neither u nor temp, for the arg-max); "
                               "the typical sampler reports no log-probabilities")
         S, lead, tail, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u)
-        lp = ranks = top_tok = top_lp = None
-        if logprobs is not None:
-            lp = np.empty((S, max_new), np.float64)
-            ranks = np.empty((S, max_new), np.uint64)
-            if top_n > 0:
-                top_tok = np.empty((S, max_new, top_n), np.uint64)
-                top_lp = np.empty((S, max_new, top_n), np.float64)
-        P = ctypes.c_ulonglong
+        lp_args, cargs, scored = _scored_args(S, max_new, logprobs, top_n, constraints, "generate_streams")
         sp = _samplers(sampling, S) if sampling is not None else None
-        args = (self.h, *lead, sp, *tail, modes[logprobs], int(top_n), _ptr(lp, ctypes.c_double), _ptr(ranks, P),
-                _ptr(top_tok, P), _ptr(top_lp, ctypes.c_double))
-        ids = starts = states = None
-        if constraints is not None:
-            spec = [constraints] * S if isinstance(constraints, (int, np.integer)) else list(constraints)
-            if len(spec) != S:
-                raise EngineError("generate_streams: %d constraints for %d streams" % (len(spec), S))
-            pairs = [(NO_CONSTRAINT, 0) if c is None else (int(c[0]), int(c[1])) if isinstance(c, (tuple, list))
-                     else (int(c), 0) for c in spec]
-            ids = np.ascontiguousarray([c for c, _ in pairs], np.uint64)
-            starts = np.ascontiguousarray([q for _, q in pairs], np.uint64)
-            states = np.zeros(S, np.uint64)
-        cargs = (_ptr(ids, P), _ptr(starts, P), _ptr(states, P))
+        args = (self.h, *lead, sp, *tail, *lp_args)
         if stop_strings is not None:
             sreq, sres = self._stop_request(stop_strings, S, "generate_streams")
             self._ck(self.lib.rwkv_b200_generate_streams_stop(*args, *cargs, ctypes.byref(sreq)), "generate_streams_stop")
@@ -527,12 +557,7 @@ class Engine:
             d = {"tokens": out[s, :n].copy()}
             if stop_strings is not None:
                 d.update(sres(s))
-            if constraints is not None:
-                d["state"] = int(states[s]) if ids[s] != np.uint64(NO_CONSTRAINT) else None
-            if lp is not None:
-                d["logprobs"], d["ranks"] = lp[s, :n].copy(), ranks[s, :n].copy()
-                if top_n > 0:
-                    d["top_tokens"], d["top_logprobs"] = top_tok[s, :n].copy(), top_lp[s, :n].copy()
+            d.update(scored(s, n))
             res.append(d)
         return res
 
@@ -666,13 +691,18 @@ class Engine:
         return res
 
     def generate_speculative(self, streams, max_new, draft, ngram=3, context=None, budgets=None, stop=(), overrides=None,
-                             sampling=None, u=None, stop_strings=None):
+                             sampling=None, u=None, stop_strings=None, logprobs=None, top_n=0, constraints=None):
         """generate_streams(sampling=...) with prompt-lookup drafts (rwkv_b200_generate_streams_speculative): the same
         tokens and first-slot states, several tokens per step where the drafts are right. streams = [(slots, first_token),
         ...], each with draft + 1 distinct slots, the first holding the conversation (the others are scratch). context:
         None, or one token list (or None) per stream of extra lookup tokens. sampling None is the arg-max. Returns one
         dict per stream: "tokens" (uint64) and "steps" (the steps that emitted a token). stop_strings as in
-        generate_streams (rwkv_b200_generate_streams_speculative_stop) adds "stop_hit", "stop_tail" and "stop_state"."""
+        generate_streams (rwkv_b200_generate_streams_speculative_stop) adds "stop_hit", "stop_tail" and "stop_state".
+        logprobs, top_n and constraints as in generate_streams (rwkv_b200_generate_streams_speculative_constrained) add
+        "logprobs", "ranks", "top_tokens", "top_logprobs" and "state", bit for bit generate_streams' values."""
+        extended = logprobs is not None or constraints is not None
+        if extended:
+            _logprob_mode(logprobs, "generate_speculative")
         if any(len(slots) != draft + 1 for slots, _ in streams):
             raise EngineError("generate_speculative: every stream needs draft + 1 = %d slots" % (draft + 1))
         S, lead, tail, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u,
@@ -685,9 +715,25 @@ class Engine:
             seqs = [[int(x) for x in (c if c is not None else ())] for c in context]
             cstart = np.ascontiguousarray(np.cumsum([0] + [len(c) for c in seqs]), dtype=np.uint64)
             ctx = np.ascontiguousarray([x for c in seqs for x in c], dtype=np.uint64)
+        if extended:
+            lp_args, cargs, scored = _scored_args(S, max_new, logprobs, top_n, constraints, "generate_speculative")
         sp = _samplers(sampling, S) if sampling is not None else None
         P = ctypes.c_ulonglong
         args = (self.h, *lead, sp, *tail, int(draft), int(ngram), _ptr(cstart, P), _ptr(ctx, P), _ptr(steps, P))
+        if extended:
+            sreq, sres = self._stop_request(stop_strings, S, "generate_speculative") if stop_strings is not None else (None, None)
+            self._ck(self.lib.rwkv_b200_generate_streams_speculative_constrained(
+                *args, *lp_args, *cargs, ctypes.byref(sreq) if sreq is not None else None),
+                "generate_streams_speculative_constrained")
+            res = []
+            for s in range(S):
+                n = int(lens[s])
+                d = {"tokens": out[s, :n].copy(), "steps": int(steps[s])}
+                if sres is not None:
+                    d.update(sres(s))
+                d.update(scored(s, n))
+                res.append(d)
+            return res
         if stop_strings is None:
             self._ck(self.lib.rwkv_b200_generate_streams_speculative(*args), "generate_streams_speculative")
             return [{"tokens": out[s, :int(lens[s])].copy(), "steps": int(steps[s])} for s in range(S)]
@@ -830,9 +876,7 @@ class Batcher:
                                                                    int(starts[0]), ctypes.byref(rid)), "batcher_submit")
             self._stop.add(int(rid.value))
             return int(rid.value)
-        modes = {None: LOGPROBS_RAW, "raw": LOGPROBS_RAW, "processed": LOGPROBS_PROCESSED}
-        if logprobs not in modes:
-            raise EngineError("batcher.submit: logprobs must be 'raw' or 'processed', not %r" % (logprobs,))
+        mode = _logprob_mode(logprobs, "batcher.submit")
         ovr = dict(overrides or {})
         otok = np.ascontiguousarray(list(ovr.keys()), dtype=np.uint64)
         oval = np.ascontiguousarray(list(ovr.values()), dtype=np.float32)
@@ -840,7 +884,7 @@ class Batcher:
         if constraint is not None:
             cid, q0 = (int(constraint[0]), int(constraint[1])) if isinstance(constraint, (tuple, list)) else (int(constraint), 0)
         x = RequestEx(_ptr(otok, P), _ptr(oval, ctypes.c_float), len(otok), cid, q0, 1 if logprobs is not None else 0,
-                      modes[logprobs], int(top_n))
+                      mode, int(top_n))
         if stop_strings is None:
             self.engine._ck(self.lib.rwkv_b200_batcher_submit_ex(self.h, ctypes.byref(req), ctypes.byref(x),
                                                                  ctypes.byref(rid)), "batcher_submit")
