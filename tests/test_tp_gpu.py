@@ -37,6 +37,8 @@ def test_tp_matches_oracle(pkg, make_model, tmp_path, world, L, E, steps):
     assert r.returncode == 0, "tp worker failed:\n" + r.stdout[-3000:] + r.stderr[-3000:]
     res = json.load(open(out))
     print(res)
-    assert res["worst_vs_oracle"] < 1e-3
-    assert res["worst_vs_single_gpu"] < 1e-4
+    # the engine's budget (tests/numerics.py TOL): the oracle is ~5e-7 from the engine's arithmetic, and the ranks
+    # add exact integer partial sums and f64 offsets, which only the order of f64 additions separates from one GPU
+    assert res["worst_vs_oracle"] < 1e-5
+    assert res["worst_vs_single_gpu"] < 1e-5
     assert res["ranks_agree"] and res["greedy_agree"]

@@ -43,7 +43,8 @@ def token_stream(n, seed):
 
 
 def stress_model(src, dst, kind, L=3, E=768):
-    """A copy of the L x E synthetic model `src` at `dst` with its layernorm parameters edited in place.
+    """A copy of the L x E synthetic model `src` at `dst` with its layernorm parameters edited in place (the
+    negative_keys / one_positive_key kinds also rewrite ffn_ko and, for one_positive_key, the ffn_k bytes).
     LAYERNORMS = f64 [4(L+1)][E] after xbuf (f64 [E]) and embed (f32 [V][E]): rows 0,1 = ln0 w,b;
     4i+2, 4i+3 = ln1 of layer i; 4(i+1), 4(i+1)+1 = ln2 of layer i (convert_model.py:30-46)."""
     import shutil
@@ -62,6 +63,25 @@ def stress_model(src, dst, kind, L=3, E=768):
         ln[1] *= 1e-3
     elif kind == "offset_residual":
         ln[1] += 50.0                       # ln0 bias: |mean| >> std in every later layernorm
+    elif kind in ("negative_keys", "one_positive_key"):
+        # Every ffn input positive: ln2 weight 0, bias > 0 (the ffn token-shift state is an earlier ln2 output).
+        # Offsets o_j = -c * r_j make every coefficient w * r_j + o_j of ffn K negative for c > 255, so every key
+        # is negative, relu^2 is zero and the ffn-V input is all zeros (the m == 0 path of the quantiser).
+        # one_positive_key: c = 254.5, every byte at most 253 except column 4E / 3, all 255: one positive key.
+        from numerics import tensors
+        _, _, t = tensors(dst, mode="r+")
+        kr, ko = t["ffn_kr"], t["ffn_ko"]
+        for i in range(L):
+            ln[4 * (i + 1)] = 0.0
+            ln[4 * (i + 1) + 1] = np.abs(ln[4 * (i + 1) + 1]) + 0.1
+        ko[:] = (-256.0 if kind == "negative_keys" else -254.5) * kr.astype(np.float64)
+        if kind == "one_positive_key":
+            fk = t["ffn_k"].reshape(L * E, 4 * E)
+            np.minimum(fk, 253, out=fk)
+            fk[:, 4 * E // 3] = 255
+        for a in t.values():
+            a.flush()
+        del t, kr, ko
     else:
         raise ValueError(kind)
     ln.flush()
