@@ -740,6 +740,60 @@ int rwkv_b200_slot_upload(rwkv_b200_model *m, unsigned long long slot, const dou
 int rwkv_b200_slot_download(rwkv_b200_model *m, unsigned long long slot, double *xy, double *aa,
                             double *bb, double *pp, double *dd);
 
+/* State indexes: store texts as their recurrent state in HBM and rank them against query slots, as
+ * examples/vectordb does on the host.
+ *  - Index. An index has a contiguous layer range [layer_begin, layer_begin + n_layers) and a fixed capacity of entries.
+ *    Its vectors have D = n_layers * E f64 elements: the vector of slot s is that slot's dd array over those layers as
+ *    stored (layer-major), bit for bit what rwkv_b200_slot_download returns for dd there. With every layer it is the
+ *    statedd that examples/vectordb reads after loadContext.
+ *  - Entries. Entries get ids 0, 1, 2, ... in the order they are added; adding appends and ids are never reused.
+ *    rwkv_b200_index_remove marks entries so that they are never returned again; their rows are not reclaimed, so the
+ *    capacity counts every add.
+ *  - Distances. For a query vector a and an entry vector b, in f64 over the D elements:
+ *      l1 = (sum_j |a_j - b_j|) / E          ("diff" in examples/vectordb)
+ *      l2 = sqrt((sum_j (a_j - b_j)^2) / E)  ("euclid")
+ *    The summation order is fixed and depends only on D: never on the index size, the entry's row, which entries are
+ *    live, the number of queries or their batch, or k. So each distance is a function of the two vectors' bits alone.
+ *    (examples/vectordb divides each term by E and accumulates in float; this is the same quantity without that
+ *    rounding.)
+ *  - Search. For each query the live entries are ranked by the chosen metric, ascending, ties to the lower id, a NaN
+ *    distance after every number. The first min(k, live) entries (found_out) are returned with both distances;
+ *    positions past found_out hold RWKV_B200_NO_ENTRY and NaN. entries_out, l1_out and l2_out are [n_queries][k].
+ *  - Queries are state slots, so a query text is embedded by the same forward as the documents. A search reads those
+ *    slots (a slot may appear more than once) and writes no slot; n_queries has no limit beyond memory (the queries
+ *    are scanned in batches).
+ * Refused before any work, changing neither the index nor any slot: a NULL handle or a missing array, an unknown or
+ * freed index id, a layer range outside the model or n_layers == 0, capacity == 0 or a device allocation that fails,
+ * an add that would pass the capacity (nothing is added), a slot >= max_gpt, a non-finite value in upload, an entry id
+ * that was never added or was removed in download and remove (nothing is removed), a metric other than the two, k == 0
+ * or k > RWKV_B200_MAX_NEIGHBOURS, n_queries == 0, and tensor parallelism. rwkv_b200_free frees every index. As for the
+ * other multi-stream calls, the model's batcher does not police a slot named by one of its unfinished requests. */
+#define RWKV_B200_INDEX_L1 0
+#define RWKV_B200_INDEX_L2 1
+#define RWKV_B200_MAX_NEIGHBOURS 256
+#define RWKV_B200_NO_ENTRY 0xFFFFFFFFFFFFFFFFULL /* entries_out past found_out */
+/* Allocate an index of `capacity` entries over layers [layer_begin, layer_begin + n_layers); *id receives its id. */
+int rwkv_b200_index_create(rwkv_b200_model *m, unsigned long long layer_begin, unsigned long long n_layers,
+                           unsigned long long capacity, unsigned long long *id);
+/* Free an index and its device memory. */
+int rwkv_b200_index_free(rwkv_b200_model *m, unsigned long long id);
+/* Append the vectors of n slots (a device-to-device copy); entries_out [n] receives their ids. */
+int rwkv_b200_index_add_slots(rwkv_b200_model *m, unsigned long long id, const unsigned long long *slots,
+                              unsigned long long n, unsigned long long *entries_out);
+/* Append n vectors given on the host, vectors [n][D]; entries_out [n] receives their ids. */
+int rwkv_b200_index_upload(rwkv_b200_model *m, unsigned long long id, const double *vectors, unsigned long long n,
+                           unsigned long long *entries_out);
+/* The vectors of n live entries into vectors_out [n][D]. */
+int rwkv_b200_index_download(rwkv_b200_model *m, unsigned long long id, const unsigned long long *entries,
+                             unsigned long long n, double *vectors_out);
+/* Remove n live entries (each at most once per call). */
+int rwkv_b200_index_remove(rwkv_b200_model *m, unsigned long long id, const unsigned long long *entries,
+                           unsigned long long n);
+/* Rank the live entries for each query slot by `metric` (RWKV_B200_INDEX_L1 or _L2) and return the first k. */
+int rwkv_b200_index_search(rwkv_b200_model *m, unsigned long long id, const unsigned long long *query_slots,
+                           unsigned long long n_queries, int metric, unsigned int k, unsigned long long *entries_out,
+                           double *l1_out, double *l2_out, unsigned long long *found_out);
+
 /* Engine knobs (all optional), key/value strings: "window" / "bwindow" (bulk copies in
  * flight per SM while streaming / while the CTAs exchange vectors), "pf_dist" (tiles the L2
  * prefetch runs ahead), "stages" (ring depth), "timeout_ms", "trace", "prefill",

@@ -37,6 +37,7 @@
 #include "beam.cuh"
 #include "binfmt.h"
 #include "generate.cuh"
+#include "index.cuh"
 #include "prefill.cuh"
 #include "sampling.cuh"
 #include "score.cuh"
@@ -196,6 +197,22 @@ struct rwkv_b200_model {
         DevBuf<unsigned long long> row_state; // [rows] each row's automaton state (constrained calls)
     } spec;
     rwkv_b200_batcher *batcher = nullptr; // the open batcher (at most one), closed by rwkv_b200_free
+    // rwkv_b200_index_create: per id the rows [capacity][D] and live flags on the device, the flags and counts on the host
+    struct Index {
+        unsigned long long lb = 0, nl = 0, D = 0, capacity = 0, count = 0, live = 0;
+        std::vector<unsigned char> alive; // [count]
+        DevBuf<double> rows;
+        DevBuf<unsigned char> d_alive;    // [capacity]
+    };
+    std::map<unsigned long long, Index> indexes;
+    unsigned long long next_index = 1;
+    // rwkv_b200_index_search: grown with the largest call
+    struct IndexScratch {
+        DevBuf<double> partial, l1, l2;            // [QB][block][G][2], [QB][count], [QB][count]
+        DevBuf<unsigned long long> key[2], id[2];  // the selection's survivors, ping-pong
+        DevBuf<unsigned long long> ent;            // [QB][k]
+        DevBuf<double> o1, o2;                     // [QB][k]
+    } isc;
 };
 
 // rwkv_b200_batcher: the requests on the host, and per lane (0..rows-1, one per admitted request, reused) its stream
@@ -2534,6 +2551,252 @@ int rwkv_b200_slot_download(rwkv_b200_model *m, unsigned long long slot, double 
     for (int i = 0; i < 5; ++i)
         if (dst[i]) CK(cudaMemcpyAsync(dst[i], a[i], (size_t)(m->L * m->E) * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
     SYNC(m);
+    return 0;
+}
+
+// ---- state indexes (csrc/index.cuh) ---------------------------------------------------------------------------------
+
+// The multi-stream checks and the index of `id`.
+static int find_index(M *m, const char *what, unsigned long long id, M::Index **out) {
+    int rc = check_streams_model(m, what);
+    if (rc) return rc;
+    const auto it = m->indexes.find(id);
+    if (it == m->indexes.end()) return fail(1, "%s: index id %llu is unknown or freed", what, id);
+    *out = &it->second;
+    return 0;
+}
+
+// n entry ids, each added and not removed; with `once`, none twice.
+static int check_entries(const M::Index &x, const char *what, const unsigned long long *entries, unsigned long long n,
+                         bool once) {
+    std::vector<char> seen(once ? x.count : 0, 0);
+    for (unsigned long long i = 0; i < n; ++i) {
+        const unsigned long long e = entries[i];
+        if (e >= x.count) return fail(1, "%s: entry %llu was never added (%llu entries)", what, e, x.count);
+        if (!x.alive[e]) return fail(1, "%s: entry %llu was removed", what, e);
+        if (once && seen[e]) return fail(1, "%s: entry %llu appears twice", what, e);
+        if (once) seen[e] = 1;
+    }
+    return 0;
+}
+
+// Room for n more entries.
+static int check_room(const M::Index &x, const char *what, unsigned long long n) {
+    if (n > x.capacity - x.count)
+        return fail(1, "%s: %llu entries would pass the capacity %llu (%llu added)", what, n, x.capacity, x.count);
+    return 0;
+}
+
+// Marks rows count .. count + n live (the copies into them are enqueued) and returns their ids.
+static int index_append(M *m, M::Index &x, unsigned long long n, unsigned long long *entries_out) {
+    CK(cudaMemsetAsync(x.d_alive.p + x.count, 1, n, m->stream));
+    SYNC(m);
+    x.alive.insert(x.alive.end(), n, 1);
+    for (unsigned long long i = 0; i < n; ++i) entries_out[i] = x.count + i;
+    x.count += n;
+    x.live += n;
+    return 0;
+}
+
+int rwkv_b200_index_create(rwkv_b200_model *m, unsigned long long layer_begin, unsigned long long n_layers,
+                           unsigned long long capacity, unsigned long long *id) {
+    const char *what = "index_create";
+    int rc = check_streams_model(m, what);
+    if (rc) return rc;
+    if (!id) return fail(1, "%s: id is NULL", what);
+    if (n_layers == 0 || layer_begin >= m->L || n_layers > m->L - layer_begin)
+        return fail(1, "%s: layers %llu .. %llu + %llu are not a non-empty range of the model's %llu layers", what, layer_begin,
+                    layer_begin, n_layers, m->L);
+    if (capacity == 0) return fail(1, "%s: capacity 0", what);
+    const unsigned long long D = n_layers * m->E;
+    if (capacity > (SIZE_MAX / sizeof(double)) / D) return fail(9, "%s: %llu entries of %llu doubles are too many", what, capacity, D);
+    M::Index x;
+    x.lb = layer_begin, x.nl = n_layers, x.D = D, x.capacity = capacity;
+    CK(cudaSetDevice(m->device));
+    if ((rc = x.rows.grow(capacity * D)) || (rc = x.d_alive.grow(capacity))) {
+        const std::string e = g_err;
+        cudaGetLastError(); // a failed allocation is not left behind as the last error
+        return fail(rc, "%s: %llu entries of %llu bytes: %s", what, capacity, D * 8, e.c_str());
+    }
+    *id = m->next_index++;
+    m->indexes.emplace(*id, std::move(x));
+    return 0;
+}
+
+int rwkv_b200_index_free(rwkv_b200_model *m, unsigned long long id) {
+    M::Index *x;
+    int rc = find_index(m, "index_free", id, &x);
+    if (rc) return rc;
+    CK(cudaSetDevice(m->device));
+    CK(cudaStreamSynchronize(m->stream));
+    m->indexes.erase(id);
+    return 0;
+}
+
+int rwkv_b200_index_add_slots(rwkv_b200_model *m, unsigned long long id, const unsigned long long *slots,
+                              unsigned long long n, unsigned long long *entries_out) {
+    const char *what = "index_add_slots";
+    M::Index *x;
+    int rc = find_index(m, what, id, &x);
+    if (rc) return rc;
+    if (!slots || !entries_out || n == 0) return fail(1, "%s: no slots (slots and entries_out are required)", what);
+    for (unsigned long long i = 0; i < n; ++i)
+        if ((rc = check_slot(m, what, slots[i]))) return rc;
+    if ((rc = check_room(*x, what, n))) return rc;
+    CK(cudaSetDevice(m->device));
+    for (unsigned long long i = 0; i < n; ++i) {
+        double *a[5];
+        slot_arrays(m, slots[i], a);
+        CK(cudaMemcpyAsync(x->rows.p + (x->count + i) * x->D, a[4] + x->lb * m->E, x->D * sizeof(double),
+                           cudaMemcpyDeviceToDevice, m->stream));
+    }
+    return index_append(m, *x, n, entries_out);
+}
+
+int rwkv_b200_index_upload(rwkv_b200_model *m, unsigned long long id, const double *vectors, unsigned long long n,
+                           unsigned long long *entries_out) {
+    const char *what = "index_upload";
+    M::Index *x;
+    int rc = find_index(m, what, id, &x);
+    if (rc) return rc;
+    if (!vectors || !entries_out || n == 0) return fail(1, "%s: no vectors (vectors and entries_out are required)", what);
+    if ((rc = check_room(*x, what, n))) return rc;
+    for (unsigned long long i = 0; i < n * x->D; ++i)
+        if (!std::isfinite(vectors[i]))
+            return fail(1, "%s: element %llu of vector %llu is not finite", what, i % x->D, i / x->D);
+    CK(cudaSetDevice(m->device));
+    CK(cudaMemcpyAsync(x->rows.p + x->count * x->D, vectors, n * x->D * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+    return index_append(m, *x, n, entries_out);
+}
+
+int rwkv_b200_index_download(rwkv_b200_model *m, unsigned long long id, const unsigned long long *entries,
+                             unsigned long long n, double *vectors_out) {
+    const char *what = "index_download";
+    M::Index *x;
+    int rc = find_index(m, what, id, &x);
+    if (rc) return rc;
+    if (!entries || !vectors_out || n == 0) return fail(1, "%s: no entries (entries and vectors_out are required)", what);
+    if ((rc = check_entries(*x, what, entries, n, false))) return rc;
+    CK(cudaSetDevice(m->device));
+    for (unsigned long long i = 0; i < n; ++i)
+        CK(cudaMemcpyAsync(vectors_out + i * x->D, x->rows.p + entries[i] * x->D, x->D * sizeof(double),
+                           cudaMemcpyDeviceToHost, m->stream));
+    SYNC(m);
+    return 0;
+}
+
+int rwkv_b200_index_remove(rwkv_b200_model *m, unsigned long long id, const unsigned long long *entries,
+                           unsigned long long n) {
+    const char *what = "index_remove";
+    M::Index *x;
+    int rc = find_index(m, what, id, &x);
+    if (rc) return rc;
+    if (!entries || n == 0) return fail(1, "%s: no entries", what);
+    if ((rc = check_entries(*x, what, entries, n, true))) return rc;
+    std::vector<unsigned char> alive = x->alive;
+    for (unsigned long long i = 0; i < n; ++i) alive[entries[i]] = 0;
+    CK(cudaSetDevice(m->device));
+    CK(cudaMemcpyAsync(x->d_alive.p, alive.data(), x->count, cudaMemcpyHostToDevice, m->stream));
+    SYNC(m);
+    x->alive.swap(alive);
+    x->live -= n;
+    return 0;
+}
+
+int rwkv_b200_index_search(rwkv_b200_model *m, unsigned long long id, const unsigned long long *query_slots,
+                           unsigned long long n_queries, int metric, unsigned int k, unsigned long long *entries_out,
+                           double *l1_out, double *l2_out, unsigned long long *found_out) {
+    const char *what = "index_search";
+    M::Index *x;
+    int rc = find_index(m, what, id, &x);
+    if (rc) return rc;
+    if (!query_slots || !entries_out || !l1_out || !l2_out || !found_out)
+        return fail(1, "%s: null argument (query_slots, entries_out, l1_out, l2_out and found_out are required)", what);
+    if (n_queries == 0) return fail(1, "%s: no queries", what);
+    if (metric != RWKV_B200_INDEX_L1 && metric != RWKV_B200_INDEX_L2) return fail(1, "%s: unknown metric %d", what, metric);
+    if (k == 0 || k > RWKV_B200_MAX_NEIGHBOURS) return fail(1, "%s: k = %u is outside 1..%d", what, k, RWKV_B200_MAX_NEIGHBOURS);
+    for (unsigned long long i = 0; i < n_queries; ++i)
+        if ((rc = check_slot(m, what, query_slots[i]))) return rc;
+    const unsigned long long N = x->count, D = x->D, QB = rk::kIdxQB;
+    if (x->live == 0) {
+        for (unsigned long long i = 0; i < n_queries * k; ++i) entries_out[i] = RWKV_B200_NO_ENTRY, l1_out[i] = l2_out[i] = NAN;
+        for (unsigned long long i = 0; i < n_queries; ++i) found_out[i] = 0;
+        return 0;
+    }
+    CK(cudaSetDevice(m->device));
+    // segments, and an entry block that keeps the partial sums at 32 MiB at most
+    const unsigned G = (unsigned)((D + rk::kIdxSeg - 1) / rk::kIdxSeg);
+    const unsigned long long NB = std::max<unsigned long long>(1, std::min<unsigned long long>(N, (4ULL << 20) / (QB * G * 2)));
+    auto pow2 = [](unsigned long long n) {
+        int p = 1;
+        while ((unsigned long long)p < n) p <<= 1;
+        return p;
+    };
+    const int sort0 = pow2(std::min<unsigned long long>(N, rk::kIdxSelN));
+    const unsigned long long chunks0 = (N + sort0 - 1) / sort0;
+    M::IndexScratch &s = m->isc;
+    if ((rc = s.partial.grow(QB * NB * G * 2)) || (rc = s.l1.grow(QB * N)) || (rc = s.l2.grow(QB * N)) ||
+        (rc = s.key[0].grow(QB * chunks0 * k)) || (rc = s.key[1].grow(QB * chunks0 * k)) ||
+        (rc = s.id[0].grow(QB * chunks0 * k)) || (rc = s.id[1].grow(QB * chunks0 * k)) || (rc = s.ent.grow(QB * k)) ||
+        (rc = s.o1.grow(QB * k)) || (rc = s.o2.grow(QB * k))) {
+        cudaGetLastError();
+        return rc;
+    }
+    const int scan_smem = (int)(QB * rk::kIdxSeg * sizeof(double)), sel_smem = 2 * rk::kIdxSelN * (int)sizeof(unsigned long long);
+    CK(cudaFuncSetAttribute(rk::k_index_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, scan_smem));
+    CK(cudaFuncSetAttribute(rk::k_index_select, cudaFuncAttributeMaxDynamicSharedMemorySize, sel_smem));
+    const double *dist = metric == RWKV_B200_INDEX_L1 ? s.l1.p : s.l2.p;
+    for (unsigned long long b0 = 0; b0 < n_queries; b0 += QB) {
+        const int nq = (int)std::min(QB, n_queries - b0);
+        // the scan, one entry block at a time: enough CTAs of at least one row per warp to fill the GPU
+        rk::IndexScanArgs a{};
+        a.rows = x->rows.p, a.alive = x->d_alive.p, a.nq = nq, a.D = D, a.G = G, a.partial = s.partial.p;
+        for (int q = 0; q < nq; ++q) {
+            double *st[5];
+            slot_arrays(m, query_slots[b0 + q], st);
+            a.q[q] = st[4] + x->lb * m->E;
+        }
+        for (unsigned long long e0 = 0; e0 < N; e0 += NB) {
+            const unsigned long long n = std::min(NB, N - e0);
+            const unsigned long long target = (4ULL * m->sms + G - 1) / G;
+            unsigned long long cy = std::min<unsigned long long>({(n + rk::kIdxWarps - 1) / rk::kIdxWarps, target, 65535});
+            cy = std::max<unsigned long long>(cy, 1);
+            a.e0 = e0, a.n = n, a.rows_per_cta = (n + cy - 1) / cy;
+            cy = (n + a.rows_per_cta - 1) / a.rows_per_cta;
+            rk::k_index_scan<<<dim3(G, (unsigned)cy), rk::kIdxWarps * 32, scan_smem, m->stream>>>(a);
+            LAUNCHED(m);
+            const unsigned long long t = (unsigned long long)nq * n;
+            rk::k_index_combine<<<(unsigned)((t + 255) / 256), 256, 0, m->stream>>>(s.partial.p, x->d_alive.p, nq, e0, n, G,
+                                                                                (double)m->E, s.l1.p, s.l2.p, N);
+            LAUNCHED(m);
+        }
+        // the selection: passes over the survivors until one CTA per query holds them all
+        const unsigned long long *ik = nullptr, *ii = nullptr;
+        unsigned long long n = N;
+        int pb = 0;
+        for (;;) {
+            const int sn = pow2(std::min<unsigned long long>(n, rk::kIdxSelN));
+            const unsigned long long ch = (n + sn - 1) / sn;
+            const rk::IndexSelArgs sa{dist, x->d_alive.p, N, ik, ii, n, (int)k, sn, s.key[pb].p, s.id[pb].p};
+            rk::k_index_select<<<dim3((unsigned)ch, nq), rk::kIdxSelThreads, 2 * sn * sizeof(unsigned long long), m->stream>>>(sa);
+            LAUNCHED(m);
+            if (ch == 1) break;
+            ik = s.key[pb].p, ii = s.id[pb].p, n = ch * k, pb ^= 1;
+        }
+        const int t = nq * (int)k;
+        rk::k_index_finish<<<(t + 255) / 256, 256, 0, m->stream>>>(s.id[pb].p, s.l1.p, s.l2.p, N, nq, (int)k, s.ent.p, s.o1.p,
+                                                                   s.o2.p);
+        LAUNCHED(m);
+        CK(cudaMemcpyAsync(entries_out + b0 * k, s.ent.p, t * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(l1_out + b0 * k, s.o1.p, t * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(l2_out + b0 * k, s.o2.p, t * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+        SYNC(m);
+        for (int q = 0; q < nq; ++q) {
+            unsigned long long f = 0;
+            while (f < k && entries_out[(b0 + q) * k + f] != RWKV_B200_NO_ENTRY) ++f;
+            found_out[b0 + q] = f;
+        }
+    }
     return 0;
 }
 

@@ -17,6 +17,9 @@ NO_CONSTRAINT = 0xFFFFFFFFFFFFFFFF       # RWKV_B200_NO_CONSTRAINT: a stream of 
 MAX_CONSTRAINT_STATES = 65536            # RWKV_B200_MAX_CONSTRAINT_STATES
 NO_STOP_SET = 0xFFFFFFFFFFFFFFFF         # RWKV_B200_NO_STOP_SET: a stream of a stop-string call without a set
 MAX_STOP_BYTES = 4096                    # RWKV_B200_MAX_STOP_BYTES
+INDEX_L1, INDEX_L2 = 0, 1                # RWKV_B200_INDEX_*: the metric a StateIndex search ranks by
+MAX_NEIGHBOURS = 256                     # RWKV_B200_MAX_NEIGHBOURS
+NO_ENTRY = 0xFFFFFFFFFFFFFFFF            # RWKV_B200_NO_ENTRY: a search position past the entries found
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
@@ -350,6 +353,13 @@ def load_library():
         "rwkv_b200_slot_copy": (i32, [vp, ull, ull]),
         "rwkv_b200_slot_upload": (i32, [vp, ull, pdbl, pdbl, pdbl, pdbl, pdbl]),
         "rwkv_b200_slot_download": (i32, [vp, ull, pdbl, pdbl, pdbl, pdbl, pdbl]),
+        "rwkv_b200_index_create": (i32, [vp, ull, ull, ull, pull]),
+        "rwkv_b200_index_free": (i32, [vp, ull]),
+        "rwkv_b200_index_add_slots": (i32, [vp, ull, pull, ull, pull]),
+        "rwkv_b200_index_upload": (i32, [vp, ull, pdbl, ull, pull]),
+        "rwkv_b200_index_download": (i32, [vp, ull, pull, ull, pdbl]),
+        "rwkv_b200_index_remove": (i32, [vp, ull, pull, ull]),
+        "rwkv_b200_index_search": (i32, [vp, ull, pull, ull, i32, c.c_uint, pull, pdbl, pdbl, pull]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)  # AttributeError if a declared symbol is missing
@@ -764,6 +774,52 @@ class Engine:
                 for k in ("xy", "aa", "bb", "pp", "dd")]
         self._ck(self.lib.rwkv_b200_slot_upload(self.h, slot, *[_ptr(a, ctypes.c_double) for a in arrs]), "slot_upload")
 
+    # -- state indexes ---------------------------------------------------------------------
+    def create_index(self, capacity, layers=None):
+        """A StateIndex of `capacity` entries (include/rwkv_b200.h, "State indexes") over `layers`: None for every
+        layer, else a range of consecutive layers."""
+        return StateIndex(self, capacity, layers)
+
+    def embed(self, docs, slots, index):
+        """The vectordb loop in ragged passes: run each document (a list of >= 1 token ids) from a zeroed slot of `slots`
+        and add its final state to `index`. The documents share forward_streams calls of at most max_gpt tokens (state
+        only; a document may span calls), a slot is reused once its document has been added, and the ids of the
+        documents are returned in document order."""
+        seqs = [np.atleast_1d(np.asarray(d, dtype=np.uint64)) for d in docs]
+        free = [int(s) for s in slots]
+        if not free:
+            raise EngineError("embed: no slots")
+        if len(set(free)) != len(free):
+            raise EngineError("embed: a slot appears twice")
+        for i, t in enumerate(seqs):
+            if t.ndim != 1 or len(t) == 0:
+                raise EngineError("embed: document %d has no tokens" % i)
+        ids = [None] * len(seqs)
+        pending = list(range(len(seqs)))[::-1]
+        active = []  # [slot, document, tokens already run], in the order the documents started
+        while pending or active:
+            while free and pending:
+                slot, d = free.pop(0), pending.pop()
+                self.slot_zero(slot)
+                active.append([slot, d, 0])
+            call, room = [], self.max_gpt
+            for a in active:
+                take = min(len(seqs[a[1]]) - a[2], room)
+                if take == 0:
+                    break
+                call.append((a[0], seqs[a[1]][a[2]:a[2] + take]))
+                a[2] += take
+                room -= take
+            self.forward_streams(call, want_logits=False)
+            done = [a for a in active if a[2] == len(seqs[a[1]])]
+            if done:
+                got = index.add([a[0] for a in done])
+                for a, e in zip(done, got):
+                    ids[a[1]] = int(e)
+                    free.append(a[0])
+                active = [a for a in active if a[2] < len(seqs[a[1]])]
+        return ids
+
     # -- state -----------------------------------------------------------------------------
     def state_zero(self):
         self._ck(self.lib.rwkv_b200_state_zero(self.h), "state_zero")
@@ -959,6 +1015,92 @@ class Batcher:
     def close(self):
         if getattr(self, "h", None) and getattr(self.engine, "h", None):
             self.lib.rwkv_b200_batcher_close(self.h)
+        self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+class StateIndex:
+    """An index of state vectors in HBM (include/rwkv_b200.h, "State indexes"): each entry is a slot's dd array over
+    the index's layers, D = n_layers * n_embed float64 elements. Entries get ids 0, 1, 2, ... in the order they are
+    added; removed entries are never returned again. A context manager; close() frees it."""
+
+    def __init__(self, engine, capacity, layers=None):
+        self.engine, self.lib = engine, engine.lib
+        if layers is None:
+            layers = range(engine.n_layers)
+        layers = list(layers)
+        if not layers or layers != list(range(layers[0], layers[0] + len(layers))):
+            raise EngineError("create_index: layers must be a non-empty range of consecutive layers")
+        self.layer_begin, self.n_layers = int(layers[0]), len(layers)
+        self.D = self.n_layers * engine.n_embed
+        self.h = None
+        iid = ctypes.c_ulonglong()
+        engine._ck(self.lib.rwkv_b200_index_create(engine.h, self.layer_begin, self.n_layers, int(capacity),
+                                                   ctypes.byref(iid)), "index_create")
+        self.h = int(iid.value)
+
+    @staticmethod
+    def _ids(ids):
+        return np.ascontiguousarray(np.atleast_1d(np.asarray(ids, dtype=np.uint64)))
+
+    def add(self, slots):
+        """Append the vectors of state slots (a device-to-device copy); returns their ids."""
+        s = self._ids(slots)
+        out = np.zeros(len(s), np.uint64)
+        self.engine._ck(self.lib.rwkv_b200_index_add_slots(self.engine.h, self.h, _ptr(s, ctypes.c_ulonglong), len(s),
+                                                           _ptr(out, ctypes.c_ulonglong)), "index_add_slots")
+        return out
+
+    def upload(self, vectors):
+        """Append vectors [n][D] (float64, finite); returns their ids."""
+        v = np.ascontiguousarray(vectors, dtype=np.float64)
+        if v.ndim == 1:
+            v = v[None, :]
+        if v.ndim != 2 or v.shape[1] != self.D:
+            raise EngineError("index upload: vectors have shape %s, expected (n, %d)" % (v.shape, self.D))
+        out = np.zeros(v.shape[0], np.uint64)
+        self.engine._ck(self.lib.rwkv_b200_index_upload(self.engine.h, self.h, _ptr(v, ctypes.c_double), v.shape[0],
+                                                        _ptr(out, ctypes.c_ulonglong)), "index_upload")
+        return out
+
+    def vectors(self, ids):
+        """The vectors of live entries, [n][D] float64."""
+        e = self._ids(ids)
+        out = np.empty((len(e), self.D), np.float64)
+        self.engine._ck(self.lib.rwkv_b200_index_download(self.engine.h, self.h, _ptr(e, ctypes.c_ulonglong), len(e),
+                                                          _ptr(out, ctypes.c_double)), "index_download")
+        return out
+
+    def remove(self, ids):
+        e = self._ids(ids)
+        self.engine._ck(self.lib.rwkv_b200_index_remove(self.engine.h, self.h, _ptr(e, ctypes.c_ulonglong), len(e)),
+                        "index_remove")
+
+    def search(self, query_slots, k, metric="l2"):
+        """Rank the live entries for each query slot by metric "l1" or "l2": (entries [Q][k] uint64, l1 [Q][k], l2
+        [Q][k], found [Q]); positions past found hold NO_ENTRY and NaN."""
+        metrics = {"l1": INDEX_L1, "l2": INDEX_L2}
+        if metric not in metrics:
+            raise EngineError("index search: metric must be 'l1' or 'l2', not %r" % (metric,))
+        q = self._ids(query_slots)
+        k = int(k)
+        ent = np.zeros((len(q), max(k, 0)), np.uint64)
+        l1, l2 = np.zeros(ent.shape), np.zeros(ent.shape)
+        found = np.zeros(len(q), np.uint64)
+        P, D = ctypes.c_ulonglong, ctypes.c_double
+        self.engine._ck(self.lib.rwkv_b200_index_search(self.engine.h, self.h, _ptr(q, P), len(q), metrics[metric], max(k, 0),
+                                                        _ptr(ent, P), _ptr(l1, D), _ptr(l2, D), _ptr(found, P)),
+                        "index_search")
+        return ent, l1, l2, found
+
+    def close(self):
+        if self.h is not None and getattr(self.engine, "h", None):
+            self.lib.rwkv_b200_index_free(self.engine.h, self.h)
         self.h = None
 
     def __enter__(self):
