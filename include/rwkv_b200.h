@@ -794,8 +794,10 @@ int rwkv_b200_index_search(rwkv_b200_model *m, unsigned long long id, const unsi
                            unsigned long long n_queries, int metric, unsigned int k, unsigned long long *entries_out,
                            double *l1_out, double *l2_out, unsigned long long *found_out);
 
-/* Engine knobs (all optional), key/value strings: "window" / "bwindow" (bulk copies in
- * flight per SM while streaming / while the CTAs exchange vectors), "pf_dist" (tiles the L2
+/* Engine knobs (all optional), key/value strings: "sub_bytes" (largest bulk copy of the
+ * weight stream, a multiple of 16 up to one ring stage of 8 x n_embed bytes), "budget" /
+ * "qbudget" (bytes of copies in flight per SM while streaming, at least one stage / while
+ * the CTAs exchange vectors), "pf_dist" (tiles the L2
  * prefetch runs ahead), "stages" (ring depth), "timeout_ms", "trace", "prefill",
  * "prefill_min", "prefill_graph", "grid" (CTAs, at most the SM count). Returns non-zero for
  * an unknown key. */

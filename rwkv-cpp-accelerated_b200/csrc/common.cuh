@@ -75,9 +75,10 @@ struct Params {
     int L;
     int feed_mode;          // 0: ctrl->token, 1: ctrl->next (free-running), 2: stream[ctrl->pos]
     int greedy;             // 1: finish with an on-device argmax into ctrl->next
-    int window;             // bulk copies in flight per CTA (<= stages)
+    int budget;             // bytes of bulk copies in flight per CTA (>= tile_bytes)
     int vseg;               // segments per ffn-V row (4E/G bytes): 4, 2 or 1 so that a segment is <= E bytes and a tile 8 / vseg rows
-    int bwindow;            // bulk copies in flight per CTA while the consumers exchange vectors (latency of their loads)
+    int qbudget;            // bytes in flight per CTA while the consumers exchange vectors (latency of their loads)
+    int sub_bytes;          // largest bulk copy (a multiple of 16): a ring stage is filled by ceil(tile / sub_bytes) copies
     int pf_dist;            // tiles the L2 prefetch cursor runs ahead of the ring (0 = no L2 prefetch)
     unsigned int ep0;       // epoch before this token: layer l tags its exchanges with ep0 + 1 + l
     unsigned int tk;        // token epoch (tags of the once-per-token exchanges)
@@ -146,6 +147,17 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
                  "selp.u32 %0, 1, 0, p;\n\t}"
                  : "=r"(ok)
                  : "r"(bar), "r"(parity)
+                 : "memory");
+    return ok != 0;
+}
+// Potentially blocking test: the thread may be suspended until the phase completes or about `ns` nanoseconds pass.
+__device__ __forceinline__ bool mbar_try_wait_for(uint32_t bar, uint32_t parity, uint32_t ns) {
+    uint32_t ok;
+    asm volatile("{\n\t.reg .pred p;\n\t"
+                 "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
+                 "selp.u32 %0, 1, 0, p;\n\t}"
+                 : "=r"(ok)
+                 : "r"(bar), "r"(parity), "r"(ns)
                  : "memory");
     return ok != 0;
 }

@@ -71,7 +71,7 @@ __host__ __device__ inline Slices make_slices(int E, int Er, int Vr, int b, int 
 //
 // The schedule of one CTA is a fixed sequence of tiles: per layer the subs K, V, R (own channels), out-proj
 // (own slice), ffn-R (own channels), ffn-K (own key channels), ffn-V (own slice), then the head rows. Two
-// cursors walk it: `cp` issues the bulk copies into the ring (bounded by free stages and by `window` copies in
+// cursors walk it: `cp` fills the ring stages with bulk copies (bounded by free stages and by `budget` bytes in
 // flight), `pf` runs `pf_dist` tiles further ahead and only asks L2 to fetch the bytes
 // (cp.async.bulk.prefetch.L2). The shared-memory ring holds at most 3.7 us of HBM time; a phase boundary
 // takes longer than that, so without the second cursor HBM idles in every boundary and the following phase
@@ -129,9 +129,15 @@ __device__ __forceinline__ bool next_tile(const Params &p, const Slices &sl, Til
     return true;
 }
 
-// `window`: at most that many bulk copies of this CTA are in flight (issued, not landed). The memory
-// system serves the SMs' copies in order, so everything in flight queues AHEAD of the small latency-
-// critical loads of an exchange: 5 x 32 KB per SM is 3.7 us of queue at the HBM rate.
+// A ring stage (one tile) is filled by bulk copies of at most `sub_bytes` each on the stage's one `full` barrier.
+// Flow control counts BYTES in flight (issued, not landed): at most `budget`, `qbudget` while the consumers wait
+// for exchanged words. The memory system serves the SMs' copies in order, so everything in flight queues AHEAD of
+// the small latency-critical loads of an exchange (0.75 us per 32 KB at the HBM rate); copies smaller than a tile
+// let the producer keep some reading going through such a window with less in front of those loads.
+// What is in flight is known per stage only (a stage has landed when its barrier completes): the stages filled
+// and not landed count as whole tiles, plus the bytes issued into the stage being filled. A stage is only left
+// part-filled while the consumers exchange (they do not wait for the ring then), and budget >= tile_bytes lets
+// it be finished afterwards.
 template <bool TRACE>
 __device__ __forceinline__ void produce_token(const Params &p, const Smem &sm, const Slices &sl) {
     unsigned long long *const ptrace = TRACE ? p.ptrace : nullptr;
@@ -146,17 +152,17 @@ __device__ __forceinline__ void produce_token(const Params &p, const Smem &sm, c
     load_sub(p, sl, cp);
     pf = cp;
     bool pf_live = true;
-    int tcount = 0, landed = 0, ahead = 0; // tiles issued; tiles known to have landed; lead of the prefetch cursor over the copy cursor
+    int tcount = 0, landed = 0, ahead = 0; // stages filled; stages known to have landed; lead of the prefetch cursor over the copy cursor
     const volatile uint32_t *const quiet_flag = reinterpret_cast<volatile uint32_t *>(sm.gmax + 3);
     TileRef t;
-    // The pending tile of the copy cursor. A non-blocking loop: top up the L2 prefetches, retire landed copies,
-    // issue the pending copy when a ring stage is free and the in-flight window allows it.
+    // The pending tile of the copy cursor. A non-blocking loop: top up the L2 prefetches, retire landed stages,
+    // issue the next copy of the pending tile when its ring stage is free and the bytes in flight allow it.
     Waiter wt = waiter_begin();
     for (;;) {
         // While the consumers wait for exchanged words (`quiet`), everything this SM has in flight queues ahead of
-        // their loads (0.75 us per 32 KB tile) and every prefetch competes with them in L2: keep at most `bwindow`
-        // copies in flight and prefetch nothing. Epilogues, quantisation and the GEMV itself are not latency-bound:
-        // there the window is `window` copies and L2 is kept `pf_dist` tiles ahead, so HBM keeps streaming.
+        // their loads and every prefetch competes with them in L2: keep at most `qbudget` bytes in flight and
+        // prefetch nothing. Epilogues, quantisation and the GEMV itself are not latency-bound: there the budget is
+        // `budget` bytes and L2 is kept `pf_dist` tiles ahead, so HBM keeps streaming.
         while (pf_live && ahead < 1) { // the prefetch cursor never falls behind the copy cursor
             TileRef q;
             pf_live = next_tile(p, sl, pf, q);
@@ -169,34 +175,42 @@ __device__ __forceinline__ void produce_token(const Params &p, const Smem &sm, c
         }
         if (!next_tile(p, sl, cp, t)) break;
         --ahead;
-        for (;;) { // until the pending tile is issued
-            while (landed < tcount && mbar_test_wait(full0 + 8 * wp.stage, wp.phase)) {
-                wp.advance((uint32_t)p.stages);
-                ++landed;
-            }
-            const int win = *quiet_flag != 0u ? p.bwindow : p.window;
-            // first pass over the ring: a fresh mbarrier reports the "previous" phase as complete
-            const bool slot_free = mbar_test_wait(empty0 + 8 * rp.stage, rp.phase ^ 1);
-            if (tcount - landed < win && slot_free) break;
-            // The ring is full (the consumers are in a boundary) and nobody waits for exchanged words: HBM would idle.
-            // Only then ask L2 for tiles further ahead - while the ring still takes copies, a prefetch of a far tile
-            // would only delay the near ones (same queue, same HBM).
-            if (!slot_free && *quiet_flag == 0u && pf_live && ahead < p.pf_dist + 1) {
-                TileRef q;
-                pf_live = next_tile(p, sl, pf, q);
-                if (pf_live) {
-                    if (p.pf_dist > 0) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(q.ptr), "r"(q.bytes) : "memory");
-                    ++ahead;
+        for (uint32_t off = 0; off < t.bytes;) { // the copies of the pending tile; `off` bytes of it issued
+            for (;;) { // until the next copy is issued
+                while (landed < tcount && mbar_test_wait(full0 + 8 * wp.stage, wp.phase)) {
+                    wp.advance((uint32_t)p.stages);
+                    ++landed;
                 }
-            } else {
-                __nanosleep(40);
+                const uint32_t budget = (uint32_t)(*quiet_flag != 0u ? p.qbudget : p.budget);
+                const uint32_t inflight = (uint32_t)(tcount - landed) * (uint32_t)p.tile_bytes + off;
+                // first pass over the ring: a fresh mbarrier reports the "previous" phase as complete
+                const bool slot_free = off > 0u || mbar_test_wait(empty0 + 8 * rp.stage, rp.phase ^ 1);
+                if (slot_free && (inflight == 0u || inflight + min((uint32_t)p.sub_bytes, t.bytes - off) <= budget)) break;
+                // The ring is full (the consumers are in a boundary) and nobody waits for exchanged words: HBM would idle.
+                // Only then ask L2 for tiles further ahead - while the ring still takes copies, a prefetch of a far tile
+                // would only delay the near ones (same queue, same HBM).
+                if (!slot_free && *quiet_flag == 0u && pf_live && ahead < p.pf_dist + 1) {
+                    TileRef q;
+                    pf_live = next_tile(p, sl, pf, q);
+                    if (pf_live) {
+                        if (p.pf_dist > 0) asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(q.ptr), "r"(q.bytes) : "memory");
+                        ++ahead;
+                    }
+                } else if (!slot_free) { // wake as soon as the consumers release the stage
+                    mbar_try_wait_for(empty0 + 8 * rp.stage, rp.phase ^ 1, 200u);
+                } else { // over the budget: wake as soon as the oldest stage in flight lands
+                    mbar_try_wait_for(full0 + 8 * wp.stage, wp.phase, 200u);
+                }
+                if (waiter_tick(p, wt)) wait_expired(p, kDiagRingEmpty, 0, 0, (unsigned int)tcount, (unsigned int)landed, 0ull);
             }
-            if (waiter_tick(p, wt)) wait_expired(p, kDiagRingEmpty, 0, 0, (unsigned int)tcount, (unsigned int)landed, 0ull);
+            const uint32_t fb = full0 + 8 * rp.stage, n = min((uint32_t)p.sub_bytes, t.bytes - off);
+            if (off == 0u) {
+                mbar_expect_tx(fb, t.bytes);
+                if (ptrace != nullptr && tcount < kTileTraceMax) ptrace[(size_t)blockIdx.x * kTileTraceMax + tcount] = globaltimer();
+            }
+            bulk_g2s(ring + rp.stage * (uint32_t)p.tile_bytes + off, t.ptr + off, n, fb, pol);
+            off += n;
         }
-        const uint32_t fb = full0 + 8 * rp.stage;
-        mbar_expect_tx(fb, t.bytes);
-        bulk_g2s(ring + rp.stage * (uint32_t)p.tile_bytes, t.ptr, t.bytes, fb, pol);
-        if (ptrace != nullptr && tcount < kTileTraceMax) ptrace[(size_t)blockIdx.x * kTileTraceMax + tcount] = globaltimer();
         ++tcount;
         rp.advance((uint32_t)p.stages);
     }

@@ -1,5 +1,5 @@
 """Knob sweep on the bench workload: tokens/s of the device-resident greedy decode for a list of
-(option=value,...) settings.  usage: python sweep.py 7b 64 "window=1,stages=8" "pf_dist=8" ..."""
+(option=value,...) settings.  usage: python sweep.py 7b 64 "sub_bytes=8192,qbudget=16384" "pf_dist=8" ..."""
 import importlib
 import os
 import sys
@@ -12,7 +12,8 @@ pkg = importlib.import_module("rwkv-cpp-accelerated_b200")
 workload, steps = sys.argv[1], int(sys.argv[2])
 L, E = bench.SHAPES[workload]
 ab = bench.algorithmic_bytes_per_token(L, E)
-DEFAULTS = {"window": 2, "bwindow": 1, "pf_dist": 4, "grid": 132}
+TILE = 8 * E  # one ring stage
+DEFAULTS = {"sub_bytes": min(12288, TILE), "budget": 5 * TILE // 2, "qbudget": 5 * TILE // 4, "pf_dist": 4, "grid": 132}
 eng = pkg.Engine(bench.model_path(workload, pkg))
 stages0 = None
 for spec in sys.argv[3:]:
