@@ -731,6 +731,45 @@ int rwkv_b200_batcher_submit_stop(rwkv_b200_batcher *b, const rwkv_b200_request 
 int rwkv_b200_batcher_read_stop(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *hit,
                                 unsigned long long *tail, unsigned long long *state);
 
+/* Speculation in the batcher: a request may opt in to prompt-lookup drafts (rwkv_b200_generate_streams_speculative's
+ * draft rule), so that a step emits several of its tokens where the drafts are right. Its lookup history is context ++
+ * prompt ++ the tokens it has emitted.
+ *   1. Bit for bit the plain batcher. The emitted tokens, log-probabilities, ranks, top entries, final automaton state,
+ *      stop-string hit, tail and state, and the final state of `slot` are bit for bit what the same request gives
+ *      without spec, so the batcher rule above holds for it unchanged, whatever the other traffic, rows,
+ *      prefill_tokens, max_steps and cancellations are.
+ *   2. Steps. rwkv_b200_batcher_read_spec's steps is the steps_out of rwkv_b200_generate_streams_speculative_* for the
+ *      one stream with slots [slot, spare_slots...], first token prompt[n_prompt - 1], lookup context context ++
+ *      prompt[0 .. n_prompt - 1), draft and ngram. Row i of a step draws with u[len + i], as in that call.
+ *   3. Slots. When the request finishes, and at rwkv_b200_batcher_cancel, the state of the row holding the conversation
+ *      is copied to slot (xy, aa, bb and dd), so cancel keeps its promise. The spare slots are scratch: their contents
+ *      after the request are unspecified. Slots that no unfinished request names are never written.
+ *   4. Scheduling. Admission, prefill budgets, 16-step groups and streaming reads are unchanged. The request's decode
+ *      row becomes k + 1 consecutive rows inside one tensor-core pass (rows 1..k chain from row 0's state in the pass);
+ *      the one-token rows come first, and pad tokens that store no state fill a pass a speculative request would
+ *      straddle. A group whose decode rows do not speculate enqueues exactly what it enqueues without this feature.
+ *   5. Refusals, with nothing queued and no id used: draft outside 1..15 or ngram outside 1..8, NULL spare_slots (or
+ *      NULL context with n_context > 0), a spare slot out of range, repeated, equal to slot, or named (as slot or spare)
+ *      by an unfinished request, a context token >= 50277, a presence or frequency penalty (as in the one-shot call:
+ *      a row's counts would have to fold in its own drafts), rows x (draft + 1) > max_gpt, and every refusal of
+ *      rwkv_b200_batcher_submit_stop. A request's slot is refused as well while an unfinished request names it as a
+ *      spare. */
+typedef struct rwkv_b200_request_spec {
+    const unsigned long long *spare_slots; /* [draft] scratch slots; contents after the request are unspecified */
+    unsigned int draft;                    /* k = 1..15 drafts per step */
+    unsigned int ngram;                    /* 1..8, the longest n-gram looked up */
+    const unsigned long long *context;     /* [n_context] extra lookup tokens placed before the prompt; may be NULL if 0 */
+    unsigned long long n_context;
+} rwkv_b200_request_spec;
+
+/* rwkv_b200_batcher_submit_stop with speculation; spec == NULL is exactly submit_stop. */
+int rwkv_b200_batcher_submit_spec(rwkv_b200_batcher *b, const rwkv_b200_request *r, const rwkv_b200_request_ex *x,
+                                  unsigned long long set_id, unsigned long long start_state,
+                                  const rwkv_b200_request_spec *spec, unsigned long long *id);
+/* The steps in which a request emitted a token (0 for a request without speculation). An unknown or released id is
+ * refused. */
+int rwkv_b200_batcher_read_spec(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *steps);
+
 /* State of one slot: zero it (a new conversation), copy it onto another slot (fork a conversation), or move it
  * between the device and host arrays of n_layers x n_embed doubles each (NULL arrays are skipped). */
 int rwkv_b200_slot_zero(rwkv_b200_model *m, unsigned long long slot);

@@ -190,10 +190,11 @@ struct rwkv_b200_model {
     struct Spec {
         DevBuf<rk::SpecStream> ss;        // [n_streams]
         DevBuf<unsigned long long> hist;  // per stream: context, first token, up to max_new emitted tokens
-        DevBuf<int> live;                 // [live streams]
+        DevBuf<rk::SpecLive> live;       // [live streams]
         DevBuf<rk::PassDesc> passes;      // [passes of a step]
         DevBuf<double> u, row_u;          // [max_new][n_streams], [rows]
         DevBuf<unsigned long long> forks; // [n_streams][2] the final copies home -> first slot
+        DevBuf<rk::SpecScore> score;      // [rows] what k_spec_logprob scores (with log-probabilities)
         DevBuf<unsigned long long> row_state; // [rows] each row's automaton state (constrained calls)
     } spec;
     rwkv_b200_batcher *batcher = nullptr; // the open batcher (at most one), closed by rwkv_b200_free
@@ -242,6 +243,12 @@ struct rwkv_b200_batcher {
         // rwkv_b200_batcher_submit_stop: the stop set (gst.next == nullptr: none) with its match state and result
         rk::GenStop gst{};
         unsigned long long stop_set = RWKV_B200_NO_STOP_SET;
+        // rwkv_b200_batcher_submit_spec: k drafts per step (0: none), the n-gram, the spare slots and the lookup context;
+        // the steps that emitted a token and which of [slot, spares...] holds the conversation (home)
+        unsigned draft = 0, ngram = 0;
+        std::vector<unsigned long long> spares, context;
+        unsigned long long steps = 0;
+        int home = 0;
     };
     std::map<unsigned long long, Req> reqs;
     unsigned long long next_id = 1;
@@ -274,6 +281,15 @@ struct rwkv_b200_batcher {
     DevBuf<float> raw;                        // [rows][V] the model's rows of a step, for raw lanes (see batcher_group)
     std::vector<rk::GenStop> h_gst;           // [rows] host mirror of the lanes' stop sets (next nullptr: none)
     DevBuf<rk::GenStop> gst;                  // [rows]
+    // speculative lanes (submit_spec), grown at the first group that has one: the lanes' records, where each lane's
+    // rows lie, the histories and uniforms of the group's speculative lanes, each row's automaton state, and the
+    // copies home -> slot of finished or cancelled requests
+    std::vector<rk::SpecStream> h_ss;         // [rows]
+    DevBuf<rk::SpecStream> ss;                // [rows]
+    DevBuf<rk::SpecLive> spec_live;           // [speculative lanes]
+    DevBuf<rk::SpecScore> score;              // [speculative lanes][largest k + 1] (scored lanes only)
+    DevBuf<unsigned long long> hist, row_state, forks;
+    DevBuf<double> su;
 };
 
 namespace {
@@ -1345,6 +1361,15 @@ int batcher_boundary(B *b, std::vector<int> &dec) {
     return 0;
 }
 
+// The copies home -> slot of speculative requests that end with their conversation on a spare slot: {home, slot}
+// pairs of xy, aa, bb and dd (pp: no tensor-core pass writes it).
+int copy_home(B *b, const std::vector<unsigned long long> &forks) {
+    int rc;
+    if ((rc = b->forks.grow(forks.size()))) return rc;
+    CK(cudaMemcpyAsync(b->forks.p, forks.data(), forks.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, b->m->stream));
+    return fork_slots(b->m, b->forks.p, forks.size() / 2, false);
+}
+
 // One group of at most `max_steps` steps (<= kGenGroup); *ran receives its length. The host lays out every step's
 // passes in advance (prefill never depends on a pick) and uploads them once; the feedback of step k writes the decode
 // rows' tokens and kDescLast bits into step k + 1's layout.
@@ -1380,19 +1405,54 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
         segs.push_back(std::move(s));
     }
     const unsigned long long steps = segs.size();
-    // every step's layout: decode rows (head rows 0..R-1), then the segments without a head
-    std::vector<rk::PassDesc> all(steps * (size_t)b->max_pass);
+    // the decode rows: the one-token lanes first (rows 0..Rp-1, where k_gen_feedback writes them), then k + 1 rows per
+    // speculative lane, each lane's rows inside one pass: pad tokens (no head, no state stored) fill up a pass a lane
+    // would straddle
+    std::vector<const B::Req *> of_lane(b->rows, nullptr);
+    for (unsigned long long id : b->admitted) of_lane[b->reqs[id].lane] = &b->reqs[id];
+    std::vector<int> plain;
+    std::vector<rk::SpecLive> sl;
+    for (int l : dec)
+        if (!of_lane[l]->draft) plain.push_back(l);
+    const int Rp = (int)plain.size();
+    std::vector<unsigned long long> dtok, dslot;
+    std::vector<unsigned char> dhead;
+    std::vector<int> pads, rs(plain); // rs: the lane of each decode row
+    for (int l : plain) {
+        dtok.push_back(b->h_gs[l].tok); // steps > 0: the feedback writes the pick over it
+        dslot.push_back(b->h_gs[l].slot);
+        dhead.push_back(1);
+    }
+    int kmax = 0;
+    for (int l : dec) {
+        const B::Req &q = *of_lane[l];
+        if (!q.draft) continue;
+        const int K1 = (int)q.draft + 1;
+        kmax = std::max(kmax, (int)q.draft);
+        while ((int)dtok.size() % rk::kPfMaxTokens + K1 > rk::kPfMaxTokens) {
+            pads.push_back((int)dtok.size());
+            dtok.push_back(0);
+            dslot.push_back(q.slot);
+            dhead.push_back(0);
+        }
+        sl.push_back(rk::SpecLive{l, (int)rs.size(), (int)dtok.size()});
+        for (int i = 0; i < K1; ++i) { // k_spec_draft writes the tokens and descriptors
+            rs.push_back(l);
+            dtok.push_back(0);
+            dslot.push_back(q.slot);
+            dhead.push_back(1);
+        }
+    }
+    const bool spec = !sl.empty();
+    const int NR = (int)rs.size(); // logits rows of a step
+    // every step's layout: the decode rows, then the segments without a head
+    std::vector<std::vector<rk::PassDesc>> lay(steps);
     std::vector<int> step_rows(steps);
     std::vector<std::vector<int>> H(steps);
+    size_t ps = (size_t)b->max_pass; // passes per step in `passes`
     for (unsigned long long k = 0; k < steps; ++k) {
-        std::vector<unsigned long long> tokens, slots, lens;
-        std::vector<unsigned char> head;
-        for (int r = 0; r < R; ++r) {
-            tokens.push_back(b->h_gs[dec[r]].tok); // steps > 0: the feedback writes the pick over it
-            slots.push_back(b->h_gs[dec[r]].slot);
-            lens.push_back(1);
-            head.push_back(1);
-        }
+        std::vector<unsigned long long> tokens(dtok), slots(dslot), lens(dtok.size(), 1);
+        std::vector<unsigned char> head(dhead);
         for (const Seg &s : segs[k]) {
             const B::Req &q = b->reqs[s.id];
             tokens.insert(tokens.end(), q.prompt.begin() + (long)s.off, q.prompt.begin() + (long)(s.off + s.n));
@@ -1401,38 +1461,48 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
             head.push_back(0);
         }
         step_rows[k] = (int)tokens.size();
-        std::vector<rk::PassDesc> passes;
-        rk::pass_layout(tokens.data(), step_rows[k], slots.data(), lens.data(), 2, nullptr, passes, H[k], head.data());
-        std::copy(passes.begin(), passes.end(), all.begin() + k * b->max_pass);
+        rk::pass_layout(tokens.data(), step_rows[k], slots.data(), lens.data(), 2, nullptr, lay[k], H[k], head.data());
+        for (int p : pads) lay[k][p / rk::kPfMaxTokens].desc[p % rk::kPfMaxTokens] &= ~rk::kDescLast;
+        ps = std::max(ps, lay[k].size());
     }
+    std::vector<rk::PassDesc> all(steps * ps);
+    for (unsigned long long k = 0; k < steps; ++k) std::copy(lay[k].begin(), lay[k].end(), all.begin() + k * ps);
+    // a speculative lane emits up to kGenGroup (k + 1) tokens in a group
+    const size_t W = spec ? kGenGroup * (rk::kSpecMaxDraft + 1) : kGenGroup, ring = (size_t)b->rows * W;
+    if ((rc = b->passes.grow(kGenGroup * ps)) || (rc = b->row_stream.grow(NR)) || (rc = b->u.grow(kGenGroup * NR)) ||
+        (rc = b->out.grow(ring)))
+        return rc;
+    b->h_out.resize(ring);
     CK(cudaMemcpyAsync(b->passes.p, all.data(), all.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
     // what the decode lanes use: each feature's work is enqueued only when one of them needs it
-    bool pen = false, constrained = false, scored = false, raw = false, stopped = false;
+    bool pen = false, constrained = false, scored = false, spec_scored = false, raw = false, stopped = false;
     int top = 0; // the largest top_n of a scored lane
-    std::vector<const B::Req *> of_lane(b->rows, nullptr);
-    for (unsigned long long id : b->admitted) of_lane[b->reqs[id].lane] = &b->reqs[id];
     if (R > 0) {
         CK(cudaMemcpyAsync(b->gs.p, b->h_gs.data(), b->rows * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(b->row_stream.p, dec.data(), R * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-        // uniforms [steps][R]: row r at step k draws with its request's u[len + k]
-        std::vector<double> ug(steps * (size_t)R, 0.0);
-        for (int r = 0; r < R; ++r) {
-            const rk::GenStream &g = b->h_gs[dec[r]];
-            const B::Req &q = *of_lane[dec[r]];
-            for (unsigned long long k = 0; k < steps && !q.u.empty(); ++k)
-                if (g.len + k < q.max_new) ug[k * R + r] = q.u[g.len + k];
+        CK(cudaMemcpyAsync(b->row_stream.p, rs.data(), NR * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        // uniforms [steps][NR]: one-token row r at step k draws with its request's u[len + k] (k_spec_draft writes the
+        // speculative rows')
+        std::vector<double> ug(steps * (size_t)NR, 0.0);
+        for (int l : dec) {
+            const B::Req &q = *of_lane[l];
             pen |= q.sampler.presence_penalty != 0.0f || q.sampler.frequency_penalty != 0.0f;
             constrained |= q.gc.mask != nullptr;
             stopped |= q.gst.next != nullptr;
             if (q.lp.mode >= 0) {
-                scored = true;
+                (q.draft ? spec_scored : scored) = true;
                 raw |= q.lp.mode == RWKV_B200_LOGPROBS_RAW;
                 top = std::max(top, q.lp.top_n);
             }
         }
+        for (int r = 0; r < Rp; ++r) {
+            const rk::GenStream &g = b->h_gs[plain[r]];
+            const B::Req &q = *of_lane[plain[r]];
+            for (unsigned long long k = 0; k < steps && !q.u.empty(); ++k)
+                if (g.len + k < q.max_new) ug[k * NR + r] = q.u[g.len + k];
+        }
         CK(cudaMemcpyAsync(b->u.p, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
     }
-    const size_t V = binfmt::kVocab, ring = (size_t)b->rows * kGenGroup, top_ring = top ? ring * rk::kMaxTopN : 0;
+    const size_t V = binfmt::kVocab, top_ring = top ? ring * rk::kMaxTopN : 0;
     if (constrained) {
         if ((rc = b->gc.grow(b->rows)) || (rc = b->fault.grow(3))) return rc;
         CK(cudaMemcpyAsync(b->gc.p, b->h_gc.data(), b->rows * sizeof(rk::GenConstraint), cudaMemcpyHostToDevice, m->stream));
@@ -1442,47 +1512,107 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
         if ((rc = b->gst.grow(b->rows))) return rc;
         CK(cudaMemcpyAsync(b->gst.p, b->h_gst.data(), b->rows * sizeof(rk::GenStop), cudaMemcpyHostToDevice, m->stream));
     }
+    // the speculative lanes' records, histories (context ++ prompt ++ emitted, with room for the rest) and uniforms
+    if (spec) {
+        std::vector<unsigned long long> hist;
+        std::vector<double> su;
+        for (const rk::SpecLive &e : sl) {
+            const B::Req &q = *of_lane[e.s];
+            rk::SpecStream &g = b->h_ss[e.s];
+            g = rk::SpecStream{};
+            g.slot[0] = q.slot;
+            std::copy(q.spares.begin(), q.spares.end(), g.slot + 1);
+            g.h0 = hist.size();
+            hist.insert(hist.end(), q.context.begin(), q.context.end());
+            hist.insert(hist.end(), q.prompt.begin(), q.prompt.end());
+            hist.insert(hist.end(), q.tokens.begin(), q.tokens.end());
+            g.hl = hist.size() - g.h0;
+            hist.resize(hist.size() + q.max_new - q.tokens.size());
+            g.budget = q.max_new;
+            g.len = q.tokens.size();
+            g.steps = q.steps;
+            g.u0 = su.size();
+            su.resize(su.size() + q.max_new, 0.0);
+            std::copy(q.u.begin(), q.u.end(), su.begin() + (long)g.u0);
+            g.home = q.home;
+            g.k = (int)q.draft;
+            g.ngram = (int)q.ngram;
+        }
+        if ((rc = b->ss.grow(b->rows)) || (rc = b->spec_live.grow(b->rows)) || (rc = b->hist.grow(hist.size())) ||
+            (rc = b->su.grow(su.size())) || (constrained && (rc = b->row_state.grow(NR))) ||
+            (spec_scored && (rc = b->score.grow(sl.size() * (kmax + 1)))))
+            return rc;
+        CK(cudaMemcpyAsync(b->ss.p, b->h_ss.data(), b->rows * sizeof(rk::SpecStream), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(b->spec_live.p, sl.data(), sl.size() * sizeof(rk::SpecLive), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(b->hist.p, hist.data(), hist.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(b->su.p, su.data(), su.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+        if (constrained) { // the one-token rows are masked by their lane's record; k_spec_draft writes the others
+            const std::vector<unsigned long long> st(NR, rk::kStreamState);
+            CK(cudaMemcpyAsync(b->row_state.p, st.data(), NR * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        }
+    }
     // raw lanes read the model's rows: d_slogits itself, or a copy taken before the penalties, overrides and masks edit it
     const bool raw_copy = raw && (pen || b->n_ovr || constrained);
-    if (scored) {
+    if (scored || spec_scored) {
         if ((rc = b->lp_lane.grow(b->rows)) || (rc = b->lp.grow(ring)) || (rc = b->rank.grow(ring)) ||
-            (rc = b->top_lp.grow(top_ring)) || (rc = b->top_tok.grow(top_ring)) || (raw_copy && (rc = b->raw.grow((size_t)b->rows * V))))
+            (rc = b->top_lp.grow(top_ring)) || (rc = b->top_tok.grow(top_ring)) || (raw_copy && (rc = b->raw.grow((size_t)NR * V))))
             return rc;
         CK(cudaMemcpyAsync(b->lp_lane.p, b->h_lp.data(), b->rows * sizeof(rk::LogprobLane), cudaMemcpyHostToDevice, m->stream));
     }
-    const PickChain pc{b->gs.p, b->row_stream.p, b->samp.p, pen ? b->pen_cnt.p : nullptr, b->pen_seen.p, b->ovr_tok.p,
-                       b->ovr_val.p, b->n_ovr, constrained ? b->gc.p : nullptr, 0, b->ovr_start.p};
+    PickChain pc{b->gs.p, b->row_stream.p, b->samp.p, pen ? b->pen_cnt.p : nullptr, b->pen_seen.p, b->ovr_tok.p,
+                 b->ovr_val.p, b->n_ovr, constrained ? b->gc.p : nullptr, 0, b->ovr_start.p};
+    if (spec && constrained) pc.row_state = b->row_state.p;
     const rk::GenLogprobArgs la{m->d_slogits, (int)V, b->gs.p, b->row_stream.p, nullptr, m->d_sample, b->samp.p,
-                                top ? rk::kMaxTopN : 0, kGenGroup, b->lp.p, b->rank.p, b->top_tok.p, b->top_lp.p,
+                                top ? rk::kMaxTopN : 0, W, b->lp.p, b->rank.p, b->top_tok.p, b->top_lp.p,
                                 b->lp_lane.p, raw_copy ? b->raw.p : nullptr};
+    rk::SpecArgs sa{b->ss.p, b->spec_live.p, kmax, false, b->hist.p, nullptr, b->su.p, nullptr, 1, W, nullptr, m->d_sample,
+                    b->stop.p, 0, b->stop_start.p, b->out.p, stopped ? b->gst.p : nullptr, constrained ? b->gc.p : nullptr,
+                    b->row_state.p, b->fault.p, spec_scored ? b->score.p : nullptr};
     for (unsigned long long k = 0; k < steps; ++k) {
-        if ((rc = gen_step_passes(m, b->passes.p + k * b->max_pass, step_rows[k], rk::kPfMaxTokens, H[k].data()))) return rc;
-        if (R == 0) continue;
-        if (raw_copy) CK(cudaMemcpyAsync(b->raw.p, m->d_slogits, (size_t)R * V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
-        if ((rc = pick_rows(m, pc, R, b->u.p + k * R))) return rc;
-        if (scored) {
-            rk::k_gen_logprob<<<(unsigned)R, rk::kNucThreads, 0, m->stream>>>(la);
+        sa.passes = b->passes.p + k * ps;
+        sa.row_u = b->u.p + k * NR;
+        if (spec) {
+            rk::k_spec_draft<<<(unsigned)sl.size(), rk::kSpecDraftThreads, 0, m->stream>>>(sa);
             LAUNCHED(m);
         }
-        rk::GenFeedbackArgs fb{b->gs.p, b->row_stream.p, R, nullptr, m->d_sample, b->stop.p, 0, b->out.p, kGenGroup,
-                               k + 1 < steps ? b->passes.p + (k + 1) * b->max_pass : nullptr, constrained ? b->gc.p : nullptr,
-                               b->fault.p, b->stop_start.p, stopped ? b->gst.p : nullptr};
-        rk::k_gen_feedback<<<(unsigned)((R + 127) / 128), 128, 0, m->stream>>>(fb);
-        LAUNCHED(m);
+        if ((rc = gen_step_passes(m, b->passes.p + k * ps, step_rows[k], rk::kPfMaxTokens, H[k].data()))) return rc;
+        if (R == 0) continue;
+        if (raw_copy) CK(cudaMemcpyAsync(b->raw.p, m->d_slogits, (size_t)NR * V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
+        if ((rc = pick_rows(m, pc, NR, b->u.p + k * NR))) return rc;
+        if (scored) {
+            rk::k_gen_logprob<<<(unsigned)Rp, rk::kNucThreads, 0, m->stream>>>(la);
+            LAUNCHED(m);
+        }
+        if (Rp > 0) {
+            rk::GenFeedbackArgs fb{b->gs.p, b->row_stream.p, Rp, nullptr, m->d_sample, b->stop.p, 0, b->out.p, W,
+                                   k + 1 < steps ? b->passes.p + (k + 1) * ps : nullptr, constrained ? b->gc.p : nullptr,
+                                   b->fault.p, b->stop_start.p, stopped ? b->gst.p : nullptr};
+            rk::k_gen_feedback<<<(unsigned)((Rp + 127) / 128), 128, 0, m->stream>>>(fb);
+            LAUNCHED(m);
+        }
+        if (spec) {
+            rk::k_spec_accept<<<(unsigned)sl.size(), 32, 0, m->stream>>>(sa);
+            LAUNCHED(m);
+            if (spec_scored) {
+                rk::k_spec_logprob<<<(unsigned)(sl.size() * (kmax + 1)), rk::kNucThreads, 0, m->stream>>>(sa, la);
+                LAUNCHED(m);
+            }
+        }
     }
     // the group's end: the lanes' records and the tokens of the group (with their results and the automata's states
     // when a lane uses them) come back with one synchronisation
     unsigned long long fault[3] = {0, 0, 0};
     if (R > 0) {
         CK(cudaMemcpyAsync(b->h_gs.data(), b->gs.p, b->rows * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
-        CK(cudaMemcpyAsync(b->h_out.data(), b->out.p, b->h_out.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(b->h_out.data(), b->out.p, ring * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
     }
+    if (spec) CK(cudaMemcpyAsync(b->h_ss.data(), b->ss.p, b->rows * sizeof(rk::SpecStream), cudaMemcpyDeviceToHost, m->stream));
     if (constrained) {
         CK(cudaMemcpyAsync(b->h_gc.data(), b->gc.p, b->rows * sizeof(rk::GenConstraint), cudaMemcpyDeviceToHost, m->stream));
         CK(cudaMemcpyAsync(fault, b->fault.p, sizeof(fault), cudaMemcpyDeviceToHost, m->stream));
     }
     if (stopped) CK(cudaMemcpyAsync(b->h_gst.data(), b->gst.p, b->rows * sizeof(rk::GenStop), cudaMemcpyDeviceToHost, m->stream));
-    if (scored) {
+    if (scored || spec_scored) {
         b->h_lpv.resize(ring);
         b->h_rank.resize(ring);
         b->h_top_lp.resize(top_ring);
@@ -1502,28 +1632,42 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
         return fail(8, "batcher_run: request %llu emitted token %llu, which has no edge out of state %llu of its constraint", rid,
                     fault[1], fault[2]);
     }
+    std::vector<unsigned long long> forks; // finished speculative requests whose home is a spare: home -> slot
     for (unsigned long long id : b->admitted) {
         B::Req &q = b->reqs[id];
         if (q.status == RWKV_B200_REQ_PREFILLING) {
             q.fed = fed[id];
             continue;
         }
-        const rk::GenStream &g = b->h_gs[q.lane];
-        for (unsigned long long j = q.tokens.size(); j < g.len; ++j) {
-            const size_t e = (size_t)q.lane * kGenGroup + j % kGenGroup;
-            q.tokens.push_back(b->h_out[e]);
+        const rk::SpecStream &e = b->h_ss[q.lane];
+        const unsigned long long len = q.draft ? e.len : b->h_gs[q.lane].len;
+        for (unsigned long long j = q.tokens.size(); j < len; ++j) {
+            const size_t x = (size_t)q.lane * W + j % W;
+            q.tokens.push_back(b->h_out[x]);
             if (q.lp.mode < 0) continue;
-            q.logprobs.push_back(b->h_lpv[e]);
-            q.ranks.push_back(b->h_rank[e]);
+            q.logprobs.push_back(b->h_lpv[x]);
+            q.ranks.push_back(b->h_rank[x]);
             for (int t = 0; t < q.lp.top_n; ++t) {
-                q.top_tokens.push_back(b->h_top_tok[e * rk::kMaxTopN + t]);
-                q.top_logprobs.push_back(b->h_top_lp[e * rk::kMaxTopN + t]);
+                q.top_tokens.push_back(b->h_top_tok[x * rk::kMaxTopN + t]);
+                q.top_logprobs.push_back(b->h_top_lp[x * rk::kMaxTopN + t]);
             }
         }
         if (q.gc.mask) q.gc.state = b->h_gc[q.lane].state;
         if (q.gst.next) q.gst = b->h_gst[q.lane];
-        if (g.done) q.status = RWKV_B200_REQ_DONE;
+        if (q.draft) {
+            q.steps = e.steps;
+            q.home = e.home;
+        }
+        if (q.draft ? e.done : b->h_gs[q.lane].done) {
+            q.status = RWKV_B200_REQ_DONE;
+            if (q.home) {
+                forks.push_back(e.slot[q.home]);
+                forks.push_back(q.slot);
+                q.home = 0;
+            }
+        }
     }
+    if (!forks.empty() && (rc = copy_home(b, forks))) return rc;
     // finished requests leave here, before the next boundary admits anyone (a caller may release them in between)
     auto &ad = b->admitted;
     ad.erase(std::remove_if(ad.begin(), ad.end(),
@@ -2224,7 +2368,8 @@ int rwkv_b200_generate_streams_speculative_constrained(
     const int per_pass = rk::kPfMaxTokens / (int)K1; // streams per pass: a stream's rows never straddle two passes
     const size_t n_pass = (size_t)((S + per_pass - 1) / per_pass);
     if ((rc = sp.ss.grow(S)) || (rc = sp.hist.grow(n_hist)) || (rc = sp.live.grow(S)) || (rc = sp.passes.grow(n_pass)) ||
-        (u && ((rc = sp.u.grow(max_new * S)) || (rc = sp.row_u.grow(S * K1)))) || (rc = sp.forks.grow(2 * S)))
+        (u && ((rc = sp.u.grow(max_new * S)) || (rc = sp.row_u.grow(S * K1)))) || (rc = sp.forks.grow(2 * S)) ||
+        (scored && (rc = sp.score.grow(S * K1))))
         return rc;
     if ((rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
     m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
@@ -2240,6 +2385,9 @@ int rwkv_b200_generate_streams_speculative_constrained(
         r.h0 = h0;
         r.hl = c1 - c0 + 1;
         r.budget = budgets ? budgets[s] : max_new;
+        r.u0 = s;
+        r.k = (int)draft;
+        r.ngram = (int)ngram;
         std::copy(context + c0, context + c1, hist.begin() + h0);
         hist[h0 + c1 - c0] = first_tokens[s];
         h0 += r.hl + max_new;
@@ -2263,10 +2411,12 @@ int rwkv_b200_generate_streams_speculative_constrained(
     }
 
     std::vector<int> live(S), rs;
+    std::vector<rk::SpecLive> lv;
     for (unsigned long long s = 0; s < S; ++s) live[s] = (int)s;
-    rk::SpecArgs sa{sp.ss.p, sp.live.p, (int)draft, (int)ngram, per_pass, sp.hist.p, sp.passes.p, u ? sp.u.p : nullptr,
-                    sp.row_u.p, S, max_new, samplers ? nullptr : m->d_next, m->d_sample, g.stop.p, (int)n_stop, g.out.p,
-                    stopped ? g.gst.p : nullptr, constrained ? g.gc.p : nullptr, sp.row_state.p, g.fault.p};
+    rk::SpecArgs sa{sp.ss.p, sp.live.p, (int)draft, true, sp.hist.p, sp.passes.p, u ? sp.u.p : nullptr, sp.row_u.p, S, max_new,
+                    samplers ? nullptr : m->d_next, m->d_sample, g.stop.p, (int)n_stop, nullptr, g.out.p,
+                    stopped ? g.gst.p : nullptr, constrained ? g.gc.p : nullptr, sp.row_state.p, g.fault.p,
+                    scored ? sp.score.p : nullptr};
     PickChain pc{nullptr, g.row_stream, samplers ? g.samp.p : nullptr, nullptr, nullptr, g.ovr_tok.p, g.ovr_val.p, n_override};
     if (constrained) {
         pc.gc = g.gc.p;
@@ -2290,7 +2440,10 @@ int rwkv_b200_generate_streams_speculative_constrained(
         const unsigned long long steps = std::min(kGenGroup, max_new - step);
         rs.resize(rows);
         for (int r = 0; r < rows; ++r) rs[r] = live[r / (int)K1];
-        CK(cudaMemcpyAsync(sp.live.p, live.data(), n_live * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        lv.resize(n_live);
+        for (int li = 0; li < n_live; ++li)
+            lv[li] = rk::SpecLive{live[li], li * (int)K1, li / per_pass * rk::kPfMaxTokens + li % per_pass * (int)K1};
+        CK(cudaMemcpyAsync(sp.live.p, lv.data(), n_live * sizeof(rk::SpecLive), cudaMemcpyHostToDevice, m->stream));
         CK(cudaMemcpyAsync(g.row_stream, rs.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
         for (unsigned long long k = 0; k < steps; ++k) {
             rk::k_spec_draft<<<(unsigned)n_live, rk::kSpecDraftThreads, 0, m->stream>>>(sa);
@@ -2829,6 +2982,7 @@ int rwkv_b200_batcher_open(rwkv_b200_model *m, unsigned long long rows, unsigned
     b->h_gc.assign(rows, rk::GenConstraint{});
     b->h_lp.assign(rows, rk::LogprobLane{-1, 0});
     b->h_gst.assign(rows, rk::GenStop{});
+    b->h_ss.assign(rows, rk::SpecStream{});
     if ((rc = b->gs.grow(rows)) || (rc = b->row_stream.grow(rows)) || (rc = b->passes.grow(kGenGroup * (size_t)b->max_pass)) ||
         (rc = b->samp.grow(rows)) || (rc = b->stop_start.grow(rows + 1)) || (rc = b->out.grow(rows * kGenGroup)) ||
         (rc = b->u.grow(kGenGroup * rows))) {
@@ -2865,9 +3019,12 @@ int rwkv_b200_batcher_submit_ex(rwkv_b200_batcher *b, const rwkv_b200_request *r
             (x->logprobs && (rc = check_logprob_mode(what, x->logprob_mode, x->top_n))))
             return rc;
     }
-    for (const auto &e : b->reqs)
-        if (e.second.slot == r->slot && e.second.status <= RWKV_B200_REQ_GENERATING)
+    for (const auto &e : b->reqs) {
+        const B::Req &o = e.second;
+        if (o.status <= RWKV_B200_REQ_GENERATING &&
+            (o.slot == r->slot || std::find(o.spares.begin(), o.spares.end(), r->slot) != o.spares.end()))
             return fail(1, "%s: slot %llu is held by unfinished request %llu", what, r->slot, e.first);
+    }
     B::Req q;
     q.slot = r->slot;
     q.max_new = r->max_new;
@@ -2965,6 +3122,59 @@ int rwkv_b200_batcher_submit_stop(rwkv_b200_batcher *b, const rwkv_b200_request 
     return 0;
 }
 
+int rwkv_b200_batcher_submit_spec(rwkv_b200_batcher *b, const rwkv_b200_request *r, const rwkv_b200_request_ex *x,
+                                  unsigned long long set_id, unsigned long long start_state, const rwkv_b200_request_spec *spec,
+                                  unsigned long long *id) {
+    const char *what = "batcher_submit_spec";
+    int rc = check_batcher(b);
+    if (rc) return rc;
+    if (spec) {
+        M *m = b->m;
+        if (!r) return fail(1, "%s: null argument (the request and id are required)", what);
+        if (spec->draft < 1 || spec->draft > (unsigned)rk::kSpecMaxDraft)
+            return fail(1, "%s: draft %u is outside 1..%d", what, spec->draft, rk::kSpecMaxDraft);
+        if (spec->ngram < 1 || spec->ngram > (unsigned)rk::kSpecMaxNgram)
+            return fail(1, "%s: ngram %u is outside 1..%d", what, spec->ngram, rk::kSpecMaxNgram);
+        if (!spec->spare_slots) return fail(1, "%s: spare_slots is NULL", what);
+        if (spec->n_context && !spec->context) return fail(1, "%s: %llu context tokens with NULL context", what, spec->n_context);
+        if ((unsigned long long)b->rows * (spec->draft + 1ull) > m->max_gpt)
+            return fail(1, "%s: rows %d x (draft %u + 1) > max_gpt %llu", what, b->rows, spec->draft, m->max_gpt);
+        if (r->sampler.presence_penalty != 0.0f || r->sampler.frequency_penalty != 0.0f)
+            return fail(1, "%s: presence and frequency penalties are not supported (a row's counts would have to include "
+                           "its own drafts)", what);
+        if ((rc = check_slots(m, what, spec->spare_slots, spec->draft)) ||
+            (rc = check_tokens(what, "context token", spec->context, spec->n_context)))
+            return rc;
+        for (unsigned i = 0; i < spec->draft; ++i) {
+            const unsigned long long z = spec->spare_slots[i];
+            if (z == r->slot) return fail(1, "%s: spare slot %llu is the request's slot", what, z);
+            for (const auto &e : b->reqs) {
+                const B::Req &o = e.second;
+                if (o.status <= RWKV_B200_REQ_GENERATING &&
+                    (o.slot == z || std::find(o.spares.begin(), o.spares.end(), z) != o.spares.end()))
+                    return fail(1, "%s: spare slot %llu is held by unfinished request %llu", what, z, e.first);
+            }
+        }
+    }
+    if ((rc = rwkv_b200_batcher_submit_stop(b, r, x, set_id, start_state, id)) || !spec) return rc;
+    B::Req &q = b->reqs.at(*id);
+    q.draft = spec->draft;
+    q.ngram = spec->ngram;
+    q.spares.assign(spec->spare_slots, spec->spare_slots + spec->draft);
+    if (spec->n_context) q.context.assign(spec->context, spec->context + spec->n_context);
+    return 0;
+}
+
+int rwkv_b200_batcher_read_spec(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *steps) {
+    int rc = check_batcher(b);
+    if (rc) return rc;
+    const auto it = b->reqs.find(id);
+    if (it == b->reqs.end()) return fail(1, "batcher_read_spec: request %llu is unknown or released", id);
+    if (!steps) return fail(1, "batcher_read_spec: steps is NULL");
+    *steps = it->second.steps;
+    return 0;
+}
+
 int rwkv_b200_batcher_read_stop(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *hit, unsigned long long *tail,
                                 unsigned long long *state) {
     int rc = check_batcher(b);
@@ -2988,6 +3198,11 @@ int rwkv_b200_batcher_cancel(rwkv_b200_batcher *b, unsigned long long id) {
     if (q.status == RWKV_B200_REQ_QUEUED) {
         b->queue.erase(std::find(b->queue.begin(), b->queue.end(), id));
     } else {
+        if (q.home) { // the conversation is on a spare slot
+            CK(cudaSetDevice(b->m->device));
+            if ((rc = copy_home(b, {q.spares[q.home - 1], q.slot}))) return rc;
+            q.home = 0;
+        }
         b->admitted.erase(std::find(b->admitted.begin(), b->admitted.end(), id));
         b->lane_used[q.lane] = 0;
     }

@@ -66,6 +66,8 @@ struct GenConstraint {
 
 // No state: a missing edge, and the per-row state of a row that is not masked (k_gen_mask's row_state).
 constexpr unsigned long long kNoState = ~0ull;
+// The row_state of a batcher row that is not speculative: masked by its stream's record, as without row_state.
+constexpr unsigned long long kStreamState = ~0ull - 1;
 
 // The target of token tok's edge out of state q, or kNoState when q has no edge for tok: a binary search over q's
 // ascending edge tokens.
@@ -100,18 +102,16 @@ __device__ __forceinline__ bool gen_constraint_step(GenConstraint &c, unsigned l
 // (ceil(V / kMaskThreads), rows), one thread per token. Unconstrained and finished streams are left alone: a finished
 // stream may sit in a state without edges, and masking its row would leave the pick no finite value. With row_state
 // (speculative generation), row r is masked by state row_state[r] of its stream's automaton instead, and left alone
-// where that is kNoState; gs is not read.
+// where that is kNoState; where it is kStreamState (a batcher's one-token lane) the row follows the rule without it.
 constexpr int kMaskThreads = 256;
 __global__ void __launch_bounds__(kMaskThreads) k_gen_mask(float *logits, int V, const GenStream *gs, const int *row_stream,
                                                            const GenConstraint *gc,
                                                            const unsigned long long *row_state = nullptr) {
     const int r = blockIdx.y, s = row_stream[r];
     const GenConstraint &c = gc[s];
-    unsigned long long q;
-    if (row_state) {
-        q = row_state[r];
-        if (q == kNoState) return;
-    } else {
+    unsigned long long q = row_state ? row_state[r] : kStreamState;
+    if (q == kNoState) return;
+    if (q == kStreamState) {
         if (!c.mask || gs[s].done) return;
         q = c.state;
     }

@@ -160,15 +160,10 @@ struct GenLogprobArgs {
     const float *raw;
 };
 
-// generate_streams_logprobs: one CTA of kNucThreads per row of the step, between the pick and k_gen_feedback. It scores
-// the picked token of a live stream at entry [s][len]; with `lane` (the batcher) at [s][len % max_new], a ring of
-// kGenGroup entries per lane, as k_gen_feedback keeps its tokens. A stream that finished earlier in the group still has a row, and its len may equal max_new, so writing
-// for it would land on stream s + 1; it and a batcher lane without scoring return at once (the whole CTA, before any
-// barrier).
-__global__ void __launch_bounds__(kNucThreads) k_gen_logprob(const GenLogprobArgs a) {
-    const int r = blockIdx.x, s = a.row_stream[r];
-    const GenStream &g = a.gs[s];
-    if (g.done) return;
+// Score pick y of row r of the step, stream s, into entry o of the result arrays: on a.logits divided by the stream's
+// temperature with a.samp (processed mode), else on a.logits; a batcher lane by its own mode and top_n, raw lanes on
+// a.raw when set. A lane without scoring returns at once (the whole CTA, before any barrier).
+__device__ __forceinline__ void gen_logprob_at(const GenLogprobArgs &a, int s, int r, int y, size_t o) {
     const float *logits = a.logits;
     const rwkv_b200_sampler *samp = a.samp;
     int top_n = a.top_n;
@@ -181,12 +176,23 @@ __global__ void __launch_bounds__(kNucThreads) k_gen_logprob(const GenLogprobArg
             if (a.raw) logits = a.raw;
         }
     }
-    const int y = a.next ? (int)a.next[r] : (int)a.sample[2 * r];
     const float T = samp ? samp[s].temperature : 0.0f;
-    // the division only where it can matter: a 64-bit `%` on every path costs k_gen_logprob spills at 64 registers
-    const size_t o = (size_t)s * a.max_new + (a.lane ? g.len % a.max_new : g.len);
     logprob_row(logits + (size_t)r * a.V, a.V, y, T > 0.0f ? (double)T : 1.0, top_n, a.logprob + o, a.rank + o,
                 a.top_tokens + o * a.top_n, a.top_logprobs + o * a.top_n);
+}
+
+// generate_streams_logprobs: one CTA of kNucThreads per row of the step, between the pick and k_gen_feedback. It scores
+// the picked token of a live stream at entry [s][len]; with `lane` (the batcher) at [s][len % max_new], a ring of
+// entries per lane, as k_gen_feedback keeps its tokens. A stream that finished earlier in the group still has a row, and
+// its len may equal max_new, so writing for it would land on stream s + 1; it returns at once (the whole CTA, before any
+// barrier).
+__global__ void __launch_bounds__(kNucThreads) k_gen_logprob(const GenLogprobArgs a) {
+    const int r = blockIdx.x, s = a.row_stream[r];
+    const GenStream &g = a.gs[s];
+    if (g.done) return;
+    const int y = a.next ? (int)a.next[r] : (int)a.sample[2 * r];
+    // the division only where it can matter: a 64-bit `%` on every path costs k_gen_logprob spills at 64 registers
+    gen_logprob_at(a, s, r, y, (size_t)s * a.max_new + (a.lane ? g.len % a.max_new : g.len));
 }
 
 } // namespace rk

@@ -1,5 +1,6 @@
-// speculate.cuh — device side of rwkv_b200_generate_streams_speculative: prompt-lookup drafts verified in the tensor-core
-// pass, so that a step can emit several tokens per stream with the bits of one-token-per-step generation.
+// speculate.cuh — device side of rwkv_b200_generate_streams_speculative and of the batcher's speculative lanes
+// (rwkv_b200_batcher_submit_spec): prompt-lookup drafts verified in the tensor-core pass, so that a step can emit several
+// tokens per stream with the bits of one-token-per-step generation.
 //
 // A call keeps one record per stream (SpecStream): its k + 1 slots, which of them is home (holds the conversation),
 // its history (lookup context ++ first token ++ tokens emitted so far) and its length, budget and step count. Each step
@@ -9,15 +10,20 @@
 //                  then the step's layout: row 0 = the current input on the home slot (first | last), row i = draft i on
 //                  the stream's i-th other slot (last), so every row stores its state in its own slot; and the uniform
 //                  of each row for k_sample_nucleus;
-//   forward        the tensor-core passes, floor(128 / (k + 1)) streams per pass, every row a head row;
+//   forward        the tensor-core passes; a stream's k + 1 rows are consecutive head rows inside one pass (SpecLive);
 //   k_gen_override, then k_sample_nucleus or k_argmax_rows on the rows (row_stream maps every row of s to s);
 //   k_spec_accept  one CTA per live stream: the picks, the accepted prefix, stops and budget, the emitted tokens into
 //                  the output and the history, and the new home: the slot of the row that produced the last emitted token;
 //   k_spec_logprob (with log-probabilities) one CTA per row: the emitted token of the row, if it emitted one, scored.
 // With token automata, k_spec_draft also walks the drafts through the stream's automaton into a state per row, by which
 // k_gen_mask masks the rows, and k_spec_accept advances the automaton by each emitted token (DESIGN §4.3).
-// At the end of the call, a stream whose home is not its first slot has the home's xy, aa, bb and dd copied to the first
-// slot (k_beam_fork with four arrays). The rule is stated in include/rwkv_b200.h and DESIGN §4.3.
+// The one-shot call gives every stream the same k and lays out floor(128 / (k + 1)) streams per pass, every row a head
+// row, and k_spec_draft writes the passes' head maps. The batcher mixes streams of different k with one-token lanes
+// (k_gen_feedback's) and prefill segments: the host lays out the head maps once per group, and each stream's outputs go
+// to a ring of kGenGroup (kSpecMaxDraft + 1) entries per lane (`% max_new`, which leaves the one-shot index alone).
+// At the end of the call, or when a batcher request ends, a stream whose home is not its first slot has the home's xy,
+// aa, bb and dd copied to the first slot (k_beam_fork with four arrays). The rule is stated in include/rwkv_b200.h and
+// DESIGN §4.3.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -38,38 +44,57 @@ struct SpecStream {
     unsigned long long h0, hl;                  // the history is hist[h0 .. h0 + hl); its last token is the next input
     unsigned long long budget, len, steps;      // tokens it may emit, tokens emitted, steps that emitted a token
     unsigned long long done;                    // 1 after a stop token or the budget
+    unsigned long long u0;                      // row i of a step draws u[u0 + (len + i) * u_stride] (SpecArgs)
     int home;                                   // index into slot[] of the slot holding the conversation
-    int emitted;                                // tokens the last step emitted: len - emitted .. len - 1
+    int k, ngram;                               // drafts per step (1..kSpecMaxDraft), longest n-gram looked up
+};
+
+// Where a live stream's rows lie in a step: its record, the logits row of its row 0 (rows row0 .. row0 + k), and the
+// position of row 0 in the step's layout (pass pos0 / 128, token pos0 % 128; the k + 1 rows never straddle a pass).
+struct SpecLive {
+    int s, row0, pos0;
+};
+
+// What k_spec_logprob scores for row i of live stream li, at [li * (SpecArgs::k + 1) + i]: the row, its stream and the
+// result entry of the token it emitted this step; s < 0: the row emitted nothing.
+struct SpecScore {
+    int r, s;
+    unsigned long long o;
 };
 
 struct SpecArgs {
     SpecStream *ss;                  // [n_streams]
-    const int *live;                 // [live streams] the stream of CTA i; its rows are i * (k + 1) .. + k
-    int k, ngram, per_pass;          // drafts, longest n-gram, streams per pass
+    const SpecLive *live;            // [live streams] CTA i's stream and rows
+    int k;                           // the largest k of the live streams: k_spec_logprob's CTAs per stream, less one
+    bool heads;                      // k_spec_draft writes the head maps (every row of a pass a head row, in order)
     unsigned long long *hist;        // the histories
     PassDesc *passes;                // the step's passes
-    const double *u;                 // [max_new][n_streams], or nullptr
+    const double *u;                 // the uniforms, or nullptr
     double *row_u;                   // [rows] the uniform of each row (with u only)
-    unsigned long long n_streams, max_new;
+    unsigned long long u_stride, max_new;
     const unsigned long long *next;  // arg-max per row, or nullptr when sampling
     const double *sample;            // {token, margin} per row when sampling
-    const unsigned long long *stop;  // [n_stop]
+    const unsigned long long *stop;  // [n_stop], or the tokens stop_start indexes
     int n_stop;
-    unsigned long long *out;         // [n_streams][max_new]
+    const unsigned long long *stop_start; // the batcher: stream s's stop tokens are stop[stop_start[s] .. [s + 1])
+    unsigned long long *out;         // [n_streams][max_new]: token j of stream s at [s][j % max_new]
     GenStop *gst;                    // [n_streams] generate_streams_speculative_stop, else nullptr
     // generate_streams_speculative_constrained with token automata, else nullptr: each stream's automaton and state, the
     // state of each row this step (kNoState: not masked) and the record of an emitted token without an edge
     GenConstraint *gc;               // [n_streams]
     unsigned long long *row_state;   // [rows]
     unsigned long long *fault;       // [3]
+    SpecScore *score;                // [live streams][k + 1] with log-probabilities, else nullptr
 };
 
 // Draft rule: for n = ngram down to 1 with n < L, the largest j <= L - n - 1 with h[j .. j + n) == h[L - n .. L); the
 // first n with such a j gives the proposal h[j + n .. min(j + n + k, L)], padded with its last token; no match at any n:
 // k copies of h[L - 1]. Draft i (1-based) is then h[min(j + n + i - 1, L - 1)].
 __global__ void __launch_bounds__(kSpecDraftThreads) k_spec_draft(const SpecArgs a) {
-    const int li = blockIdx.x, s = a.live[li], tid = threadIdx.x, k = a.k;
+    const SpecLive lv = a.live[blockIdx.x];
+    const int s = lv.s, tid = threadIdx.x;
     SpecStream &g = a.ss[s];
+    const int k = g.k, ngram = g.ngram;
     const unsigned long long *h = a.hist + g.h0;
     const long long L = (long long)g.hl;
     const bool live = g.done == 0;
@@ -77,9 +102,9 @@ __global__ void __launch_bounds__(kSpecDraftThreads) k_spec_draft(const SpecArgs
     __shared__ int wmax[kSpecDraftThreads / 32];
     long long from = -1; // the proposal starts at h[from]
     if (live) {
-        if (tid < a.ngram && tid < L) suf[tid] = h[L - 1 - tid];
+        if (tid < ngram && tid < L) suf[tid] = h[L - 1 - tid];
         __syncthreads();
-        for (int n = a.ngram; n >= 1 && from < 0; --n) {
+        for (int n = ngram; n >= 1 && from < 0; --n) {
             if (n >= L) continue;
             int best = -1;
             for (long long j = tid; j <= L - n - 1; j += kSpecDraftThreads) {
@@ -99,7 +124,7 @@ __global__ void __launch_bounds__(kSpecDraftThreads) k_spec_draft(const SpecArgs
     auto row_tok = [&](int i) { return i == 0 || from < 0 ? h[L - 1] : h[min(from + i - 1, L - 1)]; };
     const unsigned long long tok = row_tok(tid);
     g.row[tid] = tok;
-    const int r = li * (k + 1) + tid, pi = li / a.per_pass, t = (li % a.per_pass) * (k + 1) + tid;
+    const int r = lv.row0 + tid, pi = (lv.pos0 + tid) / kPfMaxTokens, t = (lv.pos0 + tid) % kPfMaxTokens;
     if (a.gc && tid == 0) {
         // row 0 has the stream's state; row i is live while row i - 1 is, draft i has an edge out of its state and that
         // edge leads to a state with edges. A dead row cannot be emitted: with no edge, the pick of the masked row
@@ -118,25 +143,30 @@ __global__ void __launch_bounds__(kSpecDraftThreads) k_spec_draft(const SpecArgs
     PassDesc &pd = a.passes[pi];
     pd.tokens[t] = tok;
     pd.desc[t] = (uint32_t)g.slot[(g.home + tid) % (k + 1)] | (tid == 0 ? kDescFirst : 0u) | (live ? kDescLast : 0u);
-    pd.rows[t] = t;
-    if (t == 0) pd.out_row0 = pi * a.per_pass * (k + 1);
-    if (a.u) {
+    if (a.heads) {
+        pd.rows[t] = t;
+        if (t == 0) pd.out_row0 = r;
+    }
+    if (a.u) { // a row past the budget is never emitted
         const unsigned long long pos = g.len + (unsigned long long)tid;
-        a.row_u[r] = pos < a.max_new ? a.u[pos * a.n_streams + (unsigned long long)s] : 0.0;
+        a.row_u[r] = pos < g.budget ? a.u[g.u0 + pos * a.u_stride] : 0.0;
     }
 }
 
 // One warp per live stream: lane i holds the pick p_i of row i; a = the leading i in 1..k with row[i] == p_{i - 1}.
 // Lane 0 emits p_0 .. p_a with k_gen_feedback's checks in its order (budget, stop tokens, automaton, stop strings) and
-// moves home to the slot of the last row used.
+// moves home to the slot of the last row used. With `score`, it records what k_spec_logprob scores: row i emitted p_i at
+// entry [s][(len + i) % max_new] (the one-shot index is below max_new; the batcher's is a ring), or nothing.
 __global__ void __launch_bounds__(32) k_spec_accept(const SpecArgs a) {
-    const int li = blockIdx.x, s = a.live[li], lane = threadIdx.x, k = a.k;
+    const SpecLive lv = a.live[blockIdx.x];
+    const int s = lv.s, lane = threadIdx.x;
     SpecStream &g = a.ss[s];
+    SpecScore *sc = a.score ? a.score + (size_t)blockIdx.x * (a.k + 1) : nullptr;
     if (g.done) {
-        if (lane == 0) g.emitted = 0;
+        if (sc && lane <= a.k) sc[lane].s = -1;
         return;
     }
-    const int r = li * (k + 1) + lane;
+    const int k = g.k, r = lv.row0 + lane;
     unsigned long long p = 0;
     if (lane <= k) p = a.next ? a.next[r] : (unsigned long long)a.sample[2 * r];
     const unsigned long long prev = __shfl_up_sync(0xffffffffu, p, 1);
@@ -151,37 +181,39 @@ __global__ void __launch_bounds__(32) k_spec_accept(const SpecArgs a) {
     bool stop = false;
     for (int i = 0; i <= acc && !stop; ++i) {
         const unsigned long long tok = pk[i];
-        a.out[(size_t)s * a.max_new + len] = tok;
+        a.out[(size_t)s * a.max_new + len % a.max_new] = tok;
         a.hist[g.h0 + hl] = tok;
         ++len;
         ++hl;
         e = i;
         stop = len == g.budget;
-        for (int z = 0; z < a.n_stop; ++z) stop |= a.stop[z] == tok;
+        if (a.stop_start) {
+            for (unsigned long long z = a.stop_start[s]; z < a.stop_start[s + 1]; ++z) stop |= a.stop[z] == tok;
+        } else {
+            for (int z = 0; z < a.n_stop; ++z) stop |= a.stop[z] == tok;
+        }
         if (a.gc && a.gc[s].mask) stop |= gen_constraint_step(a.gc[s], tok, s, a.fault);
         if (a.gst && a.gst[s].next) stop |= gen_stop_walk(a.gst[s], tok);
+    }
+    for (int i = 0; sc && i <= a.k; ++i) {
+        const unsigned long long j = g.len + (unsigned long long)i;
+        sc[i] = i <= e ? SpecScore{lv.row0 + i, s, (size_t)s * a.max_new + j % a.max_new} : SpecScore{0, -1, 0};
     }
     g.len = len;
     g.hl = hl;
     g.steps += 1;
-    g.emitted = e + 1;
     g.home = (g.home + e) % (k + 1);
     g.done = stop ? 1ull : 0ull;
 }
 
-// The log-probabilities of a step's emitted tokens, after k_spec_accept: one CTA of kNucThreads per row r = li * (k + 1)
-// + i; row i of a stream that emitted more than i tokens this step scores its pick p_i, emitted at position len -
-// emitted + i, on la.logits (the raw copy, or the rows the pick read) divided by the stream's temperature in processed
-// mode (la.samp), with generate_streams_logprobs' rule (logprob_row). Other rows return at once (the whole CTA).
+// The log-probabilities of a step's emitted tokens, after k_spec_accept: CTA j of kNucThreads scores the token of
+// score[j] by gen_logprob_at (generate_streams_logprobs' rule: raw or processed, and a batcher lane's own mode and
+// top_n); a row that emitted nothing returns at once (the whole CTA).
 __global__ void __launch_bounds__(kNucThreads) k_spec_logprob(const SpecArgs a, const GenLogprobArgs la) {
-    const int r = blockIdx.x, li = r / (a.k + 1), i = r % (a.k + 1), s = a.live[li];
-    const SpecStream &g = a.ss[s];
-    if (i >= g.emitted) return;
-    const int y = a.next ? (int)a.next[r] : (int)a.sample[2 * r];
-    const float T = la.samp ? la.samp[s].temperature : 0.0f;
-    const size_t o = (size_t)s * a.max_new + (size_t)(g.len - (unsigned long long)g.emitted + (unsigned long long)i);
-    logprob_row(la.logits + (size_t)r * la.V, la.V, y, T > 0.0f ? (double)T : 1.0, la.top_n, la.logprob + o, la.rank + o,
-                la.top_tokens + o * la.top_n, la.top_logprobs + o * la.top_n);
+    const SpecScore c = a.score[blockIdx.x];
+    if (c.s < 0) return;
+    const int y = a.next ? (int)a.next[c.r] : (int)a.sample[2 * c.r];
+    gen_logprob_at(la, c.s, c.r, y, (size_t)c.o);
 }
 
 } // namespace rk

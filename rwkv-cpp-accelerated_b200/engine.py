@@ -57,6 +57,12 @@ class RequestEx(ctypes.Structure):
                 ("top_n", ctypes.c_uint)]
 
 
+class RequestSpec(ctypes.Structure):
+    """rwkv_b200_request_spec: prompt-lookup speculation for one batcher request."""
+    _fields_ = [("spare_slots", ctypes.POINTER(ctypes.c_ulonglong)), ("draft", ctypes.c_uint), ("ngram", ctypes.c_uint),
+                ("context", ctypes.POINTER(ctypes.c_ulonglong)), ("n_context", ctypes.c_ulonglong)]
+
+
 class StopRequest(ctypes.Structure):
     """rwkv_b200_stop_request: per stream its stop set id and start state, and where the results go."""
     P = ctypes.POINTER(ctypes.c_ulonglong)
@@ -346,6 +352,9 @@ def load_library():
                                                                      pull, pdbl, pull, pull, pull, c.POINTER(StopRequest)]),
         "rwkv_b200_batcher_submit_stop": (i32, [vp, c.POINTER(Request), c.POINTER(RequestEx), ull, ull, pull]),
         "rwkv_b200_batcher_read_stop": (i32, [vp, ull, pull, pull, pull]),
+        "rwkv_b200_batcher_submit_spec": (i32, [vp, c.POINTER(Request), c.POINTER(RequestEx), ull, ull,
+                                                c.POINTER(RequestSpec), pull]),
+        "rwkv_b200_batcher_read_spec": (i32, [vp, ull, pull]),
         "rwkv_b200_batcher_cancel": (i32, [vp, ull]),
         "rwkv_b200_batcher_release": (i32, [vp, ull]),
         "rwkv_b200_batcher_close": (None, [vp]),
@@ -904,15 +913,27 @@ class Batcher:
         self.h = h
         self._ext = {}  # id -> (top_n or None without log-probabilities, constrained) of requests sent through submit_ex
         self._stop = set()  # ids of requests with a stop set
+        self._spec = set()  # ids of requests with speculation
 
     def submit(self, slot, prompt, max_new, sampling=None, u=None, stop=(), overrides=None, constraint=None, logprobs=None,
-               top_n=0, stop_strings=None):
+               top_n=0, stop_strings=None, draft=0, spare_slots=(), ngram=3, context=None):
         """Queue a request on state slot `slot`: prompt (>= 1 token ids), up to max_new new tokens, a Sampler or dict
         (None: arg-max), u: max_new uniforms in [0, 1) (None only at temperature 0), stop: this request's stop tokens.
         overrides = {token: logit value} as in generate_streams; constraint: an id of Engine.add_constraint, or (id,
         start_state); logprobs = "raw" or "processed" scores every emitted token, with top_n top entries (read them with
-        result); stop_strings: an id of Engine.add_stop_set, or (id, start_state). Returns its id. Every array is
-        copied."""
+        result); stop_strings: an id of Engine.add_stop_set, or (id, start_state). draft > 0 speculates with
+        prompt-lookup drafts (rwkv_b200_batcher_submit_spec): spare_slots are its draft scratch slots, ngram the longest
+        n-gram looked up and context extra lookup tokens before the prompt; the tokens are those without speculation and
+        result adds "steps". Returns its id. Every array is copied."""
+        if int(draft) < 0:
+            raise EngineError("batcher.submit: draft %d < 0" % int(draft))
+        spares = np.ascontiguousarray([int(z) for z in spare_slots], dtype=np.uint64)
+        if len(spares) != int(draft):
+            raise EngineError("batcher.submit: draft = %d needs %d spare slots, got %d" % (int(draft), int(draft),
+                                                                                         len(spares)))
+        ctx = np.ascontiguousarray([int(t) for t in (context if context is not None else ())], dtype=np.uint64)
+        if len(ctx) and not draft:
+            raise EngineError("batcher.submit: a lookup context needs draft > 0")
         sp = _samplers(sampling if sampling is not None else Sampler(temperature=0.0), 1)[0]
         pr = np.ascontiguousarray(np.atleast_1d(np.asarray(prompt, dtype=np.uint64)))
         st = np.ascontiguousarray(list(stop), dtype=np.uint64)
@@ -921,36 +942,45 @@ class Batcher:
             raise EngineError("batcher.submit: u has shape %s, expected (%d,)" % (us.shape, int(max_new)))
         P = ctypes.c_ulonglong
         req = Request(int(slot), _ptr(pr, P), len(pr), int(max_new), sp, _ptr(us, ctypes.c_double), _ptr(st, P), len(st))
+        extended = overrides is not None or constraint is not None or logprobs is not None
+        x = None
+        if extended:
+            mode = _logprob_mode(logprobs, "batcher.submit")
+            ovr = dict(overrides or {})
+            otok = np.ascontiguousarray(list(ovr.keys()), dtype=np.uint64)
+            oval = np.ascontiguousarray(list(ovr.values()), dtype=np.float32)
+            cid, q0 = NO_CONSTRAINT, 0
+            if constraint is not None:
+                cid, q0 = ((int(constraint[0]), int(constraint[1])) if isinstance(constraint, (tuple, list))
+                           else (int(constraint), 0))
+            x = RequestEx(_ptr(otok, P), _ptr(oval, ctypes.c_float), len(otok), cid, q0, 1 if logprobs is not None else 0,
+                          mode, int(top_n))
+        sid, s0 = NO_STOP_SET, 0
+        if stop_strings is not None:
+            ids, starts = stop_spec([stop_strings], 1, "batcher.submit")
+            sid, s0 = int(ids[0]), int(starts[0])
         rid = ctypes.c_ulonglong()
-        plain = overrides is None and constraint is None and logprobs is None
-        if plain and stop_strings is None:
-            self.engine._ck(self.lib.rwkv_b200_batcher_submit(self.h, ctypes.byref(req), ctypes.byref(rid)), "batcher_submit")
-            return int(rid.value)
-        if plain:
-            ids, starts = stop_spec([stop_strings], 1, "batcher.submit")
-            self.engine._ck(self.lib.rwkv_b200_batcher_submit_stop(self.h, ctypes.byref(req), None, int(ids[0]),
-                                                                   int(starts[0]), ctypes.byref(rid)), "batcher_submit")
-            self._stop.add(int(rid.value))
-            return int(rid.value)
-        mode = _logprob_mode(logprobs, "batcher.submit")
-        ovr = dict(overrides or {})
-        otok = np.ascontiguousarray(list(ovr.keys()), dtype=np.uint64)
-        oval = np.ascontiguousarray(list(ovr.values()), dtype=np.float32)
-        cid, q0 = NO_CONSTRAINT, 0
-        if constraint is not None:
-            cid, q0 = (int(constraint[0]), int(constraint[1])) if isinstance(constraint, (tuple, list)) else (int(constraint), 0)
-        x = RequestEx(_ptr(otok, P), _ptr(oval, ctypes.c_float), len(otok), cid, q0, 1 if logprobs is not None else 0,
-                      mode, int(top_n))
-        if stop_strings is None:
-            self.engine._ck(self.lib.rwkv_b200_batcher_submit_ex(self.h, ctypes.byref(req), ctypes.byref(x),
-                                                                 ctypes.byref(rid)), "batcher_submit")
+        xr = ctypes.byref(x) if x is not None else None
+        # the entry point of what the request uses: each one is exactly the next one's call with its extension NULL
+        if draft:
+            spec = RequestSpec(_ptr(spares, P), int(draft), int(ngram), _ptr(ctx, P) if len(ctx) else None, len(ctx))
+            rc = self.lib.rwkv_b200_batcher_submit_spec(self.h, ctypes.byref(req), xr, sid, s0, ctypes.byref(spec),
+                                                        ctypes.byref(rid))
+        elif stop_strings is not None:
+            rc = self.lib.rwkv_b200_batcher_submit_stop(self.h, ctypes.byref(req), xr, sid, s0, ctypes.byref(rid))
+        elif extended:
+            rc = self.lib.rwkv_b200_batcher_submit_ex(self.h, ctypes.byref(req), xr, ctypes.byref(rid))
         else:
-            ids, starts = stop_spec([stop_strings], 1, "batcher.submit")
-            self.engine._ck(self.lib.rwkv_b200_batcher_submit_stop(self.h, ctypes.byref(req), ctypes.byref(x), int(ids[0]),
-                                                                   int(starts[0]), ctypes.byref(rid)), "batcher_submit")
-            self._stop.add(int(rid.value))
-        self._ext[int(rid.value)] = (int(top_n) if logprobs is not None else None, constraint is not None)
-        return int(rid.value)
+            rc = self.lib.rwkv_b200_batcher_submit(self.h, ctypes.byref(req), ctypes.byref(rid))
+        self.engine._ck(rc, "batcher_submit")
+        rid = int(rid.value)
+        if stop_strings is not None:
+            self._stop.add(rid)
+        if extended:
+            self._ext[rid] = (int(top_n) if logprobs is not None else None, constraint is not None)
+        if draft:
+            self._spec.add(rid)
+        return rid
 
     def run(self, max_steps):
         """Run up to max_steps steps (groups of 16); returns the steps run (fewer when everything has finished)."""
@@ -973,7 +1003,7 @@ class Batcher:
         with logprobs "logprobs" (float64) and "ranks" (uint64), and with top_n > 0 "top_tokens" / "top_logprobs"
         [len][top_n], as generate_streams(logprobs=...) returns them; with a constraint "state" (the automaton's
         current state); with a stop set "stop_hit", "stop_tail" and "stop_state" as generate_streams(stop_strings=...)
-        returns them."""
+        returns them; with speculation "steps" (the steps that emitted a token)."""
         top_n, constrained = self._ext.get(int(rid), (None, False))
         n, status = ctypes.c_ulonglong(), ctypes.c_int()
         self.engine._ck(self.lib.rwkv_b200_batcher_read(self.h, int(rid), None, 0, ctypes.byref(n), ctypes.byref(status)),
@@ -1002,6 +1032,10 @@ class Batcher:
                                                                  ctypes.byref(mstate)), "batcher_read_stop")
             d.update(stop_hit=int(hit.value) - 1 if hit.value else None, stop_tail=int(tail.value),
                      stop_state=int(mstate.value))
+        if int(rid) in self._spec:
+            steps = ctypes.c_ulonglong()
+            self.engine._ck(self.lib.rwkv_b200_batcher_read_spec(self.h, int(rid), ctypes.byref(steps)), "batcher_read_spec")
+            d["steps"] = int(steps.value)
         return d
 
     def cancel(self, rid):
@@ -1011,6 +1045,7 @@ class Batcher:
         self.engine._ck(self.lib.rwkv_b200_batcher_release(self.h, int(rid)), "batcher_release")
         self._ext.pop(int(rid), None)
         self._stop.discard(int(rid))
+        self._spec.discard(int(rid))
 
     def close(self):
         if getattr(self, "h", None) and getattr(self.engine, "h", None):
