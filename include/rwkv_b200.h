@@ -833,6 +833,54 @@ int rwkv_b200_index_search(rwkv_b200_model *m, unsigned long long id, const unsi
                            unsigned long long n_queries, int metric, unsigned int k, unsigned long long *entries_out,
                            double *l1_out, double *l2_out, unsigned long long *found_out);
 
+/* LoRA adapters bound to state slots: serve many low-rank fine-tunes of one base model in the same tensor-core pass.
+ *  - Adapter. A rank r in 1..RWKV_B200_MAX_ADAPTER_RANK, a scale s (alpha / r), and for any non-empty subset of the
+ *    seven projections a pair A [n_layers][r][in] and B [n_layers][out][r] of f32 (row-major, copied at add). The
+ *    projections are indexed by RWKV_B200_AD_*: att key, value, receptance and output (E -> E), ffn key (E -> 4E), ffn
+ *    value (4E -> E) and ffn receptance (E -> E). The head and the embedding are not adapted.
+ *  - Value. For a token whose slot is bound, each adapted projection's value is f32(S * tot + off + delta) instead of
+ *    f32(S * tot + off), with delta_m = s * sum_i B[m][i] * h_i and h_i = sum_j A[i][j] * f_j, both in f64. f is the
+ *    f32 activation the projection quantises, before the r-scaling and the 22-bit rounding: the token-shift mix for att
+ *    key/value/receptance and ffn key/receptance, the WKV output rw for att output, and relu(k)^2 for ffn value. The
+ *    summation orders are fixed, so delta depends only on the token's own f and its adapter: results are
+ *    bit-deterministic and independent of the other tokens of a pass. A token whose slot is unbound, or whose adapter
+ *    lacks a projection, gets exactly the bits it gets without adapters.
+ *  - Bindings belong to slots, not to states: slot_copy, slot_zero, slot_upload, slot_download and the forks inside
+ *    beam search and speculation move states only.
+ *  - Path. Adapters run on the tensor cores only. A multi-stream call (forward_streams, score_streams, the
+ *    generate_streams calls, beam search, speculation, the batcher) that names a bound slot runs on the tensor cores
+ *    whatever its token count, and is refused when the "prefill" option is 0. rwkv_b200_forward, forward_greedy,
+ *    decode_timed and profile (the decode kernel) refuse when a slot they touch is bound. A call that names no bound
+ *    slot enqueues exactly the launches it does without adapters.
+ *  - Refused before any work, with every slot and binding untouched: a speculative stream's slots, a beam group's
+ *    slots, or a batcher request's slot and spare slots that do not all share one binding; binding or unbinding a slot
+ *    held by a queued or admitted batcher request; removing an adapter that is still bound; a rank outside 1..64, an
+ *    adapter without matrices, a matrix with only one of A and B, a non-finite value; an unknown id; any adapter call
+ *    on a tensor-parallel model. The adapters live in device memory owned by the model (20 n_embed r n_layers floats
+ *    with every projection) and rwkv_b200_free frees them. */
+#define RWKV_B200_MAX_ADAPTER_RANK 64
+#define RWKV_B200_NO_ADAPTER 0xFFFFFFFFFFFFFFFFULL /* rwkv_b200_slot_adapter: unbind */
+#define RWKV_B200_AD_ATT_KEY 0
+#define RWKV_B200_AD_ATT_VALUE 1
+#define RWKV_B200_AD_ATT_RECEPTANCE 2
+#define RWKV_B200_AD_ATT_OUTPUT 3
+#define RWKV_B200_AD_FFN_KEY 4
+#define RWKV_B200_AD_FFN_VALUE 5
+#define RWKV_B200_AD_FFN_RECEPTANCE 6
+#define RWKV_B200_AD_MATRICES 7
+typedef struct {
+    unsigned int rank;                       /* 1..RWKV_B200_MAX_ADAPTER_RANK */
+    double scale;                            /* s = alpha / rank, finite */
+    const float *A[RWKV_B200_AD_MATRICES];   /* [n_layers][rank][in] host arrays, or NULL: not adapted */
+    const float *B[RWKV_B200_AD_MATRICES];   /* [n_layers][out][rank], NULL exactly where A is */
+} rwkv_b200_adapter;
+/* Copy an adapter to the device; *id receives its id (ids are never reused). */
+int rwkv_b200_adapter_add(rwkv_b200_model *m, const rwkv_b200_adapter *desc, unsigned long long *id);
+/* Free an adapter that no slot is bound to. */
+int rwkv_b200_adapter_remove(rwkv_b200_model *m, unsigned long long id);
+/* Bind `slot` to adapter `id`, or unbind it with RWKV_B200_NO_ADAPTER (in stream order: later calls see it). */
+int rwkv_b200_slot_adapter(rwkv_b200_model *m, unsigned long long slot, unsigned long long id);
+
 /* Engine knobs (all optional), key/value strings: "sub_bytes" (largest bulk copy of the
  * weight stream, a multiple of 16 up to one ring stage of 8 x n_embed bytes), "budget" /
  * "qbudget" (bytes of copies in flight per SM while streaming, at least one stage / while

@@ -214,6 +214,16 @@ struct rwkv_b200_model {
         DevBuf<unsigned long long> ent;            // [QB][k]
         DevBuf<double> o1, o2;                     // [QB][k]
     } isc;
+    // rwkv_b200_adapter_add: per id its matrices in one device block and the record the passes read; per slot the bound
+    // id (RWKV_B200_NO_ADAPTER: none; empty until the first binding) and, on the device, the bound record (rank 0: none)
+    struct Adapter {
+        DevBuf<float> data;
+        rk::AdapterRec rec{};
+    };
+    std::map<unsigned long long, Adapter> adapters;
+    unsigned long long next_adapter = 1;
+    std::vector<unsigned long long> slot_ad;
+    DevBuf<rk::AdapterRec> ad_table; // [max_gpt]
 };
 
 // rwkv_b200_batcher: the requests on the host, and per lane (0..rows-1, one per admitted request, reused) its stream
@@ -784,10 +794,50 @@ int check_ragged(M *m, const char *what, const unsigned long long *tokens, unsig
     return 0;
 }
 
+// The adapter bound to a slot, or RWKV_B200_NO_ADAPTER.
+unsigned long long slot_binding(const M *m, unsigned long long slot) {
+    return slot < m->slot_ad.size() ? m->slot_ad[slot] : RWKV_B200_NO_ADAPTER;
+}
+bool any_bound(const M *m, const unsigned long long *slots, unsigned long long n) {
+    for (unsigned long long i = 0; i < n; ++i)
+        if (slot_binding(m, slots[i]) != RWKV_B200_NO_ADAPTER) return true;
+    return false;
+}
+// The slots of one conversation (a speculative stream, a beam group, a batcher request) hold it in turn, so they must
+// all carry the same binding.
+int check_same_binding(M *m, const char *what, const char *whose, unsigned long long index, const unsigned long long *slots,
+                       unsigned long long n) {
+    for (unsigned long long i = 1; i < n; ++i)
+        if (slot_binding(m, slots[i]) != slot_binding(m, slots[0]))
+            return fail(1, "%s: the slots of %s %llu are not bound to the same adapter (slot %llu and slot %llu)", what, whose,
+                        index, slots[0], slots[i]);
+    return 0;
+}
+// The decode kernel has no adapters: a call that runs on it refuses a bound slot.
+int check_unbound(M *m, const char *what, const unsigned long long *slots, unsigned long long n) {
+    for (unsigned long long i = 0; i < n; ++i)
+        if (slot_binding(m, slots[i]) != RWKV_B200_NO_ADAPTER)
+            return fail(1, "%s: slot %llu is bound to an adapter, which runs on the tensor cores only (use forward_streams)",
+                        what, slots[i]);
+    return 0;
+}
+
 // Tensor cores or the decode kernel for a forward of n tokens: forward_streams' rule, which every call that has a
-// choice follows (the multi-stream calls refuse tensor parallelism).
-bool tensor_cores(const M *m, unsigned long long n) {
-    return n >= (unsigned long long)m->pf.min_tokens && m->tp_size == 1 && rk::prefill_enabled(m->pf);
+// choice follows (the multi-stream calls refuse tensor parallelism). A call that names a bound slot (`bound`) takes the
+// tensor cores whatever n, since adapters run there only.
+bool tensor_cores(const M *m, unsigned long long n, bool bound = false) {
+    return (bound || n >= (unsigned long long)m->pf.min_tokens) && m->tp_size == 1 && rk::prefill_enabled(m->pf);
+}
+
+// The adapter bit of a call's passes: set when one of its slots is bound (then the tensor cores are required); a call
+// without bound slots enqueues exactly the passes it enqueues on a model without adapters.
+int set_pass_adapters(M *m, const char *what, const unsigned long long *slots, unsigned long long n, bool &bound) {
+    bound = any_bound(m, slots, n);
+    m->pf.adapt = bound;
+    m->pf.ad_table = m->ad_table.p;
+    if (bound && !rk::prefill_enabled(m->pf))
+        return fail(1, "%s: a slot bound to an adapter needs the tensor cores, and the \"prefill\" option is 0", what);
+    return 0;
 }
 
 // Token by token through the decode kernel: stream i's lengths[i] tokens (stream-major) on slot slots[i]. Token t gets
@@ -1157,6 +1207,8 @@ int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, cons
             return fail(1, "%s: top_n = %u needs top_tokens_out and top_logprobs_out", what, lpq->top_n);
     }
     if ((rc = check_gen(m, what, c, 1, ex))) return rc;
+    bool bound;
+    if ((rc = set_pass_adapters(m, what, c.slots, c.n_streams, bound))) return rc;
     const size_t V = binfmt::kVocab;
     const unsigned long long n_streams = c.n_streams, max_new = c.max_new;
     bool pen = false; // some stream has a presence or frequency penalty
@@ -1181,7 +1233,7 @@ int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, cons
                 (raw_copy && (rc = g.raw.grow(n_streams * V)))))
         return rc;
     // the path is chosen once, for n_streams tokens; a stream's numbers depend only on its row
-    const bool tc = tensor_cores(m, n_streams);
+    const bool tc = tensor_cores(m, n_streams, bound);
     if (tc && (rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
     m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
 
@@ -1381,6 +1433,10 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
     *ran = 0;
     if (b->admitted.empty()) return 0;
     const int R = (int)dec.size();
+    // the group's passes add adapter deltas when an admitted request's slot is bound (its spares share the binding)
+    m->pf.adapt = false;
+    m->pf.ad_table = m->ad_table.p;
+    for (unsigned long long id : b->admitted) m->pf.adapt |= slot_binding(m, b->reqs[id].slot) != RWKV_B200_NO_ADAPTER;
     // the prefill segments of each step: the budget goes to the prefilling requests in admission order
     struct Seg {
         unsigned long long id, off, n;
@@ -1840,6 +1896,8 @@ int rwkv_b200_forward(rwkv_b200_model *m, const unsigned long long *tokens, unsi
     const bool par = mode == RWKV_B200_MODE_PARRALEL;
     std::vector<unsigned long long> slots(par ? n_tokens : 1), lens(par ? n_tokens : 1, par ? 1 : n_tokens);
     for (size_t i = 0; i < slots.size(); ++i) slots[i] = i;
+    if ((rc = check_unbound(m, "forward", slots.data(), slots.size()))) return rc;
+    m->pf.adapt = false;
     if (tensor_cores(m, n_tokens)) {
         if (par && n_tokens > (unsigned long long)rk::kPfMaxTokens)
             return fail(3, "batched prefill: PARRALEL chunks above 128 tokens are not supported");
@@ -1863,6 +1921,8 @@ int rwkv_b200_forward_greedy(rwkv_b200_model *m, unsigned long long token, unsig
     if (rc) return rc;
     const size_t V = binfmt::kVocab;
     if (token >= V) return fail(1, "token id %llu out of range", token);
+    const unsigned long long slot0 = 0;
+    if ((rc = check_unbound(m, "forward_greedy", &slot0, 1))) return rc;
     CK(cudaSetDevice(m->device));
     m->stream_rows = 0;
     rk::Ctrl &c = m->h_ctrl[0];
@@ -1899,11 +1959,13 @@ int rwkv_b200_forward_streams(rwkv_b200_model *m, const unsigned long long *toke
                               unsigned long long n_streams, float *logits_out, unsigned long long *next_out) {
     int rc = check_ragged(m, "forward_streams", tokens, n_tokens, slots, lengths, n_streams);
     if (rc) return rc;
+    bool bound;
+    if ((rc = set_pass_adapters(m, "forward_streams", slots, n_streams, bound))) return rc;
     const size_t V = binfmt::kVocab;
     CK(cudaSetDevice(m->device));
     const bool head = logits_out || next_out;
     m->stream_rows = 0;
-    if (tensor_cores(m, n_tokens)) {
+    if (tensor_cores(m, n_tokens, bound)) {
         rc = rk::prefill_forward(m->pf, m->p, m->stream, tokens, (int)n_tokens, slots, lengths, head ? 2 : 0, m->d_slogits);
         if (rc) return fail(rc, "%s", rk::prefill_error());
         m->launches += rk::prefill_launches(m->pf);
@@ -2190,6 +2252,10 @@ int rwkv_b200_beam_search(rwkv_b200_model *m, const unsigned long long *slots, c
     if ((rc = check_slots(m, what, slots, G * B)) || (rc = check_tokens(what, "first token", first_tokens, G, "group")) ||
         (rc = check_tokens(what, "stop token", stop_tokens, n_stop)))
         return rc;
+    for (unsigned long long g = 0; g < G; ++g)
+        if ((rc = check_same_binding(m, what, "group", g, slots + g * B, B))) return rc;
+    bool bound;
+    if ((rc = set_pass_adapters(m, what, slots, G * B, bound))) return rc;
     // the length penalties on the host, with the C library's pow: a host restatement gets the same bits
     if (N > ((unsigned long long)SIZE_MAX / sizeof(rk::BeamBack)) / (G * B))
         return fail(1, "%s: max_new = %llu: the backpointers of %llu beams do not fit in memory", what, N, G * B);
@@ -2208,7 +2274,7 @@ int rwkv_b200_beam_search(rwkv_b200_model *m, const unsigned long long *slots, c
         (rc = bm.hyp.grow(G * K)) || (rc = bm.n_hyp.grow(G)) || (rc = bm.done.grow(G)) || (rc = bm.forks.grow(2 * G * B)))
         return rc;
     // the path is chosen once, for G x B one-token streams
-    const bool tc = tensor_cores(m, G * B);
+    const bool tc = tensor_cores(m, G * B, bound);
     if (tc && (rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
     m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
 
@@ -2331,6 +2397,10 @@ int rwkv_b200_generate_streams_speculative_constrained(
     const GenCall c{slots, first_tokens, S, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values, n_override,
                     samplers, u, tokens_out, lengths_out};
     if ((rc = check_gen(m, what, c, K1, true, steps_out, "steps_out"))) return rc;
+    for (unsigned long long s = 0; s < S; ++s)
+        if ((rc = check_same_binding(m, what, "stream", s, slots + s * K1, K1))) return rc;
+    bool bound;
+    if ((rc = set_pass_adapters(m, what, slots, S * K1, bound))) return rc;
     for (unsigned long long s = 0; samplers && s < S; ++s)
         if (samplers[s].presence_penalty != 0.0f || samplers[s].frequency_penalty != 0.0f)
             return fail(1, "%s: stream %llu: presence and frequency penalties are not supported (a row's counts would have "
@@ -2607,13 +2677,15 @@ int rwkv_b200_score_streams(rwkv_b200_model *m, const unsigned long long *tokens
             need[t] = 1;
         }
     const size_t n = pos.size();
+    bool bound;
+    if ((rc = set_pass_adapters(m, what, slots, n_streams, bound))) return rc;
     CK(cudaSetDevice(m->device));
     m->stream_rows = 0; // the compact rows hold this call's scored positions, not per-stream logits
     auto &sc = m->score;
     if (n && ((rc = sc.rows.grow(n)) || (rc = sc.tgt.grow(n)) || (rc = sc.lp.grow(n)) || (rc = sc.rank.grow(n)) ||
               (rc = sc.top_tok.grow(n * top_n)) || (rc = sc.top_lp.grow(n * top_n))))
         return rc;
-    if (tensor_cores(m, n_tokens)) {
+    if (tensor_cores(m, n_tokens, bound)) {
         // logits of every token of a pass that holds a scored position, row t of d_slogits for token t
         rc = rk::prefill_forward(m->pf, m->p, m->stream, tokens, (int)n_tokens, slots, lengths, n ? 1 : 0, m->d_slogits, need.data());
         if (rc) return fail(rc, "%s", rk::prefill_error());
@@ -2714,6 +2786,100 @@ int rwkv_b200_slot_download(rwkv_b200_model *m, unsigned long long slot, double 
 // ---- state indexes (csrc/index.cuh) ---------------------------------------------------------------------------------
 
 // The multi-stream checks and the index of `id`.
+// ---- adapters ----------------------------------------------------------------------------------------------------
+// The input and output widths of projection k (RWKV_B200_AD_*).
+static void adapter_dims(const M *m, int k, unsigned long long &in, unsigned long long &out) {
+    in = k == RWKV_B200_AD_FFN_VALUE ? 4 * m->E : m->E;
+    out = k == RWKV_B200_AD_FFN_KEY ? 4 * m->E : m->E;
+}
+
+int rwkv_b200_adapter_add(rwkv_b200_model *m, const rwkv_b200_adapter *desc, unsigned long long *id) {
+    const char *what = "adapter_add";
+    int rc = check_streams_model(m, what);
+    if (rc) return rc;
+    if (!desc || !id) return fail(1, "%s: null argument", what);
+    const unsigned long long r = desc->rank, L = m->L;
+    if (r < 1 || r > RWKV_B200_MAX_ADAPTER_RANK) return fail(1, "%s: rank %llu is outside 1..%d", what, r, RWKV_B200_MAX_ADAPTER_RANK);
+    if (!std::isfinite(desc->scale)) return fail(1, "%s: scale %g is not finite", what, desc->scale);
+    size_t total = 0;
+    for (int k = 0; k < RWKV_B200_AD_MATRICES; ++k) {
+        if (!desc->A[k] != !desc->B[k]) return fail(1, "%s: matrix %d has only one of A and B", what, k);
+        if (!desc->A[k]) continue;
+        unsigned long long in, out;
+        adapter_dims(m, k, in, out);
+        const size_t na = (size_t)(L * r * in), nb = (size_t)(L * out * r);
+        for (size_t i = 0; i < na; ++i)
+            if (!std::isfinite(desc->A[k][i])) return fail(1, "%s: A of matrix %d has a non-finite value at %zu", what, k, i);
+        for (size_t i = 0; i < nb; ++i)
+            if (!std::isfinite(desc->B[k][i])) return fail(1, "%s: B of matrix %d has a non-finite value at %zu", what, k, i);
+        total += na + nb;
+    }
+    if (total == 0) return fail(1, "%s: the adapter has no matrices", what);
+    CK(cudaSetDevice(m->device));
+    if ((rc = m->ad_table.grow(m->max_gpt))) return rc;
+    if (m->slot_ad.empty()) { // the table starts all unbound (rank 0)
+        CK(cudaMemsetAsync(m->ad_table.p, 0, m->max_gpt * sizeof(rk::AdapterRec), m->stream));
+        m->slot_ad.assign(m->max_gpt, RWKV_B200_NO_ADAPTER);
+    }
+    M::Adapter a;
+    if ((rc = a.data.grow(total))) return rc;
+    a.rec.rank = (int)r;
+    a.rec.scale = desc->scale;
+    size_t o = 0;
+    for (int k = 0; k < RWKV_B200_AD_MATRICES; ++k) {
+        if (!desc->A[k]) continue;
+        unsigned long long in, out;
+        adapter_dims(m, k, in, out);
+        const size_t na = (size_t)(L * r * in), nb = (size_t)(L * out * r);
+        a.rec.A[k] = a.data.p + o;
+        a.rec.B[k] = a.data.p + o + na;
+        CK(cudaMemcpyAsync(a.data.p + o, desc->A[k], na * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(a.data.p + o + na, desc->B[k], nb * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+        o += na + nb;
+    }
+    SYNC(m);
+    *id = m->next_adapter++;
+    m->adapters.emplace(*id, std::move(a));
+    return 0;
+}
+
+int rwkv_b200_adapter_remove(rwkv_b200_model *m, unsigned long long id) {
+    const char *what = "adapter_remove";
+    int rc = check_streams_model(m, what);
+    if (rc) return rc;
+    const auto it = m->adapters.find(id);
+    if (it == m->adapters.end()) return fail(1, "%s: adapter id %llu is unknown or removed", what, id);
+    for (unsigned long long s = 0; s < m->slot_ad.size(); ++s)
+        if (m->slot_ad[s] == id) return fail(1, "%s: adapter %llu is still bound to slot %llu", what, id, s);
+    CK(cudaSetDevice(m->device));
+    SYNC(m); // no pass in flight still reads it
+    m->adapters.erase(it);
+    return 0;
+}
+
+int rwkv_b200_slot_adapter(rwkv_b200_model *m, unsigned long long slot, unsigned long long id) {
+    const char *what = "slot_adapter";
+    int rc = check_streams_model(m, what);
+    if (rc || (rc = check_slot(m, what, slot))) return rc;
+    const auto it = m->adapters.find(id);
+    if (id != RWKV_B200_NO_ADAPTER && it == m->adapters.end()) return fail(1, "%s: adapter id %llu is unknown or removed", what, id);
+    if (const rwkv_b200_batcher *b = m->batcher)
+        for (const auto &kv : b->reqs) {
+            const B::Req &q = kv.second;
+            if (q.status > RWKV_B200_REQ_GENERATING) continue;
+            if (q.slot == slot || std::find(q.spares.begin(), q.spares.end(), slot) != q.spares.end())
+                return fail(1, "%s: slot %llu is held by batcher request %llu", what, slot, kv.first);
+        }
+    if (m->slot_ad.empty() && id == RWKV_B200_NO_ADAPTER) return 0; // nothing was ever bound
+    CK(cudaSetDevice(m->device));
+    if (m->slot_ad.empty()) return fail(1, "%s: no adapter table", what); // unreachable: an id exists only after an add
+    const rk::AdapterRec rec = id == RWKV_B200_NO_ADAPTER ? rk::AdapterRec{} : it->second.rec;
+    CK(cudaMemcpyAsync(m->ad_table.p + slot, &rec, sizeof(rec), cudaMemcpyHostToDevice, m->stream));
+    SYNC(m); // the source is on this stack
+    m->slot_ad[slot] = id;
+    return 0;
+}
+
 static int find_index(M *m, const char *what, unsigned long long id, M::Index **out) {
     int rc = check_streams_model(m, what);
     if (rc) return rc;
@@ -3155,6 +3321,9 @@ int rwkv_b200_batcher_submit_spec(rwkv_b200_batcher *b, const rwkv_b200_request 
                     return fail(1, "%s: spare slot %llu is held by unfinished request %llu", what, z, e.first);
             }
         }
+        std::vector<unsigned long long> all(1, r->slot);
+        all.insert(all.end(), spec->spare_slots, spec->spare_slots + spec->draft);
+        if ((rc = check_same_binding(m, what, "request", b->next_id, all.data(), all.size()))) return rc;
     }
     if ((rc = rwkv_b200_batcher_submit_stop(b, r, x, set_id, start_state, id)) || !spec) return rc;
     B::Req &q = b->reqs.at(*id);
@@ -3236,6 +3405,8 @@ int rwkv_b200_decode_timed(rwkv_b200_model *m, const unsigned long long *tokens,
     int rc = check_model(m);
     if (rc) return rc;
     if (!tokens || n == 0 || !ms) return fail(1, "decode_timed: bad arguments");
+    const unsigned long long slot0 = 0;
+    if ((rc = check_unbound(m, "decode_timed", &slot0, 1))) return rc;
     CK(cudaSetDevice(m->device));
     const unsigned long long cnt = teacher_forced ? n : 1;
     for (unsigned long long i = 0; i < cnt; ++i)
@@ -3272,6 +3443,8 @@ int rwkv_b200_profile(rwkv_b200_model *m, const unsigned long long *tokens, unsi
     int rc = check_model(m);
     if (rc) return rc;
     if (!tokens || !ms_sum || !launches || !bytes) return fail(1, "profile: bad arguments");
+    const unsigned long long slot0 = 0;
+    if ((rc = check_unbound(m, "profile", &slot0, 1))) return rc;
     CK(cudaSetDevice(m->device));
     ms_sum[0] = 0.f;
     launches[0] = 0;

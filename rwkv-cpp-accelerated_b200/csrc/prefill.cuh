@@ -60,6 +60,18 @@ struct PassDesc {
     int out_row0;           // head row i goes to logits row out_row0 + i
 };
 
+// ---- LoRA adapters (include/rwkv_b200.h, "adapters") ----------------------------------------------------------
+// A slot's adapter record lives in a per-slot device table, so a token finds its adapter through its descriptor's slot
+// and no layout code knows about adapters. Matrix m of the record: A [L][rank][in] and B [L][out][rank] in f32, or both
+// NULL (not adapted). rank 0: the slot is unbound.
+constexpr int kAdMats = 7, kAdMaxRank = 64;
+enum : int { kAdAttK = 0, kAdAttV, kAdAttR, kAdAttO, kAdFfnK, kAdFfnV, kAdFfnR };
+struct AdapterRec {
+    int rank;
+    double scale;
+    const float *A[kAdMats], *B[kAdMats];
+};
+
 // ---- wgmma / TMA helpers ---------------------------------------------------------------------------------
 __device__ __forceinline__ void pf_mbar_wait(uint32_t bar, uint32_t parity) {
     uint32_t ok = 0;
@@ -283,6 +295,7 @@ struct MixArgs {
     int nv, E, Tp;
     uint8_t *limbs;
     double *scale, *offs;
+    float *fout; // NULL, or [nv][Tp][E]: the mixed activation f (before the r-scaling and the 22-bit rounding), for adapters
 };
 __global__ void __launch_bounds__(256) k_pf_mix_quant(const __grid_constant__ MixArgs a) {
     __shared__ double sh[8];
@@ -297,6 +310,7 @@ __global__ void __launch_bounds__(256) k_pf_mix_quant(const __grid_constant__ Mi
         for (int j = threadIdx.x; j < E; j += blockDim.x) {
             const double m = a.mix[v][j];
             const float f = (float)(m * cur[j] + (1.0 - m) * prev[j]);
+            if (a.fout) a.fout[((size_t)v * a.Tp + t) * E + j] = f;
             const float xs = (float)((double)f * (double)a.r[v][j]);
             mx = max(mx, ((__float_as_uint(xs) + 2u) & ~3u) & 0x7fffffffu);
             of += (double)f * (double)a.oc[v][j];
@@ -354,11 +368,12 @@ __global__ void __launch_bounds__(256) k_pf_quant_rows(const float *xs, const fl
     }
 }
 
-// value of output row m for token t from the three plane sums: S * ((t2*256 + t1)*256 + t0) + off
-__device__ __forceinline__ float pf_combine(const int *C, int Tp, size_t m, int t, double S, double off) {
+// value of output row m for token t from the three plane sums: S * ((t2*256 + t1)*256 + t0) + off, plus an adapter's
+// delta. A token without one adds -0.0, which leaves every double (signed zeros included) exactly as it was.
+__device__ __forceinline__ float pf_combine(const int *C, int Tp, size_t m, int t, double S, double off, double delta = -0.0) {
     const int *c = C + m * 3 * Tp;
     const long long tot = (((long long)c[2 * Tp + t] << 8) + (long long)c[Tp + t]) * 256 + (long long)c[t];
-    return (float)(S * (double)tot + off);
+    return (float)(S * (double)tot + off + delta);
 }
 
 // WKV over the pass (rwkv.cu:221-259): thread = channel, sequential over t. The state is loaded from the slot at
@@ -374,6 +389,7 @@ struct WkvArgs {
     const uint32_t *desc;             // [T] stream descriptors
     int E, T, Tp;
     float *rw, *xs;                   // [T][E]
+    const double *dk, *dv, *dr;       // NULL, or the adapters' deltas [T][E]
 };
 __global__ void __launch_bounds__(256) k_pf_wkv(const __grid_constant__ WkvArgs a) {
     __shared__ uint32_t desc[kPfMaxTokens]; // read once per t by every thread of the sequential scan
@@ -392,9 +408,10 @@ __global__ void __launch_bounds__(256) k_pf_wkv(const __grid_constant__ WkvArgs 
             aa = a.aa[so];
             bb = a.bb[so];
         }
-        const float kf = pf_combine(a.Ck, a.Tp, (size_t)c, t, a.scale[0 * a.Tp + t], a.offs[0 * a.Tp + t]);
-        const float vf = pf_combine(a.Cv, a.Tp, (size_t)c, t, a.scale[1 * a.Tp + t], a.offs[1 * a.Tp + t]);
-        const float rf = pf_combine(a.Cr, a.Tp, (size_t)c, t, a.scale[2 * a.Tp + t], a.offs[2 * a.Tp + t]);
+        const size_t tc = (size_t)t * a.E + c;
+        const float kf = pf_combine(a.Ck, a.Tp, (size_t)c, t, a.scale[0 * a.Tp + t], a.offs[0 * a.Tp + t], a.dk ? a.dk[tc] : -0.0);
+        const float vf = pf_combine(a.Cv, a.Tp, (size_t)c, t, a.scale[1 * a.Tp + t], a.offs[1 * a.Tp + t], a.dv ? a.dv[tc] : -0.0);
+        const float rf = pf_combine(a.Cr, a.Tp, (size_t)c, t, a.scale[2 * a.Tp + t], a.offs[2 * a.Tp + t], a.dr ? a.dr[tc] : -0.0);
         const double vv = (double)vf;
         const double e1 = exp(ub + wd + (double)kf);
         double y = (aa + e1 * vv) / (bb + e1);
@@ -414,27 +431,30 @@ __global__ void __launch_bounds__(256) k_pf_wkv(const __grid_constant__ WkvArgs 
 }
 
 // x[t][j] = f32(x) + y  (out-proj, rwkv.cu:548-553)   /   x[t][j] += kv * sr  (ffn, rwkv.cu:574-577)
-__global__ void __launch_bounds__(256) k_pf_residual(const int *C, const double *scale, const double *offs, const float *sr, int E, int T, int Tp, double *x) {
+// delta: NULL, or the adapters' deltas [T][E].
+__global__ void __launch_bounds__(256) k_pf_residual(const int *C, const double *scale, const double *offs, const float *sr, int E, int T, int Tp, double *x,
+                                                     const double *delta) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (size_t)T * E) return;
     const int t = (int)(i / E), j = (int)(i % E);
-    const float y = pf_combine(C, Tp, (size_t)j, t, scale[t], offs[t]);
+    const float y = pf_combine(C, Tp, (size_t)j, t, scale[t], offs[t], delta ? delta[i] : -0.0);
     if (sr == nullptr) x[i] = (double)((float)x[i] + y);
     else x[i] = x[i] + (double)(y * sr[i]);
 }
 
-// sigmoid(ffn r) [T][E]; a = relu(k)^2 [T][4E] and xs = a * r_ffnv rounded to 22 bits (rwkv.cu:566-573)
+// sigmoid(ffn r) [T][E]; a = relu(k)^2 [T][4E] and xs = a * r_ffnv rounded to 22 bits (rwkv.cu:566-573).
+// dr, dk: NULL, or the adapters' deltas of ffn r [T][E] and ffn k [T][4E].
 __global__ void __launch_bounds__(256) k_pf_ffn_act(const int *Cr, const int *Ck, const double *scale, const double *offs, const float *rfv, int E, int T,
-                                                    int Tp, float *sr, float *act, float *xs) {
+                                                    int Tp, float *sr, float *act, float *xs, const double *dr, const double *dk) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (size_t)T * 5 * E) return;
     const int t = (int)(i / (5 * (size_t)E)), j = (int)(i % (5 * (size_t)E));
     if (j < E) {
-        const float y = pf_combine(Cr, Tp, (size_t)j, t, scale[0 * Tp + t], offs[0 * Tp + t]);
+        const float y = pf_combine(Cr, Tp, (size_t)j, t, scale[0 * Tp + t], offs[0 * Tp + t], dr ? dr[(size_t)t * E + j] : -0.0);
         sr[(size_t)t * E + j] = (float)(1.0 / (1.0 + exp(-(double)y)));
     } else {
         const int k = j - E;
-        float a = pf_combine(Ck, Tp, (size_t)k, t, scale[1 * Tp + t], offs[1 * Tp + t]);
+        float a = pf_combine(Ck, Tp, (size_t)k, t, scale[1 * Tp + t], offs[1 * Tp + t], dk ? dk[(size_t)t * 4 * E + k] : -0.0);
         a = a > 0.0f ? a : 0.0f;
         a = a * a;
         act[(size_t)t * 4 * E + k] = a;
@@ -461,6 +481,66 @@ __global__ void __launch_bounds__(256) k_pf_store_state(const double *ln, int E,
     for (int j = threadIdx.x; j < E; j += blockDim.x) dst[j] = ln[(size_t)t * E + j];
 }
 
+// ---- adapter deltas: delta[t][m] = s * sum_i B[m][i] * h[t][i],  h[t][i] = sum_j A[i][j] * f[t][j], both in f64 ----
+// One adaptation point adapts nv <= 3 matrices of layer l whose inputs are rows of f. Each token's sums run in an order
+// fixed by the shapes alone (lane-strided products and a butterfly for h, i ascending for delta), so a token's delta
+// depends only on its own f and its slot's adapter, never on the other tokens of the pass.
+struct AdArgs {
+    const AdapterRec *table; // [slots]
+    const uint32_t *desc;    // [T] stream descriptors
+    int T, l;
+    int nv, mat[3], K, M[3]; // matrix, input width and output width of each vector
+    const float *f;          // vector v, token t at f + v * f_vstride + t * K
+    size_t f_vstride;
+    double *h;               // [3][T][kAdMaxRank]
+    double *delta;           // vector v, token t at delta + v * d_vstride + t * M[v]
+    size_t d_vstride;
+};
+constexpr int kAdThreads = 256;
+constexpr int kAdShrinkTokens = kAdThreads / 32; // tokens of a k_ad_shrink block: one per warp
+constexpr int kAdExpandTokens = 4;               // tokens of a k_ad_expand block, in turn
+
+// h: block (i, v, g) = rank row i of matrix v for the tokens of group g, one per warp. A row of A is read from HBM once
+// per pass and from L2 by the other groups of tokens with the same adapter.
+__global__ void __launch_bounds__(kAdThreads) k_ad_shrink(const __grid_constant__ AdArgs a) {
+    const int i = blockIdx.x, v = blockIdx.y, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int t = blockIdx.z * kAdShrinkTokens + warp;
+    if (t < a.T) {
+        const AdapterRec &r = a.table[desc_slot(a.desc[t])];
+        const float *A = r.A[a.mat[v]];
+        if (A == nullptr || i >= r.rank) return;
+        const float *row = A + ((size_t)a.l * r.rank + i) * a.K, *f = a.f + v * a.f_vstride + (size_t)t * a.K;
+        double s = 0.0;
+        for (int j = lane; j < a.K; j += 32) s += (double)row[j] * (double)f[j];
+        s = warp_sum(s);
+        if (lane == 0) a.h[((size_t)v * a.T + t) * kAdMaxRank + i] = s;
+    }
+}
+
+// delta: block (x, v, g) = output rows of vector v for the tokens of group g, thread = output row m, sequential over
+// the group's tokens (a row of B stays in L1 across them). Tokens without the matrix get -0.0, which pf_combine adds
+// without changing a bit.
+__global__ void __launch_bounds__(kAdThreads) k_ad_expand(const __grid_constant__ AdArgs a) {
+    const int v = blockIdx.y, M = a.M[v];
+    const int m = blockIdx.x * kAdThreads + threadIdx.x;
+    if (m >= M) return;
+    double *out = a.delta + v * a.d_vstride + m;
+    const int t1 = min(a.T, (int)(blockIdx.z + 1) * kAdExpandTokens);
+    for (int t = blockIdx.z * kAdExpandTokens; t < t1; ++t) {
+        const AdapterRec &r = a.table[desc_slot(a.desc[t])];
+        const float *B = r.B[a.mat[v]];
+        if (B == nullptr || r.rank == 0) {
+            out[(size_t)t * M] = -0.0;
+            continue;
+        }
+        const float *b = B + ((size_t)a.l * M + m) * r.rank;
+        const double *h = a.h + ((size_t)v * a.T + t) * kAdMaxRank;
+        double s = 0.0;
+        for (int i = 0; i < r.rank; ++i) s += (double)b[i] * h[i];
+        out[(size_t)t * M] = r.scale * s;
+    }
+}
+
 // ---- host side -------------------------------------------------------------------------------------------------
 typedef CUresult (*PfnEncodeTiled)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
                                    const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -477,6 +557,12 @@ struct PrefillState {
     uint8_t *limbs = nullptr;   // [3 vectors][3 planes][Tp][4E] worst case
     int *C = nullptr;           // the largest accumulator set of a step
     float *rw = nullptr, *xs = nullptr, *sr = nullptr, *act = nullptr;
+    // adapters: `adapt` is set by the caller for the passes of a call that names a bound slot, which then add the
+    // deltas of the slots' records in `ad_table`. Allocated at the first such pass.
+    bool adapt = false;
+    const AdapterRec *ad_table = nullptr;
+    float *ad_f = nullptr;                    // [3][T][E] the mixed activations of k_pf_mix_quant
+    double *ad_h = nullptr, *ad_d = nullptr;  // [3][T][kAdMaxRank], [5][T][E]
     unsigned long long launches = 0;
     std::string err;
     // One pass is ~21 small launches per layer: replayed as a CUDA graph per (tokens, head rows) shape, so that a
@@ -484,6 +570,7 @@ struct PrefillState {
     // are data in `pass`, never part of the key: a decode loop whose set of slots changes replays the same graph.
     struct Graph {
         int T, H;
+        bool adapt;
         cudaGraphExec_t exec;
         unsigned long long launches;
     };
@@ -506,7 +593,7 @@ inline void prefill_free(PrefillState &s) {
     for (auto &g : s.graphs) cudaGraphExecDestroy(g.exec);
     s.graphs.clear();
     for (void *p : {(void *)s.pass, (void *)s.iota, (void *)s.head_desc, (void *)s.x, (void *)s.ln, (void *)s.scale, (void *)s.offs, (void *)s.limbs,
-                    (void *)s.C, (void *)s.rw, (void *)s.xs, (void *)s.sr, (void *)s.act})
+                    (void *)s.C, (void *)s.rw, (void *)s.xs, (void *)s.sr, (void *)s.act, (void *)s.ad_f, (void *)s.ad_h, (void *)s.ad_d})
         if (p) cudaFree(p);
     s = PrefillState{};
 }
@@ -606,7 +693,33 @@ inline int pf_padded(int n) { return (n + kPfTokenAlign - 1) / kPfTokenAlign * k
 
 // One pass of T <= 128 tokens on a single GPU, laid out by s.pass. H > 0: the head runs on the H rows of the row
 // map and writes logits rows pass->out_row0 .. + H - 1 of `logits` ([rows][V], device).
-inline int prefill_chunk_body(PrefillState &s, const Params &p, cudaStream_t st, int T, int H, float *logits) {
+// The deltas of one adaptation point: nv matrices of layer l whose inputs are at f (vector stride f_vstride, row K),
+// into s.ad_d (vector stride T * E, row M[v]).
+inline void pf_adapt(PrefillState &s, const Params &p, cudaStream_t st, int T, int l, int nv, const int (&mat)[3], int K,
+                     const int (&M)[3], const float *f, size_t f_vstride) {
+    AdArgs a{};
+    a.table = s.ad_table;
+    a.desc = s.pass->desc;
+    a.T = T;
+    a.l = l;
+    a.nv = nv;
+    a.K = K;
+    int maxM = 0;
+    for (int v = 0; v < 3; ++v) {
+        a.mat[v] = mat[v];
+        a.M[v] = M[v];
+        maxM = std::max(maxM, M[v]);
+    }
+    a.f = f;
+    a.f_vstride = f_vstride;
+    a.h = s.ad_h;
+    a.delta = s.ad_d;
+    a.d_vstride = (size_t)T * p.E;
+    k_ad_shrink<<<dim3(kAdMaxRank, nv, (T + kAdShrinkTokens - 1) / kAdShrinkTokens), kAdThreads, 0, st>>>(a);
+    k_ad_expand<<<dim3((maxM + kAdThreads - 1) / kAdThreads, nv, (T + kAdExpandTokens - 1) / kAdExpandTokens), kAdThreads, 0, st>>>(a);
+}
+
+inline int prefill_chunk_body(PrefillState &s, const Params &p, cudaStream_t st, int T, int H, float *logits, bool ad) {
     const int E = p.E, L = p.L, Tp = pf_padded(T);
     const size_t LE = (size_t)L * E;
     double *saa = reinterpret_cast<double *>(p.xch[p.rank] + p.off_saa), *sbb = reinterpret_cast<double *>(p.xch[p.rank] + p.off_sbb);
@@ -630,6 +743,7 @@ inline int prefill_chunk_body(PrefillState &s, const Params &p, cudaStream_t st,
         m.oc[0] = p.ock + lo; m.oc[1] = p.ocv + lo; m.oc[2] = p.ocr + lo;
         m.nv = 3; m.E = E; m.Tp = Tp;
         m.limbs = s.limbs; m.scale = s.scale; m.offs = s.offs;
+        m.fout = ad ? s.ad_f : nullptr;
         k_pf_mix_quant<<<gT, 256, 0, st>>>(m);
         k_pf_store_state<<<gT, 256, 0, st>>>(s.ln, E, s.pass->desc, LE, p.sxy + lo);
         const size_t mo = (size_t)l * E * E;
@@ -646,10 +760,16 @@ inline int prefill_chunk_body(PrefillState &s, const Params &p, cudaStream_t st,
         w.desc = s.pass->desc;
         w.E = E; w.T = T; w.Tp = Tp;
         w.rw = s.rw; w.xs = s.xs;
+        const size_t TE = (size_t)T * E;
+        if (ad) {
+            pf_adapt(s, p, st, T, l, 3, {kAdAttK, kAdAttV, kAdAttR}, E, {E, E, E}, s.ad_f, (size_t)Tp * E);
+            w.dk = s.ad_d; w.dv = s.ad_d + TE; w.dr = s.ad_d + 2 * TE;
+        }
         k_pf_wkv<<<blocks(E), 256, 0, st>>>(w);
         k_pf_quant_rows<<<gT, 256, 0, st>>>(s.xs, s.rw, p.oco + lo, E, Tp, s.limbs, s.scale, s.offs);
         if ((rc = pf_gemm(s, st, p.wo + mo, E, E, s.limbs, (size_t)3 * Tp, 0, Tp, Ca))) return rc;
-        k_pf_residual<<<blocks((size_t)T * E), 256, 0, st>>>(Ca, s.scale, s.offs, nullptr, E, T, Tp, s.x);
+        if (ad) pf_adapt(s, p, st, T, l, 1, {kAdAttO, 0, 0}, E, {E, 0, 0}, s.rw, 0);
+        k_pf_residual<<<blocks((size_t)T * E), 256, 0, st>>>(Ca, s.scale, s.offs, nullptr, E, T, Tp, s.x, ad ? s.ad_d : nullptr);
         // ---- ffn: LN2, token shift, R/K, activations, V -------------------------------------------------------
         k_pf_ln<<<gT, 256, 0, st>>>(s.x, p.ln + (size_t)(4 * (l + 1)) * E, p.ln + (size_t)(4 * (l + 1) + 1) * E, E, s.iota, s.ln);
         MixArgs f{};
@@ -662,16 +782,20 @@ inline int prefill_chunk_body(PrefillState &s, const Params &p, cudaStream_t st,
         f.oc[0] = p.ocfr + lo; f.oc[1] = p.ocfk + lo;
         f.nv = 2; f.E = E; f.Tp = Tp;
         f.limbs = s.limbs; f.scale = s.scale; f.offs = s.offs;
+        f.fout = ad ? s.ad_f : nullptr;
         k_pf_mix_quant<<<gT, 256, 0, st>>>(f);
         k_pf_store_state<<<gT, 256, 0, st>>>(s.ln, E, s.pass->desc, LE, p.sdd + lo);
         int *Ck4 = s.C + (size_t)E * 3 * Tp; // [4E][3Tp] behind the ffn-R accumulators
         if ((rc = pf_gemm(s, st, p.wfr + mo, E, E, s.limbs, (size_t)6 * Tp, 0 * Tp, Tp, Ca))) return rc;
         if ((rc = pf_gemm(s, st, p.wfk + 4 * mo, 4 * E, E, s.limbs, (size_t)6 * Tp, 3 * Tp, Tp, Ck4))) return rc;
-        k_pf_ffn_act<<<blocks((size_t)T * 5 * E), 256, 0, st>>>(Ca, Ck4, s.scale, s.offs, p.rfv + (size_t)l * 4 * E, E, T, Tp, s.sr, s.act, s.xs);
+        if (ad) pf_adapt(s, p, st, T, l, 2, {kAdFfnR, kAdFfnK, 0}, E, {E, 4 * E, 0}, s.ad_f, (size_t)Tp * E);
+        k_pf_ffn_act<<<blocks((size_t)T * 5 * E), 256, 0, st>>>(Ca, Ck4, s.scale, s.offs, p.rfv + (size_t)l * 4 * E, E, T, Tp, s.sr, s.act, s.xs,
+                                                                ad ? s.ad_d : nullptr, ad ? s.ad_d + TE : nullptr);
         k_pf_quant_rows<<<gT, 256, 0, st>>>(s.xs, s.act, p.ocfv + (size_t)l * 4 * E, 4 * E, Tp, s.limbs, s.scale, s.offs);
         if ((rc = pf_gemm(s, st, p.wfv + 4 * mo, E, 4 * E, s.limbs, (size_t)3 * Tp, 0, Tp, Ca))) return rc;
-        k_pf_residual<<<blocks((size_t)T * E), 256, 0, st>>>(Ca, s.scale, s.offs, s.sr, E, T, Tp, s.x);
-        s.launches += 10;
+        if (ad) pf_adapt(s, p, st, T, l, 1, {kAdFfnV, 0, 0}, 4 * E, {E, 0, 0}, s.act, 0);
+        k_pf_residual<<<blocks((size_t)T * E), 256, 0, st>>>(Ca, s.scale, s.offs, s.sr, E, T, Tp, s.x, ad ? s.ad_d : nullptr);
+        s.launches += ad ? 18 : 10;
     }
     // ---- head: the rows of the row map only -----------------------------------------------------------------------
     if (H > 0) {
@@ -700,14 +824,25 @@ inline int prefill_chunk_body(PrefillState &s, const Params &p, cudaStream_t st,
 // One pass of the layout already in s.pass: replay (or record) the graph of its shape.
 inline int prefill_run(PrefillState &s, const Params &p, cudaStream_t st, int T, int H, float *logits) {
     int rc;
+    const bool ad = s.adapt;
+    if (ad && !s.ad_f) {
+        if (!s.ad_table) {
+            prefill_err_slot() = "batched prefill: a pass with adapters but no adapter table";
+            return 3;
+        }
+        const size_t E = (size_t)p.E, Tm = kPfMaxTokens;
+        PF_CK(cudaMalloc((void **)&s.ad_f, 3 * Tm * E * 4));
+        PF_CK(cudaMalloc((void **)&s.ad_h, 3 * Tm * kAdMaxRank * 8));
+        PF_CK(cudaMalloc((void **)&s.ad_d, 5 * Tm * E * 8));
+    }
     PrefillState::Graph *g = nullptr;
     for (auto &e : s.graphs)
-        if (e.T == T && e.H == H) g = &e;
+        if (e.T == T && e.H == H && e.adapt == ad) g = &e;
     if (!g && s.use_graph) {
         // record the pass once (nothing runs during the capture), then replay it
         const unsigned long long before = s.launches;
         PF_CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-        rc = prefill_chunk_body(s, p, st, T, H, logits);
+        rc = prefill_chunk_body(s, p, st, T, H, logits, ad);
         cudaGraph_t graph = nullptr;
         const cudaError_t ee = cudaStreamEndCapture(st, &graph);
         const unsigned long long n = s.launches - before;
@@ -725,14 +860,14 @@ inline int prefill_run(PrefillState &s, const Params &p, cudaStream_t st, int T,
             cudaGraphExecDestroy(s.graphs.front().exec);
             s.graphs.erase(s.graphs.begin());
         }
-        s.graphs.push_back(PrefillState::Graph{T, H, exec, n});
+        s.graphs.push_back(PrefillState::Graph{T, H, ad, exec, n});
         s.records += 1;
         g = &s.graphs.back();
     }
     if (g) {
         PF_CK(cudaGraphLaunch(g->exec, st));
         s.launches += g->launches;
-    } else if ((rc = prefill_chunk_body(s, p, st, T, H, logits))) {
+    } else if ((rc = prefill_chunk_body(s, p, st, T, H, logits, ad))) {
         return rc;
     }
     return 0;

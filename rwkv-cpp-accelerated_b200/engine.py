@@ -20,6 +20,10 @@ MAX_STOP_BYTES = 4096                    # RWKV_B200_MAX_STOP_BYTES
 INDEX_L1, INDEX_L2 = 0, 1                # RWKV_B200_INDEX_*: the metric a StateIndex search ranks by
 MAX_NEIGHBOURS = 256                     # RWKV_B200_MAX_NEIGHBOURS
 NO_ENTRY = 0xFFFFFFFFFFFFFFFF            # RWKV_B200_NO_ENTRY: a search position past the entries found
+NO_ADAPTER = 0xFFFFFFFFFFFFFFFF          # RWKV_B200_NO_ADAPTER: Engine.bind_adapter(slot, None)
+MAX_ADAPTER_RANK = 64                    # RWKV_B200_MAX_ADAPTER_RANK
+# RWKV_B200_AD_* in order: the checkpoint's Linear name inside a block of each projection an adapter may adapt
+ADAPTER_MATRICES = ("att.key", "att.value", "att.receptance", "att.output", "ffn.key", "ffn.value", "ffn.receptance")
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
@@ -69,7 +73,67 @@ class StopRequest(ctypes.Structure):
     _fields_ = [("set_ids", P), ("start_states", P), ("states_out", P), ("hit_out", P), ("tail_out", P)]
 
 
+class Adapter(ctypes.Structure):
+    """rwkv_b200_adapter: the rank, the scale and per projection the A and B arrays (NULL: not adapted)."""
+    PF = ctypes.POINTER(ctypes.c_float)
+    _fields_ = [("rank", ctypes.c_uint), ("scale", ctypes.c_double), ("A", PF * 7), ("B", PF * 7)]
+
+
 REQ_STATUS = ("queued", "prefilling", "generating", "done", "cancelled")  # RWKV_B200_REQ_* in order
+
+
+def adapter_dims(name, E):
+    """(in, out) of the projection `name` (an entry of ADAPTER_MATRICES) at width E."""
+    return (4 * E if name == "ffn.value" else E), (4 * E if name == "ffn.key" else E)
+
+
+def parse_adapter(weights, L, E):
+    """(rank, {name: (A [L][r][in], B [L][out][r]) float32}) of a LoRA state dict whose keys are the checkpoint's Linear
+    names with ".lora_A" ([r][in]) or ".lora_B" ([out][r]), e.g. "blocks.3.att.key.lora_A". Layers a projection lacks
+    get zeros. Raises ValueError, naming the key, for an unknown key, a key without its partner, a rank that differs
+    from the others or is outside 1..64, a wrong shape, and an empty dict."""
+    per = {}  # (layer, name) -> {"A": array, "B": array}
+    for key, val in weights.items():
+        parts = key.split(".")
+        ok = (len(parts) == 5 and parts[0] == "blocks" and parts[1].isdigit() and ".".join(parts[2:4]) in ADAPTER_MATRICES
+              and parts[4] in ("lora_A", "lora_B"))
+        if not ok:
+            hint = ""
+            if any(p.startswith("time_") or p.startswith("ln") for p in parts):
+                hint = (" (full-parameter tensors such as time_* and ln are not adapters; merge them into the model with "
+                        "tools/convert_model.py --lora)")
+            raise ValueError("adapter key %r is not <blocks.N.{att,ffn}.<projection>.lora_A|lora_B>%s" % (key, hint))
+        l, name = int(parts[1]), ".".join(parts[2:4])
+        if l >= L:
+            raise ValueError("adapter key %r: layer %d >= n_layers %d" % (key, l, L))
+        a = np.asarray(val.detach().cpu().numpy() if hasattr(val, "detach") else val, np.float32)
+        per.setdefault((l, name), {})[parts[4][-1]] = (key, a)
+    if not per:
+        raise ValueError("the adapter has no lora_A / lora_B tensors")
+    rank = None
+    mats = {}
+    for (l, name), ab in sorted(per.items()):
+        for half in "AB":
+            if half not in ab:
+                other = ab["B" if half == "A" else "A"][0]
+                raise ValueError("adapter key %r has no lora_%s partner" % (other, half))
+        n_in, n_out = adapter_dims(name, E)
+        (ka, A), (kb, B) = ab["A"], ab["B"]
+        r = A.shape[0] if A.ndim == 2 else -1
+        if rank is None:
+            rank = r
+        if not 1 <= r <= MAX_ADAPTER_RANK:
+            raise ValueError("adapter key %r: rank %d is outside 1..%d" % (ka, r, MAX_ADAPTER_RANK))
+        if r != rank:
+            raise ValueError("adapter key %r has rank %d, other projections have rank %d" % (ka, r, rank))
+        if A.shape != (rank, n_in):
+            raise ValueError("adapter key %r has shape %s, expected %s" % (ka, A.shape, (rank, n_in)))
+        if B.shape != (n_out, rank):
+            raise ValueError("adapter key %r has shape %s, expected %s" % (kb, B.shape, (n_out, rank)))
+        if name not in mats:
+            mats[name] = (np.zeros((L, rank, n_in), np.float32), np.zeros((L, n_out, rank), np.float32))
+        mats[name][0][l], mats[name][1][l] = A, B
+    return rank, mats
 
 
 def _stop_strings(strings):
@@ -369,6 +433,9 @@ def load_library():
         "rwkv_b200_index_download": (i32, [vp, ull, pull, ull, pdbl]),
         "rwkv_b200_index_remove": (i32, [vp, ull, pull, ull]),
         "rwkv_b200_index_search": (i32, [vp, ull, pull, ull, i32, c.c_uint, pull, pdbl, pdbl, pull]),
+        "rwkv_b200_adapter_add": (i32, [vp, c.POINTER(Adapter), pull]),
+        "rwkv_b200_adapter_remove": (i32, [vp, ull]),
+        "rwkv_b200_slot_adapter": (i32, [vp, ull, ull]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)  # AttributeError if a declared symbol is missing
@@ -591,6 +658,38 @@ class Engine:
         self._ck(self.lib.rwkv_b200_constraint_add(self.h, len(start) - 1, _ptr(start, P), _ptr(toks, P), _ptr(nxt, P),
                                                    ctypes.byref(cid)), "constraint_add")
         return int(cid.value)
+
+    def add_adapter(self, weights, alpha):
+        """Register a LoRA adapter and return its id; bind it to slots with bind_adapter. `weights` is a state dict or
+        the path of a .pth file loaded with torch. Keys follow the RWKV-4 LoRA trainers' convention: the checkpoint's
+        Linear name plus ".lora_A" [r][in] or ".lora_B" [out][r] (e.g. "blocks.3.att.key.lora_A"), for att key, value,
+        receptance and output and ffn key, value and receptance. The scale is alpha / r. Only synthetic checkpoints in
+        this naming have been tested. Unknown keys, mismatched ranks and wrong shapes raise ValueError; full-parameter
+        tensors (time_*, ln) cannot be applied at run time: merge them with tools/convert_model.py --lora."""
+        if isinstance(weights, (str, os.PathLike)):
+            import torch
+            weights = torch.load(weights, map_location="cpu", weights_only=True)
+        rank, mats = parse_adapter(weights, self.n_layers, self.n_embed)
+        d = Adapter()
+        d.rank, d.scale = rank, float(alpha) / rank
+        keep = []
+        for k, name in enumerate(ADAPTER_MATRICES):
+            if name in mats:
+                A, B = (np.ascontiguousarray(x) for x in mats[name])
+                keep += [A, B]
+                d.A[k], d.B[k] = _ptr(A, ctypes.c_float), _ptr(B, ctypes.c_float)
+        aid = ctypes.c_ulonglong()
+        self._ck(self.lib.rwkv_b200_adapter_add(self.h, ctypes.byref(d), ctypes.byref(aid)), "adapter_add")
+        return aid.value
+
+    def remove_adapter(self, aid):
+        self._ck(self.lib.rwkv_b200_adapter_remove(self.h, int(aid)), "adapter_remove")
+
+    def bind_adapter(self, slot, aid):
+        """Bind state slot `slot` to adapter `aid`, or unbind it with None. Every multi-stream call on the slot then
+        applies the adapter (on the tensor cores); the binding stays with the slot, not with the state."""
+        self._ck(self.lib.rwkv_b200_slot_adapter(self.h, int(slot), NO_ADAPTER if aid is None else int(aid)),
+                 "slot_adapter")
 
     def remove_constraint(self, cid):
         self._ck(self.lib.rwkv_b200_constraint_remove(self.h, int(cid)), "constraint_remove")

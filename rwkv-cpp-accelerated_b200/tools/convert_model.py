@@ -2,7 +2,11 @@
 
 Produces byte-for-byte what the reference's converter produces (converter/convert_model.py:14-176 builds
 the tensors, converter/cpp_save_tensor.cpp:75-95 writes them) without its torch C++ extension:
-    python convert_model.py model.pth [model.bin]
+    python convert_model.py model.pth [model.bin] [--lora adapter.pth --lora-alpha A]
+
+--lora merges a LoRA fine-tune into the weights before quantising (merge_lora): the fast path for one fine-tune on one
+stream, since the decode kernel then runs it at full speed. Several fine-tunes of one base model served together bind
+runtime adapters to state slots instead (Engine.add_adapter).
 
 File layout (include/rwkv/rwkv/format.h is the table this follows): two little-endian int64
 {n_layers, n_embed}, then the 46 tensors in enum order, unpadded - including the scratch buffers and the
@@ -14,8 +18,8 @@ Q8 scheme (convert_model.py:108-119) for a Linear weight W[out][in]: per INPUT c
 stored transposed [in][out] uint8 with ranges[in], zp[in] as f32; all arithmetic in f64.
 Pinned bit-exact against the reference's own Python class: tests/golden/converter_golden.json.
 """
+import argparse
 import struct
-import sys
 
 import numpy as np
 import torch
@@ -136,11 +140,48 @@ def write_bin(path, L, E, tensors):
             f.write(a.tobytes())
 
 
-def convert(pth_path, bin_path):
+def merge_lora(w, lora, alpha):
+    """The state dict w with a LoRA fine-tune merged in. Each pair "<linear>.lora_A" [r][in] / "<linear>.lora_B"
+    [out][r] (the RWKV-4 LoRA trainers' naming) adds s * B @ A, s = alpha / r, to "<linear>.weight" in float64; any other
+    key of `lora` that the checkpoint has (the trainers' full-parameter time_* and ln tensors) replaces it. Unknown
+    keys, a missing partner and wrong shapes raise ValueError."""
+    w = dict(w)
+    for key, val in lora.items():
+        if key.endswith(".lora_A") or key.endswith(".lora_B"):
+            base = key[:-len(".lora_A")]
+            if base + ".weight" not in w:
+                raise ValueError("LoRA key %s: the checkpoint has no %s.weight" % (key, base))
+            if key.endswith(".lora_B"):
+                continue
+            if base + ".lora_B" not in lora:
+                raise ValueError("LoRA key %s has no lora_B partner" % key)
+            A, B = val.to(torch.float64), lora[base + ".lora_B"].to(torch.float64)
+            W = w[base + ".weight"]
+            if A.dim() != 2 or B.dim() != 2 or B.shape[1] != A.shape[0] or (B.shape[0], A.shape[1]) != tuple(W.shape):
+                raise ValueError("LoRA %s: A %s and B %s do not fit the weight %s" % (base, tuple(A.shape), tuple(B.shape),
+                                                                                     tuple(W.shape)))
+            w[base + ".weight"] = W.to(torch.float64) + (alpha / A.shape[0]) * (B @ A)
+        elif key in w:
+            if tuple(val.shape) != tuple(w[key].shape):
+                raise ValueError("LoRA key %s has shape %s, the checkpoint's has %s" % (key, tuple(val.shape), tuple(w[key].shape)))
+            w[key] = val
+        else:
+            raise ValueError("LoRA key %s is neither a lora_A / lora_B pair nor a tensor of the checkpoint" % key)
+    for key in lora:
+        if key.endswith(".lora_B") and key[:-len(".lora_B")] + ".lora_A" not in lora:
+            raise ValueError("LoRA key %s has no lora_A partner" % key)
+    return w
+
+
+def convert(pth_path, bin_path, lora=None, lora_alpha=None):
     w = torch.load(pth_path, map_location="cpu")
     for k in ("emb.weight", "ln_out.weight", "ln_out.bias", "blocks.0.ln0.weight", "blocks.0.ln0.bias", "head.weight"):
         if k not in w:
             raise ValueError("not an RWKV-4 checkpoint: missing %s" % k)
+    if lora is not None:
+        if lora_alpha is None:
+            raise ValueError("--lora needs --lora-alpha")
+        w = merge_lora(w, torch.load(lora, map_location="cpu"), float(lora_alpha))
     L, E, tensors = build_tensors(w)
     print("n_layers %d  n_embed %d" % (L, E))
     write_bin(bin_path, L, E, tensors)
@@ -174,6 +215,10 @@ def synthetic_state_dict(L, E, seed, dtype=torch.float32):
 
 
 if __name__ == "__main__":
-    if len(sys.argv) < 2:
-        sys.exit(__doc__)
-    convert(sys.argv[1], sys.argv[2] if len(sys.argv) > 2 else "model.bin")
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("pth")
+    ap.add_argument("bin", nargs="?", default="model.bin")
+    ap.add_argument("--lora", help="a LoRA checkpoint to merge before quantising")
+    ap.add_argument("--lora-alpha", type=float, help="the LoRA alpha: the scale is alpha / rank")
+    a = ap.parse_args()
+    convert(a.pth, a.bin, a.lora, a.lora_alpha)
