@@ -17,6 +17,8 @@ or misread limb plane, a coarser quantiser, a dequantisation scale off by one pa
 Streams are independent token sequences, each on its own state (a dict of the engine's arrays, L * E doubles each),
 run layer by layer over all tokens at once like the tensor-core pass: the GEMMs see every token, the token shift and
 the WKV scan follow each stream."""
+import os
+
 import numpy as np
 
 V = 50277
@@ -79,16 +81,35 @@ class Model:
         self.head = (t["head"].reshape(E, V), t["head_r"], t["head_o"])
 
 
+_POOL = []
+
+
+def _widen(w, centre):
+    """The u8 block w as float64 (minus 128 if centre), converted by row blocks on every host core: at 7B and 14B the
+    single-threaded conversion, not the product, is most of a forward's time."""
+    threads = os.cpu_count() or 1
+    if not _POOL:
+        from concurrent.futures import ThreadPoolExecutor
+        _POOL.append(ThreadPoolExecutor(threads))
+    out = np.empty(w.shape)
+    rows = -(-w.shape[0] // threads)
+
+    def part(i):
+        if centre:
+            np.subtract(w[i:i + rows], 128.0, out=out[i:i + rows])
+        else:
+            out[i:i + rows] = w[i:i + rows]
+    list(_POOL[0].map(part, range(0, w.shape[0], rows)))
+    return out
+
+
 def _product(a, w, centre):
     """a [T][N] float64 times the u8 matrix w [N][M] (minus 128 if centre), in column chunks of <= 256 MB."""
     n, m = w.shape
     out = np.empty((a.shape[0], m))
     step = max(1, (1 << 25) // n)
     for c in range(0, m, step):
-        wc = np.asarray(w[:, c:c + step], np.float64)
-        if centre:
-            wc -= 128.0
-        out[:, c:c + step] = a @ wc
+        out[:, c:c + step] = a @ _widen(w[:, c:c + step], centre)
     return out
 
 
@@ -167,10 +188,15 @@ def expf(x, nudge=None):
     return e
 
 
-def forward(model, streams, states=None, mode="engine", mutation=None, nudge=None):
+def forward(model, streams, states=None, mode="engine", mutation=None, nudge=None, mutation_layers=None, inputs=None):
     """Run every stream (a list of token ids) from its state (None: zeros). Returns (logits [T_s][V] f32 per stream,
     the state after each stream's last token). nudge: a seed; a random half of the expf results of sigma(r) in the WKV
-    then come out one ulp higher (see sensitivity)."""
+    then come out one ulp higher (see sensitivity).
+
+    mutation_layers: the layers whose projections `mutation` applies to (None: every layer and the head), a bug that
+    hits one layer of many. inputs: a dict that a run without mutation fills with the residual stream entering each
+    layer ("x", [L] of [T][E]) and its states ("states"); a run of the same streams and states with mutation_layers
+    given that dict starts at the first mutated layer, since every layer before it computes what the plain run did."""
     nudge = None if nudge is None else np.random.default_rng(nudge)
     L, E = model.L, model.E
     sts = [{k: np.array(s[k], np.float64).reshape(L, E) for k in ("xy", "aa", "bb", "pp", "dd")}
@@ -179,7 +205,18 @@ def forward(model, streams, states=None, mode="engine", mutation=None, nudge=Non
     sid = np.concatenate([np.full(len(s), i) for i, s in enumerate(streams)])
     first = np.concatenate([np.arange(len(s)) == 0 for s in streams])
     last = np.concatenate([np.arange(len(s)) == len(s) - 1 for s in streams])
-    proj = lambda f, name, l: project(f, *(a[l] for a in model.proj[name]), mode=mode, mutation=mutation)
+    hit = lambda l: mutation_layers is None or l in mutation_layers
+    proj = lambda f, name, l: project(f, *(a[l] for a in model.proj[name]), mode=mode,
+                                      mutation=mutation if hit(l) else None)
+    l0 = 0
+    if inputs is not None and mutation is None:
+        inputs["x"] = []
+    elif inputs is not None:
+        assert mutation_layers and nudge is None and "states" in inputs, "inputs: a plain run fills it, a mutated one reads it"
+        l0 = min(mutation_layers)
+        for st, done in zip(sts, inputs["states"]):
+            for k in st:
+                st[k][:l0] = done[k].reshape(L, E)[:l0]
 
     def shifted(cur, key, l):
         """Token-shift input of every row: the previous row of its stream, or the stream's state at its first row."""
@@ -194,8 +231,10 @@ def forward(model, streams, states=None, mode="engine", mutation=None, nudge=Non
         return (m * cur + (1.0 - m) * prev).astype(np.float32)
 
     ln = model.ln
-    x = layernorm(np.asarray(model.embed[toks], np.float64), ln[0], ln[1])
-    for l in range(L):
+    x = layernorm(np.asarray(model.embed[toks], np.float64), ln[0], ln[1]) if l0 == 0 else inputs["x"][l0]
+    for l in range(l0, L):
+        if inputs is not None and mutation is None:
+            inputs["x"].append(x)
         a = layernorm(x, ln[4 * l + 2], ln[4 * l + 3])
         prev = shifted(a, "xy", l)
         k = proj(mix(model.mix_k[l], a, prev), "k", l)
@@ -224,10 +263,13 @@ def forward(model, streams, states=None, mode="engine", mutation=None, nudge=Non
         kk = np.maximum(proj(mix(model.ffn_mix_k[l], b, prev), "ffn_k", l), np.float32(0))
         x = x + (proj(kk * kk, "ffn_v", l) * sr).astype(np.float64)
     h = layernorm(x, ln[4 * L + 2], ln[4 * L + 3]).astype(np.float32)
-    logits = project(h, *model.head, mode=mode, mutation=mutation)
+    logits = project(h, *model.head, mode=mode, mutation=mutation if mutation_layers is None else None)
     ends = np.cumsum([len(s) for s in streams])
     out = np.split(logits, ends[:-1])
-    return out, [{k: s[k].reshape(-1) for k in s} for s in sts]
+    final = [{k: s[k].reshape(-1) for k in s} for s in sts]
+    if inputs is not None and mutation is None:
+        inputs["states"] = final
+    return out, final
 
 
 def sensitivity(model, streams, states=None, seeds=(1, 2)):
@@ -342,3 +384,68 @@ def case_model(case, make_model, tmp_dir):
     if not os.path.exists(dst):
         stress_model(src, dst, case["kind"], L=case["L"], E=case["E"])
     return dst
+
+
+# -- the cases of tests/test_depth_numerics_gpu.py ------------------------------------------------------------------
+# Production depth and width. Each model's cases are restated together, as independent streams of one pass, since the
+# restatement's cost is one conversion of every weight per pass; each stream comes out as it would alone.
+DEPTH_L = 3
+WIDE = {4096: {"decode": 8, "tc": 128}, 5104: {"decode": 8, "tc": 140}, 5120: {"decode": 8}}  # tc at 5104: two passes
+# The ragged calls at 3 x 4096: 24 one-token rows (generate_streams' decode step) and three streams, 128 tokens a call,
+# on 27 slots that hold state; the second call runs on the state the first wrote.
+RAGGED_CALLS = ((1,) * 10 + (40,) + (1,) * 7 + (33,) + (1,) * 7 + (31,),
+                (1,) * 5 + (37,) + (1,) * 12 + (45,) + (1,) * 7 + (22,))
+RAGGED_SLOTS = tuple((5 * i + 3) % 27 for i in range(27))
+BENCH_CASES = {"7b": {"decode": 16, "tc": 64, "greedy": 32}, "14b": {"decode": 8, "tc": 64},
+               "1b5": {"long": 1024, "switch": 264}}
+SWITCH = (200, 24, 40)   # 1b5: tensor cores, then the decode kernel, then tensor cores again, on one state
+
+
+def depth_passes(group, model, greedy=None):
+    """The restatement passes of a group (a width of WIDE or a workload of BENCH_CASES), in order: a list of
+    (case ids, streams, initial states or None). A "ragged-2" pass starts from the state a "ragged-1" pass ends in,
+    so passes() resolves its states (None here) from the previous pass. greedy: the tokens the 7B greedy chain fed the
+    device (the reference's greedy tokens where no device ran, on the host)."""
+    from util import reference_golden, token_stream
+    if group in WIDE:
+        ids = ["%s-%dx%d" % (p, DEPTH_L, group) for p in WIDE[group]]
+        streams = [token_stream(T, seed=group + i) for i, T in enumerate(WIDE[group].values())]
+        if group != 4096:
+            return [(ids, streams, None)]
+        pre = forward(model, [token_stream(3, seed=100 + i) for i in range(len(RAGGED_SLOTS))])[1]
+        rag = [[[int(t) for t in np.random.default_rng(1000 * c + i).integers(0, V, size=n)] for i, n in enumerate(lens)]
+               for c, lens in enumerate(RAGGED_CALLS)]
+        first = (ids + ["ragged-1"] * len(rag[0]), streams + rag[0], [zero_state(model.L, model.E)] * len(streams) + pre)
+        return [first, (["ragged-2"] * len(rag[1]), rag[1], None)]
+    g = [int(t) for t in reference_golden(group)["tokens"]]
+    ids, streams = [], []
+    for what, T in BENCH_CASES[group].items():
+        ids.append("%s-%s" % (what, group))
+        streams.append(token_stream(T, seed=2048) if what == "switch" else
+                       list(greedy) if what == "greedy" and greedy is not None else g[:T])
+    return [(ids, streams, None)]
+
+
+def stream_tols(model, streams, states, base, seeds=(1, 2)):
+    """case_tol of every stream of one pass, from the pass restated plainly (base) and nudged with each of `seeds`."""
+    tol = [[TOL, TOL] for _ in streams]
+    for seed in seeds:
+        l, s = forward(model, streams, states, nudge=seed)
+        for i in range(len(streams)):
+            le, se, _ = worst([l[i]], [base[0][i]], [s[i]], [base[1][i]], model.L, model.E)
+            tol[i] = [max(tol[i][0], 4 * le), max(tol[i][1], 4 * se)]
+    return [tuple(t) for t in tol]
+
+
+def passes(group, model, greedy=None, inputs=False):
+    """depth_passes with each pass restated: a list of dicts of ids, streams, states (initial), logits, final (states),
+    tols and, with inputs, the per-layer inputs of forward(inputs=) for layer-restricted mutations."""
+    out = []
+    for ids, streams, states in depth_passes(group, model, greedy):
+        if states is None and out:
+            states = [out[-1]["final"][i] for i, c in enumerate(out[-1]["ids"]) if c == "ragged-1"]
+        rec = {} if inputs else None
+        logits, final = forward(model, streams, states, inputs=rec)
+        out.append({"ids": ids, "streams": streams, "states": states, "logits": logits, "final": final, "inputs": rec,
+                    "tols": stream_tols(model, streams, states, (logits, final))})
+    return out
