@@ -1092,15 +1092,10 @@ struct GenCall {
 };
 
 // The checks of a GenCall whose streams name `per_stream` slots each. `values`: the override values are checked too.
-// `also`: a result array the caller requires as well, named `also_name` in the message.
-int check_gen(M *m, const char *what, const GenCall &c, unsigned long long per_stream, bool values, const void *also = nullptr,
-              const char *also_name = nullptr) {
+int check_gen(M *m, const char *what, const GenCall &c, unsigned long long per_stream, bool values) {
     if (c.n_streams == 0) return fail(1, "%s: no streams", what);
-    if (!c.slots || !c.first_tokens || !c.tokens_out || !c.lengths_out || (also_name && !also)) {
-        if (also_name)
-            return fail(1, "%s: null argument (slots, first_tokens, tokens_out, lengths_out and %s are required)", what, also_name);
+    if (!c.slots || !c.first_tokens || !c.tokens_out || !c.lengths_out)
         return fail(1, "%s: null argument (slots, first_tokens, tokens_out and lengths_out are required)", what);
-    }
     if (c.n_stop && !c.stop_tokens) return fail(1, "%s: n_stop = %llu with NULL stop_tokens", what, c.n_stop);
     if (c.n_override && (!c.override_tokens || !c.override_values))
         return fail(1, "%s: n_override = %llu with NULL override_tokens or override_values", what, c.n_override);
@@ -1191,6 +1186,167 @@ int pick_rows(M *m, const PickChain &pc, int rows, const double *u) {
     return 0;
 }
 
+// The log-probability request of generate_streams_logprobs and the calls after it, refused before any work.
+int check_logprobs(const char *what, const LogprobRequest &lpq) {
+    int rc;
+    if ((rc = check_logprob_mode(what, lpq.mode, lpq.top_n))) return rc;
+    if (!lpq.logprobs_out) return fail(1, "%s: logprobs_out is NULL", what);
+    if (lpq.top_n && (!lpq.top_tokens_out || !lpq.top_logprobs_out))
+        return fail(1, "%s: top_n = %u needs top_tokens_out and top_logprobs_out", what, lpq.top_n);
+    return 0;
+}
+
+// What a one-shot decoding call (generate() and speculate()) does besides emitting tokens: score them (lpq), follow
+// token automata (cq) and stop sets (sq), and count penalties; each request is NULL when the call has none. Built by
+// check_features, its buffers in m->gen readied by upload_features and its results written by finish_features.
+struct CallFeatures {
+    const LogprobRequest *lpq = nullptr;
+    const ConstraintRequest *cq = nullptr;
+    const rwkv_b200_stop_request *sq = nullptr;
+    std::vector<rk::GenConstraint> gc; // each stream's automaton (a zero record: none)
+    std::vector<rk::GenStop> st;       // each stream's stop set (a zero record: none)
+    // pen: some stream has a presence or frequency penalty; raw_copy: raw log-probabilities read a copy of the model's
+    // rows taken before the penalties, overrides and masks edit d_slogits
+    bool pen = false, constrained = false, stopped = false, raw_copy = false;
+    size_t n_lp = 0, n_top = 0; // entries of the log-probability and top arrays
+};
+
+// The automata and stop sets of a call's streams, checked against the model (the log-probability request is checked
+// by the caller, where its message comes first), and the flags and sizes that follow from them.
+int check_features(M *m, const char *what, const GenCall &c, const LogprobRequest *lpq, const ConstraintRequest *cq,
+                   const rwkv_b200_stop_request *sq, CallFeatures &f) {
+    const unsigned long long n = c.n_streams;
+    f.lpq = lpq;
+    f.cq = cq;
+    f.sq = sq;
+    for (unsigned long long s = 0; c.samplers && s < n; ++s)
+        f.pen |= c.samplers[s].presence_penalty != 0.0f || c.samplers[s].frequency_penalty != 0.0f;
+    int rc;
+    if (cq && (rc = check_constraints(m, what, *cq, n, c.override_tokens, c.override_values, c.n_override, f.gc))) return rc;
+    f.constrained = std::any_of(f.gc.begin(), f.gc.end(), [](const rk::GenConstraint &gc) { return gc.mask != nullptr; });
+    if ((rc = check_stops(m, what, sq, n, f.st))) return rc;
+    f.stopped = std::any_of(f.st.begin(), f.st.end(), [](const rk::GenStop &st) { return st.next != nullptr; });
+    f.raw_copy = lpq && lpq->mode == RWKV_B200_LOGPROBS_RAW && (f.pen || c.n_override || f.constrained);
+    f.n_lp = (size_t)(n * c.max_new);
+    f.n_top = lpq ? f.n_lp * lpq->top_n : 0;
+    return 0;
+}
+
+// The feature buffers of m->gen grown for n_streams streams and steps of at most `rows` logits rows, then filled: the
+// automata and stop sets uploaded, the fault record and penalty counts cleared, the result arrays set to all ones.
+int upload_features(M *m, const CallFeatures &f, unsigned long long n_streams, size_t rows) {
+    const size_t V = binfmt::kVocab;
+    auto &g = m->gen;
+    int rc;
+    if ((f.constrained && ((rc = g.gc.grow(n_streams)) || (rc = g.fault.grow(3)))) || (f.stopped && (rc = g.gst.grow(n_streams))) ||
+        (f.pen && ((rc = g.pen_cnt.grow(n_streams * V)) || (rc = g.pen_seen.grow(n_streams * V)))) ||
+        (f.lpq && ((rc = g.lp.grow(f.n_lp)) || (rc = g.rank.grow(f.n_lp)) || (rc = g.top_tok.grow(f.n_top)) ||
+                   (rc = g.top_lp.grow(f.n_top)) || (f.raw_copy && (rc = g.raw.grow(rows * V))))))
+        return rc;
+    if (f.constrained) {
+        CK(cudaMemcpyAsync(g.gc.p, f.gc.data(), n_streams * sizeof(rk::GenConstraint), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemsetAsync(g.fault.p, 0, 3 * sizeof(unsigned long long), m->stream));
+    }
+    if (f.stopped) CK(cudaMemcpyAsync(g.gst.p, f.st.data(), n_streams * sizeof(rk::GenStop), cudaMemcpyHostToDevice, m->stream));
+    if (f.pen) { // the history starts empty in every call: prompt tokens are not counted
+        CK(cudaMemsetAsync(g.pen_cnt.p, 0, n_streams * V * sizeof(float), m->stream));
+        CK(cudaMemsetAsync(g.pen_seen.p, 0, n_streams * V, m->stream));
+    }
+    if (f.lpq) { // all ones: NaN logprobs and RWKV_B200_NO_TARGET ranks and tokens wherever no token is emitted
+        CK(cudaMemsetAsync(g.lp.p, 0xFF, f.n_lp * sizeof(double), m->stream));
+        CK(cudaMemsetAsync(g.rank.p, 0xFF, f.n_lp * sizeof(unsigned long long), m->stream));
+        if (f.n_top) {
+            CK(cudaMemsetAsync(g.top_tok.p, 0xFF, f.n_top * sizeof(unsigned long long), m->stream));
+            CK(cudaMemsetAsync(g.top_lp.p, 0xFF, f.n_top * sizeof(double), m->stream));
+        }
+    }
+    return 0;
+}
+
+// The arguments every step of the call shares, over the buffers upload_features readied: the pick chain, the emit
+// rule and the scoring (all zero without scoring). The caller adds what its own steps need.
+void step_args(M *m, const CallFeatures &f, const GenCall &c, PickChain &pc, rk::GenEmit &e, rk::GenLogprobArgs &la) {
+    auto &g = m->gen;
+    pc = PickChain{};
+    pc.gs = g.gs;
+    pc.row_stream = g.row_stream;
+    pc.samp = c.samplers ? g.samp.p : nullptr;
+    pc.pen_cnt = f.pen ? g.pen_cnt.p : nullptr;
+    pc.pen_seen = g.pen_seen.p;
+    pc.ovr_tok = g.ovr_tok.p;
+    pc.ovr_val = g.ovr_val.p;
+    pc.n_override = c.n_override;
+    pc.gc = f.constrained ? g.gc.p : nullptr;
+    e = rk::GenEmit{};
+    e.out = g.out.p;
+    e.max_new = c.max_new;
+    e.stop = g.stop.p;
+    e.n_stop = (int)c.n_stop;
+    e.gc = f.constrained ? g.gc.p : nullptr;
+    e.fault = g.fault.p;
+    e.gst = f.stopped ? g.gst.p : nullptr;
+    la = rk::GenLogprobArgs{};
+    if (!f.lpq) return;
+    la.logits = f.raw_copy ? g.raw.p : m->d_slogits;
+    la.V = (int)binfmt::kVocab;
+    la.gs = g.gs;
+    la.row_stream = g.row_stream;
+    la.next = c.u || c.samplers ? nullptr : m->d_next;
+    la.sample = m->d_sample;
+    la.samp = f.lpq->mode == RWKV_B200_LOGPROBS_PROCESSED ? pc.samp : nullptr;
+    la.top_n = (int)f.lpq->top_n;
+    la.max_new = c.max_new;
+    la.logprob = g.lp.p;
+    la.rank = g.rank.p;
+    la.top_tokens = g.top_tok.p;
+    la.top_logprobs = g.top_lp.p;
+}
+
+// A step's copy of its `rows` model rows for raw log-probabilities, taken before the pick chain edits d_slogits.
+int copy_raw(M *m, const CallFeatures &f, int rows) {
+    if (f.raw_copy)
+        CK(cudaMemcpyAsync(m->gen.raw.p, m->d_slogits, (size_t)rows * binfmt::kVocab * sizeof(float), cudaMemcpyDeviceToDevice,
+                           m->stream));
+    return 0;
+}
+
+// The end of a group: `bytes` of stream records at `dev` come back into `host` with the automaton fault record, in one
+// synchronisation; an emitted token without an edge fails the call.
+int end_group(M *m, const char *what, const CallFeatures &f, void *host, const void *dev, size_t bytes) {
+    unsigned long long fault[3] = {0, 0, 0};
+    CK(cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, m->stream));
+    if (f.constrained) CK(cudaMemcpyAsync(fault, m->gen.fault.p, sizeof(fault), cudaMemcpyDeviceToHost, m->stream));
+    SYNC(m);
+    if (fault[0])
+        return fail(8, "%s: stream %llu emitted token %llu, which has no edge out of state %llu of its constraint", what,
+                    fault[0] - 1, fault[1], fault[2]);
+    return 0;
+}
+
+// The end of a call: the tokens, scores, automaton states and stop records come back (one synchronisation) and go to
+// the caller's arrays.
+int finish_features(M *m, CallFeatures &f, const GenCall &c) {
+    const auto &g = m->gen;
+    const unsigned long long n_streams = c.n_streams;
+    CK(cudaMemcpyAsync(c.tokens_out, g.out.p, n_streams * c.max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+    if (const LogprobRequest *lpq = f.lpq) {
+        CK(cudaMemcpyAsync(lpq->logprobs_out, g.lp.p, f.n_lp * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+        if (lpq->ranks_out) CK(cudaMemcpyAsync(lpq->ranks_out, g.rank.p, f.n_lp * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+        if (f.n_top) {
+            CK(cudaMemcpyAsync(lpq->top_tokens_out, g.top_tok.p, f.n_top * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+            CK(cudaMemcpyAsync(lpq->top_logprobs_out, g.top_lp.p, f.n_top * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+        }
+    }
+    if (f.constrained && f.cq->states_out)
+        CK(cudaMemcpyAsync(f.gc.data(), g.gc.p, n_streams * sizeof(rk::GenConstraint), cudaMemcpyDeviceToHost, m->stream));
+    if (f.stopped) CK(cudaMemcpyAsync(f.st.data(), g.gst.p, n_streams * sizeof(rk::GenStop), cudaMemcpyDeviceToHost, m->stream));
+    SYNC(m);
+    if (f.cq && f.cq->states_out)
+        for (unsigned long long s = 0; s < n_streams; ++s) f.cq->states_out[s] = f.gc[s].mask ? f.gc[s].state : 0;
+    write_stops(f.sq, f.st);
+    return 0;
+}
+
 // The body of generate_streams (samplers == NULL, `temp` and `u` pick the typical sampler or the arg-max), of
 // generate_streams_ex (`ex`: every stream has its own sampler, or all pick the arg-max when samplers == NULL), of
 // generate_streams_logprobs (generate_streams_ex with `lpq`: each emitted token is scored after its pick) and of
@@ -1200,38 +1356,16 @@ int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, cons
              const ConstraintRequest *cq = nullptr, const rwkv_b200_stop_request *sq = nullptr) {
     int rc = check_streams_model(m, what);
     if (rc) return rc;
-    if (lpq) {
-        if ((rc = check_logprob_mode(what, lpq->mode, lpq->top_n))) return rc;
-        if (!lpq->logprobs_out) return fail(1, "%s: logprobs_out is NULL", what);
-        if (lpq->top_n && (!lpq->top_tokens_out || !lpq->top_logprobs_out))
-            return fail(1, "%s: top_n = %u needs top_tokens_out and top_logprobs_out", what, lpq->top_n);
-    }
+    if (lpq && (rc = check_logprobs(what, *lpq))) return rc;
     if ((rc = check_gen(m, what, c, 1, ex))) return rc;
     bool bound;
     if ((rc = set_pass_adapters(m, what, c.slots, c.n_streams, bound))) return rc;
-    const size_t V = binfmt::kVocab;
+    CallFeatures f;
+    if ((rc = check_features(m, what, c, lpq, cq, sq, f))) return rc;
     const unsigned long long n_streams = c.n_streams, max_new = c.max_new;
-    bool pen = false; // some stream has a presence or frequency penalty
-    for (unsigned long long s = 0; c.samplers && s < n_streams; ++s)
-        pen |= c.samplers[s].presence_penalty != 0.0f || c.samplers[s].frequency_penalty != 0.0f;
-    std::vector<rk::GenConstraint> hgc;
-    if (cq && (rc = check_constraints(m, what, *cq, n_streams, c.override_tokens, c.override_values, c.n_override, hgc))) return rc;
-    const bool constrained = std::any_of(hgc.begin(), hgc.end(), [](const rk::GenConstraint &gc) { return gc.mask != nullptr; });
-    std::vector<rk::GenStop> hst;
-    if ((rc = check_stops(m, what, sq, n_streams, hst))) return rc;
-    const bool stopped = std::any_of(hst.begin(), hst.end(), [](const rk::GenStop &st) { return st.next != nullptr; });
     CK(cudaSetDevice(m->device));
     auto &g = m->gen;
-    if (constrained && ((rc = g.gc.grow(n_streams)) || (rc = g.fault.grow(3)))) return rc;
-    if (stopped && (rc = g.gst.grow(n_streams))) return rc;
-    if (pen && ((rc = g.pen_cnt.grow(n_streams * V)) || (rc = g.pen_seen.grow(n_streams * V)))) return rc;
     if (c.u && (rc = g.u.grow(kGenGroup * m->max_gpt))) return rc;
-    // raw mode reads the model's rows: d_slogits itself, or a copy taken before the penalties, overrides and mask edit it
-    const bool raw_copy = lpq && lpq->mode == RWKV_B200_LOGPROBS_RAW && (pen || c.n_override || constrained);
-    const size_t n_lp = (size_t)(n_streams * max_new), n_top = lpq ? n_lp * lpq->top_n : 0;
-    if (lpq && ((rc = g.lp.grow(n_lp)) || (rc = g.rank.grow(n_lp)) || (rc = g.top_tok.grow(n_top)) || (rc = g.top_lp.grow(n_top)) ||
-                (raw_copy && (rc = g.raw.grow(n_streams * V)))))
-        return rc;
     // the path is chosen once, for n_streams tokens; a stream's numbers depend only on its row
     const bool tc = tensor_cores(m, n_streams, bound);
     if (tc && (rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
@@ -1241,29 +1375,20 @@ int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, cons
     for (unsigned long long s = 0; s < n_streams; ++s)
         hg[s] = rk::GenStream{c.slots[s], c.budgets ? c.budgets[s] : max_new, c.first_tokens[s], 0, 0};
     CK(cudaMemcpyAsync(g.gs, hg, n_streams * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
-    if ((rc = upload_gen(m, c))) return rc;
-    if (constrained) {
-        CK(cudaMemcpyAsync(g.gc.p, hgc.data(), n_streams * sizeof(rk::GenConstraint), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemsetAsync(g.fault.p, 0, 3 * sizeof(unsigned long long), m->stream));
-    }
-    if (stopped) CK(cudaMemcpyAsync(g.gst.p, hst.data(), n_streams * sizeof(rk::GenStop), cudaMemcpyHostToDevice, m->stream));
-    if (pen) { // the history starts empty in every call: prompt tokens are not counted
-        CK(cudaMemsetAsync(g.pen_cnt.p, 0, n_streams * V * sizeof(float), m->stream));
-        CK(cudaMemsetAsync(g.pen_seen.p, 0, n_streams * V, m->stream));
-    }
-    if (lpq) { // all ones: NaN logprobs and RWKV_B200_NO_TARGET ranks and tokens wherever no token is emitted
-        CK(cudaMemsetAsync(g.lp.p, 0xFF, n_lp * sizeof(double), m->stream));
-        CK(cudaMemsetAsync(g.rank.p, 0xFF, n_lp * sizeof(unsigned long long), m->stream));
-        if (n_top) {
-            CK(cudaMemsetAsync(g.top_tok.p, 0xFF, n_top * sizeof(unsigned long long), m->stream));
-            CK(cudaMemsetAsync(g.top_lp.p, 0xFF, n_top * sizeof(double), m->stream));
-        }
-    }
+    if ((rc = upload_gen(m, c)) || (rc = upload_features(m, f, n_streams, n_streams))) return rc;
     std::vector<int> live(n_streams);
     for (unsigned long long s = 0; s < n_streams; ++s) live[s] = (int)s;
     std::vector<double> ug;
-    const PickChain pc{g.gs, g.row_stream, c.samplers ? g.samp.p : nullptr, pen ? g.pen_cnt.p : nullptr, g.pen_seen.p,
-                       g.ovr_tok.p, g.ovr_val.p, c.n_override, constrained ? g.gc.p : nullptr, sample_exponent(temp)};
+    PickChain pc;
+    rk::GenFeedbackArgs fb{};
+    rk::GenLogprobArgs la;
+    step_args(m, f, c, pc, fb.emit, la);
+    pc.exponent = sample_exponent(temp);
+    fb.gs = g.gs;
+    fb.row_stream = g.row_stream;
+    fb.next = c.u || c.samplers ? nullptr : m->d_next;
+    fb.sample = m->d_sample;
+    fb.passes = tc ? g.passes : nullptr;
     for (unsigned long long step = 0; !live.empty() && step < max_new;) {
         // a group: the live streams are rows 0..rows-1; their inputs, and the uniforms of its steps, go up once
         const int rows = (int)live.size();
@@ -1276,19 +1401,11 @@ int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, cons
                 for (int r = 0; r < rows; ++r) ug[k * rows + r] = c.u[(step + k) * n_streams + live[r]];
             CK(cudaMemcpyAsync(g.u.p, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
         }
-        rk::GenFeedbackArgs fb{g.gs, g.row_stream, rows, c.u || c.samplers ? nullptr : m->d_next, m->d_sample, g.stop.p, (int)c.n_stop,
-                               g.out.p, max_new, tc ? g.passes : nullptr, constrained ? g.gc.p : nullptr, g.fault.p, nullptr,
-                               stopped ? g.gst.p : nullptr};
-        rk::GenLogprobArgs la{};
-        if (lpq)
-            la = rk::GenLogprobArgs{raw_copy ? g.raw.p : m->d_slogits, (int)V, g.gs, g.row_stream, fb.next, m->d_sample,
-                                    lpq->mode == RWKV_B200_LOGPROBS_PROCESSED ? pc.samp : nullptr, (int)lpq->top_n, max_new,
-                                    g.lp.p, g.rank.p, g.top_tok.p, g.top_lp.p};
+        fb.rows = rows;
         for (unsigned long long k = 0; k < steps; ++k) {
-            if ((rc = tc ? gen_step_passes(m, g.passes, rows, rk::kPfMaxTokens) : gen_step_decode(m, rows, g.row_stream))) return rc;
-            if (raw_copy)
-                CK(cudaMemcpyAsync(g.raw.p, m->d_slogits, (size_t)rows * V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
-            if ((rc = pick_rows(m, pc, rows, c.u ? g.u.p + k * rows : nullptr))) return rc;
+            if ((rc = tc ? gen_step_passes(m, g.passes, rows, rk::kPfMaxTokens) : gen_step_decode(m, rows, g.row_stream)) ||
+                (rc = copy_raw(m, f, rows)) || (rc = pick_rows(m, pc, rows, c.u ? g.u.p + k * rows : nullptr)))
+                return rc;
             if (lpq) {
                 rk::k_gen_logprob<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(la);
                 LAUNCHED(m);
@@ -1297,33 +1414,172 @@ int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, cons
             LAUNCHED(m);
         }
         // the end of a group: which streams are done (a few bytes, one synchronisation); drop them from the rows
-        CK(cudaMemcpyAsync(hg, g.gs, n_streams * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
-        unsigned long long fault[3] = {0, 0, 0};
-        if (constrained) CK(cudaMemcpyAsync(fault, g.fault.p, sizeof(fault), cudaMemcpyDeviceToHost, m->stream));
-        SYNC(m);
-        if (fault[0])
-            return fail(8, "%s: stream %llu emitted token %llu, which has no edge out of state %llu of its constraint", what,
-                        fault[0] - 1, fault[1], fault[2]);
+        if ((rc = end_group(m, what, f, hg, g.gs, n_streams * sizeof(rk::GenStream)))) return rc;
         step += steps;
         live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hg[s].done != 0; }), live.end());
     }
-    CK(cudaMemcpyAsync(c.tokens_out, g.out.p, n_streams * max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
-    if (lpq) {
-        CK(cudaMemcpyAsync(lpq->logprobs_out, g.lp.p, n_lp * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
-        if (lpq->ranks_out) CK(cudaMemcpyAsync(lpq->ranks_out, g.rank.p, n_lp * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
-        if (n_top) {
-            CK(cudaMemcpyAsync(lpq->top_tokens_out, g.top_tok.p, n_top * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
-            CK(cudaMemcpyAsync(lpq->top_logprobs_out, g.top_lp.p, n_top * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
-        }
-    }
-    if (constrained && cq->states_out)
-        CK(cudaMemcpyAsync(hgc.data(), g.gc.p, n_streams * sizeof(rk::GenConstraint), cudaMemcpyDeviceToHost, m->stream));
-    if (stopped) CK(cudaMemcpyAsync(hst.data(), g.gst.p, n_streams * sizeof(rk::GenStop), cudaMemcpyDeviceToHost, m->stream));
-    SYNC(m);
+    if ((rc = finish_features(m, f, c))) return rc;
     for (unsigned long long s = 0; s < n_streams; ++s) c.lengths_out[s] = hg[s].len;
-    if (cq && cq->states_out)
-        for (unsigned long long s = 0; s < n_streams; ++s) cq->states_out[s] = hgc[s].mask ? hgc[s].state : 0;
-    write_stops(sq, hst);
+    return 0;
+}
+
+// What the speculative calls add to a GenCall: the drafts per step, the longest n-gram looked up, each stream's lookup
+// context (tokens context[context_start[s] .. context_start[s + 1]); NULL context_start: none) and the result array of
+// each stream's steps.
+struct SpecRequest {
+    unsigned draft, ngram;
+    const unsigned long long *context_start, *context;
+    unsigned long long *steps_out;
+};
+
+// Speculative generation: generate()'s group loop with k + 1 rows per live stream. Each step is k_spec_draft -> passes
+// -> pick_rows (overrides, automaton masks, pick) -> k_spec_accept (-> k_spec_logprob); at each group's end the records
+// come back and the finished streams leave the rows. At the end a stream whose home is a spare has it copied to its first
+// slot. With a stop request, k_spec_accept also walks each emitted token through the stream's stop set; with token
+// automata, k_spec_draft gives each row its state and k_spec_accept advances the automaton; with logprobs_out, each
+// emitted token is scored after k_spec_accept.
+int speculate(M *m, const char *what, const GenCall &c, const SpecRequest &sr, const LogprobRequest *lpq,
+              const ConstraintRequest *cq, const rwkv_b200_stop_request *sq) {
+    int rc = check_streams_model(m, what);
+    if (rc) return rc;
+    if (lpq && (rc = check_logprobs(what, *lpq))) return rc;
+    const unsigned draft = sr.draft, ngram = sr.ngram;
+    if (draft < 1 || draft > (unsigned)rk::kSpecMaxDraft) return fail(1, "%s: draft %u is outside 1..%d", what, draft, rk::kSpecMaxDraft);
+    if (ngram < 1 || ngram > (unsigned)rk::kSpecMaxNgram) return fail(1, "%s: ngram %u is outside 1..%d", what, ngram, rk::kSpecMaxNgram);
+    if (!rk::prefill_enabled(m->pf)) return fail(1, "%s: needs the tensor cores (the \"prefill\" option is 0)", what);
+    const unsigned long long K1 = draft + 1ull, S = c.n_streams, max_new = c.max_new;
+    if (S > m->max_gpt / K1)
+        return fail(1, "%s: %llu streams x %llu rows > max_gpt %llu", what, S, K1, m->max_gpt);
+    // steps_out joins check_gen's required arrays, in its message
+    if (S && (!c.slots || !c.first_tokens || !c.tokens_out || !c.lengths_out || !sr.steps_out))
+        return fail(1, "%s: null argument (slots, first_tokens, tokens_out, lengths_out and steps_out are required)", what);
+    if ((rc = check_gen(m, what, c, K1, true))) return rc;
+    for (unsigned long long s = 0; s < S; ++s)
+        if ((rc = check_same_binding(m, what, "stream", s, c.slots + s * K1, K1))) return rc;
+    bool bound;
+    if ((rc = set_pass_adapters(m, what, c.slots, S * K1, bound))) return rc;
+    for (unsigned long long s = 0; c.samplers && s < S; ++s)
+        if (c.samplers[s].presence_penalty != 0.0f || c.samplers[s].frequency_penalty != 0.0f)
+            return fail(1, "%s: stream %llu: presence and frequency penalties are not supported (a row's counts would have "
+                           "to include its own drafts)", what, s);
+    const unsigned long long *context_start = sr.context_start, *context = sr.context;
+    unsigned long long n_ctx = 0;
+    if (context_start) {
+        if (context_start[0] != 0) return fail(1, "%s: context_start[0] = %llu, not 0", what, context_start[0]);
+        for (unsigned long long s = 0; s < S; ++s)
+            if (context_start[s + 1] < context_start[s])
+                return fail(1, "%s: context_start decreases from stream %llu to %llu (%llu > %llu)", what, s, s + 1,
+                            context_start[s], context_start[s + 1]);
+        n_ctx = context_start[S];
+        if (n_ctx && !context) return fail(1, "%s: %llu context tokens with NULL context", what, n_ctx);
+        if ((rc = check_tokens(what, "context token", context, n_ctx))) return rc;
+    }
+    CallFeatures f;
+    if ((rc = check_features(m, what, c, lpq, cq, sq, f))) return rc;
+    const unsigned long long n_hist = n_ctx + S * (1 + max_new);
+    CK(cudaSetDevice(m->device));
+    auto &g = m->gen;
+    auto &sp = m->spec;
+    const int per_pass = rk::kPfMaxTokens / (int)K1; // streams per pass: a stream's rows never straddle two passes
+    const size_t n_pass = (size_t)((S + per_pass - 1) / per_pass);
+    if ((rc = sp.ss.grow(S)) || (rc = sp.hist.grow(n_hist)) || (rc = sp.live.grow(S)) || (rc = sp.passes.grow(n_pass)) ||
+        (c.u && ((rc = sp.u.grow(max_new * S)) || (rc = sp.row_u.grow(S * K1)))) || (rc = sp.forks.grow(2 * S)) ||
+        (f.constrained && (rc = sp.row_state.grow(S * K1))) || (lpq && (rc = sp.score.grow(S * K1))))
+        return rc;
+    if ((rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
+    m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
+
+    // the records and the histories: stream s's history starts with its context and its first token
+    std::vector<rk::SpecStream> hs(S);
+    std::vector<unsigned long long> hist(n_hist, 0); // stream s: its context, its first token, then room for max_new
+    for (unsigned long long s = 0, h0 = 0; s < S; ++s) {
+        rk::SpecStream &r = hs[s];
+        r = rk::SpecStream{};
+        for (unsigned long long i = 0; i < K1; ++i) r.slot[i] = c.slots[s * K1 + i];
+        const unsigned long long c0 = context_start ? context_start[s] : 0, c1 = context_start ? context_start[s + 1] : 0;
+        r.h0 = h0;
+        r.hl = c1 - c0 + 1;
+        r.budget = c.budgets ? c.budgets[s] : max_new;
+        r.u0 = s;
+        r.k = (int)draft;
+        r.ngram = (int)ngram;
+        std::copy(context + c0, context + c1, hist.begin() + h0);
+        hist[h0 + c1 - c0] = c.first_tokens[s];
+        h0 += r.hl + max_new;
+    }
+    CK(cudaMemcpyAsync(sp.hist.p, hist.data(), n_hist * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemcpyAsync(sp.ss.p, hs.data(), S * sizeof(rk::SpecStream), cudaMemcpyHostToDevice, m->stream));
+    if ((rc = upload_gen(m, c))) return rc;
+    if (c.u) CK(cudaMemcpyAsync(sp.u.p, c.u, max_new * S * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+    if ((rc = upload_features(m, f, S, S * K1))) return rc;
+
+    std::vector<int> live(S), rs;
+    std::vector<rk::SpecLive> lv;
+    for (unsigned long long s = 0; s < S; ++s) live[s] = (int)s;
+    rk::SpecArgs sa{};
+    sa.ss = sp.ss.p;
+    sa.live = sp.live.p;
+    sa.k = (int)draft;
+    sa.heads = true;
+    sa.hist = sp.hist.p;
+    sa.passes = sp.passes.p;
+    sa.u = c.u ? sp.u.p : nullptr;
+    sa.row_u = sp.row_u.p;
+    sa.u_stride = S;
+    sa.next = c.samplers ? nullptr : m->d_next;
+    sa.sample = m->d_sample;
+    sa.row_state = sp.row_state.p;
+    sa.score = lpq ? sp.score.p : nullptr;
+    PickChain pc;
+    rk::GenLogprobArgs la;
+    step_args(m, f, c, pc, sa.emit, la);
+    if (f.constrained) pc.row_state = sp.row_state.p;
+    // each step emits at least one token per live stream, so max_new steps finish every stream
+    for (unsigned long long step = 0; !live.empty() && step < max_new;) {
+        const int n_live = (int)live.size(), rows = n_live * (int)K1;
+        const unsigned long long steps = std::min(kGenGroup, max_new - step);
+        rs.resize(rows);
+        for (int r = 0; r < rows; ++r) rs[r] = live[r / (int)K1];
+        lv.resize(n_live);
+        for (int li = 0; li < n_live; ++li)
+            lv[li] = rk::SpecLive{live[li], li * (int)K1, li / per_pass * rk::kPfMaxTokens + li % per_pass * (int)K1};
+        CK(cudaMemcpyAsync(sp.live.p, lv.data(), n_live * sizeof(rk::SpecLive), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(g.row_stream, rs.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        for (unsigned long long k = 0; k < steps; ++k) {
+            rk::k_spec_draft<<<(unsigned)n_live, rk::kSpecDraftThreads, 0, m->stream>>>(sa);
+            LAUNCHED(m);
+            if ((rc = gen_step_passes(m, sp.passes.p, rows, per_pass * (int)K1)) || (rc = copy_raw(m, f, rows)) ||
+                (rc = pick_rows(m, pc, rows, c.u ? sp.row_u.p : nullptr)))
+                return rc;
+            rk::k_spec_accept<<<(unsigned)n_live, 32, 0, m->stream>>>(sa);
+            LAUNCHED(m);
+            if (lpq) {
+                rk::k_spec_logprob<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(sa, la);
+                LAUNCHED(m);
+            }
+        }
+        // the end of a group: which streams are done and any token without an edge (one synchronisation); drop the
+        // finished streams from the rows
+        if ((rc = end_group(m, what, f, hs.data(), sp.ss.p, S * sizeof(rk::SpecStream)))) return rc;
+        step += steps;
+        live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hs[s].done != 0; }), live.end());
+    }
+    // a home on a spare: its xy, aa, bb and dd go to the first slot (pp: no forward writes it)
+    std::vector<unsigned long long> forks;
+    for (unsigned long long s = 0; s < S; ++s)
+        if (hs[s].home != 0) {
+            forks.push_back(hs[s].slot[hs[s].home]);
+            forks.push_back(hs[s].slot[0]);
+        }
+    if (!forks.empty()) {
+        CK(cudaMemcpyAsync(sp.forks.p, forks.data(), forks.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        if ((rc = fork_slots(m, sp.forks.p, forks.size() / 2, false))) return rc;
+    }
+    if ((rc = finish_features(m, f, c))) return rc;
+    for (unsigned long long s = 0; s < S; ++s) {
+        c.lengths_out[s] = hs[s].len;
+        sr.steps_out[s] = hs[s].steps;
+    }
     return 0;
 }
 
@@ -1615,15 +1871,59 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
             return rc;
         CK(cudaMemcpyAsync(b->lp_lane.p, b->h_lp.data(), b->rows * sizeof(rk::LogprobLane), cudaMemcpyHostToDevice, m->stream));
     }
-    PickChain pc{b->gs.p, b->row_stream.p, b->samp.p, pen ? b->pen_cnt.p : nullptr, b->pen_seen.p, b->ovr_tok.p,
-                 b->ovr_val.p, b->n_ovr, constrained ? b->gc.p : nullptr, 0, b->ovr_start.p};
+    PickChain pc{};
+    pc.gs = b->gs.p;
+    pc.row_stream = b->row_stream.p;
+    pc.samp = b->samp.p;
+    pc.pen_cnt = pen ? b->pen_cnt.p : nullptr;
+    pc.pen_seen = b->pen_seen.p;
+    pc.ovr_tok = b->ovr_tok.p;
+    pc.ovr_val = b->ovr_val.p;
+    pc.n_override = b->n_ovr;
+    pc.gc = constrained ? b->gc.p : nullptr;
+    pc.ovr_start = b->ovr_start.p;
     if (spec && constrained) pc.row_state = b->row_state.p;
-    const rk::GenLogprobArgs la{m->d_slogits, (int)V, b->gs.p, b->row_stream.p, nullptr, m->d_sample, b->samp.p,
-                                top ? rk::kMaxTopN : 0, W, b->lp.p, b->rank.p, b->top_tok.p, b->top_lp.p,
-                                b->lp_lane.p, raw_copy ? b->raw.p : nullptr};
-    rk::SpecArgs sa{b->ss.p, b->spec_live.p, kmax, false, b->hist.p, nullptr, b->su.p, nullptr, 1, W, nullptr, m->d_sample,
-                    b->stop.p, 0, b->stop_start.p, b->out.p, stopped ? b->gst.p : nullptr, constrained ? b->gc.p : nullptr,
-                    b->row_state.p, b->fault.p, spec_scored ? b->score.p : nullptr};
+    rk::GenLogprobArgs la{};
+    la.logits = m->d_slogits;
+    la.V = (int)V;
+    la.gs = b->gs.p;
+    la.row_stream = b->row_stream.p;
+    la.sample = m->d_sample;
+    la.samp = b->samp.p;
+    la.top_n = top ? rk::kMaxTopN : 0;
+    la.max_new = W;
+    la.logprob = b->lp.p;
+    la.rank = b->rank.p;
+    la.top_tokens = b->top_tok.p;
+    la.top_logprobs = b->top_lp.p;
+    la.lane = b->lp_lane.p;
+    la.raw = raw_copy ? b->raw.p : nullptr;
+    // the emitted tokens of both kinds of lane: each lane's ring of W entries, its own stop tokens, automaton and set
+    rk::GenEmit emit{};
+    emit.out = b->out.p;
+    emit.max_new = W;
+    emit.stop = b->stop.p;
+    emit.stop_start = b->stop_start.p;
+    emit.gc = constrained ? b->gc.p : nullptr;
+    emit.fault = b->fault.p;
+    emit.gst = stopped ? b->gst.p : nullptr;
+    rk::SpecArgs sa{};
+    sa.ss = b->ss.p;
+    sa.live = b->spec_live.p;
+    sa.k = kmax;
+    sa.hist = b->hist.p;
+    sa.u = b->su.p;
+    sa.u_stride = 1;
+    sa.sample = m->d_sample;
+    sa.emit = emit;
+    sa.row_state = b->row_state.p;
+    sa.score = spec_scored ? b->score.p : nullptr;
+    rk::GenFeedbackArgs fb{};
+    fb.gs = b->gs.p;
+    fb.row_stream = b->row_stream.p;
+    fb.rows = Rp;
+    fb.sample = m->d_sample;
+    fb.emit = emit;
     for (unsigned long long k = 0; k < steps; ++k) {
         sa.passes = b->passes.p + k * ps;
         sa.row_u = b->u.p + k * NR;
@@ -1640,9 +1940,7 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
             LAUNCHED(m);
         }
         if (Rp > 0) {
-            rk::GenFeedbackArgs fb{b->gs.p, b->row_stream.p, Rp, nullptr, m->d_sample, b->stop.p, 0, b->out.p, W,
-                                   k + 1 < steps ? b->passes.p + (k + 1) * ps : nullptr, constrained ? b->gc.p : nullptr,
-                                   b->fault.p, b->stop_start.p, stopped ? b->gst.p : nullptr};
+            fb.passes = k + 1 < steps ? b->passes.p + (k + 1) * ps : nullptr;
             rk::k_gen_feedback<<<(unsigned)((Rp + 127) / 128), 128, 0, m->stream>>>(fb);
             LAUNCHED(m);
         }
@@ -2362,12 +2660,8 @@ int rwkv_b200_beam_search(rwkv_b200_model *m, const unsigned long long *slots, c
     return 0;
 }
 
-// Speculative generation: generate()'s group loop with k + 1 rows per live stream. Each step is k_spec_draft -> passes
-// -> pick_rows (overrides, automaton masks, pick) -> k_spec_accept (-> k_spec_logprob); at each group's end the records
-// come back and the finished streams leave the rows. At the end a stream whose home is a spare has it copied to its first
-// slot. With a stop request, k_spec_accept also walks each emitted token through the stream's stop set; with token
-// automata, k_spec_draft gives each row its state and k_spec_accept advances the automaton; with logprobs_out, each
-// emitted token is scored after k_spec_accept.
+// The speculative entry points. A call that asks for none of an entry's features is named after the narrower entry
+// that has only the features it uses.
 int rwkv_b200_generate_streams_speculative_constrained(
     rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens, unsigned long long n_streams,
     unsigned long long max_new, const unsigned long long *budgets, const unsigned long long *stop_tokens, unsigned long long n_stop,
@@ -2377,203 +2671,14 @@ int rwkv_b200_generate_streams_speculative_constrained(
     unsigned long long *steps_out, int logprob_mode, unsigned int top_n, double *logprobs_out, unsigned long long *ranks_out,
     unsigned long long *top_tokens_out, double *top_logprobs_out, const unsigned long long *constraint_ids,
     const unsigned long long *start_states, unsigned long long *states_out, const rwkv_b200_stop_request *sq) {
-    const char *what = logprobs_out || constraint_ids ? "generate_streams_speculative_constrained"
-                       : sq                           ? "generate_streams_speculative_stop"
-                                                      : "generate_streams_speculative";
-    int rc = check_streams_model(m, what);
-    if (rc) return rc;
-    if (logprobs_out) {
-        if ((rc = check_logprob_mode(what, logprob_mode, top_n))) return rc;
-        if (top_n && (!top_tokens_out || !top_logprobs_out))
-            return fail(1, "%s: top_n = %u needs top_tokens_out and top_logprobs_out", what, top_n);
-    }
-    if (draft < 1 || draft > (unsigned)rk::kSpecMaxDraft) return fail(1, "%s: draft %u is outside 1..%d", what, draft, rk::kSpecMaxDraft);
-    if (ngram < 1 || ngram > (unsigned)rk::kSpecMaxNgram) return fail(1, "%s: ngram %u is outside 1..%d", what, ngram, rk::kSpecMaxNgram);
-    if (!rk::prefill_enabled(m->pf)) return fail(1, "%s: needs the tensor cores (the \"prefill\" option is 0)", what);
-    const unsigned long long K1 = draft + 1ull, S = n_streams;
-    if (S > m->max_gpt / K1)
-        return fail(1, "%s: %llu streams x %llu rows > max_gpt %llu", what, S, K1, m->max_gpt);
-    if (!samplers) u = nullptr; // every stream takes the arg-max
-    const GenCall c{slots, first_tokens, S, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values, n_override,
-                    samplers, u, tokens_out, lengths_out};
-    if ((rc = check_gen(m, what, c, K1, true, steps_out, "steps_out"))) return rc;
-    for (unsigned long long s = 0; s < S; ++s)
-        if ((rc = check_same_binding(m, what, "stream", s, slots + s * K1, K1))) return rc;
-    bool bound;
-    if ((rc = set_pass_adapters(m, what, slots, S * K1, bound))) return rc;
-    for (unsigned long long s = 0; samplers && s < S; ++s)
-        if (samplers[s].presence_penalty != 0.0f || samplers[s].frequency_penalty != 0.0f)
-            return fail(1, "%s: stream %llu: presence and frequency penalties are not supported (a row's counts would have "
-                           "to include its own drafts)", what, s);
-    unsigned long long n_ctx = 0;
-    if (context_start) {
-        if (context_start[0] != 0) return fail(1, "%s: context_start[0] = %llu, not 0", what, context_start[0]);
-        for (unsigned long long s = 0; s < S; ++s)
-            if (context_start[s + 1] < context_start[s])
-                return fail(1, "%s: context_start decreases from stream %llu to %llu (%llu > %llu)", what, s, s + 1,
-                            context_start[s], context_start[s + 1]);
-        n_ctx = context_start[S];
-        if (n_ctx && !context) return fail(1, "%s: %llu context tokens with NULL context", what, n_ctx);
-        if ((rc = check_tokens(what, "context token", context, n_ctx))) return rc;
-    }
-    std::vector<rk::GenConstraint> hgc;
+    const GenCall c{slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values,
+                    n_override, samplers, samplers ? u : nullptr, tokens_out, lengths_out};
+    const LogprobRequest lpq{logprob_mode, top_n, logprobs_out, ranks_out, top_tokens_out, top_logprobs_out};
     const ConstraintRequest cq{constraint_ids, start_states, states_out};
-    if ((rc = check_constraints(m, what, cq, S, override_tokens, override_values, n_override, hgc))) return rc;
-    const bool constrained = std::any_of(hgc.begin(), hgc.end(), [](const rk::GenConstraint &gc) { return gc.mask != nullptr; });
-    std::vector<rk::GenStop> hst;
-    if ((rc = check_stops(m, what, sq, S, hst))) return rc;
-    const bool stopped = std::any_of(hst.begin(), hst.end(), [](const rk::GenStop &st) { return st.next != nullptr; });
-    const unsigned long long n_hist = n_ctx + S * (1 + max_new);
-    CK(cudaSetDevice(m->device));
-    auto &g = m->gen;
-    auto &sp = m->spec;
-    if (stopped && (rc = g.gst.grow(S))) return rc;
-    if (constrained && ((rc = g.gc.grow(S)) || (rc = g.fault.grow(3)) || (rc = sp.row_state.grow(S * K1)))) return rc;
-    // raw mode reads the model's rows: d_slogits itself, or a copy taken before the overrides and masks edit it
-    const bool scored = logprobs_out != nullptr, raw_copy = scored && logprob_mode == RWKV_B200_LOGPROBS_RAW && (n_override || constrained);
-    const size_t n_lp = (size_t)(S * max_new), n_top = scored ? n_lp * top_n : 0;
-    if (scored && ((rc = g.lp.grow(n_lp)) || (rc = g.rank.grow(n_lp)) || (rc = g.top_tok.grow(n_top)) || (rc = g.top_lp.grow(n_top)) ||
-                   (raw_copy && (rc = g.raw.grow(S * K1 * binfmt::kVocab)))))
-        return rc;
-    const int per_pass = rk::kPfMaxTokens / (int)K1; // streams per pass: a stream's rows never straddle two passes
-    const size_t n_pass = (size_t)((S + per_pass - 1) / per_pass);
-    if ((rc = sp.ss.grow(S)) || (rc = sp.hist.grow(n_hist)) || (rc = sp.live.grow(S)) || (rc = sp.passes.grow(n_pass)) ||
-        (u && ((rc = sp.u.grow(max_new * S)) || (rc = sp.row_u.grow(S * K1)))) || (rc = sp.forks.grow(2 * S)) ||
-        (scored && (rc = sp.score.grow(S * K1))))
-        return rc;
-    if ((rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
-    m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
-
-    // the records and the histories: stream s's history starts with its context and its first token
-    std::vector<rk::SpecStream> hs(S);
-    std::vector<unsigned long long> hist(n_hist, 0); // stream s: its context, its first token, then room for max_new
-    for (unsigned long long s = 0, h0 = 0; s < S; ++s) {
-        rk::SpecStream &r = hs[s];
-        r = rk::SpecStream{};
-        for (unsigned long long i = 0; i < K1; ++i) r.slot[i] = slots[s * K1 + i];
-        const unsigned long long c0 = context_start ? context_start[s] : 0, c1 = context_start ? context_start[s + 1] : 0;
-        r.h0 = h0;
-        r.hl = c1 - c0 + 1;
-        r.budget = budgets ? budgets[s] : max_new;
-        r.u0 = s;
-        r.k = (int)draft;
-        r.ngram = (int)ngram;
-        std::copy(context + c0, context + c1, hist.begin() + h0);
-        hist[h0 + c1 - c0] = first_tokens[s];
-        h0 += r.hl + max_new;
-    }
-    CK(cudaMemcpyAsync(sp.hist.p, hist.data(), n_hist * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-    CK(cudaMemcpyAsync(sp.ss.p, hs.data(), S * sizeof(rk::SpecStream), cudaMemcpyHostToDevice, m->stream));
-    if ((rc = upload_gen(m, c))) return rc;
-    if (u) CK(cudaMemcpyAsync(sp.u.p, u, max_new * S * sizeof(double), cudaMemcpyHostToDevice, m->stream));
-    if (stopped) CK(cudaMemcpyAsync(g.gst.p, hst.data(), S * sizeof(rk::GenStop), cudaMemcpyHostToDevice, m->stream));
-    if (constrained) {
-        CK(cudaMemcpyAsync(g.gc.p, hgc.data(), S * sizeof(rk::GenConstraint), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemsetAsync(g.fault.p, 0, 3 * sizeof(unsigned long long), m->stream));
-    }
-    if (scored) { // all ones: NaN logprobs and RWKV_B200_NO_TARGET ranks and tokens wherever no token is emitted
-        CK(cudaMemsetAsync(g.lp.p, 0xFF, n_lp * sizeof(double), m->stream));
-        CK(cudaMemsetAsync(g.rank.p, 0xFF, n_lp * sizeof(unsigned long long), m->stream));
-        if (n_top) {
-            CK(cudaMemsetAsync(g.top_tok.p, 0xFF, n_top * sizeof(unsigned long long), m->stream));
-            CK(cudaMemsetAsync(g.top_lp.p, 0xFF, n_top * sizeof(double), m->stream));
-        }
-    }
-
-    std::vector<int> live(S), rs;
-    std::vector<rk::SpecLive> lv;
-    for (unsigned long long s = 0; s < S; ++s) live[s] = (int)s;
-    rk::SpecArgs sa{sp.ss.p, sp.live.p, (int)draft, true, sp.hist.p, sp.passes.p, u ? sp.u.p : nullptr, sp.row_u.p, S, max_new,
-                    samplers ? nullptr : m->d_next, m->d_sample, g.stop.p, (int)n_stop, nullptr, g.out.p,
-                    stopped ? g.gst.p : nullptr, constrained ? g.gc.p : nullptr, sp.row_state.p, g.fault.p,
-                    scored ? sp.score.p : nullptr};
-    PickChain pc{nullptr, g.row_stream, samplers ? g.samp.p : nullptr, nullptr, nullptr, g.ovr_tok.p, g.ovr_val.p, n_override};
-    if (constrained) {
-        pc.gc = g.gc.p;
-        pc.row_state = sp.row_state.p;
-    }
-    rk::GenLogprobArgs la{};
-    if (scored) {
-        la.logits = raw_copy ? g.raw.p : m->d_slogits;
-        la.V = (int)binfmt::kVocab;
-        la.samp = logprob_mode == RWKV_B200_LOGPROBS_PROCESSED ? pc.samp : nullptr;
-        la.top_n = (int)top_n;
-        la.max_new = max_new;
-        la.logprob = g.lp.p;
-        la.rank = g.rank.p;
-        la.top_tokens = g.top_tok.p;
-        la.top_logprobs = g.top_lp.p;
-    }
-    // each step emits at least one token per live stream, so max_new steps finish every stream
-    for (unsigned long long step = 0; !live.empty() && step < max_new;) {
-        const int n_live = (int)live.size(), rows = n_live * (int)K1;
-        const unsigned long long steps = std::min(kGenGroup, max_new - step);
-        rs.resize(rows);
-        for (int r = 0; r < rows; ++r) rs[r] = live[r / (int)K1];
-        lv.resize(n_live);
-        for (int li = 0; li < n_live; ++li)
-            lv[li] = rk::SpecLive{live[li], li * (int)K1, li / per_pass * rk::kPfMaxTokens + li % per_pass * (int)K1};
-        CK(cudaMemcpyAsync(sp.live.p, lv.data(), n_live * sizeof(rk::SpecLive), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(g.row_stream, rs.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-        for (unsigned long long k = 0; k < steps; ++k) {
-            rk::k_spec_draft<<<(unsigned)n_live, rk::kSpecDraftThreads, 0, m->stream>>>(sa);
-            LAUNCHED(m);
-            if ((rc = gen_step_passes(m, sp.passes.p, rows, per_pass * (int)K1))) return rc;
-            if (raw_copy)
-                CK(cudaMemcpyAsync(g.raw.p, m->d_slogits, (size_t)rows * binfmt::kVocab * sizeof(float), cudaMemcpyDeviceToDevice,
-                                   m->stream));
-            if ((rc = pick_rows(m, pc, rows, u ? sp.row_u.p : nullptr))) return rc;
-            rk::k_spec_accept<<<(unsigned)n_live, 32, 0, m->stream>>>(sa);
-            LAUNCHED(m);
-            if (scored) {
-                rk::k_spec_logprob<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(sa, la);
-                LAUNCHED(m);
-            }
-        }
-        // the end of a group: which streams are done and any token without an edge (one synchronisation); drop the
-        // finished streams from the rows
-        CK(cudaMemcpyAsync(hs.data(), sp.ss.p, S * sizeof(rk::SpecStream), cudaMemcpyDeviceToHost, m->stream));
-        unsigned long long fault[3] = {0, 0, 0};
-        if (constrained) CK(cudaMemcpyAsync(fault, g.fault.p, sizeof(fault), cudaMemcpyDeviceToHost, m->stream));
-        SYNC(m);
-        if (fault[0])
-            return fail(8, "%s: stream %llu emitted token %llu, which has no edge out of state %llu of its constraint", what,
-                        fault[0] - 1, fault[1], fault[2]);
-        step += steps;
-        live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hs[s].done != 0; }), live.end());
-    }
-    // a home on a spare: its xy, aa, bb and dd go to the first slot (pp: no forward writes it)
-    std::vector<unsigned long long> forks;
-    for (unsigned long long s = 0; s < S; ++s)
-        if (hs[s].home != 0) {
-            forks.push_back(hs[s].slot[hs[s].home]);
-            forks.push_back(hs[s].slot[0]);
-        }
-    if (!forks.empty()) {
-        CK(cudaMemcpyAsync(sp.forks.p, forks.data(), forks.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-        if ((rc = fork_slots(m, sp.forks.p, forks.size() / 2, false))) return rc;
-    }
-    CK(cudaMemcpyAsync(tokens_out, g.out.p, S * max_new * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
-    if (scored) {
-        CK(cudaMemcpyAsync(logprobs_out, g.lp.p, n_lp * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
-        if (ranks_out) CK(cudaMemcpyAsync(ranks_out, g.rank.p, n_lp * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
-        if (n_top) {
-            CK(cudaMemcpyAsync(top_tokens_out, g.top_tok.p, n_top * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
-            CK(cudaMemcpyAsync(top_logprobs_out, g.top_lp.p, n_top * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
-        }
-    }
-    if (constrained && states_out)
-        CK(cudaMemcpyAsync(hgc.data(), g.gc.p, S * sizeof(rk::GenConstraint), cudaMemcpyDeviceToHost, m->stream));
-    if (stopped) CK(cudaMemcpyAsync(hst.data(), g.gst.p, S * sizeof(rk::GenStop), cudaMemcpyDeviceToHost, m->stream));
-    SYNC(m);
-    for (unsigned long long s = 0; s < S; ++s) {
-        lengths_out[s] = hs[s].len;
-        steps_out[s] = hs[s].steps;
-    }
-    if (states_out)
-        for (unsigned long long s = 0; s < S; ++s) states_out[s] = hgc[s].mask ? hgc[s].state : 0;
-    write_stops(sq, hst);
-    return 0;
+    return speculate(m, logprobs_out || constraint_ids ? "generate_streams_speculative_constrained"
+                        : sq                           ? "generate_streams_speculative_stop"
+                                                       : "generate_streams_speculative",
+                     c, SpecRequest{draft, ngram, context_start, context, steps_out}, logprobs_out ? &lpq : nullptr, &cq, sq);
 }
 
 int rwkv_b200_generate_streams_speculative_stop(rwkv_b200_model *m, const unsigned long long *slots,
@@ -2586,10 +2691,10 @@ int rwkv_b200_generate_streams_speculative_stop(rwkv_b200_model *m, const unsign
                                                 unsigned int ngram, const unsigned long long *context_start,
                                                 const unsigned long long *context, unsigned long long *steps_out,
                                                 const rwkv_b200_stop_request *sq) {
-    return rwkv_b200_generate_streams_speculative_constrained(
-        m, slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values, n_override,
-        samplers, u, tokens_out, lengths_out, draft, ngram, context_start, context, steps_out, RWKV_B200_LOGPROBS_RAW, 0, nullptr,
-        nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, sq);
+    const GenCall c{slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values,
+                    n_override, samplers, samplers ? u : nullptr, tokens_out, lengths_out};
+    return speculate(m, sq ? "generate_streams_speculative_stop" : "generate_streams_speculative", c,
+                     SpecRequest{draft, ngram, context_start, context, steps_out}, nullptr, nullptr, sq);
 }
 
 int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
@@ -2600,9 +2705,10 @@ int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned lo
                                            unsigned long long *tokens_out, unsigned long long *lengths_out, unsigned int draft,
                                            unsigned int ngram, const unsigned long long *context_start,
                                            const unsigned long long *context, unsigned long long *steps_out) {
-    return rwkv_b200_generate_streams_speculative_stop(m, slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop,
-                                                       override_tokens, override_values, n_override, samplers, u, tokens_out,
-                                                       lengths_out, draft, ngram, context_start, context, steps_out, nullptr);
+    const GenCall c{slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values,
+                    n_override, samplers, samplers ? u : nullptr, tokens_out, lengths_out};
+    return speculate(m, "generate_streams_speculative", c, SpecRequest{draft, ngram, context_start, context, steps_out}, nullptr,
+                     nullptr, nullptr);
 }
 
 int rwkv_b200_sample_streams(rwkv_b200_model *m, unsigned long long n_streams, const rwkv_b200_sampler *params, const double *u,

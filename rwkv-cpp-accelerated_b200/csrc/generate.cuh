@@ -9,7 +9,9 @@
 // generate_streams_logprobs adds k_gen_logprob (score.cuh) between the pick and k_gen_feedback.
 // generate_streams_constrained adds k_gen_mask after the overrides, and k_gen_feedback advances each constrained
 // stream's token automaton (GenConstraint) after appending its token. generate_streams_stop has k_gen_feedback walk each
-// emitted token's bytes through the stream's stop-string automaton (GenStop) as well.
+// emitted token's bytes through the stream's stop-string automaton (GenStop) as well. The rule that appends a token and
+// decides whether it ends its stream is gen_emit, over the arguments in GenEmit; k_spec_accept (speculate.cuh) emits its
+// accepted tokens by the same function.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -143,31 +145,52 @@ __device__ __forceinline__ bool gen_stop_walk(GenStop &m, unsigned long long tok
     return true;
 }
 
+// Where emitted tokens go and what ends a stream: k_gen_feedback's and k_spec_accept's shared arguments (gen_emit).
+struct GenEmit {
+    unsigned long long *out;         // [n_streams][max_new]: token k of stream s at [s][k % max_new]
+    unsigned long long max_new;
+    const unsigned long long *stop;  // [n_stop], or the tokens stop_start indexes
+    int n_stop;
+    // the batcher: stream s's own stop tokens are stop[stop_start[s] .. stop_start[s + 1]) (n_stop is not read);
+    // nullptr: stop[0 .. n_stop) for every stream
+    const unsigned long long *stop_start;
+    GenConstraint *gc;               // [n_streams] token automata (generate_streams_constrained), else nullptr
+    unsigned long long *fault;       // {stream + 1, token, state} of the first emitted token without an edge (gc only)
+    GenStop *gst;                    // [n_streams] stop sets (generate_streams_stop, batcher lanes with sets), else nullptr
+};
+
+// Append token tok of stream s as its entry number len (0-based) and say whether the stream ends with it. The checks
+// run in this order: the stream's budget, the stop tokens, its automaton (advanced by tok) and its stop strings (tok's
+// bytes walked through its stop set). A generate_streams call emits at most max_new tokens per stream, so `% max_new`
+// leaves its index alone; a batcher lane keeps one group's tokens in a ring.
+__device__ __forceinline__ bool gen_emit(const GenEmit &e, int s, unsigned long long len, unsigned long long budget,
+                                         unsigned long long tok) {
+    e.out[(size_t)s * e.max_new + len % e.max_new] = tok;
+    bool stop = len + 1 == budget;
+    if (e.stop_start) {
+        for (unsigned long long i = e.stop_start[s]; i < e.stop_start[s + 1]; ++i) stop |= e.stop[i] == tok;
+    } else {
+        for (int i = 0; i < e.n_stop; ++i) stop |= e.stop[i] == tok;
+    }
+    if (e.gc && e.gc[s].mask) stop |= gen_constraint_step(e.gc[s], tok, s, e.fault);
+    if (e.gst && e.gst[s].next) stop |= gen_stop_walk(e.gst[s], tok);
+    return stop;
+}
+
 struct GenFeedbackArgs {
     GenStream *gs;
     const int *row_stream;           // [rows] stream of each row
     int rows;
     const unsigned long long *next;  // arg-max per row, or nullptr when sampling
     const double *sample;            // {token, margin} per row when sampling
-    const unsigned long long *stop;  // [n_stop], or the tokens stop_start indexes
-    int n_stop;
-    unsigned long long *out;         // [n_streams][max_new]: token k of stream s at [s][k % max_new]
-    unsigned long long max_new;
     PassDesc *passes;                // tensor-core path: the descriptors of the next step, else nullptr
-    GenConstraint *gc;               // [n_streams] generate_streams_constrained, else nullptr
-    unsigned long long *fault;       // {stream + 1, token, state} of the first emitted token without an edge (gc only)
-    // the batcher: stream s's own stop tokens are stop[stop_start[s] .. stop_start[s + 1]) (n_stop is not read);
-    // nullptr: stop[0 .. n_stop) for every stream
-    const unsigned long long *stop_start;
-    GenStop *gst; // [n_streams] generate_streams_stop and batcher lanes with stop sets, else nullptr
+    GenEmit emit;
 };
 
-// One thread per row: emit the picked token of a live stream, then write the next step's input. On the tensor-core
-// path that is the row's token and descriptor in its pass; a finished stream loses kDescLast, so no pass stores its
-// slot again. `passes` is the next step's layout, whose row r is token r (the rows lead every pass set); the batcher
-// passes each step the layout of the step after it, since their prefill tokens differ. A generate_streams call emits at
-// most max_new tokens per stream, so `% max_new` leaves its index alone; a batcher lane keeps one group's tokens in a
-// ring of kGenGroup entries.
+// One thread per row: emit the picked token of a live stream (gen_emit), then write the next step's input. On the
+// tensor-core path that is the row's token and descriptor in its pass; a finished stream loses kDescLast, so no pass
+// stores its slot again. `passes` is the next step's layout, whose row r is token r (the rows lead every pass set); the
+// batcher passes each step the layout of the step after it, since their prefill tokens differ.
 __global__ void k_gen_feedback(const GenFeedbackArgs a) {
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= a.rows) return;
@@ -175,18 +198,9 @@ __global__ void k_gen_feedback(const GenFeedbackArgs a) {
     GenStream g = a.gs[s];
     if (!g.done) {
         const unsigned long long tok = a.next ? a.next[r] : (unsigned long long)a.sample[2 * r];
-        a.out[(size_t)s * a.max_new + g.len % a.max_new] = tok;
+        g.done = gen_emit(a.emit, s, g.len, g.budget, tok) ? 1ull : 0ull;
         g.len += 1;
         g.tok = tok;
-        bool stop = g.len == g.budget;
-        if (a.stop_start) {
-            for (unsigned long long i = a.stop_start[s]; i < a.stop_start[s + 1]; ++i) stop |= a.stop[i] == tok;
-        } else {
-            for (int i = 0; i < a.n_stop; ++i) stop |= a.stop[i] == tok;
-        }
-        if (a.gc && a.gc[s].mask) stop |= gen_constraint_step(a.gc[s], tok, s, a.fault);
-        if (a.gst && a.gst[s].next) stop |= gen_stop_walk(a.gst[s], tok);
-        g.done = stop ? 1ull : 0ull;
         a.gs[s] = g;
     }
     if (a.passes) {

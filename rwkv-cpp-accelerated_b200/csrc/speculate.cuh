@@ -12,8 +12,9 @@
 //                  of each row for k_sample_nucleus;
 //   forward        the tensor-core passes; a stream's k + 1 rows are consecutive head rows inside one pass (SpecLive);
 //   k_gen_override, then k_sample_nucleus or k_argmax_rows on the rows (row_stream maps every row of s to s);
-//   k_spec_accept  one CTA per live stream: the picks, the accepted prefix, stops and budget, the emitted tokens into
-//                  the output and the history, and the new home: the slot of the row that produced the last emitted token;
+//   k_spec_accept  one CTA per live stream: the picks, the accepted prefix, the emitted tokens into the output (by
+//                  gen_emit over SpecArgs::emit, the GenEmit of k_gen_feedback: budget, stops, automaton) and into the
+//                  history, and the new home: the slot of the row that produced the last emitted token;
 //   k_spec_logprob (with log-probabilities) one CTA per row: the emitted token of the row, if it emitted one, scored.
 // With token automata, k_spec_draft also walks the drafts through the stream's automaton into a state per row, by which
 // k_gen_mask masks the rows, and k_spec_accept advances the automaton by each emitted token (DESIGN §4.3).
@@ -71,19 +72,13 @@ struct SpecArgs {
     PassDesc *passes;                // the step's passes
     const double *u;                 // the uniforms, or nullptr
     double *row_u;                   // [rows] the uniform of each row (with u only)
-    unsigned long long u_stride, max_new;
+    unsigned long long u_stride;
     const unsigned long long *next;  // arg-max per row, or nullptr when sampling
     const double *sample;            // {token, margin} per row when sampling
-    const unsigned long long *stop;  // [n_stop], or the tokens stop_start indexes
-    int n_stop;
-    const unsigned long long *stop_start; // the batcher: stream s's stop tokens are stop[stop_start[s] .. [s + 1])
-    unsigned long long *out;         // [n_streams][max_new]: token j of stream s at [s][j % max_new]
-    GenStop *gst;                    // [n_streams] generate_streams_speculative_stop, else nullptr
-    // generate_streams_speculative_constrained with token automata, else nullptr: each stream's automaton and state, the
-    // state of each row this step (kNoState: not masked) and the record of an emitted token without an edge
-    GenConstraint *gc;               // [n_streams]
+    // the emitted tokens and what ends a stream (generate.cuh); emit.gc is set with token automata, and then row_state
+    // is the state of each row this step (kNoState: not masked)
+    GenEmit emit;
     unsigned long long *row_state;   // [rows]
-    unsigned long long *fault;       // [3]
     SpecScore *score;                // [live streams][k + 1] with log-probabilities, else nullptr
 };
 
@@ -125,11 +120,11 @@ __global__ void __launch_bounds__(kSpecDraftThreads) k_spec_draft(const SpecArgs
     const unsigned long long tok = row_tok(tid);
     g.row[tid] = tok;
     const int r = lv.row0 + tid, pi = (lv.pos0 + tid) / kPfMaxTokens, t = (lv.pos0 + tid) % kPfMaxTokens;
-    if (a.gc && tid == 0) {
+    if (a.emit.gc && tid == 0) {
         // row 0 has the stream's state; row i is live while row i - 1 is, draft i has an edge out of its state and that
         // edge leads to a state with edges. A dead row cannot be emitted: with no edge, the pick of the masked row
         // i - 1 differs from draft i; at a complete state, emitting draft i ends the stream
-        const GenConstraint &c = a.gc[s];
+        const GenConstraint &c = a.emit.gc[s];
         unsigned long long q = live && c.mask ? c.state : kNoState;
         a.row_state[r] = q;
         for (int i = 1; i <= k; ++i) {
@@ -154,9 +149,9 @@ __global__ void __launch_bounds__(kSpecDraftThreads) k_spec_draft(const SpecArgs
 }
 
 // One warp per live stream: lane i holds the pick p_i of row i; a = the leading i in 1..k with row[i] == p_{i - 1}.
-// Lane 0 emits p_0 .. p_a with k_gen_feedback's checks in its order (budget, stop tokens, automaton, stop strings) and
-// moves home to the slot of the last row used. With `score`, it records what k_spec_logprob scores: row i emitted p_i at
-// entry [s][(len + i) % max_new] (the one-shot index is below max_new; the batcher's is a ring), or nothing.
+// Lane 0 emits p_0 .. p_a by k_gen_feedback's rule (gen_emit) until one ends the stream, and moves home to the slot of
+// the last row used. With `score`, it records what k_spec_logprob scores: row i emitted p_i at entry
+// [s][(len + i) % max_new] (the one-shot index is below max_new; the batcher's is a ring), or nothing.
 __global__ void __launch_bounds__(32) k_spec_accept(const SpecArgs a) {
     const SpecLive lv = a.live[blockIdx.x];
     const int s = lv.s, lane = threadIdx.x;
@@ -181,23 +176,16 @@ __global__ void __launch_bounds__(32) k_spec_accept(const SpecArgs a) {
     bool stop = false;
     for (int i = 0; i <= acc && !stop; ++i) {
         const unsigned long long tok = pk[i];
-        a.out[(size_t)s * a.max_new + len % a.max_new] = tok;
+        stop = gen_emit(a.emit, s, len, g.budget, tok);
         a.hist[g.h0 + hl] = tok;
         ++len;
         ++hl;
         e = i;
-        stop = len == g.budget;
-        if (a.stop_start) {
-            for (unsigned long long z = a.stop_start[s]; z < a.stop_start[s + 1]; ++z) stop |= a.stop[z] == tok;
-        } else {
-            for (int z = 0; z < a.n_stop; ++z) stop |= a.stop[z] == tok;
-        }
-        if (a.gc && a.gc[s].mask) stop |= gen_constraint_step(a.gc[s], tok, s, a.fault);
-        if (a.gst && a.gst[s].next) stop |= gen_stop_walk(a.gst[s], tok);
     }
+    const unsigned long long max_new = a.emit.max_new;
     for (int i = 0; sc && i <= a.k; ++i) {
         const unsigned long long j = g.len + (unsigned long long)i;
-        sc[i] = i <= e ? SpecScore{lv.row0 + i, s, (size_t)s * a.max_new + j % a.max_new} : SpecScore{0, -1, 0};
+        sc[i] = i <= e ? SpecScore{lv.row0 + i, s, (size_t)s * max_new + j % max_new} : SpecScore{0, -1, 0};
     }
     g.len = len;
     g.hl = hl;

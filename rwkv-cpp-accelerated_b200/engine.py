@@ -838,27 +838,26 @@ class Engine:
         sp = _samplers(sampling, S) if sampling is not None else None
         P = ctypes.c_ulonglong
         args = (self.h, *lead, sp, *tail, int(draft), int(ngram), _ptr(cstart, P), _ptr(ctx, P), _ptr(steps, P))
+        sreq, sres = self._stop_request(stop_strings, S, "generate_speculative") if stop_strings is not None else (None, None)
+        sq = ctypes.byref(sreq) if sreq is not None else None
+        # the narrowest entry point that has the features asked for
         if extended:
-            sreq, sres = self._stop_request(stop_strings, S, "generate_speculative") if stop_strings is not None else (None, None)
-            self._ck(self.lib.rwkv_b200_generate_streams_speculative_constrained(
-                *args, *lp_args, *cargs, ctypes.byref(sreq) if sreq is not None else None),
-                "generate_streams_speculative_constrained")
-            res = []
-            for s in range(S):
-                n = int(lens[s])
-                d = {"tokens": out[s, :n].copy(), "steps": int(steps[s])}
-                if sres is not None:
-                    d.update(sres(s))
+            name, more = "generate_streams_speculative_constrained", (*lp_args, *cargs, sq)
+        elif sq is not None:
+            name, more = "generate_streams_speculative_stop", (sq,)
+        else:
+            name, more = "generate_streams_speculative", ()
+        self._ck(getattr(self.lib, "rwkv_b200_" + name)(*args, *more), name)
+        res = []
+        for s in range(S):
+            n = int(lens[s])
+            d = {"tokens": out[s, :n].copy(), "steps": int(steps[s])}
+            if sres is not None:
+                d.update(sres(s))
+            if extended:
                 d.update(scored(s, n))
-                res.append(d)
-            return res
-        if stop_strings is None:
-            self._ck(self.lib.rwkv_b200_generate_streams_speculative(*args), "generate_streams_speculative")
-            return [{"tokens": out[s, :int(lens[s])].copy(), "steps": int(steps[s])} for s in range(S)]
-        sreq, sres = self._stop_request(stop_strings, S, "generate_speculative")
-        self._ck(self.lib.rwkv_b200_generate_streams_speculative_stop(*args, ctypes.byref(sreq)),
-                 "generate_streams_speculative_stop")
-        return [dict({"tokens": out[s, :int(lens[s])].copy(), "steps": int(steps[s])}, **sres(s)) for s in range(S)]
+            res.append(d)
+        return res
 
     def batcher(self, rows, prefill_tokens):
         """Continuous batching (include/rwkv_b200.h, rwkv_b200_batcher_open): a Batcher with at most `rows` admitted
