@@ -881,6 +881,99 @@ int rwkv_b200_adapter_remove(rwkv_b200_model *m, unsigned long long id);
 /* Bind `slot` to adapter `id`, or unbind it with RWKV_B200_NO_ADAPTER (in stream order: later calls see it). */
 int rwkv_b200_slot_adapter(rwkv_b200_model *m, unsigned long long slot, unsigned long long id);
 
+/* Prefix state cache: requests that share a prompt prefix (a system prompt, a few-shot template, n samples of one
+ * prompt, the earlier turns of a chat) restore its recurrent state instead of prefilling it. The state after any prefix
+ * has a fixed size (xy, aa, bb and dd: 4 x n_layers x n_embed f64), so restoring it is one device copy however long the
+ * prefix is.
+ *  - Entries. A cache holds `capacity` entries in its own device allocation (4 x capacity x n_layers x n_embed f64). An
+ *    entry's key is the pair (the adapter bound to the stream's slot, or none; the exact token sequence run from the zero
+ *    state), and it holds the state after that sequence. Adapter ids are never reused, so the entries of a removed
+ *    adapter are unreachable and age out.
+ *  - Lookup. A stream hits the longest live entry whose key is a prefix of its tokens under its slot's binding. Keys are
+ *    compared token by token: a hash collision never returns a wrong state.
+ *  - Snapshots. A stream that restores r tokens and runs to its length n stores the state after every position p in
+ *    (r, n] that is a multiple of block_tokens, and after n. The pass writes it as it goes: the state after any token of
+ *    a pass is the state a pass ending there would store ("a stream's bits depend only on its own rows and its own
+ *    predecessors"), so a snapshot is bit for bit the state a zeroed slot reaches after its key. A position whose key is
+ *    already live is not written again and counts as a use of its entry.
+ *  - Eviction. A snapshot takes a free entry, else evicts the least recently used entry among those that no live entry
+ *    extends (leaves first: an entry is never evicted before a live entry whose key it is a proper prefix of) and that the
+ *    call is not itself writing. When no entry qualifies the snapshot is skipped and counted; results never depend on it.
+ *    Recency is a counter of uses (hits, existing keys, snapshots, inserts), not a clock, so every count below is a
+ *    function of the calls alone.
+ *  - Ordering. Everything runs on the model's one stream, in call order: a lookup sees every entry a finished call wrote,
+ *    and a restore reads an entry before a later pass of the same call overwrites it. A stream never hits a snapshot
+ *    taken in the same call.
+ *  - Memory and lifetime: the cache belongs to the model; rwkv_b200_free closes the model's caches.
+ * Refused before any work, with every slot and entry untouched: tensor parallelism, the "prefill" option 0, capacity 0,
+ * block_tokens outside 1..RWKV_B200_BATCHER_MAX_PREFILL, the refusals of rwkv_b200_forward_streams, an empty insert key
+ * or a token >= 50277. Not available: tensor parallelism, a cached prefix that does not start from the zero state,
+ * snapshots during generation (insert covers multi-turn chat), and the decode-kernel path. */
+typedef struct rwkv_b200_prefix_cache rwkv_b200_prefix_cache;
+struct rwkv_b200_prefix_stats { /* a struct tag, like struct stat beside stat() */
+    unsigned long long live;             /* entries that hold a state */
+    unsigned long long lookups;          /* streams looked up by prefix_forward */
+    unsigned long long hit_tokens;       /* tokens those streams restored instead of running */
+    unsigned long long prefilled_tokens; /* tokens those streams ran */
+    unsigned long long snapshots;        /* entries written: snapshots taken and inserts of a new key */
+    unsigned long long skipped;          /* snapshots skipped because no entry could be evicted */
+    unsigned long long evictions;
+};
+#define RWKV_B200_PREFIX_NOT_CACHED 2 /* rwkv_b200_prefix_download: no entry has the key */
+
+/* Open a cache of `capacity` entries that snapshots every block_tokens tokens; *out receives its handle. */
+int rwkv_b200_prefix_cache_open(rwkv_b200_model *m, unsigned long long capacity, unsigned long long block_tokens,
+                                rwkv_b200_prefix_cache **out);
+/* Wait for the model's work in flight, then free the cache. NULL is ignored; a cache that an unfinished batcher request
+ * names is refused. */
+int rwkv_b200_prefix_cache_close(rwkv_b200_prefix_cache *c);
+/* rwkv_b200_forward_streams in which every stream starts from the zero state (the slot's old contents are ignored) and
+ * restores its longest cached prefix: at most lengths[s] - 1 tokens when logits_out or next_out asks for a head, up to
+ * lengths[s] for a state-only call (a fully cached stream then runs no token). The rest runs on the tensor cores whatever
+ * its size, with the snapshots above; cached_out[s] (required, [n_streams]) receives the restored count.
+ * The rule: the logits, the arg-max and all five arrays of every named slot are bit for bit rwkv_b200_slot_zero of the
+ * slot followed by rwkv_b200_forward_streams of the full tokens on the tensor cores (prefill_min = 2, for calls of two
+ * tokens or more). Restoring writes xy, aa, bb and dd from the entry and pp = 0, which is what a zeroed slot holds after
+ * any forward. Enqueues one copy kernel per call (k_prefix_copy, also when nothing hits: it zeroes the slots), then the
+ * passes of the tokens not restored. */
+int rwkv_b200_prefix_forward(rwkv_b200_prefix_cache *c, const unsigned long long *tokens, unsigned long long n_tokens,
+                             const unsigned long long *slots, const unsigned long long *lengths, unsigned long long n_streams,
+                             float *logits_out, unsigned long long *next_out, unsigned long long *cached_out);
+/* Copy slot's xy, aa, bb and dd into the entry keyed by (slot's binding, tokens[0 .. n)), taking an entry by the
+ * eviction rule (an existing key is overwritten). The caller asserts that the slot holds the state a zeroed slot reaches
+ * after those tokens: for a chat turn, the prompt and every emitted token but the last, which is emitted and not fed. */
+int rwkv_b200_prefix_insert(rwkv_b200_prefix_cache *c, unsigned long long slot, const unsigned long long *tokens,
+                            unsigned long long n);
+/* The state of the entry keyed exactly by (no adapter, tokens[0 .. n)) into the host arrays [n_layers][n_embed] (NULL
+ * arrays are skipped); RWKV_B200_PREFIX_NOT_CACHED when there is none. Not a use of the entry. */
+int rwkv_b200_prefix_download(rwkv_b200_prefix_cache *c, const unsigned long long *tokens, unsigned long long n, double *xy,
+                              double *aa, double *bb, double *dd);
+/* The batcher with a prefix cache: rwkv_b200_batcher_submit_spec (spec may be NULL) whose request starts from the zero
+ * state and reuses the cache. cache == NULL is exactly submit_spec.
+ *  - Admission. When the request is admitted (a group boundary), it looks up its longest cached prefix of
+ *    prompt[0 .. n_prompt - 1) under its slot's binding and restores it into its slot (or zeroes the slot on a miss)
+ *    with one k_prefix_copy per cache, enqueued before the group's passes; its prefill continues after the restored
+ *    tokens, and lookups, hit tokens and prefilled tokens count in the cache's stats.
+ *  - Snapshots. Its prefill segments store the state after every block multiple and after n_prompt - 1 by the rules
+ *    above, into entries taken when the group's layouts are built (pinned until they are uploaded). A pass carries one
+ *    pool, so a snapshot into a second cache inside a pass that already writes another cache's pool is skipped and
+ *    counted. A request never hits a snapshot taken in its own group.
+ *  - The rule. Its emitted tokens, log-probabilities, ranks and top entries, automaton and stop-string state, steps and
+ *    final slot state are bit for bit those of the same request submitted without the cache on a zeroed slot, whatever
+ *    the other traffic, evictions, cancellations, prefill_tokens and max_steps.
+ *  - Refused as well, with nothing queued: a cache that is not an open cache of the batcher's model, and every refusal
+ *    of submit_spec (its spare slots must share the slot's binding). rwkv_b200_prefix_cache_close refuses a cache that an
+ *    unfinished request names. A failed run clears the caches its admitted requests name. */
+int rwkv_b200_batcher_submit_prefix(rwkv_b200_batcher *b, const rwkv_b200_request *r, const rwkv_b200_request_ex *x,
+                                    unsigned long long set_id, unsigned long long start_state,
+                                    const rwkv_b200_request_spec *spec, rwkv_b200_prefix_cache *cache, unsigned long long *id);
+/* The prompt tokens a request restored at admission (0 before admission or without a cache). An unknown or released id
+ * is refused. */
+int rwkv_b200_batcher_read_prefix(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *cached);
+/* Forget every entry (the counters other than live keep counting). */
+int rwkv_b200_prefix_clear(rwkv_b200_prefix_cache *c);
+int rwkv_b200_prefix_stats(rwkv_b200_prefix_cache *c, struct rwkv_b200_prefix_stats *out);
+
 /* Engine knobs (all optional), key/value strings: "sub_bytes" (largest bulk copy of the
  * weight stream, a multiple of 16 up to one ring stage of 8 x n_embed bytes), "budget" /
  * "qbudget" (bytes of copies in flight per SM while streaming, at least one stage / while

@@ -7,7 +7,7 @@ ABI) plus build helpers. The directory name contains a hyphen, so import it with
     import importlib
     pkg = importlib.import_module("rwkv-cpp-accelerated_b200")
 """
-from .engine import Batcher, Engine, EngineError, Sampler, StateIndex, lib_path, load_library  # noqa: F401
+from .engine import Batcher, Engine, EngineError, PrefixCache, Sampler, StateIndex, lib_path, load_library  # noqa: F401
 from . import build as build  # noqa: F401
 from . import constrain as constrain  # noqa: F401
 from . import tp as tp  # noqa: F401

@@ -39,6 +39,8 @@
 #include "generate.cuh"
 #include "index.cuh"
 #include "prefill.cuh"
+#include "prefix.cuh"
+#include "prefix_index.h"
 #include "sampling.cuh"
 #include "score.cuh"
 #include "speculate.cuh"
@@ -224,6 +226,17 @@ struct rwkv_b200_model {
     unsigned long long next_adapter = 1;
     std::vector<unsigned long long> slot_ad;
     DevBuf<rk::AdapterRec> ad_table; // [max_gpt]
+    std::vector<rwkv_b200_prefix_cache *> prefix_caches; // open caches, closed by rwkv_b200_free
+};
+
+// rwkv_b200_prefix_cache_open: the index on the host, the pool on the device, and the {entry, slot} pairs of a copy
+struct rwkv_b200_prefix_cache {
+    rwkv_b200_model *m = nullptr;
+    prefix::Index index;
+    unsigned long long block = 0;
+    DevBuf<double> pool;               // xy, aa, bb, dd: each [capacity][L][E]
+    DevBuf<unsigned long long> pairs;  // [max_gpt][2]
+    explicit rwkv_b200_prefix_cache(size_t capacity) : index(capacity) {}
 };
 
 // rwkv_b200_batcher: the requests on the host, and per lane (0..rows-1, one per admitted request, reused) its stream
@@ -259,6 +272,9 @@ struct rwkv_b200_batcher {
         std::vector<unsigned long long> spares, context;
         unsigned long long steps = 0;
         int home = 0;
+        // rwkv_b200_batcher_submit_prefix: the cache (nullptr: none) and the prompt tokens restored at admission
+        rwkv_b200_prefix_cache *cache = nullptr;
+        unsigned long long cached = 0;
     };
     std::map<unsigned long long, Req> reqs;
     unsigned long long next_id = 1;
@@ -716,6 +732,10 @@ int do_load(M *m, const char *path, int quiet) {
     if ((rc = dmalloc(m, &m->gen.gs, m->max_gpt)) || (rc = dmalloc(m, &m->gen.row_stream, m->max_gpt)) ||
         (rc = dmalloc(m, &m->gen.passes, (m->max_gpt + rk::kPfMaxTokens - 1) / rk::kPfMaxTokens)))
         return rc;
+    // every pass of the generation calls starts zeroed: an upload fills the first step's passes, and k_beam_select and
+    // k_gen_feedback then fill tokens, descriptors and row maps of passes no upload reached, so no snapshot field there
+    // may hold leftover bytes
+    CK(cudaMemsetAsync(m->gen.passes, 0, (m->max_gpt + rk::kPfMaxTokens - 1) / rk::kPfMaxTokens * sizeof(rk::PassDesc), m->stream));
     CK(cudaMallocHost((void **)&m->gen.h_gs, sizeof(rk::GenStream) * m->max_gpt));
     CK(cudaHostAlloc((void **)&m->h_diag, sizeof(rk::Diag), cudaHostAllocMapped));
     memset(m->h_diag, 0, sizeof(rk::Diag));
@@ -1488,6 +1508,8 @@ int speculate(M *m, const char *what, const GenCall &c, const SpecRequest &sr, c
         return rc;
     if ((rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
     m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
+    // k_spec_draft fills the tokens, descriptors and row maps only: the rest of each pass (no snapshots) stays zero
+    CK(cudaMemsetAsync(sp.passes.p, 0, n_pass * sizeof(rk::PassDesc), m->stream));
 
     // the records and the histories: stream s's history starts with its context and its first token
     std::vector<rk::SpecStream> hs(S);
@@ -1584,6 +1606,9 @@ int speculate(M *m, const char *what, const GenCall &c, const SpecRequest &sr, c
 }
 
 using B = rwkv_b200_batcher;
+using PC = rwkv_b200_prefix_cache;
+int prefix_copy(PC *c, const std::vector<unsigned long long> &pairs, bool restore);
+void prefix_pool(const PC *c, double *(&pool)[4]);
 
 int check_batcher(const B *b) {
     if (!b) return fail(1, "null batcher handle");
@@ -1598,10 +1623,18 @@ int batcher_boundary(B *b, std::vector<int> &dec) {
     M *m = b->m;
     const size_t V = binfmt::kVocab;
     auto &ad = b->admitted;
+    std::map<PC *, std::vector<unsigned long long>> restores; // per cache, the {entry, slot} pairs of its admissions
     while (!b->queue.empty() && ad.size() < (size_t)b->rows) {
         const unsigned long long id = b->queue.front();
         b->queue.pop_front();
         B::Req &q = b->reqs[id];
+        if (q.cache) { // the longest cached prefix of prompt[0 .. n_prompt - 1), restored before the group's passes
+            long e = -1;
+            prefix::Index &ix = q.cache->index;
+            q.fed = q.cached = ix.lookup(slot_binding(m, q.slot), q.prompt.data(), q.prompt.size() - 1, &e);
+            ix.stats().prefilled_tokens += q.prompt.size() - 1 - q.cached;
+            restores[q.cache].insert(restores[q.cache].end(), {e >= 0 ? (unsigned long long)e : rk::kPrefixZero, q.slot});
+        }
         q.lane = (int)(std::find(b->lane_used.begin(), b->lane_used.end(), 0) - b->lane_used.begin());
         b->lane_used[q.lane] = 1;
         q.status = RWKV_B200_REQ_PREFILLING;
@@ -1617,6 +1650,8 @@ int batcher_boundary(B *b, std::vector<int> &dec) {
             CK(cudaMemsetAsync(b->pen_seen.p + (size_t)q.lane * V, 0, V, m->stream));
         }
     }
+    for (auto &r : restores)
+        if (int rc = prefix_copy(r.first, r.second, true)) return rc;
     dec.clear();
     for (unsigned long long id : ad) {
         B::Req &q = b->reqs[id];
@@ -1762,11 +1797,14 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
     std::vector<int> step_rows(steps);
     std::vector<std::vector<int>> H(steps);
     size_t ps = (size_t)b->max_pass; // passes per step in `passes`
+    std::vector<PC *> snapped; // caches with entries pinned by this group's layouts
     for (unsigned long long k = 0; k < steps; ++k) {
         std::vector<unsigned long long> tokens(dtok), slots(dslot), lens(dtok.size(), 1);
         std::vector<unsigned char> head(dhead);
+        std::vector<size_t> seg0; // each segment's first token in the step
         for (const Seg &s : segs[k]) {
             const B::Req &q = b->reqs[s.id];
+            seg0.push_back(tokens.size());
             tokens.insert(tokens.end(), q.prompt.begin() + (long)s.off, q.prompt.begin() + (long)(s.off + s.n));
             slots.push_back(q.slot);
             lens.push_back(s.n);
@@ -1775,8 +1813,33 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
         step_rows[k] = (int)tokens.size();
         rk::pass_layout(tokens.data(), step_rows[k], slots.data(), lens.data(), 2, nullptr, lay[k], H[k], head.data());
         for (int p : pads) lay[k][p / rk::kPfMaxTokens].desc[p % rk::kPfMaxTokens] &= ~rk::kDescLast;
+        // snapshots of cached requests at block multiples and at n_prompt - 1 inside their segments. A pass carries one
+        // pool: a snapshot into a second cache's pool in the same pass is skipped (and counted)
+        for (size_t i = 0; i < segs[k].size(); ++i) {
+            const Seg &sg = segs[k][i];
+            const B::Req &q = b->reqs[sg.id];
+            if (!q.cache) continue;
+            double *pool[4];
+            prefix_pool(q.cache, pool);
+            for (unsigned long long pos = sg.off + 1; pos <= sg.off + sg.n; ++pos) {
+                if (pos % q.cache->block != 0 && pos + 1 != q.prompt.size()) continue;
+                const size_t g = seg0[i] + (size_t)(pos - sg.off - 1);
+                rk::PassDesc &pd = lay[k][g / rk::kPfMaxTokens];
+                if (pd.pool[0] && pd.pool[0] != pool[0]) {
+                    q.cache->index.stats().skipped += 1;
+                    continue;
+                }
+                bool fresh = false;
+                const long e = q.cache->index.take(slot_binding(m, q.slot), q.prompt.data(), (size_t)pos, &fresh);
+                if (std::find(snapped.begin(), snapped.end(), q.cache) == snapped.end()) snapped.push_back(q.cache);
+                if (e < 0 || !fresh) continue;
+                pd.snap[g % rk::kPfMaxTokens] = (uint32_t)e + 1u;
+                std::copy(pool, pool + 4, pd.pool);
+            }
+        }
         ps = std::max(ps, lay[k].size());
     }
+    for (PC *c : snapped) c->index.unpin_all();
     std::vector<rk::PassDesc> all(steps * ps);
     for (unsigned long long k = 0; k < steps; ++k) std::copy(lay[k].begin(), lay[k].end(), all.begin() + k * ps);
     // a speculative lane emits up to kGenGroup (k + 1) tokens in a group
@@ -2041,6 +2104,86 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
 // =================================================================================================
 // C ABI
 // =================================================================================================
+// ---- prefix state cache (csrc/prefix.cuh, csrc/prefix_index.h) -----------------------------------------------------
+namespace {
+// The base pointers of the pool's xy, aa, bb and dd arrays.
+void prefix_pool(const PC *c, double *(&pool)[4]) {
+    const size_t per = c->index.capacity() * (size_t)(c->m->L * c->m->E);
+    for (int i = 0; i < 4; ++i) pool[i] = c->pool.p + i * per;
+}
+
+int check_cache(PC *c, const char *what) {
+    if (!c) return fail(1, "%s: null prefix cache handle", what);
+    return check_streams_model(c->m, what);
+}
+
+// k_prefix_copy over the {entry, slot} pairs (kPrefixZero: the zero state): restore = entry -> slot, else slot -> entry
+int prefix_copy(PC *c, const std::vector<unsigned long long> &pairs, bool restore) {
+    M *m = c->m;
+    const unsigned long long n = pairs.size() / 2;
+    if (n == 0) return 0;
+    CK(cudaMemcpyAsync(c->pairs.p, pairs.data(), pairs.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    rk::PrefixCopyArgs a{};
+    const size_t LE = (size_t)(m->L * m->E);
+    prefix_pool(c, a.pool);
+    slot_arrays(m, 0, a.slot);
+    a.LE = LE;
+    a.pairs = c->pairs.p;
+    a.restore = restore ? 1 : 0;
+    rk::k_prefix_copy<<<rk::prefix_copy_grid(LE, restore, n), rk::kPrefixThreads, 0, m->stream>>>(a);
+    LAUNCHED(m);
+    return 0;
+}
+
+// The ragged call of rwkv_b200_prefix_forward after its checks. The index changes before the device work is enqueued,
+// so a call that fails after that point clears it: no entry may promise a state that was never written.
+int prefix_forward(PC *c, const unsigned long long *tokens, const unsigned long long *slots, const unsigned long long *lengths,
+                   unsigned long long S, bool head, std::vector<unsigned long long> &cached) {
+    M *m = c->m;
+    prefix::Index &ix = c->index;
+    std::vector<unsigned long long> pairs(2 * S), rtok, rslot, rlen, off(S);
+    std::vector<long> hit(S);
+    for (unsigned long long s = 0, o = 0; s < S; o += lengths[s], ++s) {
+        off[s] = o;
+        cached[s] = ix.lookup(slot_binding(m, slots[s]), tokens + o, lengths[s] - (head ? 1 : 0), &hit[s]);
+        pairs[2 * s] = hit[s] >= 0 ? (unsigned long long)hit[s] : rk::kPrefixZero;
+        pairs[2 * s + 1] = slots[s];
+        if (cached[s] == lengths[s]) continue; // state only and fully cached: no token runs
+        rtok.insert(rtok.end(), tokens + o + cached[s], tokens + o + lengths[s]);
+        rslot.push_back(slots[s]);
+        rlen.push_back(lengths[s] - cached[s]);
+    }
+    const int n = (int)rtok.size();
+    std::vector<rk::PassDesc> passes;
+    std::vector<int> heads;
+    if (n > 0) rk::pass_layout(rtok.data(), n, rslot.data(), rlen.data(), head ? 2 : 0, nullptr, passes, heads);
+    // snapshots: the state after p tokens, for p in (cached, length] at multiples of the block and at the length
+    for (unsigned long long s = 0, g0 = 0; s < S; ++s) {
+        const unsigned long long r = cached[s], len = lengths[s];
+        for (unsigned long long p = r + 1; p <= len; ++p) {
+            if (p % c->block != 0 && p != len) continue;
+            bool fresh = false;
+            const long e = ix.take(slot_binding(m, slots[s]), tokens + off[s], (size_t)p, &fresh);
+            if (e < 0 || !fresh) continue;
+            const unsigned long long g = g0 + (p - r - 1); // its token in the remainder list
+            passes[g / rk::kPfMaxTokens].snap[g % rk::kPfMaxTokens] = (uint32_t)e + 1u;
+        }
+        g0 += len - r;
+    }
+    ix.unpin_all();
+    ix.stats().prefilled_tokens += (unsigned long long)n;
+    for (rk::PassDesc &pd : passes) prefix_pool(c, pd.pool);
+    int rc = prefix_copy(c, pairs, true);
+    if (!rc && n > 0) {
+        rc = rk::prefill_passes(m->pf, m->p, m->stream, passes, heads, n, m->d_slogits);
+        if (rc) rc = fail(rc, "%s", rk::prefill_error());
+        m->launches += rk::prefill_launches(m->pf);
+    }
+    if (rc) ix.clear();
+    return rc;
+}
+} // namespace
+
 extern "C" {
 
 const char *rwkv_b200_last_error(void) { return g_err.c_str(); }
@@ -2091,6 +2234,7 @@ void rwkv_b200_free(rwkv_b200_model *m) {
     cudaSetDevice(m->device);
     if (m->stream) cudaStreamSynchronize(m->stream);
     rwkv_b200_batcher_close(m->batcher);
+    while (!m->prefix_caches.empty()) rwkv_b200_prefix_cache_close(m->prefix_caches.back());
     rk::prefill_free(m->pf);
     for (void *p : m->ipc_opened) cudaIpcCloseMemHandle(p);
     for (void *p : m->allocs) cudaFree(p);
@@ -3331,7 +3475,12 @@ int rwkv_b200_batcher_run(rwkv_b200_batcher *b, unsigned long long max_steps, un
     b->m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
     for (unsigned long long done = 0; done < max_steps;) {
         unsigned long long ran = 0;
-        if ((rc = batcher_group(b, std::min(kGenGroup, max_steps - done), &ran))) return rc;
+        if ((rc = batcher_group(b, std::min(kGenGroup, max_steps - done), &ran))) {
+            // the caches of the admitted requests may name snapshots that were never written
+            for (unsigned long long id : b->admitted)
+                if (b->reqs[id].cache) b->reqs[id].cache->index.clear();
+            return rc;
+        }
         if (ran == 0) break;
         done += ran;
         if (steps_run) *steps_run = done;
@@ -3440,6 +3589,27 @@ int rwkv_b200_batcher_submit_spec(rwkv_b200_batcher *b, const rwkv_b200_request 
     return 0;
 }
 
+int rwkv_b200_batcher_submit_prefix(rwkv_b200_batcher *b, const rwkv_b200_request *r, const rwkv_b200_request_ex *x,
+                                    unsigned long long set_id, unsigned long long start_state,
+                                    const rwkv_b200_request_spec *spec, rwkv_b200_prefix_cache *cache, unsigned long long *id) {
+    int rc = check_batcher(b);
+    if (rc) return rc;
+    if (cache && std::find(b->m->prefix_caches.begin(), b->m->prefix_caches.end(), cache) == b->m->prefix_caches.end())
+        return fail(1, "batcher_submit_prefix: the prefix cache is not an open cache of the batcher's model");
+    if ((rc = rwkv_b200_batcher_submit_spec(b, r, x, set_id, start_state, spec, id)) || !cache) return rc;
+    b->reqs.at(*id).cache = cache;
+    return 0;
+}
+
+int rwkv_b200_batcher_read_prefix(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *cached) {
+    int rc = check_batcher(b);
+    if (rc) return rc;
+    const auto it = b->reqs.find(id);
+    if (it == b->reqs.end()) return fail(1, "batcher_read_prefix: request %llu is unknown or released", id);
+    if (cached) *cached = it->second.cached;
+    return 0;
+}
+
 int rwkv_b200_batcher_read_spec(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *steps) {
     int rc = check_batcher(b);
     if (rc) return rc;
@@ -3504,6 +3674,139 @@ void rwkv_b200_batcher_close(rwkv_b200_batcher *b) {
         b->m->batcher = nullptr;
     }
     delete b;
+}
+
+
+int rwkv_b200_prefix_cache_open(rwkv_b200_model *m, unsigned long long capacity, unsigned long long block_tokens,
+                                rwkv_b200_prefix_cache **out) {
+    int rc = check_streams_model(m, "prefix_cache_open");
+    if (rc) return rc;
+    if (!out) return fail(1, "prefix_cache_open: null argument");
+    if (!rk::prefill_enabled(m->pf)) return fail(1, "prefix_cache_open: the cache runs on the tensor cores, and the \"prefill\" option is 0");
+    if (capacity == 0) return fail(1, "prefix_cache_open: capacity 0");
+    if (block_tokens == 0 || block_tokens > RWKV_B200_BATCHER_MAX_PREFILL)
+        return fail(1, "prefix_cache_open: block_tokens %llu outside 1..%llu", block_tokens, RWKV_B200_BATCHER_MAX_PREFILL);
+    const size_t LE = (size_t)(m->L * m->E);
+    if (capacity > SIZE_MAX / (4 * LE * sizeof(double))) return fail(1, "prefix_cache_open: capacity %llu is too large", capacity);
+    CK(cudaSetDevice(m->device));
+    PC *c = new (std::nothrow) PC((size_t)capacity);
+    if (!c) return fail(1, "prefix_cache_open: out of host memory");
+    c->m = m;
+    c->block = block_tokens;
+    if ((rc = c->pool.grow(4 * (size_t)capacity * LE)) || (rc = c->pairs.grow(2 * m->max_gpt))) {
+        delete c;
+        return rc;
+    }
+    m->prefix_caches.push_back(c);
+    *out = c;
+    return 0;
+}
+
+int rwkv_b200_prefix_cache_close(rwkv_b200_prefix_cache *c) {
+    if (!c) return 0;
+    M *m = c->m;
+    if (m->batcher)
+        for (const auto &e : m->batcher->reqs)
+            if (e.second.cache == c && e.second.status <= RWKV_B200_REQ_GENERATING)
+                return fail(1, "prefix_cache_close: unfinished batcher request %llu uses the cache", e.first);
+    cudaSetDevice(m->device);
+    cudaStreamSynchronize(m->stream); // passes and copies in flight may still write or read the pool
+    m->prefix_caches.erase(std::find(m->prefix_caches.begin(), m->prefix_caches.end(), c));
+    delete c;
+    return 0;
+}
+
+int rwkv_b200_prefix_forward(rwkv_b200_prefix_cache *c, const unsigned long long *tokens, unsigned long long n_tokens,
+                             const unsigned long long *slots, const unsigned long long *lengths, unsigned long long n_streams,
+                             float *logits_out, unsigned long long *next_out, unsigned long long *cached_out) {
+    const char *what = "prefix_forward";
+    int rc = check_cache(c, what);
+    if (rc) return rc;
+    M *m = c->m;
+    if ((rc = check_ragged(m, what, tokens, n_tokens, slots, lengths, n_streams))) return rc;
+    if (!cached_out) return fail(1, "%s: null cached_out", what);
+    if (!rk::prefill_enabled(m->pf)) return fail(1, "%s: the cache runs on the tensor cores, and the \"prefill\" option is 0", what);
+    bool bound;
+    if ((rc = set_pass_adapters(m, what, slots, n_streams, bound))) return rc;
+    CK(cudaSetDevice(m->device));
+    const size_t V = binfmt::kVocab;
+    const bool head = logits_out || next_out;
+    m->stream_rows = 0;
+    std::vector<unsigned long long> cached(n_streams);
+    if ((rc = prefix_forward(c, tokens, slots, lengths, n_streams, head, cached))) return rc;
+    if (next_out) {
+        rk::k_argmax_rows<<<(unsigned)n_streams, rk::kArgmaxThreads, 0, m->stream>>>(m->d_slogits, (int)V, m->d_next);
+        LAUNCHED(m);
+        CK(cudaMemcpyAsync(m->h_next, m->d_next, n_streams * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+    }
+    if (logits_out) CK(cudaMemcpyAsync(m->h_logits, m->d_slogits, n_streams * V * sizeof(float), cudaMemcpyDeviceToHost, m->stream));
+    SYNC(m);
+    if (next_out) memcpy(next_out, m->h_next, n_streams * sizeof(unsigned long long));
+    if (logits_out && logits_out != m->h_logits) memcpy(logits_out, m->h_logits, n_streams * V * sizeof(float));
+    std::copy(cached.begin(), cached.end(), cached_out);
+    m->stream_rows = head ? n_streams : 0;
+    return 0;
+}
+
+int rwkv_b200_prefix_insert(rwkv_b200_prefix_cache *c, unsigned long long slot, const unsigned long long *tokens,
+                            unsigned long long n) {
+    const char *what = "prefix_insert";
+    int rc = check_cache(c, what);
+    if (rc || (rc = check_slot(c->m, what, slot))) return rc;
+    if (!tokens || n == 0) return fail(1, "%s: empty key", what);
+    if ((rc = check_tokens(what, "token id", tokens, n))) return rc;
+    M *m = c->m;
+    CK(cudaSetDevice(m->device));
+    bool fresh = false;
+    const long e = c->index.take(slot_binding(m, slot), tokens, (size_t)n, &fresh);
+    c->index.unpin_all(); // with nothing else pinned, some entry is always evictable
+    if (e < 0) return fail(3, "%s: no entry could be taken", what);
+    if ((rc = prefix_copy(c, {(unsigned long long)e, slot}, false))) {
+        c->index.clear();
+        return rc;
+    }
+    SYNC(m);
+    return 0;
+}
+
+int rwkv_b200_prefix_download(rwkv_b200_prefix_cache *c, const unsigned long long *tokens, unsigned long long n, double *xy,
+                              double *aa, double *bb, double *dd) {
+    const char *what = "prefix_download";
+    int rc = check_cache(c, what);
+    if (rc) return rc;
+    if (!tokens || n == 0) return fail(1, "%s: empty key", what);
+    const long e = c->index.find(RWKV_B200_NO_ADAPTER, tokens, (size_t)n);
+    if (e < 0) return fail(RWKV_B200_PREFIX_NOT_CACHED, "%s: no entry has this key", what);
+    M *m = c->m;
+    CK(cudaSetDevice(m->device));
+    const size_t LE = (size_t)(m->L * m->E), per = c->index.capacity() * LE;
+    double *dst[4] = {xy, aa, bb, dd};
+    for (int i = 0; i < 4; ++i)
+        if (dst[i]) CK(cudaMemcpyAsync(dst[i], c->pool.p + i * per + (size_t)e * LE, LE * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+    SYNC(m);
+    return 0;
+}
+
+int rwkv_b200_prefix_clear(rwkv_b200_prefix_cache *c) {
+    int rc = check_cache(c, "prefix_clear");
+    if (rc) return rc;
+    c->index.clear();
+    return 0;
+}
+
+int rwkv_b200_prefix_stats(rwkv_b200_prefix_cache *c, struct rwkv_b200_prefix_stats *out) {
+    int rc = check_cache(c, "prefix_stats");
+    if (rc) return rc;
+    if (!out) return fail(1, "prefix_stats: null argument");
+    const prefix::Stats &s = c->index.stats();
+    out->live = s.live;
+    out->lookups = s.lookups;
+    out->hit_tokens = s.hit_tokens;
+    out->prefilled_tokens = s.prefilled_tokens;
+    out->snapshots = s.snapshots;
+    out->skipped = s.skipped;
+    out->evictions = s.evictions;
+    return 0;
 }
 
 int rwkv_b200_decode_timed(rwkv_b200_model *m, const unsigned long long *tokens, unsigned long long n,

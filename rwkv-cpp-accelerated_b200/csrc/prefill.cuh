@@ -53,12 +53,19 @@ __host__ __device__ __forceinline__ size_t desc_slot(uint32_t d) { return (size_
 
 // Everything a pass reads that changes from pass to pass; one host-to-device copy per pass. The kernels of a
 // recorded graph read it through fixed pointers, so the layout is data and never part of the graph.
+// Snapshots (prefix caches, prefix.cuh): snap[t] = e + 1 writes the state after token t into entry e of the pool whose
+// xy, aa, bb and dd arrays start at pool[0..3] (entry stride L * E, like the slots); 0 takes none. A zero-initialised
+// descriptor takes no snapshot, so every producer that fills only tokens and desc stays correct, and a graph recorded
+// for one pass serves passes with and without a cache.
 struct PassDesc {
     unsigned long long tokens[kPfMaxTokens];
     uint32_t desc[kPfMaxTokens];
     int rows[kPfMaxTokens]; // head row i = token rows[i] of the pass
     int out_row0;           // head row i goes to logits row out_row0 + i
+    uint32_t snap[kPfMaxTokens];
+    double *pool[4];
 };
+enum : int { kPoolXY = 0, kPoolAA, kPoolBB, kPoolDD };
 
 // ---- LoRA adapters (include/rwkv_b200.h, "adapters") ----------------------------------------------------------
 // A slot's adapter record lives in a per-slot device table, so a token finds its adapter through its descriptor's slot
@@ -390,10 +397,15 @@ struct WkvArgs {
     int E, T, Tp;
     float *rw, *xs;                   // [T][E]
     const double *dk, *dv, *dr;       // NULL, or the adapters' deltas [T][E]
+    const PassDesc *pass;             // its snap and pool (snapshots of aa, bb)
+    size_t lo;                        // this layer's offset inside an entry
 };
 __global__ void __launch_bounds__(256) k_pf_wkv(const __grid_constant__ WkvArgs a) {
-    __shared__ uint32_t desc[kPfMaxTokens]; // read once per t by every thread of the sequential scan
-    for (int t = threadIdx.x; t < a.T; t += blockDim.x) desc[t] = a.desc[t];
+    __shared__ uint32_t desc[kPfMaxTokens], snap[kPfMaxTokens]; // read once per t by every thread of the sequential scan
+    for (int t = threadIdx.x; t < a.T; t += blockDim.x) {
+        desc[t] = a.desc[t];
+        snap[t] = a.pass->snap[t];
+    }
     __syncthreads();
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= a.E) return;
@@ -423,6 +435,11 @@ __global__ void __launch_bounds__(256) k_pf_wkv(const __grid_constant__ WkvArgs 
             const size_t o = desc_slot(d) * a.slot_stride + c;
             a.aa[o] = aa;
             a.bb[o] = bb;
+        }
+        if (const uint32_t e = snap[t]) { // the state after this token into a prefix cache entry
+            const size_t o = (size_t)(e - 1) * a.slot_stride + a.lo + c;
+            a.pass->pool[kPoolAA][o] = aa;
+            a.pass->pool[kPoolBB][o] = bb;
         }
         const float rw = (float)y;
         a.rw[(size_t)t * a.E + c] = rw;
@@ -471,14 +488,21 @@ __global__ void __launch_bounds__(256) k_pf_logits(const int *C, const double *s
     logits[(size_t)*row0 * V + i] = pf_combine(C, Tp, (size_t)v, h, scale[h], offs[h]);
 }
 
-// token-shift state after the pass: state[slot] = ln[t] for the last token t of each stream in the pass
-// (block = token; the blocks of the other tokens leave at once)
-__global__ void __launch_bounds__(256) k_pf_store_state(const double *ln, int E, const uint32_t *desc, size_t slot_stride, double *state) {
+// token-shift state after the pass: state[slot] = ln[t] for the last token t of each stream in the pass, and array
+// `which` of entry snap[t] - 1 at layer offset lo for a snapshot token (block = token; the blocks of the other tokens
+// leave at once)
+__global__ void __launch_bounds__(256) k_pf_store_state(const double *ln, int E, const PassDesc *pass, size_t slot_stride, double *state,
+                                                        int which, size_t lo) {
     const int t = blockIdx.x;
-    const uint32_t d = desc[t];
-    if (!(d & kDescLast)) return;
-    double *dst = state + desc_slot(d) * slot_stride;
-    for (int j = threadIdx.x; j < E; j += blockDim.x) dst[j] = ln[(size_t)t * E + j];
+    const uint32_t d = pass->desc[t], e = pass->snap[t];
+    if (d & kDescLast) {
+        double *dst = state + desc_slot(d) * slot_stride;
+        for (int j = threadIdx.x; j < E; j += blockDim.x) dst[j] = ln[(size_t)t * E + j];
+    }
+    if (e) {
+        double *dst = pass->pool[which] + (size_t)(e - 1) * slot_stride + lo;
+        for (int j = threadIdx.x; j < E; j += blockDim.x) dst[j] = ln[(size_t)t * E + j];
+    }
 }
 
 // ---- adapter deltas: delta[t][m] = s * sum_i B[m][i] * h[t][i],  h[t][i] = sum_j A[i][j] * f[t][j], both in f64 ----
@@ -745,7 +769,7 @@ inline int prefill_chunk_body(PrefillState &s, const Params &p, cudaStream_t st,
         m.limbs = s.limbs; m.scale = s.scale; m.offs = s.offs;
         m.fout = ad ? s.ad_f : nullptr;
         k_pf_mix_quant<<<gT, 256, 0, st>>>(m);
-        k_pf_store_state<<<gT, 256, 0, st>>>(s.ln, E, s.pass->desc, LE, p.sxy + lo);
+        k_pf_store_state<<<gT, 256, 0, st>>>(s.ln, E, s.pass, LE, p.sxy + lo, kPoolXY, lo);
         const size_t mo = (size_t)l * E * E;
         if ((rc = pf_gemm(s, st, p.wk + mo, E, E, s.limbs, (size_t)9 * Tp, 0 * Tp, Tp, Ca))) return rc;
         if ((rc = pf_gemm(s, st, p.wv + mo, E, E, s.limbs, (size_t)9 * Tp, 3 * Tp, Tp, Cb))) return rc;
@@ -760,6 +784,7 @@ inline int prefill_chunk_body(PrefillState &s, const Params &p, cudaStream_t st,
         w.desc = s.pass->desc;
         w.E = E; w.T = T; w.Tp = Tp;
         w.rw = s.rw; w.xs = s.xs;
+        w.pass = s.pass; w.lo = lo;
         const size_t TE = (size_t)T * E;
         if (ad) {
             pf_adapt(s, p, st, T, l, 3, {kAdAttK, kAdAttV, kAdAttR}, E, {E, E, E}, s.ad_f, (size_t)Tp * E);
@@ -784,7 +809,7 @@ inline int prefill_chunk_body(PrefillState &s, const Params &p, cudaStream_t st,
         f.limbs = s.limbs; f.scale = s.scale; f.offs = s.offs;
         f.fout = ad ? s.ad_f : nullptr;
         k_pf_mix_quant<<<gT, 256, 0, st>>>(f);
-        k_pf_store_state<<<gT, 256, 0, st>>>(s.ln, E, s.pass->desc, LE, p.sdd + lo);
+        k_pf_store_state<<<gT, 256, 0, st>>>(s.ln, E, s.pass, LE, p.sdd + lo, kPoolDD, lo);
         int *Ck4 = s.C + (size_t)E * 3 * Tp; // [4E][3Tp] behind the ffn-R accumulators
         if ((rc = pf_gemm(s, st, p.wfr + mo, E, E, s.limbs, (size_t)6 * Tp, 0 * Tp, Tp, Ca))) return rc;
         if ((rc = pf_gemm(s, st, p.wfk + 4 * mo, 4 * E, E, s.limbs, (size_t)6 * Tp, 3 * Tp, Tp, Ck4))) return rc;
@@ -912,21 +937,27 @@ inline void pass_layout(const unsigned long long *tokens, int n, const unsigned 
     }
 }
 
-// A ragged forward (the layout and `head` of pass_layout): per pass, upload its layout, then run it. `logits` is a
-// device buffer of at least n (head 1) / one per stream (head 2) rows.
-inline int prefill_forward(PrefillState &s, const Params &p, cudaStream_t st, const unsigned long long *tokens, int n,
-                           const unsigned long long *slots, const unsigned long long *lens, int head, float *logits,
-                           const unsigned char *need = nullptr) {
+// The passes of a layout of n tokens (pass_layout's, possibly with snapshots added): per pass, upload it, then run it.
+inline int prefill_passes(PrefillState &s, const Params &p, cudaStream_t st, const std::vector<PassDesc> &passes,
+                          const std::vector<int> &heads, int n, float *logits) {
     int rc = prefill_init(s, p);
     if (rc) return rc;
-    std::vector<PassDesc> passes;
-    std::vector<int> heads;
-    pass_layout(tokens, n, slots, lens, head, need, passes, heads);
     for (size_t i = 0; i < passes.size(); ++i) {
         PF_CK(cudaMemcpyAsync(s.pass, &passes[i], sizeof(PassDesc), cudaMemcpyHostToDevice, st));
         if ((rc = prefill_run(s, p, st, std::min(kPfMaxTokens, n - (int)i * kPfMaxTokens), heads[i], logits))) return rc;
     }
     return 0;
+}
+
+// A ragged forward (the layout and `head` of pass_layout): per pass, upload its layout, then run it. `logits` is a
+// device buffer of at least n (head 1) / one per stream (head 2) rows.
+inline int prefill_forward(PrefillState &s, const Params &p, cudaStream_t st, const unsigned long long *tokens, int n,
+                           const unsigned long long *slots, const unsigned long long *lens, int head, float *logits,
+                           const unsigned char *need = nullptr) {
+    std::vector<PassDesc> passes;
+    std::vector<int> heads;
+    pass_layout(tokens, n, slots, lens, head, need, passes, heads);
+    return prefill_passes(s, p, st, passes, heads, n, logits);
 }
 
 } // namespace rk

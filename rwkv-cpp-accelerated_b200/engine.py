@@ -73,6 +73,12 @@ class StopRequest(ctypes.Structure):
     _fields_ = [("set_ids", P), ("start_states", P), ("states_out", P), ("hit_out", P), ("tail_out", P)]
 
 
+class PrefixStats(ctypes.Structure):
+    """struct rwkv_b200_prefix_stats (include/rwkv_b200.h)."""
+    _fields_ = [(f, ctypes.c_ulonglong) for f in ("live", "lookups", "hit_tokens", "prefilled_tokens", "snapshots", "skipped",
+                                                  "evictions")]
+
+
 class Adapter(ctypes.Structure):
     """rwkv_b200_adapter: the rank, the scale and per projection the A and B arrays (NULL: not adapted)."""
     PF = ctypes.POINTER(ctypes.c_float)
@@ -436,6 +442,16 @@ def load_library():
         "rwkv_b200_adapter_add": (i32, [vp, c.POINTER(Adapter), pull]),
         "rwkv_b200_adapter_remove": (i32, [vp, ull]),
         "rwkv_b200_slot_adapter": (i32, [vp, ull, ull]),
+        "rwkv_b200_prefix_cache_open": (i32, [vp, ull, ull, c.POINTER(vp)]),
+        "rwkv_b200_prefix_cache_close": (i32, [vp]),
+        "rwkv_b200_prefix_forward": (i32, [vp, pull, ull, pull, pull, ull, pflt, pull, pull]),
+        "rwkv_b200_prefix_insert": (i32, [vp, ull, pull, ull]),
+        "rwkv_b200_prefix_download": (i32, [vp, pull, ull, pdbl, pdbl, pdbl, pdbl]),
+        "rwkv_b200_prefix_clear": (i32, [vp]),
+        "rwkv_b200_batcher_submit_prefix": (i32, [vp, c.POINTER(Request), c.POINTER(RequestEx), ull, ull,
+                                                  c.POINTER(RequestSpec), vp, pull]),
+        "rwkv_b200_batcher_read_prefix": (i32, [vp, ull, pull]),
+        "rwkv_b200_prefix_stats": (i32, [vp, c.POINTER(PrefixStats)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)  # AttributeError if a declared symbol is missing
@@ -864,6 +880,11 @@ class Engine:
         requests and `prefill_tokens` prompt tokens per step."""
         return Batcher(self, rows, prefill_tokens)
 
+    def prefix_cache(self, capacity, block=64):
+        """A PrefixCache of `capacity` entries that snapshots every `block` tokens (include/rwkv_b200.h, "Prefix state
+        cache")."""
+        return PrefixCache(self, capacity, block)
+
     def slot_zero(self, slot):
         self._ck(self.lib.rwkv_b200_slot_zero(self.h, slot), "slot_zero")
 
@@ -1012,9 +1033,10 @@ class Batcher:
         self._ext = {}  # id -> (top_n or None without log-probabilities, constrained) of requests sent through submit_ex
         self._stop = set()  # ids of requests with a stop set
         self._spec = set()  # ids of requests with speculation
+        self._prefix = set()  # ids of requests with a prefix cache
 
     def submit(self, slot, prompt, max_new, sampling=None, u=None, stop=(), overrides=None, constraint=None, logprobs=None,
-               top_n=0, stop_strings=None, draft=0, spare_slots=(), ngram=3, context=None):
+               top_n=0, stop_strings=None, draft=0, spare_slots=(), ngram=3, context=None, prefix_cache=None):
         """Queue a request on state slot `slot`: prompt (>= 1 token ids), up to max_new new tokens, a Sampler or dict
         (None: arg-max), u: max_new uniforms in [0, 1) (None only at temperature 0), stop: this request's stop tokens.
         overrides = {token: logit value} as in generate_streams; constraint: an id of Engine.add_constraint, or (id,
@@ -1022,7 +1044,9 @@ class Batcher:
         result); stop_strings: an id of Engine.add_stop_set, or (id, start_state). draft > 0 speculates with
         prompt-lookup drafts (rwkv_b200_batcher_submit_spec): spare_slots are its draft scratch slots, ngram the longest
         n-gram looked up and context extra lookup tokens before the prompt; the tokens are those without speculation and
-        result adds "steps". Returns its id. Every array is copied."""
+        result adds "steps". prefix_cache: a PrefixCache of the engine (rwkv_b200_batcher_submit_prefix): the request
+        starts from the zero state, restores its longest cached prompt prefix at admission and snapshots its prefill;
+        result adds "cached". Returns its id. Every array is copied."""
         if int(draft) < 0:
             raise EngineError("batcher.submit: draft %d < 0" % int(draft))
         spares = np.ascontiguousarray([int(z) for z in spare_slots], dtype=np.uint64)
@@ -1060,8 +1084,12 @@ class Batcher:
         rid = ctypes.c_ulonglong()
         xr = ctypes.byref(x) if x is not None else None
         # the entry point of what the request uses: each one is exactly the next one's call with its extension NULL
-        if draft:
-            spec = RequestSpec(_ptr(spares, P), int(draft), int(ngram), _ptr(ctx, P) if len(ctx) else None, len(ctx))
+        spec = RequestSpec(_ptr(spares, P), int(draft), int(ngram), _ptr(ctx, P) if len(ctx) else None, len(ctx))
+        if prefix_cache is not None:
+            rc = self.lib.rwkv_b200_batcher_submit_prefix(self.h, ctypes.byref(req), xr, sid, s0,
+                                                          ctypes.byref(spec) if draft else None,
+                                                          prefix_cache._handle("batcher.submit"), ctypes.byref(rid))
+        elif draft:
             rc = self.lib.rwkv_b200_batcher_submit_spec(self.h, ctypes.byref(req), xr, sid, s0, ctypes.byref(spec),
                                                         ctypes.byref(rid))
         elif stop_strings is not None:
@@ -1078,6 +1106,8 @@ class Batcher:
             self._ext[rid] = (int(top_n) if logprobs is not None else None, constraint is not None)
         if draft:
             self._spec.add(rid)
+        if prefix_cache is not None:
+            self._prefix.add(rid)
         return rid
 
     def run(self, max_steps):
@@ -1134,6 +1164,11 @@ class Batcher:
             steps = ctypes.c_ulonglong()
             self.engine._ck(self.lib.rwkv_b200_batcher_read_spec(self.h, int(rid), ctypes.byref(steps)), "batcher_read_spec")
             d["steps"] = int(steps.value)
+        if int(rid) in self._prefix:
+            cached = ctypes.c_ulonglong()
+            self.engine._ck(self.lib.rwkv_b200_batcher_read_prefix(self.h, int(rid), ctypes.byref(cached)),
+                            "batcher_read_prefix")
+            d["cached"] = int(cached.value)
         return d
 
     def cancel(self, rid):
@@ -1234,6 +1269,89 @@ class StateIndex:
     def close(self):
         if self.h is not None and getattr(self.engine, "h", None):
             self.lib.rwkv_b200_index_free(self.engine.h, self.h)
+        self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+PREFIX_NOT_CACHED = 2  # RWKV_B200_PREFIX_NOT_CACHED
+
+
+class PrefixCache:
+    """Recurrent states after token prefixes, kept on the device (include/rwkv_b200.h, "Prefix state cache"): a stream
+    run through forward() starts from the zero state, restores its longest cached prefix and stores snapshots of the
+    rest. A context manager; close() frees the cache."""
+
+    def __init__(self, engine, capacity, block=64):
+        self.engine, self.lib = engine, engine.lib
+        self.h = None
+        h = ctypes.c_void_p()
+        engine._ck(self.lib.rwkv_b200_prefix_cache_open(engine.h, int(capacity), int(block), ctypes.byref(h)),
+                   "prefix_cache_open")
+        self.h = h
+
+    @staticmethod
+    def _tokens(tokens):
+        return np.ascontiguousarray(np.atleast_1d(np.asarray(tokens, dtype=np.uint64)))
+
+    def _handle(self, what):
+        if self.h is None or not getattr(self.engine, "h", None):
+            raise EngineError("%s: the prefix cache is closed" % what)
+        return self.h
+
+    def forward(self, streams, want_logits=True, want_next=False):
+        """forward_streams from the zero state with cached prefixes: streams = [(slot, tokens), ...]. Returns (logits
+        [S][V] | None, arg-max [S] | None, cached [S]: the tokens each stream restored)."""
+        h = self._handle("prefix_forward")
+        slots = np.ascontiguousarray([int(s) for s, _ in streams], dtype=np.uint64)
+        seqs = [self._tokens(t) for _, t in streams]
+        lens = np.ascontiguousarray([len(t) for t in seqs], dtype=np.uint64)
+        toks = np.ascontiguousarray(np.concatenate(seqs) if seqs else np.zeros(0, np.uint64))
+        logits = np.empty((len(seqs), VOCAB), np.float32) if want_logits else None
+        nxt = np.empty(len(seqs), np.uint64) if want_next else None
+        cached = np.zeros(len(seqs), np.uint64)
+        P = ctypes.c_ulonglong
+        self.engine._ck(self.lib.rwkv_b200_prefix_forward(h, _ptr(toks, P), len(toks), _ptr(slots, P), _ptr(lens, P),
+                                                          len(seqs), _ptr(logits, ctypes.c_float), _ptr(nxt, P),
+                                                          _ptr(cached, P)), "prefix_forward")
+        return logits, nxt, cached
+
+    def insert(self, slot, tokens):
+        """Store slot's state as the state after `tokens` (a zeroed slot fed exactly those tokens)."""
+        h = self._handle("prefix_insert")
+        t = self._tokens(tokens)
+        self.engine._ck(self.lib.rwkv_b200_prefix_insert(h, int(slot), _ptr(t, ctypes.c_ulonglong), len(t)),
+                        "prefix_insert")
+
+    def download(self, tokens):
+        """The state of the unbound entry keyed exactly by `tokens`: a dict of xy, aa, bb, dd, or None."""
+        h = self._handle("prefix_download")
+        t = self._tokens(tokens)
+        n = self.engine.n_layers * self.engine.n_embed
+        arrs = [np.empty(n, np.float64) for _ in range(4)]
+        rc = self.lib.rwkv_b200_prefix_download(h, _ptr(t, ctypes.c_ulonglong), len(t),
+                                                *[_ptr(a, ctypes.c_double) for a in arrs])
+        if rc == PREFIX_NOT_CACHED:
+            return None
+        self.engine._ck(rc, "prefix_download")
+        return dict(zip(("xy", "aa", "bb", "dd"), arrs))
+
+    def stats(self):
+        h, st = self._handle("prefix_stats"), PrefixStats()
+        self.engine._ck(self.lib.rwkv_b200_prefix_stats(h, ctypes.byref(st)), "prefix_stats")
+        return {f: int(getattr(st, f)) for f, _ in PrefixStats._fields_}
+
+    def clear(self):
+        h = self._handle("prefix_clear")
+        self.engine._ck(self.lib.rwkv_b200_prefix_clear(h), "prefix_clear")
+
+    def close(self):
+        if self.h is not None and getattr(self.engine, "h", None):
+            self.engine._ck(self.lib.rwkv_b200_prefix_cache_close(self.h), "prefix_cache_close")
         self.h = None
 
     def __enter__(self):
