@@ -95,6 +95,39 @@ template <class T> struct DevBuf {
 
 const char *kKernelNames[1] = {"token"};
 
+// The device buffers of a decode group (step_args, run_step): the model keeps one set for the one-shot generation calls
+// and the batcher its own, so a call between runs leaves the batcher's requests alone. Each grows with its largest
+// user; what a buffer holds is counted in streams (the one-shot calls) or lanes (the batcher).
+struct StepBuffers {
+    DevBuf<rk::GenStream> gs;          // stream records (the model's are sized at load)
+    DevBuf<int> row_stream;            // [rows] the stream of each logits row (the model's are sized at load)
+    DevBuf<rk::PassDesc> passes;       // the steps' passes (the model's: [ceil(max_gpt / 128)], zeroed at load)
+    DevBuf<double> u;                  // [steps][rows] each row's uniform of a group's steps
+    DevBuf<rwkv_b200_sampler> samp;    // [streams] each stream's sampler
+    DevBuf<float> pen_cnt;             // [streams][V] decayed counts of the emitted tokens (penalties only)
+    DevBuf<unsigned char> pen_seen;    // [streams][V] emitted in this call or request
+    DevBuf<unsigned long long> out;    // [streams][max_new] emitted tokens (the batcher's: a ring per lane)
+    // stop tokens and overrides: the call's lists, or each lane's by its CSR start ([lanes + 1]; the batcher only)
+    DevBuf<unsigned long long> stop, stop_start, ovr_tok, ovr_start;
+    DevBuf<float> ovr_val;
+    DevBuf<rk::GenConstraint> gc;      // [streams] token automata
+    DevBuf<unsigned long long> fault;  // [3] k_gen_feedback's and k_spec_accept's record of a token without an edge
+    DevBuf<rk::GenStop> gst;           // [streams] stop sets
+    // log-probabilities: the results of each emitted token, each lane's scoring (the batcher only), and the model's rows
+    // of a step (raw mode with penalties, overrides or automata, which edit d_slogits in place)
+    DevBuf<double> lp, top_lp;         // [streams][max_new], [..][top]
+    DevBuf<unsigned long long> rank, top_tok;
+    DevBuf<rk::LogprobLane> lp_lane;   // [lanes]
+    DevBuf<float> raw;                 // [rows][V]
+    // speculative streams: records, the live list, what k_spec_logprob scores ([rows]), histories, each row's automaton
+    // state ([rows]), the copies home -> first slot ([streams][2]) and the streams' uniforms (SpecArgs::u)
+    DevBuf<rk::SpecStream> ss;
+    DevBuf<rk::SpecLive> live;
+    DevBuf<rk::SpecScore> score;
+    DevBuf<unsigned long long> hist, row_state, forks;
+    DevBuf<double> su;
+};
+
 } // namespace
 
 struct rwkv_b200_model {
@@ -125,29 +158,14 @@ struct rwkv_b200_model {
     unsigned int epoch = 0, tk = 0; // exchange epochs (token_kernel.cuh); identical on every rank
     int tp_rank = 0, tp_size = 1;
     rk::PrefillState pf{};
-    // generate_streams: per-stream records (device, and their pinned host mirror), the row map and the pass
-    // descriptors are sized at load; the rest grows with the largest call and is freed with the model
-    struct Gen {
-        rk::GenStream *gs = nullptr, *h_gs = nullptr; // [max_gpt]
-        int *row_stream = nullptr;                     // [max_gpt] stream of each row of the current group
-        rk::PassDesc *passes = nullptr;                // [ceil(max_gpt / 128)] next step's passes (tensor cores)
-        DevBuf<unsigned long long> out;                // [n_streams][max_new] emitted tokens
-        DevBuf<unsigned long long> stop, ovr_tok;
-        DevBuf<float> ovr_val;
-        DevBuf<double> u;               // [group steps][rows] uniforms of the current group
-        DevBuf<rwkv_b200_sampler> samp; // [n_streams] sampler of each stream (generate_streams_ex, sample_streams)
-        DevBuf<float> pen_cnt;          // [n_streams][V] decayed counts of the emitted tokens (penalties only)
-        DevBuf<unsigned char> pen_seen; // [n_streams][V] emitted in this call
-        // generate_streams_logprobs: the results of each emitted token, and the model's rows of the step (raw mode with
-        // penalties or overrides, which edit d_slogits in place)
-        DevBuf<double> lp, top_lp;                 // [n_streams][max_new], [..][top_n]
-        DevBuf<unsigned long long> rank, top_tok;  // [n_streams][max_new], [..][top_n]
-        DevBuf<float> raw;                         // [rows][V]
-        // generate_streams_constrained: each stream's automaton and state, and the record of a token without an edge
-        DevBuf<rk::GenConstraint> gc;      // [n_streams]
-        DevBuf<unsigned long long> fault;  // [3]
-        DevBuf<rk::GenStop> gst;           // [n_streams] generate_streams_stop and the speculative call: stop sets
-    } gen;
+    // the one-shot generation calls (generate_streams*, generate_streams_speculative*, beam_search) and sample_streams:
+    // the stream records (device, and their pinned host mirror [max_gpt]), the row map and the passes are sized at
+    // load; the rest grows with the largest call and is freed with the model
+    StepBuffers gen;
+    rk::GenStream *h_gs = nullptr;
+    // the speculative call's passes, sized by its own rule (streams of k + 1 rows never straddle a pass), so apart from
+    // gen.passes, which must stay zeroed from load
+    DevBuf<rk::PassDesc> spec_passes;
     // stop strings: the token bytes (rwkv_b200_token_bytes_set) and per set id its automaton (rwkv_b200_stop_set_add):
     // next [states][256] then hit [states] in one device block
     DevBuf<unsigned long long> tb_start; // [V + 1]
@@ -186,19 +204,6 @@ struct rwkv_b200_model {
         DevBuf<int> n_hyp;                      // [G]
         DevBuf<unsigned long long> done, forks; // [G], [G * B][2]
     } beam;
-    // generate_streams_speculative: the streams' records, histories, live list, passes, per-row uniforms and automaton
-    // states, grown with the largest call; the emitted tokens, stops, overrides, samplers, automata, log-probabilities
-    // and the raw copy use gen's buffers
-    struct Spec {
-        DevBuf<rk::SpecStream> ss;        // [n_streams]
-        DevBuf<unsigned long long> hist;  // per stream: context, first token, up to max_new emitted tokens
-        DevBuf<rk::SpecLive> live;       // [live streams]
-        DevBuf<rk::PassDesc> passes;      // [passes of a step]
-        DevBuf<double> u, row_u;          // [max_new][n_streams], [rows]
-        DevBuf<unsigned long long> forks; // [n_streams][2] the final copies home -> first slot
-        DevBuf<rk::SpecScore> score;      // [rows] what k_spec_logprob scores (with log-probabilities)
-        DevBuf<unsigned long long> row_state; // [rows] each row's automaton state (constrained calls)
-    } spec;
     rwkv_b200_batcher *batcher = nullptr; // the open batcher (at most one), closed by rwkv_b200_free
     // rwkv_b200_index_create: per id the rows [capacity][D] and live flags on the device, the flags and counts on the host
     struct Index {
@@ -241,8 +246,7 @@ struct rwkv_b200_prefix_cache {
 
 // rwkv_b200_batcher: the requests on the host, and per lane (0..rows-1, one per admitted request, reused) its stream
 // record, sampler, penalty rows, stop tokens, overrides, automaton, log-probability choice and a ring of the current
-// group's tokens (and their log-probabilities) on the device. Nothing is shared with m->gen, so a generate_streams call
-// between runs leaves the batcher's requests alone.
+// group's tokens (and their log-probabilities) on the device, in its own StepBuffers.
 struct rwkv_b200_batcher {
     rwkv_b200_model *m = nullptr;
     int rows = 0, prefill_tokens = 0, max_pass = 0; // max_pass: passes of a step at most
@@ -281,41 +285,20 @@ struct rwkv_b200_batcher {
     std::deque<unsigned long long> queue;     // queued ids, submission order
     std::vector<unsigned long long> admitted; // admitted ids, admission order
     std::vector<char> lane_used;              // [rows]
-    std::vector<rk::GenStream> h_gs;          // [rows] host mirror of the lanes' records
-    std::vector<unsigned long long> h_out;    // [rows][kGenGroup]
-    DevBuf<rk::GenStream> gs;                 // [rows]
-    DevBuf<int> row_stream;                   // [rows] lane of each decode row
-    DevBuf<rk::PassDesc> passes;              // [kGenGroup][max_pass] the layouts of a group's steps
-    DevBuf<rwkv_b200_sampler> samp;           // [rows]
-    DevBuf<float> pen_cnt;                    // [rows][V] (allocated at the first request with penalties)
-    DevBuf<unsigned char> pen_seen;           // [rows][V]
-    DevBuf<unsigned long long> stop, stop_start, out; // lanes' stop tokens (CSR), [rows + 1], [rows][kGenGroup]
-    DevBuf<double> u;                         // [kGenGroup][rows] uniforms of the current group
-    // the features of submit_ex, each grown at the first group whose decode lanes use it
-    DevBuf<unsigned long long> ovr_tok, ovr_start; // decode lanes' overrides (CSR), [rows + 1]
-    DevBuf<float> ovr_val;
-    unsigned long long n_ovr = 0;             // the overrides of the current group's decode lanes
-    std::vector<rk::GenConstraint> h_gc;      // [rows] host mirror of the lanes' automata (mask nullptr: none)
-    DevBuf<rk::GenConstraint> gc;             // [rows]
-    DevBuf<unsigned long long> fault;         // [3] k_gen_feedback's record of a token without an edge
-    std::vector<rk::LogprobLane> h_lp;        // [rows] each lane's scoring (mode < 0: none)
-    DevBuf<rk::LogprobLane> lp_lane;          // [rows]
-    DevBuf<double> lp, top_lp;                // rings [rows][kGenGroup], [rows][kGenGroup][kMaxTopN]
-    DevBuf<unsigned long long> rank, top_tok; // [rows][kGenGroup], [rows][kGenGroup][kMaxTopN]
-    std::vector<double> h_lpv, h_top_lp;      // host copies of the rings
-    std::vector<unsigned long long> h_rank, h_top_tok;
-    DevBuf<float> raw;                        // [rows][V] the model's rows of a step, for raw lanes (see batcher_group)
-    std::vector<rk::GenStop> h_gst;           // [rows] host mirror of the lanes' stop sets (next nullptr: none)
-    DevBuf<rk::GenStop> gst;                  // [rows]
-    // speculative lanes (submit_spec), grown at the first group that has one: the lanes' records, where each lane's
-    // rows lie, the histories and uniforms of the group's speculative lanes, each row's automaton state, and the
-    // copies home -> slot of finished or cancelled requests
-    std::vector<rk::SpecStream> h_ss;         // [rows]
-    DevBuf<rk::SpecStream> ss;                // [rows]
-    DevBuf<rk::SpecLive> spec_live;           // [speculative lanes]
-    DevBuf<rk::SpecScore> score;              // [speculative lanes][largest k + 1] (scored lanes only)
-    DevBuf<unsigned long long> hist, row_state, forks;
-    DevBuf<double> su;
+    // the lanes' device buffers: records, row map, samplers, stop tokens (CSR), the passes of a group's steps
+    // ([kGenGroup][max_pass]) and its uniforms are sized at open; pen_cnt and pen_seen grow at the first request with
+    // penalties; the overrides, automata, stop sets, scoring and speculative buffers at the first group whose decode
+    // lanes use them
+    StepBuffers bufs;
+    // host mirrors, [rows] each: the lanes' records, automata (mask nullptr: none), scoring (mode < 0: none), stop sets
+    // (next nullptr: none) and speculative records, and the group's rings of tokens and their results
+    std::vector<rk::GenStream> h_gs;
+    std::vector<rk::GenConstraint> h_gc;
+    std::vector<rk::LogprobLane> h_lp;
+    std::vector<rk::GenStop> h_gst;
+    std::vector<rk::SpecStream> h_ss;
+    std::vector<unsigned long long> h_out, h_rank, h_top_tok;
+    std::vector<double> h_lpv, h_top_lp;
 };
 
 namespace {
@@ -729,14 +712,14 @@ int do_load(M *m, const char *path, int quiet) {
     if ((rc = dmalloc(m, &m->d_slogits, (size_t)V * m->max_gpt)) || (rc = dmalloc(m, &m->d_next, m->max_gpt)) ||
         (rc = dmalloc(m, &m->d_sample, 2 * m->max_gpt)) || (rc = dmalloc(m, &m->d_u, m->max_gpt)))
         return rc;
-    if ((rc = dmalloc(m, &m->gen.gs, m->max_gpt)) || (rc = dmalloc(m, &m->gen.row_stream, m->max_gpt)) ||
-        (rc = dmalloc(m, &m->gen.passes, (m->max_gpt + rk::kPfMaxTokens - 1) / rk::kPfMaxTokens)))
+    const size_t n_pass = (m->max_gpt + rk::kPfMaxTokens - 1) / rk::kPfMaxTokens;
+    if ((rc = m->gen.gs.grow(m->max_gpt)) || (rc = m->gen.row_stream.grow(m->max_gpt)) || (rc = m->gen.passes.grow(n_pass)))
         return rc;
     // every pass of the generation calls starts zeroed: an upload fills the first step's passes, and k_beam_select and
     // k_gen_feedback then fill tokens, descriptors and row maps of passes no upload reached, so no snapshot field there
     // may hold leftover bytes
-    CK(cudaMemsetAsync(m->gen.passes, 0, (m->max_gpt + rk::kPfMaxTokens - 1) / rk::kPfMaxTokens * sizeof(rk::PassDesc), m->stream));
-    CK(cudaMallocHost((void **)&m->gen.h_gs, sizeof(rk::GenStream) * m->max_gpt));
+    CK(cudaMemsetAsync(m->gen.passes.p, 0, n_pass * sizeof(rk::PassDesc), m->stream));
+    CK(cudaMallocHost((void **)&m->h_gs, sizeof(rk::GenStream) * m->max_gpt));
     CK(cudaHostAlloc((void **)&m->h_diag, sizeof(rk::Diag), cudaHostAllocMapped));
     memset(m->h_diag, 0, sizeof(rk::Diag));
     CK(cudaHostGetDevicePointer((void **)&p.diag, m->h_diag, 0));
@@ -904,7 +887,7 @@ constexpr float kMaxPenalty = 1e6f;
 int gen_step_decode(M *m, int rows, const int *row_stream) {
     const size_t V = binfmt::kVocab;
     for (int r = 0; r < rows; ++r) {
-        rk::k_gen_gate<<<1, 1, 0, m->stream>>>(m->gen.gs, row_stream, r, m->max_gpt, m->p.ctrl);
+        rk::k_gen_gate<<<1, 1, 0, m->stream>>>(m->gen.gs.p, row_stream, r, m->max_gpt, m->p.ctrl);
         LAUNCHED(m);
         int rc = launch_token(m, 0, false, nullptr, m->stream);
         if (rc) return rc;
@@ -933,13 +916,13 @@ int gen_step_passes(M *m, const rk::PassDesc *passes, int rows, int per_pass, co
 int upload_step_passes(M *m, const int *rec, int rows) {
     std::vector<unsigned long long> tokens(rows), slots(rows), lens(rows, 1);
     for (int r = 0; r < rows; ++r) {
-        tokens[r] = m->gen.h_gs[rec[r]].tok;
-        slots[r] = m->gen.h_gs[rec[r]].slot;
+        tokens[r] = m->h_gs[rec[r]].tok;
+        slots[r] = m->h_gs[rec[r]].slot;
     }
     std::vector<rk::PassDesc> passes;
     std::vector<int> heads;
     rk::pass_layout(tokens.data(), rows, slots.data(), lens.data(), 2, nullptr, passes, heads);
-    CK(cudaMemcpyAsync(m->gen.passes, passes.data(), passes.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemcpyAsync(m->gen.passes.p, passes.data(), passes.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
     return 0;
 }
 
@@ -1216,18 +1199,34 @@ int check_logprobs(const char *what, const LogprobRequest &lpq) {
     return 0;
 }
 
+// What the steps of a call or of a batcher group enqueue besides the forward, and how their kernels read their inputs:
+// derived from the call (check_features) or from the group's decode lanes (batcher_upload).
+struct StepFlags {
+    // samplers: every stream picks by its own sampler; uniforms: the rows draw uniforms (the typical sampler's, or the
+    // samplers'); neither: the arg-max
+    bool samplers = false, uniforms = false;
+    // pen: some stream has a presence or frequency penalty; n_override: the overrides of the rows
+    bool pen = false, constrained = false, stopped = false;
+    unsigned long long n_override = 0;
+    // scored, spec_scored: the one-token rows, the speculative rows are scored; raw: the scoring reads the model's rows
+    // (the call's mode, or some batcher lane's); raw_copy (set_raw_copy): from a copy taken before the penalties,
+    // overrides and masks edit d_slogits; top: the stride of the top arrays
+    bool scored = false, spec_scored = false, raw = false, raw_copy = false;
+    int top = 0;
+};
+
+// Raw log-probabilities read a copy of the model's rows when the pick chain edits d_slogits.
+void set_raw_copy(StepFlags &f) { f.raw_copy = f.raw && (f.pen || f.n_override || f.constrained); }
+
 // What a one-shot decoding call (generate() and speculate()) does besides emitting tokens: score them (lpq), follow
 // token automata (cq) and stop sets (sq), and count penalties; each request is NULL when the call has none. Built by
 // check_features, its buffers in m->gen readied by upload_features and its results written by finish_features.
-struct CallFeatures {
+struct CallFeatures : StepFlags {
     const LogprobRequest *lpq = nullptr;
     const ConstraintRequest *cq = nullptr;
     const rwkv_b200_stop_request *sq = nullptr;
     std::vector<rk::GenConstraint> gc; // each stream's automaton (a zero record: none)
     std::vector<rk::GenStop> st;       // each stream's stop set (a zero record: none)
-    // pen: some stream has a presence or frequency penalty; raw_copy: raw log-probabilities read a copy of the model's
-    // rows taken before the penalties, overrides and masks edit d_slogits
-    bool pen = false, constrained = false, stopped = false, raw_copy = false;
     size_t n_lp = 0, n_top = 0; // entries of the log-probability and top arrays
 };
 
@@ -1239,6 +1238,9 @@ int check_features(M *m, const char *what, const GenCall &c, const LogprobReques
     f.lpq = lpq;
     f.cq = cq;
     f.sq = sq;
+    f.samplers = c.samplers != nullptr;
+    f.uniforms = c.u != nullptr;
+    f.n_override = c.n_override;
     for (unsigned long long s = 0; c.samplers && s < n; ++s)
         f.pen |= c.samplers[s].presence_penalty != 0.0f || c.samplers[s].frequency_penalty != 0.0f;
     int rc;
@@ -1246,7 +1248,10 @@ int check_features(M *m, const char *what, const GenCall &c, const LogprobReques
     f.constrained = std::any_of(f.gc.begin(), f.gc.end(), [](const rk::GenConstraint &gc) { return gc.mask != nullptr; });
     if ((rc = check_stops(m, what, sq, n, f.st))) return rc;
     f.stopped = std::any_of(f.st.begin(), f.st.end(), [](const rk::GenStop &st) { return st.next != nullptr; });
-    f.raw_copy = lpq && lpq->mode == RWKV_B200_LOGPROBS_RAW && (f.pen || c.n_override || f.constrained);
+    f.scored = f.spec_scored = lpq != nullptr;
+    f.raw = lpq && lpq->mode == RWKV_B200_LOGPROBS_RAW;
+    set_raw_copy(f);
+    f.top = lpq ? (int)lpq->top_n : 0;
     f.n_lp = (size_t)(n * c.max_new);
     f.n_top = lpq ? f.n_lp * lpq->top_n : 0;
     return 0;
@@ -1283,50 +1288,120 @@ int upload_features(M *m, const CallFeatures &f, unsigned long long n_streams, s
     return 0;
 }
 
-// The arguments every step of the call shares, over the buffers upload_features readied: the pick chain, the emit
-// rule and the scoring (all zero without scoring). The caller adds what its own steps need.
-void step_args(M *m, const CallFeatures &f, const GenCall &c, PickChain &pc, rk::GenEmit &e, rk::GenLogprobArgs &la) {
-    auto &g = m->gen;
-    pc = PickChain{};
-    pc.gs = g.gs;
-    pc.row_stream = g.row_stream;
-    pc.samp = c.samplers ? g.samp.p : nullptr;
-    pc.pen_cnt = f.pen ? g.pen_cnt.p : nullptr;
-    pc.pen_seen = g.pen_seen.p;
-    pc.ovr_tok = g.ovr_tok.p;
-    pc.ovr_val = g.ovr_val.p;
-    pc.n_override = c.n_override;
-    pc.gc = f.constrained ? g.gc.p : nullptr;
-    e = rk::GenEmit{};
-    e.out = g.out.p;
-    e.max_new = c.max_new;
-    e.stop = g.stop.p;
-    e.n_stop = (int)c.n_stop;
-    e.gc = f.constrained ? g.gc.p : nullptr;
-    e.fault = g.fault.p;
-    e.gst = f.stopped ? g.gst.p : nullptr;
-    la = rk::GenLogprobArgs{};
-    if (!f.lpq) return;
-    la.logits = f.raw_copy ? g.raw.p : m->d_slogits;
+// The arguments of a step's kernels; `raw` is where the step copies its model rows (nullptr: no copy).
+struct StepArgs {
+    PickChain pc;
+    rk::GenLogprobArgs la;
+    rk::SpecArgs sa;
+    rk::GenFeedbackArgs fb;
+    float *raw;
+};
+
+// The arguments every step of a call or batcher group shares, over the buffers of `sb` as its upload readied them:
+// each stream's tokens (and results) at [s][len % max_new], and n_stop stop tokens for every stream. Buffers only the
+// batcher grows give each lane its own overrides (ovr_start), stop tokens (stop_start) and scoring (lp_lane: raw lanes
+// read the copy, the others d_slogits with their sampler). The caller adds the shape of its steps: the one-token rows,
+// the speculative k and uniform stride, the passes and the uniforms.
+void step_args(M *m, StepBuffers &sb, const StepFlags &f, unsigned long long max_new, unsigned long long n_stop, StepArgs &a) {
+    a = StepArgs{};
+    const unsigned long long *next = f.samplers || f.uniforms ? nullptr : m->d_next;
+    PickChain &pc = a.pc;
+    pc.gs = sb.gs.p;
+    pc.row_stream = sb.row_stream.p;
+    pc.samp = f.samplers ? sb.samp.p : nullptr;
+    pc.pen_cnt = f.pen ? sb.pen_cnt.p : nullptr;
+    pc.pen_seen = sb.pen_seen.p;
+    pc.ovr_tok = sb.ovr_tok.p;
+    pc.ovr_val = sb.ovr_val.p;
+    pc.n_override = f.n_override;
+    pc.gc = f.constrained ? sb.gc.p : nullptr;
+    pc.ovr_start = sb.ovr_start.p;
+    rk::GenEmit &e = a.fb.emit;
+    e.out = sb.out.p;
+    e.max_new = max_new;
+    e.stop = sb.stop.p;
+    e.n_stop = (int)n_stop;
+    e.stop_start = sb.stop_start.p;
+    e.gc = f.constrained ? sb.gc.p : nullptr;
+    e.fault = sb.fault.p;
+    e.gst = f.stopped ? sb.gst.p : nullptr;
+    a.raw = f.raw_copy ? sb.raw.p : nullptr;
+    rk::GenLogprobArgs &la = a.la;
+    la.lane = sb.lp_lane.p;
+    la.raw = a.raw;
+    la.logits = a.raw && !la.lane ? a.raw : m->d_slogits;
     la.V = (int)binfmt::kVocab;
-    la.gs = g.gs;
-    la.row_stream = g.row_stream;
-    la.next = c.u || c.samplers ? nullptr : m->d_next;
+    la.gs = sb.gs.p;
+    la.row_stream = sb.row_stream.p;
+    la.next = next;
     la.sample = m->d_sample;
-    la.samp = f.lpq->mode == RWKV_B200_LOGPROBS_PROCESSED ? pc.samp : nullptr;
-    la.top_n = (int)f.lpq->top_n;
-    la.max_new = c.max_new;
-    la.logprob = g.lp.p;
-    la.rank = g.rank.p;
-    la.top_tokens = g.top_tok.p;
-    la.top_logprobs = g.top_lp.p;
+    la.samp = la.lane || !f.raw ? pc.samp : nullptr;
+    la.top_n = f.top;
+    la.max_new = max_new;
+    la.logprob = sb.lp.p;
+    la.rank = sb.rank.p;
+    la.top_tokens = sb.top_tok.p;
+    la.top_logprobs = sb.top_lp.p;
+    rk::SpecArgs &sa = a.sa;
+    sa.ss = sb.ss.p;
+    sa.live = sb.live.p;
+    sa.hist = sb.hist.p;
+    sa.u = f.uniforms ? sb.su.p : nullptr;
+    sa.row_u = sb.u.p;
+    sa.next = next;
+    sa.sample = m->d_sample;
+    sa.emit = e;
+    sa.row_state = sb.row_state.p;
+    sa.score = f.spec_scored ? sb.score.p : nullptr;
+    a.fb.gs = sb.gs.p;
+    a.fb.row_stream = sb.row_stream.p;
+    a.fb.next = next;
+    a.fb.sample = m->d_sample;
 }
 
-// A step's copy of its `rows` model rows for raw log-probabilities, taken before the pick chain edits d_slogits.
-int copy_raw(M *m, const CallFeatures &f, int rows) {
-    if (f.raw_copy)
-        CK(cudaMemcpyAsync(m->gen.raw.p, m->d_slogits, (size_t)rows * binfmt::kVocab * sizeof(float), cudaMemcpyDeviceToDevice,
-                           m->stream));
+// One decoding step of generate(), speculate() and the batcher, enqueued in this order: k_spec_draft over n_spec
+// speculative streams; the forward, on the tensor cores (fwd_rows tokens in passes of per_pass at `passes`, heads[i]
+// head rows in pass i; heads NULL: every row a head row, whose head maps k_spec_draft writes) or, with passes NULL, on
+// the decode kernel; nothing more when the step has no logits rows; the raw copy and the pick chain over `rows` rows
+// with uniforms u; k_gen_logprob and k_gen_feedback over the a.fb.rows one-token rows (rows 0..); k_spec_accept, then
+// k_spec_logprob over n_spec x (a.sa.k + 1) rows.
+int run_step(M *m, const StepFlags &f, StepArgs &a, const rk::PassDesc *passes, int fwd_rows, int per_pass, const int *heads,
+             int rows, int n_spec, const double *u) {
+    const int plain = a.fb.rows;
+    if (n_spec) {
+        a.sa.heads = heads == nullptr;
+        rk::k_spec_draft<<<(unsigned)n_spec, rk::kSpecDraftThreads, 0, m->stream>>>(a.sa);
+        LAUNCHED(m);
+    }
+    int rc = passes ? gen_step_passes(m, passes, fwd_rows, per_pass, heads) : gen_step_decode(m, fwd_rows, a.pc.row_stream);
+    if (rc || rows == 0) return rc;
+    if (a.raw)
+        CK(cudaMemcpyAsync(a.raw, m->d_slogits, (size_t)rows * binfmt::kVocab * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
+    if ((rc = pick_rows(m, a.pc, rows, u))) return rc;
+    if (f.scored && plain) {
+        rk::k_gen_logprob<<<(unsigned)plain, rk::kNucThreads, 0, m->stream>>>(a.la);
+        LAUNCHED(m);
+    }
+    if (plain) {
+        rk::k_gen_feedback<<<(unsigned)((plain + 127) / 128), 128, 0, m->stream>>>(a.fb);
+        LAUNCHED(m);
+    }
+    if (n_spec) {
+        rk::k_spec_accept<<<(unsigned)n_spec, 32, 0, m->stream>>>(a.sa);
+        LAUNCHED(m);
+        if (f.spec_scored) {
+            rk::k_spec_logprob<<<(unsigned)(n_spec * (a.sa.k + 1)), rk::kNucThreads, 0, m->stream>>>(a.sa, a.la);
+            LAUNCHED(m);
+        }
+    }
+    return 0;
+}
+
+// Enqueues the read-back of a group's automaton fault record into `fault` (with automata), read after the group's
+// synchronisation: fault[0] - 1 is the stream that emitted token fault[1], which has no edge out of state
+// fault[2] of its constraint.
+int read_fault(M *m, const StepBuffers &sb, bool constrained, unsigned long long (&fault)[3]) {
+    if (constrained) CK(cudaMemcpyAsync(fault, sb.fault.p, sizeof(fault), cudaMemcpyDeviceToHost, m->stream));
     return 0;
 }
 
@@ -1335,7 +1410,7 @@ int copy_raw(M *m, const CallFeatures &f, int rows) {
 int end_group(M *m, const char *what, const CallFeatures &f, void *host, const void *dev, size_t bytes) {
     unsigned long long fault[3] = {0, 0, 0};
     CK(cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, m->stream));
-    if (f.constrained) CK(cudaMemcpyAsync(fault, m->gen.fault.p, sizeof(fault), cudaMemcpyDeviceToHost, m->stream));
+    if (int rc = read_fault(m, m->gen, f.constrained, fault)) return rc;
     SYNC(m);
     if (fault[0])
         return fail(8, "%s: stream %llu emitted token %llu, which has no edge out of state %llu of its constraint", what,
@@ -1391,29 +1466,23 @@ int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, cons
     if (tc && (rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
     m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
 
-    rk::GenStream *hg = g.h_gs;
+    rk::GenStream *hg = m->h_gs;
     for (unsigned long long s = 0; s < n_streams; ++s)
         hg[s] = rk::GenStream{c.slots[s], c.budgets ? c.budgets[s] : max_new, c.first_tokens[s], 0, 0};
-    CK(cudaMemcpyAsync(g.gs, hg, n_streams * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemcpyAsync(g.gs.p, hg, n_streams * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
     if ((rc = upload_gen(m, c)) || (rc = upload_features(m, f, n_streams, n_streams))) return rc;
     std::vector<int> live(n_streams);
     for (unsigned long long s = 0; s < n_streams; ++s) live[s] = (int)s;
     std::vector<double> ug;
-    PickChain pc;
-    rk::GenFeedbackArgs fb{};
-    rk::GenLogprobArgs la;
-    step_args(m, f, c, pc, fb.emit, la);
-    pc.exponent = sample_exponent(temp);
-    fb.gs = g.gs;
-    fb.row_stream = g.row_stream;
-    fb.next = c.u || c.samplers ? nullptr : m->d_next;
-    fb.sample = m->d_sample;
-    fb.passes = tc ? g.passes : nullptr;
+    StepArgs a;
+    step_args(m, g, f, max_new, c.n_stop, a);
+    a.pc.exponent = sample_exponent(temp);
+    a.fb.passes = tc ? g.passes.p : nullptr;
     for (unsigned long long step = 0; !live.empty() && step < max_new;) {
         // a group: the live streams are rows 0..rows-1; their inputs, and the uniforms of its steps, go up once
         const int rows = (int)live.size();
         const unsigned long long steps = std::min(kGenGroup, max_new - step);
-        CK(cudaMemcpyAsync(g.row_stream, live.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(g.row_stream.p, live.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
         if (tc && (rc = upload_step_passes(m, live.data(), rows))) return rc;
         if (c.u) {
             ug.resize((size_t)steps * rows);
@@ -1421,26 +1490,27 @@ int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, cons
                 for (int r = 0; r < rows; ++r) ug[k * rows + r] = c.u[(step + k) * n_streams + live[r]];
             CK(cudaMemcpyAsync(g.u.p, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
         }
-        fb.rows = rows;
-        for (unsigned long long k = 0; k < steps; ++k) {
-            if ((rc = tc ? gen_step_passes(m, g.passes, rows, rk::kPfMaxTokens) : gen_step_decode(m, rows, g.row_stream)) ||
-                (rc = copy_raw(m, f, rows)) || (rc = pick_rows(m, pc, rows, c.u ? g.u.p + k * rows : nullptr)))
+        a.fb.rows = rows;
+        for (unsigned long long k = 0; k < steps; ++k)
+            if ((rc = run_step(m, f, a, a.fb.passes, rows, rk::kPfMaxTokens, nullptr, rows, 0, c.u ? g.u.p + k * rows : nullptr)))
                 return rc;
-            if (lpq) {
-                rk::k_gen_logprob<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(la);
-                LAUNCHED(m);
-            }
-            rk::k_gen_feedback<<<(unsigned)((rows + 127) / 128), 128, 0, m->stream>>>(fb);
-            LAUNCHED(m);
-        }
         // the end of a group: which streams are done (a few bytes, one synchronisation); drop them from the rows
-        if ((rc = end_group(m, what, f, hg, g.gs, n_streams * sizeof(rk::GenStream)))) return rc;
+        if ((rc = end_group(m, what, f, hg, g.gs.p, n_streams * sizeof(rk::GenStream)))) return rc;
         step += steps;
         live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hg[s].done != 0; }), live.end());
     }
     if ((rc = finish_features(m, f, c))) return rc;
     for (unsigned long long s = 0; s < n_streams; ++s) c.lengths_out[s] = hg[s].len;
     return 0;
+}
+
+// The copies home -> first slot of speculative streams that end with their conversation on a spare slot: {home, slot}
+// pairs of xy, aa, bb and dd (pp: no tensor-core pass writes it).
+int copy_home(M *m, StepBuffers &sb, const std::vector<unsigned long long> &forks) {
+    int rc;
+    if ((rc = sb.forks.grow(forks.size()))) return rc;
+    CK(cudaMemcpyAsync(sb.forks.p, forks.data(), forks.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    return fork_slots(m, sb.forks.p, forks.size() / 2, false);
 }
 
 // What the speculative calls add to a GenCall: the drafts per step, the longest n-gram looked up, each stream's lookup
@@ -1499,17 +1569,16 @@ int speculate(M *m, const char *what, const GenCall &c, const SpecRequest &sr, c
     const unsigned long long n_hist = n_ctx + S * (1 + max_new);
     CK(cudaSetDevice(m->device));
     auto &g = m->gen;
-    auto &sp = m->spec;
     const int per_pass = rk::kPfMaxTokens / (int)K1; // streams per pass: a stream's rows never straddle two passes
     const size_t n_pass = (size_t)((S + per_pass - 1) / per_pass);
-    if ((rc = sp.ss.grow(S)) || (rc = sp.hist.grow(n_hist)) || (rc = sp.live.grow(S)) || (rc = sp.passes.grow(n_pass)) ||
-        (c.u && ((rc = sp.u.grow(max_new * S)) || (rc = sp.row_u.grow(S * K1)))) || (rc = sp.forks.grow(2 * S)) ||
-        (f.constrained && (rc = sp.row_state.grow(S * K1))) || (lpq && (rc = sp.score.grow(S * K1))))
+    if ((rc = g.ss.grow(S)) || (rc = g.hist.grow(n_hist)) || (rc = g.live.grow(S)) || (rc = m->spec_passes.grow(n_pass)) ||
+        (c.u && ((rc = g.su.grow(max_new * S)) || (rc = g.u.grow(S * K1)))) || (rc = g.forks.grow(2 * S)) ||
+        (f.constrained && (rc = g.row_state.grow(S * K1))) || (lpq && (rc = g.score.grow(S * K1))))
         return rc;
     if ((rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
     m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
     // k_spec_draft fills the tokens, descriptors and row maps only: the rest of each pass (no snapshots) stays zero
-    CK(cudaMemsetAsync(sp.passes.p, 0, n_pass * sizeof(rk::PassDesc), m->stream));
+    CK(cudaMemsetAsync(m->spec_passes.p, 0, n_pass * sizeof(rk::PassDesc), m->stream));
 
     // the records and the histories: stream s's history starts with its context and its first token
     std::vector<rk::SpecStream> hs(S);
@@ -1529,33 +1598,21 @@ int speculate(M *m, const char *what, const GenCall &c, const SpecRequest &sr, c
         hist[h0 + c1 - c0] = c.first_tokens[s];
         h0 += r.hl + max_new;
     }
-    CK(cudaMemcpyAsync(sp.hist.p, hist.data(), n_hist * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-    CK(cudaMemcpyAsync(sp.ss.p, hs.data(), S * sizeof(rk::SpecStream), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemcpyAsync(g.hist.p, hist.data(), n_hist * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemcpyAsync(g.ss.p, hs.data(), S * sizeof(rk::SpecStream), cudaMemcpyHostToDevice, m->stream));
     if ((rc = upload_gen(m, c))) return rc;
-    if (c.u) CK(cudaMemcpyAsync(sp.u.p, c.u, max_new * S * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+    if (c.u) CK(cudaMemcpyAsync(g.su.p, c.u, max_new * S * sizeof(double), cudaMemcpyHostToDevice, m->stream));
     if ((rc = upload_features(m, f, S, S * K1))) return rc;
 
     std::vector<int> live(S), rs;
     std::vector<rk::SpecLive> lv;
     for (unsigned long long s = 0; s < S; ++s) live[s] = (int)s;
-    rk::SpecArgs sa{};
-    sa.ss = sp.ss.p;
-    sa.live = sp.live.p;
-    sa.k = (int)draft;
-    sa.heads = true;
-    sa.hist = sp.hist.p;
-    sa.passes = sp.passes.p;
-    sa.u = c.u ? sp.u.p : nullptr;
-    sa.row_u = sp.row_u.p;
-    sa.u_stride = S;
-    sa.next = c.samplers ? nullptr : m->d_next;
-    sa.sample = m->d_sample;
-    sa.row_state = sp.row_state.p;
-    sa.score = lpq ? sp.score.p : nullptr;
-    PickChain pc;
-    rk::GenLogprobArgs la;
-    step_args(m, f, c, pc, sa.emit, la);
-    if (f.constrained) pc.row_state = sp.row_state.p;
+    StepArgs a;
+    step_args(m, g, f, max_new, c.n_stop, a);
+    a.sa.k = (int)draft;
+    a.sa.passes = m->spec_passes.p;
+    a.sa.u_stride = S;
+    if (f.constrained) a.pc.row_state = g.row_state.p;
     // each step emits at least one token per live stream, so max_new steps finish every stream
     for (unsigned long long step = 0; !live.empty() && step < max_new;) {
         const int n_live = (int)live.size(), rows = n_live * (int)K1;
@@ -1565,24 +1622,14 @@ int speculate(M *m, const char *what, const GenCall &c, const SpecRequest &sr, c
         lv.resize(n_live);
         for (int li = 0; li < n_live; ++li)
             lv[li] = rk::SpecLive{live[li], li * (int)K1, li / per_pass * rk::kPfMaxTokens + li % per_pass * (int)K1};
-        CK(cudaMemcpyAsync(sp.live.p, lv.data(), n_live * sizeof(rk::SpecLive), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(g.row_stream, rs.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-        for (unsigned long long k = 0; k < steps; ++k) {
-            rk::k_spec_draft<<<(unsigned)n_live, rk::kSpecDraftThreads, 0, m->stream>>>(sa);
-            LAUNCHED(m);
-            if ((rc = gen_step_passes(m, sp.passes.p, rows, per_pass * (int)K1)) || (rc = copy_raw(m, f, rows)) ||
-                (rc = pick_rows(m, pc, rows, c.u ? sp.row_u.p : nullptr)))
+        CK(cudaMemcpyAsync(g.live.p, lv.data(), n_live * sizeof(rk::SpecLive), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(g.row_stream.p, rs.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        for (unsigned long long k = 0; k < steps; ++k)
+            if ((rc = run_step(m, f, a, a.sa.passes, rows, per_pass * (int)K1, nullptr, rows, n_live, c.u ? g.u.p : nullptr)))
                 return rc;
-            rk::k_spec_accept<<<(unsigned)n_live, 32, 0, m->stream>>>(sa);
-            LAUNCHED(m);
-            if (lpq) {
-                rk::k_spec_logprob<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(sa, la);
-                LAUNCHED(m);
-            }
-        }
         // the end of a group: which streams are done and any token without an edge (one synchronisation); drop the
         // finished streams from the rows
-        if ((rc = end_group(m, what, f, hs.data(), sp.ss.p, S * sizeof(rk::SpecStream)))) return rc;
+        if ((rc = end_group(m, what, f, hs.data(), g.ss.p, S * sizeof(rk::SpecStream)))) return rc;
         step += steps;
         live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hs[s].done != 0; }), live.end());
     }
@@ -1593,10 +1640,7 @@ int speculate(M *m, const char *what, const GenCall &c, const SpecRequest &sr, c
             forks.push_back(hs[s].slot[hs[s].home]);
             forks.push_back(hs[s].slot[0]);
         }
-    if (!forks.empty()) {
-        CK(cudaMemcpyAsync(sp.forks.p, forks.data(), forks.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-        if ((rc = fork_slots(m, sp.forks.p, forks.size() / 2, false))) return rc;
-    }
+    if (!forks.empty() && (rc = copy_home(m, g, forks))) return rc;
     if ((rc = finish_features(m, f, c))) return rc;
     for (unsigned long long s = 0; s < S; ++s) {
         c.lengths_out[s] = hs[s].len;
@@ -1613,6 +1657,26 @@ void prefix_pool(const PC *c, double *(&pool)[4]);
 int check_batcher(const B *b) {
     if (!b) return fail(1, "null batcher handle");
     return check_model(b->m);
+}
+
+// The batcher's request `id` into *out, after the handle checks; an unknown id is an error naming the call.
+int find_req(B *b, const char *what, unsigned long long id, B::Req **out) {
+    if (int rc = check_batcher(b)) return rc;
+    const auto it = b->reqs.find(id);
+    if (it == b->reqs.end()) return fail(1, "%s: request %llu is unknown or released", what, id);
+    *out = &it->second;
+    return 0;
+}
+
+// The unfinished request that holds `slot` as its slot or a spare (0: none).
+unsigned long long slot_holder(const B *b, unsigned long long slot) {
+    for (const auto &e : b->reqs) {
+        const B::Req &o = e.second;
+        if (o.status <= RWKV_B200_REQ_GENERATING &&
+            (o.slot == slot || std::find(o.spares.begin(), o.spares.end(), slot) != o.spares.end()))
+            return e.first;
+    }
+    return 0;
 }
 
 // A group boundary (the previous group's finished requests have left): queued requests are admitted in submission
@@ -1642,12 +1706,12 @@ int batcher_boundary(B *b, std::vector<int> &dec) {
         b->h_gc[q.lane] = rk::GenConstraint{};
         b->h_lp[q.lane] = rk::LogprobLane{-1, 0};
         b->h_gst[q.lane] = rk::GenStop{};
-        CK(cudaMemcpyAsync(b->samp.p + q.lane, &q.sampler, sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(b->bufs.samp.p + q.lane, &q.sampler, sizeof(rwkv_b200_sampler), cudaMemcpyHostToDevice, m->stream));
         if (q.sampler.presence_penalty != 0.0f || q.sampler.frequency_penalty != 0.0f) {
             int rc;
-            if ((rc = b->pen_cnt.grow((size_t)b->rows * V)) || (rc = b->pen_seen.grow((size_t)b->rows * V))) return rc;
-            CK(cudaMemsetAsync(b->pen_cnt.p + (size_t)q.lane * V, 0, V * sizeof(float), m->stream));
-            CK(cudaMemsetAsync(b->pen_seen.p + (size_t)q.lane * V, 0, V, m->stream));
+            if ((rc = b->bufs.pen_cnt.grow((size_t)b->rows * V)) || (rc = b->bufs.pen_seen.grow((size_t)b->rows * V))) return rc;
+            CK(cudaMemsetAsync(b->bufs.pen_cnt.p + (size_t)q.lane * V, 0, V * sizeof(float), m->stream));
+            CK(cudaMemsetAsync(b->bufs.pen_seen.p + (size_t)q.lane * V, 0, V, m->stream));
         }
     }
     for (auto &r : restores)
@@ -1664,145 +1728,133 @@ int batcher_boundary(B *b, std::vector<int> &dec) {
         }
         if (q.status == RWKV_B200_REQ_GENERATING) dec.push_back(q.lane);
     }
-    // the decode lanes' overrides, in CSR over the lanes, when one of them has some
-    b->n_ovr = 0;
-    for (unsigned long long id : ad)
-        if (b->reqs[id].status == RWKV_B200_REQ_GENERATING) b->n_ovr += b->reqs[id].ovr_tok.size();
-    if (b->n_ovr) {
-        std::vector<unsigned long long> start(b->rows + 1, 0), tok;
-        std::vector<float> val;
-        for (int l = 0; l < b->rows; ++l) {
-            start[l] = tok.size();
-            for (unsigned long long id : ad) {
-                const B::Req &q = b->reqs[id];
-                if (q.lane != l || q.status != RWKV_B200_REQ_GENERATING) continue;
-                tok.insert(tok.end(), q.ovr_tok.begin(), q.ovr_tok.end());
-                val.insert(val.end(), q.ovr_val.begin(), q.ovr_val.end());
-            }
-        }
-        start[b->rows] = tok.size();
-        int rc;
-        if ((rc = b->ovr_tok.grow(tok.size())) || (rc = b->ovr_val.grow(val.size())) || (rc = b->ovr_start.grow(b->rows + 1)))
-            return rc;
-        CK(cudaMemcpyAsync(b->ovr_tok.p, tok.data(), tok.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(b->ovr_val.p, val.data(), val.size() * sizeof(float), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(b->ovr_start.p, start.data(), start.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-    }
-    // the lanes' stop tokens, in CSR over the lanes
-    std::vector<unsigned long long> start(b->rows + 1, 0), stop;
+    // the lanes' lists in CSR over the lanes: the stop tokens of every admitted request, and the overrides of the decode
+    // lanes, uploaded when one of them has some
+    auto &bf = b->bufs;
+    std::vector<const B::Req *> on(b->rows, nullptr);
+    for (unsigned long long id : ad) on[b->reqs[id].lane] = &b->reqs[id];
+    std::vector<unsigned long long> stop_start(b->rows + 1, 0), stop, ovr_start(b->rows + 1, 0), ovr_tok;
+    std::vector<float> ovr_val;
     for (int l = 0; l < b->rows; ++l) {
-        start[l] = stop.size();
-        for (unsigned long long id : ad)
-            if (b->reqs[id].lane == l) stop.insert(stop.end(), b->reqs[id].stop.begin(), b->reqs[id].stop.end());
+        stop_start[l] = stop.size();
+        ovr_start[l] = ovr_tok.size();
+        if (const B::Req *q = on[l]) {
+            stop.insert(stop.end(), q->stop.begin(), q->stop.end());
+            if (q->status != RWKV_B200_REQ_GENERATING) continue;
+            ovr_tok.insert(ovr_tok.end(), q->ovr_tok.begin(), q->ovr_tok.end());
+            ovr_val.insert(ovr_val.end(), q->ovr_val.begin(), q->ovr_val.end());
+        }
     }
-    start[b->rows] = stop.size();
+    stop_start[b->rows] = stop.size();
+    const size_t n_ovr = ovr_start[b->rows] = ovr_tok.size();
     int rc;
-    if ((rc = b->stop.grow(stop.size()))) return rc;
+    if (n_ovr) {
+        if ((rc = bf.ovr_tok.grow(n_ovr)) || (rc = bf.ovr_val.grow(n_ovr)) || (rc = bf.ovr_start.grow(b->rows + 1))) return rc;
+        CK(cudaMemcpyAsync(bf.ovr_tok.p, ovr_tok.data(), n_ovr * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(bf.ovr_val.p, ovr_val.data(), n_ovr * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(bf.ovr_start.p, ovr_start.data(), ovr_start.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice,
+                           m->stream));
+    }
+    if ((rc = bf.stop.grow(stop.size()))) return rc;
     if (!stop.empty())
-        CK(cudaMemcpyAsync(b->stop.p, stop.data(), stop.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-    CK(cudaMemcpyAsync(b->stop_start.p, start.data(), start.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(bf.stop.p, stop.data(), stop.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemcpyAsync(bf.stop_start.p, stop_start.data(), stop_start.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice,
+                       m->stream));
     return 0;
 }
 
-// The copies home -> slot of speculative requests that end with their conversation on a spare slot: {home, slot}
-// pairs of xy, aa, bb and dd (pp: no tensor-core pass writes it).
-int copy_home(B *b, const std::vector<unsigned long long> &forks) {
-    int rc;
-    if ((rc = b->forks.grow(forks.size()))) return rc;
-    CK(cudaMemcpyAsync(b->forks.p, forks.data(), forks.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, b->m->stream));
-    return fork_slots(b->m, b->forks.p, forks.size() / 2, false);
-}
-
-// One group of at most `max_steps` steps (<= kGenGroup); *ran receives its length. The host lays out every step's
-// passes in advance (prefill never depends on a pick) and uploads them once; the feedback of step k writes the decode
-// rows' tokens and kDescLast bits into step k + 1's layout.
-int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
-    M *m = b->m;
-    std::vector<int> dec;
-    int rc = batcher_boundary(b, dec);
-    if (rc) return rc;
-    *ran = 0;
-    if (b->admitted.empty()) return 0;
-    const int R = (int)dec.size();
-    // the group's passes add adapter deltas when an admitted request's slot is bound (its spares share the binding)
-    m->pf.adapt = false;
-    m->pf.ad_table = m->ad_table.p;
-    for (unsigned long long id : b->admitted) m->pf.adapt |= slot_binding(m, b->reqs[id].slot) != RWKV_B200_NO_ADAPTER;
-    // the prefill segments of each step: the budget goes to the prefilling requests in admission order
+// A batcher group's host plan: each step's prefill segments, the decode rows and every step's passes.
+struct GroupPlan {
     struct Seg {
         unsigned long long id, off, n;
     };
-    std::vector<std::vector<Seg>> segs;
-    std::map<unsigned long long, unsigned long long> fed;
+    std::vector<int> dec;                                 // the decode lanes, admission order (batcher_boundary)
+    std::vector<std::vector<Seg>> segs;                   // [steps] each step's prefill segments
+    std::map<unsigned long long, unsigned long long> fed; // each prefilling request's prompt tokens fed after the group
+    std::vector<const B::Req *> of_lane;                  // [rows] the request of each lane
+    std::vector<int> plain, rs;       // the one-token lanes (rows 0..Rp-1), the lane of each decode row
+    std::vector<rk::SpecLive> sl;     // the speculative lanes
+    int kmax = 0;                     // their largest k
+    size_t ps = 0;                     // passes per step
+    std::vector<rk::PassDesc> all;     // [steps][ps] every step's passes
+    std::vector<int> step_rows;        // each step's tokens
+    std::vector<std::vector<int>> H;   // each step's head rows per pass
+    StepFlags f;                       // what the decode lanes use (batcher_upload)
+    size_t W = 0, ring = 0;            // each lane's ring of tokens of the group, and all of them
+    unsigned long long steps() const { return segs.size(); }
+    int rows() const { return (int)rs.size(); } // logits rows of a step
+};
+
+// The host plan of a group of at most max_steps steps after its boundary (g.dec).
+void batcher_plan(B *b, unsigned long long max_steps, GroupPlan &g) {
+    // the prefill segments of each step: the budget goes to the prefilling requests in admission order
     for (unsigned long long id : b->admitted)
-        if (b->reqs[id].status == RWKV_B200_REQ_PREFILLING) fed[id] = b->reqs[id].fed;
+        if (b->reqs[id].status == RWKV_B200_REQ_PREFILLING) g.fed[id] = b->reqs[id].fed;
     for (unsigned long long k = 0; k < max_steps; ++k) {
-        std::vector<Seg> s;
+        std::vector<GroupPlan::Seg> s;
         unsigned long long budget = (unsigned long long)b->prefill_tokens;
         for (unsigned long long id : b->admitted) {
             const B::Req &q = b->reqs[id];
             if (q.status != RWKV_B200_REQ_PREFILLING || budget == 0) continue;
-            const unsigned long long take = std::min(budget, q.prompt.size() - 1 - fed[id]);
+            const unsigned long long take = std::min(budget, q.prompt.size() - 1 - g.fed[id]);
             if (take == 0) continue;
-            s.push_back(Seg{id, fed[id], take});
-            fed[id] += take;
+            s.push_back(GroupPlan::Seg{id, g.fed[id], take});
+            g.fed[id] += take;
             budget -= take;
         }
-        if (R == 0 && s.empty()) break; // nothing left for this group's steps to do
-        segs.push_back(std::move(s));
+        if (g.dec.empty() && s.empty()) break; // nothing left for this group's steps to do
+        g.segs.push_back(std::move(s));
     }
-    const unsigned long long steps = segs.size();
     // the decode rows: the one-token lanes first (rows 0..Rp-1, where k_gen_feedback writes them), then k + 1 rows per
     // speculative lane, each lane's rows inside one pass: pad tokens (no head, no state stored) fill up a pass a lane
     // would straddle
-    std::vector<const B::Req *> of_lane(b->rows, nullptr);
-    for (unsigned long long id : b->admitted) of_lane[b->reqs[id].lane] = &b->reqs[id];
-    std::vector<int> plain;
-    std::vector<rk::SpecLive> sl;
-    for (int l : dec)
-        if (!of_lane[l]->draft) plain.push_back(l);
-    const int Rp = (int)plain.size();
+    g.of_lane.assign(b->rows, nullptr);
+    for (unsigned long long id : b->admitted) g.of_lane[b->reqs[id].lane] = &b->reqs[id];
+    for (int l : g.dec)
+        if (!g.of_lane[l]->draft) g.plain.push_back(l);
+    g.rs = g.plain;
     std::vector<unsigned long long> dtok, dslot;
     std::vector<unsigned char> dhead;
-    std::vector<int> pads, rs(plain); // rs: the lane of each decode row
-    for (int l : plain) {
+    std::vector<int> pads;
+    for (int l : g.plain) {
         dtok.push_back(b->h_gs[l].tok); // steps > 0: the feedback writes the pick over it
         dslot.push_back(b->h_gs[l].slot);
         dhead.push_back(1);
     }
-    int kmax = 0;
-    for (int l : dec) {
-        const B::Req &q = *of_lane[l];
+    for (int l : g.dec) {
+        const B::Req &q = *g.of_lane[l];
         if (!q.draft) continue;
         const int K1 = (int)q.draft + 1;
-        kmax = std::max(kmax, (int)q.draft);
+        g.kmax = std::max(g.kmax, (int)q.draft);
         while ((int)dtok.size() % rk::kPfMaxTokens + K1 > rk::kPfMaxTokens) {
             pads.push_back((int)dtok.size());
             dtok.push_back(0);
             dslot.push_back(q.slot);
             dhead.push_back(0);
         }
-        sl.push_back(rk::SpecLive{l, (int)rs.size(), (int)dtok.size()});
+        g.sl.push_back(rk::SpecLive{l, (int)g.rs.size(), (int)dtok.size()});
         for (int i = 0; i < K1; ++i) { // k_spec_draft writes the tokens and descriptors
-            rs.push_back(l);
+            g.rs.push_back(l);
             dtok.push_back(0);
             dslot.push_back(q.slot);
             dhead.push_back(1);
         }
     }
-    const bool spec = !sl.empty();
-    const int NR = (int)rs.size(); // logits rows of a step
+    // a speculative lane emits up to kGenGroup (k + 1) tokens in a group
+    g.W = g.sl.empty() ? kGenGroup : kGenGroup * (rk::kSpecMaxDraft + 1);
+    g.ring = (size_t)b->rows * g.W;
     // every step's layout: the decode rows, then the segments without a head
+    const unsigned long long steps = g.steps();
     std::vector<std::vector<rk::PassDesc>> lay(steps);
-    std::vector<int> step_rows(steps);
-    std::vector<std::vector<int>> H(steps);
-    size_t ps = (size_t)b->max_pass; // passes per step in `passes`
+    g.step_rows.resize(steps);
+    g.H.resize(steps);
+    g.ps = (size_t)b->max_pass;
     std::vector<PC *> snapped; // caches with entries pinned by this group's layouts
     for (unsigned long long k = 0; k < steps; ++k) {
         std::vector<unsigned long long> tokens(dtok), slots(dslot), lens(dtok.size(), 1);
         std::vector<unsigned char> head(dhead);
         std::vector<size_t> seg0; // each segment's first token in the step
-        for (const Seg &s : segs[k]) {
+        for (const GroupPlan::Seg &s : g.segs[k]) {
             const B::Req &q = b->reqs[s.id];
             seg0.push_back(tokens.size());
             tokens.insert(tokens.end(), q.prompt.begin() + (long)s.off, q.prompt.begin() + (long)(s.off + s.n));
@@ -1810,235 +1862,171 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
             lens.push_back(s.n);
             head.push_back(0);
         }
-        step_rows[k] = (int)tokens.size();
-        rk::pass_layout(tokens.data(), step_rows[k], slots.data(), lens.data(), 2, nullptr, lay[k], H[k], head.data());
+        g.step_rows[k] = (int)tokens.size();
+        rk::pass_layout(tokens.data(), g.step_rows[k], slots.data(), lens.data(), 2, nullptr, lay[k], g.H[k], head.data());
         for (int p : pads) lay[k][p / rk::kPfMaxTokens].desc[p % rk::kPfMaxTokens] &= ~rk::kDescLast;
         // snapshots of cached requests at block multiples and at n_prompt - 1 inside their segments. A pass carries one
         // pool: a snapshot into a second cache's pool in the same pass is skipped (and counted)
-        for (size_t i = 0; i < segs[k].size(); ++i) {
-            const Seg &sg = segs[k][i];
+        for (size_t i = 0; i < g.segs[k].size(); ++i) {
+            const GroupPlan::Seg &sg = g.segs[k][i];
             const B::Req &q = b->reqs[sg.id];
             if (!q.cache) continue;
             double *pool[4];
             prefix_pool(q.cache, pool);
             for (unsigned long long pos = sg.off + 1; pos <= sg.off + sg.n; ++pos) {
                 if (pos % q.cache->block != 0 && pos + 1 != q.prompt.size()) continue;
-                const size_t g = seg0[i] + (size_t)(pos - sg.off - 1);
-                rk::PassDesc &pd = lay[k][g / rk::kPfMaxTokens];
+                const size_t t = seg0[i] + (size_t)(pos - sg.off - 1);
+                rk::PassDesc &pd = lay[k][t / rk::kPfMaxTokens];
                 if (pd.pool[0] && pd.pool[0] != pool[0]) {
                     q.cache->index.stats().skipped += 1;
                     continue;
                 }
                 bool fresh = false;
-                const long e = q.cache->index.take(slot_binding(m, q.slot), q.prompt.data(), (size_t)pos, &fresh);
+                const long e = q.cache->index.take(slot_binding(b->m, q.slot), q.prompt.data(), (size_t)pos, &fresh);
                 if (std::find(snapped.begin(), snapped.end(), q.cache) == snapped.end()) snapped.push_back(q.cache);
                 if (e < 0 || !fresh) continue;
-                pd.snap[g % rk::kPfMaxTokens] = (uint32_t)e + 1u;
+                pd.snap[t % rk::kPfMaxTokens] = (uint32_t)e + 1u;
                 std::copy(pool, pool + 4, pd.pool);
             }
         }
-        ps = std::max(ps, lay[k].size());
+        g.ps = std::max(g.ps, lay[k].size());
     }
     for (PC *c : snapped) c->index.unpin_all();
-    std::vector<rk::PassDesc> all(steps * ps);
-    for (unsigned long long k = 0; k < steps; ++k) std::copy(lay[k].begin(), lay[k].end(), all.begin() + k * ps);
-    // a speculative lane emits up to kGenGroup (k + 1) tokens in a group
-    const size_t W = spec ? kGenGroup * (rk::kSpecMaxDraft + 1) : kGenGroup, ring = (size_t)b->rows * W;
-    if ((rc = b->passes.grow(kGenGroup * ps)) || (rc = b->row_stream.grow(NR)) || (rc = b->u.grow(kGenGroup * NR)) ||
-        (rc = b->out.grow(ring)))
+    g.all.resize(steps * g.ps);
+    for (unsigned long long k = 0; k < steps; ++k) std::copy(lay[k].begin(), lay[k].end(), g.all.begin() + k * g.ps);
+}
+
+// The upload of a group: its passes, the decode lanes' records, row map and uniforms, and the buffers of the features
+// they use (g.f), each enqueued only when one of them needs it.
+int batcher_upload(B *b, GroupPlan &g) {
+    M *m = b->m;
+    auto &bf = b->bufs;
+    const unsigned long long steps = g.steps();
+    const int NR = g.rows(), Rp = (int)g.plain.size();
+    int rc;
+    if ((rc = bf.passes.grow(kGenGroup * g.ps)) || (rc = bf.row_stream.grow(NR)) || (rc = bf.u.grow(kGenGroup * NR)) ||
+        (rc = bf.out.grow(g.ring)))
         return rc;
-    b->h_out.resize(ring);
-    CK(cudaMemcpyAsync(b->passes.p, all.data(), all.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
-    // what the decode lanes use: each feature's work is enqueued only when one of them needs it
-    bool pen = false, constrained = false, scored = false, spec_scored = false, raw = false, stopped = false;
-    int top = 0; // the largest top_n of a scored lane
-    if (R > 0) {
-        CK(cudaMemcpyAsync(b->gs.p, b->h_gs.data(), b->rows * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(b->row_stream.p, rs.data(), NR * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+    b->h_out.resize(g.ring);
+    CK(cudaMemcpyAsync(bf.passes.p, g.all.data(), g.all.size() * sizeof(rk::PassDesc), cudaMemcpyHostToDevice, m->stream));
+    StepFlags &f = g.f;
+    f.samplers = f.uniforms = true; // every lane has a sampler; a request without uniforms draws zeros
+    for (int l : g.dec) {
+        const B::Req &q = *g.of_lane[l];
+        f.n_override += q.ovr_tok.size();
+        f.pen |= q.sampler.presence_penalty != 0.0f || q.sampler.frequency_penalty != 0.0f;
+        f.constrained |= q.gc.mask != nullptr;
+        f.stopped |= q.gst.next != nullptr;
+        if (q.lp.mode >= 0) {
+            (q.draft ? f.spec_scored : f.scored) = true;
+            f.raw |= q.lp.mode == RWKV_B200_LOGPROBS_RAW;
+            if (q.lp.top_n) f.top = rk::kMaxTopN; // each lane's top entries at its own stride
+        }
+    }
+    set_raw_copy(f);
+    if (!g.dec.empty()) {
+        CK(cudaMemcpyAsync(bf.gs.p, b->h_gs.data(), b->rows * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(bf.row_stream.p, g.rs.data(), NR * sizeof(int), cudaMemcpyHostToDevice, m->stream));
         // uniforms [steps][NR]: one-token row r at step k draws with its request's u[len + k] (k_spec_draft writes the
         // speculative rows')
         std::vector<double> ug(steps * (size_t)NR, 0.0);
-        for (int l : dec) {
-            const B::Req &q = *of_lane[l];
-            pen |= q.sampler.presence_penalty != 0.0f || q.sampler.frequency_penalty != 0.0f;
-            constrained |= q.gc.mask != nullptr;
-            stopped |= q.gst.next != nullptr;
-            if (q.lp.mode >= 0) {
-                (q.draft ? spec_scored : scored) = true;
-                raw |= q.lp.mode == RWKV_B200_LOGPROBS_RAW;
-                top = std::max(top, q.lp.top_n);
-            }
-        }
         for (int r = 0; r < Rp; ++r) {
-            const rk::GenStream &g = b->h_gs[plain[r]];
-            const B::Req &q = *of_lane[plain[r]];
+            const rk::GenStream &gs = b->h_gs[g.plain[r]];
+            const B::Req &q = *g.of_lane[g.plain[r]];
             for (unsigned long long k = 0; k < steps && !q.u.empty(); ++k)
-                if (g.len + k < q.max_new) ug[k * NR + r] = q.u[g.len + k];
+                if (gs.len + k < q.max_new) ug[k * NR + r] = q.u[gs.len + k];
         }
-        CK(cudaMemcpyAsync(b->u.p, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(bf.u.p, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
     }
-    const size_t V = binfmt::kVocab, top_ring = top ? ring * rk::kMaxTopN : 0;
-    if (constrained) {
-        if ((rc = b->gc.grow(b->rows)) || (rc = b->fault.grow(3))) return rc;
-        CK(cudaMemcpyAsync(b->gc.p, b->h_gc.data(), b->rows * sizeof(rk::GenConstraint), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemsetAsync(b->fault.p, 0, 3 * sizeof(unsigned long long), m->stream));
+    const size_t V = binfmt::kVocab, top_ring = g.ring * f.top;
+    if (f.constrained) {
+        if ((rc = bf.gc.grow(b->rows)) || (rc = bf.fault.grow(3))) return rc;
+        CK(cudaMemcpyAsync(bf.gc.p, b->h_gc.data(), b->rows * sizeof(rk::GenConstraint), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemsetAsync(bf.fault.p, 0, 3 * sizeof(unsigned long long), m->stream));
     }
-    if (stopped) {
-        if ((rc = b->gst.grow(b->rows))) return rc;
-        CK(cudaMemcpyAsync(b->gst.p, b->h_gst.data(), b->rows * sizeof(rk::GenStop), cudaMemcpyHostToDevice, m->stream));
+    if (f.stopped) {
+        if ((rc = bf.gst.grow(b->rows))) return rc;
+        CK(cudaMemcpyAsync(bf.gst.p, b->h_gst.data(), b->rows * sizeof(rk::GenStop), cudaMemcpyHostToDevice, m->stream));
     }
     // the speculative lanes' records, histories (context ++ prompt ++ emitted, with room for the rest) and uniforms
-    if (spec) {
+    if (!g.sl.empty()) {
         std::vector<unsigned long long> hist;
         std::vector<double> su;
-        for (const rk::SpecLive &e : sl) {
-            const B::Req &q = *of_lane[e.s];
-            rk::SpecStream &g = b->h_ss[e.s];
-            g = rk::SpecStream{};
-            g.slot[0] = q.slot;
-            std::copy(q.spares.begin(), q.spares.end(), g.slot + 1);
-            g.h0 = hist.size();
+        for (const rk::SpecLive &e : g.sl) {
+            const B::Req &q = *g.of_lane[e.s];
+            rk::SpecStream &r = b->h_ss[e.s];
+            r = rk::SpecStream{};
+            r.slot[0] = q.slot;
+            std::copy(q.spares.begin(), q.spares.end(), r.slot + 1);
+            r.h0 = hist.size();
             hist.insert(hist.end(), q.context.begin(), q.context.end());
             hist.insert(hist.end(), q.prompt.begin(), q.prompt.end());
             hist.insert(hist.end(), q.tokens.begin(), q.tokens.end());
-            g.hl = hist.size() - g.h0;
+            r.hl = hist.size() - r.h0;
             hist.resize(hist.size() + q.max_new - q.tokens.size());
-            g.budget = q.max_new;
-            g.len = q.tokens.size();
-            g.steps = q.steps;
-            g.u0 = su.size();
+            r.budget = q.max_new;
+            r.len = q.tokens.size();
+            r.steps = q.steps;
+            r.u0 = su.size();
             su.resize(su.size() + q.max_new, 0.0);
-            std::copy(q.u.begin(), q.u.end(), su.begin() + (long)g.u0);
-            g.home = q.home;
-            g.k = (int)q.draft;
-            g.ngram = (int)q.ngram;
+            std::copy(q.u.begin(), q.u.end(), su.begin() + (long)r.u0);
+            r.home = q.home;
+            r.k = (int)q.draft;
+            r.ngram = (int)q.ngram;
         }
-        if ((rc = b->ss.grow(b->rows)) || (rc = b->spec_live.grow(b->rows)) || (rc = b->hist.grow(hist.size())) ||
-            (rc = b->su.grow(su.size())) || (constrained && (rc = b->row_state.grow(NR))) ||
-            (spec_scored && (rc = b->score.grow(sl.size() * (kmax + 1)))))
+        if ((rc = bf.ss.grow(b->rows)) || (rc = bf.live.grow(b->rows)) || (rc = bf.hist.grow(hist.size())) ||
+            (rc = bf.su.grow(su.size())) || (f.constrained && (rc = bf.row_state.grow(NR))) ||
+            (f.spec_scored && (rc = bf.score.grow(g.sl.size() * (g.kmax + 1)))))
             return rc;
-        CK(cudaMemcpyAsync(b->ss.p, b->h_ss.data(), b->rows * sizeof(rk::SpecStream), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(b->spec_live.p, sl.data(), sl.size() * sizeof(rk::SpecLive), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(b->hist.p, hist.data(), hist.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
-        CK(cudaMemcpyAsync(b->su.p, su.data(), su.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
-        if (constrained) { // the one-token rows are masked by their lane's record; k_spec_draft writes the others
+        CK(cudaMemcpyAsync(bf.ss.p, b->h_ss.data(), b->rows * sizeof(rk::SpecStream), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(bf.live.p, g.sl.data(), g.sl.size() * sizeof(rk::SpecLive), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(bf.hist.p, hist.data(), hist.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(bf.su.p, su.data(), su.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
+        if (f.constrained) { // the one-token rows are masked by their lane's record; k_spec_draft writes the others
             const std::vector<unsigned long long> st(NR, rk::kStreamState);
-            CK(cudaMemcpyAsync(b->row_state.p, st.data(), NR * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
+            CK(cudaMemcpyAsync(bf.row_state.p, st.data(), NR * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
         }
     }
     // raw lanes read the model's rows: d_slogits itself, or a copy taken before the penalties, overrides and masks edit it
-    const bool raw_copy = raw && (pen || b->n_ovr || constrained);
-    if (scored || spec_scored) {
-        if ((rc = b->lp_lane.grow(b->rows)) || (rc = b->lp.grow(ring)) || (rc = b->rank.grow(ring)) ||
-            (rc = b->top_lp.grow(top_ring)) || (rc = b->top_tok.grow(top_ring)) || (raw_copy && (rc = b->raw.grow((size_t)NR * V))))
+    if (f.scored || f.spec_scored) {
+        if ((rc = bf.lp_lane.grow(b->rows)) || (rc = bf.lp.grow(g.ring)) || (rc = bf.rank.grow(g.ring)) ||
+            (rc = bf.top_lp.grow(top_ring)) || (rc = bf.top_tok.grow(top_ring)) || (f.raw_copy && (rc = bf.raw.grow((size_t)NR * V))))
             return rc;
-        CK(cudaMemcpyAsync(b->lp_lane.p, b->h_lp.data(), b->rows * sizeof(rk::LogprobLane), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(bf.lp_lane.p, b->h_lp.data(), b->rows * sizeof(rk::LogprobLane), cudaMemcpyHostToDevice, m->stream));
     }
-    PickChain pc{};
-    pc.gs = b->gs.p;
-    pc.row_stream = b->row_stream.p;
-    pc.samp = b->samp.p;
-    pc.pen_cnt = pen ? b->pen_cnt.p : nullptr;
-    pc.pen_seen = b->pen_seen.p;
-    pc.ovr_tok = b->ovr_tok.p;
-    pc.ovr_val = b->ovr_val.p;
-    pc.n_override = b->n_ovr;
-    pc.gc = constrained ? b->gc.p : nullptr;
-    pc.ovr_start = b->ovr_start.p;
-    if (spec && constrained) pc.row_state = b->row_state.p;
-    rk::GenLogprobArgs la{};
-    la.logits = m->d_slogits;
-    la.V = (int)V;
-    la.gs = b->gs.p;
-    la.row_stream = b->row_stream.p;
-    la.sample = m->d_sample;
-    la.samp = b->samp.p;
-    la.top_n = top ? rk::kMaxTopN : 0;
-    la.max_new = W;
-    la.logprob = b->lp.p;
-    la.rank = b->rank.p;
-    la.top_tokens = b->top_tok.p;
-    la.top_logprobs = b->top_lp.p;
-    la.lane = b->lp_lane.p;
-    la.raw = raw_copy ? b->raw.p : nullptr;
-    // the emitted tokens of both kinds of lane: each lane's ring of W entries, its own stop tokens, automaton and set
-    rk::GenEmit emit{};
-    emit.out = b->out.p;
-    emit.max_new = W;
-    emit.stop = b->stop.p;
-    emit.stop_start = b->stop_start.p;
-    emit.gc = constrained ? b->gc.p : nullptr;
-    emit.fault = b->fault.p;
-    emit.gst = stopped ? b->gst.p : nullptr;
-    rk::SpecArgs sa{};
-    sa.ss = b->ss.p;
-    sa.live = b->spec_live.p;
-    sa.k = kmax;
-    sa.hist = b->hist.p;
-    sa.u = b->su.p;
-    sa.u_stride = 1;
-    sa.sample = m->d_sample;
-    sa.emit = emit;
-    sa.row_state = b->row_state.p;
-    sa.score = spec_scored ? b->score.p : nullptr;
-    rk::GenFeedbackArgs fb{};
-    fb.gs = b->gs.p;
-    fb.row_stream = b->row_stream.p;
-    fb.rows = Rp;
-    fb.sample = m->d_sample;
-    fb.emit = emit;
-    for (unsigned long long k = 0; k < steps; ++k) {
-        sa.passes = b->passes.p + k * ps;
-        sa.row_u = b->u.p + k * NR;
-        if (spec) {
-            rk::k_spec_draft<<<(unsigned)sl.size(), rk::kSpecDraftThreads, 0, m->stream>>>(sa);
-            LAUNCHED(m);
-        }
-        if ((rc = gen_step_passes(m, b->passes.p + k * ps, step_rows[k], rk::kPfMaxTokens, H[k].data()))) return rc;
-        if (R == 0) continue;
-        if (raw_copy) CK(cudaMemcpyAsync(b->raw.p, m->d_slogits, (size_t)NR * V * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
-        if ((rc = pick_rows(m, pc, NR, b->u.p + k * NR))) return rc;
-        if (scored) {
-            rk::k_gen_logprob<<<(unsigned)Rp, rk::kNucThreads, 0, m->stream>>>(la);
-            LAUNCHED(m);
-        }
-        if (Rp > 0) {
-            fb.passes = k + 1 < steps ? b->passes.p + (k + 1) * ps : nullptr;
-            rk::k_gen_feedback<<<(unsigned)((Rp + 127) / 128), 128, 0, m->stream>>>(fb);
-            LAUNCHED(m);
-        }
-        if (spec) {
-            rk::k_spec_accept<<<(unsigned)sl.size(), 32, 0, m->stream>>>(sa);
-            LAUNCHED(m);
-            if (spec_scored) {
-                rk::k_spec_logprob<<<(unsigned)(sl.size() * (kmax + 1)), rk::kNucThreads, 0, m->stream>>>(sa, la);
-                LAUNCHED(m);
-            }
-        }
-    }
-    // the group's end: the lanes' records and the tokens of the group (with their results and the automata's states
-    // when a lane uses them) come back with one synchronisation
+    return 0;
+}
+
+// The end of a group: the lanes' records and the tokens of the group (with their results and the automata's states when
+// a lane uses them) come back with one synchronisation and go to their requests; finished speculative requests have
+// their home copied to their slot, and finished requests leave.
+int batcher_collect(B *b, GroupPlan &g) {
+    M *m = b->m;
+    const auto &bf = b->bufs;
+    const StepFlags &f = g.f;
+    const size_t W = g.W, ring = g.ring, top_ring = ring * f.top;
     unsigned long long fault[3] = {0, 0, 0};
-    if (R > 0) {
-        CK(cudaMemcpyAsync(b->h_gs.data(), b->gs.p, b->rows * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
-        CK(cudaMemcpyAsync(b->h_out.data(), b->out.p, ring * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+    if (!g.dec.empty()) {
+        CK(cudaMemcpyAsync(b->h_gs.data(), bf.gs.p, b->rows * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(b->h_out.data(), bf.out.p, ring * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
     }
-    if (spec) CK(cudaMemcpyAsync(b->h_ss.data(), b->ss.p, b->rows * sizeof(rk::SpecStream), cudaMemcpyDeviceToHost, m->stream));
-    if (constrained) {
-        CK(cudaMemcpyAsync(b->h_gc.data(), b->gc.p, b->rows * sizeof(rk::GenConstraint), cudaMemcpyDeviceToHost, m->stream));
-        CK(cudaMemcpyAsync(fault, b->fault.p, sizeof(fault), cudaMemcpyDeviceToHost, m->stream));
-    }
-    if (stopped) CK(cudaMemcpyAsync(b->h_gst.data(), b->gst.p, b->rows * sizeof(rk::GenStop), cudaMemcpyDeviceToHost, m->stream));
-    if (scored || spec_scored) {
+    if (!g.sl.empty())
+        CK(cudaMemcpyAsync(b->h_ss.data(), bf.ss.p, b->rows * sizeof(rk::SpecStream), cudaMemcpyDeviceToHost, m->stream));
+    if (f.constrained)
+        CK(cudaMemcpyAsync(b->h_gc.data(), bf.gc.p, b->rows * sizeof(rk::GenConstraint), cudaMemcpyDeviceToHost, m->stream));
+    int rc;
+    if ((rc = read_fault(m, bf, f.constrained, fault))) return rc;
+    if (f.stopped) CK(cudaMemcpyAsync(b->h_gst.data(), bf.gst.p, b->rows * sizeof(rk::GenStop), cudaMemcpyDeviceToHost, m->stream));
+    if (f.scored || f.spec_scored) {
         b->h_lpv.resize(ring);
         b->h_rank.resize(ring);
         b->h_top_lp.resize(top_ring);
         b->h_top_tok.resize(top_ring);
-        CK(cudaMemcpyAsync(b->h_lpv.data(), b->lp.p, ring * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
-        CK(cudaMemcpyAsync(b->h_rank.data(), b->rank.p, ring * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
-        if (top) {
-            CK(cudaMemcpyAsync(b->h_top_lp.data(), b->top_lp.p, top_ring * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
-            CK(cudaMemcpyAsync(b->h_top_tok.data(), b->top_tok.p, top_ring * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(b->h_lpv.data(), bf.lp.p, ring * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(b->h_rank.data(), bf.rank.p, ring * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+        if (f.top) {
+            CK(cudaMemcpyAsync(b->h_top_lp.data(), bf.top_lp.p, top_ring * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+            CK(cudaMemcpyAsync(b->h_top_tok.data(), bf.top_tok.p, top_ring * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
         }
     }
     SYNC(m);
@@ -2053,7 +2041,7 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
     for (unsigned long long id : b->admitted) {
         B::Req &q = b->reqs[id];
         if (q.status == RWKV_B200_REQ_PREFILLING) {
-            q.fed = fed[id];
+            q.fed = g.fed[id];
             continue;
         }
         const rk::SpecStream &e = b->h_ss[q.lane];
@@ -2084,7 +2072,7 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
             }
         }
     }
-    if (!forks.empty() && (rc = copy_home(b, forks))) return rc;
+    if (!forks.empty() && (rc = copy_home(m, b->bufs, forks))) return rc;
     // finished requests leave here, before the next boundary admits anyone (a caller may release them in between)
     auto &ad = b->admitted;
     ad.erase(std::remove_if(ad.begin(), ad.end(),
@@ -2095,6 +2083,43 @@ int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
                                 return true;
                             }),
              ad.end());
+    return 0;
+}
+
+// One group of at most `max_steps` steps (<= kGenGroup); *ran receives its length. The host lays out every step's
+// passes in advance (prefill never depends on a pick) and uploads them once; the feedback of step k writes the decode
+// rows' tokens and kDescLast bits into step k + 1's layout.
+int batcher_group(B *b, unsigned long long max_steps, unsigned long long *ran) {
+    M *m = b->m;
+    GroupPlan g;
+    int rc = batcher_boundary(b, g.dec);
+    if (rc) return rc;
+    *ran = 0;
+    if (b->admitted.empty()) return 0;
+    // the group's passes add adapter deltas when an admitted request's slot is bound (its spares share the binding)
+    m->pf.adapt = false;
+    m->pf.ad_table = m->ad_table.p;
+    for (unsigned long long id : b->admitted) m->pf.adapt |= slot_binding(m, b->reqs[id].slot) != RWKV_B200_NO_ADAPTER;
+    batcher_plan(b, max_steps, g);
+    if ((rc = batcher_upload(b, g))) return rc;
+    const unsigned long long steps = g.steps();
+    const int NR = g.rows();
+    auto &bf = b->bufs;
+    StepArgs a;
+    step_args(m, bf, g.f, g.W, 0, a);
+    a.fb.rows = (int)g.plain.size();
+    a.sa.k = g.kmax;
+    a.sa.u_stride = 1;
+    if (!g.sl.empty() && g.f.constrained) a.pc.row_state = bf.row_state.p;
+    for (unsigned long long k = 0; k < steps; ++k) {
+        rk::PassDesc *passes = bf.passes.p + k * g.ps;
+        a.sa.passes = passes;
+        a.sa.row_u = bf.u.p + k * NR;
+        a.fb.passes = k + 1 < steps ? passes + g.ps : nullptr;
+        if ((rc = run_step(m, g.f, a, passes, g.step_rows[k], rk::kPfMaxTokens, g.H[k].data(), NR, (int)g.sl.size(), a.sa.row_u)))
+            return rc;
+    }
+    if ((rc = batcher_collect(b, g))) return rc;
     *ran = steps;
     return 0;
 }
@@ -2243,7 +2268,7 @@ void rwkv_b200_free(rwkv_b200_model *m) {
     if (m->h_next) cudaFreeHost(m->h_next);
     if (m->h_sample) cudaFreeHost(m->h_sample);
     if (m->h_diag) cudaFreeHost(m->h_diag);
-    if (m->gen.h_gs) cudaFreeHost(m->gen.h_gs);
+    if (m->h_gs) cudaFreeHost(m->h_gs);
     if (m->stream) cudaStreamDestroy(m->stream);
     delete m; // frees the grow-only buffers and the automata
     cudaGetLastError(); // a context killed by a trap makes every call above fail; do not leave that as "last error"
@@ -2720,14 +2745,14 @@ int rwkv_b200_beam_search(rwkv_b200_model *m, const unsigned long long *slots, c
     if (tc && (rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
     m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
 
-    rk::GenStream *hg = g.h_gs;
+    rk::GenStream *hg = m->h_gs;
     for (unsigned long long s = 0; s < G * B; ++s) hg[s] = rk::GenStream{slots[s], N, s % B == 0 ? first_tokens[s / B] : 0, 0, 0};
     std::vector<int> row0(G), live(G);
     for (unsigned long long i = 0; i < G; ++i) {
         row0[i] = (int)(i * B);
         live[i] = (int)i;
     }
-    CK(cudaMemcpyAsync(g.gs, hg, G * B * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
+    CK(cudaMemcpyAsync(g.gs.p, hg, G * B * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
     CK(cudaMemcpyAsync(bm.row0.p, row0.data(), G * sizeof(int), cudaMemcpyHostToDevice, m->stream));
     CK(cudaMemcpyAsync(bm.P.p, P.data(), (N + 1) * sizeof(double), cudaMemcpyHostToDevice, m->stream));
     if (n_stop) CK(cudaMemcpyAsync(g.stop.p, stop_tokens, n_stop * sizeof(unsigned long long), cudaMemcpyHostToDevice, m->stream));
@@ -2743,18 +2768,18 @@ int rwkv_b200_beam_search(rwkv_b200_model *m, const unsigned long long *slots, c
         rs.resize((size_t)Gl * B);
         for (int gi = 0; gi < Gl; ++gi)
             for (unsigned long long j = 0; j < B; ++j) rs[gi * B + j] = (int)(live[gi] * B + j);
-        CK(cudaMemcpyAsync(g.row_stream, rs.data(), rs.size() * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        CK(cudaMemcpyAsync(g.row_stream.p, rs.data(), rs.size() * sizeof(int), cudaMemcpyHostToDevice, m->stream));
         CK(cudaMemcpyAsync(bm.groups.p, live.data(), Gl * sizeof(int), cudaMemcpyHostToDevice, m->stream));
         if (tc && (rc = upload_step_passes(m, step == 0 ? row0.data() : rs.data(), step == 0 ? Gl : Gl * (int)B))) return rc;
-        rk::BeamArgs ba{g.gs, bm.cum.p, bm.groups.p, bm.cand_tok.p, bm.cand_lp.p, (int)C, (int)B, (int)K, 0, 0, N, bm.P.p,
+        rk::BeamArgs ba{g.gs.p, bm.cum.p, bm.groups.p, bm.cand_tok.p, bm.cand_lp.p, (int)C, (int)B, (int)K, 0, 0, N, bm.P.p,
                         length_penalty < 0.0 ? 1 : 0, g.stop.p, (int)n_stop, bm.back.p, bm.hyp.p, bm.n_hyp.p, bm.done.p, bm.forks.p,
-                        tc ? g.passes : nullptr};
+                        tc ? g.passes.p : nullptr};
         for (unsigned long long k = 0; k < steps; ++k) {
             const unsigned long long st = step + k;
             const int nb = st == 0 ? 1 : (int)B, rows = Gl * nb;
-            const int *rmap = st == 0 ? bm.row0.p : g.row_stream;
-            if ((rc = tc ? gen_step_passes(m, g.passes, rows, rk::kPfMaxTokens) : gen_step_decode(m, rows, rmap))) return rc;
-            rk::k_beam_expand<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs, rmap, (int)C,
+            const int *rmap = st == 0 ? bm.row0.p : g.row_stream.p;
+            if ((rc = tc ? gen_step_passes(m, g.passes.p, rows, rk::kPfMaxTokens) : gen_step_decode(m, rows, rmap))) return rc;
+            rk::k_beam_expand<<<(unsigned)rows, rk::kNucThreads, 0, m->stream>>>(m->d_slogits, (int)V, g.gs.p, rmap, (int)C,
                                                                                 bm.cand_tok.p, bm.cand_lp.p);
             LAUNCHED(m);
             ba.step = (int)st;
@@ -2766,7 +2791,7 @@ int rwkv_b200_beam_search(rwkv_b200_model *m, const unsigned long long *slots, c
         }
         // the end of a host group: which groups are done and the beams' records (one synchronisation)
         CK(cudaMemcpyAsync(hdone.data(), bm.done.p, G * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
-        CK(cudaMemcpyAsync(hg, g.gs, G * B * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
+        CK(cudaMemcpyAsync(hg, g.gs.p, G * B * sizeof(rk::GenStream), cudaMemcpyDeviceToHost, m->stream));
         SYNC(m);
         step += steps;
         live.erase(std::remove_if(live.begin(), live.end(), [&](int gg) { return hdone[gg] != 0; }), live.end());
@@ -3394,14 +3419,14 @@ int rwkv_b200_batcher_open(rwkv_b200_model *m, unsigned long long rows, unsigned
     b->max_pass = (int)((rows + prefill_tokens + rk::kPfMaxTokens - 1) / rk::kPfMaxTokens);
     b->lane_used.assign(rows, 0);
     b->h_gs.assign(rows, rk::GenStream{});
-    b->h_out.assign(rows * kGenGroup, 0);
     b->h_gc.assign(rows, rk::GenConstraint{});
     b->h_lp.assign(rows, rk::LogprobLane{-1, 0});
     b->h_gst.assign(rows, rk::GenStop{});
     b->h_ss.assign(rows, rk::SpecStream{});
-    if ((rc = b->gs.grow(rows)) || (rc = b->row_stream.grow(rows)) || (rc = b->passes.grow(kGenGroup * (size_t)b->max_pass)) ||
-        (rc = b->samp.grow(rows)) || (rc = b->stop_start.grow(rows + 1)) || (rc = b->out.grow(rows * kGenGroup)) ||
-        (rc = b->u.grow(kGenGroup * rows))) {
+    auto &bf = b->bufs;
+    if ((rc = bf.gs.grow(rows)) || (rc = bf.row_stream.grow(rows)) || (rc = bf.passes.grow(kGenGroup * (size_t)b->max_pass)) ||
+        (rc = bf.samp.grow(rows)) || (rc = bf.stop_start.grow(rows + 1)) || (rc = bf.out.grow(rows * kGenGroup)) ||
+        (rc = bf.u.grow(kGenGroup * rows))) {
         delete b;
         return rc;
     }
@@ -3435,12 +3460,8 @@ int rwkv_b200_batcher_submit_ex(rwkv_b200_batcher *b, const rwkv_b200_request *r
             (x->logprobs && (rc = check_logprob_mode(what, x->logprob_mode, x->top_n))))
             return rc;
     }
-    for (const auto &e : b->reqs) {
-        const B::Req &o = e.second;
-        if (o.status <= RWKV_B200_REQ_GENERATING &&
-            (o.slot == r->slot || std::find(o.spares.begin(), o.spares.end(), r->slot) != o.spares.end()))
-            return fail(1, "%s: slot %llu is held by unfinished request %llu", what, r->slot, e.first);
-    }
+    if (const unsigned long long h = slot_holder(b, r->slot))
+        return fail(1, "%s: slot %llu is held by unfinished request %llu", what, r->slot, h);
     B::Req q;
     q.slot = r->slot;
     q.max_new = r->max_new;
@@ -3490,16 +3511,13 @@ int rwkv_b200_batcher_run(rwkv_b200_batcher *b, unsigned long long max_steps, un
 
 int rwkv_b200_batcher_read(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *tokens_out, unsigned long long cap,
                            unsigned long long *len, int *status) {
-    int rc = check_batcher(b);
-    if (rc) return rc;
-    const auto it = b->reqs.find(id);
-    if (it == b->reqs.end()) return fail(1, "batcher_read: request %llu is unknown or released", id);
-    const B::Req &q = it->second;
+    B::Req *q = nullptr;
+    if (int rc = find_req(b, "batcher_read", id, &q)) return rc;
     if (cap && !tokens_out) return fail(1, "batcher_read: cap = %llu with NULL tokens_out", cap);
-    const size_t n = std::min<size_t>(cap, q.tokens.size());
-    if (n) memcpy(tokens_out, q.tokens.data(), n * sizeof(unsigned long long));
-    if (len) *len = q.tokens.size();
-    if (status) *status = q.status;
+    const size_t n = std::min<size_t>(cap, q->tokens.size());
+    if (n) memcpy(tokens_out, q->tokens.data(), n * sizeof(unsigned long long));
+    if (len) *len = q->tokens.size();
+    if (status) *status = q->status;
     return 0;
 }
 
@@ -3508,23 +3526,20 @@ int rwkv_b200_batcher_read_ex(rwkv_b200_batcher *b, unsigned long long id, unsig
                               unsigned long long *top_tokens_out, double *top_logprobs_out, unsigned long long *state_out,
                               unsigned long long *len, int *status) {
     const char *what = "batcher_read_ex";
-    int rc = check_batcher(b);
-    if (rc) return rc;
-    const auto it = b->reqs.find(id);
-    if (it == b->reqs.end()) return fail(1, "%s: request %llu is unknown or released", what, id);
-    const B::Req &q = it->second;
-    if (q.lp.mode < 0 && (logprobs_out || ranks_out || top_tokens_out || top_logprobs_out))
+    B::Req *q = nullptr;
+    if (int rc = find_req(b, what, id, &q)) return rc;
+    if (q->lp.mode < 0 && (logprobs_out || ranks_out || top_tokens_out || top_logprobs_out))
         return fail(1, "%s: request %llu has no log-probabilities (submit_ex with logprobs = 0 or without an extension)", what,
                     id);
-    const size_t n = std::min<size_t>(cap, q.tokens.size()), nt = n * (size_t)std::max(q.lp.top_n, 0);
-    if (tokens_out && n) memcpy(tokens_out, q.tokens.data(), n * sizeof(unsigned long long));
-    if (logprobs_out && n) memcpy(logprobs_out, q.logprobs.data(), n * sizeof(double));
-    if (ranks_out && n) memcpy(ranks_out, q.ranks.data(), n * sizeof(unsigned long long));
-    if (top_tokens_out && nt) memcpy(top_tokens_out, q.top_tokens.data(), nt * sizeof(unsigned long long));
-    if (top_logprobs_out && nt) memcpy(top_logprobs_out, q.top_logprobs.data(), nt * sizeof(double));
-    if (state_out) *state_out = q.gc.mask ? q.gc.state : 0;
-    if (len) *len = q.tokens.size();
-    if (status) *status = q.status;
+    const size_t n = std::min<size_t>(cap, q->tokens.size()), nt = n * (size_t)std::max(q->lp.top_n, 0);
+    if (tokens_out && n) memcpy(tokens_out, q->tokens.data(), n * sizeof(unsigned long long));
+    if (logprobs_out && n) memcpy(logprobs_out, q->logprobs.data(), n * sizeof(double));
+    if (ranks_out && n) memcpy(ranks_out, q->ranks.data(), n * sizeof(unsigned long long));
+    if (top_tokens_out && nt) memcpy(top_tokens_out, q->top_tokens.data(), nt * sizeof(unsigned long long));
+    if (top_logprobs_out && nt) memcpy(top_logprobs_out, q->top_logprobs.data(), nt * sizeof(double));
+    if (state_out) *state_out = q->gc.mask ? q->gc.state : 0;
+    if (len) *len = q->tokens.size();
+    if (status) *status = q->status;
     return 0;
 }
 
@@ -3569,12 +3584,8 @@ int rwkv_b200_batcher_submit_spec(rwkv_b200_batcher *b, const rwkv_b200_request 
         for (unsigned i = 0; i < spec->draft; ++i) {
             const unsigned long long z = spec->spare_slots[i];
             if (z == r->slot) return fail(1, "%s: spare slot %llu is the request's slot", what, z);
-            for (const auto &e : b->reqs) {
-                const B::Req &o = e.second;
-                if (o.status <= RWKV_B200_REQ_GENERATING &&
-                    (o.slot == z || std::find(o.spares.begin(), o.spares.end(), z) != o.spares.end()))
-                    return fail(1, "%s: spare slot %llu is held by unfinished request %llu", what, z, e.first);
-            }
+            if (const unsigned long long h = slot_holder(b, z))
+                return fail(1, "%s: spare slot %llu is held by unfinished request %llu", what, z, h);
         }
         std::vector<unsigned long long> all(1, r->slot);
         all.insert(all.end(), spec->spare_slots, spec->spare_slots + spec->draft);
@@ -3602,31 +3613,25 @@ int rwkv_b200_batcher_submit_prefix(rwkv_b200_batcher *b, const rwkv_b200_reques
 }
 
 int rwkv_b200_batcher_read_prefix(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *cached) {
-    int rc = check_batcher(b);
-    if (rc) return rc;
-    const auto it = b->reqs.find(id);
-    if (it == b->reqs.end()) return fail(1, "batcher_read_prefix: request %llu is unknown or released", id);
-    if (cached) *cached = it->second.cached;
+    B::Req *q = nullptr;
+    if (int rc = find_req(b, "batcher_read_prefix", id, &q)) return rc;
+    if (cached) *cached = q->cached;
     return 0;
 }
 
 int rwkv_b200_batcher_read_spec(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *steps) {
-    int rc = check_batcher(b);
-    if (rc) return rc;
-    const auto it = b->reqs.find(id);
-    if (it == b->reqs.end()) return fail(1, "batcher_read_spec: request %llu is unknown or released", id);
+    B::Req *q = nullptr;
+    if (int rc = find_req(b, "batcher_read_spec", id, &q)) return rc;
     if (!steps) return fail(1, "batcher_read_spec: steps is NULL");
-    *steps = it->second.steps;
+    *steps = q->steps;
     return 0;
 }
 
 int rwkv_b200_batcher_read_stop(rwkv_b200_batcher *b, unsigned long long id, unsigned long long *hit, unsigned long long *tail,
                                 unsigned long long *state) {
-    int rc = check_batcher(b);
-    if (rc) return rc;
-    const auto it = b->reqs.find(id);
-    if (it == b->reqs.end()) return fail(1, "batcher_read_stop: request %llu is unknown or released", id);
-    const rk::GenStop &g = it->second.gst;
+    B::Req *q = nullptr;
+    if (int rc = find_req(b, "batcher_read_stop", id, &q)) return rc;
+    const rk::GenStop &g = q->gst;
     if (hit) *hit = g.next ? g.match : 0;
     if (tail) *tail = g.next ? g.tail : 0;
     if (state) *state = g.next ? g.state : 0;
@@ -3634,35 +3639,29 @@ int rwkv_b200_batcher_read_stop(rwkv_b200_batcher *b, unsigned long long id, uns
 }
 
 int rwkv_b200_batcher_cancel(rwkv_b200_batcher *b, unsigned long long id) {
-    int rc = check_batcher(b);
-    if (rc) return rc;
-    const auto it = b->reqs.find(id);
-    if (it == b->reqs.end()) return fail(1, "batcher_cancel: request %llu is unknown or released", id);
-    B::Req &q = it->second;
-    if (q.status > RWKV_B200_REQ_GENERATING) return fail(1, "batcher_cancel: request %llu has already ended", id);
-    if (q.status == RWKV_B200_REQ_QUEUED) {
+    B::Req *q = nullptr;
+    if (int rc = find_req(b, "batcher_cancel", id, &q)) return rc;
+    if (q->status > RWKV_B200_REQ_GENERATING) return fail(1, "batcher_cancel: request %llu has already ended", id);
+    if (q->status == RWKV_B200_REQ_QUEUED) {
         b->queue.erase(std::find(b->queue.begin(), b->queue.end(), id));
     } else {
-        if (q.home) { // the conversation is on a spare slot
+        if (q->home) { // the conversation is on a spare slot
             CK(cudaSetDevice(b->m->device));
-            if ((rc = copy_home(b, {q.spares[q.home - 1], q.slot}))) return rc;
-            q.home = 0;
+            if (int rc = copy_home(b->m, b->bufs, {q->spares[q->home - 1], q->slot})) return rc;
+            q->home = 0;
         }
         b->admitted.erase(std::find(b->admitted.begin(), b->admitted.end(), id));
-        b->lane_used[q.lane] = 0;
+        b->lane_used[q->lane] = 0;
     }
-    q.status = RWKV_B200_REQ_CANCELLED;
+    q->status = RWKV_B200_REQ_CANCELLED;
     return 0;
 }
 
 int rwkv_b200_batcher_release(rwkv_b200_batcher *b, unsigned long long id) {
-    int rc = check_batcher(b);
-    if (rc) return rc;
-    const auto it = b->reqs.find(id);
-    if (it == b->reqs.end()) return fail(1, "batcher_release: request %llu is unknown or released", id);
-    if (it->second.status <= RWKV_B200_REQ_GENERATING)
-        return fail(1, "batcher_release: request %llu has not ended (cancel it first)", id);
-    b->reqs.erase(it);
+    B::Req *q = nullptr;
+    if (int rc = find_req(b, "batcher_release", id, &q)) return rc;
+    if (q->status <= RWKV_B200_REQ_GENERATING) return fail(1, "batcher_release: request %llu has not ended (cancel it first)", id);
+    b->reqs.erase(id);
     return 0;
 }
 
