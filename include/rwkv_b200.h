@@ -667,6 +667,49 @@ int rwkv_b200_generate_streams_stop(rwkv_b200_model *m, const unsigned long long
                                     const unsigned long long *constraint_ids, const unsigned long long *start_states,
                                     unsigned long long *states_out, const rwkv_b200_stop_request *stop);
 
+/* Classifier-free guidance (rwkv_b200_generate_streams_guided). A guided stream s has a guidance slot g_s, a guidance
+ * first token f'_s and a scale gamma_s.
+ * 1. Rows. Each step the stream's current input goes to its own slot, as in rwkv_b200_generate_streams_stop, and its
+ *    guidance input to g_s in the same forward: f'_s at the first step, then the token the stream emitted last, so the
+ *    guidance history is [f'_s] ++ emitted tokens.
+ * 2. Combination. With c the stream's f32 logits row, q its guidance row and w = gamma_s - 1 in f32, the row becomes
+ *    l[v] = c[v] + w * (c[v] - q[v]), each operation rounded to nearest f32 and none fused (numpy float32
+ *    c + np.float32(w) * (c - q)). l replaces c, and the step goes on exactly as generate_streams_stop's: penalties,
+ *    overrides, automaton mask, pick, scoring, emit and stop checks. Logits are finite, so gamma = 1 gives l == c bit
+ *    for bit: a stream with scale 1 is the unguided stream, whatever its guidance slot holds.
+ * 3. Log-probabilities. Raw mode scores c, the conditional row (bit for bit rwkv_b200_score_streams on the stream's
+ *    slot); processed mode scores the row the pick read, guidance included.
+ * 4. End of a stream. Neither of its slots is written again: its own slot ends as generate_streams_stop leaves it, and
+ *    g_s holds the state after [f'_s] ++ tokens[:-1] (emitted, not fed), bit for bit rwkv_b200_forward_streams of
+ *    those tokens on g_s on the same path. Slots the call does not name are untouched.
+ * 5. Path. With G guided streams the call has S + G rows and chooses once: the tensor cores when S + G >= prefill_min
+ *    or when any named slot (stream or guidance) is bound to an adapter, else the decode kernel. A guidance slot may be
+ *    bound to another adapter than its stream's slot (or to none). */
+#define RWKV_B200_NO_GUIDANCE 0xFFFFFFFFFFFFFFFFULL /* guidance slots entry of an unguided stream */
+typedef struct rwkv_b200_guidance {
+    const unsigned long long *slots;        /* [n_streams] guidance slot, or RWKV_B200_NO_GUIDANCE */
+    const unsigned long long *first_tokens; /* [n_streams] read where slots[s] names a slot */
+    const float *scales;                    /* [n_streams] gamma, finite, 0 <= gamma <= 100 */
+} rwkv_b200_guidance;
+
+/* rwkv_b200_generate_streams_stop with classifier-free guidance by the rule above; guidance == NULL is exactly that call
+ * and enqueues the same launches. Guided and unguided streams may share a call; samplers == NULL is the arg-max.
+ * Refused before any work (every slot untouched): every refusal of generate_streams_stop, guidance with NULL slots or
+ * with NULL first_tokens or scales while a slot is named, a guidance slot >= max_gpt, repeated or equal to any stream's
+ * slot, a guidance first token >= 50277, a scale that is not finite or outside [0, 100], and tensor parallelism. */
+int rwkv_b200_generate_streams_guided(rwkv_b200_model *m, const unsigned long long *slots,
+                                      const unsigned long long *first_tokens, unsigned long long n_streams,
+                                      unsigned long long max_new, const unsigned long long *budgets,
+                                      const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                      const unsigned long long *override_tokens, const float *override_values,
+                                      unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
+                                      unsigned long long *tokens_out, unsigned long long *lengths_out, int logprob_mode,
+                                      unsigned int top_n, double *logprobs_out, unsigned long long *ranks_out,
+                                      unsigned long long *top_tokens_out, double *top_logprobs_out,
+                                      const unsigned long long *constraint_ids, const unsigned long long *start_states,
+                                      unsigned long long *states_out, const rwkv_b200_stop_request *stop,
+                                      const rwkv_b200_guidance *guidance);
+
 /* rwkv_b200_generate_streams_speculative with stop strings (stop == NULL: exactly that call). Each emitted token of a
  * step is walked in order, so a string that ends inside an accepted run of drafts ends the stream at that token. The
  * tokens, lengths, first slots and hit, tail and state are bit for bit those of rwkv_b200_generate_streams_stop on the

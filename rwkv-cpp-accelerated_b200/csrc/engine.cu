@@ -126,6 +126,7 @@ struct StepBuffers {
     DevBuf<rk::SpecScore> score;
     DevBuf<unsigned long long> hist, row_state, forks;
     DevBuf<double> su;
+    DevBuf<rk::GenGuide> guide;        // [rows] each guided row's conditional row and scale (generate_streams_guided)
 };
 
 } // namespace
@@ -881,6 +882,8 @@ constexpr unsigned long long kGenGroup = 16;
 
 // Largest |presence| or |frequency| penalty accepted: penalised logits stay far inside the f32 range.
 constexpr float kMaxPenalty = 1e6f;
+// Largest guidance scale accepted (rwkv_b200_generate_streams_guided): guided logits stay far inside the f32 range.
+constexpr float kMaxGuidance = 100.0f;
 
 // One step of generate_streams over `rows` rows on the decode kernel: each row on its stream's slot (or the scratch
 // slot once the stream is done), its logits into row r of d_slogits. row_stream: the stream record of each row.
@@ -1213,10 +1216,12 @@ struct StepFlags {
     // overrides and masks edit d_slogits; top: the stride of the top arrays
     bool scored = false, spec_scored = false, raw = false, raw_copy = false;
     int top = 0;
+    // guided: some stream has a guidance slot (k_gen_guide edits its row before the pick chain)
+    bool guided = false;
 };
 
-// Raw log-probabilities read a copy of the model's rows when the pick chain edits d_slogits.
-void set_raw_copy(StepFlags &f) { f.raw_copy = f.raw && (f.pen || f.n_override || f.constrained); }
+// Raw log-probabilities read a copy of the model's rows when the guidance or the pick chain edits d_slogits.
+void set_raw_copy(StepFlags &f) { f.raw_copy = f.raw && (f.pen || f.n_override || f.constrained || f.guided); }
 
 // What a one-shot decoding call (generate() and speculate()) does besides emitting tokens: score them (lpq), follow
 // token automata (cq) and stop sets (sq), and count penalties; each request is NULL when the call has none. Built by
@@ -1295,6 +1300,9 @@ struct StepArgs {
     rk::SpecArgs sa;
     rk::GenFeedbackArgs fb;
     float *raw;
+    // classifier-free guidance: n_guide guided rows of the step, each with its GenGuide (generate() sets them per group)
+    const rk::GenGuide *guide;
+    int n_guide;
 };
 
 // The arguments every step of a call or batcher group shares, over the buffers of `sb` as its upload readied them:
@@ -1363,8 +1371,9 @@ void step_args(M *m, StepBuffers &sb, const StepFlags &f, unsigned long long max
 // speculative streams; the forward, on the tensor cores (fwd_rows tokens in passes of per_pass at `passes`, heads[i]
 // head rows in pass i; heads NULL: every row a head row, whose head maps k_spec_draft writes) or, with passes NULL, on
 // the decode kernel; nothing more when the step has no logits rows; the raw copy and the pick chain over `rows` rows
-// with uniforms u; k_gen_logprob and k_gen_feedback over the a.fb.rows one-token rows (rows 0..); k_spec_accept, then
-// k_spec_logprob over n_spec x (a.sa.k + 1) rows.
+// with uniforms u, after k_gen_guide over the a.n_guide guided rows (their guidance rows follow the `rows` rows);
+// k_gen_logprob and k_gen_feedback over the a.fb.rows one-token rows (rows 0..), then k_gen_guide_feedback;
+// k_spec_accept, then k_spec_logprob over n_spec x (a.sa.k + 1) rows.
 int run_step(M *m, const StepFlags &f, StepArgs &a, const rk::PassDesc *passes, int fwd_rows, int per_pass, const int *heads,
              int rows, int n_spec, const double *u) {
     const int plain = a.fb.rows;
@@ -1377,6 +1386,11 @@ int run_step(M *m, const StepFlags &f, StepArgs &a, const rk::PassDesc *passes, 
     if (rc || rows == 0) return rc;
     if (a.raw)
         CK(cudaMemcpyAsync(a.raw, m->d_slogits, (size_t)rows * binfmt::kVocab * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
+    if (a.n_guide) {
+        const dim3 grid((unsigned)((binfmt::kVocab + rk::kGuideThreads - 1) / rk::kGuideThreads), (unsigned)a.n_guide);
+        rk::k_gen_guide<<<grid, rk::kGuideThreads, 0, m->stream>>>(m->d_slogits, (int)binfmt::kVocab, rows, a.guide);
+        LAUNCHED(m);
+    }
     if ((rc = pick_rows(m, a.pc, rows, u))) return rc;
     if (f.scored && plain) {
         rk::k_gen_logprob<<<(unsigned)plain, rk::kNucThreads, 0, m->stream>>>(a.la);
@@ -1384,6 +1398,11 @@ int run_step(M *m, const StepFlags &f, StepArgs &a, const rk::PassDesc *passes, 
     }
     if (plain) {
         rk::k_gen_feedback<<<(unsigned)((plain + 127) / 128), 128, 0, m->stream>>>(a.fb);
+        LAUNCHED(m);
+    }
+    if (a.n_guide) {
+        rk::k_gen_guide_feedback<<<(unsigned)((a.n_guide + 127) / 128), 128, 0, m->stream>>>(a.fb.gs, a.fb.row_stream, plain,
+                                                                                            a.n_guide, a.guide, a.fb.passes);
         LAUNCHED(m);
     }
     if (n_spec) {
@@ -1442,48 +1461,104 @@ int finish_features(M *m, CallFeatures &f, const GenCall &c) {
     return 0;
 }
 
+// The guidance of a guided call, refused before any work: NULL slots, NULL first tokens or scales while a slot is named,
+// a guidance slot out of range, repeated or equal to a stream's slot, a first token out of the vocabulary, and a scale
+// that is not finite or outside [0, 100]. The stream slots are checked already.
+int check_guidance(M *m, const char *what, const GenCall &c, const rwkv_b200_guidance &gd) {
+    if (!gd.slots) return fail(1, "%s: guidance with NULL slots", what);
+    std::vector<char> used(m->max_gpt, 0); // 1: a stream's slot, 2: a guidance slot
+    for (unsigned long long s = 0; s < c.n_streams; ++s) used[c.slots[s]] = 1;
+    for (unsigned long long s = 0; s < c.n_streams; ++s) {
+        const unsigned long long g = gd.slots[s];
+        if (g == RWKV_B200_NO_GUIDANCE) continue;
+        if (!gd.first_tokens || !gd.scales)
+            return fail(1, "%s: stream %llu names guidance slot %llu with NULL first_tokens or scales", what, s, g);
+        if (g >= m->max_gpt) return fail(1, "%s: stream %llu: guidance slot %llu >= max_gpt %llu", what, s, g, m->max_gpt);
+        if (used[g] == 1) return fail(1, "%s: stream %llu: guidance slot %llu is the slot of a stream", what, s, g);
+        if (used[g] == 2) return fail(1, "%s: stream %llu: guidance slot %llu appears twice", what, s, g);
+        used[g] = 2;
+        if (gd.first_tokens[s] >= binfmt::kVocab)
+            return fail(1, "%s: stream %llu: guidance first token %llu out of range", what, s, gd.first_tokens[s]);
+        const float w = gd.scales[s];
+        if (!(w >= 0.0f && w <= kMaxGuidance))
+            return fail(1, "%s: stream %llu: guidance scale %g is not a finite value in [0, %g]", what, s, w, kMaxGuidance);
+    }
+    return 0;
+}
+
 // The body of generate_streams (samplers == NULL, `temp` and `u` pick the typical sampler or the arg-max), of
 // generate_streams_ex (`ex`: every stream has its own sampler, or all pick the arg-max when samplers == NULL), of
 // generate_streams_logprobs (generate_streams_ex with `lpq`: each emitted token is scored after its pick) and of
 // generate_streams_constrained (with `cq`: token automata mask the rows after the overrides; `lpq` may be NULL) and of
-// generate_streams_stop (with `sq` as well: k_gen_feedback walks each emitted token through the stream's stop set).
+// generate_streams_stop (with `sq` as well: k_gen_feedback walks each emitted token through the stream's stop set) and
+// of generate_streams_guided (with `gd`: a guided stream's guidance row runs on its guidance slot in the same forward,
+// and k_gen_guide combines the two rows before the pick chain).
 int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, const LogprobRequest *lpq = nullptr,
-             const ConstraintRequest *cq = nullptr, const rwkv_b200_stop_request *sq = nullptr) {
+             const ConstraintRequest *cq = nullptr, const rwkv_b200_stop_request *sq = nullptr,
+             const rwkv_b200_guidance *gd = nullptr) {
     int rc = check_streams_model(m, what);
     if (rc) return rc;
     if (lpq && (rc = check_logprobs(what, *lpq))) return rc;
     if ((rc = check_gen(m, what, c, 1, ex))) return rc;
+    if (gd && (rc = check_guidance(m, what, c, *gd))) return rc;
+    const unsigned long long n_streams = c.n_streams, max_new = c.max_new;
+    // every slot the call names: the streams', then the guidance slots (stream record n_streams + j: guided stream j)
+    std::vector<unsigned long long> named(c.slots, c.slots + n_streams);
+    std::vector<int> guide_rec(n_streams, -1);
+    for (unsigned long long s = 0; gd && s < n_streams; ++s)
+        if (gd->slots[s] != RWKV_B200_NO_GUIDANCE) {
+            guide_rec[s] = (int)named.size();
+            named.push_back(gd->slots[s]);
+        }
+    const unsigned long long n_rec = named.size();
     bool bound;
-    if ((rc = set_pass_adapters(m, what, c.slots, c.n_streams, bound))) return rc;
+    if ((rc = set_pass_adapters(m, what, named.data(), n_rec, bound))) return rc;
     CallFeatures f;
     if ((rc = check_features(m, what, c, lpq, cq, sq, f))) return rc;
-    const unsigned long long n_streams = c.n_streams, max_new = c.max_new;
+    f.guided = n_rec > n_streams;
+    set_raw_copy(f);
     CK(cudaSetDevice(m->device));
     auto &g = m->gen;
     if (c.u && (rc = g.u.grow(kGenGroup * m->max_gpt))) return rc;
-    // the path is chosen once, for n_streams tokens; a stream's numbers depend only on its row
-    const bool tc = tensor_cores(m, n_streams, bound);
+    if (f.guided && (rc = g.guide.grow(n_rec - n_streams))) return rc;
+    // the path is chosen once, for the rows of every stream and guidance slot; a stream's numbers depend only on its row
+    const bool tc = tensor_cores(m, n_rec, bound);
     if (tc && (rc = rk::prefill_init(m->pf, m->p))) return fail(rc, "%s", rk::prefill_error());
     m->stream_rows = 0; // the compact logits rows no longer belong to a call the caller made
 
     rk::GenStream *hg = m->h_gs;
-    for (unsigned long long s = 0; s < n_streams; ++s)
+    for (unsigned long long s = 0; s < n_streams; ++s) {
         hg[s] = rk::GenStream{c.slots[s], c.budgets ? c.budgets[s] : max_new, c.first_tokens[s], 0, 0};
-    CK(cudaMemcpyAsync(g.gs.p, hg, n_streams * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
+        if (guide_rec[s] >= 0) hg[guide_rec[s]] = rk::GenStream{gd->slots[s], hg[s].budget, gd->first_tokens[s], 0, 0};
+    }
+    CK(cudaMemcpyAsync(g.gs.p, hg, n_rec * sizeof(rk::GenStream), cudaMemcpyHostToDevice, m->stream));
     if ((rc = upload_gen(m, c)) || (rc = upload_features(m, f, n_streams, n_streams))) return rc;
-    std::vector<int> live(n_streams);
+    std::vector<int> live(n_streams), rs;
     for (unsigned long long s = 0; s < n_streams; ++s) live[s] = (int)s;
     std::vector<double> ug;
+    std::vector<rk::GenGuide> guide;
     StepArgs a;
     step_args(m, g, f, max_new, c.n_stop, a);
     a.pc.exponent = sample_exponent(temp);
     a.fb.passes = tc ? g.passes.p : nullptr;
+    a.guide = g.guide.p;
     for (unsigned long long step = 0; !live.empty() && step < max_new;) {
-        // a group: the live streams are rows 0..rows-1; their inputs, and the uniforms of its steps, go up once
+        // a group: the live streams are rows 0..rows-1, then the guidance rows of the live guided streams; their
+        // inputs, and the uniforms of its steps, go up once
         const int rows = (int)live.size();
         const unsigned long long steps = std::min(kGenGroup, max_new - step);
-        CK(cudaMemcpyAsync(g.row_stream.p, live.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-        if (tc && (rc = upload_step_passes(m, live.data(), rows))) return rc;
+        rs = live;
+        guide.clear();
+        for (int r = 0; r < rows; ++r)
+            if (guide_rec[live[r]] >= 0) {
+                rs.push_back(guide_rec[live[r]]);
+                guide.push_back(rk::GenGuide{r, gd->scales[live[r]]});
+            }
+        const int fwd_rows = (int)rs.size();
+        CK(cudaMemcpyAsync(g.row_stream.p, rs.data(), fwd_rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        if (!guide.empty())
+            CK(cudaMemcpyAsync(g.guide.p, guide.data(), guide.size() * sizeof(rk::GenGuide), cudaMemcpyHostToDevice, m->stream));
+        if (tc && (rc = upload_step_passes(m, rs.data(), fwd_rows))) return rc;
         if (c.u) {
             ug.resize((size_t)steps * rows);
             for (unsigned long long k = 0; k < steps; ++k)
@@ -1491,11 +1566,13 @@ int generate(M *m, const char *what, bool ex, const GenCall &c, float temp, cons
             CK(cudaMemcpyAsync(g.u.p, ug.data(), ug.size() * sizeof(double), cudaMemcpyHostToDevice, m->stream));
         }
         a.fb.rows = rows;
+        a.n_guide = (int)guide.size();
         for (unsigned long long k = 0; k < steps; ++k)
-            if ((rc = run_step(m, f, a, a.fb.passes, rows, rk::kPfMaxTokens, nullptr, rows, 0, c.u ? g.u.p + k * rows : nullptr)))
+            if ((rc = run_step(m, f, a, a.fb.passes, fwd_rows, rk::kPfMaxTokens, nullptr, rows, 0, c.u ? g.u.p + k * rows : nullptr)))
                 return rc;
-        // the end of a group: which streams are done (a few bytes, one synchronisation); drop them from the rows
-        if ((rc = end_group(m, what, f, hg, g.gs.p, n_streams * sizeof(rk::GenStream)))) return rc;
+        // the end of a group: which streams are done (a few bytes, one synchronisation); drop them (and their guidance
+        // rows) from the rows
+        if ((rc = end_group(m, what, f, hg, g.gs.p, n_rec * sizeof(rk::GenStream)))) return rc;
         step += steps;
         live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hg[s].done != 0; }), live.end());
     }
@@ -2687,6 +2764,25 @@ int rwkv_b200_generate_streams_stop(rwkv_b200_model *m, const unsigned long long
     const ConstraintRequest cq{constraint_ids, start_states, states_out};
     return generate(m, stop ? "generate_streams_stop" : "generate_streams_constrained", true, c, 1.0f,
                     logprobs_out ? &lpq : nullptr, &cq, stop);
+}
+
+int rwkv_b200_generate_streams_guided(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
+                                      unsigned long long n_streams, unsigned long long max_new, const unsigned long long *budgets,
+                                      const unsigned long long *stop_tokens, unsigned long long n_stop,
+                                      const unsigned long long *override_tokens, const float *override_values,
+                                      unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u,
+                                      unsigned long long *tokens_out, unsigned long long *lengths_out, int logprob_mode,
+                                      unsigned int top_n, double *logprobs_out, unsigned long long *ranks_out,
+                                      unsigned long long *top_tokens_out, double *top_logprobs_out,
+                                      const unsigned long long *constraint_ids, const unsigned long long *start_states,
+                                      unsigned long long *states_out, const rwkv_b200_stop_request *stop,
+                                      const rwkv_b200_guidance *guidance) {
+    const GenCall c{slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values,
+                    n_override, samplers, samplers ? u : nullptr, tokens_out, lengths_out};
+    const LogprobRequest lpq{logprob_mode, top_n, logprobs_out, ranks_out, top_tokens_out, top_logprobs_out};
+    const ConstraintRequest cq{constraint_ids, start_states, states_out};
+    const char *what = guidance ? "generate_streams_guided" : stop ? "generate_streams_stop" : "generate_streams_constrained";
+    return generate(m, what, true, c, 1.0f, logprobs_out ? &lpq : nullptr, &cq, stop, guidance);
 }
 
 // Beam search: generate()'s group loop over beams. Step 0 has one row per group, later steps B rows per live group

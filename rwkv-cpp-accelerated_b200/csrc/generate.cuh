@@ -11,7 +11,9 @@
 // stream's token automaton (GenConstraint) after appending its token. generate_streams_stop has k_gen_feedback walk each
 // emitted token's bytes through the stream's stop-string automaton (GenStop) as well. The rule that appends a token and
 // decides whether it ends its stream is gen_emit, over the arguments in GenEmit; k_spec_accept (speculate.cuh) emits its
-// accepted tokens by the same function.
+// accepted tokens by the same function. generate_streams_guided adds a guidance row per guided stream after the
+// streams' rows: k_gen_guide combines each pair of rows before the pick chain, and k_gen_guide_feedback feeds the
+// stream's emitted token to its guidance row after k_gen_feedback.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -208,6 +210,51 @@ __global__ void k_gen_feedback(const GenFeedbackArgs a) {
         const int t = r % kPfMaxTokens;
         pd.tokens[t] = g.tok;
         pd.desc[t] = (uint32_t)g.slot | kDescFirst | (g.done ? 0u : kDescLast);
+    }
+}
+
+// Classifier-free guidance (rwkv_b200_generate_streams_guided). A guided stream has a second stream record, its
+// guidance record: the guidance slot, and as tok the guidance first token, then the token the stream emitted last.
+// A step's rows are the `rows` conditional rows (the pick chain's), then one guidance row per live guided stream, in
+// the order of their conditional rows. Guided row j has its conditional row and scale gamma in GenGuide j, and its
+// guidance row is rows + j. Gate and passes read the guidance rows' records like any other row's.
+struct GenGuide {
+    int row;     // the stream's conditional row
+    float scale; // gamma
+};
+
+// Rule 2 of include/rwkv_b200.h on guided row j, in place on its conditional row c with guidance row q:
+// c[v] + (gamma - 1) * (c[v] - q[v]), each operation rounded to nearest f32 and none fused. Grid
+// (ceil(V / kGuideThreads), guided rows), one thread per token.
+constexpr int kGuideThreads = 256;
+__global__ void __launch_bounds__(kGuideThreads) k_gen_guide(float *logits, int V, int rows, const GenGuide *guide) {
+    const int j = blockIdx.y, v = blockIdx.x * kGuideThreads + threadIdx.x;
+    if (v >= V) return;
+    const GenGuide g = guide[j];
+    float *c = logits + (size_t)g.row * V + v;
+    const float q = logits[(size_t)(rows + j) * V + v];
+    const float w = __fsub_rn(g.scale, 1.0f);
+    *c = __fadd_rn(*c, __fmul_rn(w, __fsub_rn(*c, q)));
+}
+
+// After k_gen_feedback, one thread per guided row j: the guidance record takes the stream's emitted token and done
+// flag, so the guidance slot is fed what the stream emitted and is frozen with it. On the tensor-core path the
+// guidance row's token and descriptor go into the next step's passes (a finished stream's loses kDescLast). A separate
+// launch, so that k_gen_feedback has written every stream record before it is read here.
+__global__ void k_gen_guide_feedback(GenStream *gs, const int *row_stream, int rows, int n_guide, const GenGuide *guide,
+                                     PassDesc *passes) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n_guide) return;
+    const int r = rows + j;
+    const GenStream c = gs[row_stream[guide[j].row]];
+    GenStream &g = gs[row_stream[r]];
+    g.tok = c.tok;
+    g.done = c.done;
+    if (passes) {
+        PassDesc &pd = passes[r / kPfMaxTokens];
+        const int t = r % kPfMaxTokens;
+        pd.tokens[t] = c.tok;
+        pd.desc[t] = (uint32_t)g.slot | kDescFirst | (c.done ? 0u : kDescLast);
     }
 }
 

@@ -21,6 +21,7 @@ INDEX_L1, INDEX_L2 = 0, 1                # RWKV_B200_INDEX_*: the metric a State
 MAX_NEIGHBOURS = 256                     # RWKV_B200_MAX_NEIGHBOURS
 NO_ENTRY = 0xFFFFFFFFFFFFFFFF            # RWKV_B200_NO_ENTRY: a search position past the entries found
 NO_ADAPTER = 0xFFFFFFFFFFFFFFFF          # RWKV_B200_NO_ADAPTER: Engine.bind_adapter(slot, None)
+NO_GUIDANCE = 0xFFFFFFFFFFFFFFFF         # RWKV_B200_NO_GUIDANCE: an unguided stream of generate_streams(guidance=...)
 MAX_ADAPTER_RANK = 64                    # RWKV_B200_MAX_ADAPTER_RANK
 # RWKV_B200_AD_* in order: the checkpoint's Linear name inside a block of each projection an adapter may adapt
 ADAPTER_MATRICES = ("att.key", "att.value", "att.receptance", "att.output", "ffn.key", "ffn.value", "ffn.receptance")
@@ -71,6 +72,34 @@ class StopRequest(ctypes.Structure):
     """rwkv_b200_stop_request: per stream its stop set id and start state, and where the results go."""
     P = ctypes.POINTER(ctypes.c_ulonglong)
     _fields_ = [("set_ids", P), ("start_states", P), ("states_out", P), ("hit_out", P), ("tail_out", P)]
+
+
+class Guidance(ctypes.Structure):
+    """rwkv_b200_guidance: per stream its guidance slot (or NO_GUIDANCE), guidance first token and scale gamma."""
+    _fields_ = [("slots", ctypes.POINTER(ctypes.c_ulonglong)), ("first_tokens", ctypes.POINTER(ctypes.c_ulonglong)),
+                ("scales", ctypes.POINTER(ctypes.c_float))]
+
+
+def guide_rows(c, q, scale):
+    """Rule 2 of classifier-free guidance (include/rwkv_b200.h) in numpy: c + (scale - 1) * (c - q) in float32, each
+    operation rounded once, with w = scale - 1 itself rounded to float32. c, q: the conditional and guidance logits."""
+    c = np.asarray(c, np.float32)
+    q = np.asarray(q, np.float32)
+    w = np.float32(np.float32(scale) - np.float32(1.0))
+    return c + w * (c - q)
+
+
+def _guidance(guidance, S, what):
+    """The Guidance struct of one entry per stream: None, or (slot, first_token, scale)."""
+    spec = list(guidance)
+    if len(spec) != S:
+        raise EngineError("%s: %d guidance entries for %d streams" % (what, len(spec), S))
+    slots = np.ascontiguousarray([NO_GUIDANCE if g is None else int(g[0]) for g in spec], np.uint64)
+    first = np.ascontiguousarray([0 if g is None else int(g[1]) for g in spec], np.uint64)
+    scales = np.ascontiguousarray([1.0 if g is None else float(g[2]) for g in spec], np.float32)
+    gd = Guidance(_ptr(slots, ctypes.c_ulonglong), _ptr(first, ctypes.c_ulonglong), _ptr(scales, ctypes.c_float))
+    gd._keep = (slots, first, scales)
+    return gd
 
 
 class PrefixStats(ctypes.Structure):
@@ -413,6 +442,9 @@ def load_library():
         "rwkv_b200_generate_streams_stop": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull,
                                                   c.POINTER(Sampler), pdbl, pull, pull, i32, c.c_uint, pdbl, pull, pull,
                                                   pdbl, pull, pull, pull, c.POINTER(StopRequest)]),
+        "rwkv_b200_generate_streams_guided": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull,
+                                                    c.POINTER(Sampler), pdbl, pull, pull, i32, c.c_uint, pdbl, pull, pull,
+                                                    pdbl, pull, pull, pull, c.POINTER(StopRequest), c.POINTER(Guidance)]),
         "rwkv_b200_generate_streams_speculative_stop": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull,
                                                               c.POINTER(Sampler), pdbl, pull, pull, c.c_uint, c.c_uint,
                                                               pull, pull, pull, c.POINTER(StopRequest)]),
@@ -593,7 +625,7 @@ class Engine:
         return toks, margins
 
     def generate_streams(self, streams, max_new, budgets=None, stop=(), overrides=None, temp=None, u=None, sampling=None,
-                         logprobs=None, top_n=0, constraints=None, stop_strings=None):
+                         logprobs=None, top_n=0, constraints=None, stop_strings=None, guidance=None):
         """Generate up to max_new tokens per stream on the device: streams = [(slot, first_token), ...].
         Arg-max when u is None, else the typical sampler with u[step][stream] and temp (default 1.0). budgets: tokens
         per stream (None = max_new each); stop: token ids that end a stream (emitted, not fed); overrides = {token:
@@ -614,10 +646,23 @@ class Engine:
         (rwkv_b200_generate_streams_stop: a stream ends after the token whose bytes complete one of its set's strings).
         Then it returns one dict per stream with "tokens", "stop_hit" (the index of the matched string, or None),
         "stop_tail" (bytes of the last token after the match) and "stop_state" (the final match state, None without a
-        set), plus the logprob and constraint fields when those are given. It needs sampling=... or the arg-max too."""
-        if logprobs is not None or constraints is not None or stop_strings is not None:
+        set), plus the logprob and constraint fields when those are given. It needs sampling=... or the arg-max too.
+        guidance: classifier-free guidance, one entry per stream: None, or (slot, first_token, scale)
+        (rwkv_b200_generate_streams_guided). Each step also runs the guidance slot on first_token, then on the token the
+        stream emitted last, and the stream picks from c + (scale - 1) * (c - q) (guide_rows) of its own row c and the
+        guidance row q. The return shapes stay as above; it needs sampling=... or the arg-max too. Three uses:
+
+            # a negative prompt: its state on slot 9, its last token fed by the call
+            eng.slot_zero(9); eng.forward_streams([(9, neg[:-1])], want_logits=False)
+            eng.generate_streams([(0, tok)], 64, guidance=[(9, neg[-1], 1.5)])
+            # unconditional guidance: an empty context on a zeroed slot, token 0
+            eng.slot_zero(9); eng.generate_streams([(0, tok)], 64, guidance=[(9, 0, 1.5)])
+            # adapter contrast: slot 0 bound to a fine-tune, its copy on slot 9 to the base model
+            eng.slot_copy(0, 9); eng.bind_adapter(0, ft); eng.bind_adapter(9, None)
+            eng.generate_streams([(0, tok)], 64, guidance=[(9, tok, 2.0)])"""
+        if logprobs is not None or constraints is not None or stop_strings is not None or guidance is not None:
             return self._generate_scored(streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n,
-                                         constraints, stop_strings)
+                                         constraints, stop_strings, guidance)
         temp = 1.0 if temp is None else temp
         S, lead, tail, out, lens = _gen_args(streams, max_new, budgets, stop, overrides, u)
         if sampling is not None:
@@ -628,12 +673,15 @@ class Engine:
         return [out[s, :int(lens[s])].copy() for s in range(S)]
 
     def _generate_scored(self, streams, max_new, budgets, stop, overrides, temp, u, sampling, logprobs, top_n, constraints,
-                         stop_strings=None):
-        """generate_streams with logprobs, constraints or stop strings: rwkv_b200_generate_streams_stop with stop
-        strings, rwkv_b200_generate_streams_constrained with constraints, else rwkv_b200_generate_streams_logprobs. One
-        dict per stream."""
+                         stop_strings=None, guidance=None):
+        """generate_streams with logprobs, constraints, stop strings or guidance: rwkv_b200_generate_streams_guided with
+        guidance, rwkv_b200_generate_streams_stop with stop strings, rwkv_b200_generate_streams_constrained with
+        constraints, else rwkv_b200_generate_streams_logprobs. One dict per stream, or with guidance alone one array."""
         _logprob_mode(logprobs, "generate_streams")
         if sampling is None and (u is not None or temp is not None):
+            if guidance is not None:
+                raise EngineError("generate_streams: guidance needs sampling=... (or neither u nor temp, for the arg-max); "
+                                  "the typical sampler does not take it")
             if stop_strings is not None:
                 raise EngineError("generate_streams: stop_strings need sampling=... (or neither u nor temp, for the "
                                   "arg-max); the typical sampler does not take them")
@@ -648,6 +696,13 @@ class Engine:
         args = (self.h, *lead, sp, *tail, *lp_args)
         if stop_strings is not None:
             sreq, sres = self._stop_request(stop_strings, S, "generate_streams")
+        if guidance is not None:
+            gd = _guidance(guidance, S, "generate_streams")
+            self._ck(self.lib.rwkv_b200_generate_streams_guided(*args, *cargs, ctypes.byref(sreq) if stop_strings is not None
+                                                                else None, ctypes.byref(gd)), "generate_streams_guided")
+            if logprobs is None and constraints is None and stop_strings is None:
+                return [out[s, :int(lens[s])].copy() for s in range(S)]
+        elif stop_strings is not None:
             self._ck(self.lib.rwkv_b200_generate_streams_stop(*args, *cargs, ctypes.byref(sreq)), "generate_streams_stop")
         elif constraints is not None:
             self._ck(self.lib.rwkv_b200_generate_streams_constrained(*args, *cargs), "generate_streams_constrained")
