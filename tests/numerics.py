@@ -401,6 +401,13 @@ BENCH_CASES = {"7b": {"decode": 16, "tc": 64, "greedy": 32}, "14b": {"decode": 8
 SWITCH = (200, 24, 40)   # 1b5: tensor cores, then the decode kernel, then tensor cores again, on one state
 
 
+def wide_streams(E):
+    """(case ids, streams) of the single-stream cases of width E of WIDE, each from the zero state."""
+    from util import token_stream
+    ids = ["%s-%dx%d" % (p, DEPTH_L, E) for p in WIDE[E]]
+    return ids, [token_stream(T, seed=E + i) for i, T in enumerate(WIDE[E].values())]
+
+
 def depth_passes(group, model, greedy=None):
     """The restatement passes of a group (a width of WIDE or a workload of BENCH_CASES), in order: a list of
     (case ids, streams, initial states or None). A "ragged-2" pass starts from the state a "ragged-1" pass ends in,
@@ -408,8 +415,7 @@ def depth_passes(group, model, greedy=None):
     device (the reference's greedy tokens where no device ran, on the host)."""
     from util import reference_golden, token_stream
     if group in WIDE:
-        ids = ["%s-%dx%d" % (p, DEPTH_L, group) for p in WIDE[group]]
-        streams = [token_stream(T, seed=group + i) for i, T in enumerate(WIDE[group].values())]
+        ids, streams = wide_streams(group)
         if group != 4096:
             return [(ids, streams, None)]
         pre = forward(model, [token_stream(3, seed=100 + i) for i in range(len(RAGGED_SLOTS))])[1]
