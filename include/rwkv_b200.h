@@ -762,6 +762,48 @@ int rwkv_b200_generate_streams_speculative_constrained(
     const unsigned long long *constraint_ids, const unsigned long long *start_states, unsigned long long *states_out,
     const rwkv_b200_stop_request *stop);
 
+/* Speculative generation with a draft model: rwkv_b200_generate_streams_speculative_constrained with the prompt-lookup
+ * drafts replaced by the picks of a second, smaller model of the same vocabulary (e.g. RWKV-4 169M drafting for 7B).
+ * Every argument keeps that call's meaning (slots [n_streams][draft + 1], first tokens, budgets, stops, overrides,
+ * samplers, u, steps_out, log-probabilities, automata and stop strings; NULL logprobs_out, constraint_ids and stop switch
+ * those off); ngram, context_start and context give way to `drafter`.
+ * The drafter names the draft model and two of its slots per stream, slots [n_streams][2] = {D0, D1}. D0 holds the draft
+ * model's state over the same tokens as the stream's first target slot (the caller primes it, e.g. with forward_streams
+ * of the same prompt on both models); D1 is scratch.
+ * The drafts. x is a step's input. The draft model feeds x on top of the stream's draft state; the pick on that row is
+ * d_1. It then feeds d_1, ..., d_(k-1) one at a time; the pick after feeding d_(i-1) is d_i. Pick i (1-based) takes the
+ * call's overrides, then, with a token automaton, the mask of r_(i-1), the state target row i - 1 has by the speculative
+ * automaton rule above (a dead row is not masked), then the stream's sampler with the uniform of target row i - 1,
+ * u[(len + i - 1) * n_streams + s] (0 when len + i - 1 reaches the budget; temperature 0 is the arg-max). Because the
+ * draft shares the target's uniforms, a draft model close to the target proposes the token the target will sample.
+ * Verification and emission are the speculative rule's, so the tokens, lengths, the first target slots' xy, aa, bb and
+ * dd, log-probabilities, automaton and stop states are bit for bit rwkv_b200_generate_streams_stop with the same features
+ * on the tensor cores, whatever the draft model is. The draft logits are bit for bit rwkv_b200_forward_streams of the
+ * same tokens on the draft model on the tensor cores, so a host loop of that call and the pick chain restates steps_out.
+ * D0 ends bit for bit as the draft model's forward_streams over exactly the tokens the first target slot absorbed in the
+ * call, from its starting state, so the next call (the next turn of a chat) reuses the pair (first slot, D0). D1's
+ * contents after the call are unspecified; no other draft slot and nothing else of the draft model's state is written.
+ * Adapters bound to draft slots apply as in any forward. Both models' work is enqueued on the target's CUDA stream.
+ * Refused before any work, with every slot of both models untouched: every refusal of
+ * rwkv_b200_generate_streams_speculative_constrained (penalties included); a NULL drafter, drafter->model or
+ * drafter->slots; a draft model that is the target model, on another device, tensor-parallel or with "prefill" 0; a draft
+ * slot >= the draft's max_gpt or repeated; the two draft slots of a stream bound to different adapters; and n_streams x 2
+ * > the draft's max_gpt. */
+typedef struct rwkv_b200_drafter {
+    rwkv_b200_model *model;          /* the draft model */
+    const unsigned long long *slots; /* [n_streams][2]: D0, D1 of each stream, slots of the draft model */
+} rwkv_b200_drafter;
+
+int rwkv_b200_generate_streams_drafted(
+    rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens, unsigned long long n_streams,
+    unsigned long long max_new, const unsigned long long *budgets, const unsigned long long *stop_tokens,
+    unsigned long long n_stop, const unsigned long long *override_tokens, const float *override_values,
+    unsigned long long n_override, const rwkv_b200_sampler *samplers, const double *u, unsigned long long *tokens_out,
+    unsigned long long *lengths_out, unsigned int draft, const rwkv_b200_drafter *drafter, unsigned long long *steps_out,
+    int logprob_mode, unsigned int top_n, double *logprobs_out, unsigned long long *ranks_out,
+    unsigned long long *top_tokens_out, double *top_logprobs_out, const unsigned long long *constraint_ids,
+    const unsigned long long *start_states, unsigned long long *states_out, const rwkv_b200_stop_request *stop);
+
 /* rwkv_b200_batcher_submit_ex (x may be NULL) with a stop set: set_id (RWKV_B200_NO_STOP_SET: exactly submit_ex) and its
  * start state. The batcher rule's step 2 becomes rwkv_b200_generate_streams_stop of the one stream with the set and start
  * state; a request whose stop string matches ends as RWKV_B200_REQ_DONE. Refused as well, with nothing queued: an unknown

@@ -127,6 +127,7 @@ struct StepBuffers {
     DevBuf<unsigned long long> hist, row_state, forks;
     DevBuf<double> su;
     DevBuf<rk::GenGuide> guide;        // [rows] each guided row's conditional row and scale (generate_streams_guided)
+    DevBuf<rk::SpecDraft> ds;          // [streams] a draft model's records of a drafted call (generate_streams_drafted)
 };
 
 } // namespace
@@ -1293,6 +1294,8 @@ int upload_features(M *m, const CallFeatures &f, unsigned long long n_streams, s
     return 0;
 }
 
+struct DraftStep;
+
 // The arguments of a step's kernels; `raw` is where the step copies its model rows (nullptr: no copy).
 struct StepArgs {
     PickChain pc;
@@ -1303,6 +1306,8 @@ struct StepArgs {
     // classifier-free guidance: n_guide guided rows of the step, each with its GenGuide (generate() sets them per group)
     const rk::GenGuide *guide;
     int n_guide;
+    // speculative streams whose drafts come from a draft model (generate_streams_drafted); nullptr: prompt lookup
+    DraftStep *draft;
 };
 
 // The arguments every step of a call or batcher group shares, over the buffers of `sb` as its upload readied them:
@@ -1368,21 +1373,29 @@ void step_args(M *m, StepBuffers &sb, const StepFlags &f, unsigned long long max
 }
 
 // One decoding step of generate(), speculate() and the batcher, enqueued in this order: k_spec_draft over n_spec
-// speculative streams; the forward, on the tensor cores (fwd_rows tokens in passes of per_pass at `passes`, heads[i]
+// speculative streams (with a.draft: draft_step, then k_spec_layout); the forward, on the tensor cores (fwd_rows tokens in passes of per_pass at `passes`, heads[i]
 // head rows in pass i; heads NULL: every row a head row, whose head maps k_spec_draft writes) or, with passes NULL, on
 // the decode kernel; nothing more when the step has no logits rows; the raw copy and the pick chain over `rows` rows
 // with uniforms u, after k_gen_guide over the a.n_guide guided rows (their guidance rows follow the `rows` rows);
 // k_gen_logprob and k_gen_feedback over the a.fb.rows one-token rows (rows 0..), then k_gen_guide_feedback;
 // k_spec_accept, then k_spec_logprob over n_spec x (a.sa.k + 1) rows.
+int draft_step(const DraftStep &d);
+
 int run_step(M *m, const StepFlags &f, StepArgs &a, const rk::PassDesc *passes, int fwd_rows, int per_pass, const int *heads,
              int rows, int n_spec, const double *u) {
     const int plain = a.fb.rows;
+    int rc;
     if (n_spec) {
         a.sa.heads = heads == nullptr;
-        rk::k_spec_draft<<<(unsigned)n_spec, rk::kSpecDraftThreads, 0, m->stream>>>(a.sa);
+        if (a.draft) {
+            if ((rc = draft_step(*a.draft))) return rc;
+            rk::k_spec_layout<<<(unsigned)n_spec, 32, 0, m->stream>>>(a.sa);
+        } else {
+            rk::k_spec_draft<<<(unsigned)n_spec, rk::kSpecDraftThreads, 0, m->stream>>>(a.sa);
+        }
         LAUNCHED(m);
     }
-    int rc = passes ? gen_step_passes(m, passes, fwd_rows, per_pass, heads) : gen_step_decode(m, fwd_rows, a.pc.row_stream);
+    rc = passes ? gen_step_passes(m, passes, fwd_rows, per_pass, heads) : gen_step_decode(m, fwd_rows, a.pc.row_stream);
     if (rc || rows == 0) return rc;
     if (a.raw)
         CK(cudaMemcpyAsync(a.raw, m->d_slogits, (size_t)rows * binfmt::kVocab * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
@@ -1597,6 +1610,130 @@ struct SpecRequest {
     unsigned draft, ngram;
     const unsigned long long *context_start, *context;
     unsigned long long *steps_out;
+    const rwkv_b200_drafter *drafter; // generate_streams_drafted: the draft model instead of prompt lookup (no n-gram, no context)
+};
+
+// A drafted call's draft model and what each step enqueues there (speculate.cuh, "drafts from a draft model"): the
+// kernels' arguments, the pick chain on the draft's rows (the call's sampler, overrides and automata; the draft's row
+// map, row states and uniforms) and the head rows of each first pass.
+struct DraftStep {
+    M *dm = nullptr;
+    rk::DraftArgs da{};
+    PickChain pc{};
+    const double *row_u = nullptr;
+    std::vector<int> heads;
+};
+
+// One step's drafts on the draft model: k_draft_first, the first pass, then k times the pick chain and k_draft_pick,
+// with the one-token pass of the next draft between them.
+int draft_step(const DraftStep &d) {
+    M *dm = d.dm;
+    const rk::DraftArgs &da = d.da;
+    const int n = da.n, W = da.k + 2;
+    const unsigned blocks = (unsigned)((n + rk::kDraftThreads - 1) / rk::kDraftThreads);
+    rk::k_draft_first<<<blocks, rk::kDraftThreads, 0, dm->stream>>>(da);
+    LAUNCHED(dm);
+    int rc = gen_step_passes(dm, da.first, n * W, da.per_first * W, d.heads.data());
+    for (int i = 1; !rc && i <= da.k; ++i) {
+        if ((rc = pick_rows(dm, d.pc, n, d.row_u))) return rc;
+        rk::k_draft_pick<<<blocks, rk::kDraftThreads, 0, dm->stream>>>(da, i);
+        LAUNCHED(dm);
+        if (i < da.k) rc = gen_step_passes(dm, da.next, n, rk::kPfMaxTokens);
+    }
+    return rc;
+}
+
+// The drafter of a drafted call of S streams, refused before any work: a NULL handle, the target itself, another
+// device, tensor parallelism, "prefill" 0, draft slots out of range or repeated, and a stream whose two draft slots are
+// bound to different adapters. Then the draft's passes take its slots' adapters.
+int check_drafter(M *m, const char *what, const rwkv_b200_drafter *dr, unsigned long long S) {
+    if (!dr || !dr->model || !dr->slots) return fail(1, "%s: the drafter, its model or its slots is NULL", what);
+    M *dm = dr->model;
+    if (dm == m) return fail(1, "%s: the draft model is the target model", what);
+    if (dm->device != m->device)
+        return fail(1, "%s: the draft model is on device %d, the target on device %d", what, dm->device, m->device);
+    if (dm->tp_size > 1) return fail(7, "%s: the draft model uses tensor parallelism", what);
+    if (!rk::prefill_enabled(dm->pf)) return fail(1, "%s: the draft model needs the tensor cores (its \"prefill\" option is 0)", what);
+    if (S > dm->max_gpt / 2)
+        return fail(1, "%s: %llu streams x 2 draft slots > the draft model's max_gpt %llu", what, S, dm->max_gpt);
+    const std::string dwhat = std::string(what) + ": draft model";
+    int rc;
+    if ((rc = check_slots(dm, dwhat.c_str(), dr->slots, 2 * S))) return rc;
+    for (unsigned long long s = 0; s < S; ++s)
+        if ((rc = check_same_binding(dm, dwhat.c_str(), "stream", s, dr->slots + 2 * s, 2))) return rc;
+    bool bound;
+    return set_pass_adapters(dm, dwhat.c_str(), dr->slots, 2 * S, bound);
+}
+
+// The draft model's buffers of a drafted call, after step_args: its records (D0, D1, nothing fed), its passes zeroed
+// (k_draft_first and k_draft_pick fill tokens, descriptors and head maps only), D0 forked into D1, and the step's
+// arguments over them.
+int draft_setup(M *dm, const unsigned long long *slots, unsigned long long S, int k, const StepArgs &a, DraftStep &d) {
+    auto &dg = dm->gen;
+    const int per_first = rk::kPfMaxTokens / (k + 2), per_flush = rk::kPfMaxTokens / (k + 1);
+    const size_t n_first = (S + per_first - 1) / per_first, n_next = (S + rk::kPfMaxTokens - 1) / rk::kPfMaxTokens;
+    const size_t n_pass = std::max(n_first + n_next, (size_t)((S + per_flush - 1) / per_flush));
+    int rc;
+    if ((rc = dg.ds.grow(S)) || (rc = dm->spec_passes.grow(n_pass)) || (rc = dg.forks.grow(2 * S)) ||
+        (a.sa.u && (rc = dg.u.grow(S))) || (a.pc.gc && (rc = dg.row_state.grow(S))))
+        return rc;
+    if ((rc = rk::prefill_init(dm->pf, dm->p))) return fail(rc, "%s", rk::prefill_error());
+    dm->stream_rows = 0; // the draft's compact logits rows no longer belong to a call the caller made
+    CK(cudaMemsetAsync(dm->spec_passes.p, 0, n_pass * sizeof(rk::PassDesc), dm->stream));
+    std::vector<rk::SpecDraft> rec(S);
+    for (unsigned long long s = 0; s < S; ++s) rec[s] = rk::SpecDraft{slots[2 * s], slots[2 * s + 1], 0};
+    CK(cudaMemcpyAsync(dg.ds.p, rec.data(), S * sizeof(rk::SpecDraft), cudaMemcpyHostToDevice, dm->stream));
+    // the first step's input continues D0's state on D1: the pairs {D0, D1} are the fork's {source, destination}
+    CK(cudaMemcpyAsync(dg.forks.p, slots, 2 * S * sizeof(unsigned long long), cudaMemcpyHostToDevice, dm->stream));
+    if ((rc = fork_slots(dm, dg.forks.p, S, false))) return rc;
+    rk::DraftArgs &da = d.da;
+    da.ss = a.sa.ss;
+    da.live = a.sa.live;
+    da.ds = dg.ds.p;
+    da.hist = a.sa.hist;
+    da.first = dm->spec_passes.p;
+    da.next = dm->spec_passes.p + n_first;
+    da.k = k;
+    da.per_first = per_first;
+    da.pick_next = a.sa.next ? dm->d_next : nullptr;
+    da.pick_sample = dm->d_sample;
+    da.u = a.sa.u;
+    da.row_u = dg.u.p;
+    da.u_stride = a.sa.u_stride;
+    da.gc = a.pc.gc;
+    da.row_state = dg.row_state.p;
+    d.dm = dm;
+    d.pc = a.pc;
+    d.pc.row_stream = dg.row_stream.p;
+    d.pc.row_state = a.pc.gc ? dg.row_state.p : nullptr;
+    d.row_u = a.sa.u ? dg.u.p : nullptr;
+    return 0;
+}
+
+// The call's end on the draft model: one pass without logits absorbs each stream's remaining tokens into D0.
+int draft_flush(const DraftStep &d, unsigned long long S) {
+    M *dm = d.dm;
+    rk::DraftArgs da = d.da;
+    const int W = da.k + 1;
+    da.n = (int)S;
+    da.per_first = rk::kPfMaxTokens / W;
+    rk::k_draft_flush<<<(unsigned)((S + rk::kDraftThreads - 1) / rk::kDraftThreads), rk::kDraftThreads, 0, dm->stream>>>(da);
+    LAUNCHED(dm);
+    const std::vector<int> heads((S + da.per_first - 1) / da.per_first, 0);
+    return gen_step_passes(dm, da.first, (int)S * W, da.per_first * W, heads.data());
+}
+
+// A draft model's work goes on the target's CUDA stream while the loan lasts, so the two models' launches keep one
+// order without events or synchronisation.
+struct StreamLoan {
+    M *dm;
+    cudaStream_t own;
+    StreamLoan(M *d, cudaStream_t s) : dm(d), own(d ? d->stream : nullptr) {
+        if (dm) dm->stream = s;
+    }
+    ~StreamLoan() {
+        if (dm) dm->stream = own;
+    }
 };
 
 // Speculative generation: generate()'s group loop with k + 1 rows per live stream. Each step is k_spec_draft -> passes
@@ -1604,7 +1741,8 @@ struct SpecRequest {
 // come back and the finished streams leave the rows. At the end a stream whose home is a spare has it copied to its first
 // slot. With a stop request, k_spec_accept also walks each emitted token through the stream's stop set; with token
 // automata, k_spec_draft gives each row its state and k_spec_accept advances the automaton; with logprobs_out, each
-// emitted token is scored after k_spec_accept.
+// emitted token is scored after k_spec_accept. With sr.drafter (generate_streams_drafted) each step's drafts come from
+// the draft model's passes (draft_step) on this call's CUDA stream, and the call ends with draft_flush.
 int speculate(M *m, const char *what, const GenCall &c, const SpecRequest &sr, const LogprobRequest *lpq,
               const ConstraintRequest *cq, const rwkv_b200_stop_request *sq) {
     int rc = check_streams_model(m, what);
@@ -1612,7 +1750,8 @@ int speculate(M *m, const char *what, const GenCall &c, const SpecRequest &sr, c
     if (lpq && (rc = check_logprobs(what, *lpq))) return rc;
     const unsigned draft = sr.draft, ngram = sr.ngram;
     if (draft < 1 || draft > (unsigned)rk::kSpecMaxDraft) return fail(1, "%s: draft %u is outside 1..%d", what, draft, rk::kSpecMaxDraft);
-    if (ngram < 1 || ngram > (unsigned)rk::kSpecMaxNgram) return fail(1, "%s: ngram %u is outside 1..%d", what, ngram, rk::kSpecMaxNgram);
+    if (!sr.drafter && (ngram < 1 || ngram > (unsigned)rk::kSpecMaxNgram))
+        return fail(1, "%s: ngram %u is outside 1..%d", what, ngram, rk::kSpecMaxNgram);
     if (!rk::prefill_enabled(m->pf)) return fail(1, "%s: needs the tensor cores (the \"prefill\" option is 0)", what);
     const unsigned long long K1 = draft + 1ull, S = c.n_streams, max_new = c.max_new;
     if (S > m->max_gpt / K1)
@@ -1643,6 +1782,7 @@ int speculate(M *m, const char *what, const GenCall &c, const SpecRequest &sr, c
     }
     CallFeatures f;
     if ((rc = check_features(m, what, c, lpq, cq, sq, f))) return rc;
+    if (sr.drafter && (rc = check_drafter(m, what, sr.drafter, S))) return rc;
     const unsigned long long n_hist = n_ctx + S * (1 + max_new);
     CK(cudaSetDevice(m->device));
     auto &g = m->gen;
@@ -1690,6 +1830,13 @@ int speculate(M *m, const char *what, const GenCall &c, const SpecRequest &sr, c
     a.sa.passes = m->spec_passes.p;
     a.sa.u_stride = S;
     if (f.constrained) a.pc.row_state = g.row_state.p;
+    // a draft model works on this call's stream once its own earlier work is done
+    M *dm = sr.drafter ? sr.drafter->model : nullptr;
+    if (dm) CK(cudaStreamSynchronize(dm->stream));
+    StreamLoan loan(dm, m->stream);
+    DraftStep dstep;
+    if (dm && (rc = draft_setup(dm, sr.drafter->slots, S, (int)draft, a, dstep))) return rc;
+    a.draft = dm ? &dstep : nullptr;
     // each step emits at least one token per live stream, so max_new steps finish every stream
     for (unsigned long long step = 0; !live.empty() && step < max_new;) {
         const int n_live = (int)live.size(), rows = n_live * (int)K1;
@@ -1701,6 +1848,13 @@ int speculate(M *m, const char *what, const GenCall &c, const SpecRequest &sr, c
             lv[li] = rk::SpecLive{live[li], li * (int)K1, li / per_pass * rk::kPfMaxTokens + li % per_pass * (int)K1};
         CK(cudaMemcpyAsync(g.live.p, lv.data(), n_live * sizeof(rk::SpecLive), cudaMemcpyHostToDevice, m->stream));
         CK(cudaMemcpyAsync(g.row_stream.p, rs.data(), rows * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+        if (dm) { // draft row li is live stream live[li]'s; its first passes hold per_first streams each
+            CK(cudaMemcpyAsync(dm->gen.row_stream.p, live.data(), n_live * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+            const int pf = dstep.da.per_first;
+            dstep.da.n = n_live;
+            dstep.heads.assign((n_live + pf - 1) / pf, pf);
+            dstep.heads.back() = n_live - (int)(dstep.heads.size() - 1) * pf;
+        }
         for (unsigned long long k = 0; k < steps; ++k)
             if ((rc = run_step(m, f, a, a.sa.passes, rows, per_pass * (int)K1, nullptr, rows, n_live, c.u ? g.u.p : nullptr)))
                 return rc;
@@ -1710,6 +1864,7 @@ int speculate(M *m, const char *what, const GenCall &c, const SpecRequest &sr, c
         step += steps;
         live.erase(std::remove_if(live.begin(), live.end(), [&](int s) { return hs[s].done != 0; }), live.end());
     }
+    if (dm && (rc = draft_flush(dstep, S))) return rc;
     // a home on a spare: its xy, aa, bb and dd go to the first slot (pp: no forward writes it)
     std::vector<unsigned long long> forks;
     for (unsigned long long s = 0; s < S; ++s)
@@ -2943,7 +3098,25 @@ int rwkv_b200_generate_streams_speculative_constrained(
     return speculate(m, logprobs_out || constraint_ids ? "generate_streams_speculative_constrained"
                         : sq                           ? "generate_streams_speculative_stop"
                                                        : "generate_streams_speculative",
-                     c, SpecRequest{draft, ngram, context_start, context, steps_out}, logprobs_out ? &lpq : nullptr, &cq, sq);
+                     c, SpecRequest{draft, ngram, context_start, context, steps_out, nullptr}, logprobs_out ? &lpq : nullptr, &cq, sq);
+}
+
+int rwkv_b200_generate_streams_drafted(
+    rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens, unsigned long long n_streams,
+    unsigned long long max_new, const unsigned long long *budgets, const unsigned long long *stop_tokens, unsigned long long n_stop,
+    const unsigned long long *override_tokens, const float *override_values, unsigned long long n_override,
+    const rwkv_b200_sampler *samplers, const double *u, unsigned long long *tokens_out, unsigned long long *lengths_out,
+    unsigned int draft, const rwkv_b200_drafter *drafter, unsigned long long *steps_out, int logprob_mode, unsigned int top_n,
+    double *logprobs_out, unsigned long long *ranks_out, unsigned long long *top_tokens_out, double *top_logprobs_out,
+    const unsigned long long *constraint_ids, const unsigned long long *start_states, unsigned long long *states_out,
+    const rwkv_b200_stop_request *sq) {
+    const GenCall c{slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values,
+                    n_override, samplers, samplers ? u : nullptr, tokens_out, lengths_out};
+    const LogprobRequest lpq{logprob_mode, top_n, logprobs_out, ranks_out, top_tokens_out, top_logprobs_out};
+    const ConstraintRequest cq{constraint_ids, start_states, states_out};
+    static const rwkv_b200_drafter none{}; // a NULL drafter is refused with the other drafter checks
+    return speculate(m, "generate_streams_drafted", c, SpecRequest{draft, 0, nullptr, nullptr, steps_out, drafter ? drafter : &none},
+                     logprobs_out ? &lpq : nullptr, &cq, sq);
 }
 
 int rwkv_b200_generate_streams_speculative_stop(rwkv_b200_model *m, const unsigned long long *slots,
@@ -2959,7 +3132,7 @@ int rwkv_b200_generate_streams_speculative_stop(rwkv_b200_model *m, const unsign
     const GenCall c{slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values,
                     n_override, samplers, samplers ? u : nullptr, tokens_out, lengths_out};
     return speculate(m, sq ? "generate_streams_speculative_stop" : "generate_streams_speculative", c,
-                     SpecRequest{draft, ngram, context_start, context, steps_out}, nullptr, nullptr, sq);
+                     SpecRequest{draft, ngram, context_start, context, steps_out, nullptr}, nullptr, nullptr, sq);
 }
 
 int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned long long *slots, const unsigned long long *first_tokens,
@@ -2972,7 +3145,7 @@ int rwkv_b200_generate_streams_speculative(rwkv_b200_model *m, const unsigned lo
                                            const unsigned long long *context, unsigned long long *steps_out) {
     const GenCall c{slots, first_tokens, n_streams, max_new, budgets, stop_tokens, n_stop, override_tokens, override_values,
                     n_override, samplers, samplers ? u : nullptr, tokens_out, lengths_out};
-    return speculate(m, "generate_streams_speculative", c, SpecRequest{draft, ngram, context_start, context, steps_out}, nullptr,
+    return speculate(m, "generate_streams_speculative", c, SpecRequest{draft, ngram, context_start, context, steps_out, nullptr}, nullptr,
                      nullptr, nullptr);
 }
 

@@ -18,6 +18,8 @@
 //   k_spec_logprob (with log-probabilities) one CTA per row: the emitted token of the row, if it emitted one, scored.
 // With token automata, k_spec_draft also walks the drafts through the stream's automaton into a state per row, by which
 // k_gen_mask masks the rows, and k_spec_accept advances the automaton by each emitted token (DESIGN §4.3).
+// rwkv_b200_generate_streams_drafted takes the drafts from a draft model instead ("drafts from a draft model" below):
+// k_spec_layout then lays out the rows of the drafts the draft model's passes stored in the record.
 // The one-shot call gives every stream the same k and lays out floor(128 / (k + 1)) streams per pass, every row a head
 // row, and k_spec_draft writes the passes' head maps. The batcher mixes streams of different k with one-token lanes
 // (k_gen_feedback's) and prefill segments: the host lays out the head maps once per group, and each stream's outputs go
@@ -84,15 +86,10 @@ struct SpecArgs {
 
 // Draft rule: for n = ngram down to 1 with n < L, the largest j <= L - n - 1 with h[j .. j + n) == h[L - n .. L); the
 // first n with such a j gives the proposal h[j + n .. min(j + n + k, L)], padded with its last token; no match at any n:
-// k copies of h[L - 1]. Draft i (1-based) is then h[min(j + n + i - 1, L - 1)].
-__global__ void __launch_bounds__(kSpecDraftThreads) k_spec_draft(const SpecArgs a) {
-    const SpecLive lv = a.live[blockIdx.x];
-    const int s = lv.s, tid = threadIdx.x;
-    SpecStream &g = a.ss[s];
-    const int k = g.k, ngram = g.ngram;
-    const unsigned long long *h = a.hist + g.h0;
-    const long long L = (long long)g.hl;
-    const bool live = g.done == 0;
+// k copies of h[L - 1]. Draft i (1-based) is then h[min(j + n + i - 1, L - 1)]. Returns j + n, or -1 without a match
+// (and for a finished stream). Every thread of the CTA calls it.
+__device__ __forceinline__ long long spec_propose(const SpecStream &g, const unsigned long long *h, long long L, bool live) {
+    const int ngram = g.ngram, tid = threadIdx.x;
     __shared__ unsigned long long suf[kSpecMaxNgram]; // suf[i] = h[L - 1 - i]
     __shared__ int wmax[kSpecDraftThreads / 32];
     long long from = -1; // the proposal starts at h[from]
@@ -115,8 +112,16 @@ __global__ void __launch_bounds__(kSpecDraftThreads) k_spec_draft(const SpecArgs
             if (best >= 0) from = best + n;
         }
     }
-    if (tid > k) return;
-    auto row_tok = [&](int i) { return i == 0 || from < 0 ? h[L - 1] : h[min(from + i - 1, L - 1)]; };
+    return from;
+}
+
+// A step's layout for live stream lv, whatever proposed its drafts: thread tid <= k writes row tid's token
+// (row_tok(tid): 0 the input, i draft i) into the record, the pass and its descriptor (row 0 on the home slot first |
+// last, row i on the stream's i-th other slot last; a finished stream stores nothing), with a.heads the head map, and
+// with uniforms the row's uniform; with token automata thread 0 walks the drafts into a state per row.
+template <class RowTok>
+__device__ __forceinline__ void spec_layout(const SpecArgs &a, const SpecLive lv, SpecStream &g, bool live, RowTok row_tok) {
+    const int s = lv.s, tid = threadIdx.x, k = g.k;
     const unsigned long long tok = row_tok(tid);
     g.row[tid] = tok;
     const int r = lv.row0 + tid, pi = (lv.pos0 + tid) / kPfMaxTokens, t = (lv.pos0 + tid) % kPfMaxTokens;
@@ -146,6 +151,145 @@ __global__ void __launch_bounds__(kSpecDraftThreads) k_spec_draft(const SpecArgs
         const unsigned long long pos = g.len + (unsigned long long)tid;
         a.row_u[r] = pos < g.budget ? a.u[g.u0 + pos * a.u_stride] : 0.0;
     }
+}
+
+// Prompt lookup: one CTA per live stream proposes (spec_propose) and lays out (spec_layout) its rows.
+__global__ void __launch_bounds__(kSpecDraftThreads) k_spec_draft(const SpecArgs a) {
+    const SpecLive lv = a.live[blockIdx.x];
+    SpecStream &g = a.ss[lv.s];
+    const unsigned long long *h = a.hist + g.h0;
+    const long long L = (long long)g.hl;
+    const bool live = g.done == 0;
+    const long long from = spec_propose(g, h, L, live);
+    if ((int)threadIdx.x > g.k) return;
+    spec_layout(a, lv, g, live, [&](int i) { return i == 0 || from < 0 ? h[L - 1] : h[min(from + i - 1, L - 1)]; });
+}
+
+// ---- drafts from a draft model (rwkv_b200_generate_streams_drafted) ------------------------------------------------
+// Each stream keeps two slots of the draft model: D0 holds the tokens the stream's home has absorbed (the history but
+// its last token, h[0 .. fed) of this call so far), D1 is scratch. A step, before spec_layout, enqueues on the draft
+// model (one CUDA stream with the target's work, no synchronisation):
+//   k_draft_first  one thread per live stream: a segment of k + 2 positions, h[fed .. hl) then pads. h[fed .. hl - 1)
+//                  (the tokens the home absorbed in the last step) starts on D0 (first) and stores into D0 (last at its
+//                  end); h[hl - 1], the step's input, continues it and stores into D1 (last) and is the stream's head
+//                  row. At the first step the segment is the input alone, first | last on D1, which the call forked
+//                  from D0. Pads continue the segment and store nothing;
+//   pass, then per draft i = 1..k: the pick chain on the draft's rows with the call's overrides, sampler, the row's
+//   automaton state and the uniform of target row i - 1; k_draft_pick stores d_i into the stream record and, for
+//   i < k, lays out pass i + 1: d_i first | last on D1, one token per stream;
+//   k_spec_layout  the layout of the target's rows from the record's drafts.
+// At the end of the call k_draft_flush lays out one pass without logits that absorbs each stream's h[fed .. hl - 1)
+// into D0, so D0 ends with exactly the tokens the first slot absorbed. A finished stream stores nothing in any pass.
+constexpr int kDraftThreads = 128;
+
+struct SpecDraft {
+    unsigned long long d0, d1; // the stream's draft slots
+    unsigned long long fed;    // D0 holds the call's history h[0 .. fed)
+};
+
+struct DraftArgs {
+    SpecStream *ss;                  // the target's stream records: history, budget, uniforms, drafts
+    const SpecLive *live;            // [n_live] the live streams (only .s is read)
+    SpecDraft *ds;                   // [n_streams]
+    const unsigned long long *hist;
+    PassDesc *first, *next;          // the first pass's descriptors, those of passes 2..k
+    int n, k, per_first;             // live streams (all streams: k_draft_flush), drafts, streams per first pass
+    const unsigned long long *pick_next; // the draft model's arg-max per row, or nullptr when sampling
+    const double *pick_sample;       // its {token, margin} per row when sampling
+    const double *u;                 // the call's uniforms (SpecArgs::u), or nullptr
+    double *row_u;                   // [n_live] each draft row's uniform
+    unsigned long long u_stride;
+    const GenConstraint *gc;         // the call's automata, or nullptr
+    unsigned long long *row_state;   // [n_live] each draft row's automaton state (with gc)
+};
+
+// The uniform of target row i of g this step (spec_layout's rule: 0 past the budget).
+__device__ __forceinline__ double draft_u(const DraftArgs &a, const SpecStream &g, int i) {
+    const unsigned long long pos = g.len + (unsigned long long)i;
+    return pos < g.budget ? a.u[g.u0 + pos * a.u_stride] : 0.0;
+}
+
+__global__ void __launch_bounds__(kDraftThreads) k_draft_first(const DraftArgs a) {
+    const int li = blockIdx.x * kDraftThreads + threadIdx.x;
+    if (li >= a.n) return;
+    const int s = a.live[li].s, W = a.k + 2;
+    const SpecStream &g = a.ss[s];
+    SpecDraft &d = a.ds[s];
+    const unsigned long long *h = a.hist + g.h0, hl = g.hl;
+    const bool live = g.done == 0;
+    const int n = live ? (int)(hl - d.fed) : 0; // the segment: h[fed .. hl)
+    const int j = li % a.per_first, t0 = j * W;
+    PassDesc &pd = a.first[li / a.per_first];
+    for (int t = 0; t < W; ++t) {
+        uint32_t desc;
+        if (!live) desc = (uint32_t)d.d1 | (t == 0 ? kDescFirst : 0u);
+        else if (n == 1) desc = (uint32_t)d.d1 | (t == 0 ? kDescFirst | kDescLast : 0u);
+        else if (t < n - 1) desc = (uint32_t)d.d0 | (t == 0 ? kDescFirst : 0u) | (t == n - 2 ? kDescLast : 0u);
+        else desc = (uint32_t)d.d1 | (t == n - 1 ? kDescLast : 0u);
+        pd.tokens[t0 + t] = t < n ? h[d.fed + t] : h[hl - 1];
+        pd.desc[t0 + t] = desc;
+    }
+    pd.rows[j] = t0 + (live ? n - 1 : 0);
+    if (j == 0) pd.out_row0 = li;
+    if (live) d.fed = hl - 1;
+    if (a.gc) a.row_state[li] = live && a.gc[s].mask ? a.gc[s].state : kNoState;
+    if (a.u) a.row_u[li] = draft_u(a, g, 0);
+}
+
+// After draft i's pick: d_i into the record; for i < k, pass i + 1 (d_i on D1), the state and uniform of its row.
+__global__ void __launch_bounds__(kDraftThreads) k_draft_pick(const DraftArgs a, int i) {
+    const int li = blockIdx.x * kDraftThreads + threadIdx.x;
+    if (li >= a.n) return;
+    const int s = a.live[li].s;
+    SpecStream &g = a.ss[s];
+    const bool live = g.done == 0;
+    const unsigned long long d = a.pick_next ? a.pick_next[li] : (unsigned long long)a.pick_sample[2 * li];
+    if (live) g.row[i] = d;
+    if (i == a.k) return;
+    PassDesc &pd = a.next[li / kPfMaxTokens];
+    const int t = li % kPfMaxTokens;
+    pd.tokens[t] = d;
+    pd.desc[t] = (uint32_t)a.ds[s].d1 | kDescFirst | (live ? kDescLast : 0u);
+    pd.rows[t] = t;
+    if (t == 0) pd.out_row0 = li;
+    if (a.gc) {
+        unsigned long long q = a.row_state[li];
+        if (q != kNoState) {
+            const GenConstraint &c = a.gc[s];
+            q = gen_edge(c, q, d);
+            if (q != kNoState && c.start[q] == c.start[q + 1]) q = kNoState;
+        }
+        a.row_state[li] = q;
+    }
+    if (a.u) a.row_u[li] = draft_u(a, g, i);
+}
+
+// The target's rows of a drafted step: spec_layout with the drafts k_draft_pick stored (one CTA per live stream).
+__global__ void __launch_bounds__(32) k_spec_layout(const SpecArgs a) {
+    const SpecLive lv = a.live[blockIdx.x];
+    SpecStream &g = a.ss[lv.s];
+    if ((int)threadIdx.x > g.k) return;
+    const unsigned long long *h = a.hist + g.h0;
+    const unsigned long long last = h[g.hl - 1];
+    spec_layout(a, lv, g, g.done == 0, [&](int i) { return i == 0 ? last : g.row[i]; });
+}
+
+// The call's end: stream s (of a.n, every stream of the call) absorbs h[fed .. hl - 1) into D0, in k + 1 positions
+// (a.per_first streams per pass, no head rows).
+__global__ void __launch_bounds__(kDraftThreads) k_draft_flush(const DraftArgs a) {
+    const int s = blockIdx.x * kDraftThreads + threadIdx.x;
+    if (s >= a.n) return;
+    const int W = a.k + 1;
+    const SpecStream &g = a.ss[s];
+    SpecDraft &d = a.ds[s];
+    const unsigned long long *h = a.hist + g.h0, hl = g.hl;
+    const int n = (int)(hl - 1 - d.fed), t0 = s % a.per_first * W;
+    PassDesc &pd = a.first[s / a.per_first];
+    for (int t = 0; t < W; ++t) {
+        pd.tokens[t0 + t] = t < n ? h[d.fed + t] : h[hl - 1];
+        pd.desc[t0 + t] = (uint32_t)d.d0 | (t == 0 ? kDescFirst : 0u) | (t == n - 1 ? kDescLast : 0u);
+    }
+    d.fed = hl - 1;
 }
 
 // One warp per live stream: lane i holds the pick p_i of row i; a = the leading i in 1..k with row[i] == p_{i - 1}.

@@ -80,6 +80,11 @@ class Guidance(ctypes.Structure):
                 ("scales", ctypes.POINTER(ctypes.c_float))]
 
 
+class Drafter(ctypes.Structure):
+    """rwkv_b200_drafter: the draft model of rwkv_b200_generate_streams_drafted and its slots [n_streams][2] (D0, D1)."""
+    _fields_ = [("model", ctypes.c_void_p), ("slots", ctypes.POINTER(ctypes.c_ulonglong))]
+
+
 def guide_rows(c, q, scale):
     """Rule 2 of classifier-free guidance (include/rwkv_b200.h) in numpy: c + (scale - 1) * (c - q) in float32, each
     operation rounded once, with w = scale - 1 itself rounded to float32. c, q: the conditional and guidance logits."""
@@ -452,6 +457,10 @@ def load_library():
                                                                      ull, c.POINTER(Sampler), pdbl, pull, pull, c.c_uint,
                                                                      c.c_uint, pull, pull, pull, i32, c.c_uint, pdbl, pull,
                                                                      pull, pdbl, pull, pull, pull, c.POINTER(StopRequest)]),
+        "rwkv_b200_generate_streams_drafted": (i32, [vp, pull, pull, ull, ull, pull, pull, ull, pull, pflt, ull,
+                                                     c.POINTER(Sampler), pdbl, pull, pull, c.c_uint, c.POINTER(Drafter),
+                                                     pull, i32, c.c_uint, pdbl, pull, pull, pdbl, pull, pull, pull,
+                                                     c.POINTER(StopRequest)]),
         "rwkv_b200_batcher_submit_stop": (i32, [vp, c.POINTER(Request), c.POINTER(RequestEx), ull, ull, pull]),
         "rwkv_b200_batcher_read_stop": (i32, [vp, ull, pull, pull, pull]),
         "rwkv_b200_batcher_submit_spec": (i32, [vp, c.POINTER(Request), c.POINTER(RequestEx), ull, ull,
@@ -880,7 +889,8 @@ class Engine:
         return res
 
     def generate_speculative(self, streams, max_new, draft, ngram=3, context=None, budgets=None, stop=(), overrides=None,
-                             sampling=None, u=None, stop_strings=None, logprobs=None, top_n=0, constraints=None):
+                             sampling=None, u=None, stop_strings=None, logprobs=None, top_n=0, constraints=None,
+                             drafter=None):
         """generate_streams(sampling=...) with prompt-lookup drafts (rwkv_b200_generate_streams_speculative): the same
         tokens and first-slot states, several tokens per step where the drafts are right. streams = [(slots, first_token),
         ...], each with draft + 1 distinct slots, the first holding the conversation (the others are scratch). context:
@@ -888,7 +898,20 @@ class Engine:
         dict per stream: "tokens" (uint64) and "steps" (the steps that emitted a token). stop_strings as in
         generate_streams (rwkv_b200_generate_streams_speculative_stop) adds "stop_hit", "stop_tail" and "stop_state".
         logprobs, top_n and constraints as in generate_streams (rwkv_b200_generate_streams_speculative_constrained) add
-        "logprobs", "ranks", "top_tokens", "top_logprobs" and "state", bit for bit generate_streams' values."""
+        "logprobs", "ranks", "top_tokens", "top_logprobs" and "state", bit for bit generate_streams' values.
+        drafter = (draft_engine, draft_slots): the drafts come from a second, smaller model of the same vocabulary
+        (rwkv_b200_generate_streams_drafted) instead of prompt lookup; draft_slots holds one (D0, D1) pair of
+        draft_engine's slots per stream, D0 primed with the same tokens as the stream's first slot, D1 scratch. D0 ends
+        holding the tokens the first slot absorbed. It takes neither context nor ngram; the results are as above."""
+        if drafter is not None:
+            deng, dslots = drafter
+            if context is not None or ngram != 3:
+                raise EngineError("generate_speculative: a drafter takes neither context nor ngram")
+            if deng is self:
+                raise EngineError("generate_speculative: the draft engine is the target engine")
+            if len(dslots) != len(streams) or any(len(pair) != 2 for pair in dslots):
+                raise EngineError("generate_speculative: the drafter needs one (D0, D1) slot pair per stream (%d)"
+                                  % len(streams))
         extended = logprobs is not None or constraints is not None
         if extended:
             _logprob_mode(logprobs, "generate_speculative")
@@ -904,21 +927,28 @@ class Engine:
             seqs = [[int(x) for x in (c if c is not None else ())] for c in context]
             cstart = np.ascontiguousarray(np.cumsum([0] + [len(c) for c in seqs]), dtype=np.uint64)
             ctx = np.ascontiguousarray([x for c in seqs for x in c], dtype=np.uint64)
-        if extended:
+        if extended or drafter is not None:
             lp_args, cargs, scored = _scored_args(S, max_new, logprobs, top_n, constraints, "generate_speculative")
         sp = _samplers(sampling, S) if sampling is not None else None
         P = ctypes.c_ulonglong
         args = (self.h, *lead, sp, *tail, int(draft), int(ngram), _ptr(cstart, P), _ptr(ctx, P), _ptr(steps, P))
         sreq, sres = self._stop_request(stop_strings, S, "generate_speculative") if stop_strings is not None else (None, None)
         sq = ctypes.byref(sreq) if sreq is not None else None
+        if drafter is not None:
+            dsl = np.ascontiguousarray([int(x) for pair in dslots for x in pair], dtype=np.uint64)
+            dr = Drafter(deng.h.value if deng.h is not None else None, _ptr(dsl, P))
+            self._ck(self.lib.rwkv_b200_generate_streams_drafted(self.h, *lead, sp, *tail, int(draft), ctypes.byref(dr),
+                                                                 _ptr(steps, P), *lp_args, *cargs, sq),
+                     "generate_streams_drafted")
         # the narrowest entry point that has the features asked for
-        if extended:
+        elif extended:
             name, more = "generate_streams_speculative_constrained", (*lp_args, *cargs, sq)
         elif sq is not None:
             name, more = "generate_streams_speculative_stop", (sq,)
         else:
             name, more = "generate_streams_speculative", ()
-        self._ck(getattr(self.lib, "rwkv_b200_" + name)(*args, *more), name)
+        if drafter is None:
+            self._ck(getattr(self.lib, "rwkv_b200_" + name)(*args, *more), name)
         res = []
         for s in range(S):
             n = int(lens[s])
